@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- headline benchmark of the B200-native MyScaleDB hot path.
+"""bench.py -- headline benchmark of the H100-native (sm_90a) MyScaleDB hot path.
 
 Workload (BASELINE.json configs[1], the largest single-GPU configuration):
     FLAT brute-force inner product, 10M x 768-d bf16 corpus, batch of 1024 queries, top-10.
@@ -15,6 +15,9 @@ per-shard top-k, one merge kernel.
 --impl reference: the CPU arm -- the oracle's restatement of the reference's brute-force path
 (one thread per part, SIMD inner-product blocks; the reference binary cannot be built here,
 see DESIGN.md), timed on a bounded row sample and scaled linearly to the full corpus.
+--dump-outputs DIR: after the timed steps, the last timed step's results (what a caller of the timed path receives:
+distances and ids of the top-k of every query) are written as DIR/distances.npy (float32) and DIR/ids.npy (float64).
+The corpus and the queries are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -50,8 +53,9 @@ def parse():
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="target CPU-baseline sample duration")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--headline-only", action="store_true", help="A/B runs: skip verification and the extra keys")
-    ap.add_argument("--index-rows", type=int, default=100_000_000, help="rows of the MSTG-class index extra (BASELINE configs[2]); 0 = skip")
+    ap.add_argument("--index-rows", type=int, default=20_000_000, help="rows of the MSTG-class index extra (fits one 80 GB H100 beside the corpus); 0 = skip")
     ap.add_argument("--index-nq", type=int, default=256)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's distances / ids as .npy files into DIR")
     return ap.parse_args()
 
 
@@ -61,7 +65,7 @@ def config_of(a, n):
             "rows": a.rows, "dim": a.dim, "batch_queries": a.nq, "k": a.k,
             "sharding": (f"rows/{n} per GPU; b200_sharded_corpus_search(): tensor-core scan -> one ncclAllGather of the packed per-shard "
                          "top-k -> merge kernel, replayed as one CUDA graph per step") if n > 1 else "single GPU",
-            "cache": f"inputs ({a.rows * a.dim * 2 / n / 1e9:.1f} GB of corpus rows per GPU) larger than the 126 MB L2; no flush needed"}
+            "cache": f"inputs ({a.rows * a.dim * 2 / n / 1e9:.1f} GB of corpus rows per GPU) larger than the 50 MB L2; no flush needed"}
 
 
 _NVML_LOOP = r"""
@@ -309,18 +313,6 @@ def verify_results(a, index, corpus, q_host, q_dev, d_res, i_res, row0, shard_ro
                     + ") vs the fp32 scan kernel over every shard merged on the host, and vs oracle/vs_oracle.c over all rows"}
 
 
-def traffic_from_profile(a, n_gpus):
-    """DRAM bytes per launch of the headline kernel on THIS workload from the committed ncu capture, or None."""
-    try:
-        rec = json.load(open(os.path.join(ROOT, "profiles", "gemm_topk_traffic.json")))
-        w = rec["workload"]
-        if n_gpus == 1 and (w["rows"], w["dim"], w["nq"], w["k"]) == (a.rows, a.dim, a.nq, a.k):
-            return rec["dram_bytes_read"] + rec["dram_bytes_write"]
-    except Exception:
-        pass
-    return None
-
-
 def latency_extra():
     """BASELINE configs[0]: FLAT L2 distance(), 10k x 128 fp32, ONE query, top-10, a part resident in HBM: median latency of
     the C-ABI host call (single fused launch) next to the reference's CPU form on one core (faiss nx < 20: exact differences,
@@ -358,9 +350,9 @@ def latency_extra():
 
 
 def index_extra(a, dev, N, rank, comm):
-    """BASELINE configs[2] / the metric's own scale: MSTG-class index, 100 M x 768 fp32 clustered rows (SURVEY 8d: 10 000 Gaussian
+    """BASELINE configs[2] at the size one 80 GB GPU holds: MSTG-class index, --index-rows x 768 fp32 clustered rows (SURVEY 8d: 10 000 Gaussian
     centres, points = centre + N(0, 0.3^2)), batch of 256 queries, top-10, rows sharded over the N GPUs.  Rows are generated
-    chunk by chunk in HBM and streamed into b200_index_add_device (bf16 lists; the fp32 rows are not kept: 307 GB);
+    chunk by chunk in HBM and streamed into b200_index_add_device (bf16 lists; the fp32 rows are not kept);
     ground truth = exact fp32 scan of the regenerated chunks; the sharded search is b200_sharded_index_search."""
     import numpy as np
     import torch
@@ -449,7 +441,7 @@ def index_extra(a, dev, N, rank, comm):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = peaks.get("hbm_gbs", 6650.0)
+    hbm = peaks.get("hbm_gbs", 3350.0)   # H100 SXM data sheet
     ix.enable_timing(True)
     runs = []
     for nprobe in (1, 2, 4, 8):
@@ -498,8 +490,7 @@ def index_extra(a, dev, N, rank, comm):
             "truth": f"exact fp32 scan of all rows for {nt} queries ({truth_s:.1f} s)",
             "qps_at_recall_0.95": best["qps"] if best else None, "best": best, "runs": runs,
             "hbm_peak_GB_per_s": hbm,
-            "note": "QPS device-timed (CUDA events, max over ranks), queries resident; exact brute force over the same rows on the "
-                    "tensor cores runs at ~8 k QPS per 100 M rows (round 1, profiles/r01_bench_line_100m_n1.json)"}
+            "note": "QPS device-timed (CUDA events, max over ranks), queries resident"}
 
 
 def main():
@@ -635,6 +626,12 @@ def main():
     barrier()
     ms = e0.elapsed_time(e1)
     launches = S.launch_count()
+    if a.dump_outputs and rank == 0:
+        # the last timed step's results, as the timed path left them on the device
+        d_out, i_out = (o_dis, o_ids) if N == 1 else (f_dis, f_ids)
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        np.save(os.path.join(a.dump_outputs, "distances.npy"), d_out.cpu().numpy().astype(np.float32))
+        np.save(os.path.join(a.dump_outputs, "ids.npy"), i_out.cpu().numpy().astype(np.float64))
     kern_ms, kern_n = index.kernel_time(reset=True)
     clocks = sampler.stop()
     if N > 1:  # kernel time for the roofline: a few eager steps with per-launch events, outside the timed region
@@ -686,7 +683,7 @@ def main():
             torch.cuda.synchronize()
             kms3, kn3 = ix32.kernel_time(reset=True)
             per = kms3 / max(kn3, 1)
-            fp32_batch = {"kernel": "gemm3_topk_kernel (fp32 rows, 3 x tcgen05.mma.kind::tf32 per k-step, fused top-k)",
+            fp32_batch = {"kernel": "gemm_topk_kernel<true> (fp32 rows, 3 x wgmma tf32 per k-step, fused top-k)",
                           "rows": m, "batch_queries": nq, "ms_per_launch": per,
                           "effective_fp32_TFLOP_per_s": 2.0 * nq * m * a.dim / (per * 1e-3) / 1e12,
                           "tf32_mma_TFLOP_per_s": 3 * 2.0 * nq * m * a.dim / (per * 1e-3) / 1e12,
@@ -699,7 +696,7 @@ def main():
     # ---- verification of the TIMED path's results (the run fails on a mismatch) ----
     d_res, i_res = res
     verified = None
-    if not os.environ.get("B200_GEMM_DEBUG") and not a.headline_only:  # kernel experiments produce garbage on purpose
+    if not a.headline_only:
         assert (np.diff(d_res, axis=1) <= 0).all() and (i_res >= 0).all() and (i_res < a.rows).all()
         verified = verify_results(a, index, corpus, q_host, q_dev, d_res, i_res, row0, shard_rows, N, rank, dev)
 
@@ -728,8 +725,8 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = peaks.get("bf16_tflops", 1590.0)
-        peak_src = "MEASURED_PEAKS.json bf16_tflops (burst, of measured)" if peaks else "fallback 1590 TFLOP/s"
+        peak = peaks.get("bf16_tflops", 989.0)
+        peak_src = "MEASURED_PEAKS.json bf16_tflops (burst, of measured)" if peaks else "H100 SXM data sheet, dense bf16 at 700 W"
         flops_per_launch = 2.0 * nq * shard_rows * a.dim
         achieved = flops_per_launch / (kern_ms / max(kern_n, 1) * 1e-3) / 1e12 if kern_n else None
         out = {
@@ -741,19 +738,14 @@ def main():
                     "note": "b200_corpus_search(): pinned host queries -> H2D -> kernels -> D2H results; corpus resident "
                             "(index state)"},
             "gpu_launches": int(launches), "verified": verified,
-            "roofline": {"bound": "tensor", "kernel": "b200::gemm::gemm_topk_kernel (tcgen05 bf16 GEMM + fused top-k)",
+            "roofline": {"bound": "tensor", "kernel": "b200::gemm::gemm_topk_kernel<false> (wgmma bf16 GEMM + fused top-k)",
                          "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
                          "frac": (achieved / peak) if achieved else None,
-                         # dram__bytes_read.sum + dram__bytes_write.sum of one launch of this kernel on this workload,
-                         # from the committed ncu --set full capture (profiles/r01_gemm_topk_cg2_mc2.ncu-rep:
-                         # 15.363287 GB + 8.07 MB); other shapes have no capture -> null
-                         "traffic": traffic_from_profile(a, N), "traffic_unit": "bytes per launch",
-                         "traffic_source": "profiles/gemm_topk_traffic.json (dram__bytes_read.sum + dram__bytes_write.sum of one launch, ncu --set full)",
                          "flops_per_launch": flops_per_launch, "launch_ms": kern_ms / max(kern_n, 1),
                          "launches_timed": int(kern_n), "peak_source": peak_src,
                          "hbm_algorithmic_bytes_per_launch": shard_rows * a.dim * 2},
         }
-        hbm = peaks.get("hbm_gbs", 6650.0)
+        hbm = peaks.get("hbm_gbs", 3350.0)   # H100 SXM data sheet
         for fs in flat_scan:
             if "GB_per_s" not in fs:
                 continue

@@ -1,5 +1,5 @@
 /*
- * b200_search.h -- C ABI of libb200search.so, the B200-native (sm_100a) engine for
+ * b200_search.h -- C ABI of libb200search.so, the H100-native (sm_90a) engine for
  * MyScaleDB's ANN / BM25 hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes only, no C++/torch types.
@@ -36,7 +36,7 @@ extern "C" {
 #define B200_ERR_INVALID 1     /* bad argument */
 #define B200_ERR_CUDA 2        /* CUDA runtime / driver failure */
 #define B200_ERR_UNSUPPORTED 3 /* valid request this build does not implement */
-#define B200_ERR_NO_DEVICE 4   /* no sm_100 device visible */
+#define B200_ERR_NO_DEVICE 4   /* no sm_90 device visible */
 #define B200_ERR_NOMEM 5
 #define B200_ERR_NOT_FOUND 6   /* cache miss */
 
@@ -114,17 +114,14 @@ int b200_corpus_search_device(b200_corpus *c, const float *d_queries, int64_t nq
                               const uint8_t *d_alive_bits /*nullable*/, int64_t id_offset, float *d_out_dis,
                               int64_t *d_out_ids, void *stream);
 /* Force a search path (tests, A/B measurements; production leaves 0):
- *   0 auto | 1 memory-bound scan kernel | 2 tensor cores, exactly the variant auto picks for a batch (operands
- *   streamed through shared memory, CTA pairs from 2 query tiles up, TMA multicast in clusters of 2 / 4 pairs when
- *   the batch has a multiple of 4 / 8 query tiles; fp32 corpora: the 3xTF32 kernel) | 3 single-CTA MMAs <1,1> |
- *   4 CTA pairs, no multicast <2,1> | 5 at most two pairs per cluster <2,2> | 6 up to four pairs per cluster <2,4>
- *   (same as 2, explicit) | 7 queries stationary in TMEM ("TS" form; k <= 30, d <= 768, bf16 corpora). */
+ *   0 auto | 1 memory-bound scan kernel | 2 tensor cores (bf16 corpora: the bf16 wgmma kernel; fp32 corpora: the
+ *   3xTF32 kernel) | 3 .. 7 the same as 2 (they named tensor-core variants of an earlier target and stay accepted). */
 int b200_corpus_set_path(b200_corpus *c, int path);
 /* which kernel the last search on this corpus launched (so a test can prove it exercised the variant it meant to) */
 #define B200_KERNEL_SCAN 1
-#define B200_KERNEL_GEMM_BF16 2   /* gemm_topk_kernel<cta_group, pairs_per_cluster> */
-#define B200_KERNEL_GEMM_TS 3     /* gemm_topk_ts_kernel */
-#define B200_KERNEL_GEMM_TF32X3 4 /* gemm3_topk_kernel */
+#define B200_KERNEL_GEMM_BF16 2   /* gemm_topk_kernel<false> (cta_group and pairs_per_cluster report 1) */
+#define B200_KERNEL_GEMM_TS 3     /* no longer launched; the value stays reserved */
+#define B200_KERNEL_GEMM_TF32X3 4 /* gemm_topk_kernel<true> */
 int b200_corpus_last_variant(b200_corpus *c, int *kernel, int *cta_group, int *pairs_per_cluster, int *grid);
 /* CUDA-event timing of the dominant kernel (scan or GEMM) of every search on this corpus,
  * recorded on the launching stream; used by bench.py for the roofline report. */

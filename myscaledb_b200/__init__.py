@@ -1,10 +1,10 @@
-"""myscaledb_b200 -- B200-native (sm_100a) engine for MyScaleDB's ANN / BM25 hot path.
+"""myscaledb_b200 -- H100-native (sm_90a) engine for MyScaleDB's ANN / BM25 hot path.
 
 The product is ``libb200search.so`` (hand-written CUDA behind the C ABI of
 ``include/b200_search.h``).  This package is the thin host-side mirror used by the
 tests and the benchmark: ctypes bindings (``_lib``) and Python classes named after the
 reference's operator surface (``search``).  There is no CPU fallback: importing works
-anywhere, computing needs an sm_100 GPU and the built library.
+anywhere, computing needs an sm_90 GPU and the built library.
 """
 from . import _lib  # noqa: F401
 from .search import (  # noqa: F401

@@ -296,8 +296,8 @@ __global__ void __launch_bounds__(256) bm25_score_kernel(const Bm25ScoreParams p
 }
 
 // ------------------------------------------------------------------------------------
-// Round 2: document-at-a-time inside doc RANGES.  The kernel above scores posting by posting and searches every other
-// clause's list for each group of 32 postings (33 GB/s of posting bytes: 0.5 % of HBM).  Here a warp owns a CONTIGUOUS run of
+// Document-at-a-time inside doc RANGES.  The kernel above scores posting by posting and searches every other
+// clause's list for each group of 32 postings (a small fraction of the HBM bandwidth).  Here a warp owns a CONTIGUOUS run of
 // doc ranges of one query; for a range [r W, (r + 1) W) it
 //   1. advances one cursor per clause (lanes = clauses) to the range end by a galloping + binary search from the previous
 //      cursor (lists are sorted by doc: the cursors only move forward, every posting is read exactly once, coalesced),
@@ -311,9 +311,9 @@ __global__ void __launch_bounds__(256) bm25_score_kernel(const Bm25ScoreParams p
 constexpr int kDaatSlots = 512;           // per warp: doc u32 + score f32 + mask u64 = 8 KB (+ the list of occupied slots)
 constexpr int kDaatFill = 352;            // postings a table takes in one go (load factor ~0.69)
 constexpr int kDaatTarget = 192;          // postings per range the host aims for
-// bytes of shared memory per warp: the table and the u16 list of occupied slots (the sweep visits only those).  The first
-// version used 1024-slot tables (16 KB per warp, 1 CTA per SM) and swept all slots of every range: the kernel was bound by
-// dependent-load latency at 8 warps per SM (1.8 ms for 512 queries x 25 k postings); 8.7 KB per warp keeps 3 CTAs resident.
+// bytes of shared memory per warp: the table and the u16 list of occupied slots (the sweep visits only those).  1024-slot
+// tables (16 KB per warp, 1 CTA per SM) swept in full leave the kernel bound by dependent-load latency at 8 warps per SM;
+// 8.7 KB per warp keeps 3 CTAs resident.  The table size was chosen on an earlier GPU and is not re-measured on the H100.
 constexpr int kDaatWarpBytes = kDaatSlots * 16 + ((kDaatFill * 2 + 15) / 16) * 16;
 constexpr uint32_t kDaatEmpty = 0xffffffffu;
 

@@ -1,9 +1,9 @@
 // capi.cu -- the C ABI of libb200search.so (declared in include/b200_search.h) and the host
 // orchestration under it: device-resident corpora, path selection (memory-bound scan vs
-// tcgen05 GEMM), query staging, partial-list merge.
+// wgmma GEMM), query staging, partial-list merge.
 //
 // There is deliberately no CPU compute path in this file: every entry point either runs
-// CUDA kernels on an sm_100 device or fails with B200_ERR_NO_DEVICE / B200_ERR_CUDA.
+// CUDA kernels on an sm_90 device or fails with B200_ERR_NO_DEVICE / B200_ERR_CUDA.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -37,14 +37,14 @@ static int ensure_device() {
     B200_CUDA_OK(cudaGetDevice(&dev));
     int major = 0;
     B200_CUDA_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    if (major != 10)
+    if (major != 9)
         return fail(B200_ERR_NO_DEVICE, "device compute capability major is " + std::to_string(major) +
-                                            "; this library carries sm_100a code only");
+                                            "; this library carries sm_90a code only");
     return B200_OK;
 }
 
 static int num_sms() {
-    int dev = 0, n = 148;
+    int dev = 0, n = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     return n;
 }
@@ -94,8 +94,7 @@ struct b200_corpus {
     float *row_bias = nullptr;   // L2: ||y||^2 (GEMM path)
     int device = 0;
     int path = 0;
-    int gemm_cta_group = 0;  // 0 auto, 1 force single-CTA MMA (A/B experiments)
-    int sms = 148;
+    int sms = 132;
     cudaStream_t stream = nullptr;
     std::mutex mu;
     // workspaces
@@ -109,10 +108,8 @@ struct b200_corpus {
     int d_tickets_d = 0;           // row length the query staging behind d_tickets was sized for
     int fused_enabled = 1;         // B200_FUSED_SCAN=0 disables (A/B)
     int rescore_l2 = 1;      // tensor-core L2: re-score the k winners exactly (B200_GEMM_RESCORE_L2=0 disables, A/B only)
-    int gemm_multicast = 1;  // CTA pairs per cluster sharing each corpus tile: 1 auto (4, else 2), 2, 4; B200_GEMM_MULTICAST=0 disables
-    int gemm_ts = 0;  // 0 streaming (default: faster at every measured d), 1 TS when d_pad <= 512, 2 TS whenever it fits
-    // what the last tensor-core launch really was (tests assert on it): cta_group, pairs per cluster, TS form, grid, kernel id
-    int last_cg = 0, last_mc = 0, last_ts = 0, last_grid = 0, last_kernel = 0;
+    // what the last launch really was (tests assert on it): kernel id, CTAs per MMA and per operand fetch (1 on sm_90), grid
+    int last_cg = 0, last_mc = 0, last_grid = 0, last_kernel = 0;
     // optional CUDA-event timing of the dominant kernel (scan or GEMM) for the roofline report
     bool timing = false;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_used, ev_free;
@@ -196,7 +193,7 @@ static int pad_for(int dtype, int d) {
 }
 
 extern "C" const char *b200_last_error(void) { return g_error.c_str(); }
-extern "C" const char *b200_version(void) { return "b200search 0.1 (sm_100a)"; }
+extern "C" const char *b200_version(void) { return "b200search 0.1 (sm_90a)"; }
 
 extern "C" int b200_device_count(int *out_n) {
     if (!out_n) return fail(B200_ERR_INVALID, "out_n is null");
@@ -246,8 +243,6 @@ extern "C" int b200_corpus_create(int metric, int dtype, int d, int64_t capacity
     if (const char *ev = getenv("B200_GEMM_SYNC_SLACK")) c->sync_slack = atoi(ev);
     if (const char *ev = getenv("B200_GEMM_RESCORE_L2")) c->rescore_l2 = atoi(ev);
     if (const char *ev = getenv("B200_FUSED_SCAN")) c->fused_enabled = atoi(ev);
-    if (const char *ev = getenv("B200_GEMM_TS")) c->gemm_ts = atoi(ev);
-    if (const char *ev = getenv("B200_GEMM_MULTICAST")) c->gemm_multicast = atoi(ev);
     cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
     if (e != cudaSuccess) {
         delete c;
@@ -377,8 +372,9 @@ namespace b200 {
 // slots of a per-thread top-k list (kernels.h): k, unless B200_LIST_APPEND_MIN_K selects the append form for this k
 int list_cap_for(int k) {
     static const int min_k = getenv("B200_LIST_APPEND_MIN_K") ? atoi(getenv("B200_LIST_APPEND_MIN_K")) : 0;
-    // default: the two-level (tournament) form from k = 17 (k = 100: 25.7 ms per launch against 36.8 for the plain rescan, k = 64:
-    // 18.7 against 22.3; k <= 16 keeps the plain form, which is what the k = 10 headline runs); B200_LIST_TOURN_MIN_K=0 turns it off
+    // default: the two-level (tournament) form from k = 17 (an insert rescans one group and the group worsts instead of all k
+    // entries); k <= 16 keeps the plain form.  The crossover k = 17 was chosen on an earlier GPU and is not re-measured on the H100.
+    // B200_LIST_TOURN_MIN_K=0 turns it off
     static const int tourn_k = getenv("B200_LIST_TOURN_MIN_K") ? atoi(getenv("B200_LIST_TOURN_MIN_K")) : 17;
     if (min_k > 0 && k >= min_k) return list_cap_append(k);
     if (tourn_k > 0 && k >= tourn_k) return list_cap_tourn(k);
@@ -389,17 +385,9 @@ int list_cap_for(int k) {
 extern "C" int b200_corpus_set_path(b200_corpus *c, int path) {
     if (!c || path < 0 || path > 7) return fail(B200_ERR_INVALID, "path must be 0..7");
     std::lock_guard<std::mutex> lk(c->mu);
-    // 0 auto | 1 scan | 2 tensor cores, the variant auto picks (streaming operands, TMA multicast in the largest cluster
-    // the batch allows) | 3 single-CTA MMAs <1,1> | 4 CTA pairs without multicast <2,1> | 5 at most two pairs per
-    // cluster <2,2> | 6 up to four pairs per cluster <2,4> (= 2, explicit) | 7 queries stationary in TMEM (TS form)
+    // 0 auto | 1 scan | 2 tensor cores.  3..7 named the tensor-core instantiations of an earlier target (CTA pairs,
+    // multicast clusters, queries in tensor memory); sm_90 has one tensor-core kernel per operand type, so they select it.
     c->path = path >= 2 ? 2 : path;
-    c->gemm_cta_group = path == 3 ? 1 : 0;
-    c->gemm_ts = path == 7 ? 2 : 0;
-    c->gemm_multicast = path == 4 ? 0 : path == 5 ? 2 : 1;
-    if (path == 0) {  // auto honours the environment overrides again
-        if (const char *ev = getenv("B200_GEMM_TS")) c->gemm_ts = atoi(ev);
-        if (const char *ev = getenv("B200_GEMM_MULTICAST")) c->gemm_multicast = atoi(ev);
-    }
     return B200_OK;
 }
 
@@ -506,10 +494,10 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
     float *q32 = c->w_q32.as<float>();
     B200_CUDA_OK(launch_pad_rows_f32(reinterpret_cast<const float *>(d_queries), c->d, q32, c->d_pad, nq, s));
     int path = c->path;
-    // auto: when the batch goes to the tensor cores (bf16 rows: kind::f16 GEMM; fp32 rows: 3xTF32 split GEMM, same
-    // accuracy class as the fp32 FMA scan).  Measured crossovers (profiles/r01_small_batch.log, 4M x 768): bf16 rows
-    // 0.92 ms per <= 128-query batch (the HBM floor) vs 1.3 ms for ONE query on the scan; fp32 rows 3.6 ms vs 5.1 ms
-    // for 8 queries on the scan.  L2 keeps faiss' own switch: below distance_compute_blas_threshold = 20 queries the
+    // auto: when the batch goes to the tensor cores (bf16 rows: bf16 wgmma GEMM; fp32 rows: 3xTF32 split GEMM, same
+    // accuracy class as the fp32 FMA scan).  A <= 128-query tensor-core pass reads the corpus once, the scan reads it once
+    // per few queries, so the tensor cores take bf16 batches from 2 queries and fp32 batches from 5.  These crossovers were
+    // chosen on an earlier GPU and are not re-measured on the H100.  L2 keeps faiss' own switch: below distance_compute_blas_threshold = 20 queries the
     // reference sums exact differences, from 20 up it uses ||x||^2 + ||y||^2 - 2xy like the GEMM kernels do (which
     // cancels badly for far-from-origin data), so L2 batches move to the tensor cores at 20.  Very large k stays on
     // the scan path, whose lists are warp-cooperative.
@@ -580,19 +568,16 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
         return B200_OK;
     }
 
-    // ---- path 2: tcgen05 GEMM with fused top-k, <= 1024 queries (8 query tiles) per launch
+    // ---- path 2: wgmma GEMM with fused top-k, <= 1024 queries (8 query tiles) per launch
     if (k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 not supported on the GEMM path");
     const int64_t QCHUNK = 1024;
     for (int64_t qb = 0; qb < nq; qb += QCHUNK) {
         const int64_t nq_c = std::min(QCHUNK, nq - qb);
         const bool f32 = c->dtype == B200_DTYPE_F32;
-        // >= 2 query tiles: CTA pairs (tcgen05 cta_group::2), query tiles padded to an even count;
-        // up to 128 queries: one CTA per MMA (a pair would spend half of its rows on padding)
-        const int cta_group = (nq_c > 128 && c->gemm_cta_group != 1) ? 2 : 1;
-        const int nq_pad = (int)round_up(nq_c, 128 * cta_group);
+        const int nq_pad = (int)round_up(nq_c, 128);
         const int q_tiles = nq_pad / 128;
         if (f32) {
-            // fp32 rows: queries split once per batch into TF32 hi / lo planes (ip_gemm_tf32x3_sm100.cu)
+            // fp32 rows: queries split once per batch into TF32 hi / lo planes (ip_gemm_sm90.cu)
             B200_TRY(c->w_qbf.reserve((size_t)nq_pad * c->d_pad * 4));
             B200_TRY(c->w_qlo.reserve((size_t)nq_pad * c->d_pad * 4));
             B200_CUDA_OK(launch_split_tf32(q32 + qb * c->d_pad, nq_c, c->d_pad, c->w_qbf.as<float>(), c->w_qlo.as<float>(), nq_pad, s));
@@ -613,26 +598,7 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
                                               c->w_qnorm.as<float>(), s));
             q_add = c->w_qnorm.as<float>();
         }
-        // 2 or 4 CTA pairs per cluster share every corpus tile through TMA multicast when the query tiles allow it
-        // (gemm_multicast: 0 off, 2 / 4 pairs per cluster, 1 = auto: 4 when q_tiles % 8 == 0 else 2)
-        int pairs = 1;
-        if (cta_group == 2 && c->gemm_multicast && !f32) {
-            const int want = c->gemm_multicast == 1 ? 4 : c->gemm_multicast;
-            if (want >= 4 && q_tiles % 8 == 0) pairs = 4;
-            else if (want >= 2 && q_tiles % 4 == 0) pairs = 2;
-        }
         int grid = gemm_topk_grid(q_tiles, c->n, sms);
-        while (pairs > 1) {
-            // persistent + paced kernel: never launch more clusters than can be co-resident
-            const int maxc = gemm_topk_max_clusters(2, pairs, k);
-            const int groups = q_tiles / (2 * pairs);
-            const int per_group = maxc / groups;
-            if (per_group >= 1) {
-                grid = std::min(grid, per_group * groups * 2 * pairs);
-                break;
-            }
-            pairs /= 2;
-        }
         grid = (grid / q_tiles) * q_tiles;
         if (grid < q_tiles) grid = q_tiles;
         B200_TRY(c->w_pk.reserve((size_t)grid * 128 * k * 4));
@@ -659,10 +625,7 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
         gp.d_pad = c->d_pad;
         gp.k = k;
         gp.q_tiles = q_tiles;
-        gp.cta_group = cta_group;
-        gp.pairs_per_cluster = pairs;
-        if (const char *dv = getenv("B200_GEMM_DEBUG")) gp.debug = atoi(dv);
-        if (q_tiles > cta_group && c->sync_slack > 0) {
+        if (q_tiles > 1 && c->sync_slack > 0) {
             B200_TRY(c->w_prog.reserve((size_t)grid * 4));
             B200_CUDA_OK(cudaMemsetAsync(c->w_prog.p, 0, (size_t)grid * 4, s));
             gp.progress = c->w_prog.as<int>();
@@ -671,16 +634,10 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
         const char *detail = nullptr;
         std::pair<cudaEvent_t, cudaEvent_t> ev;
         timing_begin(c, s, ev);
-        // TS (queries stationary in TMEM): measured slower than streaming at d = 768 (N = 64 MMAs are bound
-        // by the 64 B/clk TMEM->tensor-core operand path: 75 vs 32 cycles per MMA); auto-enabled only
-        // where a 2 x 128-column accumulator ring fits (d_pad <= 512); gemm_ts = 2 forces it.
-        const bool use_ts = !f32 && cta_group == 2 && k <= 30 && gemm_topk_ts_supported(c->d_pad, q_tiles) &&
-                            (c->gemm_ts == 2 || (c->gemm_ts == 1 && c->d_pad <= 512));
-        cudaError_t e = f32 ? launch_gemm3_topk(gp, grid, s, &detail)
-                            : use_ts ? launch_gemm_topk_ts(gp, grid, s, &detail) : launch_gemm_topk(gp, grid, s, &detail);
+        cudaError_t e = f32 ? launch_gemm3_topk(gp, grid, s, &detail) : launch_gemm_topk(gp, grid, s, &detail);
         timing_end(c, s, ev);
-        c->last_kernel = f32 ? B200_KERNEL_GEMM_TF32X3 : use_ts ? B200_KERNEL_GEMM_TS : B200_KERNEL_GEMM_BF16;
-        c->last_cg = cta_group; c->last_mc = (f32 || use_ts) ? 1 : pairs; c->last_grid = grid;
+        c->last_kernel = f32 ? B200_KERNEL_GEMM_TF32X3 : B200_KERNEL_GEMM_BF16;
+        c->last_cg = 1; c->last_mc = 1; c->last_grid = grid;
         if (e != cudaSuccess)
             return fail(B200_ERR_CUDA, std::string("gemm_topk launch: ") + (detail ? detail : cudaGetErrorString(e)));
         MergeParams mp{};
@@ -725,7 +682,7 @@ extern "C" int b200_corpus_search_device(b200_corpus *c, const float *d_queries,
 // ThreadPool, MergeTreeSelectWithHybridSearchProcessor.cpp:1212-1241).  The query is written to mapped pinned memory and
 // read by the kernel directly, the last block to finish merges the partial lists and writes the result to mapped pinned
 // memory, the host waits on a flag in that memory: no pad / merge launches, no H2D / D2H copies, no stream synchronise
-// (round 1: 103 us per resident call against a 16 us kernel).
+// (the staged form spends most of a resident call on those).
 static int search_host_fused(b200_corpus *c, const float *queries, int64_t nq, int k, const uint8_t *alive_bits, int ip_min_quirk,
                              float *out_dis, int64_t *out_ids, bool *done) {
     *done = false;
@@ -768,7 +725,7 @@ static int search_host_fused(b200_corpus *c, const float *queries, int64_t nq, i
     B200_CUDA_OK(cudaHostGetDevicePointer(&dp, c->h_pin, 0));
     char *dpc = reinterpret_cast<char *>(dp);
     // the query goes pinned -> device with one small async copy (reading it from the kernel over PCIe, 4 bytes per thread and
-    // block, cost 45 us of a 60 us kernel at 296 blocks); the RESULT is written to mapped host memory by one block
+    // block, would cost most of the kernel); the RESULT is written to mapped host memory by one block
     const bool q_inline = nq * c->d <= 256;   // small queries ride in the kernel parameters: no copy at all
     if (!q_inline) {
         memcpy(h_q, queries, (size_t)nq * c->d * 4);

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for libb200search (sm_100a only).
+// common.cuh -- shared device/host helpers for libb200search (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -134,7 +134,7 @@ using WarpTopK = WarpTopKT<uint32_t>;
 // list, the number of entries ahead of it (lower bound by binary search; ties -> smaller id, then smaller list index).
 // Every thread of the CTA calls it after a __syncthreads() that completes the lists; out may be shared or global
 // (distinct from the inputs).  Replaces "warp 0 inserts the other warps' lists one element at a time", which is
-// O(L k^2 / 32) and dominated IVF probes with k in the hundreds (2 ms per query at k = 160).
+// O(L k^2 / 32) and dominated IVF probes with k in the hundreds.
 template <typename IdT>
 __device__ __forceinline__ void block_rank_merge(const float *keys, const IdT *ids, int L, int list_stride, int k,
                                                  float *out_keys, IdT *out_ids) {

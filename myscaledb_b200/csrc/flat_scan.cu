@@ -49,8 +49,8 @@ struct ChunkTraits<true> {
 };
 
 // QT queries per pass; U rows x CU 16-byte chunks per lane are loaded BEFORE any arithmetic, so
-// every lane keeps U * CU independent 128-bit loads in flight (the first version issued U and
-// reached 3.9 TB/s = 61 % of the measured HBM peak at 25 % occupancy, profiles/r01_flat_scan_v1).
+// every lane keeps U * CU independent 128-bit loads in flight (issuing only U left the scan well short of the HBM peak at
+// the low occupancy this kernel runs at).
 // L2 = squared-L2 vs inner product (cosine = inner product scaled by the stored inverse row norm).
 // candidate read of the fused tail: partial lists in global memory written by other blocks (L2, .cg) or staged in shared memory
 __device__ __forceinline__ unsigned long long gtimer() {
@@ -243,7 +243,7 @@ __global__ void __launch_bounds__(kScanThreads, 2) flat_scan_kernel(const ScanPa
         const int64_t ncand = (int64_t)gridDim.x * p.k;
         const bool staged = p.stage_cap >= ncand;
         if (staged) {
-            // Staged form.  The tail is ONE block and latency-bound (ncu: 45 us kernel of which the SMs are busy for ~10): every
+            // Staged form.  The tail is ONE block and latency-bound (the SMs are idle for most of it): every
             // L2 round trip on its critical path counts.  All candidates come in with independent loads, 4 per thread in flight;
             // the bound, the survivor compaction and the warp lists then work from shared memory.
             float *sk = reinterpret_cast<float *>(fi + p.k);
@@ -330,7 +330,7 @@ __global__ void __launch_bounds__(kScanThreads, 2) flat_scan_kernel(const ScanPa
         B200_TS(5);   // bounds
         // Survivors of the bound are few (~k): every thread first sweeps its share of the candidates with independent loads
         // (no vote between them, so the L2 latencies overlap) and appends survivors to a compact shared array; only those go
-        // through the warp lists.  (The first version voted after every load: 12 dependent L2 round trips, ~12 us of a 45 us call.)
+        // through the warp lists.  (Voting after every load would put 12 dependent L2 round trips on the critical path.)
         if (threadIdx.x == 0) cand_n = 0;
         __syncthreads();
         const float bound_key = list.thr_key;
@@ -692,7 +692,7 @@ __global__ void __launch_bounds__(kScanThreads) topk_merge_ext_kernel(const Merg
 // ------------------------------------------------------------------------------------
 // Exact L2 of the winners.  The tensor-core paths rank by ||y||^2 - 2 x.y (+ ||x||^2), faiss' BLAS form
 // (BruteForceSearch.h:77-88 for nx >= 20); for data far from the origin the expansion cancels and the ~1e-5 relative
-// error of the product (3xTF32, bf16 operands) grows to ~2e-4 of the distance (measured: 768-d clusters at |y|^2 = 840,
+// error of the product (3xTF32, bf16 operands) grows to ~2e-4 of the distance (for example 768-d clusters at |y|^2 = 840,
 // d^2 = 115).  The k winners of every query are therefore re-scored with the direct sum of squared differences in fp32
 // (one warp per winner, the same arithmetic as the scan kernel) and re-ordered by (distance, id).  One CTA per query.
 // ------------------------------------------------------------------------------------

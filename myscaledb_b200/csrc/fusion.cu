@@ -168,9 +168,9 @@ extern "C" int b200_hybrid_fusion_batch(int fusion_type, int64_t nq, const uint3
     const size_t o_vs = carve(nv * 4), o_vp = carve(nv * 8), o_vl = carve(nv * 8), o_vsc = carve(nv * 4), o_vc = carve(nq * 4);
     const size_t o_ts = carve(nt * 4), o_tp = carve(nt * 8), o_tl = carve(nt * 8), o_tsc = carve(nt * 4), o_tc = carve(nq * 4);
     const size_t o_os = carve(no * 4), o_op = carve(no * 8), o_ol = carve(no * 8), o_osc = carve(no * 4), o_oc = carve(nq * 4);
-    // Per-device scratch, grown on demand and kept: a device buffer, a pinned host mirror and a stream of its own.  (The first
-    // version called cudaMalloc / cudaFree and 15 pageable copies on the legacy stream per call: 0.7 ms per 512-query batch
-    // that became 50 ms next to a 160 GB index -- cudaFree synchronises the device and walks the allocator.)
+    // Per-device scratch, grown on demand and kept: a device buffer, a pinned host mirror and a stream of its own.  (cudaMalloc /
+    // cudaFree and pageable copies per call would synchronise the device and walk the allocator, which is slow next to a large
+    // resident index.)
     int dev = 0;
     B200_CUDA_OK(cudaGetDevice(&dev));
     static std::mutex g_mu;

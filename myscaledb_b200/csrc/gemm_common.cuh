@@ -1,5 +1,5 @@
-// gemm_common.cuh -- PTX wrappers (mbarrier, TMA, tcgen05), the per-thread top-k list and the
-// chunk filter shared by the tcgen05 kernels (ip_gemm_sm100.cu, ip_gemm_ts_sm100.cu).
+// gemm_common.cuh -- PTX wrappers (mbarrier, TMA, wgmma), the accumulator hand-off, the per-thread top-k list and the
+// chunk filter shared by the tensor-core kernels (ip_gemm_sm90.cu, ivf_gemm_sm90.cu).
 #pragma once
 #include <cuda.h>
 
@@ -10,44 +10,43 @@ namespace b200 {
 namespace gemm {
 
 
-constexpr int BM = 128;
-constexpr int BN = 256;
-constexpr int BK = 64;
-constexpr int ACC_STAGES = 2;
-constexpr int UMMA_K = 16;
-constexpr int A_BYTES = BM * BK * 2;           // 16 KB
-constexpr int NUM_THREADS = 192;
-constexpr int EPI_THREADS = 128;
-constexpr int TMEM_COLS = 512;
+constexpr int BM = 128;            // queries per CTA tile (two wgmma M = 64 halves)
+constexpr int BN = 256;            // corpus rows per tile (side arrays, pacing, IVF pages)
+constexpr int HN = 128;            // corpus rows per MMA pass: the tile is computed as two N = 128 halves
+constexpr int BK = 64;             // bf16 per k-block = one 128-byte swizzle row
+constexpr int UMMA_K = 16;         // bf16 wgmma K
+constexpr int EPI_THREADS = 128;   // the consumer warpgroup: MMAs, then the top-k epilogue (thread t = query row t)
+constexpr int NUM_THREADS = EPI_THREADS + 32;  // + one TMA producer warp (warp 4)
 constexpr int SMEM_ALIGN_SLACK = 1024;
-constexpr int MAX_STAGES = 6;
+constexpr int MAX_STAGES = 4;
+constexpr int SMEM_LIMIT = 232448;  // 227 KB of opt-in shared memory per block (sm_90)
 
-// CG = CTAs per MMA (cta_group): 1 or 2
 constexpr int SCRATCH_BYTES = 32 * EPI_THREADS * 4;  // epilogue slow-path scratch [32][128] floats
+// Accumulator hand-off: the warpgroup's registers are written column-major into shared memory, 64 columns at a time
+// ([ACC_COLS][ACC_LD] floats; the padding of 4 makes both the fragment stores and the per-row reads of the epilogue
+// conflict-free).  It takes the place of tensor memory: the epilogue reads its query row in chunks of 32 columns.  Staging a
+// quarter of the tile rather than a half keeps 33 KB of shared memory for the operand ring, the lists and the PQ codebook.
+constexpr int ACC_COLS = 64;
+constexpr int ACC_LD = BM + 4;
+constexpr int ACC_BYTES = ACC_COLS * ACC_LD * 4;     // 33 KB
 
-template <int CG>
-struct Cfg {
-    static constexpr int B_ROWS = BN / CG;                 // corpus rows staged by one CTA
-    static constexpr int B_BYTES = B_ROWS * BK * 2;        // 32 KB / 16 KB
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;  // per CTA
-    static constexpr int TX_BYTES = STAGE_BYTES * CG;      // what the (leader's) full barrier expects
-    // smem layout for a ring of `stages` stages (runtime: 6/5 for pairs, 4/3 single, by top-k list size)
-    __host__ __device__ static constexpr int off_a() { return 0; }
-    __host__ __device__ static constexpr int off_b(int stages) { return stages * A_BYTES; }
-    __host__ __device__ static constexpr int off_side(int stages) { return stages * STAGE_BYTES; }  // scale[256], bias[256]
-    __host__ __device__ static constexpr int off_bar(int stages) { return off_side(stages) + 2 * BN * 4; }
-    __host__ __device__ static constexpr int off_scratch(int stages) { return off_bar(stages) + 256; }
-    __host__ __device__ static constexpr int off_list(int stages) { return off_scratch(stages) + SCRATCH_BYTES; }
-    // deepest ring that leaves room for the per-thread lists (k <= kGemmSmemK) in 227 KB
-    __host__ __device__ static int stages_for(int k_smem) {
-        const int max_stages = CG == 1 ? 4 : 6;
-        int st = max_stages;
-        while (st > 2 && off_list(st) + k_smem * EPI_THREADS * 8 + SMEM_ALIGN_SLACK > 232448) st--;
-        return st;
-    }
-    __host__ __device__ static bool lists_fit(int k) {
-        return off_list(2) + k * EPI_THREADS * 8 + SMEM_ALIGN_SLACK <= 232448;   // k: slots per list
-    }
+// Shared-memory layout of the tensor-core kernels for a ring of `st` stages.  Stage s holds the query k-block and the half
+// tile's corpus k-block; fp32 rows (F32X3) add the lo planes of both: [A hi][A lo][B hi][B lo].  Every k-block row is one
+// 128-byte swizzle row (64 bf16 or 32 fp32).
+template <bool F32X3>
+struct Layout {
+    static constexpr int KB = F32X3 ? 32 : 64;              // elements per k-block
+    static constexpr int MMA_K = F32X3 ? 8 : 16;
+    static constexpr int A_PLANE = BM * 128;                // 16 KB
+    static constexpr int B_PLANE = HN * 128;                // 16 KB
+    static constexpr int PLANES = F32X3 ? 2 : 1;            // hi / lo
+    static constexpr int STAGE_BYTES = PLANES * (A_PLANE + B_PLANE);
+    static constexpr int TX_BYTES = STAGE_BYTES - (PLANES - 1) * B_PLANE;   // what TMA writes (the B lo plane is computed)
+    __host__ __device__ static constexpr int off_acc(int st) { return st * STAGE_BYTES; }
+    __host__ __device__ static constexpr int off_side(int st) { return off_acc(st) + ACC_BYTES; }  // scale[256], bias[256]
+    __host__ __device__ static constexpr int off_bar(int st) { return off_side(st) + 2 * BN * 4; }
+    __host__ __device__ static constexpr int off_scratch(int st) { return off_bar(st) + 256; }
+    __host__ __device__ static constexpr int off_list(int st) { return off_scratch(st) + SCRATCH_BYTES; }
 };
 
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
@@ -72,18 +71,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t addr, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Experiment knob (default 0 = plain spin, identical code): `make EXTRA=-DB200_MBAR_BACKOFF_NS=64` inserts a nanosleep
-// between failed try_waits.  The committed ncu capture attributes ~30 % of the bf16 kernel's issued instructions to these
-// spin loops; on a power-capped kernel that is worth measuring (DESIGN.md section 6, item 1).
-#ifndef B200_MBAR_BACKOFF_NS
-#define B200_MBAR_BACKOFF_NS 0
-#endif
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     const uint32_t addr = smem_u32(bar);
     while (!mbar_try_wait(addr, parity)) {
-#if B200_MBAR_BACKOFF_NS > 0
-        __nanosleep(B200_MBAR_BACKOFF_NS);
-#endif
     }
 }
 
@@ -95,48 +85,7 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap *map, uint64_t *ba
         : "memory");
 }
 
-// 2-CTA form: dst in this CTA, completion signalled on the LEADER CTA's mbarrier (the shared
-// window address carries the CTA rank in bit 24; clearing it names the even CTA of the pair).
-__device__ __forceinline__ void tma_load_2d_cg2(const CUtensorMap *map, uint64_t *bar, void *dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-        "[%2];" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-        : "memory");
-}
-
-// 2-CTA + multicast: the box is written at the same CTA-relative offset in every CTA of cta_mask and
-// completes bytes on the mbarrier at `bar`'s offset in the LEADER of each destination's pair.
-__device__ __forceinline__ void tma_load_2d_cg2_mc(const CUtensorMap *map, uint64_t *bar, void *dst, int c0, int c1, uint16_t cta_mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster "
-        "[%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "h"(cta_mask)
-        : "memory");
-}
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t *bar, uint32_t cta) {
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 remote;\n\t"
-        "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
-        "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(cta)
-        : "memory");
-}
-// one lane of a converged warp (keeps the surrounding control flow warp-uniform, so the
-// compiler holds descriptors / barrier addresses in uniform registers)
+// one lane of a converged warp (keeps the surrounding control flow warp-uniform)
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile(
@@ -149,77 +98,93 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
-// K-major, 128-byte swizzled operand tile: rows of 64 bf16 (128 B), 8-row atoms of 1024 B.
+// named barrier of the consumer warpgroup (id 1; 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+
+// wgmma shared-memory descriptor of a K-major, 128-byte swizzled operand tile: rows of 128 B, 8-row atoms of 1024 B.
+// Other stages / k-steps / row offsets are plain adds on the 14-bit (address >> 4) field (shared addresses < 2^18).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);  // start address
-    d |= (uint64_t)1 << 16;                      // leading byte offset (unused for SW128 K-major)
+    d |= (uint64_t)1 << 16;                      // leading byte offset (unused for swizzled K-major)
     d |= (uint64_t)(1024 >> 4) << 32;            // stride byte offset: 8 rows * 128 B
-    d |= (uint64_t)1 << 46;                      // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                      // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                      // SWIZZLE_128B
     return d;
 }
 
-// kind::f16, A = B = bf16 (K-major), D = f32, M = 128 * CG, N = 256
-__device__ __forceinline__ constexpr uint32_t make_idesc(int cg) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)((BM * cg) >> 4) << 24);
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+#define B200_ACC64(v)                                                                                                           \
+    "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]), "+f"(v[8]), "+f"(v[9]),     \
+        "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15]), "+f"(v[16]), "+f"(v[17]), "+f"(v[18]),    \
+        "+f"(v[19]), "+f"(v[20]), "+f"(v[21]), "+f"(v[22]), "+f"(v[23]), "+f"(v[24]), "+f"(v[25]), "+f"(v[26]), "+f"(v[27]),    \
+        "+f"(v[28]), "+f"(v[29]), "+f"(v[30]), "+f"(v[31]), "+f"(v[32]), "+f"(v[33]), "+f"(v[34]), "+f"(v[35]), "+f"(v[36]),    \
+        "+f"(v[37]), "+f"(v[38]), "+f"(v[39]), "+f"(v[40]), "+f"(v[41]), "+f"(v[42]), "+f"(v[43]), "+f"(v[44]), "+f"(v[45]),    \
+        "+f"(v[46]), "+f"(v[47]), "+f"(v[48]), "+f"(v[49]), "+f"(v[50]), "+f"(v[51]), "+f"(v[52]), "+f"(v[53]), "+f"(v[54]),    \
+        "+f"(v[55]), "+f"(v[56]), "+f"(v[57]), "+f"(v[58]), "+f"(v[59]), "+f"(v[60]), "+f"(v[61]), "+f"(v[62]), "+f"(v[63])
+#define B200_ACC64_REGS                                                                                                         \
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, " \
+    "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "   \
+    "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, bf16 operands (both K-major in shared memory), fp32 accumulators
+__device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " B200_ACC64_REGS ", %64, %65, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : B200_ACC64(d)
+        : "l"(adesc), "l"(bdesc), "r"(accum));
 }
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void umma_cg2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// D[64 x 128] (+)= A[64 x 8] * B[128 x 8]^T, tf32 operands (K-major), fp32 accumulators
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " B200_ACC64_REGS ", %64, %65, p, 1, 1;\n\t"
+        "}\n"
+        : B200_ACC64(d)
+        : "l"(adesc), "l"(bdesc), "r"(accum));
 }
-// arrive (once all prior MMAs retire) on the barrier at this offset in every CTA of `mask` (cluster ranks)
-__device__ __forceinline__ void umma_commit_cg2(uint64_t *bar, uint16_t mask = 3) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(mask)
-        : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, float (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]), "=f"(v[8]),
-          "=f"(v[9]), "=f"(v[10]), "=f"(v[11]), "=f"(v[12]), "=f"(v[13]), "=f"(v[14]), "=f"(v[15]), "=f"(v[16]),
-          "=f"(v[17]), "=f"(v[18]), "=f"(v[19]), "=f"(v[20]), "=f"(v[21]), "=f"(v[22]), "=f"(v[23]), "=f"(v[24]),
-          "=f"(v[25]), "=f"(v[26]), "=f"(v[27]), "=f"(v[28]), "=f"(v[29]), "=f"(v[30]), "=f"(v[31])
-        : "r"(taddr)
-        : "memory");
+// Store columns [64 Q, 64 Q + 64) of the warpgroup's two 64 x 128 accumulator fragments column-major into acc
+// ([ACC_COLS][ACC_LD]).  Fragment layout of wgmma m64nN (fp32 D): warp w, lane l holds rows 16 w + l / 4 (+ 8) and columns
+// 8 i + 2 (l % 4) (+ 1).
+template <int Q>
+__device__ __forceinline__ void acc_store(float *acc, const float (&d0)[64], const float (&d1)[64]) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int r = warp * 16 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < ACC_COLS / 8; j++) {
+        const int i = Q * (ACC_COLS / 8) + j;
+        float *col = acc + (8 * j + c) * ACC_LD + r;
+        col[0] = d0[4 * i];
+        col[ACC_LD] = d0[4 * i + 1];
+        col[8] = d0[4 * i + 2];
+        col[ACC_LD + 8] = d0[4 * i + 3];
+        col[64] = d1[4 * i];
+        col[ACC_LD + 64] = d1[4 * i + 1];
+        col[72] = d1[4 * i + 2];
+        col[ACC_LD + 72] = d1[4 * i + 3];
+    }
 }
-// all tcgen05.ld issued by this thread have landed in their registers
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// this thread's query row, 32 columns from column c0 of the staged accumulator
+__device__ __forceinline__ void acc_load32(const float *acc, int row, int c0, float (&v)[32]) {
+    const float *p = acc + c0 * ACC_LD + row;
+#pragma unroll
+    for (int j = 0; j < 32; j++) v[j] = p[j * ACC_LD];
+}
 
 // Per-thread top-k as an UNSORTED buffer (element j at [j * EPI_THREADS]: bank-conflict free in smem,
 // coalesced in global scratch) plus the position of its current worst element.  An insert overwrites
-// the worst slot and rescans the k slots with independent loads (~60 cycles at k = 10); the first
-// version kept the list sorted and paid a dependent load-compare-store chain per shifted element
-// (~400 cycles per insert, 1.7 ms of start-up "insert storm" per launch, profiles/r01_summary.md).
+// the worst slot and rescans the k slots with independent loads; a sorted list would pay a dependent
+// load-compare-store chain per shifted element, which makes the start-up "insert storm" of a launch expensive.
 // The buffer is sorted once, when the CTA publishes its partial list.
 struct ThreadTopK {
     float *keys;       // entry j of this thread's list: keys[j * stride]
@@ -238,17 +203,16 @@ struct ThreadTopK {
 //  * interleaved lists, each lane inserts into its own list -- the default at every k;
 //  * contiguous lists and COOPERATIVE inserts (k >= B200_LIST_COOP_MIN_K, off by default): the accepted candidate of one lane
 //    is broadcast, lane 0 overwrites that list's worst entry, all 32 lanes rescan the list (k / 32 entries each) and a shuffle
-//    arg-max yields the new worst.  Measured (profiles/r02_list_modes.md): it does NOT pay.  A slow-path event carries ~5
-//    candidates spread over the lanes; the one-lane form retires them in ~1.5 parallel rounds of one k-entry rescan each, the
-//    cooperative form in ~5 serial steps of ~100 instructions -- 15.6 vs 13.2 ms per launch at k = 17 / 16, 17.9 vs 14.4 at
-//    k = 30, equal at k = 100.  Kept for the unit test and the record.
+//    arg-max yields the new worst.  It did not pay where it was measured (an earlier GPU; not re-measured on the H100): a
+//    slow-path event carries a few candidates spread over the lanes, which the one-lane form retires in parallel rounds of one
+//    k-entry rescan each and the cooperative form in serial steps.  Kept for the unit test.
 #ifndef B200_LIST_COOP_MIN_K
 #define B200_LIST_COOP_MIN_K (1 << 30)
 #endif
 constexpr int kListCoopMinK = B200_LIST_COOP_MIN_K;
 // Element j of a list sits at keys[j * LIST_STRIDE(t)].  Production builds have no contiguous (cooperative) lists, so the stride is
-// the compile-time constant EPI_THREADS and the rescans address their entries with immediate offsets; a run-time stride cost the
-// default form 16 % at k = 30 and 36 % at k = 100 (profiles/r02_gpu35.log vs r02_gpu22.log).
+// the compile-time constant EPI_THREADS and the rescans address their entries with immediate offsets (a run-time stride costs
+// an address computation per entry of every rescan).
 #if B200_LIST_COOP_MIN_K >= (1 << 30)
 #define LIST_STRIDE(t) EPI_THREADS
 #else
@@ -270,11 +234,10 @@ __device__ __forceinline__ void list_bind(ThreadTopK &t, float *keys_base, uint3
 //    worst -- O(k) dependent-free loads per insert; the threshold is always exact.
 //  * append (cap >= 2k + 32, opt-in): an accepted candidate is stored behind the others (two stores, nothing to wait for);
 //    when some lane of the warp is within 32 slots of the end, EVERY lane of the warp compacts its own buffer in lock-step
-//    (quickselect for the k-th entry, then one partition pass) and tightens its threshold.  Measured on a synthetic stream
-//    shaped like the flat kernel's epilogue (tests/cuda/list_perf.cu, profiles/r02_list_modes.md): in shared memory it
-//    halves the list cost at k = 100 (+8 ms against +21 ms per launch) and is equal at k <= 30, but it needs twice the
-//    slots -- 200 KB at k = 100, which the operand ring does not leave -- and from global scratch it is no better than
-//    the rescan form in shared memory.  The slack must be real: with k + 32 slots every slow-path event compacts (3x slower).
+//    (quickselect for the k-th entry, then one partition pass) and tightens its threshold.  It needs twice the slots -- 200 KB
+//    at k = 100, which the operand ring does not leave -- and from global scratch it loses the point of cheap inserts; the
+//    slack must be real: with k + 32 slots every slow-path event compacts.  tests/cuda/list_perf.cu times both forms on a
+//    synthetic stream shaped like the flat kernel's epilogue; they have not been compared on the H100.
 // (slot counts: list_cap_for / list_cap_append in kernels.h)
 
 struct ListThr {
@@ -578,8 +541,8 @@ __device__ __forceinline__ void list_insert_coop(ThreadTopK &t, int src, float k
 // done.  Slow path (some lane of the warp can improve its list; frequent only during the first
 // tiles of a launch): every lane parks its 32 keys in a shared-memory scratch column and the WARP
 // loops while any lane still has a candidate bit, each lane popping its own lowest bit and doing
-// an inlined insert.  Compared with per-element calls under divergence this removed a fixed
-// ~1.3 ms "insert storm" per launch (profiles/r01_summary.md).
+// an inlined insert (per-element calls under divergence serialise the lanes during the start-up
+// "insert storm" of a launch).
 // scratch: this thread's column of a [32][EPI_THREADS] float array.
 __device__ __forceinline__ void epilogue_chunk(ThreadTopK &list, float (&v)[32], bool use_side, const float *scale,
                                                const float *bias, uint32_t id0, bool tail, int64_t n, float *scratch,

@@ -29,7 +29,7 @@ struct Stager {
     cudaEvent_t ev[kSlots] = {};
     bool tried = false;
     // events belong to the device that is current when they are created: one stager per device, created with that
-    // device current (round 1 kept one process-wide event set and failed on the second GPU of a multi-device process)
+    // device current (one process-wide event set fails on the second GPU of a multi-device process)
     bool init(int device) {
         if (tried) return pinned != nullptr;
         tried = true;

@@ -1,0 +1,365 @@
+// ip_gemm_sm90.cu -- K2: batched multi-query x corpus inner product as a dense GEMM on the Hopper tensor cores
+// (wgmma, operands staged by TMA), with the top-k selection FUSED into the epilogue: the [nq x N] score matrix is
+// never written to memory.  Two operand types share the kernel:
+//   * bf16 queries x bf16 corpus (K2);
+//   * fp32 queries x fp32 corpus with fp32-level accuracy ("3xTF32", K2b): every fp32 value is split into two TF32
+//     numbers  x = hi + lo  (hi = x with the low 13 mantissa bits cleared, lo = tf32(x - hi)) and
+//     q.y = q_lo.y_hi + q_hi.y_lo + q_hi.y_hi  (+ q_lo.y_lo ~ 2^-22, dropped) is accumulated in fp32 by three wgmma per
+//     k-step: error ~2^-21 relative per product, the same class as an fp32 FMA chain in another summation order
+//     (tests/test_gpu_flat.py bounds it).  The queries are split once per batch (split_tf32_kernel); the corpus k-block
+//     is split in shared memory by the consumer warpgroup itself while the previous k-block's MMAs run.
+//
+// Replaces faiss::knn_inner_product / knn_L2sqr for nx >= 20 (the BLAS sgemm path) reached from tryBruteForceSearch
+// (reference: VectorIndex/Common/BruteForceSearch.h:77-88) and the FLAT Search::VectorIndex::search scan
+// (VectorIndex/Common/VIWithDataPart.cpp:926).
+//
+// One CTA = 128 queries (one query tile for its whole life) x corpus tiles of 256 rows (worker, worker + W, ...):
+//   warps 0..3  consumer warpgroup: a tile is computed as two N = 128 halves; per half, two wgmma m64n128 (query rows
+//               0..63 / 64..127) per k-step accumulate in registers, the result is staged column-major in shared memory
+//               and thread t then filters query row t in chunks of 32 columns into its private top-k list;
+//   warp 4      TMA producer (one lane): A = the query k-block, B = the half tile's corpus k-block, ring of full/empty
+//               mbarriers.
+// The key that is ranked is  acc * row_scale[j] + row_bias[j]  (smaller = better):
+//   IP: -acc | L2: ||y||^2 - 2 acc (+||q||^2 added at merge) | cosine: -acc / ||y||;  filtered / out-of-range rows: scale
+//   0, bias +inf.
+#include <cstdlib>
+
+#include "gemm_common.cuh"
+
+namespace b200 {
+namespace gemm {
+
+// Ring depth and list placement per operand type (layout: Layout in gemm_common.cuh)
+template <bool F32X3>
+struct Op : Layout<F32X3> {
+    using L = Layout<F32X3>;
+    static constexpr int MAX_ST = F32X3 ? 2 : 4;
+    static int stages_for(int k_smem) {
+        int st = MAX_ST;
+        while (st > 2 && L::off_list(st) + k_smem * EPI_THREADS * 8 + SMEM_ALIGN_SLACK > SMEM_LIMIT) st--;
+        return st;
+    }
+    static bool lists_fit(int k) { return L::off_list(2) + k * EPI_THREADS * 8 + SMEM_ALIGN_SLACK <= SMEM_LIMIT; }
+    static size_t smem_bytes(int st, int k_smem) { return (size_t)L::off_list(st) + (size_t)k_smem * EPI_THREADS * 8 + SMEM_ALIGN_SLACK; }
+};
+
+// x = hi + lo with both parts exactly representable in TF32 (so the result does not depend on how the tensor core
+// would round a raw fp32 operand).  hi by truncation: FLT_MAX (the reference's padding value for empty rows,
+// MergeTreeVSManager.cpp:1380) stays finite.
+__device__ __forceinline__ void split_tf32(uint32_t x, uint32_t &hi, uint32_t &lo) {
+    hi = x & 0xffffe000u;
+    const float r = __uint_as_float(x) - __uint_as_float(hi);
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
+}
+
+__global__ void split_tf32_kernel(const float *__restrict__ src, int64_t n_src, int d_pad, float *__restrict__ hi,
+                                  float *__restrict__ lo, int64_t n_pad) {
+    const int64_t total = n_pad * d_pad;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / d_pad;
+        uint32_t h = 0, l = 0;
+        if (r < n_src) split_tf32(__float_as_uint(src[i]), h, l);
+        hi[i] = __uint_as_float(h);
+        lo[i] = __uint_as_float(l);
+    }
+}
+
+template <bool F32X3>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_qlo,
+                 const __grid_constant__ CUtensorMap map_c, const GemmTopkParams p) {
+    using O = Op<F32X3>;
+    const int STAGES = p.stages;
+    extern __shared__ unsigned char smem_dyn[];
+    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
+    // stage s: [A hi][A lo][B (hi after the split)][B lo], planes present per operand type
+    float *acc = reinterpret_cast<float *>(smem + O::off_acc(STAGES));
+    float *side_scale = reinterpret_cast<float *>(smem + O::off_side(STAGES));
+    float *side_bias = side_scale + BN;
+    uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + O::off_bar(STAGES));
+    uint64_t *empty_bar = full_bar + MAX_STAGES;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int qt = blockIdx.x % p.q_tiles;
+    const int worker = blockIdx.x / p.q_tiles;
+    const int W = gridDim.x / p.q_tiles;  // the host launches a multiple of q_tiles CTAs
+    const int64_t n_tiles = (p.n + BN - 1) / BN;
+    const int kb_count = (p.d_pad + O::KB - 1) / O::KB;
+
+    if (warp == 4 && lane == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_q)) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_c)) : "memory");
+        for (int i = 0; i < STAGES; i++) {
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], 4);  // one arrival per consumer warp
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp == 4) {
+        // ===================== TMA producer =====================
+        int stage = 0;
+        uint32_t phase = 0;
+        int ordinal = 0;
+        bool pacing = p.progress != nullptr;
+        for (int64_t t = worker; t < n_tiles; t += W, ordinal++) {
+            // Pacing: the CTAs that stream the SAME corpus tiles for different query tiles stay within `sync_slack`
+            // tiles of each other, so a tile is fetched from HBM once and served to the others from L2.  Only pacing, no
+            // data dependency: plain volatile counters.  Bounded wait (~50 us): if the sharers are not co-resident
+            // (another kernel holds SMs) pacing is dropped instead of risking a co-residency deadlock.
+            if (pacing) {
+                int ok = 1;
+                if (lane == 0) {
+                    volatile int *prog = p.progress + (size_t)worker * p.q_tiles;
+                    prog[qt] = ordinal + 1;
+                    int spins = 0;
+                    for (int g = 0; g < p.q_tiles; g++)
+                        while (prog[g] < ordinal + 1 - p.sync_slack && spins < 256) {
+                            __nanosleep(200);
+                            spins++;
+                        }
+                    if (spins >= 256) prog[qt] = 0x7fffffff;  // never hold anybody back again
+                    ok = spins < 256;
+                }
+                pacing = __shfl_sync(0xffffffffu, ok, 0) != 0;
+            }
+            __syncwarp();
+            for (int h = 0; h < BN / HN; h++) {
+                for (int kb = 0; kb < kb_count; kb++) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    if (elect_one()) {
+                        unsigned char *st = smem + stage * O::STAGE_BYTES;
+                        mbar_arrive_expect_tx(&full_bar[stage], O::TX_BYTES);
+                        tma_load_2d(&map_q, &full_bar[stage], st, kb * O::KB, qt * BM);
+                        if (F32X3) tma_load_2d(&map_qlo, &full_bar[stage], st + O::A_PLANE, kb * O::KB, qt * BM);
+                        tma_load_2d(&map_c, &full_bar[stage], st + O::PLANES * O::A_PLANE, kb * O::KB, (int)(t * BN + h * HN));
+                    }
+                    __syncwarp();
+                    if (++stage == STAGES) {
+                        stage = 0;
+                        phase ^= 1;
+                    }
+                }
+            }
+        }
+    } else {
+        // ===================== consumer warpgroup: MMAs, then the fused top-k =====================
+        const int row = threadIdx.x;  // query row inside the tile
+        const bool use_side = p.row_scale || p.row_bias || p.alive || p.scale_const != -1.f;
+        float *scratch = reinterpret_cast<float *>(smem + O::off_scratch(STAGES)) + row;
+        ThreadTopK list;
+        list.n = 0;
+        list.worst = 0;
+        // rows past the batch (zero padding up to the tile size) must never pay for the slow path: nothing beats -FLT_MAX
+        list.thr_key = (qt * BM + row < p.nq_valid) ? FLT_MAX : -FLT_MAX;
+        list.thr_id = 0;
+        if (p.lists_in_smem)
+            list_bind(list, reinterpret_cast<float *>(smem + O::off_list(STAGES)),
+                      reinterpret_cast<uint32_t *>(smem + O::off_list(STAGES) + (size_t)p.list_cap * EPI_THREADS * 4), row, p.k, p.list_cap);
+        else
+            list_bind(list, p.list_keys_gmem + (size_t)blockIdx.x * p.list_cap * EPI_THREADS,
+                      p.list_ids_gmem + (size_t)blockIdx.x * p.list_cap * EPI_THREADS, row, p.k, p.list_cap);
+        const uint32_t smem0 = smem_u32(smem);
+        int stage = 0;
+        uint32_t phase = 0;
+        float d0[64], d1[64];
+        for (int64_t t = worker; t < n_tiles; t += W) {
+            const int64_t n0 = t * BN;
+            // this tile's side entries (in flight during the MMAs; written after the barrier below)
+            float sc[BN / EPI_THREADS], bi[BN / EPI_THREADS];
+            if (use_side) {
+#pragma unroll
+                for (int i = 0; i < BN / EPI_THREADS; i++) {
+                    const int64_t r = n0 + row + i * EPI_THREADS;
+                    bool ok = r < p.n;
+                    if (ok && p.alive) ok = (p.alive[r >> 3] >> (r & 7)) & 1;
+                    sc[i] = ok ? (p.row_scale ? p.row_scale[r] : p.scale_const) : 0.f;
+                    bi[i] = ok ? (p.row_bias ? p.row_bias[r] : 0.f) : __int_as_float(0x7f800000);
+                }
+            }
+            const bool tail = n0 + BN > p.n;
+            for (int h = 0; h < BN / HN; h++) {
+                int prev = -1;
+                for (int kb = 0; kb < kb_count; kb++) {
+                    mbar_wait(&full_bar[stage], phase);
+                    const uint32_t st = smem0 + stage * O::STAGE_BYTES;
+                    if (F32X3) {
+                        // corpus k-block -> (y_hi in place, y_lo in the 4th plane); same swizzled offsets
+                        uint4 *b = reinterpret_cast<uint4 *>(smem + stage * O::STAGE_BYTES + 2 * O::A_PLANE);
+                        uint4 *bl = b + O::B_PLANE / 16;
+#pragma unroll
+                        for (int i = 0; i < O::B_PLANE / 16 / EPI_THREADS; i++) {
+                            const uint4 raw = b[row + i * EPI_THREADS];
+                            uint4 hi, lo;
+                            split_tf32(raw.x, hi.x, lo.x);
+                            split_tf32(raw.y, hi.y, lo.y);
+                            split_tf32(raw.z, hi.z, lo.z);
+                            split_tf32(raw.w, hi.w, lo.w);
+                            b[row + i * EPI_THREADS] = hi;
+                            bl[row + i * EPI_THREADS] = lo;
+                        }
+                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic stores -> wgmma operand reads
+                        wg_bar();
+                    }
+                    wgmma_fence();
+                    if (F32X3) {
+                        const uint64_t ahi = make_smem_desc(st), alo = make_smem_desc(st + O::A_PLANE);
+                        const uint64_t b = make_smem_desc(st + 2 * O::A_PLANE), blo = make_smem_desc(st + 2 * O::A_PLANE + O::B_PLANE);
+                        constexpr uint64_t M1 = (64 * 128) >> 4;  // second M half: 64 rows further
+#pragma unroll
+                        for (int k = 0; k < O::KB / O::MMA_K; k++) {
+                            const uint64_t off = (uint64_t)(k * (O::MMA_K * 4 >> 4));
+                            const uint32_t acc0 = (kb | k) != 0 ? 1u : 0u;  // small terms first
+                            wgmma_tf32_n128(d0, alo + off, b + off, acc0);
+                            wgmma_tf32_n128(d1, alo + M1 + off, b + off, acc0);
+                            wgmma_tf32_n128(d0, ahi + off, blo + off, 1u);
+                            wgmma_tf32_n128(d1, ahi + M1 + off, blo + off, 1u);
+                            wgmma_tf32_n128(d0, ahi + off, b + off, 1u);
+                            wgmma_tf32_n128(d1, ahi + M1 + off, b + off, 1u);
+                        }
+                    } else {
+                        const uint64_t a = make_smem_desc(st), b = make_smem_desc(st + O::A_PLANE);
+                        constexpr uint64_t M1 = (64 * 128) >> 4;
+#pragma unroll
+                        for (int k = 0; k < O::KB / O::MMA_K; k++) {
+                            const uint64_t off = (uint64_t)(k * (O::MMA_K * 2 >> 4));
+                            const uint32_t acc0 = (kb | k) != 0 ? 1u : 0u;
+                            wgmma_bf16_n128(d0, a + off, b + off, acc0);
+                            wgmma_bf16_n128(d1, a + M1 + off, b + off, acc0);
+                        }
+                    }
+                    wgmma_commit();
+                    // the previous k-block's MMAs have retired: its stage goes back to the producer
+                    wgmma_wait<1>();
+                    if (prev >= 0) {
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                    }
+                    prev = stage;
+                    if (++stage == STAGES) {
+                        stage = 0;
+                        phase ^= 1;
+                    }
+                }
+                wgmma_wait<0>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+#pragma unroll
+                for (int q = 0; q < HN / ACC_COLS; q++) {
+                    wg_bar();  // every row's reads of the previous staging (and of the previous tile's side arrays) are done
+                    if (h == 0 && q == 0 && use_side) {
+#pragma unroll
+                        for (int i = 0; i < BN / EPI_THREADS; i++) {
+                            side_scale[row + i * EPI_THREADS] = sc[i];
+                            side_bias[row + i * EPI_THREADS] = bi[i];
+                        }
+                    }
+                    if (q == 0) acc_store<0>(acc, d0, d1);
+                    else acc_store<1>(acc, d0, d1);
+                    wg_bar();
+                    // Chunks of 32 columns.  A chunk is first reduced to its best key (31 FMNMX); the per-element test only
+                    // runs for the rare chunk that can beat the current k-th key.
+#pragma unroll 1
+                    for (int cc = 0; cc < ACC_COLS / 32; cc++) {
+                        float v[32];
+                        acc_load32(acc, row, cc * 32, v);
+                        const int c0 = h * HN + q * ACC_COLS + cc * 32;
+                        epilogue_chunk(list, v, use_side, side_scale + c0, side_bias + c0, (uint32_t)(n0 + c0), tail, p.n, scratch);
+                    }
+                }
+            }
+        }
+        // publish this CTA's per-query partial list
+        float *ok = p.part_keys + ((size_t)blockIdx.x * BM + row) * p.k;
+        uint32_t *oi = p.part_ids + ((size_t)blockIdx.x * BM + row) * p.k;
+        list_publish(list, ok, oi);
+    }
+}
+
+// 2-D tensor map over row-major [rows][d_pad] (bf16 or fp32), box = [box_rows][one 128-byte row], 128-byte swizzle.
+// fp32: the last k-block may hang over d_pad (TMA zero-fills), so fp32 corpora keep their 16-byte row padding.
+static bool encode_map(CUtensorMap *map, const void *base, int64_t rows, int d_pad, int box_rows, bool f32) {
+    EncodeTiledFn fn = get_encode_fn();
+    if (!fn) return false;
+    const int es = f32 ? 4 : 2;
+    const cuuint64_t dims[2] = {(cuuint64_t)d_pad, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)d_pad * es};
+    const cuuint32_t box[2] = {(cuuint32_t)(128 / es), (cuuint32_t)box_rows};
+    const cuuint32_t estr[2] = {1, 1};
+    return fn(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(base), dims, strides, box,
+              estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+template <bool F32X3>
+static cudaError_t launch(const CUtensorMap &map_q, const CUtensorMap &map_qlo, const CUtensorMap &map_c, const GemmTopkParams &p_in,
+                          int grid, cudaStream_t s) {
+    using O = Op<F32X3>;
+    GemmTopkParams p = p_in;
+    // Per-thread lists sit in shared memory whenever they fit, even when that squeezes the operand ring: every insert rescans
+    // the list, and from global scratch that is k L2 round trips.
+    p.list_cap = list_cap_for(p.k);
+    p.lists_in_smem = O::lists_fit(p.list_cap) ? 1 : 0;
+    const int k_smem = p.lists_in_smem ? p.list_cap : 0;
+    p.stages = O::stages_for(k_smem);
+    const size_t smem = O::smem_bytes(p.stages, k_smem);
+    auto kern = gemm_topk_kernel<F32X3>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    kern<<<grid, NUM_THREADS, smem, s>>>(map_q, map_qlo, map_c, p);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+}  // namespace gemm
+
+int gemm_topk_grid(int q_tiles, int64_t n, int num_sms) {
+    const int64_t n_tiles = ceil_div(n, gemm::BN);
+    int64_t g = (int64_t)q_tiles * (n_tiles < 1 ? 1 : n_tiles);
+    if (g > num_sms) g = num_sms;
+    if (g < q_tiles) g = q_tiles;
+    return (int)g;
+}
+
+cudaError_t launch_split_tf32(const float *src, int64_t n_src, int d_pad, float *hi, float *lo, int64_t n_pad, cudaStream_t s) {
+    if (n_pad == 0) return cudaSuccess;
+    int64_t b = ceil_div(n_pad * d_pad, 256);
+    if (b > 132 * 8) b = 132 * 8;
+    gemm::split_tf32_kernel<<<(int)b, 256, 0, s>>>(src, n_src, d_pad, hi, lo, n_pad);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_gemm_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail) {
+    *err_detail = nullptr;
+    if (grid % p.q_tiles != 0) {
+        *err_detail = "grid must be a multiple of q_tiles";
+        return cudaErrorInvalidValue;
+    }
+    CUtensorMap map_q, map_c;
+    if (!gemm::encode_map(&map_q, p.queries_bf16, p.nq_pad, p.d_pad, gemm::BM, false) ||
+        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::HN, false)) {
+        *err_detail = "cuTensorMapEncodeTiled failed";
+        return cudaErrorInvalidValue;
+    }
+    return gemm::launch<false>(map_q, map_q, map_c, p, grid, s);
+}
+
+cudaError_t launch_gemm3_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail) {
+    *err_detail = nullptr;
+    if (grid % p.q_tiles != 0 || !p.queries_lo) {
+        *err_detail = "gemm3: grid must be a multiple of q_tiles, queries_lo set";
+        return cudaErrorInvalidValue;
+    }
+    CUtensorMap map_qhi, map_qlo, map_c;
+    if (!gemm::encode_map(&map_qhi, p.queries_bf16, p.nq_pad, p.d_pad, gemm::BM, true) ||
+        !gemm::encode_map(&map_qlo, p.queries_lo, p.nq_pad, p.d_pad, gemm::BM, true) ||
+        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::HN, true)) {
+        *err_detail = "cuTensorMapEncodeTiled failed";
+        return cudaErrorInvalidValue;
+    }
+    return gemm::launch<true>(map_qhi, map_qlo, map_c, p, grid, s);
+}
+
+}  // namespace b200

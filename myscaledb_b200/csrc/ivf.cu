@@ -9,13 +9,13 @@
 // IVF ones, the layout and the execution model are ours:
 //   * coarse quantiser: nlist fp32 centroids, k-means on device (assignment = exact top-1 search of the centroid table
 //     on the tensor cores, 3xTF32);
-//   * PAGED inverted lists: a page = 256 consecutive rows of one list in a pre-reserved pool (exactly one tcgen05 tile);
+//   * PAGED inverted lists: a page = 256 consecutive rows of one list in a pre-reserved pool (exactly one tensor-core tile);
 //     `add` appends chunk after chunk (assign -> sort by list -> allocate pages by prefix sums -> scatter), nothing is
 //     ever compacted or moved, so 100 M x 768 rows stream through a few GB of scratch (VIPartReader's chunked build);
 //   * payload of a row: bf16 vector (IVFFLAT / MSTG-class first stage), one byte per dimension (IVFSQ) or m PQ codes of
 //     the residual (IVFPQ / SCANN-class); + its row id and, for L2, the norm term of the expanded distance;
 //   * search: coarse top-nprobe, then ALL (query, list) pairs of the batch are radix-sorted by list and cut into work
-//     items (<= 128 queries x a run of pages) for the grouped tensor-core scan of ivf_gemm_sm100.cu, so a list is read
+//     items (<= 128 queries x a run of pages) for the grouped tensor-core scan of ivf_gemm_sm90.cu, so a list is read
 //     from HBM once per batch however many queries probe it; per-pair partial lists are merged per query;
 //   * optional fp32 rows in id order (`keep_raw`) for the exact second stage (refine_kernel, warp per candidate).
 #include <algorithm>
@@ -190,7 +190,7 @@ __global__ void iota_kernel(uint32_t *v, int64_t n) {
 
 static inline int gridsz(int64_t work, int threads = 256) {
     int64_t b = ceil_div(work, threads);
-    return (int)std::max<int64_t>(1, std::min<int64_t>(b, 148 * 32));
+    return (int)std::max<int64_t>(1, std::min<int64_t>(b, 132 * 32));
 }
 
 // ------------------------------------------------------------------------------------
@@ -521,7 +521,7 @@ __global__ void __launch_bounds__(1024) search_plan_kernel(const SearchPlan p) {
 // ------------------------------------------------------------------------------------
 // Coarse probe for nprobe > 8: the centroid table is small (nlist x d fp32, L2-resident) and nprobe is a large k for it --
 // the fused top-k kernels keep one k-entry list per query and, with only nlist / workers rows per list, almost every row is
-// an insert (measured 21 ms for 10 000 queries x 4 096 centroids x 96, nprobe 32, on either path).  Here the ranking keys
+// an insert.  Here the ranking keys
 // ||c||^2 - 2 <x, c> of a chunk of queries are written out by a plain fp32 tile kernel (64 x 64 tiles, 4 x 4 per thread) and
 // one warp per query selects its nprobe smallest with a sorted warp list: scores are read once, coalesced, and an insert is
 // O(nprobe / 32).
@@ -890,7 +890,7 @@ struct b200_index {
     uint32_t *d_list_page_off = nullptr, *d_list_pages = nullptr, *d_list_order = nullptr;   // after finalize
     std::vector<uint32_t> list_len;  // host copy after finalize
     uint32_t max_list_pages = 0;
-    int device = 0, sms = 148;
+    int device = 0, sms = 132;
     cudaStream_t stream = nullptr;
     std::mutex mu;
     // workspaces (grow-only)
@@ -1644,9 +1644,10 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
     {
         // The centroid table is small and nprobe is a large k for it: the tensor-core path keeps one k-list per query lane
-        // and never gets a selective threshold when k / nlist is a few percent (measured 9 ms for 10 000 x 4096 x 96, k = 32).
-        // The scan kernel's warp lists cost O(k / 32) per insert: use it when its estimated time (FMA-bound at ~1.4 TB/s of
-        // table bytes per 8-query pass) undercuts ~1 us per (query, 32 probes) of the tensor-core path.
+        // and never gets a selective threshold when k / nlist is a few percent.  The scan kernel's warp lists cost O(k / 32) per
+        // insert: use it when its estimated time (FMA-bound, ~1.4 TB/s of table bytes per 8-query pass) undercuts ~1 us per
+        // (query, 32 probes) of the tensor-core path.  Both rates of this model were taken on an earlier GPU and are
+        // not re-measured on the H100; they only pick between two exact paths.
         const double t_scan = (double)ceil_div(nq, 8) * nl * ix->d_pad * 4.0 / 1.4e12;
         const double t_gemm = 1e-6 * (double)nq * std::max(1.0, nprobe / 32.0) + 30e-6;
         bool use_scan = nprobe > 8 && t_scan < t_gemm;
@@ -1701,18 +1702,17 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     //      chosen from host-side knowledge only (no device -> host round trip on the query path).
     // Lists are cut into chunks of `ppc` pages: an item never streams more than 16 pages (bounds the tail of the static
     // round-robin schedule), and small batches are split further so that every SM gets ~4 items.  Finer is NOT better: every item
-    // pays one cold start of its top-k lists (sweep at 100 M x 768, nprobe 1: 4-page items 0.64 of the HBM peak, 8 to 16-page
-    // items 0.77-0.78; nprobe 4: 0.33 vs 0.45; profiles/r02_gpu17_*).  The estimate uses host-side knowledge only (no device ->
-    // host round trip on the query path): probed lists <= min(pairs, nlist), their length size-biased.
+    // pays one cold start of its top-k lists.  The page counts (8 to 16, 48 below) were chosen on an earlier GPU and are
+    // not re-measured on the H100.  The estimate uses host-side knowledge only (no device -> host round trip on the query path): probed
+    // lists <= min(pairs, nlist), their length size-biased.
     const double avg_pages = std::max(1.0, (double)ix->pages_used / std::max(1, nl));
     const double est_lists = std::min<double>((double)n_pairs, (double)nl);
     const double est_pages = est_lists * std::min<double>(ix->max_list_pages ? ix->max_list_pages : 1, 1.5 * avg_pages);
     uint32_t ppc;
     {
         const double want_items = 4.0 * ix->sms;
-        // Lists probed by more than 16 queries run on per-lane top-k lists, whose cold start is paid per item: longer items pay
-        // (cfg-4 shape, ~78 queries per list: 21.5 / 18.6 / 18.5 / 16.5 ms at 8 / 16 / 32 / 48 pages per item, profiles/r02_gpu32.log);
-        // cooperative items (<= 16 queries) keep the 16-page cap (sweep at 100 M x 768 above).
+        // Lists probed by more than 16 queries run on per-lane top-k lists, whose cold start is paid per item: longer items pay;
+        // cooperative items (<= 16 queries) keep the 16-page cap.
         const double q_per_list = (double)n_pairs / std::max(1.0, est_lists);
         const double cap = q_per_list > 16.0 ? 48.0 : 16.0;
         ppc = (uint32_t)std::min(cap, std::max(8.0, std::ceil(est_pages / want_items)));
@@ -1748,7 +1748,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     g_launches++;
     // ---- gather queries, per-pair bookkeeping
     B200_TRY(ix->w_qbuf.reserve(((size_t)n_pairs + 128) * ix->d_pad64 * 2));
-    // the 128 rows behind the last pair are read by the last items' A tiles (TMEM lanes without a query): keep them finite
+    // the 128 rows behind the last pair are read by the last items' A tiles (query slots without a query): keep them finite
     B200_CUDA_OK(cudaMemsetAsync(ix->w_qbuf.as<char>() + (size_t)n_pairs * ix->d_pad64 * 2, 0, (size_t)128 * ix->d_pad64 * 2, s));
     B200_TRY(ix->w_inv.reserve((size_t)n_pairs * 4));
     B200_TRY(ix->w_ppb.reserve((size_t)n_pairs * 4));

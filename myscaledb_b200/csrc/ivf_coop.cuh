@@ -1,4 +1,4 @@
-// ivf_coop.cuh -- tile-wise cooperative top-k of the grouped IVF scan (ivf_gemm_sm100.cu), kept in a header so that
+// ivf_coop.cuh -- tile-wise cooperative top-k of the grouped IVF scan (ivf_gemm_sm90.cu), kept in a header so that
 // tests/cuda/coop_merge_test.cu can drive exactly this code with synthetic tiles and compare it with a CPU sort.
 #pragma once
 #include "gemm_common.cuh"
@@ -8,12 +8,12 @@ namespace gemm {
 
 // Items with only a few queries (the usual case for small batches: every probed list is visited by one or two queries)
 // would leave all the top-k work to one or two lanes of the per-thread scheme, and every item starts with an empty list:
-// ~k ln(rows / k) + k inserts per item, each a latency-bound ~1 us chain (ncu, profiles/r02_ivf_scan_v1: 100 us per page,
-// 52 % of the stall samples on the epilogue barrier behind the one busy warp).  For q_count <= kCoopMax the warp of TMEM
-// lanes 0..31 therefore works TILE-wise and in bulk: lanes whose chunk minimum beats their threshold park the chunk's keys
-// in a per-slot tile buffer; after the tile (TMEM already released to the MMA warp) the warp compacts each slot's
+// ~k ln(rows / k) + k inserts per item, each a latency-bound dependent chain, while the other warps wait on the epilogue
+// barrier behind the one busy warp.  For q_count <= kCoopMax the warp of query
+// slots 0..31 therefore works TILE-wise and in bulk: lanes whose chunk minimum beats their threshold park the chunk's keys
+// in a per-slot tile buffer; after the tile the warp compacts each slot's
 // candidates, sorts them with a bitonic network in shared memory and rank-merges them with the slot's sorted k-list
-// (binary searches, all lanes busy): ~2 us for a full tile of candidates instead of 256 dependent inserts.
+// (binary searches, all lanes busy) instead of up to 256 dependent inserts per tile.
 constexpr int kCoopMax = 16;
 constexpr int kTileBufStride = BN;       // [16][256] floats = exactly the 16 KB slow-path scratch of the per-thread mode, which
                                          // it aliases (an item is either cooperative or per-thread); columns are XOR-swizzled

@@ -1,4 +1,4 @@
-// ivf_gemm.h -- work items and parameters of the grouped tensor-core IVF scan (ivf_gemm_sm100.cu), built by ivf.cu.
+// ivf_gemm.h -- work items and parameters of the grouped tensor-core IVF scan (ivf_gemm_sm90.cu), built by ivf.cu.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

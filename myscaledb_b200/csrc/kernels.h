@@ -74,7 +74,7 @@ cudaError_t launch_topk_merge(const MergeParams &p, bool external, cudaStream_t 
 cudaError_t launch_rescore_l2(const void *corpus, int bf16, int64_t row_bytes, int d_pad, const float *queries, int64_t nq, int64_t id_offset,
                               int k, float *dis, int64_t *ids, cudaStream_t s);
 
-// ---- tcgen05 bf16 GEMM + fused top-k (ip_gemm_sm100.cu) ---------------------------
+// ---- wgmma GEMM + fused top-k (ip_gemm_sm90.cu): bf16 rows, or fp32 rows as 3xTF32 ------------------
 struct GemmTopkParams {
     const void *corpus_bf16;   // [n][d_pad] bf16, d_pad % 64 == 0
     const void *queries_bf16;  // [nq_pad][d_pad] bf16, nq_pad % 128 == 0 (3xTF32 kernel: fp32 hi plane; corpus_bf16 = fp32 rows)
@@ -91,22 +91,17 @@ struct GemmTopkParams {
     int nq_pad, d_pad, k;
     int nq_valid;              // queries actually in the batch (rows past it are padding)
     int q_tiles;               // nq_pad / 128
-    int cta_group;             // 1: one CTA per MMA; 2: CTA pairs (cluster of 2), q_tiles must be even
-    int pairs_per_cluster;     // 1, or 2: two CTA pairs share (TMA-multicast) every corpus tile; q_tiles % 4 == 0
     int *progress;             // [grid / q_tiles][q_tiles] zeroed pacing counters, or null
     int stages;                // smem ring depth (filled in by the launcher)
-    int kps;                   // k-blocks per full/empty barrier stage (1 or 2; filled in by the launcher)
     int lists_in_smem;         // per-thread top-k lists in shared memory (else global scratch); set by the launcher
     int list_cap;              // slots per list: k (rescan mode) or list_cap_append(k) (append mode); set by the launcher
-    int debug;                 // experiments only (B200_GEMM_DEBUG): 1 no epilogue, 2 TMEM loads only, 4 no TMA
     int sync_slack;            // tiles a CTA may run ahead of the slowest sharer of its corpus tiles
 };
-// per-thread top-k lists live in shared memory up to this k (the smem ring gets shallower: 6 stages up to k = 14,
-// 5 up to 46, 4 up to 78, 3 up to 110, 2 up to 128 for CTA pairs); larger k uses global scratch
+// per-thread top-k lists of the IVF scan may live in shared memory up to twice this k (the launcher checks the fit)
 constexpr int kGemmSmemK = 128;
 // per-thread top-k lists (gemm_common.cuh, ThreadTopK): k slots and a rescan per insert (the default), or an append buffer
-// of 2k + 32 slots compacted in lock-step (B200_LIST_APPEND_MIN_K=<k>: lists of at least that k use it; measured in
-// profiles/r02_list_modes.md -- it only pays when the doubled buffer still fits in shared memory, which it does not at k = 100)
+// of 2k + 32 slots compacted in lock-step (B200_LIST_APPEND_MIN_K=<k>: lists of at least that k use it; it can only pay when
+// the doubled buffer still fits in shared memory, which it does not at k = 100)
 __host__ __device__ inline int list_cap_append(int k) { return 2 * k + 32; }
 // tournament form: k entries + one (key, id) slot per group of 8 (k <= 64) or 16 entries holding the group's worst
 // (B200_LIST_TOURN_MIN_K); 16 keeps k = 100 at 107 slots, which still leaves the flat kernel a 3-stage operand ring
@@ -116,13 +111,7 @@ int list_cap_for(int k);   // capi.cu: k, or list_cap_append(k) when the environ
 int gemm_topk_grid(int q_tiles, int64_t n, int num_sms);
 // returns cudaSuccess or an error; tensor maps are encoded inside
 cudaError_t launch_gemm_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail);
-int gemm_topk_max_clusters(int cta_group, int pairs_per_cluster, int k);
-// queries-stationary-in-TMEM form (ip_gemm_ts_sm100.cu): CTA pairs, d_pad <= 768, even q_tiles
-bool gemm_topk_ts_supported(int d_pad, int q_tiles);
-int gemm_topk_ts_tile_rows(int d_pad);
-cudaError_t launch_gemm_topk_ts(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail);
-
-// ---- fp32 rows on the tensor cores with fp32-level accuracy (ip_gemm_tf32x3_sm100.cu): CTA pairs, even q_tiles
+// fp32 rows on the tensor cores with fp32-level accuracy (3xTF32, queries pre-split into hi / lo planes)
 cudaError_t launch_split_tf32(const float *src, int64_t n_src, int d_pad, float *hi, float *lo, int64_t n_pad, cudaStream_t s);
 cudaError_t launch_gemm3_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail);
 

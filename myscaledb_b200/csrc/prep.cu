@@ -1,6 +1,6 @@
 // prep.cu -- small elementwise kernels that put host-format columns into the HBM layout
 // the scan / GEMM kernels want: zero-padded rows (16-byte multiples; 64-element multiples
-// for the tcgen05 path), optional bf16 conversion, per-row norms.
+// for the tensor-core path), optional bf16 conversion, per-row norms.
 //
 // Reference counterparts: VectorDataset<T>::normalize (VectorIndex/Common/VectorDataset.h:99-117)
 // and the ColumnArray -> contiguous float[n*d] copy in
@@ -71,7 +71,7 @@ __global__ void normalize_rows_f32_kernel(float *rows, int d_pad, int64_t n) {
 
 static int grid_for(int64_t work, int threads) {
     int64_t b = ceil_div(work, threads);
-    if (b > 148 * 16) b = 148 * 16;
+    if (b > 132 * 16) b = 132 * 16;
     if (b < 1) b = 1;
     return (int)b;
 }

@@ -67,7 +67,7 @@ extern "C" int b200_bitmap_from_offsets_device(const uint64_t *d_offsets, int64_
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     B200_CUDA_OK(cudaMemsetAsync(d_out_bits, 0, (size_t)round_up(ceil_div(nbits, 8), 4), s));
     if (n) {
-        bitmap_from_offsets_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), 148 * 16)), 256, 0, s>>>(
+        bitmap_from_offsets_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), 132 * 16)), 256, 0, s>>>(
             d_offsets, n, nbits, reinterpret_cast<uint32_t *>(d_out_bits));
         g_launches++;
         B200_CUDA_OK(cudaGetLastError());
@@ -78,7 +78,7 @@ extern "C" int b200_bitmap_from_row_exists_device(const uint8_t *d_row_exists, i
     if ((!d_row_exists && n > 0) || !d_out_bits || n < 0) return fail(B200_ERR_INVALID, "bad arguments");
     if (n == 0) return B200_OK;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    bitmap_from_bytes_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(ceil_div(n, 8), 256), 148 * 16)), 256, 0, s>>>(d_row_exists, n, d_out_bits);
+    bitmap_from_bytes_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(ceil_div(n, 8), 256), 132 * 16)), 256, 0, s>>>(d_row_exists, n, d_out_bits);
     g_launches++;
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;
@@ -88,7 +88,7 @@ extern "C" int b200_bitmap_and_device(const uint8_t *d_a, const uint8_t *d_b, in
     if (!d_a || !d_b || !d_out || nbits < 0) return fail(B200_ERR_INVALID, "bad arguments");
     if (nbits == 0) return B200_OK;
     const int64_t nwords = ceil_div(nbits, 32);
-    bitmap_and_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(nwords, 256), 148 * 16)), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+    bitmap_and_kernel<<<(int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(nwords, 256), 132 * 16)), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<const uint32_t *>(d_a), reinterpret_cast<const uint32_t *>(d_b), nwords, reinterpret_cast<uint32_t *>(d_out));
     g_launches++;
     B200_CUDA_OK(cudaGetLastError());
@@ -108,7 +108,7 @@ int device_ok() {
     }
     return B200_OK;
 }
-int blocks_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), 148 * 16)); }
+int blocks_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), 132 * 16)); }
 }  // namespace
 
 // intersectDenseBitmaps: out = a & b over nbits bits (LSB-first bytes)

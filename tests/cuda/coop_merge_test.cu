@@ -1,6 +1,6 @@
 // Unit test of the cooperative tile merge (csrc/ivf_coop.cuh) outside the tensor-core kernel: one warp, synthetic tiles.
 // For every slot the final sorted list must equal the k smallest (key, id) of everything the slot was shown.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O2 -std=c++17 -I myscaledb_b200/csrc tests/cuda/coop_merge_test.cu -o tests/cuda/coop_merge_test
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O2 -std=c++17 -I myscaledb_b200/csrc tests/cuda/coop_merge_test.cu -o tests/cuda/coop_merge_test
 #include <algorithm>
 #include <cstdio>
 #include <random>

@@ -3,7 +3,7 @@
 // chunks of synthetic keys (heavy ties included); the published list of every thread must equal the k smallest (key, id) of
 // what it was shown -- in the default form for the k (one-lane rescan up to 16, warp-cooperative above), the append form and the
 // one-lane form at every k.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O2 -std=c++17 -DB200_LIST_COOP_MIN_K=17 -I myscaledb_b200/csrc tests/cuda/list_append_test.cu -o tests/cuda/list_append_test
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O2 -std=c++17 -DB200_LIST_COOP_MIN_K=17 -I myscaledb_b200/csrc tests/cuda/list_append_test.cu -o tests/cuda/list_append_test
 #include <algorithm>
 #include <cstdio>
 #include <random>

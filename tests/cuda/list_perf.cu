@@ -1,7 +1,7 @@
 // Micro-benchmark of the per-thread top-k list (gemm_common.cuh) on a synthetic stream shaped like one epilogue warp-group of the
 // flat tensor-core kernel: 128 lists, `chunks` 32-wide chunks of pseudo-random keys each.  Prints time and event counters for
-// rescan / append lists in shared or global memory.  Not part of the test suite (tools/r02/gpu20.sh).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O2 -std=c++17 -DB200_LIST_STATS -I myscaledb_b200/csrc tests/cuda/list_perf.cu -o tests/cuda/list_perf
+// rescan / append lists in shared or global memory.  Not part of the test suite; build with the line below and run it by hand.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O2 -std=c++17 -DB200_LIST_STATS -I myscaledb_b200/csrc tests/cuda/list_perf.cu -o tests/cuda/list_perf
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -49,7 +49,7 @@ __global__ void __launch_bounds__(128) perf_kernel(int chunks, int k, int cap, i
 
 int main(int argc, char **argv) {
     const int chunks = argc > 1 ? atoi(argv[1]) : 17000;   // 10 M rows / 18 clusters / 32
-    const int grid = 148;
+    const int grid = 132;
     const int big_smem = argc > 2 ? atoi(argv[2]) : 1;
     for (int k : {10, 30, 64, 100}) {
         for (int mode = -1; mode < 4; mode++) {          // 3: tournament (group worsts)          // -1 one-lane rescan, 0 default (cooperative from k = 17), 1 append (2k / k+32), 2 append with 4k slots

@@ -19,7 +19,7 @@ def test_library_exports_every_declared_symbol():
     assert len(syms) >= 15
     for s in syms:
         assert hasattr(L, s), f"{s} declared in include/b200_search.h but not exported"
-    assert b"sm_100a" in L.b200_version()
+    assert b"sm_90a" in L.b200_version()
 
 
 def test_product_never_references_oracle():
@@ -35,12 +35,12 @@ def test_product_never_references_oracle():
     assert not bad, bad
 
 
-def test_sass_is_blackwell_native():
+def test_sass_is_hopper_native():
     so = os.path.join(ROOT, "myscaledb_b200", "libb200search.so")
     out = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
-    assert "sm_100a" in out or "SM100a" in out.upper() or "EF_CUDA_SM100" in out
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM"):
-        assert mnemonic in out, f"{mnemonic} missing from SASS: the tcgen05/TMA path did not compile"
+    assert "sm_90a" in out or "SM90a" in out.upper() or "EF_CUDA_SM90" in out
+    for mnemonic in ("HGMMA", "UTMALDG", "SYNCS"):
+        assert mnemonic in out, f"{mnemonic} missing from SASS: the wgmma/TMA/mbarrier path did not compile"
 
 
 @pytest.mark.skipif(os.path.exists("/dev/nvidia0"), reason="only meaningful without a GPU")

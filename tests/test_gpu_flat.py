@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Every call goes through the C ABI
+"""GPU parity tests (run on an H100: pytest -m gpu).  Every call goes through the C ABI
 of libb200search.so (ctypes) and is checked against the CPU oracle / the reference goldens."""
 import numpy as np
 import pytest
@@ -207,7 +207,7 @@ def test_scan_bf16_corpus():
         c.close()
 
 
-# ------------------------------------------------------------------ tcgen05 GEMM path vs oracle
+# ------------------------------------------------------------------ tensor-core GEMM path vs oracle
 @pytest.mark.parametrize("metric", [b2.IP, b2.L2, b2.COSINE])
 @pytest.mark.parametrize("n,d,nq,k,path", [(20000, 768, 128, 10, 2), (5000, 64, 37, 30, 2), (70001, 128, 300, 10, 2),
                                            (70001, 128, 300, 10, 3), (70001, 128, 300, 10, 4), (70001, 128, 300, 10, 7), (1000, 96, 20, 50, 2),
@@ -216,9 +216,8 @@ def test_scan_bf16_corpus():
                                            (33333, 768, 512, 30, 7), (257, 64, 129, 5, 2), (9000, 512, 256, 10, 2), (9000, 512, 256, 10, 7),
                                            (9000, 832, 256, 10, 2)])
 def test_gemm_path_matches_oracle(metric, n, d, nq, k, path):
-    """b200_corpus_set_path codes: 2 = the tensor-core variant auto picks (streaming + TMA multicast), 3 = single-CTA MMAs
-    <1,1>, 4 = CTA pairs without multicast <2,1>, 5 = <2,2>, 6 = <2,4>, 7 = queries stationary in TMEM (TS form).
-    The same variants at >= 2 M rows: tests/test_gpu_gemm_scale.py."""
+    """b200_corpus_set_path codes 2..7 all select the tensor-core kernel (3..7 named instantiations of an earlier target
+    and must keep working).  The same at >= 2 M rows: tests/test_gpu_gemm_scale.py."""
     rng = np.random.default_rng(n + d + nq + metric)
     y = to_bf16_values(rng.standard_normal((n, d)).astype(F32))
     x = to_bf16_values(rng.standard_normal((nq, d)).astype(F32))
@@ -244,7 +243,7 @@ def _prep_cos(x, y):
 @pytest.mark.parametrize("n,d,nq,k", [(20000, 768, 128, 10), (5000, 64, 37, 30), (70001, 128, 300, 10), (1000, 96, 20, 50),
                                       (33333, 768, 1024, 10), (257, 50, 129, 5), (9000, 100, 256, 100), (4000, 1536, 16, 10)])
 def test_tf32x3_path_matches_oracle(metric, n, d, nq, k):
-    """fp32 corpus, batch of queries: three TF32 tensor-core products per k-step (ip_gemm_tf32x3_sm100.cu) must give
+    """fp32 corpus, batch of queries: three TF32 tensor-core products per k-step (ip_gemm_sm90.cu) must give
     fp32-class results on arbitrary fp32 inputs (NOT pre-rounded), i.e. the same tolerance as the fp32 FMA scan."""
     rng = np.random.default_rng(7 * n + d + nq + metric)
     y = rng.standard_normal((n, d)).astype(F32)
@@ -300,7 +299,7 @@ def test_gemm_path_alive_bitmap():
 
 def test_gemm_equals_scan_large_property():
     """Size-independent property at a size the oracle cannot reach quickly: the two
-    independent GPU paths (fp32 FMA scan vs tcgen05 GEMM) must return the same ids."""
+    independent GPU paths (fp32 FMA scan vs tensor-core GEMM) must return the same ids."""
     rng = np.random.default_rng(33)
     y = to_bf16_values(rng.standard_normal((400000, 768)).astype(F32))
     x = to_bf16_values(rng.standard_normal((256, 768)).astype(F32))

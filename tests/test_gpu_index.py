@@ -164,6 +164,18 @@ def test_ivfpq_ip_adc_recall():
     assert np.abs(dg - true).max() < 0.15 * np.abs(true).max()
 
 
+def test_ivfpq_codebook_of_192_dims_fits_beside_the_ring():
+    """A 192-d PQ codebook (96 KB of bf16) shares shared memory with the operand ring, the accumulator staging and the lists
+    of the decoding scan; such indexes must build and search."""
+    y, q = _clustered(20000, 192, 100, 8)
+    ix = b2.VectorIndex("IVFPQ", b2.IP, 192, "ncentroids=32, M=96").build(y)
+    do, io = orc.search_without_index(orc.IP, q, y, 10)
+    dg, ig = ix.search(q, 10, "nprobe=32")
+    assert _recall(ig, io) >= 0.6
+    true = np.array([[float(q[a] @ y[ig[a, j]]) for j in range(10)] for a in range(len(q))])
+    assert np.abs(dg - true).max() < 0.15 * np.abs(true).max()
+
+
 def test_compute_top_distance_subset_matches_oracle():
     rng = np.random.default_rng(4)
     y = rng.standard_normal((5000, 100)).astype(F32)
@@ -200,7 +212,7 @@ def test_golden_00028_mstg_small_part_falls_back_to_exact(goldens):
 
 
 def test_index_above_one_grid_of_rows_regression():
-    """n larger than one capped launch grid (148*32*256 = 1.2M threads): the per-row build kernels must
+    """n larger than one capped launch grid (132*32*256 = 1.1M threads): the per-row build kernels must
     cover every row (caught by tools/bench_aux.py: recall collapsed at 5M rows)."""
     rng = np.random.default_rng(12)
     n, d = 1_500_000, 16

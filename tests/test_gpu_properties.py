@@ -1,7 +1,7 @@
 """Randomised GPU-vs-oracle properties (hypothesis) on small integer-valued inputs, where fp32 / bf16 / tf32 sums are
 exact and ties are everywhere, so every path of the library must return EXACTLY the oracle's ids and distances.
 
-Part of the `gpu` suite since round 2."""
+Part of the `gpu` suite."""
 
 import numpy as np
 import pytest

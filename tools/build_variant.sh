@@ -1,6 +1,6 @@
 #!/bin/bash
 # A/B build of libb200search.so with extra compile-time defines, next to the default build:
-#   tools/build_variant.sh backoff64 "-DB200_MBAR_BACKOFF_NS=64"   ->  build_variants/libb200search_backoff64.so
+#   tools/build_variant.sh coop17 "-DB200_LIST_COOP_MIN_K=17"   ->  build_variants/libb200search_coop17.so
 # Use with B200_LIB_PATH=build_variants/libb200search_<name>.so python bench.py --headline-only
 set -e
 name=$1; extra=$2

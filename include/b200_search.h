@@ -69,7 +69,11 @@ int b200_flat_knn(int metric, const float *x, int64_t nx, const float *y, int64_
 
 /* Binary vectors: HAMMING (faiss::hammings_knn_mc) / JACCARD (jaccard_knn),
  * BruteForceSearch.h:94-110.  Distances are returned as float VALUES (the reference
- * writes int32 Hamming distances into the float buffer, :99; the shim re-encodes). */
+ * writes int32 Hamming distances into the float buffer, :99; the shim re-encodes).
+ * Binary corpora (these calls, binary b200_part_scan and B200_DTYPE_BIN corpora) have two kernels that return the same
+ * bytes: a popcount scan, and for rows of a multiple of 16 bytes (d % 128 == 0 bits) a tensor-core kernel (wgmma .b1 AND +
+ * popcount) that auto-selection uses from a few queries per batch up (see b200_corpus_set_path).  Both return the same
+ * ids and distances. */
 int b200_binary_knn(int metric, const uint8_t *x, int64_t nx, const uint8_t *y, int64_t ny, int nbytes, int k,
                     const uint8_t *alive_bits /*nullable*/, float *out_dis, int64_t *out_ids);
 
@@ -115,15 +119,19 @@ int b200_corpus_search_device(b200_corpus *c, const float *d_queries, int64_t nq
                               int64_t *d_out_ids, void *stream);
 /* Force a search path (tests, A/B measurements; production leaves 0):
  *   0 auto | 1 memory-bound scan kernel | 2 tensor cores (bf16 corpora: the bf16 wgmma kernel; fp32 corpora: the
- *   3xTF32 kernel) | 3 .. 7 the same as 2 (they named tensor-core variants of an earlier target and stay accepted). */
+ *   3xTF32 kernel; binary corpora: the b1 kernel, B200_ERR_UNSUPPORTED unless the rows are a multiple of 16 bytes) |
+ *   3 .. 7 the same as 2 (they named tensor-core variants of an earlier target and stay accepted).
+ * Auto on a binary corpus: the b1 kernel when the rows are a multiple of 16 bytes (d < 2^24 bits) and the batch has at
+ * least ceil(20480 / row_bytes^2) queries (2 at 1024 bits, 20 at 256 bits), else the scan. */
 int b200_corpus_set_path(b200_corpus *c, int path);
 /* which kernel the last search on this corpus launched (so a test can prove it exercised the variant it meant to) */
-#define B200_KERNEL_SCAN 1
-#define B200_KERNEL_GEMM_BF16 2   /* gemm_topk_kernel<false> (cta_group and pairs_per_cluster report 1) */
+#define B200_KERNEL_SCAN 1 /* flat_scan_kernel, or binary_scan_kernel on binary corpora */
+#define B200_KERNEL_GEMM_BF16 2   /* gemm_topk_kernel<BF16> (cta_group and pairs_per_cluster report 1) */
 #define B200_KERNEL_GEMM_TS 3     /* no longer launched; the value stays reserved */
-#define B200_KERNEL_GEMM_TF32X3 4 /* gemm_topk_kernel<true> */
+#define B200_KERNEL_GEMM_TF32X3 4 /* gemm_topk_kernel<TF32X3> */
+#define B200_KERNEL_GEMM_B1 5     /* gemm_topk_kernel<B1>: binary rows, wgmma .b1 AND + popcount */
 int b200_corpus_last_variant(b200_corpus *c, int *kernel, int *cta_group, int *pairs_per_cluster, int *grid);
-/* CUDA-event timing of the dominant kernel (scan or GEMM) of every search on this corpus,
+/* CUDA-event timing of the dominant kernel (scan or GEMM, float or binary) of every search on this corpus,
  * recorded on the launching stream; used by bench.py for the roofline report. */
 int b200_corpus_enable_timing(b200_corpus *c, int on);
 int b200_corpus_kernel_time(b200_corpus *c, int reset, double *out_total_ms, int64_t *out_launches);
@@ -297,7 +305,8 @@ int b200_cache_expire_prefix(const char *prefix, int64_t *out_removed);
 /* VICacheManager::countItem and the CurrentMetrics counters */
 int b200_cache_stats(uint64_t *capacity, uint64_t *used, uint64_t *items, uint64_t *hits, uint64_t *misses,
                      uint64_t *evictions);
-/* getResourceUsage().memory_usage_bytes of a resident object (rows + side arrays / lists + codes), for `bytes` above */
+/* getResourceUsage().memory_usage_bytes of a resident object (rows + side arrays / lists + codes), for `bytes` above.
+ * A binary corpus counts 4 bytes per row for its per-row popcounts (used by the tensor-core path). */
 int b200_corpus_memory_bytes(const b200_corpus *c, uint64_t *out_bytes);
 int b200_index_memory_bytes(const b200_index *ix, uint64_t *out_bytes);
 

@@ -91,7 +91,7 @@ struct b200_corpus {
     int64_t side_cap_rows = 0;   // rows the row_scale / row_bias arrays can hold
     bool owns = true;
     float *row_scale = nullptr;  // cosine: -1/||y||
-    float *row_bias = nullptr;   // L2: ||y||^2 (GEMM path)
+    float *row_bias = nullptr;   // L2: ||y||^2 (GEMM path); binary: popcount of the row (tensor-core path)
     int device = 0;
     int path = 0;
     int sms = 132;
@@ -256,7 +256,7 @@ static int corpus_alloc(b200_corpus *c, int64_t rows) {
     if (c->data && !c->owns) return fail(B200_ERR_INVALID, "corpus adopted device memory; cannot append");
     // +1 row of slack so that 16-byte vector loads of the last row never leave the allocation
     const size_t need = (size_t)(rows + 1) * c->row_bytes + 256;
-    const bool want_scale = c->metric == B200_METRIC_COSINE, want_bias = c->metric == B200_METRIC_L2;
+    const bool want_scale = c->metric == B200_METRIC_COSINE, want_bias = c->metric == B200_METRIC_L2 || is_bin_metric(c->metric);
     if (!c->data || c->data_cap_bytes < need) {
         void *nd = nullptr;
         cudaError_t e = cudaMalloc(&nd, need);
@@ -294,6 +294,8 @@ static int corpus_alloc(b200_corpus *c, int64_t rows) {
 
 static int corpus_norms(b200_corpus *c, int64_t first, int64_t n) {
     const char *rows = reinterpret_cast<const char *>(c->data) + first * c->row_bytes;
+    if (c->dtype == B200_DTYPE_BIN)
+        B200_CUDA_OK(launch_popc_rows(reinterpret_cast<const uint8_t *>(rows), c->row_bytes, n, c->row_bias + first, c->stream));
     if (c->metric == B200_METRIC_COSINE)
         B200_CUDA_OK(launch_row_norms(rows, c->dtype == B200_DTYPE_BF16, c->d_pad, n, 1, c->row_scale + first, c->stream));
     if (c->metric == B200_METRIC_L2)
@@ -327,7 +329,7 @@ extern "C" int b200_corpus_append(b200_corpus *c, const void *rows, int64_t n) {
             B200_CUDA_OK(cudaStreamSynchronize(c->stream));  // w_raw is reused
         }
     }
-    if (c->dtype != B200_DTYPE_BIN) B200_TRY(corpus_norms(c, c->n, n));
+    B200_TRY(corpus_norms(c, c->n, n));
     B200_CUDA_OK(cudaStreamSynchronize(c->stream));
     c->n += n;
     return B200_OK;
@@ -355,9 +357,9 @@ extern "C" int b200_corpus_adopt_device(b200_corpus *c, const void *device_rows,
     c->n = n;
     c->cap = n;
     if (c->metric == B200_METRIC_COSINE) B200_CUDA_OK(cudaMalloc(&c->row_scale, (size_t)n * 4 + 256));
-    if (c->metric == B200_METRIC_L2) B200_CUDA_OK(cudaMalloc(&c->row_bias, (size_t)n * 4 + 256));
+    if (c->metric == B200_METRIC_L2 || c->dtype == B200_DTYPE_BIN) B200_CUDA_OK(cudaMalloc(&c->row_bias, (size_t)n * 4 + 256));
     c->side_cap_rows = n;
-    if (c->dtype != B200_DTYPE_BIN) B200_TRY(corpus_norms(c, 0, n));
+    B200_TRY(corpus_norms(c, 0, n));
     B200_CUDA_OK(cudaStreamSynchronize(c->stream));
     return B200_OK;
 }
@@ -385,8 +387,9 @@ int list_cap_for(int k) {
 extern "C" int b200_corpus_set_path(b200_corpus *c, int path) {
     if (!c || path < 0 || path > 7) return fail(B200_ERR_INVALID, "path must be 0..7");
     std::lock_guard<std::mutex> lk(c->mu);
-    // 0 auto | 1 scan | 2 tensor cores.  3..7 named the tensor-core instantiations of an earlier target (CTA pairs,
-    // multicast clusters, queries in tensor memory); sm_90 has one tensor-core kernel per operand type, so they select it.
+    // 0 auto | 1 scan | 2 tensor cores (binary corpora too: the b1 kernel).  3..7 named the tensor-core instantiations of an
+    // earlier target (CTA pairs, multicast clusters, queries in tensor memory); sm_90 has one tensor-core kernel per operand
+    // type, so they select it.
     c->path = path >= 2 ? 2 : path;
     return B200_OK;
 }
@@ -444,6 +447,75 @@ extern "C" int b200_corpus_free(b200_corpus *c) {
     return B200_OK;
 }
 
+// Auto path of a binary corpus: the tensor cores (gemm_topk_kernel<B1>) from ceil(kBinaryTensorMinQB2 / row_bytes^2) queries
+// per batch, the scan below.  Up to 16 queries the tensor kernel costs about one 128-query tile pass (1.5 - 1.9 ms per 10 M
+// rows at 256 and at 1024 bits); the scan costs one pass per query, and that pass grew 9.6x from 32- to 128-byte rows.
+// Measured with tools/bench_aux.py binary on an H100 80GB HBM3 at a 400 W power limit (10 M rows, k = 10; DESIGN.md
+// section 7): the curves cross between 1 and 2 queries at 1024 bits and between 8 and 16 at 256 bits.  20480 / row_bytes^2
+// gives 2 and 20 queries (at 256 bits and 16 queries the scan is 10 % slower than the tensor path); other widths are
+// extrapolated, not measured.
+constexpr int64_t kBinaryTensorMinQB2 = 20480;
+
+// One launch of gemm_topk_kernel over a chunk of <= 1024 staged queries (gp: operands, side arrays, d_pad and alive set),
+// then the merge of the CTAs' partial lists into rows of k of d_out_dis / d_out_ids.  kernel: B200_KERNEL_GEMM_*.
+static int gemm_chunk(b200_corpus *c, GemmTopkParams &gp, int64_t nq_c, int k, int kernel, int out_mode, const float *q_add,
+                      int ip_min_quirk, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
+    const int nq_pad = (int)round_up(nq_c, 128);
+    const int q_tiles = nq_pad / 128;
+    int grid = gemm_topk_grid(q_tiles, c->n, c->sms);
+    grid = (grid / q_tiles) * q_tiles;
+    if (grid < q_tiles) grid = q_tiles;
+    B200_TRY(c->w_pk.reserve((size_t)grid * 128 * k * 4));
+    B200_TRY(c->w_pi.reserve((size_t)grid * 128 * k * 4));
+    gp.part_keys = c->w_pk.as<float>();
+    gp.part_ids = c->w_pi.as<uint32_t>();
+    {  // global scratch for the per-thread lists, used when they do not fit in shared memory (large k)
+        B200_TRY(c->w_lk.reserve((size_t)grid * 128 * list_cap_for(k) * 4));
+        B200_TRY(c->w_li.reserve((size_t)grid * 128 * list_cap_for(k) * 4));
+        gp.list_keys_gmem = c->w_lk.as<float>();
+        gp.list_ids_gmem = c->w_li.as<uint32_t>();
+    }
+    gp.n = c->n;
+    gp.nq_pad = nq_pad;
+    gp.nq_valid = (int)nq_c;
+    gp.k = k;
+    gp.q_tiles = q_tiles;
+    if (q_tiles > 1 && c->sync_slack > 0) {
+        B200_TRY(c->w_prog.reserve((size_t)grid * 4));
+        B200_CUDA_OK(cudaMemsetAsync(c->w_prog.p, 0, (size_t)grid * 4, s));
+        gp.progress = c->w_prog.as<int>();
+        gp.sync_slack = c->sync_slack;
+    }
+    const char *detail = nullptr;
+    std::pair<cudaEvent_t, cudaEvent_t> ev;
+    timing_begin(c, s, ev);
+    cudaError_t e = kernel == B200_KERNEL_GEMM_TF32X3 ? launch_gemm3_topk(gp, grid, s, &detail)
+                    : kernel == B200_KERNEL_GEMM_B1  ? launch_gemm_b1_topk(gp, grid, s, &detail)
+                                                     : launch_gemm_topk(gp, grid, s, &detail);
+    timing_end(c, s, ev);
+    c->last_kernel = kernel;
+    c->last_cg = 1; c->last_mc = 1; c->last_grid = grid;
+    if (e != cudaSuccess)
+        return fail(B200_ERR_CUDA, std::string("gemm_topk launch: ") + (detail ? detail : cudaGetErrorString(e)));
+    MergeParams mp{};
+    mp.in_keys = gp.part_keys;
+    mp.in_ids = gp.part_ids;
+    mp.list_stride = (int64_t)nq_pad * k;
+    mp.q_stride = k;
+    mp.n_lists = grid / q_tiles;
+    mp.k_in = k;
+    mp.k = k;
+    mp.nq = nq_c;
+    mp.out_mode = out_mode;
+    mp.q_add = q_add;
+    mp.ip_min_quirk = ip_min_quirk;
+    mp.id_offset = id_offset;
+    mp.out_dis = d_out_dis;
+    mp.out_ids = d_out_ids;
+    B200_CUDA_OK(launch_topk_merge(mp, false, s));
+    return B200_OK;
+}
+
 // ------------------------------------------------------------------------------------
 // search core: everything on device, asynchronous on `s`
 // d_queries: raw device fp32 [nq][d] (or bytes [nq][d/8] for binary corpora)
@@ -457,35 +529,77 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
 
     if (c->dtype == B200_DTYPE_BIN) {
         if (k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 not supported on the binary scan path");
-        int blocks_x = (int)std::min<int64_t>(std::max<int64_t>(1, ceil_div(c->n, 256)), std::max<int64_t>(1, (2 * sms) / std::max<int64_t>(1, std::min<int64_t>(nq, 2 * sms))));
-        B200_TRY(c->w_pk.reserve((size_t)nq * blocks_x * k * 4));
-        B200_TRY(c->w_pi.reserve((size_t)nq * blocks_x * k * 4));
-        BinaryScanParams bp{};
-        bp.corpus = reinterpret_cast<const uint8_t *>(c->data);
-        bp.queries = reinterpret_cast<const uint8_t *>(d_queries);
-        bp.alive = d_alive;
-        bp.part_keys = c->w_pk.as<float>();
-        bp.part_ids = c->w_pi.as<uint32_t>();
-        bp.n = c->n;
-        bp.nq = nq;
-        bp.nbytes = c->d_pad;
-        bp.k = k;
-        bp.jaccard = c->metric == B200_METRIC_JACCARD;
-        B200_CUDA_OK(launch_binary_scan(bp, blocks_x, s));
-        MergeParams mp{};
-        mp.in_keys = bp.part_keys;
-        mp.in_ids = bp.part_ids;
-        mp.list_stride = k;
-        mp.q_stride = (int64_t)blocks_x * k;
-        mp.n_lists = blocks_x;
-        mp.k_in = k;
-        mp.k = k;
-        mp.nq = nq;
-        mp.out_mode = kOutKey;
-        mp.id_offset = id_offset;
-        mp.out_dis = d_out_dis;
-        mp.out_ids = d_out_ids;
-        B200_CUDA_OK(launch_topk_merge(mp, false, s));
+        // The tensor-core path loads rows with TMA (16-byte row stride) and keeps AND counts and keys exact in fp32 (< 2^24 bits).
+        const bool tc_rows = c->row_bytes % 16 == 0, tc_exact = c->d < (1 << 24);
+        int path = c->path;
+        if (path == 0) path = (tc_rows && tc_exact && nq >= ceil_div(kBinaryTensorMinQB2, c->row_bytes * c->row_bytes)) ? 2 : 1;
+        if (path == 2 && !tc_rows)
+            return fail(B200_ERR_UNSUPPORTED, "binary tensor-core path needs rows of a multiple of 16 bytes (d % 128 == 0 bits); "
+                                              "this corpus has " + std::to_string(c->row_bytes) + "-byte rows");
+        if (path == 2 && !tc_exact) return fail(B200_ERR_UNSUPPORTED, "binary tensor-core path needs d < 2^24 bits");
+        if (c->n == 0) path = 1;
+        const bool jaccard = c->metric == B200_METRIC_JACCARD;
+        if (path == 1) {
+            int blocks_x = (int)std::min<int64_t>(std::max<int64_t>(1, ceil_div(c->n, 256)), std::max<int64_t>(1, (2 * sms) / std::max<int64_t>(1, std::min<int64_t>(nq, 2 * sms))));
+            B200_TRY(c->w_pk.reserve((size_t)nq * blocks_x * k * 4));
+            B200_TRY(c->w_pi.reserve((size_t)nq * blocks_x * k * 4));
+            BinaryScanParams bp{};
+            bp.corpus = reinterpret_cast<const uint8_t *>(c->data);
+            bp.queries = reinterpret_cast<const uint8_t *>(d_queries);
+            bp.alive = d_alive;
+            bp.part_keys = c->w_pk.as<float>();
+            bp.part_ids = c->w_pi.as<uint32_t>();
+            bp.n = c->n;
+            bp.nq = nq;
+            bp.nbytes = c->d_pad;
+            bp.k = k;
+            bp.jaccard = jaccard;
+            std::pair<cudaEvent_t, cudaEvent_t> ev;
+            timing_begin(c, s, ev);
+            B200_CUDA_OK(launch_binary_scan(bp, blocks_x, s));
+            timing_end(c, s, ev);
+            c->last_kernel = B200_KERNEL_SCAN; c->last_cg = 0; c->last_mc = 0; c->last_grid = blocks_x;
+            MergeParams mp{};
+            mp.in_keys = bp.part_keys;
+            mp.in_ids = bp.part_ids;
+            mp.list_stride = k;
+            mp.q_stride = (int64_t)blocks_x * k;
+            mp.n_lists = blocks_x;
+            mp.k_in = k;
+            mp.k = k;
+            mp.nq = nq;
+            mp.out_mode = kOutKey;
+            mp.id_offset = id_offset;
+            mp.out_dis = d_out_dis;
+            mp.out_ids = d_out_ids;
+            B200_CUDA_OK(launch_topk_merge(mp, false, s));
+            return B200_OK;
+        }
+        // ---- path 2: wgmma .b1 AND + popcount with fused top-k, <= 1024 queries per launch.  Hamming ranks popc(y) - 2 and
+        // (popc(q) is added at the merge), Jaccard is keyed in the kernel; both exactly as binary_scan_kernel keys them.
+        const int64_t QCHUNK = 1024;
+        for (int64_t qb = 0; qb < nq; qb += QCHUNK) {
+            const int64_t nq_c = std::min(QCHUNK, nq - qb);
+            const int64_t nq_pad = round_up(nq_c, 128);
+            // queries zero-padded to whole 128-query tiles, 16-byte aligned for TMA
+            B200_TRY(c->w_qbf.reserve((size_t)nq_pad * c->row_bytes));
+            B200_CUDA_OK(cudaMemsetAsync(c->w_qbf.p, 0, (size_t)nq_pad * c->row_bytes, s));
+            B200_CUDA_OK(cudaMemcpyAsync(c->w_qbf.p, reinterpret_cast<const uint8_t *>(d_queries) + qb * c->row_bytes,
+                                         (size_t)nq_c * c->row_bytes, cudaMemcpyDeviceToDevice, s));
+            B200_TRY(c->w_qnorm.reserve((size_t)nq_pad * 4));
+            B200_CUDA_OK(launch_popc_rows(c->w_qbf.as<uint8_t>(), c->row_bytes, nq_c, c->w_qnorm.as<float>(), s));
+            GemmTopkParams gp{};
+            gp.corpus_bf16 = c->data;
+            gp.queries_bf16 = c->w_qbf.p;
+            gp.row_bias = c->row_bias;
+            gp.scale_const = jaccard ? 1.f : -2.f;
+            gp.alive = d_alive;
+            gp.q_popc = jaccard ? c->w_qnorm.as<float>() : nullptr;
+            gp.jaccard = jaccard;
+            gp.d_pad = (int)c->row_bytes;
+            B200_TRY(gemm_chunk(c, gp, nq_c, k, B200_KERNEL_GEMM_B1, jaccard ? kOutKey : kOutAddQ, jaccard ? nullptr : c->w_qnorm.as<float>(),
+                                0, id_offset, d_out_dis + qb * k, d_out_ids + qb * k, s));
+        }
         return B200_OK;
     }
 
@@ -575,7 +689,6 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
         const int64_t nq_c = std::min(QCHUNK, nq - qb);
         const bool f32 = c->dtype == B200_DTYPE_F32;
         const int nq_pad = (int)round_up(nq_c, 128);
-        const int q_tiles = nq_pad / 128;
         if (f32) {
             // fp32 rows: queries split once per batch into TF32 hi / lo planes (ip_gemm_sm90.cu)
             B200_TRY(c->w_qbf.reserve((size_t)nq_pad * c->d_pad * 4));
@@ -598,11 +711,6 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
                                               c->w_qnorm.as<float>(), s));
             q_add = c->w_qnorm.as<float>();
         }
-        int grid = gemm_topk_grid(q_tiles, c->n, sms);
-        grid = (grid / q_tiles) * q_tiles;
-        if (grid < q_tiles) grid = q_tiles;
-        B200_TRY(c->w_pk.reserve((size_t)grid * 128 * k * 4));
-        B200_TRY(c->w_pi.reserve((size_t)grid * 128 * k * 4));
         GemmTopkParams gp{};
         gp.corpus_bf16 = c->data;
         gp.queries_bf16 = c->w_qbf.p;
@@ -611,51 +719,10 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
         gp.scale_const = c->metric == B200_METRIC_L2 ? -2.f : -1.f;
         gp.row_bias = c->metric == B200_METRIC_L2 ? c->row_bias : nullptr;
         gp.alive = d_alive;
-        gp.part_keys = c->w_pk.as<float>();
-        gp.part_ids = c->w_pi.as<uint32_t>();
-        {  // global scratch for the per-thread lists, used when they do not fit in shared memory (large k)
-            B200_TRY(c->w_lk.reserve((size_t)grid * 128 * list_cap_for(k) * 4));
-            B200_TRY(c->w_li.reserve((size_t)grid * 128 * list_cap_for(k) * 4));
-            gp.list_keys_gmem = c->w_lk.as<float>();
-            gp.list_ids_gmem = c->w_li.as<uint32_t>();
-        }
-        gp.n = c->n;
-        gp.nq_pad = nq_pad;
-        gp.nq_valid = (int)nq_c;
         gp.d_pad = c->d_pad;
-        gp.k = k;
-        gp.q_tiles = q_tiles;
-        if (q_tiles > 1 && c->sync_slack > 0) {
-            B200_TRY(c->w_prog.reserve((size_t)grid * 4));
-            B200_CUDA_OK(cudaMemsetAsync(c->w_prog.p, 0, (size_t)grid * 4, s));
-            gp.progress = c->w_prog.as<int>();
-            gp.sync_slack = c->sync_slack;
-        }
-        const char *detail = nullptr;
-        std::pair<cudaEvent_t, cudaEvent_t> ev;
-        timing_begin(c, s, ev);
-        cudaError_t e = f32 ? launch_gemm3_topk(gp, grid, s, &detail) : launch_gemm_topk(gp, grid, s, &detail);
-        timing_end(c, s, ev);
-        c->last_kernel = f32 ? B200_KERNEL_GEMM_TF32X3 : B200_KERNEL_GEMM_BF16;
-        c->last_cg = 1; c->last_mc = 1; c->last_grid = grid;
-        if (e != cudaSuccess)
-            return fail(B200_ERR_CUDA, std::string("gemm_topk launch: ") + (detail ? detail : cudaGetErrorString(e)));
-        MergeParams mp{};
-        mp.in_keys = gp.part_keys;
-        mp.in_ids = gp.part_ids;
-        mp.list_stride = (int64_t)nq_pad * k;
-        mp.q_stride = k;
-        mp.n_lists = grid / q_tiles;
-        mp.k_in = k;
-        mp.k = k;
-        mp.nq = nq_c;
-        mp.out_mode = c->metric == B200_METRIC_L2 ? kOutAddQ : c->metric == B200_METRIC_IP ? kOutNeg : kOutCosQ;
-        mp.q_add = q_add;
-        mp.ip_min_quirk = ip_min_quirk && c->metric == B200_METRIC_IP;
-        mp.id_offset = id_offset;
-        mp.out_dis = d_out_dis + qb * k;
-        mp.out_ids = d_out_ids + qb * k;
-        B200_CUDA_OK(launch_topk_merge(mp, false, s));
+        const int out_mode = c->metric == B200_METRIC_L2 ? kOutAddQ : c->metric == B200_METRIC_IP ? kOutNeg : kOutCosQ;
+        B200_TRY(gemm_chunk(c, gp, nq_c, k, f32 ? B200_KERNEL_GEMM_TF32X3 : B200_KERNEL_GEMM_BF16, out_mode, q_add,
+                            ip_min_quirk && c->metric == B200_METRIC_IP, id_offset, d_out_dis + qb * k, d_out_ids + qb * k, s));
         // L2: the winners' distances from the direct difference form (the expanded form above only RANKS; it cancels for
         // data far from the origin).  The query operand is what the caller passed (fp32), the rows what is stored.
         if (c->metric == B200_METRIC_L2 && k <= 1024 && c->rescore_l2)

@@ -30,13 +30,17 @@ constexpr int ACC_COLS = 64;
 constexpr int ACC_LD = BM + 4;
 constexpr int ACC_BYTES = ACC_COLS * ACC_LD * 4;     // 33 KB
 
+// Operand type of a tensor-core kernel: bf16 rows, fp32 rows as 3xTF32, or binary rows (1-bit AND + popcount, s32 sums)
+enum class Operand { BF16, TF32X3, B1 };
+
 // Shared-memory layout of the tensor-core kernels for a ring of `st` stages.  Stage s holds the query k-block and the half
-// tile's corpus k-block; fp32 rows (F32X3) add the lo planes of both: [A hi][A lo][B hi][B lo].  Every k-block row is one
-// 128-byte swizzle row (64 bf16 or 32 fp32).
-template <bool F32X3>
+// tile's corpus k-block; fp32 rows (TF32X3) add the lo planes of both: [A hi][A lo][B hi][B lo].  Every k-block row is one
+// 128-byte swizzle row (64 bf16, 32 fp32 or 1024 bits); for binary rows an "element" is a byte.
+template <Operand OP>
 struct Layout {
-    static constexpr int KB = F32X3 ? 32 : 64;              // elements per k-block
-    static constexpr int MMA_K = F32X3 ? 8 : 16;
+    static constexpr bool F32X3 = OP == Operand::TF32X3;
+    static constexpr int KB = F32X3 ? 32 : OP == Operand::B1 ? 128 : 64;     // elements per k-block
+    static constexpr int MMA_K = F32X3 ? 8 : OP == Operand::B1 ? 32 : 16;    // elements per wgmma (b1: 256 bits)
     static constexpr int A_PLANE = BM * 128;                // 16 KB
     static constexpr int B_PLANE = HN * 128;                // 16 KB
     static constexpr int PLANES = F32X3 ? 2 : 1;            // hi / lo
@@ -117,14 +121,15 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-#define B200_ACC64(v)                                                                                                           \
-    "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]), "+f"(v[8]), "+f"(v[9]),     \
-        "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15]), "+f"(v[16]), "+f"(v[17]), "+f"(v[18]),    \
-        "+f"(v[19]), "+f"(v[20]), "+f"(v[21]), "+f"(v[22]), "+f"(v[23]), "+f"(v[24]), "+f"(v[25]), "+f"(v[26]), "+f"(v[27]),    \
-        "+f"(v[28]), "+f"(v[29]), "+f"(v[30]), "+f"(v[31]), "+f"(v[32]), "+f"(v[33]), "+f"(v[34]), "+f"(v[35]), "+f"(v[36]),    \
-        "+f"(v[37]), "+f"(v[38]), "+f"(v[39]), "+f"(v[40]), "+f"(v[41]), "+f"(v[42]), "+f"(v[43]), "+f"(v[44]), "+f"(v[45]),    \
-        "+f"(v[46]), "+f"(v[47]), "+f"(v[48]), "+f"(v[49]), "+f"(v[50]), "+f"(v[51]), "+f"(v[52]), "+f"(v[53]), "+f"(v[54]),    \
-        "+f"(v[55]), "+f"(v[56]), "+f"(v[57]), "+f"(v[58]), "+f"(v[59]), "+f"(v[60]), "+f"(v[61]), "+f"(v[62]), "+f"(v[63])
+// the 64 accumulator operands of one wgmma m64n128, constraint C: "+f" (fp32) or "+r" (s32)
+#define B200_ACC64_AS(C, v)                                                                                                     \
+    C(v[0]), C(v[1]), C(v[2]), C(v[3]), C(v[4]), C(v[5]), C(v[6]), C(v[7]), C(v[8]), C(v[9]), C(v[10]), C(v[11]), C(v[12]),     \
+        C(v[13]), C(v[14]), C(v[15]), C(v[16]), C(v[17]), C(v[18]), C(v[19]), C(v[20]), C(v[21]), C(v[22]), C(v[23]), C(v[24]), \
+        C(v[25]), C(v[26]), C(v[27]), C(v[28]), C(v[29]), C(v[30]), C(v[31]), C(v[32]), C(v[33]), C(v[34]), C(v[35]), C(v[36]), \
+        C(v[37]), C(v[38]), C(v[39]), C(v[40]), C(v[41]), C(v[42]), C(v[43]), C(v[44]), C(v[45]), C(v[46]), C(v[47]), C(v[48]), \
+        C(v[49]), C(v[50]), C(v[51]), C(v[52]), C(v[53]), C(v[54]), C(v[55]), C(v[56]), C(v[57]), C(v[58]), C(v[59]), C(v[60]), \
+        C(v[61]), C(v[62]), C(v[63])
+#define B200_ACC64(v) B200_ACC64_AS("+f", v)
 #define B200_ACC64_REGS                                                                                                         \
     "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, " \
     "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "   \
@@ -152,26 +157,38 @@ __device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t adesc, 
         : B200_ACC64(d)
         : "l"(adesc), "l"(bdesc), "r"(accum));
 }
+// D[64 x 128] (+)= popc(A[64 x 256 bits] AND B[128 x 256 bits]), binary operands (K-major, 32 bytes per row and k-step), s32
+// accumulators.  Both operands share one byte layout, so which bit of a byte pairs with which does not matter.
+__device__ __forceinline__ void wgmma_b1_n128(int32_t (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k256.s32.b1.b1.and.popc " B200_ACC64_REGS ", %64, %65, p;\n\t"
+        "}\n"
+        : B200_ACC64_AS("+r", d)
+        : "l"(adesc), "l"(bdesc), "r"(accum));
+}
 
 // Store columns [64 Q, 64 Q + 64) of the warpgroup's two 64 x 128 accumulator fragments column-major into acc
-// ([ACC_COLS][ACC_LD]).  Fragment layout of wgmma m64nN (fp32 D): warp w, lane l holds rows 16 w + l / 4 (+ 8) and columns
-// 8 i + 2 (l % 4) (+ 1).
-template <int Q>
-__device__ __forceinline__ void acc_store(float *acc, const float (&d0)[64], const float (&d1)[64]) {
+// ([ACC_COLS][ACC_LD]) as fp32 (s32 AND counts convert exactly: they are below 2^24).  Fragment layout of wgmma m64nN: warp w,
+// lane l holds rows 16 w + l / 4 (+ 8) and columns 8 i + 2 (l % 4) (+ 1).
+template <int Q, typename T>
+__device__ __forceinline__ void acc_store(float *acc, const T (&d0)[64], const T (&d1)[64]) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int r = warp * 16 + (lane >> 2), c = 2 * (lane & 3);
 #pragma unroll
     for (int j = 0; j < ACC_COLS / 8; j++) {
         const int i = Q * (ACC_COLS / 8) + j;
         float *col = acc + (8 * j + c) * ACC_LD + r;
-        col[0] = d0[4 * i];
-        col[ACC_LD] = d0[4 * i + 1];
-        col[8] = d0[4 * i + 2];
-        col[ACC_LD + 8] = d0[4 * i + 3];
-        col[64] = d1[4 * i];
-        col[ACC_LD + 64] = d1[4 * i + 1];
-        col[72] = d1[4 * i + 2];
-        col[ACC_LD + 72] = d1[4 * i + 3];
+        col[0] = (float)d0[4 * i];
+        col[ACC_LD] = (float)d0[4 * i + 1];
+        col[8] = (float)d0[4 * i + 2];
+        col[ACC_LD + 8] = (float)d0[4 * i + 3];
+        col[64] = (float)d1[4 * i];
+        col[ACC_LD + 64] = (float)d1[4 * i + 1];
+        col[72] = (float)d1[4 * i + 2];
+        col[ACC_LD + 72] = (float)d1[4 * i + 3];
     }
 }
 // this thread's query row, 32 columns from column c0 of the staged accumulator

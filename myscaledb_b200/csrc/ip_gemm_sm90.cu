@@ -1,6 +1,6 @@
 // ip_gemm_sm90.cu -- K2: batched multi-query x corpus inner product as a dense GEMM on the Hopper tensor cores
 // (wgmma, operands staged by TMA), with the top-k selection FUSED into the epilogue: the [nq x N] score matrix is
-// never written to memory.  Two operand types share the kernel:
+// never written to memory.  Three operand types share the kernel:
 //   * bf16 queries x bf16 corpus (K2);
 //   * fp32 queries x fp32 corpus with fp32-level accuracy ("3xTF32", K2b): every fp32 value is split into two TF32
 //     numbers  x = hi + lo  (hi = x with the low 13 mantissa bits cleared, lo = tf32(x - hi)) and
@@ -8,6 +8,9 @@
 //     k-step: error ~2^-21 relative per product, the same class as an fp32 FMA chain in another summation order
 //     (tests/test_gpu_flat.py bounds it).  The queries are split once per batch (split_tf32_kernel); the corpus k-block
 //     is split in shared memory by the consumer warpgroup itself while the previous k-block's MMAs run.
+//   * binary queries x binary corpus (K2c): wgmma m64n128k256 .b1 AND + popcount counts the common set bits of a query and a
+//     row in s32.  Hamming = popc(q) + popc(y) - 2 and, Jaccard = (or - and) / or with or = popc(q) + popc(y) - and; every
+//     term is an integer below 2^24, so the keys are exactly those of binary_scan_kernel (flat_scan.cu).
 //
 // Replaces faiss::knn_inner_product / knn_L2sqr for nx >= 20 (the BLAS sgemm path) reached from tryBruteForceSearch
 // (reference: VectorIndex/Common/BruteForceSearch.h:77-88) and the FLAT Search::VectorIndex::search scan
@@ -20,9 +23,11 @@
 //   warp 4      TMA producer (one lane): A = the query k-block, B = the half tile's corpus k-block, ring of full/empty
 //               mbarriers.
 // The key that is ranked is  acc * row_scale[j] + row_bias[j]  (smaller = better):
-//   IP: -acc | L2: ||y||^2 - 2 acc (+||q||^2 added at merge) | cosine: -acc / ||y||;  filtered / out-of-range rows: scale
-//   0, bias +inf.
+//   IP: -acc | L2: ||y||^2 - 2 acc (+||q||^2 added at merge) | cosine: -acc / ||y|| | Hamming: popc(y) - 2 and (+popc(q) added
+//   at merge);  filtered / out-of-range rows: scale 0, bias +inf.
+//   Jaccard is not affine in the count: the thread maps its staged counts to keys itself (jaccard_keys32).
 #include <cstdlib>
+#include <type_traits>
 
 #include "gemm_common.cuh"
 
@@ -30,10 +35,11 @@ namespace b200 {
 namespace gemm {
 
 // Ring depth and list placement per operand type (layout: Layout in gemm_common.cuh)
-template <bool F32X3>
-struct Op : Layout<F32X3> {
-    using L = Layout<F32X3>;
-    static constexpr int MAX_ST = F32X3 ? 2 : 4;
+template <Operand OP>
+struct Op : Layout<OP> {
+    using L = Layout<OP>;
+    using Acc = typename std::conditional<OP == Operand::B1, int32_t, float>::type;   // wgmma accumulator type
+    static constexpr int MAX_ST = L::F32X3 ? 2 : 4;
     static int stages_for(int k_smem) {
         int st = MAX_ST;
         while (st > 2 && L::off_list(st) + k_smem * EPI_THREADS * 8 + SMEM_ALIGN_SLACK > SMEM_LIMIT) st--;
@@ -64,11 +70,31 @@ __global__ void split_tf32_kernel(const float *__restrict__ src, int64_t n_src, 
     }
 }
 
-template <bool F32X3>
+// Jaccard keys of one chunk of 32 staged AND counts, with the integer expression and the IEEE division of binary_scan_kernel.
+// They are returned negated, for the max-tree form of epilogue_chunk.  scale / popc_y are the tile's side arrays in SHARED
+// memory; rows with side scale 0 (filtered, out of range) give -inf, i.e. key +inf, which never enters a list.
+__device__ __forceinline__ void jaccard_keys32(float (&v)[32], int pq, const float *scale, const float *popc_y) {
+    const uint32_t sa = smem_u32(scale), ba = smem_u32(popc_y);
+#pragma unroll
+    for (int j = 0; j < 32; j += 4) {
+        float s[4], b[4];
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(s[0]), "=f"(s[1]), "=f"(s[2]), "=f"(s[3]) : "r"(sa + j * 4));
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(b[0]), "=f"(b[1]), "=f"(b[2]), "=f"(b[3]) : "r"(ba + j * 4));
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const bool live = s[i] != 0.f;
+            const int x_and = (int)v[j + i], x_or = pq + (live ? (int)b[i] : 0) - x_and;
+            const float key = x_or == 0 ? 0.f : (float)(x_or - x_and) / (float)x_or;
+            v[j + i] = live ? -key : __int_as_float(0xff800000);
+        }
+    }
+}
+
+template <Operand OP>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_qlo,
                  const __grid_constant__ CUtensorMap map_c, const GemmTopkParams p) {
-    using O = Op<F32X3>;
+    using O = Op<OP>;
     const int STAGES = p.stages;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
@@ -132,7 +158,7 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                         unsigned char *st = smem + stage * O::STAGE_BYTES;
                         mbar_arrive_expect_tx(&full_bar[stage], O::TX_BYTES);
                         tma_load_2d(&map_q, &full_bar[stage], st, kb * O::KB, qt * BM);
-                        if (F32X3) tma_load_2d(&map_qlo, &full_bar[stage], st + O::A_PLANE, kb * O::KB, qt * BM);
+                        if constexpr (O::F32X3) tma_load_2d(&map_qlo, &full_bar[stage], st + O::A_PLANE, kb * O::KB, qt * BM);
                         tma_load_2d(&map_c, &full_bar[stage], st + O::PLANES * O::A_PLANE, kb * O::KB, (int)(t * BN + h * HN));
                     }
                     __syncwarp();
@@ -160,10 +186,12 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
         else
             list_bind(list, p.list_keys_gmem + (size_t)blockIdx.x * p.list_cap * EPI_THREADS,
                       p.list_ids_gmem + (size_t)blockIdx.x * p.list_cap * EPI_THREADS, row, p.k, p.list_cap);
+        // binary Jaccard: popc(q) of this thread's query row (0 for padding rows)
+        const int pq = (OP == Operand::B1 && p.jaccard && qt * BM + row < p.nq_valid) ? (int)p.q_popc[qt * BM + row] : 0;
         const uint32_t smem0 = smem_u32(smem);
         int stage = 0;
         uint32_t phase = 0;
-        float d0[64], d1[64];
+        typename O::Acc d0[64], d1[64];
         for (int64_t t = worker; t < n_tiles; t += W) {
             const int64_t n0 = t * BN;
             // this tile's side entries (in flight during the MMAs; written after the barrier below)
@@ -184,7 +212,7 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                 for (int kb = 0; kb < kb_count; kb++) {
                     mbar_wait(&full_bar[stage], phase);
                     const uint32_t st = smem0 + stage * O::STAGE_BYTES;
-                    if (F32X3) {
+                    if constexpr (O::F32X3) {
                         // corpus k-block -> (y_hi in place, y_lo in the 4th plane); same swizzled offsets
                         uint4 *b = reinterpret_cast<uint4 *>(smem + stage * O::STAGE_BYTES + 2 * O::A_PLANE);
                         uint4 *bl = b + O::B_PLANE / 16;
@@ -203,7 +231,7 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                         wg_bar();
                     }
                     wgmma_fence();
-                    if (F32X3) {
+                    if constexpr (O::F32X3) {
                         const uint64_t ahi = make_smem_desc(st), alo = make_smem_desc(st + O::A_PLANE);
                         const uint64_t b = make_smem_desc(st + 2 * O::A_PLANE), blo = make_smem_desc(st + 2 * O::A_PLANE + O::B_PLANE);
                         constexpr uint64_t M1 = (64 * 128) >> 4;  // second M half: 64 rows further
@@ -217,6 +245,16 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                             wgmma_tf32_n128(d1, ahi + M1 + off, blo + off, 1u);
                             wgmma_tf32_n128(d0, ahi + off, b + off, 1u);
                             wgmma_tf32_n128(d1, ahi + M1 + off, b + off, 1u);
+                        }
+                    } else if constexpr (OP == Operand::B1) {
+                        const uint64_t a = make_smem_desc(st), b = make_smem_desc(st + O::A_PLANE);
+                        constexpr uint64_t M1 = (64 * 128) >> 4;
+#pragma unroll
+                        for (int k = 0; k < O::KB / O::MMA_K; k++) {
+                            const uint64_t off = (uint64_t)(k * (O::MMA_K >> 4));   // 32 bytes per k-step
+                            const uint32_t acc0 = (kb | k) != 0 ? 1u : 0u;
+                            wgmma_b1_n128(d0, a + off, b + off, acc0);
+                            wgmma_b1_n128(d1, a + M1 + off, b + off, acc0);
                         }
                     } else {
                         const uint64_t a = make_smem_desc(st), b = make_smem_desc(st + O::A_PLANE);
@@ -265,7 +303,12 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                         float v[32];
                         acc_load32(acc, row, cc * 32, v);
                         const int c0 = h * HN + q * ACC_COLS + cc * 32;
-                        epilogue_chunk(list, v, use_side, side_scale + c0, side_bias + c0, (uint32_t)(n0 + c0), tail, p.n, scratch);
+                        if (OP == Operand::B1 && p.jaccard) {
+                            jaccard_keys32(v, pq, side_scale + c0, side_bias + c0);
+                            epilogue_chunk(list, v, false, side_scale + c0, side_bias + c0, (uint32_t)(n0 + c0), tail, p.n, scratch);
+                        } else {
+                            epilogue_chunk(list, v, use_side, side_scale + c0, side_bias + c0, (uint32_t)(n0 + c0), tail, p.n, scratch);
+                        }
                     }
                 }
             }
@@ -277,25 +320,29 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
     }
 }
 
-// 2-D tensor map over row-major [rows][d_pad] (bf16 or fp32), box = [box_rows][one 128-byte row], 128-byte swizzle.
-// fp32: the last k-block may hang over d_pad (TMA zero-fills), so fp32 corpora keep their 16-byte row padding.
-static bool encode_map(CUtensorMap *map, const void *base, int64_t rows, int d_pad, int box_rows, bool f32) {
+// 2-D tensor map over row-major [rows][d_pad] (bf16, fp32 or bytes of binary rows), box = [box_rows][one 128-byte row],
+// 128-byte swizzle.  fp32: the last k-block may hang over d_pad (TMA zero-fills), so fp32 corpora keep their 16-byte row
+// padding.  Binary: rows shorter than 128 bytes and a partial last k-block are zero-filled as well (zero bits add nothing to
+// an AND count); the row stride must be a multiple of 16 bytes.
+static bool encode_map(CUtensorMap *map, const void *base, int64_t rows, int d_pad, int box_rows, Operand op) {
     EncodeTiledFn fn = get_encode_fn();
     if (!fn) return false;
-    const int es = f32 ? 4 : 2;
+    const int es = op == Operand::TF32X3 ? 4 : op == Operand::BF16 ? 2 : 1;
+    const CUtensorMapDataType type = op == Operand::TF32X3 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                     : op == Operand::BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                           : CU_TENSOR_MAP_DATA_TYPE_UINT8;
     const cuuint64_t dims[2] = {(cuuint64_t)d_pad, (cuuint64_t)rows};
     const cuuint64_t strides[1] = {(cuuint64_t)d_pad * es};
     const cuuint32_t box[2] = {(cuuint32_t)(128 / es), (cuuint32_t)box_rows};
     const cuuint32_t estr[2] = {1, 1};
-    return fn(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(base), dims, strides, box,
-              estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    return fn(map, type, 2, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <bool F32X3>
+template <Operand OP>
 static cudaError_t launch(const CUtensorMap &map_q, const CUtensorMap &map_qlo, const CUtensorMap &map_c, const GemmTopkParams &p_in,
                           int grid, cudaStream_t s) {
-    using O = Op<F32X3>;
+    using O = Op<OP>;
     GemmTopkParams p = p_in;
     // Per-thread lists sit in shared memory whenever they fit, even when that squeezes the operand ring: every insert rescans
     // the list, and from global scratch that is k L2 round trips.
@@ -304,7 +351,7 @@ static cudaError_t launch(const CUtensorMap &map_q, const CUtensorMap &map_qlo, 
     const int k_smem = p.lists_in_smem ? p.list_cap : 0;
     p.stages = O::stages_for(k_smem);
     const size_t smem = O::smem_bytes(p.stages, k_smem);
-    auto kern = gemm_topk_kernel<F32X3>;
+    auto kern = gemm_topk_kernel<OP>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     kern<<<grid, NUM_THREADS, smem, s>>>(map_q, map_qlo, map_c, p);
@@ -338,12 +385,12 @@ cudaError_t launch_gemm_topk(const GemmTopkParams &p, int grid, cudaStream_t s, 
         return cudaErrorInvalidValue;
     }
     CUtensorMap map_q, map_c;
-    if (!gemm::encode_map(&map_q, p.queries_bf16, p.nq_pad, p.d_pad, gemm::BM, false) ||
-        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::HN, false)) {
+    if (!gemm::encode_map(&map_q, p.queries_bf16, p.nq_pad, p.d_pad, gemm::BM, gemm::Operand::BF16) ||
+        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::HN, gemm::Operand::BF16)) {
         *err_detail = "cuTensorMapEncodeTiled failed";
         return cudaErrorInvalidValue;
     }
-    return gemm::launch<false>(map_q, map_q, map_c, p, grid, s);
+    return gemm::launch<gemm::Operand::BF16>(map_q, map_q, map_c, p, grid, s);
 }
 
 cudaError_t launch_gemm3_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail) {
@@ -353,13 +400,28 @@ cudaError_t launch_gemm3_topk(const GemmTopkParams &p, int grid, cudaStream_t s,
         return cudaErrorInvalidValue;
     }
     CUtensorMap map_qhi, map_qlo, map_c;
-    if (!gemm::encode_map(&map_qhi, p.queries_bf16, p.nq_pad, p.d_pad, gemm::BM, true) ||
-        !gemm::encode_map(&map_qlo, p.queries_lo, p.nq_pad, p.d_pad, gemm::BM, true) ||
-        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::HN, true)) {
+    if (!gemm::encode_map(&map_qhi, p.queries_bf16, p.nq_pad, p.d_pad, gemm::BM, gemm::Operand::TF32X3) ||
+        !gemm::encode_map(&map_qlo, p.queries_lo, p.nq_pad, p.d_pad, gemm::BM, gemm::Operand::TF32X3) ||
+        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::HN, gemm::Operand::TF32X3)) {
         *err_detail = "cuTensorMapEncodeTiled failed";
         return cudaErrorInvalidValue;
     }
-    return gemm::launch<true>(map_qhi, map_qlo, map_c, p, grid, s);
+    return gemm::launch<gemm::Operand::TF32X3>(map_qhi, map_qlo, map_c, p, grid, s);
+}
+
+cudaError_t launch_gemm_b1_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail) {
+    *err_detail = nullptr;
+    if (grid % p.q_tiles != 0 || p.d_pad % 16 != 0 || !p.row_bias || (p.jaccard && !p.q_popc)) {
+        *err_detail = "gemm b1: grid must be a multiple of q_tiles, rows a multiple of 16 bytes, popcounts set";
+        return cudaErrorInvalidValue;
+    }
+    CUtensorMap map_q, map_c;
+    if (!gemm::encode_map(&map_q, p.queries_bf16, p.nq_pad, p.d_pad, gemm::BM, gemm::Operand::B1) ||
+        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::HN, gemm::Operand::B1)) {
+        *err_detail = "cuTensorMapEncodeTiled failed";
+        return cudaErrorInvalidValue;
+    }
+    return gemm::launch<gemm::Operand::B1>(map_q, map_q, map_c, p, grid, s);
 }
 
 }  // namespace b200

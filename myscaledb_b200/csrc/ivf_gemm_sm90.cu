@@ -34,7 +34,7 @@ constexpr int IVF_THREADS_TMA = NUM_THREADS;   // consumer warpgroup + producer 
 constexpr int IVF_DEC_WARPS = 4;               // extra decoder warps of the code payloads
 constexpr int IVF_THREADS_DEC = IVF_THREADS_TMA + IVF_DEC_WARPS * 32;
 
-// smem: the Layout<false> of gemm_common.cuh.  Code payloads add a codebook region behind the lists.
+// smem: the Layout<Operand::BF16> of gemm_common.cuh.  Code payloads add a codebook region behind the lists.
 // order-preserving float <-> u32 (atomicMin on the encoding = min of the floats)
 __device__ __forceinline__ uint32_t bound_encode(float f) {
     const uint32_t b = __float_as_uint(f);
@@ -45,7 +45,7 @@ __device__ __forceinline__ float bound_decode(uint32_t u) { return (u & 0x800000
 template <int PRODUCER, int DSUB>
 __global__ void __launch_bounds__(PRODUCER == IVF_PRODUCER_TMA ? IVF_THREADS_TMA : IVF_THREADS_DEC, 1)
 ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c, const IvfGemmParams p) {
-    using C = Layout<false>;
+    using C = Layout<Operand::BF16>;
     const int STAGES = p.stages;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
@@ -461,7 +461,7 @@ static cudaError_t launch_ivf(const CUtensorMap &map_q, const CUtensorMap &map_c
     // insert into per-thread lists ~k ln(rows / k) times per lane, and every insert rescans the list: k L2 round trips from
     // global scratch against k shared-memory loads -- so the per-thread lists get shared memory even at the price of
     // a 3-stage ring; only when they do not fit beside 3 stages do they move to global scratch (and the ring gets 4 stages).
-    auto need = [&](int st, int k_smem) { return Layout<false>::off_list(st) + k_smem * EPI_THREADS * 8 + extra + SMEM_ALIGN_SLACK; };
+    auto need = [&](int st, int k_smem) { return Layout<Operand::BF16>::off_list(st) + k_smem * EPI_THREADS * 8 + extra + SMEM_ALIGN_SLACK; };
     const int coop_bytes = p.k <= 256 ? (int)round_up(coop_smem_bytes(p.k), 16) : 0;
     p.coop_enabled = coop_bytes > 0 && need(2, 0) + coop_bytes <= SMEM_LIMIT ? kCoopMax : 0;
     if (const char *ev = getenv("B200_IVF_COOP")) p.coop_enabled = std::min(p.coop_enabled, atoi(ev));   // A/B and debugging
@@ -482,7 +482,7 @@ static cudaError_t launch_ivf(const CUtensorMap &map_q, const CUtensorMap &map_c
     }
     p.stages = stages;
     const int k_smem = p.lists_in_smem ? p.list_cap : 0;
-    p.coop_smem_off = (int)round_up(Layout<false>::off_list(stages) + k_smem * EPI_THREADS * 8, 16);
+    p.coop_smem_off = (int)round_up(Layout<Operand::BF16>::off_list(stages) + k_smem * EPI_THREADS * 8, 16);
     p.codebook_smem_off = (int)round_up(p.coop_smem_off + coop_used, 16);
     const size_t smem = (size_t)need(stages, k_smem) + coop_used + 48;
     auto kern = ivf_gemm_topk_kernel<PRODUCER, DSUB>;

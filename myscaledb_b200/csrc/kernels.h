@@ -74,15 +74,18 @@ cudaError_t launch_topk_merge(const MergeParams &p, bool external, cudaStream_t 
 cudaError_t launch_rescore_l2(const void *corpus, int bf16, int64_t row_bytes, int d_pad, const float *queries, int64_t nq, int64_t id_offset,
                               int k, float *dis, int64_t *ids, cudaStream_t s);
 
-// ---- wgmma GEMM + fused top-k (ip_gemm_sm90.cu): bf16 rows, or fp32 rows as 3xTF32 ------------------
+// ---- wgmma GEMM + fused top-k (ip_gemm_sm90.cu): bf16 rows, fp32 rows as 3xTF32, or binary rows ------
 struct GemmTopkParams {
-    const void *corpus_bf16;   // [n][d_pad] bf16, d_pad % 64 == 0
-    const void *queries_bf16;  // [nq_pad][d_pad] bf16, nq_pad % 128 == 0 (3xTF32 kernel: fp32 hi plane; corpus_bf16 = fp32 rows)
+    const void *corpus_bf16;   // [n][d_pad] bf16, d_pad % 64 == 0 (binary kernel: [n][d_pad] bytes, d_pad % 16 == 0)
+    const void *queries_bf16;  // [nq_pad][d_pad] bf16, nq_pad % 128 == 0 (3xTF32 kernel: fp32 hi plane; corpus_bf16 = fp32 rows;
+                               // binary kernel: zero-padded query bytes)
     const void *queries_lo;    // 3xTF32 kernel only: fp32 lo plane [nq_pad][d_pad]
     const float *row_scale;    // per corpus row multiplier a[j] or null (= scale_const)
     float scale_const;         // -1 for IP, -2 for L2
-    const float *row_bias;     // per corpus row addend b[j] or null (=0)
+    const float *row_bias;     // per corpus row addend b[j] or null (=0); binary kernel: popcount of row j (both metrics)
     const uint8_t *alive;      // LSB-first bitmap or null
+    const float *q_popc;       // binary Jaccard: popcount of each query of the batch [nq_valid]
+    int jaccard;               // binary kernel: Jaccard keys (else Hamming: scale_const = -2, row_bias = popcounts)
     float *part_keys;          // [gridDim.x][128][k]
     uint32_t *part_ids;
     float *list_keys_gmem;     // scratch for lists that do not fit in shared memory: [gridDim.x][list_cap_for(k)][128]
@@ -114,6 +117,8 @@ cudaError_t launch_gemm_topk(const GemmTopkParams &p, int grid, cudaStream_t s, 
 // fp32 rows on the tensor cores with fp32-level accuracy (3xTF32, queries pre-split into hi / lo planes)
 cudaError_t launch_split_tf32(const float *src, int64_t n_src, int d_pad, float *hi, float *lo, int64_t n_pad, cudaStream_t s);
 cudaError_t launch_gemm3_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail);
+// binary rows on the tensor cores (wgmma .b1 AND + popcount): Hamming or Jaccard keys, exact
+cudaError_t launch_gemm_b1_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail);
 
 // ---- host ingest (ingest.cu): pageable host memory -> device through a multi-threaded pinned ring; returns a B200_* code
 int staged_h2d(void *dst, const void *src, size_t bytes, int device, cudaStream_t s);
@@ -125,5 +130,7 @@ cudaError_t launch_pad_rows_f32(const float *src, int d, float *dst, int d_pad, 
 cudaError_t launch_row_norms(const void *rows, int bf16, int d_pad, int64_t n, int mode, float *out, cudaStream_t s);
 // normalise fp32 query rows in place (cosine), skipping rows with ss < FLT_EPSILON
 cudaError_t launch_normalize_rows_f32(float *rows, int d_pad, int64_t n, cudaStream_t s);
+// number of set bits of each binary row [n][row_bytes], as an exact float
+cudaError_t launch_popc_rows(const uint8_t *rows, int64_t row_bytes, int64_t n, float *out, cudaStream_t s);
 
 }  // namespace b200

@@ -1,6 +1,6 @@
 // prep.cu -- small elementwise kernels that put host-format columns into the HBM layout
 // the scan / GEMM kernels want: zero-padded rows (16-byte multiples; 64-element multiples
-// for the tensor-core path), optional bf16 conversion, per-row norms.
+// for the tensor-core path), optional bf16 conversion, per-row norms, per-row popcounts of binary rows.
 //
 // Reference counterparts: VectorDataset<T>::normalize (VectorIndex/Common/VectorDataset.h:99-117)
 // and the ColumnArray -> contiguous float[n*d] copy in
@@ -69,6 +69,21 @@ __global__ void normalize_rows_f32_kernel(float *rows, int d_pad, int64_t n) {
     }
 }
 
+// one warp per binary row; byte loads, so any row length and alignment
+__global__ void popc_rows_kernel(const uint8_t *__restrict__ rows, int64_t row_bytes, int64_t n, float *__restrict__ out) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = warp_global; r < n; r += nwarps) {
+        const uint8_t *p = rows + r * row_bytes;
+        int c = 0;
+        for (int64_t j = lane; j < row_bytes; j += 32) c += __popc((uint32_t)p[j]);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+        if (lane == 0) out[r] = (float)c;
+    }
+}
+
 static int grid_for(int64_t work, int threads) {
     int64_t b = ceil_div(work, threads);
     if (b > 132 * 16) b = 132 * 16;
@@ -100,6 +115,13 @@ cudaError_t launch_row_norms(const void *rows, int bf16, int d_pad, int64_t n, i
 cudaError_t launch_normalize_rows_f32(float *rows, int d_pad, int64_t n, cudaStream_t s) {
     if (n == 0) return cudaSuccess;
     normalize_rows_f32_kernel<<<grid_for(n * 32, 256), 256, 0, s>>>(rows, d_pad, n);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_popc_rows(const uint8_t *rows, int64_t row_bytes, int64_t n, float *out, cudaStream_t s) {
+    if (n == 0) return cudaSuccess;
+    popc_rows_kernel<<<grid_for(n * 32, 256), 256, 0, s>>>(rows, row_bytes, n, out);
     g_launches++;
     return cudaGetLastError();
 }

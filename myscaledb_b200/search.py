@@ -24,7 +24,7 @@ METRIC_NAMES = {"L2": L2, "IP": IP, "COSINE": COSINE, "HAMMING": HAMMING, "JACCA
 F32, BF16, BIN = 0, 1, 2
 # b200_corpus_set_path codes and b200_corpus_last_variant kernel ids
 PATH_AUTO, PATH_SCAN, PATH_TENSOR, PATH_CG1, PATH_CG2, PATH_CG2_MC2, PATH_CG2_MC4, PATH_TS = range(8)
-KERNEL_SCAN, KERNEL_GEMM_BF16, KERNEL_GEMM_TS, KERNEL_GEMM_TF32X3 = 1, 2, 3, 4
+KERNEL_SCAN, KERNEL_GEMM_BF16, KERNEL_GEMM_TS, KERNEL_GEMM_TF32X3, KERNEL_GEMM_B1 = 1, 2, 3, 4, 5
 
 
 class B200Error(RuntimeError):
@@ -125,7 +125,8 @@ class Corpus:
         return self
 
     def last_variant(self):
-        """(kernel, cta_group, pairs_per_cluster, grid) of the last search: KERNEL_SCAN / _GEMM_BF16 / _GEMM_TS / _GEMM_TF32X3."""
+        """(kernel, cta_group, pairs_per_cluster, grid) of the last search: KERNEL_SCAN / _GEMM_BF16 / _GEMM_TS / _GEMM_TF32X3 /
+        _GEMM_B1 (binary rows on the tensor cores)."""
         kern, cg, mc, grid = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         _check(lib().b200_corpus_last_variant(self._h, C.byref(kern), C.byref(cg), C.byref(mc), C.byref(grid)))
         return kern.value, cg.value, mc.value, grid.value

@@ -1,9 +1,11 @@
 #!/usr/bin/env python3
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
-workload; results are pasted into DESIGN.md section 7.  Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25]"""
+workload; results are pasted into DESIGN.md section 7.
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary]"""
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -160,7 +162,69 @@ def bench_ingest():
     print(json.dumps(out))
 
 
+def gpu_context():
+    """Card, power limit and SM clocks, read in the same run as the numbers they qualify."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split("\n")[0]
+        name, power, sm, sm_max = [v.strip() for v in out.split(",")]
+        return {"card": name, "power_limit": power, "sm_clock": sm, "sm_clock_max": sm_max}
+    except Exception as e:  # the numbers stay usable, but say that the context is missing
+        return {"card": None, "context_error": repr(e)}
+
+
+def bench_binary():
+    """Binary FLAT search (Hamming, k = 10) on the two kernels a binary corpus has: the popcount scan (path 1, one pass over
+    the corpus per query) and the tensor-core kernel (path 2, wgmma .b1 AND + popcount, one pass per 128-query tile).  The
+    points span the auto threshold (kBinaryTensorMinNq, capi.cu) on both sides.  At every point both paths' outputs are
+    compared byte for byte, and 2 queries against the CPU oracle over all rows."""
+    n, k = 10_000_000, 10
+    ctx = gpu_context()
+    for bits in (1024, 256):
+        nbytes = bits // 8
+        rng = np.random.default_rng(bits)
+        y = rng.integers(0, 256, (n, nbytes), dtype=np.uint8)
+        qs = rng.integers(0, 256, (1024, nbytes), dtype=np.uint8)
+        do, io = orc.knn_binary(orc.HAMMING, qs[:2], y, k)
+        c = b2.Corpus(b2.HAMMING, bits, dtype=S.BIN).append(y)
+        c.enable_timing(True)
+        out = dict(workload=f"binary FLAT Hamming, {n} rows x {bits} bits ({n * nbytes / 1e9:.2f} GB), k={k}", **ctx, points=[],
+                   and_bit_rate="nq * n * bits / kernel s (pairs of bits ANDed and counted)",
+                   hbm_share="corpus bytes / kernel s / 3.35e12 (one corpus read per call; the scan re-reads it per query, "
+                             "mostly from L2)")
+        for nq in (1, 2, 4, 8, 16, 32, 64, 256, 1024):
+            q = qs[:nq]
+            reps = max(3, min(20, 256 // nq))
+            res, ms, wall = {}, {1: [], 2: []}, {1: [], 2: []}
+            for it in range(reps + 1):              # the first round warms both paths up and is not timed
+                for path in (1, 2):
+                    c.set_path(path)
+                    c.kernel_time(reset=True)
+                    t0 = time.perf_counter()
+                    res[path] = c.search(q, k)
+                    t = time.perf_counter() - t0
+                    kms, kn = c.kernel_time(reset=True)
+                    assert c.last_variant()[0] == (S.KERNEL_SCAN if path == 1 else S.KERNEL_GEMM_B1) and kn >= 1
+                    if it:
+                        ms[path].append(kms)
+                        wall[path].append(t)
+            same = bool(np.array_equal(res[1][1], res[2][1]) and np.array_equal(res[1][0].view(np.uint32), res[2][0].view(np.uint32)))
+            oracle_ok = bool(np.array_equal(res[2][1][:2], io[:min(nq, 2)]) and np.array_equal(res[2][0][:2], do[:min(nq, 2)]))
+            pt = {"nq": nq, "byte_identical": same, "oracle_2q_exact": oracle_ok}
+            for path, name in ((1, "scan"), (2, "tensor")):
+                kms = float(np.median(ms[path]))
+                pt[name] = {"kernel_ms": kms, "kernel_ms_min": float(np.min(ms[path])), "qps_call": nq / float(np.median(wall[path])),
+                            "and_bits_per_s": nq * n * bits / (kms * 1e-3), "corpus_GB_per_s": n * nbytes / (kms * 1e-3) / 1e9,
+                            "hbm_share": n * nbytes / (kms * 1e-3) / 3.35e12}
+            pt["tensor_speedup"] = pt["scan"]["kernel_ms"] / pt["tensor"]["kernel_ms"]
+            out["points"].append(pt)
+            print(json.dumps({"bits": bits, **pt}), file=sys.stderr, flush=True)
+        c.close()
+        print(json.dumps(out), flush=True)
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
-        {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest}[w]()
+        {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
+         "binary": bench_binary}[w]()

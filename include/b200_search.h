@@ -180,7 +180,19 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *   "SCANN", "HNSWFLAT", "HNSWSQ", "HNSWPQ"   accepted and SERVED BY THE INVERTED-FILE ENGINE with the payload their
  *                               name implies (PQ + re-rank, bf16, 8-bit, PQ): there is no graph traversal and no
  *                               anisotropic quantiser in this library; the contract for every ANN type is recall against
- *                               FLAT, not traversal order (SURVEY 8c: parity unpinned for ANN at large N).
+ *                               FLAT, not traversal order (SURVEY 8c: parity unpinned for ANN at large N);
+ *   "BINARYFLAT"                binary rows (metric HAMMING or JACCARD, d in bits: a multiple of 8, at most 65536), exact
+ *                               resident binary corpus (scan or b1 tensor-core kernel, chosen as for a binary corpus);
+ *   "BINARYIVF"                 inverted lists of the row bytes, coarse quantiser trained by k-majority (Hamming, for
+ *                               Jaccard too), scanned on the tensor cores (wgmma .b1 AND + popcount); list rows are exact,
+ *                               so every returned distance is exact and nprobe >= nlist returns the BINARYFLAT answer
+ *                               byte for byte.  nprobe must be <= 1024 unless it is >= nlist (B200_ERR_UNSUPPORTED);
+ *   "BINARYHNSW", "BINARYMSTG"  accepted and served by the BINARYIVF engine (no graph; same recall contract as HNSW*).
+ * Binary types take only HAMMING / JACCARD and float types only L2 / IP / COSINE (else B200_ERR_INVALID).  For a binary
+ * index every `rows` / `queries` pointer below (build, train, add, search and their _device forms) carries bytes
+ * [n][d / 8] behind the `const float *` type, the convention of the binary corpora.  Binary indexes have no second stage:
+ * b200_index_refine and "exact_batch=1" return B200_ERR_UNSUPPORTED; refine_factor / keep_raw are ignored and
+ * first_stage_only returns the normal (already exact) answer.
  * params: the reference's key=value / JSON parameter string: "ncentroids=1024" (or nlist), "M=32", "nprobe=64",
  * "refine_factor=8" (candidates per returned row handed to the exact second stage; 1 = first-stage distances),
  * "keep_raw=0" (do not keep the fp32 rows: no second stage, half the memory).  Parts smaller than

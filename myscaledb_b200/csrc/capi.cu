@@ -156,17 +156,17 @@ int corpus_metric(const b200_corpus *c) { return c->metric; }
 bool corpus_timing_enabled(const b200_corpus *c) { return c->timing; }
 // hooks for the index layer (ivf.cu): device view of the rows / in-place row normalisation
 const void *corpus_device_rows(const b200_corpus *c) { return c->data; }
-// append fp32 rows [n][d] that already live on the device (index build, centroid tables); asynchronous on s except for
-// a reallocation, synchronised before returning so that the caller may reuse d_rows
+// append fp32 rows [n][d] (binary corpora: bytes [n][d / 8]) that already live on the device (index build, centroid tables);
+// asynchronous on s except for a reallocation, synchronised before returning so that the caller may reuse d_rows
 int corpus_append_device(b200_corpus *c, const float *d_rows, int64_t n, cudaStream_t s) {
     if (!c || (!d_rows && n > 0) || n < 0) return fail(B200_ERR_INVALID, "bad arguments");
-    if (c->dtype == B200_DTYPE_BIN) return fail(B200_ERR_UNSUPPORTED, "device append: float corpora only");
     if (n == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(c->mu);
     B200_CUDA_OK(cudaSetDevice(c->device));
     B200_TRY(corpus_alloc(c, std::max(c->n + n, c->cap)));
     char *dst = reinterpret_cast<char *>(c->data) + c->n * c->row_bytes;
-    if (c->dtype == B200_DTYPE_BF16) B200_CUDA_OK(launch_f32_to_bf16_rows(d_rows, c->d, dst, c->d_pad, n, s));
+    if (c->dtype == B200_DTYPE_BIN) B200_CUDA_OK(cudaMemcpyAsync(dst, d_rows, (size_t)n * c->row_bytes, cudaMemcpyDeviceToDevice, s));
+    else if (c->dtype == B200_DTYPE_BF16) B200_CUDA_OK(launch_f32_to_bf16_rows(d_rows, c->d, dst, c->d_pad, n, s));
     else B200_CUDA_OK(launch_pad_rows_f32(d_rows, c->d, reinterpret_cast<float *>(dst), c->d_pad, n, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
     B200_TRY(corpus_norms(c, c->n, n));

@@ -488,6 +488,26 @@ __device__ __forceinline__ void side_fma32(float (&v)[32], const float *scale, c
     }
 }
 
+// Jaccard keys of one chunk of 32 staged AND counts, with the integer expression and the IEEE division of binary_scan_kernel.
+// They are returned negated, for the max-tree form of epilogue_chunk.  scale / popc_y are the tile's side arrays in SHARED
+// memory; rows with side scale 0 (filtered, out of range) give -inf, i.e. key +inf, which never enters a list.
+__device__ __forceinline__ void jaccard_keys32(float (&v)[32], int pq, const float *scale, const float *popc_y) {
+    const uint32_t sa = smem_u32(scale), ba = smem_u32(popc_y);
+#pragma unroll
+    for (int j = 0; j < 32; j += 4) {
+        float s[4], b[4];
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(s[0]), "=f"(s[1]), "=f"(s[2]), "=f"(s[3]) : "r"(sa + j * 4));
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(b[0]), "=f"(b[1]), "=f"(b[2]), "=f"(b[3]) : "r"(ba + j * 4));
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const bool live = s[i] != 0.f;
+            const int x_and = (int)v[j + i], x_or = pq + (live ? (int)b[i] : 0) - x_and;
+            const float key = x_or == 0 ? 0.f : (float)(x_or - x_and) / (float)x_or;
+            v[j + i] = live ? -key : __int_as_float(0xff800000);
+        }
+    }
+}
+
 // Cooperative insert (t.coop): called by the whole warp; lane `src` contributes the candidate and owns the list.
 __device__ __forceinline__ void list_insert_coop(ThreadTopK &t, int src, float key, uint32_t id) {
     const int lane = threadIdx.x & 31;
@@ -662,6 +682,20 @@ inline bool encode_rows_map(CUtensorMap *map, const void *base, int64_t rows, in
     const cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
     const cuuint32_t estr[2] = {1, 1};
     return fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(base), dims, strides, box, estr,
+              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// 2-D byte tensor map over row-major [rows][row_bytes] (binary rows), box = [box_rows][128 bytes], 128-byte swizzle.  Columns
+// past row_bytes are zero-filled by TMA (zero bits add nothing to an AND count); row_bytes must be a multiple of 16.
+inline bool encode_bytes_map(CUtensorMap *map, const void *base, int64_t rows, int row_bytes, int box_rows) {
+    EncodeTiledFn fn = get_encode_fn();
+    if (!fn) return false;
+    const cuuint64_t dims[2] = {(cuuint64_t)row_bytes, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)row_bytes};
+    const cuuint32_t box[2] = {128, (cuuint32_t)box_rows};
+    const cuuint32_t estr[2] = {1, 1};
+    return fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void *>(base), dims, strides, box, estr,
               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }

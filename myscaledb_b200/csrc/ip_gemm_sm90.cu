@@ -70,26 +70,6 @@ __global__ void split_tf32_kernel(const float *__restrict__ src, int64_t n_src, 
     }
 }
 
-// Jaccard keys of one chunk of 32 staged AND counts, with the integer expression and the IEEE division of binary_scan_kernel.
-// They are returned negated, for the max-tree form of epilogue_chunk.  scale / popc_y are the tile's side arrays in SHARED
-// memory; rows with side scale 0 (filtered, out of range) give -inf, i.e. key +inf, which never enters a list.
-__device__ __forceinline__ void jaccard_keys32(float (&v)[32], int pq, const float *scale, const float *popc_y) {
-    const uint32_t sa = smem_u32(scale), ba = smem_u32(popc_y);
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-        float s[4], b[4];
-        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(s[0]), "=f"(s[1]), "=f"(s[2]), "=f"(s[3]) : "r"(sa + j * 4));
-        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(b[0]), "=f"(b[1]), "=f"(b[2]), "=f"(b[3]) : "r"(ba + j * 4));
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const bool live = s[i] != 0.f;
-            const int x_and = (int)v[j + i], x_or = pq + (live ? (int)b[i] : 0) - x_and;
-            const float key = x_or == 0 ? 0.f : (float)(x_or - x_and) / (float)x_or;
-            v[j + i] = live ? -key : __int_as_float(0xff800000);
-        }
-    }
-}
-
 template <Operand OP>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_qlo,

@@ -18,6 +18,9 @@
 //     items (<= 128 queries x a run of pages) for the grouped tensor-core scan of ivf_gemm_sm90.cu, so a list is read
 //     from HBM once per batch however many queries probe it; per-pair partial lists are merged per query;
 //   * optional fp32 rows in id order (`keep_raw`) for the exact second stage (refine_kernel, warp per candidate).
+// Binary indexes (BINARYIVF and the BINARYHNSW / BINARYMSTG it serves) use the same pool, pages, plan and merge: the coarse
+// quantiser is trained by k-majority (Hamming assignment, per-bit majority; integer work, so deterministic), a page holds the
+// row bytes k-block-major, and the list rows are exact, so there is no second stage.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -291,6 +294,10 @@ struct ScatterParams {
     float *row_bias;
     uint32_t *row_ids;
     int payload;
+    // binary payload: rows [n][stride] bytes -> pool bytes [page][row_pad / kb_w][256][kb_w]
+    const uint8_t *brows;
+    uint8_t *bpool;
+    int row_bytes, row_pad, kb_w;
 };
 
 __device__ __forceinline__ uint32_t pool_row_of(const ScatterParams &p, uint32_t l, uint32_t pos) {
@@ -370,6 +377,88 @@ __global__ void __launch_bounds__(256) scatter_rows_kernel(const ScatterParams p
             p.row_ids[slot] = p.id_base + r;
             if (p.row_bias) p.row_bias[slot] = acc;
         }
+    }
+}
+
+// Binary payload: one warp per row of the list-sorted chunk; the row bytes go to their k-block-major slot ([page][kb][256][kb_w],
+// zero-padded to row_pad), the row's popcount to row_bias as an exact float.
+__global__ void __launch_bounds__(256) scatter_bin_rows_kernel(const ScatterParams p) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = warp_global; i < p.n; i += nwarps) {
+        const uint32_t l = p.sorted_list[i], r = p.sorted_row[i];
+        const uint32_t pos = p.list_len[l] + ((uint32_t)i - p.seg_start[l]);
+        const uint32_t slot = pool_row_of(p, l, pos);
+        const uint8_t *x = p.brows + (int64_t)r * p.stride;
+        const uint32_t page = slot / kPageRows, r_in = slot % kPageRows;
+        uint8_t *pbase = p.bpool + (size_t)page * kPageRows * p.row_pad;
+        int c = 0;
+        for (int j = lane; j < p.row_pad; j += 32) {
+            const uint32_t b = j < p.row_bytes ? x[j] : 0u;
+            pbase[((size_t)(j / p.kb_w) * kPageRows + r_in) * p.kb_w + j % p.kb_w] = (uint8_t)b;
+            c += __popc(b);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+        if (lane == 0) {
+            p.row_ids[slot] = p.id_base + r;
+            p.row_bias[slot] = (float)c;
+        }
+    }
+}
+
+// k-majority: per-(cluster, bit) counts of the members' set bits for clusters [c0, c1); bits[(l - c0) * rb * 8 + j * 8 + t] counts
+// bit t of byte j.  Integer atomics: the counts do not depend on the order of the adds.
+__global__ void bin_bit_count_kernel(const uint8_t *x, int64_t n, int stride, int rb, const uint32_t *idx, uint32_t c0, uint32_t c1, uint32_t *bits) {
+    const int64_t total = n * rb;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / rb;
+        const int j = (int)(i - r * rb);
+        const uint32_t l = idx[r];
+        if (l < c0 || l >= c1) continue;
+        uint32_t b = x[r * stride + j];
+        uint32_t *dst = bits + ((size_t)(l - c0) * rb + j) * 8;
+        while (b) {
+            atomicAdd(dst + (__ffs(b) - 1), 1u);
+            b &= b - 1;
+        }
+    }
+}
+
+// every bit of centroid c in [c0, c1) = the majority of its members' bits; an exact tie, or no member, keeps the bit
+__global__ void bin_majority_kernel(uint8_t *cent, int stride, int rb, const uint32_t *bits, const uint32_t *cnt, uint32_t c0, uint32_t c1) {
+    const int64_t total = (int64_t)(c1 - c0) * rb;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t cl = i / rb;
+        const int j = (int)(i - cl * rb);
+        const uint32_t m = cnt[c0 + cl];
+        if (!m) continue;
+        uint8_t *dst = cent + (size_t)(c0 + cl) * stride + j;
+        uint32_t v = *dst;
+        const uint32_t *b = bits + ((size_t)cl * rb + j) * 8;
+        for (int t = 0; t < 8; t++) {
+            const uint32_t twice = 2 * b[t];
+            if (twice > m) v |= 1u << t;
+            else if (twice < m) v &= ~(1u << t);
+        }
+        *dst = (uint8_t)v;
+    }
+}
+
+// assignments that differ from the previous iteration's (prev is updated)
+__global__ void count_changes_kernel(const uint32_t *idx, uint32_t *prev, int64_t n, uint32_t *changed) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || idx[i] == prev[i]) return;
+    prev[i] = idx[i];
+    atomicAdd(changed, 1u);
+}
+
+__global__ void gather_bytes_kernel(const uint8_t *x, int stride, const int64_t *pick, int64_t np, uint8_t *out) {
+    const int64_t total = np * stride;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / stride;
+        out[i] = x[pick[r] * stride + (i - r * stride)];
     }
 }
 
@@ -613,6 +702,11 @@ struct PairFill {
     float *pair_const;           // [n_pairs]
     int64_t n_pairs;
     int nprobe, nlist, d, d_pad, d_pad64, l2;
+    // binary payload: queries [nq][row_bytes] -> qbuf bytes [n_pairs][row_pad]; pair_const = popc(q) (Hamming) or 0 (Jaccard)
+    const uint8_t *bqueries;
+    uint8_t *bqbuf;
+    float *pair_popc;            // [n_pairs] popc(q)
+    int row_bytes, row_pad, jaccard;
 };
 
 __global__ void __launch_bounds__(256) pair_fill_kernel(const PairFill p) {
@@ -648,6 +742,44 @@ __global__ void __launch_bounds__(256) pair_fill_kernel(const PairFill p) {
         p.pair_part_base[i] = p.part_off[l] + ((uint32_t)i - p.pair_start[l]) * p.n_chunks[l];
         p.pair_const[i] = acc;
     }
+}
+
+// Binary payload: one warp per sorted pair gathers the query bytes (zero-padded to row_pad) and its popcount.
+__global__ void __launch_bounds__(256) pair_fill_bin_kernel(const PairFill p) {
+    const int lane = threadIdx.x & 31;
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= p.n_pairs) return;
+    const uint32_t l = p.sorted_list[i], pr = p.sorted_pair[i];
+    if (lane == 0) p.inv[pr] = (uint32_t)i;
+    if (l >= (uint32_t)p.nlist) {
+        if (lane == 0) {
+            p.pair_part_base[i] = 0;
+            p.pair_const[i] = 0.f;
+            p.pair_popc[i] = 0.f;
+        }
+        return;
+    }
+    const uint8_t *x = p.bqueries + (size_t)(pr / (uint32_t)p.nprobe) * p.row_bytes;
+    uint8_t *dst = p.bqbuf + (size_t)i * p.row_pad;
+    int c = 0;
+    for (int j = lane; j < p.row_pad; j += 32) {
+        const uint32_t b = j < p.row_bytes ? x[j] : 0u;
+        dst[j] = (uint8_t)b;
+        c += __popc(b);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if (lane == 0) {
+        p.pair_part_base[i] = p.part_off[l] + ((uint32_t)i - p.pair_start[l]) * p.n_chunks[l];
+        p.pair_const[i] = p.jaccard ? 0.f : (float)c;
+        p.pair_popc[i] = (float)c;
+    }
+}
+
+// nprobe >= nlist: every query probes every list
+__global__ void probe_all_kernel(int64_t *probe, int64_t nq, int nl) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < nq * nl) probe[i] = i % nl;
 }
 
 // per-query constants of the expanded distances: qc[q] = L2 ? ||q||^2 (- 2 <q, mid> for SQ8) : (- <q, mid> for SQ8, else 0)
@@ -756,7 +888,8 @@ __global__ void __launch_bounds__(256) ivf_merge_kernel(const IvfMerge p) {
         if (fi[j] != kNoId) {
             const float key = fk[j] + qc;
             id = (int64_t)fi[j] + p.id_offset;
-            dis = p.metric == B200_METRIC_L2 ? fmaxf(key, 0.f) : p.metric == B200_METRIC_IP ? -key : 1.f + key;
+            // binary metrics: the key is the distance (Hamming: popc(y) - 2 and + popc(q); Jaccard keyed in the scan)
+            dis = p.metric == B200_METRIC_L2 ? fmaxf(key, 0.f) : p.metric == B200_METRIC_IP ? -key : p.metric == B200_METRIC_COSINE ? 1.f + key : key;
         } else {
             dis = p.metric == B200_METRIC_IP ? -FLT_MAX : FLT_MAX;
         }
@@ -836,8 +969,11 @@ using namespace b200;
 // ------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------
-enum { IDX_FLAT = 0, IDX_IVFFLAT = 1, IDX_IVFPQ = 2, IDX_MSTG = 3, IDX_IVFSQ = 4, IDX_SCANN = 5, IDX_HNSWFLAT = 6, IDX_HNSWSQ = 7, IDX_HNSWPQ = 8 };
-static const char *kTypeNames[] = {"FLAT", "IVFFLAT", "IVFPQ", "MSTG", "IVFSQ", "SCANN", "HNSWFLAT", "HNSWSQ", "HNSWPQ"};
+enum { IDX_FLAT = 0, IDX_IVFFLAT = 1, IDX_IVFPQ = 2, IDX_MSTG = 3, IDX_IVFSQ = 4, IDX_SCANN = 5, IDX_HNSWFLAT = 6, IDX_HNSWSQ = 7, IDX_HNSWPQ = 8,
+       IDX_BINFLAT = 9, IDX_BINIVF = 10, IDX_BINHNSW = 11, IDX_BINMSTG = 12, IDX_NUM_TYPES = 13 };
+static const char *kTypeNames[] = {"FLAT", "IVFFLAT", "IVFPQ", "MSTG", "IVFSQ", "SCANN", "HNSWFLAT", "HNSWSQ", "HNSWPQ",
+                                   "BINARYFLAT", "BINARYIVF", "BINARYHNSW", "BINARYMSTG"};
+static bool is_flat_type(int t) { return t == IDX_FLAT || t == IDX_BINFLAT; }
 
 struct DevArr {
     void *p = nullptr;
@@ -889,13 +1025,18 @@ struct b200_index {
     int *d_flag = nullptr;
     uint32_t *d_list_page_off = nullptr, *d_list_pages = nullptr, *d_list_order = nullptr;   // after finalize
     std::vector<uint32_t> list_len;  // host copy after finalize
+    // binary indexes: rows are bytes [n][row_bytes]; pages [page][row_pad / kb_w][256 rows][kb_w bytes]; the coarse table is
+    // d_bcent zero-padded to cent_pad (16-byte) rows, searched as a Hamming corpus (zero bits change no distance)
+    bool binary = false;
+    int row_bytes = 0, kb_w = 0, row_pad = 0, cent_pad = 0;
+    uint8_t *d_bcent = nullptr;     // [nlist][cent_pad]
     uint32_t max_list_pages = 0;
     int device = 0, sms = 132;
     cudaStream_t stream = nullptr;
     std::mutex mu;
     // workspaces (grow-only)
     DevArr w_rows, w_assign_i, w_assign_d, w_u32a, w_u32b, w_u32c, w_u32d, w_cnt, w_plan, w_sort, w_q, w_qraw, w_probe, w_pd, w_items,
-        w_qbuf, w_inv, w_ppb, w_pconst, w_qconst, w_qb, w_cs, w_pk, w_pi, w_pw, w_lk, w_li, w_alive, w_od, w_oi, w_cand, w_host_q;
+        w_qbuf, w_inv, w_ppb, w_pconst, w_qconst, w_qb, w_cs, w_pk, w_pi, w_pw, w_lk, w_li, w_alive, w_od, w_oi, w_cand, w_host_q, w_ppopc;
     // statistics of the last search (tests, bench roofline): rows x payload bytes the scan kernel was asked to stream
     int64_t last_scan_rows = 0, last_items = 0;
     bool timing = false, timed_pending = false;
@@ -937,14 +1078,21 @@ static int parse_int_param(const char *json, const char *key, int defv) {
 extern "C" int b200_index_create(const char *type, int metric, int d, const char *params, b200_index **out) {
     if (!type || !out || d <= 0) return fail(B200_ERR_INVALID, "bad arguments");
     *out = nullptr;
-    if (metric != B200_METRIC_L2 && metric != B200_METRIC_IP && metric != B200_METRIC_COSINE)
-        return fail(B200_ERR_INVALID, "float indexes take L2, IP or COSINE");
+    const bool float_metric = metric == B200_METRIC_L2 || metric == B200_METRIC_IP || metric == B200_METRIC_COSINE;
+    const bool bin_metric = metric == B200_METRIC_HAMMING || metric == B200_METRIC_JACCARD;
+    if (!float_metric && !bin_metric) return fail(B200_ERR_INVALID, "unknown metric");
     std::string t(type);
     for (auto &ch : t) ch = (char)toupper((unsigned char)ch);
     int ty = -1;
-    for (int i = 0; i < 9; i++)
+    for (int i = 0; i < IDX_NUM_TYPES; i++)
         if (t == kTypeNames[i]) ty = i;
-    if (ty < 0) return fail(B200_ERR_UNSUPPORTED, "index type " + t + " is not implemented (FLAT, IVFFLAT, IVFSQ, IVFPQ, SCANN, MSTG, HNSWFLAT, HNSWSQ, HNSWPQ)");
+    if (ty < 0)
+        return fail(B200_ERR_UNSUPPORTED, "index type " + t + " is not implemented (FLAT, IVFFLAT, IVFSQ, IVFPQ, SCANN, MSTG, HNSWFLAT, HNSWSQ, HNSWPQ, "
+                                          "BINARYFLAT, BINARYIVF, BINARYHNSW, BINARYMSTG)");
+    const bool bin = ty >= IDX_BINFLAT;
+    if (bin && !bin_metric) return fail(B200_ERR_INVALID, "binary indexes take HAMMING or JACCARD");
+    if (!bin && !float_metric) return fail(B200_ERR_INVALID, "float indexes take L2, IP or COSINE");
+    if (bin && (d % 8 != 0 || d > (1 << 16))) return fail(B200_ERR_INVALID, "binary dimension must be a multiple of 8 bits, at most 65536");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
@@ -964,11 +1112,22 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
     switch (ty) {
         case IDX_IVFPQ: case IDX_SCANN: case IDX_HNSWPQ: ix->payload = IVF_PRODUCER_PQ; break;
         case IDX_IVFSQ: case IDX_HNSWSQ: ix->payload = IVF_PRODUCER_SQ8; break;
+        case IDX_BINFLAT: case IDX_BINIVF: case IDX_BINHNSW: case IDX_BINMSTG: ix->payload = IVF_PRODUCER_B1; break;
         default: ix->payload = IVF_PRODUCER_TMA;
+    }
+    if (bin) {
+        // Binary types: BINARYHNSW / BINARYMSTG are served by the binary inverted-file engine (no graph); list rows are exact,
+        // so there is no second stage.  k-block width kb_w = the row rounded up to 16 bytes, at most 128 (one 1024-bit wgmma
+        // k-block); TMA zero-fills the rest of the 128-byte box.
+        ix->binary = true;
+        ix->row_bytes = d / 8;
+        ix->kb_w = (int)std::min<int64_t>(128, round_up(ix->row_bytes, 16));
+        ix->row_pad = (int)round_up(ix->row_bytes, ix->kb_w);
+        ix->cent_pad = (int)round_up(ix->row_bytes, 16);
     }
     // candidates re-ranked exactly per returned row when fp32 rows are kept; plain IVFPQ / IVFSQ return first-stage
     // (ADC) distances like Faiss unless asked (refine_factor > 1)
-    const int dflt_refine = (ty == IDX_IVFPQ || ty == IDX_IVFSQ) ? 1 : (ix->payload == IVF_PRODUCER_PQ ? 16 : 4);
+    const int dflt_refine = (ty == IDX_IVFPQ || ty == IDX_IVFSQ || bin) ? 1 : (ix->payload == IVF_PRODUCER_PQ ? 16 : 4);
     ix->refine_factor = parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", dflt_refine));
     ix->keep_raw = parse_int_param(params, "keep_raw", -1);
     cudaGetDevice(&ix->device);
@@ -987,14 +1146,14 @@ extern "C" int b200_index_free(b200_index *ix) {
     if (ix->stream) cudaStreamSynchronize(ix->stream);
     if (ix->raw) b200_corpus_free(ix->raw);
     if (ix->coarse) b200_corpus_free(ix->coarse);
-    for (void *p : {(void *)ix->d_centroids, (void *)ix->d_cnorm, (void *)ix->d_pq, (void *)ix->d_pq_bf16, (void *)ix->d_sq, ix->d_pool, (void *)ix->d_row_bias,
+    for (void *p : {(void *)ix->d_centroids, (void *)ix->d_bcent, (void *)ix->d_cnorm, (void *)ix->d_pq, (void *)ix->d_pq_bf16, (void *)ix->d_sq, ix->d_pool, (void *)ix->d_row_bias,
                     (void *)ix->d_row_ids, (void *)ix->d_list_len, (void *)ix->d_tail_page, (void *)ix->d_page_owner, (void *)ix->d_page_seq,
                     (void *)ix->d_pages_used, (void *)ix->d_flag, (void *)ix->d_list_page_off, (void *)ix->d_list_pages, (void *)ix->d_list_order})
         if (p) cudaFree(p);
     for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_cnt, &ix->w_plan,
                       &ix->w_sort, &ix->w_q, &ix->w_qraw, &ix->w_probe, &ix->w_pd, &ix->w_items, &ix->w_qbuf, &ix->w_inv, &ix->w_ppb, &ix->w_pconst, &ix->w_qb, &ix->w_cs,
                       &ix->w_qconst, &ix->w_pk, &ix->w_pi, &ix->w_pw, &ix->w_lk, &ix->w_li, &ix->w_alive, &ix->w_od, &ix->w_oi, &ix->w_cand,
-                      &ix->w_host_q})
+                      &ix->w_host_q, &ix->w_ppopc})
         a->release();
     if (ix->ev0) cudaEventDestroy(ix->ev0);
     if (ix->ev1) cudaEventDestroy(ix->ev1);
@@ -1006,8 +1165,12 @@ extern "C" int b200_index_free(b200_index *ix) {
 }
 
 static size_t payload_row_bytes(const b200_index *ix) {
+    if (ix->payload == IVF_PRODUCER_B1) return (size_t)ix->row_pad;
     return ix->payload == IVF_PRODUCER_TMA ? (size_t)ix->d_pad64 * 2 : (size_t)ix->code_bytes;
 }
+
+// bytes of one caller row: fp32 [d], or binary [d / 8]
+static size_t in_row_bytes(const b200_index *ix) { return ix->binary ? (size_t)ix->row_bytes : (size_t)ix->d * 4; }
 
 // k-means on device rows x [n][stride]; centroids written to d_c [nc][d].  Assignment: exact top-1 search of the centroid
 // table with the FLAT engine (tensor cores from 20 rows up) when the table is large, the tiled fp32 kernel otherwise.
@@ -1118,18 +1281,175 @@ static int upload_coarse(b200_index *ix, cudaStream_t s) {
     return corpus_append_device(ix->coarse, ix->d_centroids, ix->nlist, s);
 }
 
+// binary centroid table as a Hamming corpus of cent_pad-byte rows (a multiple of 16 bytes: always on the b1 tensor path)
+static int upload_coarse_bin(b200_index *ix, cudaStream_t s) {
+    if (ix->coarse) b200_corpus_free(ix->coarse);
+    ix->coarse = nullptr;
+    B200_TRY(b200_corpus_create(B200_METRIC_HAMMING, B200_DTYPE_BIN, ix->cent_pad * 8, ix->nlist, &ix->coarse));
+    return corpus_append_device(ix->coarse, reinterpret_cast<const float *>(ix->d_bcent), ix->nlist, s);
+}
+
+// binary rows [n][row_bytes] (device) -> dst [n][cent_pad], zero-padded: the form the coarse table is searched with
+static int pad_bin_rows(const b200_index *ix, const void *d_rows, int64_t n, DevArr &dst, cudaStream_t s) {
+    B200_TRY(dst.reserve((size_t)std::max<int64_t>(n, 1) * ix->cent_pad));
+    if (n == 0) return B200_OK;
+    B200_CUDA_OK(cudaMemsetAsync(dst.p, 0, (size_t)n * ix->cent_pad, s));
+    B200_CUDA_OK(cudaMemcpy2DAsync(dst.p, ix->cent_pad, d_rows, ix->row_bytes, ix->row_bytes, n, cudaMemcpyDeviceToDevice, s));
+    return B200_OK;
+}
+
+// k-majority (binary k-means) on device rows x [n][stride] bytes (zero-padded, stride % 16 == 0, rb bytes of data); centroids
+// d_c [nc][stride].  Assignment: exact top-1 Hamming search of the centroid table (ties to the smaller centroid id); update: every
+// centroid bit is the majority of its members' bits (a tie keeps the bit); empty clusters take the middle member (in row order)
+// of the largest clusters.  Stops early when no assignment changes.  Integer work only: the result is deterministic.
+static int kmajority_device(const uint8_t *x, int64_t n, int stride, int rb, int nc, int iters, uint8_t *d_c, cudaStream_t s) {
+    std::vector<int64_t> pick(nc);
+    for (int i = 0; i < nc; i++) pick[i] = (int64_t)((double)i * (double)n / (double)nc);
+    // per-(cluster, bit) counts for <= 64 M counters (256 MB) at a time
+    const int chunk = (int)std::max<int64_t>(1, std::min<int64_t>(nc, ((int64_t)64 << 20) / ((int64_t)rb * 8)));
+    int64_t *d_pick = nullptr, *d_idx64 = nullptr;
+    float *d_dis = nullptr;
+    uint32_t *d_idx = nullptr, *d_prev = nullptr, *d_cnt = nullptr, *d_changed = nullptr, *d_bits = nullptr;
+    B200_CUDA_OK(cudaMalloc(&d_pick, (size_t)nc * 8));
+    B200_CUDA_OK(cudaMalloc(&d_idx64, (size_t)n * 8));
+    B200_CUDA_OK(cudaMalloc(&d_dis, (size_t)n * 4));
+    B200_CUDA_OK(cudaMalloc(&d_idx, (size_t)n * 4));
+    B200_CUDA_OK(cudaMalloc(&d_prev, (size_t)n * 4));
+    B200_CUDA_OK(cudaMalloc(&d_cnt, (size_t)nc * 4));
+    B200_CUDA_OK(cudaMalloc(&d_changed, 4));
+    B200_CUDA_OK(cudaMalloc(&d_bits, (size_t)chunk * rb * 8 * 4));
+    B200_CUDA_OK(cudaMemcpyAsync(d_pick, pick.data(), (size_t)nc * 8, cudaMemcpyHostToDevice, s));
+    gather_bytes_kernel<<<gridsz((int64_t)nc * stride), 256, 0, s>>>(x, stride, d_pick, nc, d_c);
+    B200_CUDA_OK(cudaMemsetAsync(d_prev, 0xff, (size_t)n * 4, s));
+    g_launches++;
+    std::vector<uint32_t> h_cnt(nc), h_idx;
+    b200_corpus *table = nullptr;
+    int rc = B200_OK;
+    for (int it = 0; it < iters && rc == B200_OK; it++) {
+        if (table) b200_corpus_free(table);
+        table = nullptr;
+        rc = b200_corpus_create(B200_METRIC_HAMMING, B200_DTYPE_BIN, stride * 8, nc, &table);
+        if (rc == B200_OK) rc = corpus_append_device(table, reinterpret_cast<const float *>(d_c), nc, s);
+        if (rc == B200_OK) rc = b200_corpus_search_device(table, reinterpret_cast<const float *>(x), n, 1, nullptr, 0, d_dis, d_idx64, s);
+        if (rc != B200_OK) break;
+        B200_CUDA_OK(cudaMemsetAsync(d_cnt, 0, (size_t)nc * 4, s));
+        B200_CUDA_OK(cudaMemsetAsync(d_changed, 0, 4, s));
+        assign_to_u32_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(d_idx64, n, d_idx, d_cnt);
+        count_changes_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(d_idx, d_prev, n, d_changed);
+        g_launches += 2;
+        uint32_t changed = 0;
+        B200_CUDA_OK(cudaMemcpyAsync(&changed, d_changed, 4, cudaMemcpyDeviceToHost, s));
+        B200_CUDA_OK(cudaMemcpyAsync(h_cnt.data(), d_cnt, (size_t)nc * 4, cudaMemcpyDeviceToHost, s));
+        B200_CUDA_OK(cudaStreamSynchronize(s));
+        if (it > 0 && changed == 0) break;   // the centroids already are the majorities of this assignment
+        for (int c0 = 0; c0 < nc; c0 += chunk) {
+            const int c1 = std::min(nc, c0 + chunk);
+            B200_CUDA_OK(cudaMemsetAsync(d_bits, 0, (size_t)(c1 - c0) * rb * 8 * 4, s));
+            bin_bit_count_kernel<<<gridsz(n * rb), 256, 0, s>>>(x, n, stride, rb, d_idx, (uint32_t)c0, (uint32_t)c1, d_bits);
+            bin_majority_kernel<<<gridsz((int64_t)(c1 - c0) * rb), 256, 0, s>>>(d_c, stride, rb, d_bits, d_cnt, (uint32_t)c0, (uint32_t)c1);
+            g_launches += 2;
+        }
+        if (it + 1 < iters && nc >= 2) {
+            std::vector<int> empties, order(nc);
+            for (int i = 0; i < nc; i++) {
+                order[i] = i;
+                if (h_cnt[i] == 0) empties.push_back(i);
+            }
+            if (empties.empty()) continue;
+            std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return h_cnt[a] > h_cnt[b]; });
+            h_idx.resize(n);
+            B200_CUDA_OK(cudaMemcpyAsync(h_idx.data(), d_idx, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+            B200_CUDA_OK(cudaStreamSynchronize(s));
+            std::vector<int> dst_of(nc, -1);   // large cluster -> the empty one that takes its middle member
+            for (size_t e = 0; e < empties.size(); e++) {
+                const int src = order[e];
+                if (h_cnt[src] < 2) break;
+                dst_of[src] = empties[e];
+            }
+            std::vector<uint32_t> seen(nc, 0);
+            for (int64_t r = 0; r < n; r++) {
+                const uint32_t l = h_idx[r];
+                if (dst_of[l] >= 0 && seen[l]++ == h_cnt[l] / 2)
+                    B200_CUDA_OK(cudaMemcpyAsync(d_c + (size_t)dst_of[l] * stride, x + r * stride, stride, cudaMemcpyDeviceToDevice, s));
+            }
+        }
+    }
+    if (rc == B200_OK) {
+        B200_CUDA_OK(cudaGetLastError());
+        B200_CUDA_OK(cudaStreamSynchronize(s));
+    }
+    if (table) b200_corpus_free(table);
+    for (void *p : {(void *)d_pick, (void *)d_idx64, (void *)d_dis, (void *)d_idx, (void *)d_prev, (void *)d_cnt, (void *)d_changed, (void *)d_bits})
+        if (p) cudaFree(p);
+    return rc;
+}
+
+// FLAT fallback for small parts (the reference's fallback_to_flat, test 00029) and the default nlist
+static void decide_ivf(b200_index *ix, int64_t total, int64_t n) {
+    const bool want_ivf = !is_flat_type(ix->type);
+    if (want_ivf && ix->nlist <= 0)
+        ix->nlist = (int)std::max<int64_t>(1, std::min<int64_t>(65536, (int64_t)(4.0 * sqrt((double)std::max<int64_t>(total, 1)))));
+    ix->use_ivf = want_ivf && total >= std::max<int64_t>(2000, 8ll * ix->nlist) && n >= ix->nlist;
+}
+
+// page pool for `total` rows: every list wastes less than one page
+static int alloc_pool(b200_index *ix, int64_t total, cudaStream_t s) {
+    const int nl = ix->nlist;
+    const int64_t pages = ceil_div(total, kPageRows) + nl;
+    if (pages * kPageRows >= (int64_t)0xffffffffll) return fail(B200_ERR_UNSUPPORTED, "an index shard is limited to 2^32 - 1 pool rows");
+    ix->pool_pages = (uint32_t)pages;
+    const size_t rows = (size_t)pages * kPageRows;
+    if (cudaMalloc(&ix->d_pool, rows * payload_row_bytes(ix) + 256) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(B200_ERR_NOMEM, "cudaMalloc of the page pool failed (" + std::to_string(rows * payload_row_bytes(ix)) + " bytes)");
+    }
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_pool, 0, rows * payload_row_bytes(ix), s));
+    B200_CUDA_OK(cudaMalloc(&ix->d_row_ids, rows * 4));
+    if (ix->metric == B200_METRIC_L2 || ix->binary) B200_CUDA_OK(cudaMalloc(&ix->d_row_bias, rows * 4));
+    B200_CUDA_OK(cudaMalloc(&ix->d_list_len, (size_t)nl * 4));
+    B200_CUDA_OK(cudaMalloc(&ix->d_tail_page, (size_t)nl * 4));
+    B200_CUDA_OK(cudaMalloc(&ix->d_page_owner, (size_t)pages * 4));
+    B200_CUDA_OK(cudaMalloc(&ix->d_page_seq, (size_t)pages * 4));
+    B200_CUDA_OK(cudaMalloc(&ix->d_pages_used, 4));
+    B200_CUDA_OK(cudaMalloc(&ix->d_flag, 32));
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_list_len, 0, (size_t)nl * 4, s));
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_tail_page, 0, (size_t)nl * 4, s));
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_pages_used, 0, 4, s));
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_flag, 0, 32, s));
+    return B200_OK;
+}
+
+// binary train: k-majority coarse quantiser on a device sample [n][row_bytes] (no codebooks)
+static int train_binary_locked(b200_index *ix, const void *d_rows, int64_t n) {
+    cudaStream_t s = ix->stream;
+    const int64_t total = ix->reserved > 0 ? ix->reserved : n;
+    decide_ivf(ix, total, n);
+    if (!ix->use_ivf) {
+        ix->keep_raw = 1;
+        ix->trained = true;
+        return B200_OK;
+    }
+    ix->keep_raw = 0;   // list rows are exact: nothing to re-rank
+    B200_TRY(pad_bin_rows(ix, d_rows, n, ix->w_rows, s));
+    B200_CUDA_OK(cudaMalloc(&ix->d_bcent, (size_t)ix->nlist * ix->cent_pad));
+    B200_TRY(kmajority_device(ix->w_rows.as<uint8_t>(), n, ix->cent_pad, ix->row_bytes, ix->nlist, 10, ix->d_bcent, s));
+    B200_TRY(upload_coarse_bin(ix, s));
+    B200_TRY(alloc_pool(ix, total, s));
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    ix->trained = true;
+    return B200_OK;
+}
+
 // Search::VectorIndex::train: coarse quantiser (+ PQ codebooks / SQ ranges) from a sample already on the device,
 // rows fp32 [n][d] contiguous.  Decides FLAT fallback for small parts (the reference's fallback_to_flat, test 00029).
 static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
     if (ix->trained) return fail(B200_ERR_INVALID, "index already trained");
     if (ix->built) return fail(B200_ERR_INVALID, "index already built");
+    if (ix->binary) return train_binary_locked(ix, d_rows, n);
     cudaStream_t s = ix->stream;
     const int d = ix->d;
     const int64_t total = ix->reserved > 0 ? ix->reserved : n;
-    const bool want_ivf = ix->type != IDX_FLAT;
-    if (want_ivf && ix->nlist <= 0)
-        ix->nlist = (int)std::max<int64_t>(1, std::min<int64_t>(65536, (int64_t)(4.0 * sqrt((double)std::max<int64_t>(total, 1)))));
-    ix->use_ivf = want_ivf && total >= std::max<int64_t>(2000, 8ll * ix->nlist) && n >= ix->nlist;
+    decide_ivf(ix, total, n);
     if (!ix->use_ivf) {
         ix->keep_raw = 1;
         ix->trained = true;
@@ -1216,30 +1536,7 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
         for (void *p : {(void *)d_a, (void *)d_ad, (void *)d_l, (void *)d_c32, (void *)d_res, (void *)d_samp}) cudaFree(p);
         B200_TRY(rc);
     }
-    // ---- page pool: every list wastes less than one page
-    {
-        const int64_t pages = ceil_div(total, kPageRows) + nl;
-        if (pages * kPageRows >= (int64_t)0xffffffffll) return fail(B200_ERR_UNSUPPORTED, "an index shard is limited to 2^32 - 1 pool rows");
-        ix->pool_pages = (uint32_t)pages;
-        const size_t rows = (size_t)pages * kPageRows;
-        if (cudaMalloc(&ix->d_pool, rows * payload_row_bytes(ix) + 256) != cudaSuccess) {
-            cudaGetLastError();
-            return fail(B200_ERR_NOMEM, "cudaMalloc of the page pool failed (" + std::to_string(rows * payload_row_bytes(ix)) + " bytes)");
-        }
-        B200_CUDA_OK(cudaMemsetAsync(ix->d_pool, 0, rows * payload_row_bytes(ix), s));
-        B200_CUDA_OK(cudaMalloc(&ix->d_row_ids, rows * 4));
-        if (ix->metric == B200_METRIC_L2) B200_CUDA_OK(cudaMalloc(&ix->d_row_bias, rows * 4));
-        B200_CUDA_OK(cudaMalloc(&ix->d_list_len, (size_t)nl * 4));
-        B200_CUDA_OK(cudaMalloc(&ix->d_tail_page, (size_t)nl * 4));
-        B200_CUDA_OK(cudaMalloc(&ix->d_page_owner, (size_t)pages * 4));
-        B200_CUDA_OK(cudaMalloc(&ix->d_page_seq, (size_t)pages * 4));
-        B200_CUDA_OK(cudaMalloc(&ix->d_pages_used, 4));
-        B200_CUDA_OK(cudaMalloc(&ix->d_flag, 32));
-        B200_CUDA_OK(cudaMemsetAsync(ix->d_list_len, 0, (size_t)nl * 4, s));
-        B200_CUDA_OK(cudaMemsetAsync(ix->d_tail_page, 0, (size_t)nl * 4, s));
-        B200_CUDA_OK(cudaMemsetAsync(ix->d_pages_used, 0, 4, s));
-        B200_CUDA_OK(cudaMemsetAsync(ix->d_flag, 0, 32, s));
-    }
+    B200_TRY(alloc_pool(ix, total, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
     ix->trained = true;
     return B200_OK;
@@ -1256,16 +1553,18 @@ extern "C" int b200_index_train(b200_index *ix, const float *rows, int64_t n) {
     if (!ix || (!rows && n > 0) || n < 0) return fail(B200_ERR_INVALID, "bad arguments");
     std::lock_guard<std::mutex> lk(ix->mu);
     B200_CUDA_OK(cudaSetDevice(ix->device));
-    B200_TRY(ix->w_host_q.reserve((size_t)std::max<int64_t>(n, 1) * ix->d * 4));
-    B200_TRY(staged_h2d(ix->w_host_q.p, rows, (size_t)n * ix->d * 4, ix->device, ix->stream));
+    B200_TRY(ix->w_host_q.reserve((size_t)std::max<int64_t>(n, 1) * in_row_bytes(ix)));
+    B200_TRY(staged_h2d(ix->w_host_q.p, rows, (size_t)n * in_row_bytes(ix), ix->device, ix->stream));
     B200_CUDA_OK(cudaStreamSynchronize(ix->stream));
     int rc = train_device_locked(ix, ix->w_host_q.as<float>(), n);
     ix->w_host_q.release();
     return rc;
 }
 
-// Search::VectorIndex::add of one chunk already on the device (fp32 [n][d] contiguous); row ids continue from ix->n
-static int add_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
+// Search::VectorIndex::add of one chunk already on the device (fp32 [n][d] contiguous, binary bytes [n][d / 8]); row ids
+// continue from ix->n
+static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
+    const float *d_rows = reinterpret_cast<const float *>(d_rows_v);
     if (!ix->trained) return fail(B200_ERR_INVALID, "train the index before adding rows");
     if (ix->built) return fail(B200_ERR_INVALID, "index already finalized");
     if (n == 0) return B200_OK;
@@ -1273,13 +1572,19 @@ static int add_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
     const int d = ix->d, nl = ix->nlist;
     if (ix->n + n >= (int64_t)0xffffffffll) return fail(B200_ERR_UNSUPPORTED, "an index shard is limited to 2^32 - 1 rows");
     const float *x = d_rows;
+    if (ix->binary && !ix->use_ivf) {   // BINARYFLAT / small part: an exact binary corpus
+        if (!ix->raw) B200_TRY(b200_corpus_create(ix->metric, B200_DTYPE_BIN, d, std::max<int64_t>(ix->reserved, n), &ix->raw));
+        B200_TRY(corpus_append_device(ix->raw, d_rows, n, s));
+        ix->n += n;
+        return B200_OK;
+    }
     if (ix->metric == B200_METRIC_COSINE) {
         B200_TRY(ix->w_rows.reserve((size_t)n * d * 4));
         B200_CUDA_OK(cudaMemcpyAsync(ix->w_rows.p, d_rows, (size_t)n * d * 4, cudaMemcpyDeviceToDevice, s));
         B200_CUDA_OK(launch_normalize_rows_f32(ix->w_rows.as<float>(), d, n, s));
         x = ix->w_rows.as<float>();
     }
-    if (ix->keep_raw == 1) {
+    if (ix->keep_raw == 1 && !ix->binary) {
         if (!ix->raw) {
             const int raw_metric = ix->metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
             B200_TRY(b200_corpus_create(raw_metric, B200_DTYPE_F32, d, std::max<int64_t>(ix->reserved, n), &ix->raw));
@@ -1299,6 +1604,10 @@ static int add_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
     B200_TRY(ix->w_u32d.reserve((size_t)n * 4));
     B200_TRY(ix->w_cnt.reserve((size_t)nl * 4));
     B200_TRY(ix->w_plan.reserve((size_t)nl * 4 * 3));
+    if (ix->binary) {
+        B200_TRY(pad_bin_rows(ix, d_rows, n, ix->w_rows, s));
+        x = ix->w_rows.as<float>();
+    }
     B200_TRY(b200_corpus_search_device(ix->coarse, x, n, 1, nullptr, 0, ix->w_assign_d.as<float>(), ix->w_assign_i.as<int64_t>(), s));
     B200_CUDA_OK(cudaMemsetAsync(ix->w_cnt.p, 0, (size_t)nl * 4, s));
     assign_to_u32_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(ix->w_assign_i.as<int64_t>(), n, ix->w_u32a.as<uint32_t>(), ix->w_cnt.as<uint32_t>());
@@ -1361,11 +1670,20 @@ static int add_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
     sp.row_bias = ix->d_row_bias;
     sp.row_ids = ix->d_row_ids;
     sp.payload = ix->payload;
+    if (ix->binary) {
+        sp.brows = reinterpret_cast<const uint8_t *>(d_rows);
+        sp.stride = ix->row_bytes;
+        sp.bpool = reinterpret_cast<uint8_t *>(ix->d_pool);
+        sp.row_bytes = ix->row_bytes;
+        sp.row_pad = ix->row_pad;
+        sp.kb_w = ix->kb_w;
+    }
     int over = 0;
     B200_CUDA_OK(cudaMemcpyAsync(&over, ix->d_flag, 4, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
     if (over) return fail(B200_ERR_NOMEM, "page pool exhausted: more rows added than b200_index_reserve() announced");
-    scatter_rows_kernel<<<gridsz(n * 32), 256, 0, s>>>(sp);
+    if (ix->binary) scatter_bin_rows_kernel<<<gridsz(n * 32), 256, 0, s>>>(sp);
+    else scatter_rows_kernel<<<gridsz(n * 32), 256, 0, s>>>(sp);
     add_commit_kernel<<<(unsigned)ceil_div(nl, 256), 256, 0, s>>>(ix->w_cnt.as<uint32_t>(), new_base, first_new, ix->d_list_len, ix->d_tail_page, nl);
     g_launches += 2;
     B200_CUDA_OK(cudaGetLastError());
@@ -1380,7 +1698,7 @@ extern "C" int b200_index_add_device(b200_index *ix, const float *d_rows, int64_
     B200_CUDA_OK(cudaSetDevice(ix->device));
     // bounded scratch: sub-chunks of <= 1 M rows
     for (int64_t off = 0; off < n; off += (1 << 20))
-        B200_TRY(add_device_locked(ix, d_rows + off * ix->d, std::min<int64_t>(1 << 20, n - off)));
+        B200_TRY(add_device_locked(ix, reinterpret_cast<const char *>(d_rows) + off * in_row_bytes(ix), std::min<int64_t>(1 << 20, n - off)));
     return B200_OK;
 }
 
@@ -1388,13 +1706,14 @@ extern "C" int b200_index_add(b200_index *ix, const float *rows, int64_t n) {
     if (!ix || (!rows && n > 0) || n < 0) return fail(B200_ERR_INVALID, "bad arguments");
     std::lock_guard<std::mutex> lk(ix->mu);
     B200_CUDA_OK(cudaSetDevice(ix->device));
-    const int64_t chunk = std::max<int64_t>(1024, std::min<int64_t>(1 << 20, (int64_t)(1ll << 30) / ((int64_t)ix->d * 4)));
+    const size_t rb = in_row_bytes(ix);
+    const int64_t chunk = std::max<int64_t>(1024, std::min<int64_t>(1 << 20, (int64_t)(1ll << 30) / (int64_t)rb));
     for (int64_t off = 0; off < n; off += chunk) {
         const int64_t mrows = std::min(chunk, n - off);
-        B200_TRY(ix->w_host_q.reserve((size_t)mrows * ix->d * 4));
-        B200_TRY(staged_h2d(ix->w_host_q.p, rows + off * ix->d, (size_t)mrows * ix->d * 4, ix->device, ix->stream));
+        B200_TRY(ix->w_host_q.reserve((size_t)mrows * rb));
+        B200_TRY(staged_h2d(ix->w_host_q.p, reinterpret_cast<const char *>(rows) + off * rb, (size_t)mrows * rb, ix->device, ix->stream));
         B200_CUDA_OK(cudaStreamSynchronize(ix->stream));
-        B200_TRY(add_device_locked(ix, ix->w_host_q.as<float>(), mrows));
+        B200_TRY(add_device_locked(ix, ix->w_host_q.p, mrows));
     }
     return B200_OK;
 }
@@ -1447,7 +1766,7 @@ static int finalize_locked(b200_index *ix) {
         a->release();
     if (!ix->raw) {  // an index without a single row still answers (empty results)
         const int raw_metric = ix->metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
-        if (!ix->use_ivf) B200_TRY(b200_corpus_create(raw_metric, B200_DTYPE_F32, ix->d, 0, &ix->raw));
+        if (!ix->use_ivf) B200_TRY(b200_corpus_create(ix->binary ? ix->metric : raw_metric, ix->binary ? B200_DTYPE_BIN : B200_DTYPE_F32, ix->d, 0, &ix->raw));
     }
     ix->built = true;
     return B200_OK;
@@ -1470,17 +1789,19 @@ extern "C" int b200_index_build(b200_index *ix, const float *rows, int64_t n) {
         ix->reserved = n;
     }
     int nl = ix->nlist;
-    if (ix->type != IDX_FLAT && nl <= 0) nl = (int)std::max<int64_t>(1, std::min<int64_t>(65536, (int64_t)(4.0 * sqrt((double)std::max<int64_t>(n, 1)))));
+    const bool flat = is_flat_type(ix->type);
+    if (!flat && nl <= 0) nl = (int)std::max<int64_t>(1, std::min<int64_t>(65536, (int64_t)(4.0 * sqrt((double)std::max<int64_t>(n, 1)))));
     const int64_t ns = std::min<int64_t>(n, std::max<int64_t>(256ll * std::max(nl, 1), 65536));
-    if (ns == n || ix->type == IDX_FLAT) {
-        B200_TRY(b200_index_train(ix, rows, ix->type == IDX_FLAT ? 0 : n));
+    if (ns == n || flat) {
+        B200_TRY(b200_index_train(ix, rows, flat ? 0 : n));
     } else {
-        std::vector<float> sample((size_t)ns * ix->d);
+        const size_t rb = in_row_bytes(ix);
+        std::vector<char> sample((size_t)ns * rb);
         for (int64_t i = 0; i < ns; i++) {
             const int64_t r = (int64_t)((double)i * (double)n / (double)ns);
-            memcpy(sample.data() + i * ix->d, rows + r * ix->d, (size_t)ix->d * 4);
+            memcpy(sample.data() + i * rb, reinterpret_cast<const char *>(rows) + r * rb, rb);
         }
-        B200_TRY(b200_index_train(ix, sample.data(), ns));
+        B200_TRY(b200_index_train(ix, reinterpret_cast<const float *>(sample.data()), ns));
     }
     B200_TRY(b200_index_add(ix, rows, n));
     return b200_index_finalize(ix);
@@ -1493,7 +1814,8 @@ extern "C" int b200_index_memory_bytes(const b200_index *ix, uint64_t *out_bytes
     if (ix->coarse && b200_corpus_memory_bytes(ix->coarse, &t) == B200_OK) b += t;
     if (ix->use_ivf) {
         const uint64_t rows = (uint64_t)ix->pool_pages * kPageRows;
-        b += (uint64_t)ix->nlist * ix->d * 4 + rows * (payload_row_bytes(ix) + 4 + (ix->d_row_bias ? 4 : 0)) + (uint64_t)ix->pool_pages * 12;
+        b += (uint64_t)ix->nlist * (ix->binary ? (uint64_t)ix->cent_pad : (uint64_t)ix->d * 4) + rows * (payload_row_bytes(ix) + 4 + (ix->d_row_bias ? 4 : 0)) +
+             (uint64_t)ix->pool_pages * 12;
         if (ix->d_pq) b += (uint64_t)ix->m * 256 * ix->dsub * 6;
     }
     *out_bytes = b;
@@ -1608,9 +1930,15 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
                                 cudaStream_t s) {
     if (out_num_candidates) *out_num_candidates = k;
     if (nq == 0) return B200_OK;
-    B200_TRY(prepare_queries_device(ix, d_queries, nq, s));
-    const float *d_q = ix->w_q.as<float>();
     const int force_exact = parse_int_param(params, "exact_batch", 0);
+    if (ix->binary) {
+        // binary queries are bytes [nq][d / 8]; list rows are exact, so refine_factor / keep_raw / first_stage_only change nothing
+        if (force_exact == 1) return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available on binary indexes (their lists are exact)");
+        if (!ix->use_ivf) return b200_corpus_search_device(ix->raw, d_queries, nq, k, d_alive, id_offset, d_out_dis, d_out_ids, s);
+    } else {
+        B200_TRY(prepare_queries_device(ix, d_queries, nq, s));
+    }
+    const float *d_q = ix->w_q.as<float>();
     if (!ix->use_ivf || force_exact == 1) {
         if (!ix->raw) return fail(B200_ERR_INVALID, "exact search needs the fp32 rows (keep_raw=0 index)");
         // FLAT / fallback-to-flat: exact scan of the raw rows.  The raw corpus wants [nq][d] rows: strip the padding again.
@@ -1628,8 +1956,10 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     const int nl = ix->nlist;
     int nprobe = parse_int_param(params, "nprobe", ix->default_nprobe);
     nprobe = std::max(1, std::min(nprobe, nl));
+    if (ix->binary && nprobe < nl && nprobe > 1024)
+        return fail(B200_ERR_UNSUPPORTED, "binary indexes probe at most 1024 lists (the binary corpus k limit), or all of them (nprobe >= nlist)");
     const int refine_factor = std::max(1, parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", ix->refine_factor)));
-    const bool two_stage = ix->raw && refine_factor > 1 && !first_stage_only;
+    const bool two_stage = ix->raw && refine_factor > 1 && !first_stage_only && !ix->binary;
     const int k1 = two_stage ? std::min(1024, k * refine_factor) : k;
     if (out_num_candidates) *out_num_candidates = k1;
     const int64_t n_pairs = nq * nprobe;
@@ -1637,12 +1967,20 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
 
     if (ix->timing) cudaEventRecord(ix->ev_ph[0], s);
     // ---- coarse probe: nprobe nearest centroids per query (exact FLAT search of the centroid table)
-    B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
     B200_TRY(ix->w_probe.reserve((size_t)n_pairs * 8));
     B200_TRY(ix->w_pd.reserve((size_t)n_pairs * 4));
-    if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
-    else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
-    {
+    if (ix->binary) {
+        if (nprobe >= nl) {
+            probe_all_kernel<<<(unsigned)ceil_div(n_pairs, 256), 256, 0, s>>>(ix->w_probe.as<int64_t>(), nq, nl);
+            g_launches++;
+        } else {
+            B200_TRY(pad_bin_rows(ix, d_queries, nq, ix->w_qraw, s));
+            B200_TRY(b200_corpus_search_device(ix->coarse, ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s));
+        }
+    } else {
+        B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
+        if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
+        else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
         // The centroid table is small and nprobe is a large k for it: the tensor-core path keeps one k-list per query lane
         // and never gets a selective threshold when k / nlist is a few percent.  The scan kernel's warp lists cost O(k / 32) per
         // insert: use it when its estimated time (FMA-bound, ~1.4 TB/s of table bytes per 8-query pass) undercuts ~1 us per
@@ -1747,9 +2085,10 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     search_plan_kernel<<<1, 1024, 0, s>>>(pl);
     g_launches++;
     // ---- gather queries, per-pair bookkeeping
-    B200_TRY(ix->w_qbuf.reserve(((size_t)n_pairs + 128) * ix->d_pad64 * 2));
+    const size_t qrow_bytes = ix->binary ? (size_t)ix->row_pad : (size_t)ix->d_pad64 * 2;
+    B200_TRY(ix->w_qbuf.reserve(((size_t)n_pairs + 128) * qrow_bytes));
     // the 128 rows behind the last pair are read by the last items' A tiles (query slots without a query): keep them finite
-    B200_CUDA_OK(cudaMemsetAsync(ix->w_qbuf.as<char>() + (size_t)n_pairs * ix->d_pad64 * 2, 0, (size_t)128 * ix->d_pad64 * 2, s));
+    B200_CUDA_OK(cudaMemsetAsync(ix->w_qbuf.as<char>() + (size_t)n_pairs * qrow_bytes, 0, (size_t)128 * qrow_bytes, s));
     B200_TRY(ix->w_inv.reserve((size_t)n_pairs * 4));
     B200_TRY(ix->w_ppb.reserve((size_t)n_pairs * 4));
     B200_TRY(ix->w_pconst.reserve((size_t)n_pairs * 4));
@@ -1774,10 +2113,22 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     pf.d_pad = ix->d_pad;
     pf.d_pad64 = ix->d_pad64;
     pf.l2 = ix->metric == B200_METRIC_L2;
-    pair_fill_kernel<<<(unsigned)ceil_div(n_pairs * 32, 256), 256, 0, s>>>(pf);
-    query_const_kernel<<<(unsigned)ceil_div(nq * 32, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq + 3 * ix->d : nullptr,
-                                                                        ix->metric == B200_METRIC_L2, ix->payload == IVF_PRODUCER_TMA, ix->w_qconst.as<float>());
-    g_launches += 2;
+    if (ix->binary) {
+        B200_TRY(ix->w_ppopc.reserve((size_t)n_pairs * 4));
+        pf.bqueries = reinterpret_cast<const uint8_t *>(d_queries);
+        pf.bqbuf = ix->w_qbuf.as<uint8_t>();
+        pf.pair_popc = ix->w_ppopc.as<float>();
+        pf.row_bytes = ix->row_bytes;
+        pf.row_pad = ix->row_pad;
+        pf.jaccard = ix->metric == B200_METRIC_JACCARD;
+        pair_fill_bin_kernel<<<(unsigned)ceil_div(n_pairs * 32, 256), 256, 0, s>>>(pf);
+        g_launches++;
+    } else {
+        pair_fill_kernel<<<(unsigned)ceil_div(n_pairs * 32, 256), 256, 0, s>>>(pf);
+        query_const_kernel<<<(unsigned)ceil_div(nq * 32, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq + 3 * ix->d : nullptr,
+                                                                            ix->metric == B200_METRIC_L2, ix->payload == IVF_PRODUCER_TMA, ix->w_qconst.as<float>());
+        g_launches += 2;
+    }
     // ---- the grouped tensor-core scan
     B200_TRY(ix->w_pk.reserve((size_t)max_parts * k1 * 4));
     B200_TRY(ix->w_pi.reserve((size_t)max_parts * k1 * 4));
@@ -1807,6 +2158,13 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     }
     gp.scale_const = ix->metric == B200_METRIC_L2 ? -2.f : -1.f;
     gp.d_pad = ix->d_pad64;
+    if (ix->binary) {   // Hamming ranks popc(y) - 2 and (+ popc(q) as the pair constant); Jaccard: scale 1 only marks live rows
+        gp.jaccard = ix->metric == B200_METRIC_JACCARD;
+        gp.scale_const = gp.jaccard ? 1.f : -2.f;
+        gp.d_pad = ix->row_pad;
+        gp.kb_w = ix->kb_w;
+        gp.pair_popc = ix->w_ppopc.as<float>();
+    }
     gp.k = k1;
     gp.producer = ix->payload;
     gp.codes = reinterpret_cast<const uint8_t *>(ix->d_pool);
@@ -1849,7 +2207,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     mg.sorted_list = ix->w_u32c.as<uint32_t>();
     mg.n_chunks = n_chunks;
     mg.pair_const = ix->w_pconst.as<float>();
-    mg.query_const = ix->w_qconst.as<float>();
+    mg.query_const = ix->binary ? nullptr : ix->w_qconst.as<float>();
     mg.part_keys = gp.part_keys;
     mg.part_worst = gp.part_worst;
     mg.part_ids = gp.part_ids;
@@ -1914,9 +2272,9 @@ extern "C" int b200_index_search(b200_index *ix, const float *queries, int64_t n
     B200_CUDA_OK(cudaSetDevice(ix->device));
     timing_collect(ix);
     cudaStream_t s = ix->stream;
-    B200_TRY(ix->w_host_q.reserve((size_t)nq * ix->d * 4));
+    B200_TRY(ix->w_host_q.reserve((size_t)nq * in_row_bytes(ix)));
     B200_TRY(ix->w_cand.reserve((size_t)nq * k * 12 + 16));
-    B200_CUDA_OK(cudaMemcpyAsync(ix->w_host_q.p, queries, (size_t)nq * ix->d * 4, cudaMemcpyHostToDevice, s));
+    B200_CUDA_OK(cudaMemcpyAsync(ix->w_host_q.p, queries, (size_t)nq * in_row_bytes(ix), cudaMemcpyHostToDevice, s));
     const uint8_t *d_alive = nullptr;
     if (alive_bits) {
         const size_t ab = (size_t)ceil_div(ix->n, 8);
@@ -1940,6 +2298,7 @@ extern "C" int b200_index_refine(b200_index *ix, const float *queries, int64_t n
     if (!ix || !queries || !cand_ids || !out_dis || !out_ids || nq < 0 || ncand <= 0 || k <= 0)
         return fail(B200_ERR_INVALID, "bad arguments");
     if (!ix->built) return fail(B200_ERR_INVALID, "index not built");
+    if (ix->binary) return fail(B200_ERR_UNSUPPORTED, "binary indexes have no second stage (their lists are exact)");
     if (!ix->raw) return fail(B200_ERR_INVALID, "this index keeps no fp32 rows (keep_raw=0): no second stage");
     if (k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 in refine");
     if (nq == 0) return B200_OK;
@@ -1965,6 +2324,9 @@ extern "C" int b200_index_refine(b200_index *ix, const float *queries, int64_t n
 // :578-764) write `<idx>-*.vidx3` through Search::IndexDataFileWriter; the on-disk format of the closed library
 // is not reproducible, so this is our own single-file layout ("B2IX" v2): header, fp32 rows (when kept), then the
 // quantisers and the pages in list order.  Loading re-uploads to HBM (pages become consecutive) and validates the header.
+// Binary types (9..12, metrics HAMMING / JACCARD, payload 3): BINARYFLAT stores its row bytes [n][d / 8] in place of the fp32
+// rows; the inverted types store the centroid bytes [nlist][cent_pad] in place of the fp32 centroids, then the list lengths
+// and the pages (pool bytes, row ids, popcounts) like the float lists.
 // ------------------------------------------------------------------------------------
 namespace {
 struct IxHeader {
@@ -1999,7 +2361,16 @@ static int index_save_io(b200_index *ix, Io *f) {
     h.use_ivf = ix->use_ivf ? 1 : 0; h.code_bytes = ix->code_bytes; h.n = ix->n; h.pages_used = ix->pages_used;
     bool ok = wr(f, &h, sizeof(h));
     try {
-        if (ok && ix->raw) {  // fp32 rows, unpadded (cosine indexes hold unit vectors; they are written as stored)
+        if (ok && ix->raw && ix->binary) {   // binary rows as stored: [n][d / 8] bytes
+            const size_t rb = (size_t)ix->row_bytes;
+            const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / (int64_t)rb);
+            std::vector<char> buf((size_t)chunk * rb);
+            const char *rows = reinterpret_cast<const char *>(corpus_device_rows(ix->raw));
+            for (int64_t off = 0; ok && off < ix->n; off += chunk) {
+                const int64_t mrows = std::min(chunk, ix->n - off);
+                ok = cudaMemcpy(buf.data(), rows + off * rb, (size_t)mrows * rb, cudaMemcpyDeviceToHost) == cudaSuccess && wr(f, buf.data(), (size_t)mrows * rb);
+            }
+        } else if (ok && ix->raw) {  // fp32 rows, unpadded (cosine indexes hold unit vectors; they are written as stored)
             const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / ((int64_t)ix->d_pad * 4));
             std::vector<float> buf((size_t)chunk * ix->d_pad);
             const float *rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
@@ -2016,7 +2387,8 @@ static int index_save_io(b200_index *ix, Io *f) {
                 if (bytes && cudaMemcpy(tmp.data(), dptr, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return false;
                 return wr(f, tmp.data(), bytes);
             };
-            ok = dump(ix->d_centroids, (size_t)ix->nlist * ix->d * 4) && wr(f, ix->list_len.data(), (size_t)ix->nlist * 4);
+            ok = (ix->binary ? dump(ix->d_bcent, (size_t)ix->nlist * ix->cent_pad) : dump(ix->d_centroids, (size_t)ix->nlist * ix->d * 4)) &&
+                 wr(f, ix->list_len.data(), (size_t)ix->nlist * 4);
             if (ok && ix->d_pq) ok = dump(ix->d_pq, (size_t)ix->m * 256 * ix->dsub * 4);
             if (ok && ix->d_sq) ok = dump(ix->d_sq, (size_t)4 * ix->d * 4);
             std::vector<uint32_t> pages(ix->pages_used);
@@ -2061,8 +2433,10 @@ static int index_load_io(Io *f, b200_index **out) {
     if (!rd(f, &h, sizeof(h)) || memcmp(h.magic, "B2IX", 4) != 0 || h.version != 2)
         return fail(B200_ERR_INVALID, "not a B2IX v2 index file");
     // a truncated or corrupt file must fail here, not in a kernel: every size below is derived from these fields
-    const bool sane = h.type >= 0 && h.type <= 8 && h.metric >= 0 && h.metric <= 2 && h.d > 0 && h.d <= (1 << 16) && h.n >= 0 &&
-                      h.n < (int64_t)0xffffffffll && h.payload >= 0 && h.payload <= 2 &&
+    const bool bin = h.type >= IDX_BINFLAT;
+    const bool sane = h.type >= 0 && h.type < IDX_NUM_TYPES && h.metric >= 0 && h.metric <= 4 && (h.metric >= B200_METRIC_HAMMING) == bin &&
+                      h.d > 0 && h.d <= (1 << 16) && (!bin || h.d % 8 == 0) && h.n >= 0 &&
+                      h.n < (int64_t)0xffffffffll && h.payload >= 0 && h.payload <= 3 && (h.payload == IVF_PRODUCER_B1) == bin &&
                       (!h.use_ivf || (h.nlist > 0 && h.nlist <= (1 << 24) && (uint64_t)h.pages_used <= (uint64_t)h.n / kPageRows + (uint64_t)h.nlist + 1)) &&
                       (h.payload != IVF_PRODUCER_PQ || !h.use_ivf || (h.m > 0 && h.dsub > 0 && h.m * h.dsub == h.d && h.code_bytes >= h.m && h.code_bytes % 16 == 0)) &&
                       (h.payload != IVF_PRODUCER_SQ8 || !h.use_ivf || (h.code_bytes >= h.d && h.code_bytes % 16 == 0)) && (h.has_raw || h.use_ivf);
@@ -2078,7 +2452,17 @@ static int index_load_io(Io *f, b200_index **out) {
         ix->nlist = h.nlist; ix->m = h.m; ix->dsub = h.dsub; ix->default_nprobe = h.default_nprobe; ix->refine_factor = h.refine_factor;
         ix->payload = h.payload; ix->use_ivf = h.use_ivf != 0; ix->code_bytes = h.code_bytes; ix->keep_raw = h.has_raw;
         const int raw_metric = h.metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
-        if (h.has_raw) {
+        if (h.has_raw && bin) {
+            if (b200_corpus_create(h.metric, B200_DTYPE_BIN, h.d, h.n, &ix->raw) != B200_OK) return bail(b200_last_error());
+            const size_t rb = (size_t)ix->row_bytes;
+            const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / (int64_t)rb);
+            std::vector<char> buf((size_t)chunk * rb);
+            for (int64_t off = 0; off < h.n; off += chunk) {
+                const int64_t mrows = std::min(chunk, h.n - off);
+                if (!rd(f, buf.data(), (size_t)mrows * rb)) return bail("truncated index file (rows)");
+                if (b200_corpus_append(ix->raw, buf.data(), mrows) != B200_OK) return bail(b200_last_error());
+            }
+        } else if (h.has_raw) {
             if (b200_corpus_create(raw_metric, B200_DTYPE_F32, h.d, h.n, &ix->raw) != B200_OK) return bail(b200_last_error());
             const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / ((int64_t)h.d * 4));
             std::vector<float> buf((size_t)chunk * h.d);
@@ -2099,7 +2483,8 @@ static int index_load_io(Io *f, b200_index **out) {
             };
             const int nl = h.nlist;
             ix->list_len.resize(nl);
-            if (!slurp((void **)&ix->d_centroids, (size_t)nl * h.d * 4) || !rd(f, ix->list_len.data(), (size_t)nl * 4))
+            if (!(bin ? slurp((void **)&ix->d_bcent, (size_t)nl * ix->cent_pad) : slurp((void **)&ix->d_centroids, (size_t)nl * h.d * 4)) ||
+                !rd(f, ix->list_len.data(), (size_t)nl * 4))
                 return bail("truncated index file (quantiser)");
             uint64_t total = 0, pages = 0;
             std::vector<uint32_t> page_off(nl + 1, 0);
@@ -2121,7 +2506,7 @@ static int index_load_io(Io *f, b200_index **out) {
             ix->pool_pages = ix->pages_used = h.pages_used;
             const size_t pb = (size_t)kPageRows * payload_row_bytes(ix), rows = (size_t)std::max<uint32_t>(h.pages_used, 1) * kPageRows;
             if (cudaMalloc(&ix->d_pool, rows * payload_row_bytes(ix) + 256) != cudaSuccess || cudaMalloc(&ix->d_row_ids, rows * 4) != cudaSuccess ||
-                (h.metric == B200_METRIC_L2 && cudaMalloc(&ix->d_row_bias, rows * 4) != cudaSuccess))
+                ((h.metric == B200_METRIC_L2 || bin) && cudaMalloc(&ix->d_row_bias, rows * 4) != cudaSuccess))
                 return bail("cudaMalloc of the page pool failed");
             std::vector<char> page(pb);
             std::vector<uint32_t> ids(kPageRows);
@@ -2154,7 +2539,7 @@ static int index_load_io(Io *f, b200_index **out) {
                 !up(&ix->d_list_order, order, nl) || !up(&ix->d_list_len, ix->list_len, nl) || cudaMalloc(&ix->d_flag, 32) != cudaSuccess)
                 return bail("cudaMalloc failed");
             cudaMemset(ix->d_flag, 0, 32);
-            if (upload_coarse(ix, ix->stream) != B200_OK) return bail(b200_last_error());
+            if ((bin ? upload_coarse_bin(ix, ix->stream) : upload_coarse(ix, ix->stream)) != B200_OK) return bail(b200_last_error());
             if (cudaStreamSynchronize(ix->stream) != cudaSuccess) return bail("upload failed");
         }
     } catch (const std::bad_alloc &) {

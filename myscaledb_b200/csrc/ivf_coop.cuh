@@ -51,10 +51,12 @@ __device__ __forceinline__ CoopSmem coop_smem_carve(unsigned char *base, unsigne
     return c;
 }
 
-// One 32-column chunk in cooperative mode: transform, and park the keys if this lane's slot can use any of them.
+// One 32-column chunk in cooperative mode: transform (AFFINE: v * scale + bias; else v already holds the keys), and park the
+// keys if this lane's slot can use any of them.
+template <bool AFFINE = true>
 __device__ __forceinline__ void coop_stage_chunk(float thr, float (&v)[32], const float *scale, const float *bias, float *tile_row /* this lane's slot */,
                                                  int chunk, uint32_t &chunk_mask, int swz /* slot & 31 */) {
-    side_fma32(v, scale, bias);
+    if (AFFINE) side_fma32(v, scale, bias);
     float m0 = fminf(v[0], v[1]), m1 = fminf(v[2], v[3]), m2 = fminf(v[4], v[5]), m3 = fminf(v[6], v[7]);
 #pragma unroll
     for (int j = 8; j < 32; j += 8) {

@@ -5,7 +5,8 @@
 
 namespace b200 {
 
-enum { IVF_PRODUCER_TMA = 0, IVF_PRODUCER_PQ = 1, IVF_PRODUCER_SQ8 = 2 };
+// TMA: bf16 rows as stored | PQ / SQ8: codes decoded by extra warps | B1: binary rows (bytes), wgmma .b1 AND + popcount
+enum { IVF_PRODUCER_TMA = 0, IVF_PRODUCER_PQ = 1, IVF_PRODUCER_SQ8 = 2, IVF_PRODUCER_B1 = 3 };
 
 // queries [q_begin, q_begin + q_count) of the list-sorted pair array x pages [page_begin, page_begin + page_count) of one list
 struct IvfGemmItem {
@@ -21,18 +22,21 @@ struct IvfGemmParams {
     const IvfGemmItem *items;
     const int *n_items_ptr;           // device scalar written by the planning kernel
     const uint32_t *list_pages;       // page ids, list after list
-    const float *row_bias;            // [pool rows] L2: ||y||^2 (PQ: 2<c, r^> + ||r^||^2); null for IP / cosine
+    const float *row_bias;            // [pool rows] L2: ||y||^2 (PQ: 2<c, r^> + ||r^||^2); binary: popc(y); null for IP / cosine
     const uint32_t *row_ids;          // [pool rows] row id inside the part
     const uint8_t *alive;             // LSB-first bitmap over row ids, or null
     const uint32_t *pair_part_base;   // [pairs] first partial list of pair i; chunk c of its list writes base + c
     float *part_keys;                 // [parts][k] unsorted
     uint32_t *part_ids;
     float *part_worst;                // [parts] worst kept key when the list is full, else FLT_MAX
-    float scale_const;                // -1 IP / cosine, -2 L2
+    float scale_const;                // -1 IP / cosine, -2 L2 and Hamming, 1 Jaccard (only marks a row live)
     float *list_keys_gmem;            // scratch when the per-thread lists do not fit in shared memory: [grid][list_cap_for(k)][128]
     uint32_t *list_ids_gmem;
-    int d_pad, k;
+    int d_pad, k;                     // d_pad: elements per query / pool row (binary: bytes, row_pad)
     int producer;                     // IVF_PRODUCER_*
+    // binary payload: pages are [page][d_pad / kb_w][256 rows][kb_w bytes], kb_w = min(128, row bytes rounded up to 16)
+    int kb_w, jaccard;
+    const float *pair_popc;           // Jaccard: popc(q) of every sorted pair
     // code payloads
     const uint8_t *codes;             // [pool rows][code_bytes]
     const void *codebook_bf16;        // PQ: [m][256][dsub] bf16
@@ -48,7 +52,8 @@ struct IvfGemmParams {
     int stages, lists_in_smem, list_cap, codebook_smem_off, coop_smem_off, coop_enabled;
 };
 
-// queries_bf16: gathered query rows [n_query_rows][d_pad] (bf16); pool_bf16: page pool [pool_rows][d_pad] (bf16 payload only)
+// queries_bf16: gathered query rows [n_query_rows][d_pad] (bf16; binary: bytes); pool_bf16: page pool [pool_rows][d_pad] (bf16 and
+// binary payloads only)
 cudaError_t launch_ivf_gemm_topk(const IvfGemmParams &p, const void *queries_bf16, int64_t n_query_rows, const void *pool_bf16,
                                  int64_t pool_rows, int grid, cudaStream_t s, const char **err_detail);
 

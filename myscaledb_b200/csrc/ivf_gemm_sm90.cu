@@ -19,9 +19,14 @@
 //               (PRODUCER_TMA: bf16 rows as stored)
 //   warps 5..8  (PRODUCER_PQ / PRODUCER_SQ8) decoder warps: read the half page's codes, look the sub-vectors up in the
 //               shared-memory codebook (PQ) or widen int8 (SQ8) and write the 128-byte-swizzled bf16 B tile themselves
+// PRODUCER_B1 (binary indexes): A = gathered query bytes, B = a half page's k-block of kb_w <= 128 bytes per row, zero-filled
+// by TMA to the 128-byte box; four wgmma m64n128k256 .b1 AND + popcount per k-block and M half (SASS BGMMA), s32 counts
+// staged as exact fp32.  Hamming key = popc(y) - 2 and (scale / bias path, popc(q) is the pair constant); Jaccard keys come
+// from jaccard_keys32 with popc(q) of the lane's pair, exactly as gemm_topk_kernel<B1> keys them.
 // HBM-bound by design: algorithmic bytes = (rows of the probed pages) x payload bytes per row, once per item.
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 
 #include "gemm_common.cuh"
 #include "ivf_coop.cuh"
@@ -43,9 +48,10 @@ __device__ __forceinline__ uint32_t bound_encode(float f) {
 __device__ __forceinline__ float bound_decode(uint32_t u) { return (u & 0x80000000u) ? __uint_as_float(u & 0x7fffffffu) : __uint_as_float(~u); }
 
 template <int PRODUCER, int DSUB>
-__global__ void __launch_bounds__(PRODUCER == IVF_PRODUCER_TMA ? IVF_THREADS_TMA : IVF_THREADS_DEC, 1)
+__global__ void __launch_bounds__(PRODUCER == IVF_PRODUCER_PQ || PRODUCER == IVF_PRODUCER_SQ8 ? IVF_THREADS_DEC : IVF_THREADS_TMA, 1)
 ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c, const IvfGemmParams p) {
-    using C = Layout<Operand::BF16>;
+    using C = Layout<Operand::BF16>;   // Layout<Operand::B1> has the same bytes
+    constexpr bool B1 = PRODUCER == IVF_PRODUCER_B1;
     const int STAGES = p.stages;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
@@ -58,8 +64,8 @@ ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
     uint64_t *empty_bar = full_bar + MAX_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int kb_count = p.d_pad / BK;
-    constexpr bool DEC = PRODUCER != IVF_PRODUCER_TMA;
+    const int kb_count = B1 ? p.d_pad / p.kb_w : p.d_pad / BK;
+    constexpr bool DEC = PRODUCER == IVF_PRODUCER_PQ || PRODUCER == IVF_PRODUCER_SQ8;
     const int n_items = *p.n_items_ptr;
 
     if (warp == 4 && lane == 0) {
@@ -95,8 +101,9 @@ ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
                         mbar_wait(&empty_bar[stage], phase ^ 1);
                         if (elect_one()) {
                             mbar_arrive_expect_tx(&full_bar[stage], DEC ? C::A_PLANE : C::TX_BYTES);
-                            tma_load_2d(&map_q, &full_bar[stage], sA + stage * C::STAGE_BYTES, kb * BK, (int)item.q_begin);
+                            tma_load_2d(&map_q, &full_bar[stage], sA + stage * C::STAGE_BYTES, kb * (B1 ? Layout<Operand::B1>::KB : BK), (int)item.q_begin);
                             // bf16 pages are stored k-block-major ([page][k-block][256 rows][64]): one B tile = 32 KB CONTIGUOUS in HBM
+                            // (binary pages: [page][k-block][256 rows][kb_w bytes], the same tile coordinates)
                             if (!DEC)
                                 tma_load_2d(&map_c, &full_bar[stage], sB + stage * C::STAGE_BYTES, 0,
                                             (int)((page * (uint32_t)kb_count + kb) * (uint32_t)BN + h * HN));
@@ -128,10 +135,12 @@ ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
         const uint32_t sa0 = smem_u32(sA), sb0 = smem_u32(sB);
         int stage = 0;
         uint32_t phase = 0;
-        float d0[64], d1[64];
+        typename std::conditional<B1, int32_t, float>::type d0[64], d1[64];
         for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
             const IvfGemmItem item = p.items[it];
             const bool coop = item.q_count <= (uint32_t)p.coop_enabled;   // 0 = off, else the largest cooperative item (<= kCoopMax)
+            // binary Jaccard: popc(q) of this lane's pair (0 for slots without a query)
+            const int pq = (B1 && p.jaccard && (uint32_t)row < item.q_count) ? (int)p.pair_popc[item.q_begin + row] : 0;
             list.n = 0;
             list.worst = 0;
             list.thr_key = ((uint32_t)row < item.q_count) ? FLT_MAX : -FLT_MAX;   // padding slots never enter the slow path
@@ -183,11 +192,21 @@ ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
                         wgmma_fence();
                         const uint64_t a = make_smem_desc(sa0 + stage * C::STAGE_BYTES), b = make_smem_desc(sb0 + stage * C::STAGE_BYTES);
                         constexpr uint64_t M1 = (64 * 128) >> 4;   // second M half: 64 rows further
+                        if constexpr (B1) {
+                            using L = Layout<Operand::B1>;
 #pragma unroll
-                        for (int k = 0; k < BK / UMMA_K; k++) {
-                            const uint64_t off = (uint64_t)(k * (UMMA_K * 2 >> 4));
-                            wgmma_bf16_n128(d0, a + off, b + off, (kb | k) != 0 ? 1u : 0u);
-                            wgmma_bf16_n128(d1, a + M1 + off, b + off, (kb | k) != 0 ? 1u : 0u);
+                            for (int k = 0; k < L::KB / L::MMA_K; k++) {
+                                const uint64_t off = (uint64_t)(k * (L::MMA_K >> 4));   // 32 bytes per k-step
+                                wgmma_b1_n128(d0, a + off, b + off, (kb | k) != 0 ? 1u : 0u);
+                                wgmma_b1_n128(d1, a + M1 + off, b + off, (kb | k) != 0 ? 1u : 0u);
+                            }
+                        } else {
+#pragma unroll
+                            for (int k = 0; k < BK / UMMA_K; k++) {
+                                const uint64_t off = (uint64_t)(k * (UMMA_K * 2 >> 4));
+                                wgmma_bf16_n128(d0, a + off, b + off, (kb | k) != 0 ? 1u : 0u);
+                                wgmma_bf16_n128(d1, a + M1 + off, b + off, (kb | k) != 0 ? 1u : 0u);
+                            }
                         }
                         wgmma_commit();
                         wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage goes back to the producer
@@ -230,8 +249,21 @@ ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
                             float v[32];
                             acc_load32(acc, row, cc * 32, v);
                             const int chunk = (h * HN + q * ACC_COLS) / 32 + cc;
-                            if (coop) coop_stage_chunk(coop_flt, v, side_scale + chunk * 32, side_bias + chunk * 32, tile_row, chunk, chunk_mask, lane);
-                            else epilogue_chunk(list, v, true, side_scale + chunk * 32, side_bias + chunk * 32, row0 + chunk * 32, false, 0, scratch, ext);
+                            if (B1 && p.jaccard) {
+                                // negated keys (max-tree form of epilogue_chunk); the cooperative form takes the keys themselves
+                                jaccard_keys32(v, pq, side_scale + chunk * 32, side_bias + chunk * 32);
+                                if (coop) {
+#pragma unroll
+                                    for (int j = 0; j < 32; j++) v[j] = -v[j];
+                                    coop_stage_chunk<false>(coop_flt, v, nullptr, nullptr, tile_row, chunk, chunk_mask, lane);
+                                } else {
+                                    epilogue_chunk(list, v, false, nullptr, nullptr, row0 + chunk * 32, false, 0, scratch, ext);
+                                }
+                            } else if (coop) {
+                                coop_stage_chunk(coop_flt, v, side_scale + chunk * 32, side_bias + chunk * 32, tile_row, chunk, chunk_mask, lane);
+                            } else {
+                                epilogue_chunk(list, v, true, side_scale + chunk * 32, side_bias + chunk * 32, row0 + chunk * 32, false, 0, scratch, ext);
+                            }
                         }
                     }
                 }
@@ -454,7 +486,7 @@ ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
 
 template <int PRODUCER, int DSUB>
 static cudaError_t launch_ivf(const CUtensorMap &map_q, const CUtensorMap &map_c, IvfGemmParams p, int grid, cudaStream_t s) {
-    constexpr bool DEC = PRODUCER != IVF_PRODUCER_TMA;
+    constexpr bool DEC = PRODUCER == IVF_PRODUCER_PQ || PRODUCER == IVF_PRODUCER_SQ8;
     // ring depth: as deep as the per-thread lists (and the PQ codebook) leave room for
     const int extra = PRODUCER == IVF_PRODUCER_PQ ? (int)round_up(p.codebook_bytes, 1024) : 0;
     // Shared-memory budget: operand ring (32 KB per stage) + accumulator staging + cooperative lists + per-thread lists.  Items with many queries
@@ -510,6 +542,20 @@ cudaError_t launch_ivf_gemm_topk(const IvfGemmParams &p, const void *queries_bf1
             return cudaErrorInvalidValue;
         }
         return gemm::launch_ivf<IVF_PRODUCER_TMA, 0>(map_q, map_c, p, grid, s);
+    }
+    if (p.producer == IVF_PRODUCER_B1) {
+        // bytes: the gathered queries [n_query_rows][row_pad] and the pool as a [pool_rows * k-blocks][kb_w] matrix, both read in
+        // 128-byte boxes (columns past a row, or past a kb_w < 128 k-block, arrive as zeros)
+        if (p.kb_w % 16 || p.d_pad % p.kb_w || !p.row_bias || (p.jaccard && !p.pair_popc)) {
+            *err_detail = "binary IVF scan: kb_w a multiple of 16 dividing the row, popcounts set";
+            return cudaErrorInvalidValue;
+        }
+        if (!gemm::encode_bytes_map(&map_q, queries_bf16, n_query_rows, p.d_pad, gemm::BM) ||
+            !gemm::encode_bytes_map(&map_c, pool_bf16, pool_rows * (p.d_pad / p.kb_w), p.kb_w, gemm::HN)) {
+            *err_detail = "cuTensorMapEncodeTiled failed (binary queries / pool)";
+            return cudaErrorInvalidValue;
+        }
+        return gemm::launch_ivf<IVF_PRODUCER_B1, 0>(map_q, map_c, p, grid, s);
     }
     map_c = map_q;  // unused by the decoding producers
     if (p.producer == IVF_PRODUCER_SQ8) return gemm::launch_ivf<IVF_PRODUCER_SQ8, 0>(map_q, map_c, p, grid, s);

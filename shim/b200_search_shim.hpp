@@ -261,8 +261,7 @@ struct IndexResourceUsage { size_t memory_usage_bytes = 0, disk_usage_bytes = 0,
 template <class IS, class OS, class Bitmap, DataType DT>
 class VectorIndex {
     using T = std::conditional_t<DT == DataType::FloatVector, float, bool>;
-    b200_index * h_ = nullptr;
-    b200_corpus * bin_ = nullptr;   // binary vectors: every Binary* type is a resident exact corpus
+    b200_index * h_ = nullptr;      // every type, binary ones too (BINARY*: rows and queries are bytes [n][dim / 8])
     std::string type_, params_;
     int metric_;
     size_t dim_, total_vec_;
@@ -277,6 +276,8 @@ class VectorIndex {
         idx_t * p = r.getResultIndices();
         for (size_t i = 0; i < r.numQueries() * size_t(r.topK()); ++i) if (p[i] >= 0 && size_t(p[i]) < data_ids_.size()) p[i] = data_ids_[size_t(p[i])];
     }
+    // the C ABI takes row pointers as const float *; binary rows (T = bool) are bytes [n][dim / 8] behind the same pointer
+    static const float * rows(const T * p) { return reinterpret_cast<const float *>(p); }
     void noteIds(const idx_t * ids, size_t n) {
         bool identity = data_ids_.empty();
         for (size_t i = 0; identity && ids && i < n; ++i) identity = ids[i] == idx_t(size_t(n_) + i);
@@ -288,10 +289,9 @@ public:
     VectorIndex(const std::string & /*name*/, IndexType type, Metric metric, size_t dim, size_t total_vec, const Parameters & params)
         : type_(enumToString(type)), params_(params.toString()), metric_(toB200(metric)), dim_(dim), total_vec_(total_vec),
           two_stage_(type == IndexType::MSTG || type == IndexType::SCANN) {
-        if constexpr (DT == DataType::BinaryVector) b200Check(b200_corpus_create(metric_, B200_DTYPE_BIN, int(dim), int64_t(total_vec), &bin_));
-        else b200Check(b200_index_create(type_.c_str(), metric_, int(dim), params_.c_str(), &h_));
+        b200Check(b200_index_create(type_.c_str(), metric_, int(dim), params_.c_str(), &h_));
     }
-    ~VectorIndex() { if (h_) b200_index_free(h_); if (bin_) b200_corpus_free(bin_); }
+    ~VectorIndex() { if (h_) b200_index_free(h_); }
     VectorIndex(const VectorIndex &) = delete;
 
     void setTrainDataChunkSize(size_t bytes) { train_chunk_ = bytes; }                             // VIWithDataPart.h:332
@@ -300,7 +300,6 @@ public:
         IndexResourceUsage u;
         uint64_t b = 0;
         if (h_ && b200_index_memory_bytes(h_, &b) == B200_OK) u.memory_usage_bytes = size_t(b);
-        if (bin_ && b200_corpus_memory_bytes(bin_, &b) == B200_OK) u.memory_usage_bytes = size_t(b);
         u.disk_usage_bytes = disk_bytes_;
         u.build_memory_usage_bytes = std::max(train_chunk_, add_chunk_) * 3;   // pinned staging + device scratch of one chunk
         return u;
@@ -311,36 +310,28 @@ public:
     void build(IndexSourceDataReader<T> * reader, int /*num_threads*/, std::function<bool()> cancel = {}) {
         const size_t row_bytes = DT == DataType::BinaryVector ? dim_ / 8 : dim_ * sizeof(float);
         const size_t add_rows = std::max<size_t>(1, add_chunk_ / row_bytes);
-        if constexpr (DT == DataType::FloatVector) {
-            b200Check(b200_index_reserve(h_, int64_t(total_vec_)));
-            auto sample = reader->sampleData(std::max<size_t>(1, std::min(total_vec_, train_chunk_ / row_bytes)));
-            b200Check(b200_index_train(h_, sample ? sample->getData() : nullptr, sample ? int64_t(sample->numData()) : 0));
-        }
+        b200Check(b200_index_reserve(h_, int64_t(total_vec_)));
+        auto sample = reader->sampleData(std::max<size_t>(1, std::min(total_vec_, train_chunk_ / row_bytes)));
+        b200Check(b200_index_train(h_, sample ? rows(sample->getData()) : nullptr, sample ? int64_t(sample->numData()) : 0));
         while (!reader->eof()) {
             if (cancel && cancel()) throw SearchIndexException(B200_ERR_INVALID, "vector index build cancelled");
             auto chunk = reader->readData(add_rows);
             if (!chunk || chunk->numData() == 0) break;
             noteIds(chunk->getDataID(), chunk->numData());
-            if constexpr (DT == DataType::BinaryVector) b200Check(b200_corpus_append(bin_, chunk->getData(), int64_t(chunk->numData())));
-            else b200Check(b200_index_add(h_, chunk->getData(), int64_t(chunk->numData())));
+            b200Check(b200_index_add(h_, rows(chunk->getData()), int64_t(chunk->numData())));
             n_ += int64_t(chunk->numData());
         }
-        if constexpr (DT == DataType::FloatVector) b200Check(b200_index_finalize(h_));
+        b200Check(b200_index_finalize(h_));
     }
     // search(queries, k, parameters, first_stage_only, filter) (VIWithDataPart.cpp:926, :935)
     std::shared_ptr<SearchResult> search(std::shared_ptr<DataSet<T>> q, int32_t k, Parameters & params, bool first_stage_only = false,
                                          Bitmap * filter = nullptr) {
         auto res = SearchResult::createTopKHolder(q->numData(), k);
         const uint8_t * bits = filter ? filter->get_bitmap() : nullptr;
-        if constexpr (DT == DataType::BinaryVector) {
-            b200Check(b200_corpus_search(bin_, reinterpret_cast<const float *>(q->getData()), q->numData(), k, bits,
-                                         res->getResultDistances(), res->getResultIndices()));
-        } else {
-            int64_t ncand = k;
-            b200Check(b200_index_search(h_, q->getData(), q->numData(), k, params.toString().c_str(), first_stage_only ? 1 : 0, bits,
-                                        res->getResultDistances(), res->getResultIndices(), &ncand));
-            res->setNumCandidates(first_stage_only ? k : ncand);
-        }
+        int64_t ncand = k;
+        b200Check(b200_index_search(h_, rows(q->getData()), q->numData(), k, params.toString().c_str(), first_stage_only ? 1 : 0, bits,
+                                    res->getResultDistances(), res->getResultIndices(), &ncand));
+        res->setNumCandidates(first_stage_only ? k : ncand);
         mapIds(*res);
         return res;
     }
@@ -367,8 +358,7 @@ public:
         if (!os) throw SearchIndexException(B200_ERR_INVALID, "cannot open the index output stream");
         struct Ctx { OS * os; size_t bytes; } ctx{os.get(), 0};
         auto wr = [](void * c, const void * p, size_t n) -> int { auto * x = static_cast<Ctx *>(c); x->os->write(static_cast<const char *>(p), std::streamsize(n)); x->bytes += n; return 0; };
-        if constexpr (DT == DataType::BinaryVector) throw SearchIndexException(B200_ERR_UNSUPPORTED, "binary indexes are rebuilt from the part, not serialized");
-        else b200Check(b200_index_save_cb(h_, wr, &ctx));
+        b200Check(b200_index_save_cb(h_, wr, &ctx));
         os->close();
         disk_bytes_ = ctx.bytes;
     }

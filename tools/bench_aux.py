@@ -2,7 +2,7 @@
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
 workload; results are pasted into DESIGN.md section 7.
-Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary]"""
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf]"""
 import json
 import os
 import subprocess
@@ -223,8 +223,82 @@ def bench_binary():
         print(json.dumps(out), flush=True)
 
 
+def binary_clustered(n, nbytes, n_centres, seed, nq=1024):
+    """seeded clustered binary rows: random centres; a row flips each bit of its centre with probability 1/16 (AND of 4
+    random bytes)"""
+    rng = np.random.default_rng(seed)
+    centres = rng.integers(0, 256, (n_centres, nbytes), dtype=np.uint8)
+
+    def draw(m):
+        flips = rng.integers(0, 256, (m, nbytes), dtype=np.uint8)
+        for _ in range(3):
+            flips &= rng.integers(0, 256, (m, nbytes), dtype=np.uint8)
+        return centres[rng.integers(0, n_centres, m)] ^ flips
+
+    y = np.empty((n, nbytes), np.uint8)
+    for i in range(0, n, 500_000):
+        y[i:i + 500_000] = draw(min(500_000, n - i))
+    return y, draw(nq)
+
+
+def bench_binary_ivf():
+    """BINARYIVF (default nlist, k = 10) against the exact BINARYFLAT answer on 10 M clustered rows of 1024 and 256 bits:
+    recall@10, scan-kernel and call time, rows streamed and list bytes per second (last_scan), the BINARYFLAT call time
+    at the same nq (alternating with the index), build times, and a byte-identity check of nprobe = nlist against BINARYFLAT."""
+    n, k = 10_000_000, 10
+    ctx = gpu_context()
+    for bits in (1024, 256):
+        nbytes = bits // 8
+        y, qs = binary_clustered(n, nbytes, 10_000, seed=bits)
+        t0 = time.perf_counter()
+        flat = b2.VectorIndex("BINARYFLAT", b2.HAMMING, bits).build(y)
+        t_flat = time.perf_counter() - t0
+        t0 = time.perf_counter()
+        ix = b2.VectorIndex("BINARYIVF", b2.HAMMING, bits).build(y)
+        t_ivf = time.perf_counter() - t0
+        nlist = ix.info()["nlist"]
+        sizes = ix.list_sizes()
+        ix.enable_timing(True)
+        out = dict(workload=f"BINARYIVF Hamming, {n} clustered rows x {bits} bits, nlist={nlist}, k={k}", **ctx,
+                   build_s={"BINARYIVF": t_ivf, "BINARYFLAT": t_flat}, list_rows={"min": int(sizes.min()), "max": int(sizes.max())}, points=[])
+        q16 = qs[:16]
+        out["all_lists_byte_identical_nq16"] = bool(
+            np.array_equal(ix.search(q16, k, params=f"nprobe={nlist}")[1], flat.search(q16, k)[1]) and
+            np.array_equal(ix.search(q16, k, params=f"nprobe={nlist}")[0].view(np.uint32), flat.search(q16, k)[0].view(np.uint32)))
+        for nq in (1, 16, 256, 1024):
+            q = qs[:nq]
+            truth = flat.search(q, k)[1]
+            for nprobe in (1, 4, 16, 64):
+                prm = f"nprobe={nprobe}"
+                reps = 10 if nq <= 16 else 4
+                wall, wall_flat, kms, rows = [], [], [], 0
+                for it in range(reps + 1):   # the first round warms both up and is not timed
+                    ix.last_scan(reset=True)
+                    t0 = time.perf_counter()
+                    _, ids = ix.search(q, k, params=prm)
+                    t = time.perf_counter() - t0
+                    sc = ix.last_scan(reset=True)
+                    t0 = time.perf_counter()
+                    flat.search(q, k)
+                    tf = time.perf_counter() - t0
+                    if it:
+                        wall.append(t)
+                        wall_flat.append(tf)
+                        kms.append(sc["kernel_ms"])
+                        rows = sc["rows_streamed"]
+                km = float(np.median(kms))
+                pt = {"nq": nq, "nprobe": nprobe, "recall@10": recall(ids, truth), "scan_kernel_ms": km,
+                      "call_ms": 1e3 * float(np.median(wall)), "binaryflat_call_ms": 1e3 * float(np.median(wall_flat)),
+                      "rows_streamed": rows, "list_GB_per_s": rows * sc["payload_row_bytes"] / (km * 1e-3) / 1e9 if km > 0 else None}
+                out["points"].append(pt)
+                print(json.dumps({"bits": bits, **pt}), file=sys.stderr, flush=True)
+        ix.close()
+        flat.close()
+        print(json.dumps(out), flush=True)
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
         {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
-         "binary": bench_binary}[w]()
+         "binary": bench_binary, "binary_ivf": bench_binary_ivf}[w]()

@@ -174,7 +174,9 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *   "FLAT"                      exact scan of the resident rows;
  *   "IVFFLAT"                   inverted lists holding bf16 rows, candidates re-ranked exactly against the fp32 rows;
  *   "IVFSQ"                     lists of 8-bit scalar-quantised rows (one byte per dimension);
- *   "IVFPQ"                     lists of m-byte product-quantiser codes of the residual (d / M in {1, 2, 4, 8}, d <= 320);
+ *   "IVFPQ"                     lists of m-byte product-quantiser codes of the residual (d / M in {1, 2, 4, 8}, d <= 220: the
+ *                               scan keeps the 512 B x d bf16 codebook in shared memory; wider PQ indexes, SCANN and HNSWPQ
+ *                               included, are refused at train with B200_ERR_UNSUPPORTED);
  *   "MSTG"                      closed source upstream; here the two-stage index of SURVEY 2.5 K6: bf16 lists + exact
  *                               fp32 second stage (supportTwoStageSearch, first_stage_only, computeTopDistanceSubset);
  *   "SCANN", "HNSWFLAT", "HNSWSQ", "HNSWPQ"   accepted and SERVED BY THE INVERTED-FILE ENGINE with the payload their
@@ -193,7 +195,9 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  * [n][d / 8] behind the `const float *` type, the convention of the binary corpora.  Binary indexes have no second stage:
  * b200_index_refine and "exact_batch=1" return B200_ERR_UNSUPPORTED; refine_factor / keep_raw are ignored and
  * first_stage_only returns the normal (already exact) answer.
- * params: the reference's key=value / JSON parameter string: "ncentroids=1024" (or nlist), "M=32", "nprobe=64",
+ * params: the reference's key=value / JSON parameter string: "ncentroids=1024" (or nlist), "M=32", "nprobe=64" (float
+ * indexes: nprobe >= nlist probes every list; below nlist, nprobe <= 2048, the k limit of the exact scan that ranks the
+ * centroids above 1024 probes, else B200_ERR_UNSUPPORTED),
  * "refine_factor=8" (candidates per returned row handed to the exact second stage; 1 = first-stage distances),
  * "keep_raw=0" (do not keep the fp32 rows: no second stage, half the memory).  Parts smaller than
  * max(2000, 8 * nlist) rows are served by an exact FLAT scan (the reference's fallback_to_flat, test 00029).

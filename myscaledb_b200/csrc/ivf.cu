@@ -782,7 +782,8 @@ __global__ void probe_all_kernel(int64_t *probe, int64_t nq, int nl) {
     if (i < nq * nl) probe[i] = i % nl;
 }
 
-// per-query constants of the expanded distances: qc[q] = L2 ? ||q||^2 (- 2 <q, mid> for SQ8) : (- <q, mid> for SQ8, else 0)
+// per-query constants of the expanded distances (bf16 and SQ8 payloads; PQ has its query term in the pair constant):
+// qc[q] = L2 ? ||q||^2 (- 2 <q, mid> for SQ8) : (- <q, mid> for SQ8, else 0)
 __global__ void query_const_kernel(const float *queries, int64_t nq, int d, int d_pad, const float *sq_mid, int l2, int round_bf16, float *qc) {
     const int lane = threadIdx.x & 31;
     const int64_t q = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -1455,6 +1456,23 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
         ix->trained = true;
         return B200_OK;
     }
+    if (ix->payload == IVF_PRODUCER_PQ) {
+        if (ix->m <= 0) {  // default: sub-vectors of <= 8 dims
+            ix->m = d;
+            for (int cand : {8, 4, 2, 1})
+                if (d % cand == 0) { ix->m = d / cand; break; }
+        }
+        if (d % ix->m) return fail(B200_ERR_INVALID, "PQ M must divide the dimension");
+        const int dsub = d / ix->m;
+        if (dsub != 1 && dsub != 2 && dsub != 4 && dsub != 8)
+            return fail(B200_ERR_UNSUPPORTED, "PQ sub-vector length d / M must be 1, 2, 4 or 8 (codes are decoded into tensor-core tiles)");
+        // the scan keeps the bf16 codebook (512 B x d) in shared memory beside at least a 2-stage operand ring
+        if (!ivf_pq_codebook_fits((int64_t)512 * d)) {
+            int dmax = d;
+            while (dmax > 1 && !ivf_pq_codebook_fits((int64_t)512 * dmax)) dmax--;
+            return fail(B200_ERR_UNSUPPORTED, "PQ codebook (512 B x d) must fit in shared memory next to the operand ring: d <= " + std::to_string(dmax));
+        }
+    }
     if (ix->keep_raw < 0) ix->keep_raw = 1;
     const int nl = ix->nlist;
     // training rows: unit length under cosine
@@ -1487,17 +1505,7 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
         B200_CUDA_OK(cudaMemcpyAsync(ix->d_sq, h.data(), (size_t)4 * d * 4, cudaMemcpyHostToDevice, s));
     }
     if (ix->payload == IVF_PRODUCER_PQ) {
-        if (ix->m <= 0) {  // default: sub-vectors of <= 8 dims
-            ix->m = d;
-            for (int cand : {8, 4, 2, 1})
-                if (d % cand == 0) { ix->m = d / cand; break; }
-        }
-        if (d % ix->m) return fail(B200_ERR_INVALID, "PQ M must divide the dimension");
-        const int m = ix->m, dsub = d / m;
-        if (dsub != 1 && dsub != 2 && dsub != 4 && dsub != 8)
-            return fail(B200_ERR_UNSUPPORTED, "PQ sub-vector length d / M must be 1, 2, 4 or 8 (codes are decoded into tensor-core tiles)");
-        if ((size_t)256 * ix->d_pad64 * 2 > 160 * 1024)
-            return fail(B200_ERR_UNSUPPORTED, "PQ codebook (512 B x d) must fit in shared memory next to the operand ring: d <= 320");
+        const int m = ix->m, dsub = d / m;   // validated above
         ix->dsub = dsub;
         ix->code_bytes = (int)round_up(m, 16);
         B200_CUDA_OK(cudaMalloc(&ix->d_pq, (size_t)m * 256 * dsub * 4));
@@ -2125,9 +2133,12 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         g_launches++;
     } else {
         pair_fill_kernel<<<(unsigned)ceil_div(n_pairs * 32, 256), 256, 0, s>>>(pf);
-        query_const_kernel<<<(unsigned)ceil_div(nq * 32, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq + 3 * ix->d : nullptr,
-                                                                            ix->metric == B200_METRIC_L2, ix->payload == IVF_PRODUCER_TMA, ix->w_qconst.as<float>());
-        g_launches += 2;
+        g_launches++;
+        if (ix->payload != IVF_PRODUCER_PQ) {   // PQ: the pair constant (||q - c||^2 or -<q, c>) is the whole query term
+            query_const_kernel<<<(unsigned)ceil_div(nq * 32, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq + 3 * ix->d : nullptr,
+                                                                                ix->metric == B200_METRIC_L2, ix->payload == IVF_PRODUCER_TMA, ix->w_qconst.as<float>());
+            g_launches++;
+        }
     }
     // ---- the grouped tensor-core scan
     B200_TRY(ix->w_pk.reserve((size_t)max_parts * k1 * 4));
@@ -2207,7 +2218,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     mg.sorted_list = ix->w_u32c.as<uint32_t>();
     mg.n_chunks = n_chunks;
     mg.pair_const = ix->w_pconst.as<float>();
-    mg.query_const = ix->binary ? nullptr : ix->w_qconst.as<float>();
+    mg.query_const = ix->binary || ix->payload == IVF_PRODUCER_PQ ? nullptr : ix->w_qconst.as<float>();
     mg.part_keys = gp.part_keys;
     mg.part_worst = gp.part_worst;
     mg.part_ids = gp.part_ids;

@@ -57,4 +57,8 @@ struct IvfGemmParams {
 cudaError_t launch_ivf_gemm_topk(const IvfGemmParams &p, const void *queries_bf16, int64_t n_query_rows, const void *pool_bf16,
                                  int64_t pool_rows, int grid, cudaStream_t s, const char **err_detail);
 
+// whether a PQ codebook of codebook_bytes (m * 256 * dsub bf16) fits in shared memory beside the smallest (2-stage) operand
+// ring of the decoding scan, by the launcher's own arithmetic: the scan of a wider codebook cannot be launched
+bool ivf_pq_codebook_fits(int64_t codebook_bytes);
+
 }  // namespace b200

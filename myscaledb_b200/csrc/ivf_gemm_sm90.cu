@@ -484,16 +484,23 @@ ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
     }
 }
 
+// Dynamic shared memory of the scan with `st` ring stages, k_smem per-thread list slots in shared memory and a PQ codebook
+// of codebook_bytes (0 for the other payloads), cooperative lists not counted: ring, accumulator staging, side arrays,
+// barriers, epilogue scratch, lists, codebook, the 1 KB alignment slack and 48 bytes of kernel-side slack.
+static int ivf_smem_need(int st, int k_smem, int codebook_bytes) {
+    return Layout<Operand::BF16>::off_list(st) + k_smem * EPI_THREADS * 8 + (int)round_up(codebook_bytes, 1024) + SMEM_ALIGN_SLACK + 48;
+}
+
 template <int PRODUCER, int DSUB>
 static cudaError_t launch_ivf(const CUtensorMap &map_q, const CUtensorMap &map_c, IvfGemmParams p, int grid, cudaStream_t s) {
     constexpr bool DEC = PRODUCER == IVF_PRODUCER_PQ || PRODUCER == IVF_PRODUCER_SQ8;
     // ring depth: as deep as the per-thread lists (and the PQ codebook) leave room for
-    const int extra = PRODUCER == IVF_PRODUCER_PQ ? (int)round_up(p.codebook_bytes, 1024) : 0;
+    const int codebook = PRODUCER == IVF_PRODUCER_PQ ? p.codebook_bytes : 0;
     // Shared-memory budget: operand ring (32 KB per stage) + accumulator staging + cooperative lists + per-thread lists.  Items with many queries
     // insert into per-thread lists ~k ln(rows / k) times per lane, and every insert rescans the list: k L2 round trips from
     // global scratch against k shared-memory loads -- so the per-thread lists get shared memory even at the price of
     // a 3-stage ring; only when they do not fit beside 3 stages do they move to global scratch (and the ring gets 4 stages).
-    auto need = [&](int st, int k_smem) { return Layout<Operand::BF16>::off_list(st) + k_smem * EPI_THREADS * 8 + extra + SMEM_ALIGN_SLACK; };
+    auto need = [&](int st, int k_smem) { return ivf_smem_need(st, k_smem, codebook); };
     const int coop_bytes = p.k <= 256 ? (int)round_up(coop_smem_bytes(p.k), 16) : 0;
     p.coop_enabled = coop_bytes > 0 && need(2, 0) + coop_bytes <= SMEM_LIMIT ? kCoopMax : 0;
     if (const char *ev = getenv("B200_IVF_COOP")) p.coop_enabled = std::min(p.coop_enabled, atoi(ev));   // A/B and debugging
@@ -516,7 +523,7 @@ static cudaError_t launch_ivf(const CUtensorMap &map_q, const CUtensorMap &map_c
     const int k_smem = p.lists_in_smem ? p.list_cap : 0;
     p.coop_smem_off = (int)round_up(Layout<Operand::BF16>::off_list(stages) + k_smem * EPI_THREADS * 8, 16);
     p.codebook_smem_off = (int)round_up(p.coop_smem_off + coop_used, 16);
-    const size_t smem = (size_t)need(stages, k_smem) + coop_used + 48;
+    const size_t smem = (size_t)need(stages, k_smem) + coop_used;
     auto kern = ivf_gemm_topk_kernel<PRODUCER, DSUB>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -526,6 +533,10 @@ static cudaError_t launch_ivf(const CUtensorMap &map_q, const CUtensorMap &map_c
 }
 
 }  // namespace gemm
+
+bool ivf_pq_codebook_fits(int64_t codebook_bytes) {
+    return codebook_bytes <= gemm::SMEM_LIMIT && gemm::ivf_smem_need(2, 0, (int)codebook_bytes) <= gemm::SMEM_LIMIT;
+}
 
 cudaError_t launch_ivf_gemm_topk(const IvfGemmParams &p, const void *queries_bf16, int64_t n_query_rows, const void *pool_bf16,
                                  int64_t pool_rows, int grid, cudaStream_t s, const char **err_detail) {

@@ -174,9 +174,14 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *   "FLAT"                      exact scan of the resident rows;
  *   "IVFFLAT"                   inverted lists holding bf16 rows, candidates re-ranked exactly against the fp32 rows;
  *   "IVFSQ"                     lists of 8-bit scalar-quantised rows (one byte per dimension);
- *   "IVFPQ"                     lists of m-byte product-quantiser codes of the residual (d / M in {1, 2, 4, 8}, d <= 220: the
- *                               scan keeps the 512 B x d bf16 codebook in shared memory; wider PQ indexes, SCANN and HNSWPQ
- *                               included, are refused at train with B200_ERR_UNSUPPORTED);
+ *   "IVFPQ"                     lists of m-byte product-quantiser codes of the residual (8-bit codes, 256 codewords per
+ *                               sub-quantiser; M must divide d).  Two list scans, chosen by d / M alone (no option, nothing
+ *                               stored): d / M in {1, 2, 4, 8} decodes codes into tensor-core tiles and keeps the 512 B x d bf16
+ *                               codebook in shared memory, so d <= 220 (wider ones, SCANN and HNSWPQ included, are refused at
+ *                               train with B200_ERR_UNSUPPORTED); any other d / M is scanned by table look-up (a per-query
+ *                               M x 256 fp32 table of <q_j, codeword>, at any width), which needs M <= 128 (larger M is refused
+ *                               at train).  Default M: d / 8 (or d / 4, d / 2, d) up to d = 220; above, d / dsub with dsub the
+ *                               smallest divisor of d that is >= 16 and keeps M <= 128 (M = 48 at d = 768, 96 at d = 1536);
  *   "MSTG"                      closed source upstream; here the two-stage index of SURVEY 2.5 K6: bf16 lists + exact
  *                               fp32 second stage (supportTwoStageSearch, first_stage_only, computeTopDistanceSubset);
  *   "SCANN", "HNSWFLAT", "HNSWSQ", "HNSWPQ"   accepted and SERVED BY THE INVERTED-FILE ENGINE with the payload their

@@ -102,6 +102,13 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
+// order-preserving float <-> u32 (atomicMin on the encoding = min of the floats): the shared per-query bound of the IVF scans
+__device__ __forceinline__ uint32_t bound_encode(float f) {
+    const uint32_t b = __float_as_uint(f);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float bound_decode(uint32_t u) { return (u & 0x80000000u) ? __uint_as_float(u & 0x7fffffffu) : __uint_as_float(~u); }
+
 // named barrier of the consumer warpgroup (id 1; 0 is __syncthreads)
 __device__ __forceinline__ void wg_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 

@@ -287,7 +287,7 @@ struct ScatterParams {
     // PQ payload
     const float *centroids;     // [nlist][d]
     const float *pq;            // [m][256][dsub] fp32 (nearest-centroid search)
-    const __nv_bfloat16 *pq_bf16;  // values the scan kernel will see
+    const __nv_bfloat16 *pq_bf16;  // values the scan kernel will see (null: the fp32 ones, table look-up scan)
     int m, dsub;
     uint8_t *codes;
     int code_bytes;
@@ -361,10 +361,11 @@ __global__ void __launch_bounds__(256) scatter_rows_kernel(const ScatterParams p
                             best = (uint32_t)e;
                         }
                     }
-                    // norm term of the expanded L2 with the bf16 codebook values the scan sees: 2 <c, r^> + ||r^||^2
-                    const __nv_bfloat16 *rb = p.pq_bf16 + ((size_t)j * 256 + best) * p.dsub;
+                    // norm term of the expanded L2 with the codebook values the scan sees: 2 <c, r^> + ||r^||^2 (bf16 for the
+                    // tensor-core decoder, fp32 for the table look-up scan, which has no bf16 codebook)
+                    const size_t cw = ((size_t)j * 256 + best) * p.dsub;
                     for (int t = 0; t < p.dsub; t++) {
-                        const float rv = __bfloat162float(rb[t]);
+                        const float rv = p.pq_bf16 ? __bfloat162float(p.pq_bf16[cw + t]) : p.pq[cw + t];
                         acc = fmaf(rv, rv + 2.f * c[j * p.dsub + t], acc);
                     }
                 }
@@ -696,7 +697,7 @@ struct PairFill {
     const float *queries;        // [nq][d_pad] fp32, prepared (cosine: unit length)
     const float *sq_step;        // SQ8: per-dimension step (null otherwise)
     const float *centroids;      // PQ: [nlist][d] (null otherwise)
-    __nv_bfloat16 *qbuf;         // [n_pairs][d_pad64]
+    __nv_bfloat16 *qbuf;         // [n_pairs][d_pad64] (null: no gathered rows, the table look-up scan reads its own table)
     uint32_t *inv;               // [n_pairs] original pair -> sorted position
     uint32_t *pair_part_base;    // [n_pairs]
     float *pair_const;           // [n_pairs]
@@ -724,7 +725,7 @@ __global__ void __launch_bounds__(256) pair_fill_kernel(const PairFill p) {
     }
     const uint32_t q = pr / (uint32_t)p.nprobe;
     const float *x = p.queries + (size_t)q * p.d_pad;
-    __nv_bfloat16 *dst = p.qbuf + (size_t)i * p.d_pad64;
+    __nv_bfloat16 *dst = p.qbuf ? p.qbuf + (size_t)i * p.d_pad64 : nullptr;
     const float *c = p.centroids ? p.centroids + (size_t)l * p.d : nullptr;
     float acc = 0.f;
     for (int j = lane; j < p.d_pad64; j += 32) {
@@ -734,7 +735,7 @@ __global__ void __launch_bounds__(256) pair_fill_kernel(const PairFill p) {
             acc = p.l2 ? fmaf(v - cv, v - cv, acc) : fmaf(-v, cv, acc);
         }
         if (p.sq_step && j < p.d) v *= p.sq_step[j];
-        dst[j] = __float2bfloat16_rn(v);
+        if (dst) dst[j] = __float2bfloat16_rn(v);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -1037,7 +1038,7 @@ struct b200_index {
     std::mutex mu;
     // workspaces (grow-only)
     DevArr w_rows, w_assign_i, w_assign_d, w_u32a, w_u32b, w_u32c, w_u32d, w_cnt, w_plan, w_sort, w_q, w_qraw, w_probe, w_pd, w_items,
-        w_qbuf, w_inv, w_ppb, w_pconst, w_qconst, w_qb, w_cs, w_pk, w_pi, w_pw, w_lk, w_li, w_alive, w_od, w_oi, w_cand, w_host_q, w_ppopc;
+        w_qbuf, w_inv, w_ppb, w_pconst, w_qconst, w_qb, w_cs, w_pk, w_pi, w_pw, w_lk, w_li, w_alive, w_od, w_oi, w_cand, w_host_q, w_ppopc, w_lut;
     // statistics of the last search (tests, bench roofline): rows x payload bytes the scan kernel was asked to stream
     int64_t last_scan_rows = 0, last_items = 0;
     bool timing = false, timed_pending = false;
@@ -1154,7 +1155,7 @@ extern "C" int b200_index_free(b200_index *ix) {
     for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_cnt, &ix->w_plan,
                       &ix->w_sort, &ix->w_q, &ix->w_qraw, &ix->w_probe, &ix->w_pd, &ix->w_items, &ix->w_qbuf, &ix->w_inv, &ix->w_ppb, &ix->w_pconst, &ix->w_qb, &ix->w_cs,
                       &ix->w_qconst, &ix->w_pk, &ix->w_pi, &ix->w_pw, &ix->w_lk, &ix->w_li, &ix->w_alive, &ix->w_od, &ix->w_oi, &ix->w_cand,
-                      &ix->w_host_q, &ix->w_ppopc})
+                      &ix->w_host_q, &ix->w_ppopc, &ix->w_lut})
         a->release();
     if (ix->ev0) cudaEventDestroy(ix->ev0);
     if (ix->ev1) cudaEventDestroy(ix->ev1);
@@ -1164,6 +1165,13 @@ extern "C" int b200_index_free(b200_index *ix) {
     delete ix;
     return B200_OK;
 }
+
+// PQ sub-vectors the tensor-core decoder takes (d / M = 1, 2, 4, 8); any other d / M is scanned by table look-up
+static bool pq_dsub_decodable(int dsub) { return dsub == 1 || dsub == 2 || dsub == 4 || dsub == 8; }
+static bool pq_uses_lut(const b200_index *ix) { return ix->payload == IVF_PRODUCER_PQ && ix->use_ivf && !pq_dsub_decodable(ix->dsub); }
+
+// the per-query tables of the look-up scan take at most this much scratch; larger batches run in query sub-batches
+constexpr int64_t kPqLutScratchBytes = (int64_t)256 << 20;
 
 static size_t payload_row_bytes(const b200_index *ix) {
     if (ix->payload == IVF_PRODUCER_B1) return (size_t)ix->row_pad;
@@ -1457,20 +1465,33 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
         return B200_OK;
     }
     if (ix->payload == IVF_PRODUCER_PQ) {
-        if (ix->m <= 0) {  // default: sub-vectors of <= 8 dims
-            ix->m = d;
-            for (int cand : {8, 4, 2, 1})
-                if (d % cand == 0) { ix->m = d / cand; break; }
+        if (ix->m <= 0) {
+            if (d <= 220) {   // sub-vectors of <= 8 dims, decoded on the tensor cores
+                ix->m = d;
+                for (int cand : {8, 4, 2, 1})
+                    if (d % cand == 0) { ix->m = d / cand; break; }
+            } else {          // table look-up: the smallest sub-vector of >= 16 dims that divides d and keeps M <= 128
+                int dsub = 16;
+                while (d % dsub || d / dsub > 128) dsub++;
+                ix->m = d / dsub;
+            }
         }
         if (d % ix->m) return fail(B200_ERR_INVALID, "PQ M must divide the dimension");
         const int dsub = d / ix->m;
-        if (dsub != 1 && dsub != 2 && dsub != 4 && dsub != 8)
-            return fail(B200_ERR_UNSUPPORTED, "PQ sub-vector length d / M must be 1, 2, 4 or 8 (codes are decoded into tensor-core tiles)");
-        // the scan keeps the bf16 codebook (512 B x d) in shared memory beside at least a 2-stage operand ring
-        if (!ivf_pq_codebook_fits((int64_t)512 * d)) {
-            int dmax = d;
-            while (dmax > 1 && !ivf_pq_codebook_fits((int64_t)512 * dmax)) dmax--;
-            return fail(B200_ERR_UNSUPPORTED, "PQ codebook (512 B x d) must fit in shared memory next to the operand ring: d <= " + std::to_string(dmax));
+        if (pq_dsub_decodable(dsub)) {
+            // the tensor-core scan keeps the bf16 codebook (512 B x d) in shared memory beside at least a 2-stage operand ring
+            if (!ivf_pq_codebook_fits((int64_t)512 * d)) {
+                int dmax = d;
+                while (dmax > 1 && !ivf_pq_codebook_fits((int64_t)512 * dmax)) dmax--;
+                return fail(B200_ERR_UNSUPPORTED, "PQ codebook (512 B x d) must fit in shared memory next to the operand ring: d <= " + std::to_string(dmax) +
+                                                      " (or choose M with d / M >= 16, scanned by table look-up)");
+            }
+        } else if (!ivf_pq_lut_fits(ix->m)) {
+            // the table look-up scan keeps one query's M x 256 fp32 table in shared memory
+            int mmax = ix->m;
+            while (mmax > 1 && !ivf_pq_lut_fits(mmax)) mmax--;
+            return fail(B200_ERR_UNSUPPORTED, "PQ with d / M outside {1, 2, 4, 8} is scanned by table look-up, whose per-query table (M x 1 KB) "
+                                              "must fit in shared memory: M <= " + std::to_string(mmax) + ", got M = " + std::to_string(ix->m));
         }
     }
     if (ix->keep_raw < 0) ix->keep_raw = 1;
@@ -1509,7 +1530,7 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
         ix->dsub = dsub;
         ix->code_bytes = (int)round_up(m, 16);
         B200_CUDA_OK(cudaMalloc(&ix->d_pq, (size_t)m * 256 * dsub * 4));
-        B200_CUDA_OK(cudaMalloc(&ix->d_pq_bf16, (size_t)m * 256 * dsub * 2));
+        if (pq_dsub_decodable(dsub)) B200_CUDA_OK(cudaMalloc(&ix->d_pq_bf16, (size_t)m * 256 * dsub * 2));   // the decoder's copy
         // residuals of (a sample of) the training rows, one sub-quantiser at a time
         const int64_t ns = std::min<int64_t>(n, 65536);
         int64_t *d_a = nullptr;
@@ -1536,7 +1557,7 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
                 rc = kmeans_device(d_res, ns, dsub, dsub, 256, 8, ix->d_pq + (size_t)j * 256 * dsub, s);
             }
         }
-        if (rc == B200_OK) {
+        if (rc == B200_OK && ix->d_pq_bf16) {
             cudaError_t e = launch_f32_to_bf16_rows(ix->d_pq, dsub, ix->d_pq_bf16, dsub, (int64_t)m * 256, s);
             if (e != cudaSuccess) rc = fail(B200_ERR_CUDA, cudaGetErrorString(e));
         }
@@ -1824,7 +1845,7 @@ extern "C" int b200_index_memory_bytes(const b200_index *ix, uint64_t *out_bytes
         const uint64_t rows = (uint64_t)ix->pool_pages * kPageRows;
         b += (uint64_t)ix->nlist * (ix->binary ? (uint64_t)ix->cent_pad : (uint64_t)ix->d * 4) + rows * (payload_row_bytes(ix) + 4 + (ix->d_row_bias ? 4 : 0)) +
              (uint64_t)ix->pool_pages * 12;
-        if (ix->d_pq) b += (uint64_t)ix->m * 256 * ix->dsub * 6;
+        if (ix->d_pq) b += (uint64_t)ix->m * 256 * ix->dsub * (ix->d_pq_bf16 ? 6 : 4);   // fp32 codebook (+ the decoder's bf16 copy)
     }
     *out_bytes = b;
     return B200_OK;
@@ -1939,6 +1960,17 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     if (out_num_candidates) *out_num_candidates = k;
     if (nq == 0) return B200_OK;
     const int force_exact = parse_int_param(params, "exact_batch", 0);
+    if (pq_uses_lut(ix) && force_exact != 1 && k <= 1024) {
+        // the look-up scan's tables are nq x M KB: a larger batch runs as consecutive query sub-batches through the whole
+        // search (every query's answer depends on that query alone, so the results are those of one batch)
+        const int64_t qmax = std::max<int64_t>(1, kPqLutScratchBytes / ((int64_t)ix->m * 1024));
+        if (nq > qmax) {
+            for (int64_t q0 = 0; q0 < nq; q0 += qmax)
+                B200_TRY(search_device_locked(ix, d_queries + q0 * ix->d, std::min(qmax, nq - q0), k, params, first_stage_only, d_alive, id_offset,
+                                              d_out_dis + q0 * k, d_out_ids + q0 * k, out_num_candidates, s));
+            return B200_OK;
+        }
+    }
     if (ix->binary) {
         // binary queries are bytes [nq][d / 8]; list rows are exact, so refine_factor / keep_raw / first_stage_only change nothing
         if (force_exact == 1) return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available on binary indexes (their lists are exact)");
@@ -2093,10 +2125,13 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     search_plan_kernel<<<1, 1024, 0, s>>>(pl);
     g_launches++;
     // ---- gather queries, per-pair bookkeeping
+    const bool lut = pq_uses_lut(ix);
     const size_t qrow_bytes = ix->binary ? (size_t)ix->row_pad : (size_t)ix->d_pad64 * 2;
-    B200_TRY(ix->w_qbuf.reserve(((size_t)n_pairs + 128) * qrow_bytes));
-    // the 128 rows behind the last pair are read by the last items' A tiles (query slots without a query): keep them finite
-    B200_CUDA_OK(cudaMemsetAsync(ix->w_qbuf.as<char>() + (size_t)n_pairs * qrow_bytes, 0, (size_t)128 * qrow_bytes, s));
+    if (!lut) {   // the table look-up scan reads no gathered query rows
+        B200_TRY(ix->w_qbuf.reserve(((size_t)n_pairs + 128) * qrow_bytes));
+        // the 128 rows behind the last pair are read by the last items' A tiles (query slots without a query): keep them finite
+        B200_CUDA_OK(cudaMemsetAsync(ix->w_qbuf.as<char>() + (size_t)n_pairs * qrow_bytes, 0, (size_t)128 * qrow_bytes, s));
+    }
     B200_TRY(ix->w_inv.reserve((size_t)n_pairs * 4));
     B200_TRY(ix->w_ppb.reserve((size_t)n_pairs * 4));
     B200_TRY(ix->w_pconst.reserve((size_t)n_pairs * 4));
@@ -2110,7 +2145,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     pf.queries = d_q;
     pf.sq_step = ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq + ix->d : nullptr;
     pf.centroids = ix->payload == IVF_PRODUCER_PQ ? ix->d_centroids : nullptr;
-    pf.qbuf = ix->w_qbuf.as<__nv_bfloat16>();
+    pf.qbuf = lut ? nullptr : ix->w_qbuf.as<__nv_bfloat16>();
     pf.inv = ix->w_inv.as<uint32_t>();
     pf.pair_part_base = ix->w_ppb.as<uint32_t>();
     pf.pair_const = ix->w_pconst.as<float>();
@@ -2134,6 +2169,10 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     } else {
         pair_fill_kernel<<<(unsigned)ceil_div(n_pairs * 32, 256), 256, 0, s>>>(pf);
         g_launches++;
+        if (lut) {   // the per-query tables T[q][j][e] = <q_j, codebook_j[e]> (fp32)
+            B200_TRY(ix->w_lut.reserve((size_t)nq * ix->m * 1024));
+            B200_CUDA_OK(launch_pq_lut(d_q, nq, ix->d_pad, ix->d_pq, ix->m, ix->dsub, ix->w_lut.as<float>(), s));
+        }
         if (ix->payload != IVF_PRODUCER_PQ) {   // PQ: the pair constant (||q - c||^2 or -<q, c>) is the whole query term
             query_const_kernel<<<(unsigned)ceil_div(nq * 32, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq + 3 * ix->d : nullptr,
                                                                                 ix->metric == B200_METRIC_L2, ix->payload == IVF_PRODUCER_TMA, ix->w_qconst.as<float>());
@@ -2184,7 +2223,11 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     gp.m = ix->m;
     gp.dsub = ix->dsub;
     gp.codebook_bytes = ix->payload == IVF_PRODUCER_PQ ? ix->m * 256 * ix->dsub * 2 : 0;
-    if (k1 > kGemmSmemK || true) {  // global scratch for lists that do not fit in shared memory (the launcher decides)
+    if (lut) {   // the look-up scan finds its table through the pair's query
+        gp.lut = ix->w_lut.as<float>();
+        gp.sorted_pair = ix->w_u32d.as<uint32_t>();
+        gp.nprobe = nprobe;
+    } else {  // global scratch for lists that do not fit in shared memory (the launcher decides)
         B200_TRY(ix->w_lk.reserve((size_t)grid * 128 * list_cap_for(k1) * 4));
         B200_TRY(ix->w_li.reserve((size_t)grid * 128 * list_cap_for(k1) * 4));
         gp.list_keys_gmem = ix->w_lk.as<float>();
@@ -2195,13 +2238,15 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         cudaEventRecord(ix->ev_ph[2], s);
         cudaEventRecord(ix->ev0, s);
     }
-    cudaError_t e = launch_ivf_gemm_topk(gp, ix->w_qbuf.p, n_pairs + 128, ix->d_pool, (int64_t)ix->pool_pages * kPageRows, grid, s, &detail);
+    cudaError_t e = lut ? launch_ivf_pq_lut_topk(gp, grid, s, &detail)
+                        : launch_ivf_gemm_topk(gp, ix->w_qbuf.p, n_pairs + 128, ix->d_pool, (int64_t)ix->pool_pages * kPageRows, grid, s, &detail);
     if (ix->timing) {
         cudaEventRecord(ix->ev1, s);
         cudaEventRecord(ix->ev_ph[3], s);
         ix->timed_pending = true;
     }
-    if (e != cudaSuccess) return fail(B200_ERR_CUDA, std::string("ivf_gemm_topk launch: ") + (detail ? detail : cudaGetErrorString(e)));
+    if (e != cudaSuccess)
+        return fail(B200_ERR_CUDA, std::string(lut ? "ivf_pq_lut_topk launch: " : "ivf_gemm_topk launch: ") + (detail ? detail : cudaGetErrorString(e)));
     ix->last_items = max_items;
     // ---- per-query merge of the partial lists
     float *m_dis = d_out_dis;
@@ -2509,9 +2554,13 @@ static int index_load_io(Io *f, b200_index **out) {
             if (total != (uint64_t)h.n || pages != h.pages_used) return bail("corrupt index file (list lengths do not add up)");
             if (h.payload == IVF_PRODUCER_PQ) {
                 if (!slurp((void **)&ix->d_pq, (size_t)h.m * 256 * h.dsub * 4)) return bail("truncated index file (codebook)");
-                if (cudaMalloc(&ix->d_pq_bf16, (size_t)h.m * 256 * h.dsub * 2) != cudaSuccess) return bail("cudaMalloc failed");
-                if (launch_f32_to_bf16_rows(ix->d_pq, h.dsub, ix->d_pq_bf16, h.dsub, (int64_t)h.m * 256, ix->stream) != cudaSuccess)
-                    return bail("codebook conversion failed");
+                if (pq_dsub_decodable(h.dsub)) {   // the tensor-core decoder's bf16 copy; the table look-up scan reads the fp32 codebook
+                    if (cudaMalloc(&ix->d_pq_bf16, (size_t)h.m * 256 * h.dsub * 2) != cudaSuccess) return bail("cudaMalloc failed");
+                    if (launch_f32_to_bf16_rows(ix->d_pq, h.dsub, ix->d_pq_bf16, h.dsub, (int64_t)h.m * 256, ix->stream) != cudaSuccess)
+                        return bail("codebook conversion failed");
+                } else if (!ivf_pq_lut_fits(h.m)) {
+                    return bail("corrupt index header (PQ M too large for the table look-up scan)");
+                }
             }
             if (h.payload == IVF_PRODUCER_SQ8 && !slurp((void **)&ix->d_sq, (size_t)4 * h.d * 4)) return bail("truncated index file (SQ ranges)");
             ix->pool_pages = ix->pages_used = h.pages_used;

@@ -41,6 +41,7 @@ struct IvfGemmParams {
     const uint8_t *codes;             // [pool rows][code_bytes]
     const void *codebook_bf16;        // PQ: [m][256][dsub] bf16
     int code_bytes, m, dsub, codebook_bytes;
+    const float *lut;                 // PQ table look-up scan: [nq][m][256] fp32, <q_j, codebook_j[e]> (needs sorted_pair, nprobe)
     // filled in by the launcher
     // Per-query bound shared by all the work items of a launch (nprobe > 1): query_bound[q] is the smallest k-th key
     // (order-preserving u32 encoding, 0xffffffff = none yet) any FULL partial list of query q has published, in absolute key space
@@ -60,5 +61,15 @@ cudaError_t launch_ivf_gemm_topk(const IvfGemmParams &p, const void *queries_bf1
 // whether a PQ codebook of codebook_bytes (m * 256 * dsub bf16) fits in shared memory beside the smallest (2-stage) operand
 // ring of the decoding scan, by the launcher's own arithmetic: the scan of a wider codebook cannot be launched
 bool ivf_pq_codebook_fits(int64_t codebook_bytes);
+
+// PQ with d / M outside {1, 2, 4, 8} (ivf_pq_lut_sm90.cu): the same work items and partial lists, scanned by table look-up.
+// launch_pq_lut fills lut_out [nq][m][256] = <q_j, codebook_j[e]> (fp32) from prepared queries [nq][d_pad] and the fp32 codebook
+// [m][256][dsub]; launch_ivf_pq_lut_topk scans with p.lut = that table (p.stages is set by the launcher: table buffers)
+cudaError_t launch_pq_lut(const float *queries, int64_t nq, int d_pad, const float *codebook, int m, int dsub, float *lut_out, cudaStream_t s);
+cudaError_t launch_ivf_pq_lut_topk(const IvfGemmParams &p, int grid, cudaStream_t s, const char **err_detail);
+
+// whether the look-up scan takes m sub-quantisers: M <= 128, and one M x 1 KB table beside the k = 1024 lists and the candidate
+// buffer in shared memory, by the launcher's own arithmetic
+bool ivf_pq_lut_fits(int m);
 
 }  // namespace b200

@@ -40,12 +40,6 @@ constexpr int IVF_DEC_WARPS = 4;               // extra decoder warps of the cod
 constexpr int IVF_THREADS_DEC = IVF_THREADS_TMA + IVF_DEC_WARPS * 32;
 
 // smem: the Layout<Operand::BF16> of gemm_common.cuh.  Code payloads add a codebook region behind the lists.
-// order-preserving float <-> u32 (atomicMin on the encoding = min of the floats)
-__device__ __forceinline__ uint32_t bound_encode(float f) {
-    const uint32_t b = __float_as_uint(f);
-    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float bound_decode(uint32_t u) { return (u & 0x80000000u) ? __uint_as_float(u & 0x7fffffffu) : __uint_as_float(~u); }
 
 template <int PRODUCER, int DSUB>
 __global__ void __launch_bounds__(PRODUCER == IVF_PRODUCER_PQ || PRODUCER == IVF_PRODUCER_SQ8 ? IVF_THREADS_DEC : IVF_THREADS_TMA, 1)

@@ -2,7 +2,7 @@
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
 workload; results are pasted into DESIGN.md section 7.
-Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf]"""
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide]"""
 import json
 import os
 import subprocess
@@ -297,8 +297,58 @@ def bench_binary_ivf():
         print(json.dumps(out), flush=True)
 
 
+def bench_pq_wide():
+    """PQ on wide vectors: 2 M clustered 768-d rows (10 000 centres), k = 10.  SCANN (default M = 48, d / M = 16: the table
+    look-up scan, refine 16), IVFPQ (M = 48, first stage only), MSTG (bf16 lists + exact refine) and FLAT, over nq x nprobe.
+    Per point: recall@10 against FLAT, the median call time, the list-scan kernel time (last_scan), the rows the scan
+    streamed, table look-ups per second (rows streamed x M / kernel time) and the list bytes per row of each index."""
+    n, d, k, nlist = 2_000_000, 768, 10, 4096
+    y, qs = clustered(n, d, 10_000, seed=768, nq=1024)
+    ctx = gpu_context()
+    flat = b2.Corpus(b2.L2, d).append(y)
+    idx = {}
+    for name, typ, params in (("SCANN", "SCANN", f"ncentroids={nlist}"), ("IVFPQ", "IVFPQ", f"ncentroids={nlist}, M=48, keep_raw=0"),
+                              ("MSTG", "MSTG", f"ncentroids={nlist}")):
+        t0 = time.perf_counter()
+        idx[name] = b2.VectorIndex(typ, b2.L2, d, params).build(y)
+        idx[name].enable_timing(True)
+        print(json.dumps({"build": name, "m": idx[name].info()["m"], "build_s": round(time.perf_counter() - t0, 1)}), flush=True)
+    del y
+
+    def median_call(fn, reps):
+        fn()
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            out = fn()
+            ts.append(time.perf_counter() - t0)
+        return float(np.median(ts)), out
+
+    for nq in (1, 16, 256, 1024):
+        q = qs[:nq]
+        reps = 20 if nq <= 16 else 7
+        t_flat, (_, truth) = median_call(lambda: flat.search(q, k), reps)
+        for nprobe in (1, 4, 16, 64):
+            pt = dict(workload=f"pq_wide {n} x {d} clustered, nlist={nlist}, k={k}", nq=nq, nprobe=nprobe, **ctx,
+                      FLAT=dict(call_ms=round(t_flat * 1e3, 3)))
+            for name, ix in idx.items():
+                prm = f"nprobe={nprobe}"
+                fso = name == "IVFPQ"
+                ix.last_scan(reset=True)
+                t, (_, ids) = median_call(lambda: ix.search(q, k, prm, first_stage_only=fso), reps)
+                ls = ix.last_scan(reset=True)
+                kern_ms = ls["kernel_ms"] / max(1, ls["launches"])
+                m = ix.info()["m"]
+                e = dict(recall=round(recall(ids, truth), 4), call_ms=round(t * 1e3, 3), scan_kernel_ms=round(kern_ms, 4),
+                         rows_streamed=ls["rows_streamed"], list_bytes_per_row=ls["payload_row_bytes"])
+                if name != "MSTG" and kern_ms > 0:
+                    e["lookups_per_s"] = float(f"{ls['rows_streamed'] * m / (kern_ms * 1e-3):.4g}")
+                pt[name] = e
+            print(json.dumps(pt), flush=True)
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
         {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
-         "binary": bench_binary, "binary_ivf": bench_binary_ivf}[w]()
+         "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide}[w]()

@@ -171,6 +171,7 @@ struct Bm25ScoreParams {
     float *part_keys;          // [nq][gridDim.x][k]
     uint32_t *part_ids;
     uint32_t n_docs;
+    uint32_t q_begin;          // query of blockIdx.y == 0: a batch launches in slices of at most 65535 queries (gridDim.y)
     int k;
     int operator_or;
 };
@@ -216,7 +217,7 @@ __global__ void __launch_bounds__(256) bm25_score_kernel(const Bm25ScoreParams p
     uint32_t *li = reinterpret_cast<uint32_t *>(lk + 8 * p.k);
     __shared__ Clause cl[kMaxClauses];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t q = blockIdx.y;
+    const uint32_t q = p.q_begin + blockIdx.y;
     const uint32_t c0 = p.clause_begin[q], nc = p.clause_begin[q + 1] - c0;
     for (uint32_t i = threadIdx.x; i < nc; i += blockDim.x) cl[i] = p.clauses[c0 + i];
     WarpTopK list;
@@ -356,7 +357,7 @@ __global__ void __launch_bounds__(256) bm25_daat_kernel(const Bm25DaatParams dp)
     unsigned long long *t_mask = reinterpret_cast<unsigned long long *>(t_score + kDaatSlots);
     unsigned short *t_occ = reinterpret_cast<unsigned short *>(t_mask + kDaatSlots);   // slots claimed in the current range
     __shared__ uint32_t n_occ_s[8];
-    const uint32_t q = blockIdx.y;
+    const uint32_t q = p.q_begin + blockIdx.y;
     const uint32_t c0 = p.clause_begin[q], nc = p.clause_begin[q + 1] - c0;
     for (uint32_t i = threadIdx.x; i < nc; i += blockDim.x) cl[i] = p.clauses[c0 + i];
     WarpTopK list;
@@ -821,10 +822,14 @@ extern "C" int b200_bm25_search_batch(b200_bm25 *ix, const char *const *sentence
     for (auto &c : clauses) ix->last_postings += c.df;
     cudaEventRecord(ix->ev0, s);
     static const int use_taat = getenv("B200_BM25_TAAT") ? atoi(getenv("B200_BM25_TAAT")) : 0;   // A/B: the round-1 kernel
+    constexpr int64_t kMaxGridY = 65535;   // queries ride on gridDim.y: larger batches launch slice after slice
     if (use_taat) {
         const size_t smem = (size_t)8 * k * 8;
         B200_CUDA_OK(cudaFuncSetAttribute(bm25_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        bm25_score_kernel<<<dim3(bx, (unsigned)nq), 256, smem, s>>>(sp);
+        for (int64_t q0 = 0; q0 < nq; q0 += kMaxGridY) {
+            sp.q_begin = (uint32_t)q0;
+            bm25_score_kernel<<<dim3(bx, (unsigned)std::min(nq - q0, kMaxGridY)), 256, smem, s>>>(sp);
+        }
     } else {
         // range width per query: ~kDaatTarget postings of all its clauses per range
         std::vector<uint32_t> range_log2(nq, 8);
@@ -843,7 +848,10 @@ extern "C" int b200_bm25_search_batch(b200_bm25 *ix, const char *const *sentence
         dpp.range_log2 = reinterpret_cast<const uint32_t *>(ix->d_ranges.p);
         const size_t smem = (size_t)8 * k * 8 + 16 + (size_t)8 * kDaatWarpBytes;
         B200_CUDA_OK(cudaFuncSetAttribute(bm25_daat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        bm25_daat_kernel<<<dim3(bx, (unsigned)nq), 256, smem, s>>>(dpp);
+        for (int64_t q0 = 0; q0 < nq; q0 += kMaxGridY) {
+            dpp.base.q_begin = (uint32_t)q0;
+            bm25_daat_kernel<<<dim3(bx, (unsigned)std::min(nq - q0, kMaxGridY)), 256, smem, s>>>(dpp);
+        }
     }
     cudaEventRecord(ix->ev1, s);
     g_launches++;

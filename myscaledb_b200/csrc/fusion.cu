@@ -72,48 +72,38 @@ __global__ void __launch_bounds__(128) hybrid_fusion_kernel(const FusionParams p
     const uint64_t *tp = p.t_part + q * p.t_stride, *tl = p.t_label + q * p.t_stride;
     const float *vsc = p.v_score + q * p.v_stride, *tsc = p.t_score + q * p.t_stride;
 
-    // vector entries first (duplicates inside one list are merged like map[key] +=)
+    // The entries are built in the reference's map order, so duplicate keys inside one list sum exactly as it does:
+    // RankFusion adds the vector ranks, then the text ranks; RelativeScoreFusion ASSIGNS the text parts (a text key listed
+    // twice keeps its last part), then ADDS the vector parts one by one.
     if (threadIdx.x == 0) {
         uint32_t n = 0;
-        for (uint32_t i = 0; i < nv; i++) {
-            float add;
-            if (p.fusion_type == 1) add = __fdiv_rn(1.0f, (float)(p.fusion_k + i + 1));
-            else {
+        auto at = [&](uint32_t s, uint64_t pa, uint64_t l) -> FEntry & {   // map[key]: new keys start at 0
+            uint32_t j = 0;
+            for (; j < n; j++)
+                if (key_eq(e[j], s, pa, l)) return e[j];
+            e[n].shard = s;
+            e[n].part = pa;
+            e[n].label = l;
+            e[n].score = 0.f;
+            return e[n++];
+        };
+        if (p.fusion_type == 1) {
+            for (uint32_t i = 0; i < nv; i++) {
+                FEntry &x = at(vs[i], vp[i], vl[i]);
+                x.score = __fadd_rn(x.score, __fdiv_rn(1.0f, (float)(p.fusion_k + i + 1)));
+            }
+            for (uint32_t i = 0; i < nt; i++) {
+                FEntry &x = at(ts[i], tp[i], tl[i]);
+                x.score = __fadd_rn(x.score, __fdiv_rn(1.0f, (float)(p.fusion_k + i + 1)));
+            }
+        } else {
+            for (uint32_t i = 0; i < nt; i++)
+                at(ts[i], tp[i], tl[i]).score = __fmul_rn(norm_score(tsc[i], tsc[0], tsc[nt - 1]), p.weight);
+            const float w1 = __fsub_rn(1.0f, p.weight);
+            for (uint32_t i = 0; i < nv; i++) {
                 const float ns = norm_score(vsc[i], vsc[0], vsc[nv - 1]);
-                const float w1 = __fsub_rn(1.0f, p.weight);
-                add = p.direction == -1 ? __fmul_rn(ns, w1) : __fmul_rn(__fsub_rn(1.0f, ns), w1);
-            }
-            uint32_t j = 0;
-            for (; j < n; j++)
-                if (key_eq(e[j], vs[i], vp[i], vl[i])) break;
-            if (j == n) {
-                e[n].shard = vs[i];
-                e[n].part = vp[i];
-                e[n].label = vl[i];
-                e[n].score = 0.f;
-                n++;
-            }
-            e[j].score = __fadd_rn(e[j].score, add);
-        }
-        const uint32_t n_vec = n;
-        for (uint32_t i = 0; i < nt; i++) {
-            uint32_t j = 0;
-            for (; j < n; j++)
-                if (key_eq(e[j], ts[i], tp[i], tl[i])) break;
-            if (j == n) {
-                e[n].shard = ts[i];
-                e[n].part = tp[i];
-                e[n].label = tl[i];
-                e[n].score = 0.f;
-                n++;
-            }
-            if (p.fusion_type == 1) {
-                e[j].score = __fadd_rn(e[j].score, __fdiv_rn(1.0f, (float)(p.fusion_k + i + 1)));
-            } else {
-                // RelativeScoreFusion assigns the text part first, then ADDS the vector part; with two
-                // addends the order does not change the fp32 sum
-                const float tpart = __fmul_rn(norm_score(tsc[i], tsc[0], tsc[nt - 1]), p.weight);
-                e[j].score = j < n_vec ? __fadd_rn(tpart, e[j].score) : tpart;
+                FEntry &x = at(vs[i], vp[i], vl[i]);
+                x.score = __fadd_rn(x.score, p.direction == -1 ? __fmul_rn(ns, w1) : __fmul_rn(__fsub_rn(1.0f, ns), w1));
             }
         }
         n_entries = n;
@@ -221,10 +211,15 @@ extern "C" int b200_hybrid_fusion_batch(int fusion_type, int64_t nq, const uint3
         p.o_shard = (uint32_t *)(d + o_os); p.o_part = (uint64_t *)(d + o_op); p.o_label = (uint64_t *)(d + o_ol);
         p.o_score = (float *)(d + o_osc); p.o_count = (uint32_t *)(d + o_oc);
         const size_t smem = (size_t)(vec_stride + txt_stride + 1) * sizeof(FEntry);
-        cudaFuncSetAttribute(hybrid_fusion_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        hybrid_fusion_kernel<<<(unsigned)nq, 128, smem, s>>>(p);
-        g_launches++;
-        if (cudaGetLastError() != cudaSuccess) rc = fail(B200_ERR_CUDA, "fusion kernel launch failed");
+        // 2048 candidates take 64 KB, above the 48 KB a kernel gets without opting in
+        if (cudaFuncSetAttribute(hybrid_fusion_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+            cudaGetLastError();
+            rc = fail(B200_ERR_CUDA, "cannot grant the fusion kernel its shared memory");
+        } else {
+            hybrid_fusion_kernel<<<(unsigned)nq, 128, smem, s>>>(p);
+            g_launches++;
+            if (cudaGetLastError() != cudaSuccess) rc = fail(B200_ERR_CUDA, "fusion kernel launch failed");
+        }
     }
     // outputs: one copy back into the mirror, then scattered to the caller's arrays
     if (rc == B200_OK && cudaMemcpyAsync(sc.h + o_os, d + o_os, off - o_os, cudaMemcpyDeviceToHost, s) != cudaSuccess)

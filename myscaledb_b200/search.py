@@ -257,10 +257,14 @@ class BM25Index:
     @staticmethod
     def query_terms(sentence):
         tls = BM25Index._qt_tls
-        if not hasattr(tls, "buf"):
-            tls.buf = (C.create_string_buffer(4096), C.c_uint32())
+        raw = sentence.encode()
+        # every distinct term is written, NUL-terminated; a term is at most 3x the bytes it came from (an invalid byte
+        # decodes to U+FFFD), so 4 bytes per input byte always suffice
+        need = max(4096, 4 * len(raw) + 16)
+        if getattr(tls, "cap", 0) < need:
+            tls.buf, tls.cap = (C.create_string_buffer(need), C.c_uint32()), need
         buf, n = tls.buf
-        _check(lib().b200_bm25_query_terms(sentence.encode(), buf, C.c_size_t(4096), C.byref(n)))
+        _check(lib().b200_bm25_query_terms(raw, buf, C.c_size_t(tls.cap), C.byref(n)))
         out, off = [], 0
         base = C.addressof(buf)
         for _ in range(n.value):

@@ -148,9 +148,9 @@ def hybrid_fusion(fusion_type, vec, txt, top_k, fusion_weight=0.5, fusion_k=60, 
     """RankFusion / RelativeScoreFusion + hybridSearch ordering.
     vec / txt: lists of (shard, part, label, score) already globally ordered."""
     def cols(lst):
-        a = np.array(lst, dtype=np.float64).reshape(-1, 4)
-        return (np.ascontiguousarray(a[:, 0], np.uint32), np.ascontiguousarray(a[:, 1], np.uint64),
-                np.ascontiguousarray(a[:, 2], np.uint64), np.ascontiguousarray(np.array([r[3] for r in lst], np.float32)))
+        # one exact column per field: labels go up to 2^64 - 1, beyond what a float64 holds exactly
+        return (np.array([int(r[0]) for r in lst], np.uint32), np.array([int(r[1]) for r in lst], np.uint64),
+                np.array([int(r[2]) for r in lst], np.uint64), np.array([r[3] for r in lst], np.float32))
     vs, vp, vl, vsc = cols(vec)
     ts, tp, tl, tsc = cols(txt)
     o_s, o_p, o_l, o_sc = (np.empty(top_k, np.uint32), np.empty(top_k, np.uint64), np.empty(top_k, np.uint64),

@@ -99,7 +99,6 @@ struct b200_corpus {
     std::mutex mu;
     // workspaces
     DevBuf w_raw, w_q32, w_qbf, w_qlo, w_qnorm, w_pk, w_pi, w_lk, w_li, w_alive, w_odis, w_oids, w_stage, w_prog;
-    int sync_slack = 2;
     // fused single-launch path of the host entry point (small batches, scan kernel): mapped pinned staging + counters
     void *h_pin = nullptr;         // [queries 8 * d fp32 | dis 8 * k | ids 8 * k | flag]
     size_t h_pin_bytes = 0;
@@ -240,7 +239,6 @@ extern "C" int b200_corpus_create(int metric, int dtype, int d, int64_t capacity
     c->cap = capacity_rows;
     cudaGetDevice(&c->device);
     c->sms = num_sms();
-    if (const char *ev = getenv("B200_GEMM_SYNC_SLACK")) c->sync_slack = atoi(ev);
     if (const char *ev = getenv("B200_GEMM_RESCORE_L2")) c->rescore_l2 = atoi(ev);
     if (const char *ev = getenv("B200_FUSED_SCAN")) c->fused_enabled = atoi(ev);
     cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
@@ -370,20 +368,6 @@ extern "C" int b200_corpus_size(const b200_corpus *c, int64_t *out_rows) {
     return B200_OK;
 }
 
-namespace b200 {
-// slots of a per-thread top-k list (kernels.h): k, unless B200_LIST_APPEND_MIN_K selects the append form for this k
-int list_cap_for(int k) {
-    static const int min_k = getenv("B200_LIST_APPEND_MIN_K") ? atoi(getenv("B200_LIST_APPEND_MIN_K")) : 0;
-    // default: the two-level (tournament) form from k = 17 (an insert rescans one group and the group worsts instead of all k
-    // entries); k <= 16 keeps the plain form.  The crossover k = 17 was chosen on an earlier GPU and is not re-measured on the H100.
-    // B200_LIST_TOURN_MIN_K=0 turns it off
-    static const int tourn_k = getenv("B200_LIST_TOURN_MIN_K") ? atoi(getenv("B200_LIST_TOURN_MIN_K")) : 17;
-    if (min_k > 0 && k >= min_k) return list_cap_append(k);
-    if (tourn_k > 0 && k >= tourn_k) return list_cap_tourn(k);
-    return k;
-}
-}  // namespace b200
-
 extern "C" int b200_corpus_set_path(b200_corpus *c, int path) {
     if (!c || path < 0 || path > 7) return fail(B200_ERR_INVALID, "path must be 0..7");
     std::lock_guard<std::mutex> lk(c->mu);
@@ -456,6 +440,9 @@ extern "C" int b200_corpus_free(b200_corpus *c) {
 // extrapolated, not measured.
 constexpr int64_t kBinaryTensorMinQB2 = 20480;
 
+// corpus tiles a CTA of gemm_topk_kernel may run ahead of the slowest CTA that streams the same tiles for another query tile
+constexpr int kGemmSyncSlack = 2;
+
 // One launch of gemm_topk_kernel over a chunk of <= 1024 staged queries (gp: operands, side arrays, d_pad and alive set),
 // then the merge of the CTAs' partial lists into rows of k of d_out_dis / d_out_ids.  kernel: B200_KERNEL_GEMM_*.
 static int gemm_chunk(b200_corpus *c, GemmTopkParams &gp, int64_t nq_c, int k, int kernel, int out_mode, const float *q_add,
@@ -480,11 +467,11 @@ static int gemm_chunk(b200_corpus *c, GemmTopkParams &gp, int64_t nq_c, int k, i
     gp.nq_valid = (int)nq_c;
     gp.k = k;
     gp.q_tiles = q_tiles;
-    if (q_tiles > 1 && c->sync_slack > 0) {
+    if (q_tiles > 1) {
         B200_TRY(c->w_prog.reserve((size_t)grid * 4));
         B200_CUDA_OK(cudaMemsetAsync(c->w_prog.p, 0, (size_t)grid * 4, s));
         gp.progress = c->w_prog.as<int>();
-        gp.sync_slack = c->sync_slack;
+        gp.sync_slack = kGemmSyncSlack;
     }
     const char *detail = nullptr;
     std::pair<cudaEvent_t, cudaEvent_t> ev;
@@ -846,10 +833,6 @@ static int search_host_fused(b200_corpus *c, const float *queries, int64_t nq, i
     sp.done_value = ++c->fused_seq ? c->fused_seq : ++c->fused_seq;   // never 0
     sp.q_inline = q_inline ? 1 : 0;
     if (q_inline) memcpy(sp.qinline, queries, (size_t)nq * c->d * 4);
-    static unsigned long long *dbg_ts = nullptr;   // B200_FUSED_DEBUG_TS=1: phase stamps of the kernel, printed every 64th call
-    static const bool dbg_on = getenv("B200_FUSED_DEBUG_TS") && atoi(getenv("B200_FUSED_DEBUG_TS"));
-    if (dbg_on && !dbg_ts) cudaMallocManaged(&dbg_ts, 16 * sizeof(unsigned long long));
-    sp.debug_ts = dbg_on ? dbg_ts : nullptr;
     *h_flag = 0;
     std::pair<cudaEvent_t, cudaEvent_t> ev;
     timing_begin(c, s, ev);
@@ -870,13 +853,6 @@ static int search_host_fused(b200_corpus *c, const float *queries, int64_t nq, i
 #if defined(__x86_64__)
         __builtin_ia32_pause();
 #endif
-    }
-    if (dbg_on && (c->fused_seq & 63) == 0) {
-        cudaStreamSynchronize(s);
-        fprintf(stderr, "fused ts (us since block 0 start): scan_done %.1f tail_start %.1f fence %.1f staged %.1f bounds %.1f compacted %.1f lists %.1f merged %.1f written %.1f sysfence %.1f survivors %llu\n",
-                (dbg_ts[1] - dbg_ts[0]) * 1e-3, (dbg_ts[2] - dbg_ts[0]) * 1e-3, (dbg_ts[3] - dbg_ts[0]) * 1e-3, (dbg_ts[4] - dbg_ts[0]) * 1e-3,
-                (dbg_ts[5] - dbg_ts[0]) * 1e-3, (dbg_ts[6] - dbg_ts[0]) * 1e-3, (dbg_ts[7] - dbg_ts[0]) * 1e-3, (dbg_ts[8] - dbg_ts[0]) * 1e-3,
-                (dbg_ts[9] - dbg_ts[0]) * 1e-3, (dbg_ts[10] - dbg_ts[0]) * 1e-3, dbg_ts[15]);
     }
     memcpy(out_dis, h_dis, (size_t)nq * k * 4);
     memcpy(out_ids, h_ids, (size_t)nq * k * 8);

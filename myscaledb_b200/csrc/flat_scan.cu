@@ -53,13 +53,6 @@ struct ChunkTraits<true> {
 // the low occupancy this kernel runs at).
 // L2 = squared-L2 vs inner product (cosine = inner product scaled by the stored inverse row norm).
 // candidate read of the fused tail: partial lists in global memory written by other blocks (L2, .cg) or staged in shared memory
-__device__ __forceinline__ unsigned long long gtimer() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-#define B200_TS(i) do { if (p.debug_ts && threadIdx.x == 0) p.debug_ts[i] = gtimer(); } while (0)
-
 template <typename T>
 __device__ __forceinline__ T ld_cand(const T *p, bool staged) { return staged ? *p : __ldcg(p); }
 
@@ -72,7 +65,6 @@ __global__ void __launch_bounds__(kScanThreads, 2) flat_scan_kernel(const ScanPa
     float *lk = qs + (size_t)QT * p.d_pad;                                   // [warps][QT][k]
     uint32_t *li = reinterpret_cast<uint32_t *>(lk + (size_t)kScanWarps * QT * p.k);
 
-    if (p.fused && blockIdx.x == 0 && blockIdx.y == 0) B200_TS(0);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t q0 = (int64_t)blockIdx.y * QT;
     const int nq_here = (int)min((int64_t)QT, p.nq - q0);
@@ -221,7 +213,6 @@ __global__ void __launch_bounds__(kScanThreads, 2) flat_scan_kernel(const ScanPa
                          p.part_keys + ((q0 + q) * (int64_t)gridDim.x + blockIdx.x) * p.k,
                          p.part_ids + ((q0 + q) * (int64_t)gridDim.x + blockIdx.x) * p.k);
     if (!p.fused) return;
-    if (blockIdx.x == 0 && blockIdx.y == 0) B200_TS(1);   // block 0: scan + block merge done
     // ---- fused form: the last block of this query tile merges the gridDim.x partial lists of each of its queries
     __shared__ unsigned int s_ticket;
     __threadfence();
@@ -229,9 +220,7 @@ __global__ void __launch_bounds__(kScanThreads, 2) flat_scan_kernel(const ScanPa
     if (threadIdx.x == 0) s_ticket = atomicAdd(&p.tickets[blockIdx.y], 1u);
     __syncthreads();
     if (s_ticket != gridDim.x - 1) return;
-    B200_TS(2);   // tail starts
     __threadfence();
-    B200_TS(3);
     // the staging area is free now: [warps][k] keys + ids, merged list behind it (launch reserves (warps + 1) * k * 8 bytes)
     float *mk = reinterpret_cast<float *>(smem_raw);
     uint32_t *mi = reinterpret_cast<uint32_t *>(mk + (size_t)kScanWarps * p.k);
@@ -272,7 +261,6 @@ __global__ void __launch_bounds__(kScanThreads, 2) flat_scan_kernel(const ScanPa
                 }
             }
             __syncthreads();
-            B200_TS(4);   // staged
             pkeys = sk;
             pids = si;
         }
@@ -332,7 +320,6 @@ __global__ void __launch_bounds__(kScanThreads, 2) flat_scan_kernel(const ScanPa
             }
             __syncthreads();
         }
-        B200_TS(5);   // bounds
         // Survivors of the bound are few (~k): every thread first sweeps its share of the candidates with independent loads
         // (no vote between them, so the L2 latencies overlap) and appends survivors to a compact shared array; only those go
         // through the warp lists.  (Voting after every load would put 12 dependent L2 round trips on the critical path.)
@@ -351,8 +338,6 @@ __global__ void __launch_bounds__(kScanThreads, 2) flat_scan_kernel(const ScanPa
             }
         }
         __syncthreads();
-        B200_TS(6);   // survivors compacted
-        if (p.debug_ts && threadIdx.x == 0) p.debug_ts[15] = (unsigned long long)cand_n;
         const int n_surv = cand_n;
         bool ranked = false;
         if (n_surv <= kScanThreads) {
@@ -406,10 +391,8 @@ __global__ void __launch_bounds__(kScanThreads, 2) flat_scan_kernel(const ScanPa
             }
         }
         __syncthreads();
-        B200_TS(7);   // warp lists
         if (!ranked) block_rank_merge(mk, mi, kScanWarps, p.k, p.k, fk, fi);
         __syncthreads();
-        B200_TS(8);   // merged
         for (int j = threadIdx.x; j < p.k; j += kScanThreads) {
             float dis;
             int64_t id;
@@ -432,10 +415,8 @@ __global__ void __launch_bounds__(kScanThreads, 2) flat_scan_kernel(const ScanPa
     }
     __syncthreads();
     if (threadIdx.x == 0) {
-        B200_TS(9);   // results written
         p.tickets[blockIdx.y] = 0;            // ready for the next call
-        __threadfence_system();
-        B200_TS(10);  // system fence               // results (mapped host memory) before the flag
+        __threadfence_system();               // results (mapped host memory) before the flag
         const unsigned int t = atomicAdd(p.tiles_done, 1u);
         if (t == gridDim.y - 1) {
             *p.tiles_done = 0;

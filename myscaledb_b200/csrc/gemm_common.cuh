@@ -209,183 +209,53 @@ __device__ __forceinline__ void acc_load32(const float *acc, int row, int c0, fl
 // coalesced in global scratch) plus the position of its current worst element.  An insert overwrites
 // the worst slot and rescans the k slots with independent loads; a sorted list would pay a dependent
 // load-compare-store chain per shifted element, which makes the start-up "insert storm" of a launch expensive.
-// The buffer is sorted once, when the CTA publishes its partial list.
+// The buffer is sorted once, when the CTA publishes its partial list.  From k = list_tourn_min_k it is the tournament form
+// (kernels.h, list_insert).
 struct ThreadTopK {
-    float *keys;       // entry j of this thread's list: keys[j * stride]
+    float *keys;       // entry j of this thread's list: keys[j * EPI_THREADS]
     uint32_t *ids;
     int k, n, worst;
-    int cap;           // slots of the buffer: == k -> "rescan" mode, > k (>= k + 32) -> "append" mode, see below
-    int stride;        // EPI_THREADS: lists interleaved (entry j of all 128 lists side by side); 1: each list contiguous
-    int coop;          // warp-uniform: inserts are done by the whole warp, one (lane, candidate) at a time (needs stride 1)
-    int append;        // cap >= 2k + 32: append form
-    int tourn;         // cap == list_cap_tourn(k): slots [k, cap) hold the worst (key, id) of every group of 8 / 16 entries; `worst` = a group
+    int tourn;         // k >= list_tourn_min_k: slots [k, list_cap_for(k)) hold the worst (key, id) of every group of 8 / 16 entries; `worst` = a group
     float thr_key;     // key of the current worst kept element (FLT_MAX while n < k)
     uint32_t thr_id;
 };
 
-// Layout and insert form (cap == k only; the append form keeps the interleaved layout):
-//  * interleaved lists, each lane inserts into its own list -- the default at every k;
-//  * contiguous lists and COOPERATIVE inserts (k >= B200_LIST_COOP_MIN_K, off by default): the accepted candidate of one lane
-//    is broadcast, lane 0 overwrites that list's worst entry, all 32 lanes rescan the list (k / 32 entries each) and a shuffle
-//    arg-max yields the new worst.  It did not pay where it was measured (an earlier GPU; not re-measured on the H100): a
-//    slow-path event carries a few candidates spread over the lanes, which the one-lane form retires in parallel rounds of one
-//    k-entry rescan each and the cooperative form in serial steps.  Kept for the unit test.
-#ifndef B200_LIST_COOP_MIN_K
-#define B200_LIST_COOP_MIN_K (1 << 30)
-#endif
-constexpr int kListCoopMinK = B200_LIST_COOP_MIN_K;
-// Element j of a list sits at keys[j * LIST_STRIDE(t)].  Production builds have no contiguous (cooperative) lists, so the stride is
-// the compile-time constant EPI_THREADS and the rescans address their entries with immediate offsets (a run-time stride costs
-// an address computation per entry of every rescan).
-#if B200_LIST_COOP_MIN_K >= (1 << 30)
-#define LIST_STRIDE(t) EPI_THREADS
-#else
-#define LIST_STRIDE(t) ((t).stride)
-#endif
-__device__ __forceinline__ void list_bind(ThreadTopK &t, float *keys_base, uint32_t *ids_base, int row, int k, int cap) {
+// keys_base / ids_base: the lists of the CTA's 128 threads, interleaved (entry j of all 128 lists side by side), with
+// list_cap_for(k) slots each.  The stride is the compile-time constant EPI_THREADS, so the rescans address their entries with
+// immediate offsets.
+__device__ __forceinline__ void list_bind(ThreadTopK &t, float *keys_base, uint32_t *ids_base, int row, int k) {
     t.k = k;
-    t.cap = cap;
-    t.append = cap >= 2 * k + 32 ? 1 : 0;
-    t.tourn = (!t.append && cap > k && cap == list_cap_tourn(k)) ? 1 : 0;
-    t.coop = (cap == k && k >= kListCoopMinK) ? 1 : 0;
-    t.stride = t.coop ? 1 : EPI_THREADS;
-    t.keys = keys_base + (t.coop ? (size_t)row * cap : (size_t)row);
-    t.ids = ids_base + (t.coop ? (size_t)row * cap : (size_t)row);
-}
-
-// Two ways to keep the k best:
-//  * rescan (cap == k, the default): an accepted candidate overwrites the worst entry and the list is rescanned for the new
-//    worst -- O(k) dependent-free loads per insert; the threshold is always exact.
-//  * append (cap >= 2k + 32, opt-in): an accepted candidate is stored behind the others (two stores, nothing to wait for);
-//    when some lane of the warp is within 32 slots of the end, EVERY lane of the warp compacts its own buffer in lock-step
-//    (quickselect for the k-th entry, then one partition pass) and tightens its threshold.  It needs twice the slots -- 200 KB
-//    at k = 100, which the operand ring does not leave -- and from global scratch it loses the point of cheap inserts; the
-//    slack must be real: with k + 32 slots every slow-path event compacts.  tests/cuda/list_perf.cu times both forms on a
-//    synthetic stream shaped like the flat kernel's epilogue; they have not been compared on the H100.
-// (slot counts: list_cap_for / list_cap_append in kernels.h)
-
-struct ListThr {
-    float key;
-    uint32_t id;
-};
-
-// counters for tests/cuda/list_append_test.cu --perf (compiled in only there)
-#ifdef B200_LIST_STATS
-__device__ unsigned long long g_list_stats[4];   // slow-path events, compaction calls (warp level), quickselect rounds, appended entries
-#define B200_LIST_STAT(i, v) atomicAdd(&g_list_stats[i], (unsigned long long)(v))
-#else
-#define B200_LIST_STAT(i, v)
-#endif
-
-// Keep the k best of this thread's n (> k) entries in slots [0, k) and return the k-th (the new threshold).  Entries are
-// distinct (unique ids), so (key, id) is a strict total order and exactly one entry has rank k.  Quickselect without
-// moving data: the pivot's rank is counted in one pass, which also picks the next pivot on either side pseudo-randomly
-// (smallest multiplicative hash of the slot), so sorted input does not degrade it.  All lanes of a warp run this together.
-static __device__ __noinline__ ListThr list_compact(float *keys, uint32_t *ids, int k, int n, int stride) {
-    float lo_k = 0.f, hi_k = 0.f;          // open interval (lo, hi) that still contains the rank-k entry
-    uint32_t lo_i = 0, hi_i = 0;
-    bool have_lo = false, have_hi = false;
-    float pk = keys[(n - 1) * stride];
-    uint32_t pi = ids[(n - 1) * stride];
-    uint32_t salt = 0x9E3779B1u;
-    for (;;) {
-        int rank = 0;
-        float ck_lo = 0.f, ck_hi = 0.f;
-        uint32_t ci_lo = 0, ci_hi = 0, h_lo = 0xffffffffu, h_hi = 0xffffffffu;
-        for (int j = 0; j < n; j++) {
-            const float kj = keys[j * stride];
-            const uint32_t ij = ids[j * stride];
-            const uint32_t h = ((uint32_t)j + 1u) * salt;
-            if (better(kj, ij, pk, pi)) {
-                rank++;
-                if ((!have_lo || better(lo_k, lo_i, kj, ij)) && h <= h_lo) {
-                    h_lo = h;
-                    ck_lo = kj;
-                    ci_lo = ij;
-                }
-            } else if (better(pk, pi, kj, ij)) {
-                if ((!have_hi || better(kj, ij, hi_k, hi_i)) && h <= h_hi) {
-                    h_hi = h;
-                    ck_hi = kj;
-                    ci_hi = ij;
-                }
-            }
-        }
-        rank++;  // the pivot itself
-        B200_LIST_STAT(2, 1);
-        if (rank == k) break;
-        if (rank < k) {          // the answer is worse than the pivot
-            lo_k = pk; lo_i = pi; have_lo = true;
-            pk = ck_hi; pi = ci_hi;
-        } else {
-            hi_k = pk; hi_i = pi; have_hi = true;
-            pk = ck_lo; pi = ci_lo;
-        }
-        salt = salt * 0x85EBCA6Bu + 0xC2B2AE35u;
-        salt |= 1u;
-    }
-    // partition: kept entries found behind slot k fill the slots of dropped entries in front of it
-    int dst = 0;
-    for (int j = k; j < n; j++) {
-        const float kj = keys[j * stride];
-        const uint32_t ij = ids[j * stride];
-        if (!better(pk, pi, kj, ij)) {   // kj <= pivot: kept
-            while (!better(pk, pi, keys[dst * stride], ids[dst * stride])) dst++;   // skip kept entries
-            keys[dst * stride] = kj;
-            ids[dst * stride] = ij;
-            dst++;
-        }
-    }
-    ListThr r;
-    r.key = pk;
-    r.id = pi;
-    return r;
-}
-
-__device__ __forceinline__ void list_compact_if_over(ThreadTopK &t) {
-    if (t.n > t.k) {
-        const ListThr r = list_compact(t.keys, t.ids, t.k, t.n, LIST_STRIDE(t));
-        t.n = t.k;
-        t.thr_key = r.key;
-        t.thr_id = r.id;
-    }
+    t.tourn = k >= list_tourn_min_k ? 1 : 0;
+    t.keys = keys_base + row;
+    t.ids = ids_base + row;
 }
 
 __device__ __forceinline__ void list_insert(ThreadTopK &t, float key, uint32_t id) {
     if (!better(key, id, t.thr_key, t.thr_id)) return;
-    if (t.append) {   // append mode: the caller keeps n + 32 <= cap before every chunk (epilogue_chunk)
-        B200_LIST_STAT(3, 1);
-        t.keys[t.n * LIST_STRIDE(t)] = key;
-        t.ids[t.n * LIST_STRIDE(t)] = id;
-        t.n++;
-        return;
-    }
     if (t.tourn) {
         // Two-level form: the worst entry of each group of G = 8 / 16 is cached behind the list, so an insert rescans ONE group (to
         // find the slot of the entry it evicts and that group's new worst) and the group worsts: 2 (G + k / G) loads instead of 2 k.
         const int G = list_tourn_group(t.k);
         const int ng = (t.k + G - 1) / G;
-        float *gk = t.keys + (size_t)t.k * LIST_STRIDE(t);
-        uint32_t *gi = t.ids + (size_t)t.k * LIST_STRIDE(t);
         if (t.n < t.k) {
-            t.keys[t.n * LIST_STRIDE(t)] = key;
-            t.ids[t.n * LIST_STRIDE(t)] = id;
+            t.keys[t.n * EPI_THREADS] = key;
+            t.ids[t.n * EPI_THREADS] = id;
             t.n++;
             if (t.n < t.k) return;
             for (int g = 0; g < ng; g++) {   // the list just became full: every group's worst, once
                 const int base = g * G, end = base + G < t.k ? base + G : t.k;
-                float wk = t.keys[base * LIST_STRIDE(t)];
-                uint32_t wi = t.ids[base * LIST_STRIDE(t)];
+                float wk = t.keys[base * EPI_THREADS];
+                uint32_t wi = t.ids[base * EPI_THREADS];
                 for (int j = base + 1; j < end; j++) {
-                    const float kj = t.keys[j * LIST_STRIDE(t)];
-                    const uint32_t ij = t.ids[j * LIST_STRIDE(t)];
+                    const float kj = t.keys[j * EPI_THREADS];
+                    const uint32_t ij = t.ids[j * EPI_THREADS];
                     if (better(wk, wi, kj, ij)) {
                         wk = kj;
                         wi = ij;
                     }
                 }
-                gk[g * LIST_STRIDE(t)] = wk;
-                gi[g * LIST_STRIDE(t)] = wi;
+                t.keys[(t.k + g) * EPI_THREADS] = wk;
+                t.ids[(t.k + g) * EPI_THREADS] = wi;
             }
         } else {
             const int g = t.worst;   // the group that holds the evicted entry (= the current threshold)
@@ -395,8 +265,8 @@ __device__ __forceinline__ void list_insert(ThreadTopK &t, float key, uint32_t i
             int slot = -1;
             bool have = false;
             for (int j = base; j < end; j++) {
-                float kj = t.keys[j * LIST_STRIDE(t)];
-                uint32_t ij = t.ids[j * LIST_STRIDE(t)];
+                float kj = t.keys[j * EPI_THREADS];
+                uint32_t ij = t.ids[j * EPI_THREADS];
                 if (slot < 0 && kj == t.thr_key && ij == t.thr_id) {
                     slot = j;
                     kj = key;
@@ -409,17 +279,17 @@ __device__ __forceinline__ void list_insert(ThreadTopK &t, float key, uint32_t i
                 }
             }
             if (slot < 0) slot = base;   // cannot happen (ids are unique and the threshold is an entry of this group); never write out of range
-            t.keys[slot * LIST_STRIDE(t)] = key;
-            t.ids[slot * LIST_STRIDE(t)] = id;
-            gk[g * LIST_STRIDE(t)] = wk;
-            gi[g * LIST_STRIDE(t)] = wi;
+            t.keys[slot * EPI_THREADS] = key;
+            t.ids[slot * EPI_THREADS] = id;
+            t.keys[(t.k + g) * EPI_THREADS] = wk;
+            t.ids[(t.k + g) * EPI_THREADS] = wi;
         }
-        float wk = gk[0];
-        uint32_t wi = gi[0];
+        float wk = t.keys[t.k * EPI_THREADS];
+        uint32_t wi = t.ids[t.k * EPI_THREADS];
         int wg = 0;
         for (int g = 1; g < ng; g++) {
-            const float kg = gk[g * LIST_STRIDE(t)];
-            const uint32_t ig = gi[g * LIST_STRIDE(t)];
+            const float kg = t.keys[(t.k + g) * EPI_THREADS];
+            const uint32_t ig = t.ids[(t.k + g) * EPI_THREADS];
             if (better(wk, wi, kg, ig)) {
                 wk = kg;
                 wi = ig;
@@ -432,21 +302,21 @@ __device__ __forceinline__ void list_insert(ThreadTopK &t, float key, uint32_t i
         return;
     }
     if (t.n < t.k) {
-        t.keys[t.n * LIST_STRIDE(t)] = key;
-        t.ids[t.n * LIST_STRIDE(t)] = id;
+        t.keys[t.n * EPI_THREADS] = key;
+        t.ids[t.n * EPI_THREADS] = id;
         t.n++;
         if (t.n < t.k) return;
     } else {
-        t.keys[t.worst * LIST_STRIDE(t)] = key;
-        t.ids[t.worst * LIST_STRIDE(t)] = id;
+        t.keys[t.worst * EPI_THREADS] = key;
+        t.ids[t.worst * EPI_THREADS] = id;
     }
     // rescan for the worst (largest key, ties -> larger id)
     float wk = t.keys[0];
     uint32_t wi = t.ids[0];
     int wp = 0;
     for (int j = 1; j < t.k; j++) {
-        const float kj = t.keys[j * LIST_STRIDE(t)];
-        const uint32_t ij = t.ids[j * LIST_STRIDE(t)];
+        const float kj = t.keys[j * EPI_THREADS];
+        const uint32_t ij = t.ids[j * EPI_THREADS];
         if (better(wk, wi, kj, ij)) {
             wk = kj;
             wi = ij;
@@ -460,22 +330,21 @@ __device__ __forceinline__ void list_insert(ThreadTopK &t, float key, uint32_t i
 
 // sort the n kept entries best-first (insertion sort, once per kernel) and publish them
 static __device__ __noinline__ void list_publish(ThreadTopK &t, float *out_keys, uint32_t *out_ids) {
-    list_compact_if_over(t);
     for (int i = 1; i < t.n; i++) {
-        const float ki = t.keys[i * LIST_STRIDE(t)];
-        const uint32_t ii = t.ids[i * LIST_STRIDE(t)];
+        const float ki = t.keys[i * EPI_THREADS];
+        const uint32_t ii = t.ids[i * EPI_THREADS];
         int j = i;
-        while (j > 0 && better(ki, ii, t.keys[(j - 1) * LIST_STRIDE(t)], t.ids[(j - 1) * LIST_STRIDE(t)])) {
-            t.keys[j * LIST_STRIDE(t)] = t.keys[(j - 1) * LIST_STRIDE(t)];
-            t.ids[j * LIST_STRIDE(t)] = t.ids[(j - 1) * LIST_STRIDE(t)];
+        while (j > 0 && better(ki, ii, t.keys[(j - 1) * EPI_THREADS], t.ids[(j - 1) * EPI_THREADS])) {
+            t.keys[j * EPI_THREADS] = t.keys[(j - 1) * EPI_THREADS];
+            t.ids[j * EPI_THREADS] = t.ids[(j - 1) * EPI_THREADS];
             j--;
         }
-        t.keys[j * LIST_STRIDE(t)] = ki;
-        t.ids[j * LIST_STRIDE(t)] = ii;
+        t.keys[j * EPI_THREADS] = ki;
+        t.ids[j * EPI_THREADS] = ii;
     }
     for (int j = 0; j < t.k; j++) {
-        out_keys[j] = j < t.n ? t.keys[j * LIST_STRIDE(t)] : FLT_MAX;
-        out_ids[j] = j < t.n ? t.ids[j * LIST_STRIDE(t)] : kNoId;
+        out_keys[j] = j < t.n ? t.keys[j * EPI_THREADS] : FLT_MAX;
+        out_ids[j] = j < t.n ? t.ids[j * EPI_THREADS] : kNoId;
     }
 }
 
@@ -515,71 +384,6 @@ __device__ __forceinline__ void jaccard_keys32(float (&v)[32], int pq, const flo
     }
 }
 
-// Cooperative insert (t.coop): called by the whole warp; lane `src` contributes the candidate and owns the list.
-__device__ __forceinline__ void list_insert_coop(ThreadTopK &t, int src, float key, uint32_t id) {
-    const int lane = threadIdx.x & 31;
-    key = __shfl_sync(0xffffffffu, key, src);
-    id = __shfl_sync(0xffffffffu, id, src);
-    const float thr_key = __shfl_sync(0xffffffffu, t.thr_key, src);
-    const uint32_t thr_id = __shfl_sync(0xffffffffu, t.thr_id, src);
-    if (!better(key, id, thr_key, thr_id)) return;   // warp-uniform
-    const unsigned long long kp = __shfl_sync(0xffffffffu, (unsigned long long)reinterpret_cast<uintptr_t>(t.keys), src);
-    const unsigned long long ip = __shfl_sync(0xffffffffu, (unsigned long long)reinterpret_cast<uintptr_t>(t.ids), src);
-    float *lk = reinterpret_cast<float *>((uintptr_t)kp);
-    uint32_t *li = reinterpret_cast<uint32_t *>((uintptr_t)ip);
-    int n = __shfl_sync(0xffffffffu, t.n, src);
-    const int k = t.k;
-    if (n < k) {
-        if (lane == 0) {
-            lk[n] = key;
-            li[n] = id;
-        }
-        n++;
-        if (n < k) {
-            if (lane == src) t.n = n;
-            return;
-        }
-    } else {
-        const int worst = __shfl_sync(0xffffffffu, t.worst, src);
-        if (lane == 0) {
-            lk[worst] = key;
-            li[worst] = id;
-        }
-    }
-    __syncwarp();
-    // the new worst: every lane scans k / 32 entries, then a shuffle arg-max over (key, id)
-    float wk = 0.f;
-    uint32_t wi = 0;
-    int wp = -1;
-    for (int j = lane; j < k; j += 32) {
-        const float kj = lk[j];
-        const uint32_t ij = li[j];
-        if (wp < 0 || better(wk, wi, kj, ij)) {
-            wk = kj;
-            wi = ij;
-            wp = j;
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const float ok = __shfl_xor_sync(0xffffffffu, wk, o);
-        const uint32_t oi = __shfl_xor_sync(0xffffffffu, wi, o);
-        const int op = __shfl_xor_sync(0xffffffffu, wp, o);
-        if (op >= 0 && (wp < 0 || better(wk, wi, ok, oi))) {
-            wk = ok;
-            wi = oi;
-            wp = op;
-        }
-    }
-    if (lane == src) {
-        t.n = n;
-        t.worst = wp;
-        t.thr_key = wk;
-        t.thr_id = wi;
-    }
-    __syncwarp();
-}
-
 // Filter one chunk of 32 accumulator columns of this thread's query row.
 // Fast path (steady state): reduce the chunk to its best key with FMNMX3 trees, one warp vote,
 // done.  Slow path (some lane of the warp can improve its list; frequent only during the first
@@ -591,7 +395,7 @@ __device__ __forceinline__ void list_insert_coop(ThreadTopK &t, int src, float k
 __device__ __forceinline__ void epilogue_chunk(ThreadTopK &list, float (&v)[32], bool use_side, const float *scale,
                                                const float *bias, uint32_t id0, bool tail, int64_t n, float *scratch,
                                                float ext_bound = FLT_MAX /* a valid upper bound of the k-th key known from elsewhere */) {
-    float thr = fminf(list.thr_key, ext_bound);
+    const float thr = fminf(list.thr_key, ext_bound);
     bool mine;
     if (use_side) {
         side_fma32(v, scale, bias);  // 16 broadcast LDS.128
@@ -617,12 +421,6 @@ __device__ __forceinline__ void epilogue_chunk(ThreadTopK &list, float (&v)[32],
         mine = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)) >= -thr;
     }
     if (__any_sync(0xffffffffu, mine)) {
-        if ((threadIdx.x & 31) == 0) B200_LIST_STAT(0, 1);
-        if (list.append && __any_sync(0xffffffffu, list.n + 32 > list.cap)) {
-            if ((threadIdx.x & 31) == 0) B200_LIST_STAT(1, 1);
-            list_compact_if_over(list);   // every lane, in lock-step: room for this chunk and a fresh threshold
-            thr = fminf(list.thr_key, ext_bound);
-        }
         uint32_t mask = 0;
 #pragma unroll
         for (int j = 0; j < 32; j++) {
@@ -634,29 +432,11 @@ __device__ __forceinline__ void epilogue_chunk(ThreadTopK &list, float (&v)[32],
             const int64_t left = n - (int64_t)id0;
             mask = left >= 32 ? mask : left <= 0 ? 0u : (mask & ((1u << left) - 1u));
         }
-        if (list.coop) {
-            // one (lane, candidate) at a time, the whole warp inserting
-            unsigned pending = __ballot_sync(0xffffffffu, mask != 0);
-            while (pending) {
-                const int src = __ffs(pending) - 1;
-                float ckey = 0.f;
-                uint32_t cid = 0;
-                if ((int)(threadIdx.x & 31) == src) {
-                    const int j = __ffs(mask) - 1;
-                    mask &= mask - 1;
-                    ckey = scratch[j * EPI_THREADS];
-                    cid = id0 + (uint32_t)j;
-                }
-                list_insert_coop(list, src, ckey, cid);
-                pending = __ballot_sync(0xffffffffu, mask != 0);
-            }
-        } else {
-            while (__any_sync(0xffffffffu, mask != 0)) {
-                if (mask) {
-                    const int j = __ffs(mask) - 1;
-                    mask &= mask - 1;
-                    list_insert(list, scratch[j * EPI_THREADS], id0 + (uint32_t)j);
-                }
+        while (__any_sync(0xffffffffu, mask != 0)) {
+            if (mask) {
+                const int j = __ffs(mask) - 1;
+                mask &= mask - 1;
+                list_insert(list, scratch[j * EPI_THREADS], id0 + (uint32_t)j);
             }
         }
     }

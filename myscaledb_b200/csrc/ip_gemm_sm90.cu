@@ -160,12 +160,13 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
         // rows past the batch (zero padding up to the tile size) must never pay for the slow path: nothing beats -FLT_MAX
         list.thr_key = (qt * BM + row < p.nq_valid) ? FLT_MAX : -FLT_MAX;
         list.thr_id = 0;
+        const int list_cap = list_cap_for(p.k);
         if (p.lists_in_smem)
             list_bind(list, reinterpret_cast<float *>(smem + O::off_list(STAGES)),
-                      reinterpret_cast<uint32_t *>(smem + O::off_list(STAGES) + (size_t)p.list_cap * EPI_THREADS * 4), row, p.k, p.list_cap);
+                      reinterpret_cast<uint32_t *>(smem + O::off_list(STAGES) + (size_t)list_cap * EPI_THREADS * 4), row, p.k);
         else
-            list_bind(list, p.list_keys_gmem + (size_t)blockIdx.x * p.list_cap * EPI_THREADS,
-                      p.list_ids_gmem + (size_t)blockIdx.x * p.list_cap * EPI_THREADS, row, p.k, p.list_cap);
+            list_bind(list, p.list_keys_gmem + (size_t)blockIdx.x * list_cap * EPI_THREADS,
+                      p.list_ids_gmem + (size_t)blockIdx.x * list_cap * EPI_THREADS, row, p.k);
         // binary Jaccard: popc(q) of this thread's query row (0 for padding rows)
         const int pq = (OP == Operand::B1 && p.jaccard && qt * BM + row < p.nq_valid) ? (int)p.q_popc[qt * BM + row] : 0;
         const uint32_t smem0 = smem_u32(smem);
@@ -326,9 +327,9 @@ static cudaError_t launch(const CUtensorMap &map_q, const CUtensorMap &map_qlo, 
     GemmTopkParams p = p_in;
     // Per-thread lists sit in shared memory whenever they fit, even when that squeezes the operand ring: every insert rescans
     // the list, and from global scratch that is k L2 round trips.
-    p.list_cap = list_cap_for(p.k);
-    p.lists_in_smem = O::lists_fit(p.list_cap) ? 1 : 0;
-    const int k_smem = p.lists_in_smem ? p.list_cap : 0;
+    const int list_cap = list_cap_for(p.k);
+    p.lists_in_smem = O::lists_fit(list_cap) ? 1 : 0;
+    const int k_smem = p.lists_in_smem ? list_cap : 0;
     p.stages = O::stages_for(k_smem);
     const size_t smem = O::smem_bytes(p.stages, k_smem);
     auto kern = gemm_topk_kernel<OP>;

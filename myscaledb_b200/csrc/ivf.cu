@@ -2196,8 +2196,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     gp.part_ids = ix->w_pi.as<uint32_t>();
     gp.part_worst = ix->w_pw.as<float>();
     {   // shared per-query bound across the items of this launch (ivf_gemm.h); nothing to share with one list per query
-        static const bool bound_on = !(getenv("B200_IVF_BOUND") && atoi(getenv("B200_IVF_BOUND")) == 0);
-        if (bound_on && nprobe > 1 && parse_int_param(params, "shared_bound", 1) != 0) {   // shared_bound=0: A/B switch
+        if (nprobe > 1 && parse_int_param(params, "shared_bound", 1) != 0) {   // shared_bound=0: A/B switch
             B200_TRY(ix->w_qb.reserve((size_t)nq * 4));
             B200_CUDA_OK(cudaMemsetAsync(ix->w_qb.p, 0xff, (size_t)nq * 4, s));
             gp.query_bound = ix->w_qb.as<uint32_t>();

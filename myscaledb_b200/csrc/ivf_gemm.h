@@ -50,7 +50,7 @@ struct IvfGemmParams {
     const uint32_t *sorted_pair;      // [n_pairs] sorted position -> original pair index (query = pair / nprobe)
     const float *pair_const;          // [n_pairs]
     int nprobe;
-    int stages, lists_in_smem, list_cap, codebook_smem_off, coop_smem_off, coop_enabled;
+    int stages, lists_in_smem, codebook_smem_off, coop_smem_off, coop_enabled;
 };
 
 // queries_bf16: gathered query rows [n_query_rows][d_pad] (bf16; binary: bytes); pool_bf16: page pool [pool_rows][d_pad] (bf16 and

@@ -117,12 +117,13 @@ ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
         const int row = threadIdx.x;                  // query slot inside the item
         float *scratch = reinterpret_cast<float *>(smem + C::off_scratch(STAGES)) + row;
         ThreadTopK list;
+        const int list_cap = list_cap_for(p.k);
         if (p.lists_in_smem)
             list_bind(list, reinterpret_cast<float *>(smem + C::off_list(STAGES)),
-                      reinterpret_cast<uint32_t *>(smem + C::off_list(STAGES) + (size_t)p.list_cap * EPI_THREADS * 4), row, p.k, p.list_cap);
+                      reinterpret_cast<uint32_t *>(smem + C::off_list(STAGES) + (size_t)list_cap * EPI_THREADS * 4), row, p.k);
         else
-            list_bind(list, p.list_keys_gmem + (size_t)blockIdx.x * p.list_cap * EPI_THREADS,
-                      p.list_ids_gmem + (size_t)blockIdx.x * p.list_cap * EPI_THREADS, row, p.k, p.list_cap);
+            list_bind(list, p.list_keys_gmem + (size_t)blockIdx.x * list_cap * EPI_THREADS,
+                      p.list_ids_gmem + (size_t)blockIdx.x * list_cap * EPI_THREADS, row, p.k);
         // cooperative lists (items with <= kCoopMax queries), owned by warp 0 (query slots 0..31)
         const CoopSmem cs = coop_smem_carve(smem + p.coop_smem_off, smem + C::off_scratch(STAGES), p.k);
         float *tile_row = cs.tilebuf + (size_t)(lane < kCoopMax ? lane : 0) * kTileBufStride;
@@ -290,14 +291,13 @@ ivf_gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
                     __syncwarp();
                 }
             } else if ((uint32_t)row < item.q_count) {
-                list_compact_if_over(list);   // append form: at most k entries leave the item
                 const size_t part = (size_t)p.pair_part_base[item.q_begin + row] + item.chunk;
                 float *ok = p.part_keys + part * p.k;
                 uint32_t *oi = p.part_ids + part * p.k;
                 for (int e = 0; e < p.k; e++) {
                     const bool have = e < list.n;
-                    ok[e] = have ? list.keys[e * list.stride] : FLT_MAX;
-                    oi[e] = have ? p.row_ids[list.ids[e * list.stride]] : kNoId;
+                    ok[e] = have ? list.keys[e * EPI_THREADS] : FLT_MAX;
+                    oi[e] = have ? p.row_ids[list.ids[e * EPI_THREADS]] : kNoId;
                 }
                 p.part_worst[part] = list.n == p.k ? list.thr_key : FLT_MAX;
             }
@@ -501,10 +501,10 @@ static cudaError_t launch_ivf(const CUtensorMap &map_q, const CUtensorMap &map_c
     const int coop_used = p.coop_enabled ? coop_bytes : 0;
     int stages = 4;
     p.lists_in_smem = 0;
-    p.list_cap = list_cap_for(p.k);
-    if (p.list_cap <= 2 * kGemmSmemK)
+    const int list_cap = list_cap_for(p.k);
+    if (list_cap <= 2 * kGemmSmemK)
         for (int st = 4; st >= 3; st--)
-            if (need(st, p.list_cap) + coop_used <= SMEM_LIMIT) {
+            if (need(st, list_cap) + coop_used <= SMEM_LIMIT) {
                 stages = st;
                 p.lists_in_smem = 1;
                 break;
@@ -514,7 +514,7 @@ static cudaError_t launch_ivf(const CUtensorMap &map_q, const CUtensorMap &map_c
         if (need(stages, 0) + coop_used > SMEM_LIMIT) return cudaErrorInvalidValue;
     }
     p.stages = stages;
-    const int k_smem = p.lists_in_smem ? p.list_cap : 0;
+    const int k_smem = p.lists_in_smem ? list_cap : 0;
     p.coop_smem_off = (int)round_up(Layout<Operand::BF16>::off_list(stages) + k_smem * EPI_THREADS * 8, 16);
     p.codebook_smem_off = (int)round_up(p.coop_smem_off + coop_used, 16);
     const size_t smem = (size_t)need(stages, k_smem) + coop_used;

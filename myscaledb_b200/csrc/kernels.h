@@ -31,7 +31,6 @@ struct ScanParams {
     unsigned int done_value;
     unsigned int *tiles_done;          // fused: one zeroed counter (reset by the last tile)
     int q_inline;                      // fused: the queries travel in the kernel parameters (nq * q_dim <= 256 floats)
-    unsigned long long *debug_ts;      // fused, debugging (B200_FUSED_DEBUG_TS=1): %globaltimer stamps of block 0's start and the tail's phases
     int stage_cap;                     // fused: candidates (gridDim.x * k) the last block may stage in shared memory, 0 = none (set by the launcher)
     float qinline[256];
 };
@@ -97,20 +96,21 @@ struct GemmTopkParams {
     int *progress;             // [grid / q_tiles][q_tiles] zeroed pacing counters, or null
     int stages;                // smem ring depth (filled in by the launcher)
     int lists_in_smem;         // per-thread top-k lists in shared memory (else global scratch); set by the launcher
-    int list_cap;              // slots per list: k (rescan mode) or list_cap_append(k) (append mode); set by the launcher
     int sync_slack;            // tiles a CTA may run ahead of the slowest sharer of its corpus tiles
 };
 // per-thread top-k lists of the IVF scan may live in shared memory up to twice this k (the launcher checks the fit)
 constexpr int kGemmSmemK = 128;
-// per-thread top-k lists (gemm_common.cuh, ThreadTopK): k slots and a rescan per insert (the default), or an append buffer
-// of 2k + 32 slots compacted in lock-step (B200_LIST_APPEND_MIN_K=<k>: lists of at least that k use it; it can only pay when
-// the doubled buffer still fits in shared memory, which it does not at k = 100)
-__host__ __device__ inline int list_cap_append(int k) { return 2 * k + 32; }
-// tournament form: k entries + one (key, id) slot per group of 8 (k <= 64) or 16 entries holding the group's worst
-// (B200_LIST_TOURN_MIN_K); 16 keeps k = 100 at 107 slots, which still leaves the flat kernel a 3-stage operand ring
+// Per-thread top-k lists (gemm_common.cuh, ThreadTopK) take one of two forms, chosen by k alone:
+//  * rescan (k < list_tourn_min_k): k slots; an insert rescans all k entries for the new worst;
+//  * tournament (k >= list_tourn_min_k): k entries + one (key, id) slot per group of 8 (k <= 64) or 16 entries holding the
+//    group's worst; an insert rescans one group and the group worsts instead of all k entries.  16 keeps k = 100 at 107 slots,
+//    which still leaves the flat kernel a 3-stage operand ring.
+// The crossover k = 17 was chosen on an earlier GPU and is not re-measured on the H100.
+constexpr int list_tourn_min_k = 17;
 __host__ __device__ inline int list_tourn_group(int k) { return k <= 64 ? 8 : 16; }
 __host__ __device__ inline int list_cap_tourn(int k) { return k + (k + list_tourn_group(k) - 1) / list_tourn_group(k); }
-int list_cap_for(int k);   // capi.cu: k, or list_cap_append(k) when the environment asks for the append form
+// slots of a per-thread list of this k
+__host__ __device__ inline int list_cap_for(int k) { return k < list_tourn_min_k ? k : list_cap_tourn(k); }
 int gemm_topk_grid(int q_tiles, int64_t n, int num_sms);
 // returns cudaSuccess or an error; tensor maps are encoded inside
 cudaError_t launch_gemm_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail);

@@ -1,7 +1,7 @@
 """FLAT search paths against the float64 reference of the stored corpus (tests/flat_reference.py): the staged scan, the
 fused single-query scan, bf16 on the tensor cores and fp32 (3xTF32) on the tensor cores, for L2, IP and cosine, at the
 shapes where such kernels break; then targeted tests of the IP quirk, the L2 re-score, tiny norms, NaN / inf rows, the
-device entry points, chunked appends, schedules, list forms, the per-thread scratch corpus and the refusals.
+device entry points, chunked appends, schedules, the per-thread scratch corpus and the refusals.
 
 Non-finite rows.  A row whose distance is not finite (a NaN coordinate; under L2 and cosine also an infinite one) is never
 returned and never displaces a finite row, on every path.  Under IP an infinite coordinate has no single meaning across
@@ -10,8 +10,6 @@ outside the IP contract and not tested.
 
 Run with -s to see the largest error / bound ratio of every path."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -26,7 +24,6 @@ from tests.util import check_topk, to_bf16_values
 pytestmark = pytest.mark.gpu
 F32 = np.float32
 METRICS = [b2.L2, b2.IP, b2.COSINE]
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 # the four flat paths: (reference path, corpus dtype or None = alternate, set_path code, entry)
 PATHS = {
@@ -483,44 +480,7 @@ def test_fused_scan_branches():
                 assert np.array_equal(ids, fr.ideal_answer(r)[1]), (n, d, k, tied)
 
 
-# ------------------------------------------------------------------ 8. list forms (read once per process)
-LIST_CHILD = r"""
-import sys, numpy as np
-sys.path.insert(0, sys.argv[1])
-import myscaledb_b200 as b2
-from myscaledb_b200 import search as S
-rng = np.random.default_rng(8)
-y = rng.standard_normal((20000, 64)).astype(np.float32)
-x = rng.standard_normal((200, 64)).astype(np.float32)
-out = {}
-for dtype in (S.BF16, S.F32):
-    for metric in (b2.L2, b2.IP, b2.COSINE):
-        c = b2.Corpus(metric, 64, dtype=dtype).append(y).set_path(2)
-        for k in (1, 16, 17, 100, 1024):
-            d, i = c.search(x, k)
-            out[f"d{dtype}m{metric}k{k}"] = d
-            out[f"i{dtype}m{metric}k{k}"] = i
-        c.close()
-np.savez(sys.argv[2], **out)
-"""
-
-
-def test_list_forms_are_byte_identical(tmp_path):
-    res = {}
-    for name, env in (("default", {}), ("append", {"B200_LIST_APPEND_MIN_K": "1"}), ("no_tournament", {"B200_LIST_TOURN_MIN_K": "0"})):
-        e = {kk: v for kk, v in os.environ.items() if not kk.startswith("B200_LIST_")}
-        e.update(env)
-        out = tmp_path / f"{name}.npz"
-        p = subprocess.run([sys.executable, "-c", LIST_CHILD, ROOT, str(out)], env=e, capture_output=True, text=True, timeout=600)
-        assert p.returncode == 0, p.stderr[-3000:]
-        res[name] = np.load(out)
-    for name in ("append", "no_tournament"):
-        for key in res["default"].files:
-            a, b = res["default"][key], res[name][key]
-            assert np.array_equal(a.view(np.uint32) if a.dtype == F32 else a, b.view(np.uint32) if b.dtype == F32 else b), (name, key)
-
-
-# ------------------------------------------------------------------ 9. the per-thread scratch corpus
+# ------------------------------------------------------------------ 8. the per-thread scratch corpus
 def _quirk(dis, ids):
     keep = dis > F32(fr.FLT_MIN)
     return np.where(keep, dis, F32(fr.FLT_MIN)), np.where(keep, ids, -1)
@@ -564,7 +524,7 @@ def test_scratch_corpus_reuse_matches_fresh_corpora():
         assert lib().b200_thread_release() == 0
 
 
-# ------------------------------------------------------------------ 10. refusals
+# ------------------------------------------------------------------ 9. refusals
 def test_out_of_limit_k_is_refused_before_any_launch():
     rng = np.random.default_rng(1)
     y = rng.standard_normal((500, 64)).astype(F32)

@@ -274,13 +274,13 @@ def test_cooperative_tile_merge_unit():
     assert r.returncode == 0 and "COOP MERGE OK" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
 
 
-def test_append_list_unit():
-    """tests/cuda/list_append_test.cu drives the per-thread top-k list of the tensor-core epilogues (gemm_common.cuh) in rescan and
-    append form through epilogue_chunk + list_publish: 64 (k, mode, distribution) cases x 128 lists against std::sort, ties included."""
+def test_list_topk_unit():
+    """tests/cuda/list_topk_test.cu drives the per-thread top-k list of the tensor-core epilogues (gemm_common.cuh) in rescan and
+    tournament form through epilogue_chunk + list_publish: 64 (k, form, distribution) cases x 128 lists against std::sort, ties included."""
     import os
     import subprocess
-    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "cuda", "list_append_test")
+    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "cuda", "list_topk_test")
     if not os.path.exists(exe):
-        pytest.skip("list_append_test not built (run __graft_entry__.build())")
+        pytest.skip("list_topk_test not built (run __graft_entry__.build())")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0 and "0 mismatching lists" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]

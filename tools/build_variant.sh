@@ -1,6 +1,6 @@
 #!/bin/bash
-# A/B build of libb200search.so with extra compile-time defines, next to the default build:
-#   tools/build_variant.sh coop17 "-DB200_LIST_COOP_MIN_K=17"   ->  build_variants/libb200search_coop17.so
+# A/B build of libb200search.so with extra nvcc flags (or none: the sources as they stand), next to the default build:
+#   tools/build_variant.sh ptxas_o1 "-Xptxas -O1"   ->  build_variants/libb200search_ptxas_o1.so
 # Use with B200_LIB_PATH=build_variants/libb200search_<name>.so python bench.py --headline-only
 set -e
 name=$1; extra=$2

@@ -108,12 +108,18 @@ int b200_corpus_adopt_device(b200_corpus *c, const void *device_rows, int64_t n)
 int b200_corpus_size(const b200_corpus *c, int64_t *out_rows);
 int b200_corpus_free(b200_corpus *c);
 
-/* search with host queries/results (H2D of queries and D2H of results inside the call) */
+/* search with host queries/results (H2D of queries and D2H of results inside the call).
+ * Pre-filtered exact search: with alive_bits given, this call (and b200_flat_knn, b200_binary_knn, b200_part_scan, and
+ * b200_index_search on FLAT / BINARYFLAT / small-part fallback / exact_batch=1) counts the bitmap's set bits on the host.
+ * When the filter keeps few enough rows (see b200_corpus_set_prefilter) only those rows are copied into a compact scratch
+ * corpus and scored; the result is byte for byte the full scan's, and the cost follows the rows kept, not the corpus size. */
 int b200_corpus_search(b200_corpus *c, const float *queries, int64_t nq, int k, const uint8_t *alive_bits /*nullable*/,
                        float *out_dis, int64_t *out_ids);
 /* same, queries and results in device memory, asynchronous on `stream` (a cudaStream_t
  * passed as void*; NULL = the corpus' own stream followed by a synchronise).
- * id_offset is added to every returned id (shard base for multi-GPU merges). */
+ * id_offset is added to every returned id (shard base for multi-GPU merges).
+ * This call, b200_index_search_device and the b200_sharded_* calls always scan the whole corpus under a filter: choosing
+ * the pre-filtered path needs the count of kept rows on the host, which would cost the synchronise they promise not to do. */
 int b200_corpus_search_device(b200_corpus *c, const float *d_queries, int64_t nq, int k,
                               const uint8_t *d_alive_bits /*nullable*/, int64_t id_offset, float *d_out_dis,
                               int64_t *d_out_ids, void *stream);
@@ -124,6 +130,17 @@ int b200_corpus_search_device(b200_corpus *c, const float *d_queries, int64_t nq
  * Auto on a binary corpus: the b1 kernel when the rows are a multiple of 16 bytes (d < 2^24 bits) and the batch has at
  * least ceil(20480 / row_bytes^2) queries (2 at 1024 bits, 20 at 256 bits), else the scan. */
 int b200_corpus_set_path(b200_corpus *c, int path);
+/* Pre-filtered exact search (tests, A/B measurements; production leaves 0):
+ *   0 auto: the gathered path when the filter keeps at most a measured share of the rows of a large enough corpus;
+ *   1 never: always the full scan that masks the filtered rows;
+ *   2 whenever a filter is given and the compact copy fits the budget.
+ * Every mode keeps the compact copy within 1/8 of the corpus' row bytes and 1 GiB; beyond that the full scan runs. */
+int b200_corpus_set_prefilter(b200_corpus *c, int mode);
+/* rows the last search on this corpus scored: its size after a full scan, the kept rows after a pre-filtered one */
+int b200_corpus_last_rows_scored(b200_corpus *c, int64_t *rows);
+/* the same for the last corpus search the CALLING THREAD ran, whatever corpus it was: the per-thread scratch corpus of
+ * b200_flat_knn / b200_binary_knn / b200_part_scan, or the rows of an index behind the exact paths of b200_index_search */
+int b200_thread_last_rows_scored(int64_t *rows);
 /* which kernel the last search on this corpus launched (so a test can prove it exercised the variant it meant to) */
 #define B200_KERNEL_SCAN 1 /* flat_scan_kernel, or binary_scan_kernel on binary corpora */
 #define B200_KERNEL_GEMM_BF16 2   /* gemm_topk_kernel<BF16> (cta_group and pairs_per_cluster report 1) */
@@ -229,7 +246,9 @@ int b200_index_info(const b200_index *ix, int64_t *n, int *nlist, int *m, int *u
  * "exact_batch=1" in `params` answers by an exact pass over the fp32 rows instead (recall 1).
  * Tuning / A-B switches, also in `params` (defaults are chosen from the batch shape): "pages_per_chunk=N" (pages of a list one work
  * item streams), "shared_bound=0" (do not share a per-query bound between the work items of a launch), "coarse_path=1|2|3" (centroid
- * probe by the scan kernel / the tensor-core top-k / score tiles + warp select; default 3 for nprobe > 8). */
+ * probe by the scan kernel / the tensor-core top-k / score tiles + warp select; default 3 for nprobe > 8), "prefilter=0|1|2" (exact
+ * paths of b200_index_search only -- FLAT, BINARYFLAT, the small-part fallback, exact_batch=1: as b200_corpus_set_prefilter;
+ * the list scans of the IVF types are not affected). */
 int b200_index_search(b200_index *ix, const float *queries, int64_t nq, int k, const char *params, int first_stage_only,
                       const uint8_t *alive_bits /*nullable*/, float *out_dis, int64_t *out_ids, int64_t *out_num_candidates);
 /* same with device buffers, asynchronous on `stream` (NULL = the index's own stream, synchronised); id_offset is added to

@@ -17,6 +17,8 @@ namespace b200 {
 
 thread_local std::string g_error;
 thread_local int64_t g_launches = 0;
+// rows the last corpus search launched on this thread scored (b200_thread_last_rows_scored)
+static thread_local int64_t t_last_rows_scored = 0;
 
 void set_error(const std::string &msg) { g_error = msg; }
 int fail(int code, const std::string &msg) {
@@ -99,6 +101,10 @@ struct b200_corpus {
     std::mutex mu;
     // workspaces
     DevBuf w_raw, w_q32, w_qbf, w_qlo, w_qnorm, w_pk, w_pi, w_lk, w_li, w_alive, w_odis, w_oids, w_stage, w_prog;
+    // pre-filtered search (prefilter.cu): kept row ids, compaction scratch, compact rows (+ a row of slack), their side arrays
+    DevBuf w_pf_ids, w_pf_tmp, w_pf_rows, w_pf_side;
+    int prefilter = 0;             // b200_corpus_set_prefilter: 0 auto | 1 never | 2 whenever the compact copy fits the budget
+    int64_t last_rows_scored = 0;  // rows the last search scored: n after a full scan, the kept rows after a gathered one
     // fused single-launch path of the host entry point (small batches, scan kernel): mapped pinned staging + counters
     void *h_pin = nullptr;         // [queries 8 * d fp32 | dis 8 * k | ids 8 * k | flag]
     size_t h_pin_bytes = 0;
@@ -419,7 +425,7 @@ extern "C" int b200_corpus_free(b200_corpus *c) {
     if (c->h_pin) cudaFreeHost(c->h_pin);
     if (c->d_tickets) cudaFree(c->d_tickets);
     for (DevBuf *b : {&c->w_raw, &c->w_q32, &c->w_qbf, &c->w_qlo, &c->w_qnorm, &c->w_pk, &c->w_pi, &c->w_lk, &c->w_li, &c->w_alive,
-                      &c->w_odis, &c->w_oids, &c->w_stage, &c->w_prog})
+                      &c->w_odis, &c->w_oids, &c->w_stage, &c->w_prog, &c->w_pf_ids, &c->w_pf_tmp, &c->w_pf_rows, &c->w_pf_side})
         b->release();
     for (auto *v : {&c->ev_used, &c->ev_free})
         for (auto &ev : *v) {
@@ -443,13 +449,13 @@ constexpr int64_t kBinaryTensorMinQB2 = 20480;
 // corpus tiles a CTA of gemm_topk_kernel may run ahead of the slowest CTA that streams the same tiles for another query tile
 constexpr int kGemmSyncSlack = 2;
 
-// One launch of gemm_topk_kernel over a chunk of <= 1024 staged queries (gp: operands, side arrays, d_pad and alive set),
+// One launch of gemm_topk_kernel over a chunk of <= 1024 staged queries (gp: operands, side arrays, rows, d_pad and alive set),
 // then the merge of the CTAs' partial lists into rows of k of d_out_dis / d_out_ids.  kernel: B200_KERNEL_GEMM_*.
 static int gemm_chunk(b200_corpus *c, GemmTopkParams &gp, int64_t nq_c, int k, int kernel, int out_mode, const float *q_add,
                       int ip_min_quirk, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
     const int nq_pad = (int)round_up(nq_c, 128);
     const int q_tiles = nq_pad / 128;
-    int grid = gemm_topk_grid(q_tiles, c->n, c->sms);
+    int grid = gemm_topk_grid(q_tiles, gp.n, c->sms);
     grid = (grid / q_tiles) * q_tiles;
     if (grid < q_tiles) grid = q_tiles;
     B200_TRY(c->w_pk.reserve((size_t)grid * 128 * k * 4));
@@ -462,7 +468,6 @@ static int gemm_chunk(b200_corpus *c, GemmTopkParams &gp, int64_t nq_c, int k, i
         gp.list_keys_gmem = c->w_lk.as<float>();
         gp.list_ids_gmem = c->w_li.as<uint32_t>();
     }
-    gp.n = c->n;
     gp.nq_pad = nq_pad;
     gp.nq_valid = (int)nq_c;
     gp.k = k;
@@ -503,40 +508,69 @@ static int gemm_chunk(b200_corpus *c, GemmTopkParams &gp, int64_t nq_c, int k, i
     return B200_OK;
 }
 
+// The path a search of nq queries at this k takes (1 scan, 2 tensor cores) before the empty-corpus and limit checks:
+// the forced one, else the auto choice.
+//
+// Auto on float corpora: when the batch goes to the tensor cores (bf16 rows: bf16 wgmma GEMM; fp32 rows: 3xTF32 split
+// GEMM, same accuracy class as the fp32 FMA scan).  A <= 128-query tensor-core pass reads the corpus once, the scan reads
+// it once per few queries, so the tensor cores take bf16 batches from 2 queries and fp32 batches from 5.  These crossovers
+// were chosen on an earlier GPU and are not re-measured on the H100.  L2 keeps faiss' own switch: below
+// distance_compute_blas_threshold = 20 queries the reference sums exact differences, from 20 up it uses
+// ||x||^2 + ||y||^2 - 2xy like the GEMM kernels do (which cancels badly for far-from-origin data), so L2 batches move to
+// the tensor cores at 20.  Very large k stays on the scan path, whose lists are warp-cooperative.
+static int resolved_path(const b200_corpus *c, int64_t nq, int k) {
+    if (c->path != 0) return c->path;
+    if (c->dtype == B200_DTYPE_BIN) {
+        // The tensor-core path loads rows with TMA (16-byte row stride) and keeps AND counts and keys exact in fp32 (< 2^24 bits).
+        const bool tc_rows = c->row_bytes % 16 == 0, tc_exact = c->d < (1 << 24);
+        return (tc_rows && tc_exact && nq >= ceil_div(kBinaryTensorMinQB2, c->row_bytes * c->row_bytes)) ? 2 : 1;
+    }
+    const int64_t min_nq = c->metric == B200_METRIC_L2 ? 20 : (c->dtype == B200_DTYPE_BF16 ? 2 : 5);
+    return (nq >= min_nq && k <= (c->dtype == B200_DTYPE_BF16 ? 1024 : 256)) ? 2 : 1;
+}
+
+// The rows a search scores: the corpus itself, or the compact copy of the rows a filter keeps (search_gathered).
+struct RowsView {
+    const void *data;
+    int64_t n;
+    const float *row_scale, *row_bias;
+};
+static RowsView full_rows(const b200_corpus *c) { return {c->data, c->n, c->row_scale, c->row_bias}; }
+
 // ------------------------------------------------------------------------------------
 // search core: everything on device, asynchronous on `s`
-// d_queries: raw device fp32 [nq][d] (or bytes [nq][d/8] for binary corpora)
+// d_queries: raw device fp32 [nq][d] (or bytes [nq][d/8] for binary corpora); rows: what is scored (r.n rows of the
+// corpus' dtype and layout); ids are row indices of r plus id_offset
 // ------------------------------------------------------------------------------------
-static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k, const uint8_t *d_alive, int64_t id_offset,
-                       int ip_min_quirk, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
+static int search_core(b200_corpus *c, const RowsView &r, const void *d_queries, int64_t nq, int k, const uint8_t *d_alive,
+                       int64_t id_offset, int ip_min_quirk, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
     if (k <= 0) return fail(B200_ERR_INVALID, "k must be positive");
     if (nq == 0) return B200_OK;
-    if (c->n >= (int64_t)0xffffffffll) return fail(B200_ERR_UNSUPPORTED, "corpus shards are limited to 2^32 - 1 rows");
+    if (r.n >= (int64_t)0xffffffffll) return fail(B200_ERR_UNSUPPORTED, "corpus shards are limited to 2^32 - 1 rows");
     const int sms = c->sms;
+    c->last_rows_scored = t_last_rows_scored = r.n;
 
     if (c->dtype == B200_DTYPE_BIN) {
         if (k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 not supported on the binary scan path");
-        // The tensor-core path loads rows with TMA (16-byte row stride) and keeps AND counts and keys exact in fp32 (< 2^24 bits).
         const bool tc_rows = c->row_bytes % 16 == 0, tc_exact = c->d < (1 << 24);
-        int path = c->path;
-        if (path == 0) path = (tc_rows && tc_exact && nq >= ceil_div(kBinaryTensorMinQB2, c->row_bytes * c->row_bytes)) ? 2 : 1;
+        int path = resolved_path(c, nq, k);
         if (path == 2 && !tc_rows)
             return fail(B200_ERR_UNSUPPORTED, "binary tensor-core path needs rows of a multiple of 16 bytes (d % 128 == 0 bits); "
                                               "this corpus has " + std::to_string(c->row_bytes) + "-byte rows");
         if (path == 2 && !tc_exact) return fail(B200_ERR_UNSUPPORTED, "binary tensor-core path needs d < 2^24 bits");
-        if (c->n == 0) path = 1;
+        if (r.n == 0) path = 1;
         const bool jaccard = c->metric == B200_METRIC_JACCARD;
         if (path == 1) {
-            int blocks_x = (int)std::min<int64_t>(std::max<int64_t>(1, ceil_div(c->n, 256)), std::max<int64_t>(1, (2 * sms) / std::max<int64_t>(1, std::min<int64_t>(nq, 2 * sms))));
+            int blocks_x = (int)std::min<int64_t>(std::max<int64_t>(1, ceil_div(r.n, 256)), std::max<int64_t>(1, (2 * sms) / std::max<int64_t>(1, std::min<int64_t>(nq, 2 * sms))));
             B200_TRY(c->w_pk.reserve((size_t)nq * blocks_x * k * 4));
             B200_TRY(c->w_pi.reserve((size_t)nq * blocks_x * k * 4));
             BinaryScanParams bp{};
-            bp.corpus = reinterpret_cast<const uint8_t *>(c->data);
+            bp.corpus = reinterpret_cast<const uint8_t *>(r.data);
             bp.queries = reinterpret_cast<const uint8_t *>(d_queries);
             bp.alive = d_alive;
             bp.part_keys = c->w_pk.as<float>();
             bp.part_ids = c->w_pi.as<uint32_t>();
-            bp.n = c->n;
+            bp.n = r.n;
             bp.nq = nq;
             bp.nbytes = c->d_pad;
             bp.k = k;
@@ -576,9 +610,10 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
             B200_TRY(c->w_qnorm.reserve((size_t)nq_pad * 4));
             B200_CUDA_OK(launch_popc_rows(c->w_qbf.as<uint8_t>(), c->row_bytes, nq_c, c->w_qnorm.as<float>(), s));
             GemmTopkParams gp{};
-            gp.corpus_bf16 = c->data;
+            gp.corpus_bf16 = r.data;
             gp.queries_bf16 = c->w_qbf.p;
-            gp.row_bias = c->row_bias;
+            gp.row_bias = r.row_bias;
+            gp.n = r.n;
             gp.scale_const = jaccard ? 1.f : -2.f;
             gp.alive = d_alive;
             gp.q_popc = jaccard ? c->w_qnorm.as<float>() : nullptr;
@@ -590,19 +625,8 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
         return B200_OK;
     }
 
-    int path = c->path;
-    // auto: when the batch goes to the tensor cores (bf16 rows: bf16 wgmma GEMM; fp32 rows: 3xTF32 split GEMM, same
-    // accuracy class as the fp32 FMA scan).  A <= 128-query tensor-core pass reads the corpus once, the scan reads it once
-    // per few queries, so the tensor cores take bf16 batches from 2 queries and fp32 batches from 5.  These crossovers were
-    // chosen on an earlier GPU and are not re-measured on the H100.  L2 keeps faiss' own switch: below distance_compute_blas_threshold = 20 queries the
-    // reference sums exact differences, from 20 up it uses ||x||^2 + ||y||^2 - 2xy like the GEMM kernels do (which
-    // cancels badly for far-from-origin data), so L2 batches move to the tensor cores at 20.  Very large k stays on
-    // the scan path, whose lists are warp-cooperative.
-    if (path == 0) {
-        const int64_t min_nq = c->metric == B200_METRIC_L2 ? 20 : (c->dtype == B200_DTYPE_BF16 ? 2 : 5);
-        path = (nq >= min_nq && k <= (c->dtype == B200_DTYPE_BF16 ? 1024 : 256)) ? 2 : 1;
-    }
-    if (c->n == 0) path = 1;  // nothing to tile: the scan kernel exits at once and the merge emits the empty result
+    int path = resolved_path(c, nq, k);
+    if (r.n == 0) path = 1;  // nothing to tile: the scan kernel exits at once and the merge emits the empty result
     // refuse out-of-limit requests before anything is launched
     if (path == 1 && k > 2048) return fail(B200_ERR_UNSUPPORTED, "k > 2048 not supported on the scan path");
     if (path == 2 && k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 not supported on the GEMM path");
@@ -629,18 +653,18 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
         const int64_t y_tiles = ceil_div(nq, qt);
         const int64_t rows_per_block_step = 8 * (32 / group);
         int64_t bx = std::max<int64_t>(1, (2 * sms) / std::min<int64_t>(y_tiles, 2 * sms));
-        bx = std::min<int64_t>(bx, std::max<int64_t>(1, ceil_div(c->n, rows_per_block_step)));
+        bx = std::min<int64_t>(bx, std::max<int64_t>(1, ceil_div(r.n, rows_per_block_step)));
         const int blocks_x = (int)bx;
         B200_TRY(c->w_pk.reserve((size_t)nq * blocks_x * k * 4));
         B200_TRY(c->w_pi.reserve((size_t)nq * blocks_x * k * 4));
         ScanParams sp{};
-        sp.corpus = c->data;
+        sp.corpus = r.data;
         sp.queries = q32;
-        sp.row_scale = c->metric == B200_METRIC_COSINE ? c->row_scale : nullptr;
+        sp.row_scale = c->metric == B200_METRIC_COSINE ? r.row_scale : nullptr;
         sp.alive = d_alive;
         sp.part_keys = c->w_pk.as<float>();
         sp.part_ids = c->w_pi.as<uint32_t>();
-        sp.n = c->n;
+        sp.n = r.n;
         sp.nq = nq;
         sp.row_bytes = c->row_bytes;
         sp.d_pad = c->d_pad;
@@ -700,12 +724,13 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
             q_add = c->w_qnorm.as<float>();
         }
         GemmTopkParams gp{};
-        gp.corpus_bf16 = c->data;
+        gp.corpus_bf16 = r.data;
         gp.queries_bf16 = c->w_qbf.p;
         gp.queries_lo = f32 ? c->w_qlo.p : nullptr;
-        gp.row_scale = c->metric == B200_METRIC_COSINE ? c->row_scale : nullptr;
+        gp.row_scale = c->metric == B200_METRIC_COSINE ? r.row_scale : nullptr;
         gp.scale_const = c->metric == B200_METRIC_L2 ? -2.f : -1.f;
-        gp.row_bias = c->metric == B200_METRIC_L2 ? c->row_bias : nullptr;
+        gp.row_bias = c->metric == B200_METRIC_L2 ? r.row_bias : nullptr;
+        gp.n = r.n;
         gp.alive = d_alive;
         gp.d_pad = c->d_pad;
         const int out_mode = c->metric == B200_METRIC_L2 ? kOutAddQ : c->metric == B200_METRIC_IP ? kOutNeg : kOutCosQ;
@@ -714,7 +739,7 @@ static int search_core(b200_corpus *c, const void *d_queries, int64_t nq, int k,
         // L2: the winners' distances from the direct difference form (the expanded form above only RANKS; it cancels for
         // data far from the origin).  The query operand is what the caller passed (fp32), the rows what is stored.
         if (c->metric == B200_METRIC_L2 && k <= 1024 && c->rescore_l2)
-            B200_CUDA_OK(launch_rescore_l2(c->data, c->dtype == B200_DTYPE_BF16, c->row_bytes, c->d_pad, q32 + qb * c->d_pad, nq_c, id_offset, k,
+            B200_CUDA_OK(launch_rescore_l2(r.data, c->dtype == B200_DTYPE_BF16, c->row_bytes, c->d_pad, q32 + qb * c->d_pad, nq_c, id_offset, k,
                                            d_out_dis + qb * k, d_out_ids + qb * k, s));
     }
     return B200_OK;
@@ -728,8 +753,137 @@ extern "C" int b200_corpus_search_device(b200_corpus *c, const float *d_queries,
     std::lock_guard<std::mutex> lk(c->mu);
     B200_CUDA_OK(cudaSetDevice(c->device));
     cudaStream_t s = stream ? reinterpret_cast<cudaStream_t>(stream) : c->stream;
-    B200_TRY(search_core(c, d_queries, nq, k, d_alive_bits, id_offset, 0, d_out_dis, d_out_ids, s));
+    B200_TRY(search_core(c, full_rows(c), d_queries, nq, k, d_alive_bits, id_offset, 0, d_out_dis, d_out_ids, s));
     if (!stream) B200_CUDA_OK(cudaStreamSynchronize(s));
+    return B200_OK;
+}
+
+// ------------------------------------------------------------------------------------
+// Pre-filtered exact search (prefilter.cu).  When the host holds the filter bitmap, its set bits are counted first; a
+// filter that keeps few enough rows has them compacted and copied to the corpus' scratch, the unchanged kernels score that
+// compact corpus, and the ids are mapped back.  The answer is the full scan's, byte for byte; only the rows read change.
+// ------------------------------------------------------------------------------------
+// Measured with tools/bench_aux.py prefilter on an H100 80GB HBM3 at a 400 W power limit, 2026-10-16 (k = 10, call time of
+// the gathered path against the full masked scan of the same search; DESIGN.md section 7).
+// Auto takes the gathered path when the filter keeps at most this share of the rows.  Scan path (float rows, nq = 1): 2.5x
+// faster at a 5 % share on 10 M x 768 bf16 rows and 1.6 - 1.7x on 2 M x 768 fp32 rows; 1.0 - 1.1x at 10 % (fp32; the bf16
+// copy is over the budget there).  The crossover lies above 5 %; auto stops there.
+constexpr double kPrefilterMaxShareScan = 0.05;
+// Tensor-core path (bf16, 3xTF32 and b1 kernels): faster at every measured share that fits the budget below (2.3x for
+// 10 M x 1024-bit rows at nq = 16 and 10 %, 7.5 - 7.6x for 2 M x 768 fp32 at nq = 1024 and 10 %), so the budget decides.
+constexpr double kPrefilterMaxShareTensor = 0.125;
+// The binary scan kernel tests the alive bit before it loads a row, so its full scan already reads little of a sparse
+// filter's corpus: the gathered path was 0.65 - 0.95x as fast at 11 of the 12 measured points (10 M x 1024 bits, nq = 1;
+// 1.16x at one).  Auto leaves that path alone.
+// Corpora below this many row bytes are not pre-filtered by auto: at 768-d fp32 and nq = 1 the gathered path was 0.6 - 0.7x as
+// fast at 65 536 rows (201 MB) and 1.1 - 1.3x faster at 262 144 rows (805 MB) for 0.1 - 1 % shares; the limit lies between.
+constexpr int64_t kPrefilterMinCorpusBytes = 512ll << 20;
+// Every mode takes the gathered path only when the compact copy fits the scratch budget: 1/8 of the corpus' row bytes and
+// at most 1 GiB.  The budget bounds the extra HBM, and with it the compact rows always go through search_core in one piece.
+constexpr int64_t kPrefilterMaxBytes = 1ll << 30;
+
+// The largest number of kept rows for which a search of nq queries at this k takes the gathered path; -1 = never.
+static int64_t prefilter_limit(const b200_corpus *c, int mode, int64_t nq, int k) {
+    if (mode == 1 || c->n == 0) return -1;
+    int64_t lim = std::min<int64_t>(c->n / 8, kPrefilterMaxBytes / c->row_bytes);
+    if (mode == 0) {
+        const int path = resolved_path(c, nq, k);
+        if (c->n * c->row_bytes < kPrefilterMinCorpusBytes || (path != 2 && c->dtype == B200_DTYPE_BIN)) return -1;
+        const double share = path == 2 ? kPrefilterMaxShareTensor : kPrefilterMaxShareScan;
+        lim = std::min<int64_t>(lim, (int64_t)((double)c->n * share));
+    }
+    return lim;
+}
+
+// Set bits among the first n of an LSB-first host bitmap (bits past n in the last byte are ignored).  Stops once the
+// count passes `limit`, so a dense filter costs a few cache lines; the result is then some value > limit.
+template <typename Popc>
+static inline __attribute__((always_inline)) int64_t count_alive_with(const uint8_t *bits, int64_t n, int64_t limit, Popc popc) {
+    const int64_t full = n / 8;
+    int64_t cnt = 0, b = 0;
+    for (; b + 64 <= full; b += 64) {
+        for (int j = 0; j < 64; j += 8) {
+            uint64_t w;
+            memcpy(&w, bits + b + j, 8);
+            cnt += popc(w);
+        }
+        if (cnt > limit) return cnt;
+    }
+    for (; b < full; b++) cnt += popc(bits[b]);
+    if (n % 8) cnt += popc(bits[full] & ((1u << (n % 8)) - 1u));
+    return cnt;
+}
+#if defined(__x86_64__)
+// The default x86-64 target has no POPCNT instruction (__builtin_popcountll becomes a library call, several times slower
+// on a 10 M-bit bitmap); this copy uses it on the CPUs that have it.
+__attribute__((target("popcnt"))) static int64_t count_alive_popcnt(const uint8_t *bits, int64_t n, int64_t limit) {
+    return count_alive_with(bits, n, limit, [](uint64_t w) { return (int64_t)__builtin_popcountll(w); });
+}
+#endif
+static int64_t count_alive(const uint8_t *bits, int64_t n, int64_t limit) {
+#if defined(__x86_64__)
+    if (__builtin_cpu_supports("popcnt")) return count_alive_popcnt(bits, n, limit);
+#endif
+    return count_alive_with(bits, n, limit, [](uint64_t w) { return (int64_t)__builtin_popcountll(w); });
+}
+
+// Scores the `alive` rows the device bitmap keeps (counted on the host) through a compact copy, then maps the ids back to
+// row ids + id_offset.  Asynchronous on s.  The kernels index the compact rows until the map-back, which runs last (after
+// the L2 re-score, which reads the winners' rows by id).
+static int search_gathered(b200_corpus *c, const void *d_queries, int64_t nq, int k, const uint8_t *d_alive, int64_t alive,
+                           int64_t id_offset, int ip_min_quirk, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
+    B200_TRY(c->w_pf_ids.reserve((size_t)alive * 4 + 16));
+    B200_TRY(c->w_pf_tmp.reserve(prefilter_compact_temp_bytes(c->n)));
+    B200_CUDA_OK(launch_prefilter_compact(d_alive, c->n, c->w_pf_ids.as<uint32_t>(), c->w_pf_tmp.p, s));
+    // same layout as the corpus: d_pad rows, 256-byte aligned base (TMA wants 16), a row of slack behind the last row
+    B200_TRY(c->w_pf_rows.reserve((size_t)(alive + 1) * c->row_bytes + 256));
+    const int64_t side_stride = round_up(alive + 1, 64);
+    B200_TRY(c->w_pf_side.reserve((size_t)side_stride * 2 * 4));
+    // only the side arrays search_core reads for this metric: a re-dimensioned per-thread scratch corpus may still hold
+    // arrays of another metric, sized for an earlier, smaller part
+    const float *scale = c->metric == B200_METRIC_COSINE ? c->row_scale : nullptr;
+    const float *bias = c->metric == B200_METRIC_L2 || c->dtype == B200_DTYPE_BIN ? c->row_bias : nullptr;
+    float *cscale = scale ? c->w_pf_side.as<float>() : nullptr, *cbias = bias ? c->w_pf_side.as<float>() + side_stride : nullptr;
+    B200_CUDA_OK(launch_prefilter_gather(c->data, c->row_bytes, scale, bias, c->w_pf_ids.as<uint32_t>(), alive, c->w_pf_rows.p,
+                                         cscale, cbias, s));
+    const RowsView r{c->w_pf_rows.p, alive, cscale, cbias};
+    B200_TRY(search_core(c, r, d_queries, nq, k, nullptr, 0, ip_min_quirk, d_out_dis, d_out_ids, s));
+    B200_CUDA_OK(launch_prefilter_map_ids(c->w_pf_ids.as<uint32_t>(), id_offset, d_out_ids, nq * k, s));
+    return B200_OK;
+}
+
+namespace b200 {
+// Exact search of a resident corpus for the index layer (FLAT, BINARYFLAT, the small-part fallback, exact_batch=1): as
+// b200_corpus_search_device on the stream s, plus the host copy of the bitmap (nullable) and a prefilter mode, so that the
+// gathered path can be chosen.
+int corpus_search_exact(b200_corpus *c, const void *d_queries, int64_t nq, int k, const uint8_t *d_alive, const uint8_t *h_alive,
+                        int prefilter_mode, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
+    std::lock_guard<std::mutex> lk(c->mu);
+    B200_CUDA_OK(cudaSetDevice(c->device));
+    const int64_t limit = h_alive && d_alive ? prefilter_limit(c, prefilter_mode, nq, k) : -1;
+    const int64_t alive = limit >= 0 ? count_alive(h_alive, c->n, limit) : -1;
+    if (alive >= 0 && alive <= limit) return search_gathered(c, d_queries, nq, k, d_alive, alive, id_offset, 0, d_out_dis, d_out_ids, s);
+    return search_core(c, full_rows(c), d_queries, nq, k, d_alive, id_offset, 0, d_out_dis, d_out_ids, s);
+}
+}  // namespace b200
+
+extern "C" int b200_corpus_set_prefilter(b200_corpus *c, int mode) {
+    if (!c || mode < 0 || mode > 2) return fail(B200_ERR_INVALID, "prefilter mode must be 0 (auto), 1 (never) or 2 (always)");
+    std::lock_guard<std::mutex> lk(c->mu);
+    c->prefilter = mode;
+    return B200_OK;
+}
+
+extern "C" int b200_corpus_last_rows_scored(b200_corpus *c, int64_t *rows) {
+    if (!c || !rows) return fail(B200_ERR_INVALID, "null argument");
+    std::lock_guard<std::mutex> lk(c->mu);
+    *rows = c->last_rows_scored;
+    return B200_OK;
+}
+
+extern "C" int b200_thread_last_rows_scored(int64_t *rows) {
+    if (!rows) return fail(B200_ERR_INVALID, "null argument");
+    *rows = t_last_rows_scored;
     return B200_OK;
 }
 
@@ -839,6 +993,7 @@ static int search_host_fused(b200_corpus *c, const float *queries, int64_t nq, i
     B200_CUDA_OK(launch_flat_scan(sp, qt, blocks_x, s));
     timing_end(c, s, ev);
     c->last_kernel = B200_KERNEL_SCAN; c->last_cg = 0; c->last_mc = 0; c->last_grid = blocks_x;
+    c->last_rows_scored = t_last_rows_scored = c->n;
     // wait for the flag; look at the stream now and then so that a failed launch cannot hang the caller
     for (uint64_t spin = 1;; spin++) {
         if (*h_flag == sp.done_value) break;
@@ -867,7 +1022,11 @@ static int search_host(b200_corpus *c, const void *queries, int64_t nq, int k, c
     if (nq == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(c->mu);
     B200_CUDA_OK(cudaSetDevice(c->device));
-    {
+    // a selective filter: score only the rows it keeps (the count is taken before the fused path is considered)
+    const int64_t limit = alive_bits ? prefilter_limit(c, c->prefilter, nq, k) : -1;
+    const int64_t alive = limit >= 0 ? count_alive(alive_bits, c->n, limit) : -1;
+    const bool gathered = alive >= 0 && alive <= limit;
+    if (!gathered) {
         bool done = false;
         B200_TRY(search_host_fused(c, reinterpret_cast<const float *>(queries), nq, k, alive_bits, ip_min_quirk, out_dis, out_ids, &done));
         if (done) return B200_OK;
@@ -885,7 +1044,10 @@ static int search_host(b200_corpus *c, const void *queries, int64_t nq, int k, c
         B200_CUDA_OK(cudaMemcpyAsync(c->w_alive.p, alive_bits, ab, cudaMemcpyHostToDevice, s));
         d_alive = c->w_alive.as<uint8_t>();
     }
-    B200_TRY(search_core(c, c->w_stage.p, nq, k, d_alive, 0, ip_min_quirk, c->w_odis.as<float>(), c->w_oids.as<int64_t>(), s));
+    if (gathered)
+        B200_TRY(search_gathered(c, c->w_stage.p, nq, k, d_alive, alive, 0, ip_min_quirk, c->w_odis.as<float>(), c->w_oids.as<int64_t>(), s));
+    else
+        B200_TRY(search_core(c, full_rows(c), c->w_stage.p, nq, k, d_alive, 0, ip_min_quirk, c->w_odis.as<float>(), c->w_oids.as<int64_t>(), s));
     B200_CUDA_OK(cudaMemcpyAsync(out_dis, c->w_odis.p, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaMemcpyAsync(out_ids, c->w_oids.p, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));

@@ -1059,6 +1059,8 @@ namespace b200 {
 const void *corpus_device_rows(const b200_corpus *c);
 int corpus_normalize_rows(b200_corpus *c);
 int corpus_append_device(b200_corpus *c, const float *d_rows, int64_t n, cudaStream_t s);
+int corpus_search_exact(b200_corpus *c, const void *d_queries, int64_t nq, int k, const uint8_t *d_alive, const uint8_t *h_alive,
+                        int prefilter_mode, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s);
 }
 
 static int parse_int_param(const char *json, const char *key, int defv) {
@@ -1953,20 +1955,23 @@ __global__ void cosine_finish_kernel(const float *q, int64_t nq, int d, int d_pa
     dis[i] = ids[i] >= 0 ? 1.f - dis[i] : FLT_MAX;
 }
 
-// The whole search on the device, asynchronous on s.  d_queries: fp32 [nq][d]; outputs [nq][k].
+// The whole search on the device, asynchronous on s.  d_queries: fp32 [nq][d]; outputs [nq][k].  h_alive: the host copy of
+// d_alive when the caller has one (the exact paths may then score only the rows it keeps), else null.
 static int search_device_locked(b200_index *ix, const float *d_queries, int64_t nq, int k, const char *params, int first_stage_only,
-                                const uint8_t *d_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, int64_t *out_num_candidates,
-                                cudaStream_t s) {
+                                const uint8_t *d_alive, const uint8_t *h_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids,
+                                int64_t *out_num_candidates, cudaStream_t s) {
     if (out_num_candidates) *out_num_candidates = k;
     if (nq == 0) return B200_OK;
     const int force_exact = parse_int_param(params, "exact_batch", 0);
+    const int prefilter = parse_int_param(params, "prefilter", 0);   // A/B: 1 never, 2 whenever it fits (exact paths only)
+    if (prefilter < 0 || prefilter > 2) return fail(B200_ERR_INVALID, "prefilter must be 0 (auto), 1 (never) or 2 (always)");
     if (pq_uses_lut(ix) && force_exact != 1 && k <= 1024) {
         // the look-up scan's tables are nq x M KB: a larger batch runs as consecutive query sub-batches through the whole
         // search (every query's answer depends on that query alone, so the results are those of one batch)
         const int64_t qmax = std::max<int64_t>(1, kPqLutScratchBytes / ((int64_t)ix->m * 1024));
         if (nq > qmax) {
             for (int64_t q0 = 0; q0 < nq; q0 += qmax)
-                B200_TRY(search_device_locked(ix, d_queries + q0 * ix->d, std::min(qmax, nq - q0), k, params, first_stage_only, d_alive, id_offset,
+                B200_TRY(search_device_locked(ix, d_queries + q0 * ix->d, std::min(qmax, nq - q0), k, params, first_stage_only, d_alive, h_alive, id_offset,
                                               d_out_dis + q0 * k, d_out_ids + q0 * k, out_num_candidates, s));
             return B200_OK;
         }
@@ -1974,7 +1979,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     if (ix->binary) {
         // binary queries are bytes [nq][d / 8]; list rows are exact, so refine_factor / keep_raw / first_stage_only change nothing
         if (force_exact == 1) return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available on binary indexes (their lists are exact)");
-        if (!ix->use_ivf) return b200_corpus_search_device(ix->raw, d_queries, nq, k, d_alive, id_offset, d_out_dis, d_out_ids, s);
+        if (!ix->use_ivf) return corpus_search_exact(ix->raw, d_queries, nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s);
     } else {
         B200_TRY(prepare_queries_device(ix, d_queries, nq, s));
     }
@@ -1985,7 +1990,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
         if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
         else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
-        B200_TRY(b200_corpus_search_device(ix->raw, ix->w_qraw.as<float>(), nq, k, d_alive, id_offset, d_out_dis, d_out_ids, s));
+        B200_TRY(corpus_search_exact(ix->raw, ix->w_qraw.as<float>(), nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s));
         if (ix->metric == B200_METRIC_COSINE) {
             cosine_finish_kernel<<<(unsigned)ceil_div(nq * k, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, k, d_out_dis, d_out_ids);
             g_launches++;
@@ -2311,7 +2316,7 @@ extern "C" int b200_index_search_device(b200_index *ix, const float *d_queries, 
     B200_CUDA_OK(cudaSetDevice(ix->device));
     timing_collect(ix);
     cudaStream_t s = stream ? reinterpret_cast<cudaStream_t>(stream) : ix->stream;
-    B200_TRY(search_device_locked(ix, d_queries, nq, k, params, first_stage_only, d_alive_bits, id_offset, d_out_dis, d_out_ids, nullptr, s));
+    B200_TRY(search_device_locked(ix, d_queries, nq, k, params, first_stage_only, d_alive_bits, nullptr, id_offset, d_out_dis, d_out_ids, nullptr, s));
     if (!stream) B200_CUDA_OK(cudaStreamSynchronize(s));
     return B200_OK;
 }
@@ -2339,7 +2344,7 @@ extern "C" int b200_index_search(b200_index *ix, const float *queries, int64_t n
     }
     float *r_d = ix->w_cand.as<float>();
     int64_t *r_i = reinterpret_cast<int64_t *>(reinterpret_cast<char *>(ix->w_cand.p) + (size_t)round_up(nq * k * 4, 8));
-    B200_TRY(search_device_locked(ix, ix->w_host_q.as<float>(), nq, k, params, first_stage_only, d_alive, 0, r_d, r_i, out_num_candidates, s));
+    B200_TRY(search_device_locked(ix, ix->w_host_q.as<float>(), nq, k, params, first_stage_only, d_alive, alive_bits, 0, r_d, r_i, out_num_candidates, s));
     B200_CUDA_OK(cudaMemcpyAsync(out_dis, r_d, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaMemcpyAsync(out_ids, r_i, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));

@@ -120,6 +120,18 @@ cudaError_t launch_gemm3_topk(const GemmTopkParams &p, int grid, cudaStream_t s,
 // binary rows on the tensor cores (wgmma .b1 AND + popcount): Hamming or Jaccard keys, exact
 cudaError_t launch_gemm_b1_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail);
 
+// ---- pre-filtered exact search (prefilter.cu) -----------------------------------------
+// scratch the compaction of an n-bit bitmap needs (per-word counts, their exclusive scan, CUB storage)
+size_t prefilter_compact_temp_bytes(int64_t n);
+// d_alive: LSB-first bitmap, 4-byte aligned, readable up to the end of its last 32-bit word (bits >= n are ignored) ->
+// d_ids: the ascending row ids of its set bits (as many as it has; the caller counted them)
+cudaError_t launch_prefilter_compact(const uint8_t *d_alive, int64_t n, uint32_t *d_ids, void *temp, cudaStream_t s);
+// out_rows[i] = rows[ids[i]] (row_bytes each), and the same for the side arrays that are not null
+cudaError_t launch_prefilter_gather(const void *rows, int64_t row_bytes, const float *scale, const float *bias, const uint32_t *ids,
+                                    int64_t m, void *out_rows, float *out_scale, float *out_bias, cudaStream_t s);
+// ids[i] = ids[i] >= 0 ? alive_ids[ids[i]] + id_offset : -1
+cudaError_t launch_prefilter_map_ids(const uint32_t *alive_ids, int64_t id_offset, int64_t *ids, int64_t count, cudaStream_t s);
+
 // ---- host ingest (ingest.cu): pageable host memory -> device through a multi-threaded pinned ring; returns a B200_* code
 int staged_h2d(void *dst, const void *src, size_t bytes, int device, cudaStream_t s);
 

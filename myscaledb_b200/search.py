@@ -124,6 +124,17 @@ class Corpus:
         _check(lib().b200_corpus_set_path(self._h, C.c_int(path)))
         return self
 
+    def set_prefilter(self, mode: int):
+        """Pre-filtered exact search: 0 auto, 1 never (full masked scan), 2 whenever the compact copy fits the budget."""
+        _check(lib().b200_corpus_set_prefilter(self._h, C.c_int(mode)))
+        return self
+
+    def last_rows_scored(self):
+        """Rows the last search scored: the corpus size after a full scan, the kept rows after a pre-filtered one."""
+        n = C.c_int64()
+        _check(lib().b200_corpus_last_rows_scored(self._h, C.byref(n)))
+        return n.value
+
     def last_variant(self):
         """(kernel, cta_group, pairs_per_cluster, grid) of the last search: KERNEL_SCAN / _GEMM_BF16 / _GEMM_TS / _GEMM_TF32X3 /
         _GEMM_B1 (binary rows on the tensor cores)."""
@@ -197,6 +208,14 @@ def topk_merge_device_ex(dis_ptr, ids_ptr, n_lists, dis_stride, ids_stride, nq, 
                                            C.c_int64(ids_stride), C.c_int64(nq), C.c_int(k_in), C.c_int(k),
                                            C.c_int(1 if descending else 0), C.c_int(tie_mode), C.c_void_p(out_dis_ptr),
                                            C.c_void_p(out_ids_ptr), C.c_void_p(out_list_ptr or None), C.c_void_p(stream or None)))
+
+
+def thread_last_rows_scored() -> int:
+    """Rows the last corpus search on this thread scored (one-shot calls, exact index paths): the corpus size after a full
+    scan, the kept rows after a pre-filtered one."""
+    n = C.c_int64()
+    _check(lib().b200_thread_last_rows_scored(C.byref(n)))
+    return n.value
 
 
 def launch_count(reset=False) -> int:

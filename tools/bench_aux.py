@@ -2,7 +2,7 @@
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
 workload; results are pasted into DESIGN.md section 7.
-Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide]"""
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [prefilter]"""
 import json
 import os
 import subprocess
@@ -347,8 +347,110 @@ def bench_pq_wide():
             print(json.dumps(pt), flush=True)
 
 
+def alive_bitmap(n, frac, clustered_runs, seed):
+    """LSB-first bitmap keeping round(frac * n) rows (at least 1): uniformly random rows, or runs of up to 4096 contiguous
+    rows at random starts (a tenant's rows are often contiguous)"""
+    rng = np.random.default_rng(seed)
+    m = max(1, int(round(frac * n)))
+    keep = np.zeros(n, bool)
+    if clustered_runs:
+        run, have = min(4096, m), 0
+        while have < m:
+            s = int(rng.integers(0, n - run + 1))
+            e = s + min(run, m - have)
+            have += (e - s) - int(keep[s:e].sum())
+            keep[s:e] = True
+    else:
+        keep[rng.choice(n, m, replace=False)] = True
+    return np.packbits(keep, bitorder="little"), int(keep.sum())
+
+
+def bench_prefilter():
+    """Pre-filtered exact search: per corpus, nq and alive share, the full masked scan (prefilter 1), the gathered path
+    (prefilter 2) and auto (0) alternate after a warm-up round; medians of the dominant kernel's CUDA-event time and of the
+    call's host time, rows scored, and a byte-for-byte comparison of the three outputs.  Corpora are generated on the
+    device (seeded) and adopted.  A second sweep over corpus sizes (nq = 1) places the smallest corpus auto pre-filters."""
+    import torch
+
+    ctx = gpu_context()
+    k = 10
+    fracs = (1e-5, 1e-4, 1e-3, 1e-2, 0.05, 0.1, 0.25)
+    g = torch.Generator(device="cuda").manual_seed(0)
+
+    def dev_float(n, d, dtype):
+        t = torch.empty((n, d), dtype=dtype, device="cuda")
+        for i in range(0, n, 1_000_000):
+            t[i:i + 1_000_000] = torch.randn((min(1_000_000, n - i), d), generator=g, device="cuda", dtype=torch.float32).to(dtype)
+        return t
+
+    def point(c, n, q, frac, clustered_runs, seed, extra):
+        bits, alive = alive_bitmap(n, frac, clustered_runs, seed)
+        reps = 10 if q.shape[0] <= 16 else 5
+        res, kms, wall, rows = {}, {0: [], 1: [], 2: []}, {0: [], 1: [], 2: []}, {}
+        for it in range(reps + 1):            # round 0 warms every mode up and is not timed
+            for mode in (1, 2, 0):
+                c.set_prefilter(mode)
+                c.kernel_time(reset=True)
+                t0 = time.perf_counter()
+                res[mode] = c.search(q, k, alive_bits=bits)
+                t = time.perf_counter() - t0
+                ms, _ = c.kernel_time(reset=True)
+                rows[mode] = c.last_rows_scored()
+                if it:
+                    kms[mode].append(ms)
+                    wall[mode].append(t)
+        same = all(np.array_equal(res[1][1], res[m][1]) and np.array_equal(res[1][0].view(np.uint32), res[m][0].view(np.uint32))
+                   for m in (0, 2))
+        pt = dict(extra, nq=int(q.shape[0]), alive_share=frac, bitmap="runs" if clustered_runs else "random", alive=alive,
+                  outputs_identical=bool(same))
+        for mode, name in ((1, "never"), (2, "always"), (0, "auto")):
+            pt[name] = {"rows_scored": rows[mode], "kernel_ms": round(float(np.median(kms[mode])), 4),
+                        "call_ms": round(1e3 * float(np.median(wall[mode])), 4)}
+        pt["auto_path"] = "gathered" if rows[0] < n else "full"
+        pt["always_speedup_call"] = round(pt["never"]["call_ms"] / pt["always"]["call_ms"], 3)
+        pt["auto_vs_never_call"] = round(pt["auto"]["call_ms"] / pt["never"]["call_ms"], 3)
+        print(json.dumps(pt), flush=True)
+        return pt
+
+    corpora = (("bf16 IP", 10_000_000, 768, S.BF16, b2.IP), ("fp32 IP", 2_000_000, 768, S.F32, b2.IP),
+               ("fp32 L2", 2_000_000, 768, S.F32, b2.L2), ("binary Hamming", 10_000_000, 1024, S.BIN, b2.HAMMING))
+    points = []
+    rng = np.random.default_rng(5)
+    for name, n, d, dtype, metric in corpora:
+        if dtype == S.BIN:
+            rows = torch.randint(0, 256, (n, d // 8), generator=g, device="cuda", dtype=torch.uint8)
+            qs = rng.integers(0, 256, (1024, d // 8), dtype=np.uint8)
+        else:
+            rows = dev_float(n, d, torch.bfloat16 if dtype == S.BF16 else torch.float32)
+            qs = rng.standard_normal((1024, d)).astype(np.float32)
+        torch.cuda.synchronize()
+        c = b2.Corpus(metric, d, dtype=dtype).adopt_device(rows.data_ptr(), n)
+        c.enable_timing(True)
+        for nq in (1, 16, 1024):
+            for frac in fracs:
+                for runs in (False, True):
+                    points.append(point(c, n, qs[:nq], frac, runs, seed=int(frac * 1e6) + nq, extra={"corpus": f"{name} {n} x {d}"}))
+        c.close()
+        del rows
+        torch.cuda.empty_cache()
+    # corpus size sweep: where the extra launches stop paying
+    for n in (16_384, 65_536, 262_144, 1_048_576):
+        rows = dev_float(n, 768, torch.float32)
+        c = b2.Corpus(b2.IP, 768).adopt_device(rows.data_ptr(), n)
+        c.enable_timing(True)
+        q = rng.standard_normal((1, 768)).astype(np.float32)
+        for frac in (1e-3, 1e-2, 0.1):
+            points.append(point(c, n, q, frac, False, seed=n, extra={"corpus": f"fp32 IP {n} x 768 (size sweep)"}))
+        c.close()
+        del rows
+    print(json.dumps({"workload": f"pre-filtered exact search, k={k}", **ctx,
+                      "all_outputs_identical": all(p["outputs_identical"] for p in points),
+                      "auto_never_slower_than_5pct": all(p["auto_vs_never_call"] <= 1.05 for p in points), "points": len(points)}),
+          flush=True)
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
         {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
-         "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide}[w]()
+         "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide, "prefilter": bench_prefilter}[w]()

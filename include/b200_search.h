@@ -198,7 +198,16 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *                               train with B200_ERR_UNSUPPORTED); any other d / M is scanned by table look-up (a per-query
  *                               M x 256 fp32 table of <q_j, codeword>, at any width), which needs M <= 128 (larger M is refused
  *                               at train).  Default M: d / 8 (or d / 4, d / 2, d) up to d = 220; above, d / dsub with dsub the
- *                               smallest divisor of d that is >= 16 and keeps M <= 128 (M = 48 at d = 768, 96 at d = 1536);
+ *                               smallest divisor of d that is >= 16 and keeps M <= 128 (M = 48 at d = 768, 96 at d = 1536).
+ *                               "bit_size=4" (IVFPQ, SCANN and HNSWPQ; other types ignore the key) selects 4-bit codes: 16
+ *                               codewords per sub-quantiser, two codes per byte (code j in byte j / 2, even j in the low
+ *                               nibble), always scanned by table look-up from a per-query M x 16 fp32 table at any d / M
+ *                               (1, 2, 4 and 8 included), which needs M <= 2048 (larger M is refused at train with
+ *                               B200_ERR_UNSUPPORTED).  Default M at 4 bits keeps the code bytes of the 8-bit default: twice
+ *                               the 8-bit default M when that default's sub-vector length is even (M = 96 at d = 768, 24 at
+ *                               d = 96), else the 8-bit default (M = 10 at d = 250).  bit_size=8, or no bit_size, is the
+ *                               8-bit index; any other value is refused at create with B200_ERR_UNSUPPORTED.  4-bit indexes
+ *                               are saved as B2IX v3 (below);
  *   "MSTG"                      closed source upstream; here the two-stage index of SURVEY 2.5 K6: bf16 lists + exact
  *                               fp32 second stage (supportTwoStageSearch, first_stage_only, computeTopDistanceSubset);
  *   "SCANN", "HNSWFLAT", "HNSWSQ", "HNSWPQ"   accepted and SERVED BY THE INVERTED-FILE ENGINE with the payload their
@@ -267,7 +276,9 @@ int b200_index_last_scan(b200_index *ix, int64_t *rows_streamed, int64_t *payloa
 int b200_index_refine(b200_index *ix, const float *queries, int64_t nq, const int64_t *cand_ids, int64_t ncand, int k,
                       float *out_dis, int64_t *out_ids);
 /* VIWithColumnInPart::serialize / load (VIWithDataPart.cpp:451-525, :578-764): one self-describing file
- * ("B2IX" v2; the closed library's .vidx3 payload cannot be reproduced).  load validates every size it derives. */
+ * ("B2IX" v2; the closed library's .vidx3 payload cannot be reproduced).  PQ indexes with 4-bit codes are written as
+ * v3: the v2 layout with the header's reserved word holding the code width (4) and a [M][16][d / M] codebook; every other
+ * index is written as v2.  load accepts both and validates every size it derives. */
 int b200_index_save(b200_index *ix, const char *path);
 int b200_index_load(const char *path, b200_index **out);
 /* the same through the host's own streams (Search::IndexDataFileWriter / Reader over ClickHouse disks,

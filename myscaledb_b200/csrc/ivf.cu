@@ -288,7 +288,7 @@ struct ScatterParams {
     const float *centroids;     // [nlist][d]
     const float *pq;            // [m][256][dsub] fp32 (nearest-centroid search)
     const __nv_bfloat16 *pq_bf16;  // values the scan kernel will see (null: the fp32 ones, table look-up scan)
-    int m, dsub;
+    int m, dsub, pq_bits;          // pq_bits 4: pq is [m][16][dsub], codes two per byte (code j in byte j / 2, even j low)
     uint8_t *codes;
     int code_bytes;
     float *row_bias;
@@ -340,6 +340,37 @@ __global__ void __launch_bounds__(256) scatter_rows_kernel(const ScatterParams p
                     acc = fmaf(v, v, acc);
                 }
                 dst[j] = (uint8_t)code;
+            }
+        } else if (p.pq_bits == 4) {
+            // 4-bit PQ on the residual: lane handles code bytes lane, lane + 32, ..., each holding codes 2b (low nibble) and
+            // 2b + 1 (high nibble); codes past M and the padding bytes stay 0
+            uint8_t *dst = p.codes + (size_t)slot * p.code_bytes;
+            const float *c = p.centroids + (size_t)l * p.d;
+            for (int b = lane; b < p.code_bytes; b += 32) {
+                uint32_t byte = 0;
+                for (int h = 0; h < 2; h++) {
+                    const int j = 2 * b + h;
+                    if (j >= p.m) break;
+                    const float *cb = p.pq + (size_t)j * 16 * p.dsub;
+                    float bd = FLT_MAX;
+                    uint32_t best = 0;
+                    for (int e = 0; e < 16; e++) {
+                        float s = 0.f;
+                        for (int t = 0; t < p.dsub; t++) {
+                            const float u = (x[j * p.dsub + t] - c[j * p.dsub + t]) - cb[e * p.dsub + t];
+                            s = fmaf(u, u, s);
+                        }
+                        if (s < bd) {
+                            bd = s;
+                            best = (uint32_t)e;
+                        }
+                    }
+                    // norm term of the expanded L2 with the fp32 codewords the look-up table is built from: 2 <c, r^> + ||r^||^2
+                    const float *rv = cb + (size_t)best * p.dsub;
+                    for (int t = 0; t < p.dsub; t++) acc = fmaf(rv[t], rv[t] + 2.f * c[j * p.dsub + t], acc);
+                    byte |= best << (4 * h);
+                }
+                dst[b] = (uint8_t)byte;
             }
         } else {
             // PQ on the residual x - centroid[l]: lane handles sub-quantisers lane, lane + 32, ...
@@ -1005,6 +1036,7 @@ struct DevArr {
 struct b200_index {
     int type = IDX_FLAT, metric = B200_METRIC_L2, d = 0, d_pad = 0, d_pad64 = 0;
     int nlist = 0, m = 0, dsub = 0;
+    int pq_bits = 8;                // PQ code width: 8 (256 codewords, one byte per code) or 4 (16 codewords, two codes per byte)
     int default_nprobe = 32, refine_factor = 4;
     int payload = IVF_PRODUCER_TMA;
     int keep_raw = -1;              // -1 auto (yes), 0 no fp32 rows (first-stage distances only), 1 yes
@@ -1097,6 +1129,10 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
     if (bin && !bin_metric) return fail(B200_ERR_INVALID, "binary indexes take HAMMING or JACCARD");
     if (!bin && !float_metric) return fail(B200_ERR_INVALID, "float indexes take L2, IP or COSINE");
     if (bin && (d % 8 != 0 || d > (1 << 16))) return fail(B200_ERR_INVALID, "binary dimension must be a multiple of 8 bits, at most 65536");
+    // PQ code width (IVFPQ, SCANN, HNSWPQ only; the other types ignore the key)
+    const bool pq_type = ty == IDX_IVFPQ || ty == IDX_SCANN || ty == IDX_HNSWPQ;
+    const int pq_bits = pq_type ? parse_int_param(params, "bit_size", 8) : 8;
+    if (pq_bits != 8 && pq_bits != 4) return fail(B200_ERR_UNSUPPORTED, "PQ bit_size must be 8 or 4, got " + std::to_string(pq_bits));
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
@@ -1110,6 +1146,7 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
     ix->d_pad64 = (int)round_up(d, 64);
     ix->nlist = parse_int_param(params, "ncentroids", parse_int_param(params, "nlist", 0));
     ix->m = parse_int_param(params, "M", parse_int_param(params, "m", 0));
+    ix->pq_bits = pq_bits;
     ix->default_nprobe = parse_int_param(params, "nprobe", 32);
     // payload of a list row.  The graph types of the reference (hnswlib) and ScaNN have no graph / anisotropic quantiser
     // here: they are SERVED by the inverted-file engine with the payload their suffix names (recall contract, SURVEY 8c).
@@ -1170,7 +1207,13 @@ extern "C" int b200_index_free(b200_index *ix) {
 
 // PQ sub-vectors the tensor-core decoder takes (d / M = 1, 2, 4, 8); any other d / M is scanned by table look-up
 static bool pq_dsub_decodable(int dsub) { return dsub == 1 || dsub == 2 || dsub == 4 || dsub == 8; }
-static bool pq_uses_lut(const b200_index *ix) { return ix->payload == IVF_PRODUCER_PQ && ix->use_ivf && !pq_dsub_decodable(ix->dsub); }
+// 4-bit codes are always scanned by table look-up (ivf_pq4_sm90.cu), whatever d / M
+static bool pq_uses_lut(const b200_index *ix) {
+    return ix->payload == IVF_PRODUCER_PQ && ix->use_ivf && (ix->pq_bits == 4 || !pq_dsub_decodable(ix->dsub));
+}
+// codewords per sub-quantiser, and the bytes of one code row: one byte per 8-bit code, two 4-bit codes per byte
+static int pq_codewords(int bits) { return bits == 4 ? 16 : 256; }
+static int pq_code_bytes(int m, int bits) { return (int)round_up(bits == 4 ? (m + 1) / 2 : m, 16); }
 
 // the per-query tables of the look-up scan take at most this much scratch; larger batches run in query sub-batches
 constexpr int64_t kPqLutScratchBytes = (int64_t)256 << 20;
@@ -1477,10 +1520,17 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
                 while (d % dsub || d / dsub > 128) dsub++;
                 ix->m = d / dsub;
             }
+            // 4-bit codes: the code bytes of the 8-bit default (twice the sub-quantisers) when its sub-vector splits in two
+            if (ix->pq_bits == 4 && (d / ix->m) % 2 == 0) ix->m *= 2;
         }
         if (d % ix->m) return fail(B200_ERR_INVALID, "PQ M must divide the dimension");
         const int dsub = d / ix->m;
-        if (pq_dsub_decodable(dsub)) {
+        if (ix->pq_bits == 4) {
+            // the 4-bit look-up scan keeps one query's M x 64 B table in shared memory, at any d / M
+            if (!ivf_pq4_fits(ix->m))
+                return fail(B200_ERR_UNSUPPORTED, "4-bit PQ is scanned by table look-up, whose per-query table (M x 64 B) must fit in shared memory: M <= " +
+                                                      std::to_string(ivf_pq4_max_m()) + ", got M = " + std::to_string(ix->m));
+        } else if (pq_dsub_decodable(dsub)) {
             // the tensor-core scan keeps the bf16 codebook (512 B x d) in shared memory beside at least a 2-stage operand ring
             if (!ivf_pq_codebook_fits((int64_t)512 * d)) {
                 int dmax = d;
@@ -1529,10 +1579,11 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
     }
     if (ix->payload == IVF_PRODUCER_PQ) {
         const int m = ix->m, dsub = d / m;   // validated above
+        const int ncw = pq_codewords(ix->pq_bits);
         ix->dsub = dsub;
-        ix->code_bytes = (int)round_up(m, 16);
-        B200_CUDA_OK(cudaMalloc(&ix->d_pq, (size_t)m * 256 * dsub * 4));
-        if (pq_dsub_decodable(dsub)) B200_CUDA_OK(cudaMalloc(&ix->d_pq_bf16, (size_t)m * 256 * dsub * 2));   // the decoder's copy
+        ix->code_bytes = pq_code_bytes(m, ix->pq_bits);
+        B200_CUDA_OK(cudaMalloc(&ix->d_pq, (size_t)m * ncw * dsub * 4));
+        if (!pq_uses_lut(ix)) B200_CUDA_OK(cudaMalloc(&ix->d_pq_bf16, (size_t)m * 256 * dsub * 2));   // the decoder's copy
         // residuals of (a sample of) the training rows, one sub-quantiser at a time
         const int64_t ns = std::min<int64_t>(n, 65536);
         int64_t *d_a = nullptr;
@@ -1556,7 +1607,7 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
             for (int j = 0; j < m && rc == B200_OK; j++) {
                 residual_sub_kernel<<<gridsz(ns * dsub), 256, 0, s>>>(d_samp, ns, d, ix->d_centroids, d_l, d, j, dsub, d_res);
                 g_launches++;
-                rc = kmeans_device(d_res, ns, dsub, dsub, 256, 8, ix->d_pq + (size_t)j * 256 * dsub, s);
+                rc = kmeans_device(d_res, ns, dsub, dsub, ncw, 8, ix->d_pq + (size_t)j * ncw * dsub, s);
             }
         }
         if (rc == B200_OK && ix->d_pq_bf16) {
@@ -1696,6 +1747,7 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     sp.pq_bf16 = ix->d_pq_bf16;
     sp.m = ix->m;
     sp.dsub = ix->dsub;
+    sp.pq_bits = ix->pq_bits;
     sp.codes = reinterpret_cast<uint8_t *>(ix->d_pool);
     sp.code_bytes = ix->code_bytes;
     sp.row_bias = ix->d_row_bias;
@@ -1847,7 +1899,7 @@ extern "C" int b200_index_memory_bytes(const b200_index *ix, uint64_t *out_bytes
         const uint64_t rows = (uint64_t)ix->pool_pages * kPageRows;
         b += (uint64_t)ix->nlist * (ix->binary ? (uint64_t)ix->cent_pad : (uint64_t)ix->d * 4) + rows * (payload_row_bytes(ix) + 4 + (ix->d_row_bias ? 4 : 0)) +
              (uint64_t)ix->pool_pages * 12;
-        if (ix->d_pq) b += (uint64_t)ix->m * 256 * ix->dsub * (ix->d_pq_bf16 ? 6 : 4);   // fp32 codebook (+ the decoder's bf16 copy)
+        if (ix->d_pq) b += (uint64_t)ix->m * pq_codewords(ix->pq_bits) * ix->dsub * (ix->d_pq_bf16 ? 6 : 4);   // fp32 codebook (+ the decoder's bf16 copy)
     }
     *out_bytes = b;
     return B200_OK;
@@ -1966,9 +2018,10 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     const int prefilter = parse_int_param(params, "prefilter", 0);   // A/B: 1 never, 2 whenever it fits (exact paths only)
     if (prefilter < 0 || prefilter > 2) return fail(B200_ERR_INVALID, "prefilter must be 0 (auto), 1 (never) or 2 (always)");
     if (pq_uses_lut(ix) && force_exact != 1 && k <= 1024) {
-        // the look-up scan's tables are nq x M KB: a larger batch runs as consecutive query sub-batches through the whole
-        // search (every query's answer depends on that query alone, so the results are those of one batch)
-        const int64_t qmax = std::max<int64_t>(1, kPqLutScratchBytes / ((int64_t)ix->m * 1024));
+        // the look-up scan's tables are nq x M KB (4-bit codes: nq x M x 64 B): a larger batch runs as consecutive query
+        // sub-batches through the whole search (every query's answer depends on that query alone, so the results are those of
+        // one batch)
+        const int64_t qmax = std::max<int64_t>(1, kPqLutScratchBytes / ((int64_t)ix->m * pq_codewords(ix->pq_bits) * 4));
         if (nq > qmax) {
             for (int64_t q0 = 0; q0 < nq; q0 += qmax)
                 B200_TRY(search_device_locked(ix, d_queries + q0 * ix->d, std::min(qmax, nq - q0), k, params, first_stage_only, d_alive, h_alive, id_offset,
@@ -2130,7 +2183,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     search_plan_kernel<<<1, 1024, 0, s>>>(pl);
     g_launches++;
     // ---- gather queries, per-pair bookkeeping
-    const bool lut = pq_uses_lut(ix);
+    const bool lut = pq_uses_lut(ix), pq4 = lut && ix->pq_bits == 4;
     const size_t qrow_bytes = ix->binary ? (size_t)ix->row_pad : (size_t)ix->d_pad64 * 2;
     if (!lut) {   // the table look-up scan reads no gathered query rows
         B200_TRY(ix->w_qbuf.reserve(((size_t)n_pairs + 128) * qrow_bytes));
@@ -2175,8 +2228,9 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         pair_fill_kernel<<<(unsigned)ceil_div(n_pairs * 32, 256), 256, 0, s>>>(pf);
         g_launches++;
         if (lut) {   // the per-query tables T[q][j][e] = <q_j, codebook_j[e]> (fp32)
-            B200_TRY(ix->w_lut.reserve((size_t)nq * ix->m * 1024));
-            B200_CUDA_OK(launch_pq_lut(d_q, nq, ix->d_pad, ix->d_pq, ix->m, ix->dsub, ix->w_lut.as<float>(), s));
+            B200_TRY(ix->w_lut.reserve((size_t)nq * ix->m * pq_codewords(ix->pq_bits) * 4));
+            B200_CUDA_OK(pq4 ? launch_pq4_lut(d_q, nq, ix->d_pad, ix->d_pq, ix->m, ix->dsub, ix->w_lut.as<float>(), s)
+                             : launch_pq_lut(d_q, nq, ix->d_pad, ix->d_pq, ix->m, ix->dsub, ix->w_lut.as<float>(), s));
         }
         if (ix->payload != IVF_PRODUCER_PQ) {   // PQ: the pair constant (||q - c||^2 or -<q, c>) is the whole query term
             query_const_kernel<<<(unsigned)ceil_div(nq * 32, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq + 3 * ix->d : nullptr,
@@ -2242,15 +2296,17 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         cudaEventRecord(ix->ev_ph[2], s);
         cudaEventRecord(ix->ev0, s);
     }
-    cudaError_t e = lut ? launch_ivf_pq_lut_topk(gp, grid, s, &detail)
-                        : launch_ivf_gemm_topk(gp, ix->w_qbuf.p, n_pairs + 128, ix->d_pool, (int64_t)ix->pool_pages * kPageRows, grid, s, &detail);
+    cudaError_t e = pq4   ? launch_ivf_pq4_topk(gp, grid, s, &detail)
+                    : lut ? launch_ivf_pq_lut_topk(gp, grid, s, &detail)
+                          : launch_ivf_gemm_topk(gp, ix->w_qbuf.p, n_pairs + 128, ix->d_pool, (int64_t)ix->pool_pages * kPageRows, grid, s, &detail);
     if (ix->timing) {
         cudaEventRecord(ix->ev1, s);
         cudaEventRecord(ix->ev_ph[3], s);
         ix->timed_pending = true;
     }
     if (e != cudaSuccess)
-        return fail(B200_ERR_CUDA, std::string(lut ? "ivf_pq_lut_topk launch: " : "ivf_gemm_topk launch: ") + (detail ? detail : cudaGetErrorString(e)));
+        return fail(B200_ERR_CUDA, std::string(pq4 ? "ivf_pq4_topk launch: " : lut ? "ivf_pq_lut_topk launch: " : "ivf_gemm_topk launch: ") +
+                                       (detail ? detail : cudaGetErrorString(e)));
     ix->last_items = max_items;
     // ---- per-query merge of the partial lists
     float *m_dis = d_out_dis;
@@ -2415,7 +2471,10 @@ static int index_save_io(b200_index *ix, Io *f) {
     B200_CUDA_OK(cudaSetDevice(ix->device));
     IxHeader h{};
     memcpy(h.magic, "B2IX", 4);
-    h.version = 2;
+    // v3: the v2 layout with reserved0 = the PQ code width (4) and a [m][16][dsub] codebook; every other index stays v2
+    const bool pq4 = pq_uses_lut(ix) && ix->pq_bits == 4;
+    h.version = pq4 ? 3 : 2;
+    h.reserved0 = pq4 ? 4 : 0;
     h.type = ix->type; h.metric = ix->metric; h.d = ix->d; h.nlist = ix->nlist; h.m = ix->m; h.dsub = ix->dsub;
     h.default_nprobe = ix->default_nprobe; h.refine_factor = ix->refine_factor; h.payload = ix->payload; h.has_raw = ix->raw ? 1 : 0;
     h.use_ivf = ix->use_ivf ? 1 : 0; h.code_bytes = ix->code_bytes; h.n = ix->n; h.pages_used = ix->pages_used;
@@ -2449,7 +2508,7 @@ static int index_save_io(b200_index *ix, Io *f) {
             };
             ok = (ix->binary ? dump(ix->d_bcent, (size_t)ix->nlist * ix->cent_pad) : dump(ix->d_centroids, (size_t)ix->nlist * ix->d * 4)) &&
                  wr(f, ix->list_len.data(), (size_t)ix->nlist * 4);
-            if (ok && ix->d_pq) ok = dump(ix->d_pq, (size_t)ix->m * 256 * ix->dsub * 4);
+            if (ok && ix->d_pq) ok = dump(ix->d_pq, (size_t)ix->m * pq_codewords(ix->pq_bits) * ix->dsub * 4);
             if (ok && ix->d_sq) ok = dump(ix->d_sq, (size_t)4 * ix->d * 4);
             std::vector<uint32_t> pages(ix->pages_used);
             if (ok && ix->pages_used)
@@ -2490,15 +2549,21 @@ extern "C" int b200_index_save_cb(b200_index *ix, int (*write)(void *ctx, const 
 static int index_load_io(Io *f, b200_index **out) {
     *out = nullptr;
     IxHeader h{};
-    if (!rd(f, &h, sizeof(h)) || memcmp(h.magic, "B2IX", 4) != 0 || h.version != 2)
-        return fail(B200_ERR_INVALID, "not a B2IX v2 index file");
+    if (!rd(f, &h, sizeof(h)) || memcmp(h.magic, "B2IX", 4) != 0 || (h.version != 2 && h.version != 3))
+        return fail(B200_ERR_INVALID, "not a B2IX v2 / v3 index file");
     // a truncated or corrupt file must fail here, not in a kernel: every size below is derived from these fields
     const bool bin = h.type >= IDX_BINFLAT;
+    // v3: an inverted-file PQ index with 4-bit codes (reserved0 = 4), nibble-packed code rows and a [m][16][dsub] codebook
+    const int pq_bits = h.version == 3 ? 4 : 8;
+    if (h.version == 3 &&
+        !(h.reserved0 == 4 && h.payload == IVF_PRODUCER_PQ && h.use_ivf && h.m > 0 && h.dsub > 0 && (int64_t)h.m * h.dsub == h.d &&
+          h.code_bytes >= pq_code_bytes(h.m, 4) && h.code_bytes % 16 == 0 && ivf_pq4_fits(h.m)))
+        return fail(B200_ERR_INVALID, "corrupt index header (v3: 4-bit PQ with M <= " + std::to_string(ivf_pq4_max_m()) + " expected)");
     const bool sane = h.type >= 0 && h.type < IDX_NUM_TYPES && h.metric >= 0 && h.metric <= 4 && (h.metric >= B200_METRIC_HAMMING) == bin &&
                       h.d > 0 && h.d <= (1 << 16) && (!bin || h.d % 8 == 0) && h.n >= 0 &&
                       h.n < (int64_t)0xffffffffll && h.payload >= 0 && h.payload <= 3 && (h.payload == IVF_PRODUCER_B1) == bin &&
                       (!h.use_ivf || (h.nlist > 0 && h.nlist <= (1 << 24) && (uint64_t)h.pages_used <= (uint64_t)h.n / kPageRows + (uint64_t)h.nlist + 1)) &&
-                      (h.payload != IVF_PRODUCER_PQ || !h.use_ivf || (h.m > 0 && h.dsub > 0 && h.m * h.dsub == h.d && h.code_bytes >= h.m && h.code_bytes % 16 == 0)) &&
+                      (h.payload != IVF_PRODUCER_PQ || !h.use_ivf || (h.m > 0 && h.dsub > 0 && h.m * h.dsub == h.d && h.code_bytes >= (pq_bits == 4 ? (h.m + 1) / 2 : h.m) && h.code_bytes % 16 == 0)) &&
                       (h.payload != IVF_PRODUCER_SQ8 || !h.use_ivf || (h.code_bytes >= h.d && h.code_bytes % 16 == 0)) && (h.has_raw || h.use_ivf);
     if (!sane) return fail(B200_ERR_INVALID, "corrupt index header");
     b200_index *ix = nullptr;
@@ -2509,7 +2574,7 @@ static int index_load_io(Io *f, b200_index **out) {
         return fail(B200_ERR_INVALID, msg);
     };
     try {
-        ix->nlist = h.nlist; ix->m = h.m; ix->dsub = h.dsub; ix->default_nprobe = h.default_nprobe; ix->refine_factor = h.refine_factor;
+        ix->nlist = h.nlist; ix->m = h.m; ix->dsub = h.dsub; ix->pq_bits = pq_bits; ix->default_nprobe = h.default_nprobe; ix->refine_factor = h.refine_factor;
         ix->payload = h.payload; ix->use_ivf = h.use_ivf != 0; ix->code_bytes = h.code_bytes; ix->keep_raw = h.has_raw;
         const int raw_metric = h.metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
         if (h.has_raw && bin) {
@@ -2557,8 +2622,10 @@ static int index_load_io(Io *f, b200_index **out) {
             page_off[nl] = (uint32_t)pages;
             if (total != (uint64_t)h.n || pages != h.pages_used) return bail("corrupt index file (list lengths do not add up)");
             if (h.payload == IVF_PRODUCER_PQ) {
-                if (!slurp((void **)&ix->d_pq, (size_t)h.m * 256 * h.dsub * 4)) return bail("truncated index file (codebook)");
-                if (pq_dsub_decodable(h.dsub)) {   // the tensor-core decoder's bf16 copy; the table look-up scan reads the fp32 codebook
+                if (!slurp((void **)&ix->d_pq, (size_t)h.m * pq_codewords(pq_bits) * h.dsub * 4)) return bail("truncated index file (codebook)");
+                if (pq_bits == 4) {
+                    // validated with the header: the 4-bit look-up scan reads the fp32 codebook
+                } else if (pq_dsub_decodable(h.dsub)) {   // the tensor-core decoder's bf16 copy; the table look-up scan reads the fp32 codebook
                     if (cudaMalloc(&ix->d_pq_bf16, (size_t)h.m * 256 * h.dsub * 2) != cudaSuccess) return bail("cudaMalloc failed");
                     if (launch_f32_to_bf16_rows(ix->d_pq, h.dsub, ix->d_pq_bf16, h.dsub, (int64_t)h.m * 256, ix->stream) != cudaSuccess)
                         return bail("codebook conversion failed");

@@ -72,4 +72,15 @@ cudaError_t launch_ivf_pq_lut_topk(const IvfGemmParams &p, int grid, cudaStream_
 // buffer in shared memory, by the launcher's own arithmetic
 bool ivf_pq_lut_fits(int m);
 
+// PQ with 4-bit codes (ivf_pq4_sm90.cu): codes nibble-packed (code j in byte j / 2, even j low), codebook [m][16][dsub] fp32.
+// launch_pq4_lut fills lut_out [nq][m][16] = <q_j, codebook_j[e]> (fp32); launch_ivf_pq4_topk scans the same work items into
+// the same partial lists with p.lut = that table
+cudaError_t launch_pq4_lut(const float *queries, int64_t nq, int d_pad, const float *codebook, int m, int dsub, float *lut_out, cudaStream_t s);
+cudaError_t launch_ivf_pq4_topk(const IvfGemmParams &p, int grid, cudaStream_t s, const char **err_detail);
+
+// the 4-bit scan's limit on M, and whether it takes m: one query's M x 64 B table beside a k = 1024 list pair and the
+// candidate buffer in shared memory, by the launcher's own arithmetic
+int ivf_pq4_max_m();
+bool ivf_pq4_fits(int m);
+
 }  // namespace b200

@@ -2,7 +2,7 @@
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
 workload; results are pasted into DESIGN.md section 7.
-Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [prefilter]"""
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter]"""
 import json
 import os
 import subprocess
@@ -347,6 +347,63 @@ def bench_pq_wide():
             print(json.dumps(pt), flush=True)
 
 
+def bench_pq4():
+    """4-bit against 8-bit PQ codes on the pq_wide data (2 M clustered 768-d rows, nlist 4096, k = 10, L2): SCANN and IVFPQ at
+    8 bits (M = 48) and at 4 bits (M = 96, the same 48 code bytes per row), MSTG and FLAT (truth), over nq x nprobe.  Per point
+    and index: recall@10 against FLAT, the median call time and the median list-scan kernel time (last_scan) with their
+    spread (min, max) over the repeats, and table look-ups per second (rows streamed x M / kernel time).  Within a repeat the
+    indexes run one after the other (8- and 4-bit alternating), so that drift of a shared machine lands on all of them."""
+    n, d, k, nlist = 2_000_000, 768, 10, 4096
+    y, qs = clustered(n, d, 10_000, seed=768, nq=1024)
+    ctx = gpu_context()
+    flat = b2.Corpus(b2.L2, d).append(y)
+    idx = {}
+    for name, typ, params in (("SCANN8", "SCANN", f"ncentroids={nlist}"), ("SCANN4", "SCANN", f"ncentroids={nlist}, bit_size=4"),
+                              ("IVFPQ8", "IVFPQ", f"ncentroids={nlist}, M=48, keep_raw=0"),
+                              ("IVFPQ4", "IVFPQ", f"ncentroids={nlist}, M=96, bit_size=4, keep_raw=0"), ("MSTG", "MSTG", f"ncentroids={nlist}")):
+        t0 = time.perf_counter()
+        idx[name] = b2.VectorIndex(typ, b2.L2, d, params).build(y)
+        idx[name].enable_timing(True)
+        print(json.dumps({"build": name, "m": idx[name].info()["m"], "build_s": round(time.perf_counter() - t0, 1)}), flush=True)
+    del y
+    order = ("SCANN8", "SCANN4", "IVFPQ8", "IVFPQ4", "MSTG")
+    for nq in (1, 16, 256, 1024):
+        q = qs[:nq]
+        reps = 15 if nq <= 16 else 5
+        flat.search(q, k)
+        t0 = time.perf_counter()
+        _, truth = flat.search(q, k)
+        t_flat = time.perf_counter() - t0
+        for nprobe in (1, 4, 16, 64):
+            prm = f"nprobe={nprobe}"
+            call, kern, out, scan = {n_: [] for n_ in order}, {n_: [] for n_ in order}, {}, {}
+            for r in range(reps + 1):              # round 0 warms every index up and is not kept
+                for name in order:
+                    ix = idx[name]
+                    fso = name.startswith("IVFPQ")
+                    ix.last_scan(reset=True)
+                    t0 = time.perf_counter()
+                    out[name] = ix.search(q, k, prm, first_stage_only=fso)
+                    t = time.perf_counter() - t0
+                    ls = ix.last_scan(reset=True)
+                    scan[name] = ls
+                    if r:
+                        call[name].append(t * 1e3)
+                        kern[name].append(ls["kernel_ms"] / max(1, ls["launches"]))
+            pt = dict(workload=f"pq4 {n} x {d} clustered, nlist={nlist}, k={k}, L2", nq=nq, nprobe=nprobe, reps=reps, **ctx,
+                      FLAT=dict(call_ms=round(t_flat * 1e3, 3)))
+            for name in order:
+                ks, cs, ls = np.array(kern[name]), np.array(call[name]), scan[name]
+                e = dict(recall=round(recall(out[name][1], truth), 4), call_ms=round(float(np.median(cs)), 3),
+                         call_ms_spread=[round(float(cs.min()), 3), round(float(cs.max()), 3)],
+                         scan_kernel_ms=round(float(np.median(ks)), 4), scan_kernel_ms_spread=[round(float(ks.min()), 4), round(float(ks.max()), 4)],
+                         rows_streamed=ls["rows_streamed"], list_bytes_per_row=ls["payload_row_bytes"])
+                if name != "MSTG" and np.median(ks) > 0:
+                    e["lookups_per_s"] = float(f"{ls['rows_streamed'] * idx[name].info()['m'] / (np.median(ks) * 1e-3):.4g}")
+                pt[name] = e
+            print(json.dumps(pt), flush=True)
+
+
 def alive_bitmap(n, frac, clustered_runs, seed):
     """LSB-first bitmap keeping round(frac * n) rows (at least 1): uniformly random rows, or runs of up to 4096 contiguous
     rows at random starts (a tenant's rows are often contiguous)"""
@@ -453,4 +510,4 @@ if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
         {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
-         "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide, "prefilter": bench_prefilter}[w]()
+         "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide, "pq4": bench_pq4, "prefilter": bench_prefilter}[w]()

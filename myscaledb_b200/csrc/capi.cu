@@ -458,13 +458,15 @@ static int gemm_chunk(b200_corpus *c, GemmTopkParams &gp, int64_t nq_c, int k, i
     int grid = gemm_topk_grid(q_tiles, gp.n, c->sms);
     grid = (grid / q_tiles) * q_tiles;
     if (grid < q_tiles) grid = q_tiles;
-    B200_TRY(c->w_pk.reserve((size_t)grid * 128 * k * 4));
-    B200_TRY(c->w_pi.reserve((size_t)grid * 128 * k * 4));
+    // every consumer warpgroup of a CTA keeps and publishes its own per-query lists
+    const size_t producers = (size_t)grid * gemm_consumer_warpgroups(kernel == B200_KERNEL_GEMM_TF32X3);
+    B200_TRY(c->w_pk.reserve(producers * 128 * k * 4));
+    B200_TRY(c->w_pi.reserve(producers * 128 * k * 4));
     gp.part_keys = c->w_pk.as<float>();
     gp.part_ids = c->w_pi.as<uint32_t>();
     {  // global scratch for the per-thread lists, used when they do not fit in shared memory (large k)
-        B200_TRY(c->w_lk.reserve((size_t)grid * 128 * list_cap_for(k) * 4));
-        B200_TRY(c->w_li.reserve((size_t)grid * 128 * list_cap_for(k) * 4));
+        B200_TRY(c->w_lk.reserve(producers * 128 * list_cap_for(k) * 4));
+        B200_TRY(c->w_li.reserve(producers * 128 * list_cap_for(k) * 4));
         gp.list_keys_gmem = c->w_lk.as<float>();
         gp.list_ids_gmem = c->w_li.as<uint32_t>();
     }
@@ -494,7 +496,7 @@ static int gemm_chunk(b200_corpus *c, GemmTopkParams &gp, int64_t nq_c, int k, i
     mp.in_ids = gp.part_ids;
     mp.list_stride = (int64_t)nq_pad * k;
     mp.q_stride = k;
-    mp.n_lists = grid / q_tiles;
+    mp.n_lists = (int)(producers / q_tiles);
     mp.k_in = k;
     mp.k = k;
     mp.nq = nq_c;

@@ -16,12 +16,12 @@ constexpr int HN = 128;            // corpus rows per MMA pass: the tile is comp
 constexpr int BK = 64;             // bf16 per k-block = one 128-byte swizzle row
 constexpr int UMMA_K = 16;         // bf16 wgmma K
 constexpr int EPI_THREADS = 128;   // the consumer warpgroup: MMAs, then the top-k epilogue (thread t = query row t)
-constexpr int NUM_THREADS = EPI_THREADS + 32;  // + one TMA producer warp (warp 4)
+constexpr int NUM_THREADS = EPI_THREADS + 32;  // IVF kernel: + one TMA producer warp (warp 4)
 constexpr int SMEM_ALIGN_SLACK = 1024;
 constexpr int MAX_STAGES = 4;
 constexpr int SMEM_LIMIT = 232448;  // 227 KB of opt-in shared memory per block (sm_90)
 
-constexpr int SCRATCH_BYTES = 32 * EPI_THREADS * 4;  // epilogue slow-path scratch [32][128] floats
+constexpr int SCRATCH_BYTES = 32 * EPI_THREADS * 4;  // IVF kernel: epilogue slow-path scratch [32][128] floats
 // Accumulator hand-off: the warpgroup's registers are written column-major into shared memory, 64 columns at a time
 // ([ACC_COLS][ACC_LD] floats; the padding of 4 makes both the fragment stores and the per-row reads of the epilogue
 // conflict-free).  It takes the place of tensor memory: the epilogue reads its query row in chunks of 32 columns.  Staging a
@@ -33,9 +33,10 @@ constexpr int ACC_BYTES = ACC_COLS * ACC_LD * 4;     // 33 KB
 // Operand type of a tensor-core kernel: bf16 rows, fp32 rows as 3xTF32, or binary rows (1-bit AND + popcount, s32 sums)
 enum class Operand { BF16, TF32X3, B1 };
 
-// Shared-memory layout of the tensor-core kernels for a ring of `st` stages.  Stage s holds the query k-block and the half
-// tile's corpus k-block; fp32 rows (TF32X3) add the lo planes of both: [A hi][A lo][B hi][B lo].  Every k-block row is one
-// 128-byte swizzle row (64 bf16, 32 fp32 or 1024 bits); for binary rows an "element" is a byte.
+// Operand geometry of the tensor-core kernels, and the shared-memory layout of the IVF kernel for a ring of `st` stages (the flat
+// kernel's is Op in ip_gemm_sm90.cu).  Every k-block row is one 128-byte swizzle row (64 bf16, 32 fp32 or 1024 bits); for binary
+// rows an "element" is a byte.  A plane is the k-block of 128 rows; fp32 rows (TF32X3, flat kernel only) have hi and lo planes.
+// IVF stage s: the query k-block and the half tile's corpus k-block.
 template <Operand OP>
 struct Layout {
     static constexpr bool F32X3 = OP == Operand::TF32X3;
@@ -177,16 +178,16 @@ __device__ __forceinline__ void wgmma_b1_n128(int32_t (&d)[64], uint64_t adesc, 
         : "l"(adesc), "l"(bdesc), "r"(accum));
 }
 
-// Store columns [64 Q, 64 Q + 64) of the warpgroup's two 64 x 128 accumulator fragments column-major into acc
-// ([ACC_COLS][ACC_LD]) as fp32 (s32 AND counts convert exactly: they are below 2^24).  Fragment layout of wgmma m64nN: warp w,
-// lane l holds rows 16 w + l / 4 (+ 8) and columns 8 i + 2 (l % 4) (+ 1).
-template <int Q, typename T>
+// Store columns [COLS Q, COLS Q + COLS) of the warpgroup's two 64 x 128 accumulator fragments column-major into acc
+// ([COLS][ACC_LD]) as fp32 (s32 AND counts convert exactly: they are below 2^24).  Fragment layout of wgmma m64nN: warp w of
+// the warpgroup, lane l holds rows 16 w + l / 4 (+ 8) and columns 8 i + 2 (l % 4) (+ 1).
+template <int Q, int COLS = ACC_COLS, typename T>
 __device__ __forceinline__ void acc_store(float *acc, const T (&d0)[64], const T (&d1)[64]) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
     const int r = warp * 16 + (lane >> 2), c = 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < ACC_COLS / 8; j++) {
-        const int i = Q * (ACC_COLS / 8) + j;
+    for (int j = 0; j < COLS / 8; j++) {
+        const int i = Q * (COLS / 8) + j;
         float *col = acc + (8 * j + c) * ACC_LD + r;
         col[0] = (float)d0[4 * i];
         col[ACC_LD] = (float)d0[4 * i + 1];
@@ -391,7 +392,9 @@ __device__ __forceinline__ void jaccard_keys32(float (&v)[32], int pq, const flo
 // loops while any lane still has a candidate bit, each lane popping its own lowest bit and doing
 // an inlined insert (per-element calls under divergence serialise the lanes during the start-up
 // "insert storm" of a launch).
-// scratch: this thread's column of a [32][EPI_THREADS] float array.
+// scratch: this thread's column of a [32][LD] float array.  It may be the 32 staged accumulator columns the chunk was loaded
+// from: only this thread reads its row of them, and it holds them in v by now.
+template <int LD = EPI_THREADS>
 __device__ __forceinline__ void epilogue_chunk(ThreadTopK &list, float (&v)[32], bool use_side, const float *scale,
                                                const float *bias, uint32_t id0, bool tail, int64_t n, float *scratch,
                                                float ext_bound = FLT_MAX /* a valid upper bound of the k-th key known from elsewhere */) {
@@ -425,7 +428,7 @@ __device__ __forceinline__ void epilogue_chunk(ThreadTopK &list, float (&v)[32],
 #pragma unroll
         for (int j = 0; j < 32; j++) {
             const float key = use_side ? v[j] : -v[j];
-            scratch[j * EPI_THREADS] = key;
+            scratch[j * LD] = key;
             if (key <= thr) mask |= 1u << j;
         }
         if (tail && !use_side) {  // rows past the end of the corpus (zero-filled by TMA) are not candidates
@@ -436,7 +439,7 @@ __device__ __forceinline__ void epilogue_chunk(ThreadTopK &list, float (&v)[32],
             if (mask) {
                 const int j = __ffs(mask) - 1;
                 mask &= mask - 1;
-                list_insert(list, scratch[j * EPI_THREADS], id0 + (uint32_t)j);
+                list_insert(list, scratch[j * LD], id0 + (uint32_t)j);
             }
         }
     }

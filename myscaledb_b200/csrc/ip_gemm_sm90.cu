@@ -16,12 +16,17 @@
 // (reference: VectorIndex/Common/BruteForceSearch.h:77-88) and the FLAT Search::VectorIndex::search scan
 // (VectorIndex/Common/VIWithDataPart.cpp:926).
 //
-// One CTA = 128 queries (one query tile for its whole life) x corpus tiles of 256 rows (worker, worker + W, ...):
-//   warps 0..3  consumer warpgroup: a tile is computed as two N = 128 halves; per half, two wgmma m64n128 (query rows
-//               0..63 / 64..127) per k-step accumulate in registers, the result is staged column-major in shared memory
-//               and thread t then filters query row t in chunks of 32 columns into its private top-k list;
-//   warp 4      TMA producer (one lane): A = the query k-block, B = the half tile's corpus k-block, ring of full/empty
-//               mbarriers.
+// One CTA = 128 queries (one query tile for its whole life) x corpus tiles of 256 rows (worker, worker + W, ...).  A tile is
+// computed as two N = 128 halves; per half, two wgmma m64n128 (query rows 0..63 / 64..127) per k-step accumulate in the
+// registers of one warpgroup, the result is staged column-major in shared memory and thread t of that warpgroup then filters
+// query row t in chunks of 32 columns into its private top-k list.
+//   bf16 and binary rows: warps 0..3 and 4..7 are two consumer warpgroups, warpgroup w owns half w of every tile.  A stage of
+//               the ring holds the query k-block and the corpus k-block of all 256 rows, so the query k-block is fetched once
+//               per tile, not once per half.  The warpgroups share nothing but the ring: each has its own accumulator
+//               staging, side arrays, named barrier and per-query lists, and a CTA publishes two partial lists per query.
+//   fp32 rows:  warps 0..3 are the one consumer warpgroup; it walks both halves, a stage holds one half's corpus k-block
+//               (with the hi / lo planes a stage of both halves would leave no room for a ring).
+//   next warp   TMA producer (one lane), ring of full / empty mbarriers.
 // The key that is ranked is  acc * row_scale[j] + row_bias[j]  (smaller = better):
 //   IP: -acc | L2: ||y||^2 - 2 acc (+||q||^2 added at merge) | cosine: -acc / ||y|| | Hamming: popc(y) - 2 and (+popc(q) added
 //   at merge);  filtered / out-of-range rows: scale 0, bias +inf.
@@ -34,20 +39,63 @@
 namespace b200 {
 namespace gemm {
 
-// Ring depth and list placement per operand type (layout: Layout in gemm_common.cuh)
+// Shared-memory layout of gemm_topk_kernel per operand type, ring depth and list placement.
+//   [stage 0] .. [stage st - 1]   stage = [A hi][A lo][B (hi after the split) of WG halves][B lo]; lo planes: fp32 rows only
+//   per consumer warpgroup: accumulator staging [COLS][ACC_LD] floats (also the slow-path scratch of epilogue_chunk)
+//   per consumer warpgroup: side scale[SIDE_N], side bias[SIDE_N] of the tile rows the warpgroup owns
+//   full / empty mbarriers
+//   per consumer warpgroup: the 128 per-thread lists, when they are kept in shared memory
+// Two warpgroups stage 32 accumulator columns at a time: 3 stages of 48 KB and two sets of 64-column staging and lists do not
+// fit in 227 KB.
 template <Operand OP>
-struct Op : Layout<OP> {
-    using L = Layout<OP>;
+struct Op {
+    using L = Layout<OP>;   // operand geometry (k-block, planes); the offsets below are this kernel's own
     using Acc = typename std::conditional<OP == Operand::B1, int32_t, float>::type;   // wgmma accumulator type
-    static constexpr int MAX_ST = L::F32X3 ? 2 : 4;
+    static constexpr bool F32X3 = L::F32X3;
+    static constexpr int KB = L::KB, MMA_K = L::MMA_K, A_PLANE = L::A_PLANE, B_PLANE = L::B_PLANE, PLANES = L::PLANES;
+    static constexpr int WG = gemm_consumer_warpgroups(F32X3);
+    // + the TMA producer warp.  With two consumer warpgroups the block is three whole warpgroups: registers are budgeted per
+    // warpgroup (65536 / 384 = 168 each), and setmaxnreg then moves the idle share of the producer's to the consumers, which need
+    // their 128 accumulators and the epilogue's working set (40 + 2 x 232 = 3 x 168).
+    static constexpr int THREADS = WG == 1 ? EPI_THREADS + 32 : 3 * EPI_THREADS;
+    static constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+    static constexpr int B_ROWS = WG * HN;                   // corpus rows per stage (one TMA box)
+    static constexpr int PASSES = BN / B_ROWS;               // halves a warpgroup walks per tile
+    static constexpr int STAGE_BYTES = PLANES * (A_PLANE + WG * B_PLANE);
+    static constexpr int TX_BYTES = PLANES * A_PLANE + WG * B_PLANE;   // what TMA writes (the B lo plane is computed)
+    static constexpr int COLS = WG == 1 ? ACC_COLS : 32;     // accumulator columns staged at a time
+    static constexpr int STAGING_BYTES = COLS * ACC_LD * 4;
+    static constexpr int SIDE_N = BN / WG;                   // side entries a warpgroup owns per tile
+    static constexpr int MAX_ST = F32X3 ? 2 : 3;
+    static_assert(MAX_ST <= MAX_STAGES, "barrier arrays");
+    __host__ __device__ static constexpr int off_acc(int st) { return st * STAGE_BYTES; }
+    __host__ __device__ static constexpr int off_side(int st) { return off_acc(st) + WG * STAGING_BYTES; }
+    __host__ __device__ static constexpr int off_bar(int st) { return off_side(st) + 2 * BN * 4; }
+    __host__ __device__ static constexpr int off_list(int st) { return off_bar(st) + 256; }
+    static constexpr int list_bytes(int k_smem) { return k_smem * EPI_THREADS * 8; }   // one warpgroup's lists
+    static size_t smem_bytes(int st, int k_smem) { return (size_t)off_list(st) + (size_t)WG * list_bytes(k_smem) + SMEM_ALIGN_SLACK; }
+    static bool lists_fit(int k_smem) { return smem_bytes(2, k_smem) <= (size_t)SMEM_LIMIT; }
     static int stages_for(int k_smem) {
         int st = MAX_ST;
-        while (st > 2 && L::off_list(st) + k_smem * EPI_THREADS * 8 + SMEM_ALIGN_SLACK > SMEM_LIMIT) st--;
+        while (st > 2 && smem_bytes(st, k_smem) > (size_t)SMEM_LIMIT) st--;
         return st;
     }
-    static bool lists_fit(int k) { return L::off_list(2) + k * EPI_THREADS * 8 + SMEM_ALIGN_SLACK <= SMEM_LIMIT; }
-    static size_t smem_bytes(int st, int k_smem) { return (size_t)L::off_list(st) + (size_t)k_smem * EPI_THREADS * 8 + SMEM_ALIGN_SLACK; }
 };
+
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// named barrier of one consumer warpgroup (ids 1 and 2; 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
+
+// acc_store<q, COLS> for the q of an unrolled loop (the accumulator registers want compile-time indices)
+template <int COLS, int Q = 0, typename T>
+__device__ __forceinline__ void acc_store_cols(float *acc, const T (&d0)[64], const T (&d1)[64], int q) {
+    if (q == Q) acc_store<Q, COLS>(acc, d0, d1);
+    else if constexpr ((Q + 1) * COLS < HN) acc_store_cols<COLS, Q + 1>(acc, d0, d1, q);
+}
 
 // x = hi + lo with both parts exactly representable in TF32 (so the result does not depend on how the tensor core
 // would round a raw fp32 operand).  hi by truncation: FLT_MAX (the reference's padding value for empty rows,
@@ -71,17 +119,13 @@ __global__ void split_tf32_kernel(const float *__restrict__ src, int64_t n_src, 
 }
 
 template <Operand OP>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __launch_bounds__(Op<OP>::THREADS, 1)
 gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_qlo,
                  const __grid_constant__ CUtensorMap map_c, const GemmTopkParams p) {
     using O = Op<OP>;
     const int STAGES = p.stages;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    // stage s: [A hi][A lo][B (hi after the split)][B lo], planes present per operand type
-    float *acc = reinterpret_cast<float *>(smem + O::off_acc(STAGES));
-    float *side_scale = reinterpret_cast<float *>(smem + O::off_side(STAGES));
-    float *side_bias = side_scale + BN;
     uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + O::off_bar(STAGES));
     uint64_t *empty_bar = full_bar + MAX_STAGES;
 
@@ -92,18 +136,20 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
     const int64_t n_tiles = (p.n + BN - 1) / BN;
     const int kb_count = (p.d_pad + O::KB - 1) / O::KB;
 
-    if (warp == 4 && lane == 0) {
+    if (warp == O::WG * 4 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_q)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_c)) : "memory");
         for (int i = 0; i < STAGES; i++) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 4);  // one arrival per consumer warp
+            mbar_init(&empty_bar[i], O::WG * 4);  // one arrival per consumer warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
-    if (warp == 4) {
+    if (warp >= O::WG * 4) {
+        if constexpr (O::WG == 2) setmaxnreg_dec<O::PRODUCER_REGS>();
+        if (warp != O::WG * 4) return;   // the rest of the producer's warpgroup only hands over its registers
         // ===================== TMA producer =====================
         int stage = 0;
         uint32_t phase = 0;
@@ -131,7 +177,7 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                 pacing = __shfl_sync(0xffffffffu, ok, 0) != 0;
             }
             __syncwarp();
-            for (int h = 0; h < BN / HN; h++) {
+            for (int h = 0; h < O::PASSES; h++) {
                 for (int kb = 0; kb < kb_count; kb++) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     if (elect_one()) {
@@ -139,7 +185,7 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                         mbar_arrive_expect_tx(&full_bar[stage], O::TX_BYTES);
                         tma_load_2d(&map_q, &full_bar[stage], st, kb * O::KB, qt * BM);
                         if constexpr (O::F32X3) tma_load_2d(&map_qlo, &full_bar[stage], st + O::A_PLANE, kb * O::KB, qt * BM);
-                        tma_load_2d(&map_c, &full_bar[stage], st + O::PLANES * O::A_PLANE, kb * O::KB, (int)(t * BN + h * HN));
+                        tma_load_2d(&map_c, &full_bar[stage], st + O::PLANES * O::A_PLANE, kb * O::KB, (int)(t * BN + h * O::B_ROWS));
                     }
                     __syncwarp();
                     if (++stage == STAGES) {
@@ -151,9 +197,16 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
         }
     } else {
         // ===================== consumer warpgroup: MMAs, then the fused top-k =====================
-        const int row = threadIdx.x;  // query row inside the tile
+        if constexpr (O::WG == 2) setmaxnreg_inc<O::CONSUMER_REGS>();
+        const int wg = threadIdx.x / EPI_THREADS;   // with two warpgroups: the half of every tile this one owns
+        const int row = threadIdx.x % EPI_THREADS;  // query row inside the tile
         const bool use_side = p.row_scale || p.row_bias || p.alive || p.scale_const != -1.f;
-        float *scratch = reinterpret_cast<float *>(smem + O::off_scratch(STAGES)) + row;
+        // everything the epilogue writes is private to the warpgroup: the two drift apart by up to the ring's depth
+        float *acc = reinterpret_cast<float *>(smem + O::off_acc(STAGES) + wg * O::STAGING_BYTES);
+        float *side_scale = reinterpret_cast<float *>(smem + O::off_side(STAGES)) + wg * 2 * O::SIDE_N;
+        float *side_bias = side_scale + O::SIDE_N;
+        // partial list  worker * WG + wg  of query tile qt (the merge reads [list][nq_pad][k])
+        const size_t producer = ((size_t)worker * O::WG + wg) * p.q_tiles + qt;
         ThreadTopK list;
         list.n = 0;
         list.worst = 0;
@@ -161,12 +214,13 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
         list.thr_key = (qt * BM + row < p.nq_valid) ? FLT_MAX : -FLT_MAX;
         list.thr_id = 0;
         const int list_cap = list_cap_for(p.k);
-        if (p.lists_in_smem)
-            list_bind(list, reinterpret_cast<float *>(smem + O::off_list(STAGES)),
-                      reinterpret_cast<uint32_t *>(smem + O::off_list(STAGES) + (size_t)list_cap * EPI_THREADS * 4), row, p.k);
-        else
-            list_bind(list, p.list_keys_gmem + (size_t)blockIdx.x * list_cap * EPI_THREADS,
-                      p.list_ids_gmem + (size_t)blockIdx.x * list_cap * EPI_THREADS, row, p.k);
+        if (p.lists_in_smem) {
+            unsigned char *lists = smem + O::off_list(STAGES) + wg * O::list_bytes(list_cap);
+            list_bind(list, reinterpret_cast<float *>(lists), reinterpret_cast<uint32_t *>(lists + O::list_bytes(list_cap) / 2), row, p.k);
+        } else {
+            list_bind(list, p.list_keys_gmem + producer * list_cap * EPI_THREADS, p.list_ids_gmem + producer * list_cap * EPI_THREADS,
+                      row, p.k);
+        }
         // binary Jaccard: popc(q) of this thread's query row (0 for padding rows)
         const int pq = (OP == Operand::B1 && p.jaccard && qt * BM + row < p.nq_valid) ? (int)p.q_popc[qt * BM + row] : 0;
         const uint32_t smem0 = smem_u32(smem);
@@ -175,12 +229,12 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
         typename O::Acc d0[64], d1[64];
         for (int64_t t = worker; t < n_tiles; t += W) {
             const int64_t n0 = t * BN;
-            // this tile's side entries (in flight during the MMAs; written after the barrier below)
-            float sc[BN / EPI_THREADS], bi[BN / EPI_THREADS];
+            // the side entries of this warpgroup's rows of the tile (in flight during the MMAs; written after the barrier below)
+            float sc[O::SIDE_N / EPI_THREADS], bi[O::SIDE_N / EPI_THREADS];
             if (use_side) {
 #pragma unroll
-                for (int i = 0; i < BN / EPI_THREADS; i++) {
-                    const int64_t r = n0 + row + i * EPI_THREADS;
+                for (int i = 0; i < O::SIDE_N / EPI_THREADS; i++) {
+                    const int64_t r = n0 + wg * O::SIDE_N + row + i * EPI_THREADS;
                     bool ok = r < p.n;
                     if (ok && p.alive) ok = (p.alive[r >> 3] >> (r & 7)) & 1;
                     sc[i] = ok ? (p.row_scale ? p.row_scale[r] : p.scale_const) : 0.f;
@@ -188,7 +242,8 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                 }
             }
             const bool tail = n0 + BN > p.n;
-            for (int h = 0; h < BN / HN; h++) {
+            for (int pass = 0; pass < O::PASSES; pass++) {
+                const int h = O::WG == 1 ? pass : wg;   // the half of the tile
                 int prev = -1;
                 for (int kb = 0; kb < kb_count; kb++) {
                     mbar_wait(&full_bar[stage], phase);
@@ -209,7 +264,7 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                             bl[row + i * EPI_THREADS] = lo;
                         }
                         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic stores -> wgmma operand reads
-                        wg_bar();
+                        wg_bar(wg);
                     }
                     wgmma_fence();
                     if constexpr (O::F32X3) {
@@ -228,7 +283,7 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                             wgmma_tf32_n128(d1, ahi + M1 + off, b + off, 1u);
                         }
                     } else if constexpr (OP == Operand::B1) {
-                        const uint64_t a = make_smem_desc(st), b = make_smem_desc(st + O::A_PLANE);
+                        const uint64_t a = make_smem_desc(st), b = make_smem_desc(st + O::A_PLANE + wg * O::B_PLANE);
                         constexpr uint64_t M1 = (64 * 128) >> 4;
 #pragma unroll
                         for (int k = 0; k < O::KB / O::MMA_K; k++) {
@@ -238,7 +293,7 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                             wgmma_b1_n128(d1, a + M1 + off, b + off, acc0);
                         }
                     } else {
-                        const uint64_t a = make_smem_desc(st), b = make_smem_desc(st + O::A_PLANE);
+                        const uint64_t a = make_smem_desc(st), b = make_smem_desc(st + O::A_PLANE + wg * O::B_PLANE);
                         constexpr uint64_t M1 = (64 * 128) >> 4;
 #pragma unroll
                         for (int k = 0; k < O::KB / O::MMA_K; k++) {
@@ -265,38 +320,39 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
-                for (int q = 0; q < HN / ACC_COLS; q++) {
-                    wg_bar();  // every row's reads of the previous staging (and of the previous tile's side arrays) are done
-                    if (h == 0 && q == 0 && use_side) {
+                for (int q = 0; q < HN / O::COLS; q++) {
+                    wg_bar(wg);  // every row's reads of the previous staging (and of the previous tile's side arrays) are done
+                    if (pass == 0 && q == 0 && use_side) {
 #pragma unroll
-                        for (int i = 0; i < BN / EPI_THREADS; i++) {
+                        for (int i = 0; i < O::SIDE_N / EPI_THREADS; i++) {
                             side_scale[row + i * EPI_THREADS] = sc[i];
                             side_bias[row + i * EPI_THREADS] = bi[i];
                         }
                     }
-                    if (q == 0) acc_store<0>(acc, d0, d1);
-                    else acc_store<1>(acc, d0, d1);
-                    wg_bar();
+                    acc_store_cols<O::COLS>(acc, d0, d1, q);
+                    wg_bar(wg);
                     // Chunks of 32 columns.  A chunk is first reduced to its best key (31 FMNMX); the per-element test only
-                    // runs for the rare chunk that can beat the current k-th key.
+                    // runs for the rare chunk that can beat the current k-th key, and parks its keys where the chunk was staged.
 #pragma unroll 1
-                    for (int cc = 0; cc < ACC_COLS / 32; cc++) {
+                    for (int cc = 0; cc < O::COLS / 32; cc++) {
                         float v[32];
                         acc_load32(acc, row, cc * 32, v);
-                        const int c0 = h * HN + q * ACC_COLS + cc * 32;
+                        float *scratch = acc + cc * 32 * ACC_LD + row;
+                        const int c0 = h * HN + q * O::COLS + cc * 32;   // column of the tile
+                        const int s0 = c0 - wg * O::SIDE_N;               // ... and of this warpgroup's side arrays
                         if (OP == Operand::B1 && p.jaccard) {
-                            jaccard_keys32(v, pq, side_scale + c0, side_bias + c0);
-                            epilogue_chunk(list, v, false, side_scale + c0, side_bias + c0, (uint32_t)(n0 + c0), tail, p.n, scratch);
+                            jaccard_keys32(v, pq, side_scale + s0, side_bias + s0);
+                            epilogue_chunk<ACC_LD>(list, v, false, side_scale + s0, side_bias + s0, (uint32_t)(n0 + c0), tail, p.n, scratch);
                         } else {
-                            epilogue_chunk(list, v, use_side, side_scale + c0, side_bias + c0, (uint32_t)(n0 + c0), tail, p.n, scratch);
+                            epilogue_chunk<ACC_LD>(list, v, use_side, side_scale + s0, side_bias + s0, (uint32_t)(n0 + c0), tail, p.n, scratch);
                         }
                     }
                 }
             }
         }
-        // publish this CTA's per-query partial list
-        float *ok = p.part_keys + ((size_t)blockIdx.x * BM + row) * p.k;
-        uint32_t *oi = p.part_ids + ((size_t)blockIdx.x * BM + row) * p.k;
+        // publish this warpgroup's per-query partial list
+        float *ok = p.part_keys + (producer * BM + row) * p.k;
+        uint32_t *oi = p.part_ids + (producer * BM + row) * p.k;
         list_publish(list, ok, oi);
     }
 }
@@ -335,7 +391,7 @@ static cudaError_t launch(const CUtensorMap &map_q, const CUtensorMap &map_qlo, 
     auto kern = gemm_topk_kernel<OP>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    kern<<<grid, NUM_THREADS, smem, s>>>(map_q, map_qlo, map_c, p);
+    kern<<<grid, O::THREADS, smem, s>>>(map_q, map_qlo, map_c, p);
     g_launches++;
     return cudaGetLastError();
 }
@@ -367,7 +423,7 @@ cudaError_t launch_gemm_topk(const GemmTopkParams &p, int grid, cudaStream_t s, 
     }
     CUtensorMap map_q, map_c;
     if (!gemm::encode_map(&map_q, p.queries_bf16, p.nq_pad, p.d_pad, gemm::BM, gemm::Operand::BF16) ||
-        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::HN, gemm::Operand::BF16)) {
+        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::Op<gemm::Operand::BF16>::B_ROWS, gemm::Operand::BF16)) {
         *err_detail = "cuTensorMapEncodeTiled failed";
         return cudaErrorInvalidValue;
     }
@@ -383,7 +439,7 @@ cudaError_t launch_gemm3_topk(const GemmTopkParams &p, int grid, cudaStream_t s,
     CUtensorMap map_qhi, map_qlo, map_c;
     if (!gemm::encode_map(&map_qhi, p.queries_bf16, p.nq_pad, p.d_pad, gemm::BM, gemm::Operand::TF32X3) ||
         !gemm::encode_map(&map_qlo, p.queries_lo, p.nq_pad, p.d_pad, gemm::BM, gemm::Operand::TF32X3) ||
-        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::HN, gemm::Operand::TF32X3)) {
+        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::Op<gemm::Operand::TF32X3>::B_ROWS, gemm::Operand::TF32X3)) {
         *err_detail = "cuTensorMapEncodeTiled failed";
         return cudaErrorInvalidValue;
     }
@@ -398,7 +454,7 @@ cudaError_t launch_gemm_b1_topk(const GemmTopkParams &p, int grid, cudaStream_t 
     }
     CUtensorMap map_q, map_c;
     if (!gemm::encode_map(&map_q, p.queries_bf16, p.nq_pad, p.d_pad, gemm::BM, gemm::Operand::B1) ||
-        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::HN, gemm::Operand::B1)) {
+        !gemm::encode_map(&map_c, p.corpus_bf16, p.n, p.d_pad, gemm::Op<gemm::Operand::B1>::B_ROWS, gemm::Operand::B1)) {
         *err_detail = "cuTensorMapEncodeTiled failed";
         return cudaErrorInvalidValue;
     }

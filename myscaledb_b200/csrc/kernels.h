@@ -85,9 +85,10 @@ struct GemmTopkParams {
     const uint8_t *alive;      // LSB-first bitmap or null
     const float *q_popc;       // binary Jaccard: popcount of each query of the batch [nq_valid]
     int jaccard;               // binary kernel: Jaccard keys (else Hamming: scale_const = -2, row_bias = popcounts)
-    float *part_keys;          // [gridDim.x][128][k]
+    float *part_keys;          // [W = gemm_consumer_warpgroups * gridDim.x / q_tiles partial lists][nq_pad][k]: consumer warpgroup w of
+                               // the CTA (worker, query tile) writes list  worker * warpgroups + w
     uint32_t *part_ids;
-    float *list_keys_gmem;     // scratch for lists that do not fit in shared memory: [gridDim.x][list_cap_for(k)][128]
+    float *list_keys_gmem;     // scratch for lists that do not fit in shared memory: [W * q_tiles][list_cap_for(k)][128]
     uint32_t *list_ids_gmem;
     int64_t n;
     int nq_pad, d_pad, k;
@@ -103,8 +104,7 @@ constexpr int kGemmSmemK = 128;
 // Per-thread top-k lists (gemm_common.cuh, ThreadTopK) take one of two forms, chosen by k alone:
 //  * rescan (k < list_tourn_min_k): k slots; an insert rescans all k entries for the new worst;
 //  * tournament (k >= list_tourn_min_k): k entries + one (key, id) slot per group of 8 (k <= 64) or 16 entries holding the
-//    group's worst; an insert rescans one group and the group worsts instead of all k entries.  16 keeps k = 100 at 107 slots,
-//    which still leaves the flat kernel a 3-stage operand ring.
+//    group's worst; an insert rescans one group and the group worsts instead of all k entries.  16 keeps k = 100 at 107 slots.
 // The crossover k = 17 was chosen on an earlier GPU and is not re-measured on the H100.
 constexpr int list_tourn_min_k = 17;
 __host__ __device__ inline int list_tourn_group(int k) { return k <= 64 ? 8 : 16; }
@@ -112,6 +112,10 @@ __host__ __device__ inline int list_cap_tourn(int k) { return k + (k + list_tour
 // slots of a per-thread list of this k
 __host__ __device__ inline int list_cap_for(int k) { return k < list_tourn_min_k ? k : list_cap_tourn(k); }
 int gemm_topk_grid(int q_tiles, int64_t n, int num_sms);
+// Consumer warpgroups per CTA of gemm_topk_kernel.  bf16 and binary rows: two, each owning one 128-row half of every 256-row
+// corpus tile and its own per-query lists, so a CTA publishes two partial lists per query.  fp32 rows (3xTF32): one, which
+// walks both halves (its hi / lo operand planes leave no room for a stage that holds both).
+constexpr int gemm_consumer_warpgroups(bool f32x3) { return f32x3 ? 1 : 2; }
 // returns cudaSuccess or an error; tensor maps are encoded inside
 cudaError_t launch_gemm_topk(const GemmTopkParams &p, int grid, cudaStream_t s, const char **err_detail);
 // fp32 rows on the tensor cores with fp32-level accuracy (3xTF32, queries pre-split into hi / lo planes)

@@ -230,7 +230,11 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  * indexes: nprobe >= nlist probes every list; below nlist, nprobe <= 2048, the k limit of the exact scan that ranks the
  * centroids above 1024 probes, else B200_ERR_UNSUPPORTED),
  * "refine_factor=8" (candidates per returned row handed to the exact second stage; 1 = first-stage distances),
- * "keep_raw=0" (do not keep the fp32 rows: no second stage, half the memory).  Parts smaller than
+ * "keep_raw=0" (do not keep the fp32 rows: no second stage, half the memory), "keep_raw=2" (keep them, in pinned, mapped
+ * host memory instead of HBM: [n][d_pad] fp32 in row-id order, the values the HBM rows would hold; the second stage gathers
+ * its nq x k x refine_factor candidate rows over PCIe, with keys and outputs byte-identical to the HBM placement.  It applies
+ * to the float types with inverted lists; FLAT, parts below the threshold below and binary types keep their rows in HBM;
+ * "exact_batch=1" is then refused with B200_ERR_UNSUPPORTED).  Parts smaller than
  * max(2000, 8 * nlist) rows are served by an exact FLAT scan (the reference's fallback_to_flat, test 00029).
  *
  * Build = the reference's reader-driven build (VIPartReader train block / add blocks, VIWithDataPart.cpp:131):
@@ -275,10 +279,17 @@ int b200_index_last_scan(b200_index *ix, int64_t *rows_streamed, int64_t *payloa
 /* computeTopDistanceSubset: exact distances of candidate ids [nq][ncand] (negative = unused) -> top-k */
 int b200_index_refine(b200_index *ix, const float *queries, int64_t nq, const int64_t *cand_ids, int64_t ncand, int k,
                       float *out_dis, int64_t *out_ids);
+/* moves the fp32 rows of a finalized index between HBM (placement 1) and pinned host memory (2), the keep_raw values, under
+ * the index mutex (waits for the device first); the move to host frees the HBM rows and their side arrays.  An index loaded
+ * from an older file can so be demoted without a rebuild.  B200_ERR_INVALID for an index without rows (keep_raw=0) or not
+ * finalized; B200_ERR_UNSUPPORTED where the rows are the index (FLAT, small parts, binary types). */
+int b200_index_set_raw_placement(b200_index *ix, int placement);
 /* VIWithColumnInPart::serialize / load (VIWithDataPart.cpp:451-525, :578-764): one self-describing file
  * ("B2IX" v2; the closed library's .vidx3 payload cannot be reproduced).  PQ indexes with 4-bit codes are written as
  * v3: the v2 layout with the header's reserved word holding the code width (4) and a [M][16][d / M] codebook; every other
- * index is written as v2.  load accepts both and validates every size it derives. */
+ * index is written as v2.  load accepts both and validates every size it derives.  An index with its fp32 rows in host
+ * memory writes the header's has_raw as 2 (every other byte as in HBM placement) and loads them straight into pinned host
+ * memory again. */
 int b200_index_save(b200_index *ix, const char *path);
 int b200_index_load(const char *path, b200_index **out);
 /* the same through the host's own streams (Search::IndexDataFileWriter / Reader over ClickHouse disks,
@@ -360,6 +371,9 @@ int b200_cache_stats(uint64_t *capacity, uint64_t *used, uint64_t *items, uint64
  * A binary corpus counts 4 bytes per row for its per-row popcounts (used by the tensor-core path). */
 int b200_corpus_memory_bytes(const b200_corpus *c, uint64_t *out_bytes);
 int b200_index_memory_bytes(const b200_index *ix, uint64_t *out_bytes);
+/* pinned host bytes of an index's fp32 rows in host placement (keep_raw=2), 0 otherwise; b200_index_memory_bytes counts HBM
+ * only, so it does not include them */
+int b200_index_host_memory_bytes(const b200_index *ix, uint64_t *out_bytes);
 
 /* ------------------------------------------------------------------------------------
  * Filter bitmaps and decoupled-part row-id maps (VIWithMeta::{row_ids_map, inverted_row_ids_map,

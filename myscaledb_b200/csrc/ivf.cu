@@ -936,7 +936,7 @@ __global__ void __launch_bounds__(256) ivf_merge_kernel(const IvfMerge p) {
 // ------------------------------------------------------------------------------------
 struct RefineParams {
     const float *queries;  // [nq][d_pad]
-    const float *rows;     // [n][d_pad]
+    const float *rows;     // [n][d_pad]; staged: the candidates' rows [nq][ncand][d_pad] (gather_host_rows_kernel)
     const int64_t *cand;   // [nq][ncand], negative = empty
     float *out_dis;        // [nq][k]
     int64_t *out_ids;
@@ -947,6 +947,9 @@ struct RefineParams {
     int64_t id_offset;     // added to every returned id (shard base)
 };
 
+// kStaged: candidate (q, c) is read from its staging slot q * ncand + c instead of row id; nothing else differs, so the keys
+// are those of the HBM rows bit for bit
+template <bool kStaged>
 __global__ void __launch_bounds__(256) refine_kernel(const RefineParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *qs = reinterpret_cast<float *>(smem_raw);
@@ -963,7 +966,7 @@ __global__ void __launch_bounds__(256) refine_kernel(const RefineParams p) {
         const int64_t id = p.cand[q * p.ncand + c];
         if (id < 0 || id >= p.n) continue;  // warp-uniform
         // duplicates in the candidate set would be returned twice; the first stage never produces them
-        const float4 *row = reinterpret_cast<const float4 *>(p.rows + (size_t)id * p.d_pad);
+        const float4 *row = reinterpret_cast<const float4 *>(p.rows + (kStaged ? (size_t)q * p.ncand + c : (size_t)id) * p.d_pad);
         float acc = 0.f;
         for (int cc = lane; cc < p.d_pad / 4; cc += 32) {
             const float4 y = row[cc];
@@ -992,6 +995,52 @@ __global__ void __launch_bounds__(256) refine_kernel(const RefineParams p) {
         const float key = have ? fk[j] : 0.f;
         p.out_ids[q * p.k + j] = have ? (int64_t)fi[j] + p.id_offset : -1;
         p.out_dis[q * p.k + j] = !have ? (p.l2 || p.cosine ? FLT_MAX : -FLT_MAX) : p.l2 ? key : p.cosine ? 1.f + key : -key;
+    }
+}
+
+// Rows in host memory (keep_raw=2): one warp per candidate slot of a chunk of queries copies the slot's row through the mapped
+// pointer over PCIe into stage[slot][d_pad].  A lane issues every 16-byte load of kGatherRows rows before its first store, so
+// that a warp keeps kGatherRows rows in flight against the link's latency.  Slots with id < 0 or id >= n are skipped, as
+// refine_kernel skips them.
+constexpr int kGatherVec = 8;    // float4 per lane and row in one pass: one pass covers d_pad <= 1024
+constexpr int kGatherRows = 2;
+
+__global__ void __launch_bounds__(256) gather_host_rows_kernel(const float *__restrict__ rows, int64_t n, int d_pad, const int64_t *__restrict__ cand,
+                                                               int64_t nslots, float *__restrict__ stage) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const int nv = d_pad / 4;
+    for (int64_t s0 = warp * kGatherRows; s0 < nslots; s0 += nwarps * kGatherRows) {
+        const float4 *src[kGatherRows];
+        float4 *dst[kGatherRows];
+        bool ok[kGatherRows];
+#pragma unroll
+        for (int r = 0; r < kGatherRows; r++) {
+            const int64_t id = s0 + r < nslots ? cand[s0 + r] : -1;
+            ok[r] = id >= 0 && id < n;
+            src[r] = reinterpret_cast<const float4 *>(rows + (size_t)(ok[r] ? id : 0) * d_pad);
+            dst[r] = reinterpret_cast<float4 *>(stage + (size_t)(s0 + r) * d_pad);
+        }
+        for (int v0 = 0; v0 < nv; v0 += 32 * kGatherVec) {
+            float4 buf[kGatherRows][kGatherVec];
+#pragma unroll
+            for (int r = 0; r < kGatherRows; r++)
+#pragma unroll
+                for (int j = 0; j < kGatherVec; j++) {
+                    const int v = v0 + j * 32 + lane;
+                    if (ok[r] && v < nv) buf[r][j] = src[r][v];
+                }
+            // a store waits for its load: keep every store behind the last load, or the first one stalls the loads after it
+            asm volatile("" ::: "memory");
+#pragma unroll
+            for (int r = 0; r < kGatherRows; r++)
+#pragma unroll
+                for (int j = 0; j < kGatherVec; j++) {
+                    const int v = v0 + j * 32 + lane;
+                    if (ok[r] && v < nv) dst[r][v] = buf[r][j];
+                }
+        }
     }
 }
 
@@ -1039,11 +1088,16 @@ struct b200_index {
     int pq_bits = 8;                // PQ code width: 8 (256 codewords, one byte per code) or 4 (16 codewords, two codes per byte)
     int default_nprobe = 32, refine_factor = 4;
     int payload = IVF_PRODUCER_TMA;
-    int keep_raw = -1;              // -1 auto (yes), 0 no fp32 rows (first-stage distances only), 1 yes
+    int keep_raw = -1;              // -1 auto (yes), 0 no fp32 rows (first-stage distances only), 1 yes, 2 yes, in host memory
     int code_bytes = 0;
     int64_t n = 0, reserved = 0;
     bool trained = false, built = false, use_ivf = false;
     b200_corpus *raw = nullptr;     // fp32 rows in id order (cosine: unit vectors), metric L2 or IP
+    // keep_raw=2 on an inverted-file float index: raw's rows [h_rows_cap][d_pad] (same values, zero padding) in pinned,
+    // mapped host memory instead; the second stage gathers its candidates over PCIe
+    float *h_rows = nullptr;
+    const float *h_rows_dev = nullptr;   // the device's address of h_rows
+    int64_t h_rows_cap = 0;
     b200_corpus *coarse = nullptr;  // centroid table as a FLAT corpus (L2)
     float *d_centroids = nullptr;   // [nlist][d]
     float *d_cnorm = nullptr;       // [nlist] ||c||^2 (coarse probe)
@@ -1070,7 +1124,8 @@ struct b200_index {
     std::mutex mu;
     // workspaces (grow-only)
     DevArr w_rows, w_assign_i, w_assign_d, w_u32a, w_u32b, w_u32c, w_u32d, w_cnt, w_plan, w_sort, w_q, w_qraw, w_probe, w_pd, w_items,
-        w_qbuf, w_inv, w_ppb, w_pconst, w_qconst, w_qb, w_cs, w_pk, w_pi, w_pw, w_lk, w_li, w_alive, w_od, w_oi, w_cand, w_host_q, w_ppopc, w_lut;
+        w_qbuf, w_inv, w_ppb, w_pconst, w_qconst, w_qb, w_cs, w_pk, w_pi, w_pw, w_lk, w_li, w_alive, w_od, w_oi, w_cand, w_host_q, w_ppopc, w_lut,
+        w_stage;
     // statistics of the last search (tests, bench roofline): rows x payload bytes the scan kernel was asked to stream
     int64_t last_scan_rows = 0, last_items = 0;
     bool timing = false, timed_pending = false;
@@ -1186,6 +1241,7 @@ extern "C" int b200_index_free(b200_index *ix) {
     cudaSetDevice(ix->device);
     if (ix->stream) cudaStreamSynchronize(ix->stream);
     if (ix->raw) b200_corpus_free(ix->raw);
+    if (ix->h_rows) cudaFreeHost(ix->h_rows);
     if (ix->coarse) b200_corpus_free(ix->coarse);
     for (void *p : {(void *)ix->d_centroids, (void *)ix->d_bcent, (void *)ix->d_cnorm, (void *)ix->d_pq, (void *)ix->d_pq_bf16, (void *)ix->d_sq, ix->d_pool, (void *)ix->d_row_bias,
                     (void *)ix->d_row_ids, (void *)ix->d_list_len, (void *)ix->d_tail_page, (void *)ix->d_page_owner, (void *)ix->d_page_seq,
@@ -1194,7 +1250,7 @@ extern "C" int b200_index_free(b200_index *ix) {
     for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_cnt, &ix->w_plan,
                       &ix->w_sort, &ix->w_q, &ix->w_qraw, &ix->w_probe, &ix->w_pd, &ix->w_items, &ix->w_qbuf, &ix->w_inv, &ix->w_ppb, &ix->w_pconst, &ix->w_qb, &ix->w_cs,
                       &ix->w_qconst, &ix->w_pk, &ix->w_pi, &ix->w_pw, &ix->w_lk, &ix->w_li, &ix->w_alive, &ix->w_od, &ix->w_oi, &ix->w_cand,
-                      &ix->w_host_q, &ix->w_ppopc, &ix->w_lut})
+                      &ix->w_host_q, &ix->w_ppopc, &ix->w_lut, &ix->w_stage})
         a->release();
     if (ix->ev0) cudaEventDestroy(ix->ev0);
     if (ix->ev1) cudaEventDestroy(ix->ev1);
@@ -1225,6 +1281,37 @@ static size_t payload_row_bytes(const b200_index *ix) {
 
 // bytes of one caller row: fp32 [d], or binary [d / 8]
 static size_t in_row_bytes(const b200_index *ix) { return ix->binary ? (size_t)ix->row_bytes : (size_t)ix->d * 4; }
+
+// fp32 rows for the exact paths, in HBM (raw) or in host memory (h_rows)
+static bool has_rows(const b200_index *ix) { return ix->raw || ix->h_rows; }
+
+// the candidates' rows gathered from host memory take at most this much staging; larger batches re-rank in query chunks
+constexpr int64_t kHostStageBytes = (int64_t)256 << 20;
+
+// keep_raw=2: room for `rows` host rows in pinned, mapped memory; grows by allocate, copy the ix->n rows held, free
+static int host_rows_reserve(b200_index *ix, int64_t rows) {
+    if (ix->h_rows && ix->h_rows_cap >= rows) return B200_OK;
+    const size_t row_b = (size_t)ix->d_pad * 4, bytes = (size_t)rows * row_b, keep = (size_t)ix->n * row_b;
+    void *p = nullptr, *dp = nullptr;
+    if (cudaHostAlloc(&p, std::max<size_t>(bytes, 16), cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(B200_ERR_NOMEM, "cudaHostAlloc of the host rows failed (" + std::to_string(bytes) + " bytes)");
+    }
+    if (cudaHostGetDevicePointer(&dp, p, 0) != cudaSuccess) {
+        cudaGetLastError();
+        cudaFreeHost(p);
+        return fail(B200_ERR_CUDA, "cudaHostGetDevicePointer of the host rows failed");
+    }
+    if (ix->h_rows) {
+        memcpy(p, ix->h_rows, keep);
+        cudaFreeHost(ix->h_rows);
+    }
+    if (ix->d != ix->d_pad) memset(reinterpret_cast<char *>(p) + keep, 0, bytes - keep);   // the padding columns stay 0
+    ix->h_rows = reinterpret_cast<float *>(p);
+    ix->h_rows_dev = reinterpret_cast<const float *>(dp);
+    ix->h_rows_cap = rows;
+    return B200_OK;
+}
 
 // k-means on device rows x [n][stride]; centroids written to d_c [nc][d].  Assignment: exact top-1 search of the centroid
 // table with the FLAT engine (tensor cores from 20 rows up) when the table is large, the tiled fp32 kernel otherwise.
@@ -1672,6 +1759,10 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
             B200_TRY(b200_corpus_create(raw_metric, B200_DTYPE_F32, d, std::max<int64_t>(ix->reserved, n), &ix->raw));
         }
         B200_TRY(corpus_append_device(ix->raw, x, n, s));
+    } else if (ix->keep_raw == 2 && !ix->binary) {   // train resolved keep_raw=2 to 1 where the rows are the index
+        B200_TRY(host_rows_reserve(ix, std::max(ix->n + n, ix->reserved)));
+        B200_CUDA_OK(cudaMemcpy2DAsync(ix->h_rows + ix->n * ix->d_pad, (size_t)ix->d_pad * 4, x, (size_t)d * 4, (size_t)d * 4, n,
+                                       cudaMemcpyDeviceToHost, s));
     }
     if (!ix->use_ivf) {
         ix->n += n;
@@ -1905,6 +1996,61 @@ extern "C" int b200_index_memory_bytes(const b200_index *ix, uint64_t *out_bytes
     return B200_OK;
 }
 
+extern "C" int b200_index_host_memory_bytes(const b200_index *ix, uint64_t *out_bytes) {
+    if (!ix || !out_bytes) return fail(B200_ERR_INVALID, "bad arguments");
+    *out_bytes = ix->h_rows ? (uint64_t)ix->h_rows_cap * ix->d_pad * 4 : 0;
+    return B200_OK;
+}
+
+// moves a finalized inverted-file float index's fp32 rows between HBM (1) and pinned host memory (2)
+extern "C" int b200_index_set_raw_placement(b200_index *ix, int placement) {
+    if (!ix) return fail(B200_ERR_INVALID, "null index");
+    if (placement != 1 && placement != 2) return fail(B200_ERR_INVALID, "placement must be 1 (HBM) or 2 (pinned host memory)");
+    std::lock_guard<std::mutex> lk(ix->mu);
+    if (!ix->built) return fail(B200_ERR_INVALID, "index not finalized");
+    if (ix->binary || !ix->use_ivf)
+        return fail(B200_ERR_UNSUPPORTED, "the rows are the index here (FLAT, a part below the inverted-file threshold or a binary index): they stay in HBM");
+    if (ix->keep_raw != 1 && ix->keep_raw != 2) return fail(B200_ERR_INVALID, "this index keeps no fp32 rows (keep_raw=0)");
+    if (placement == ix->keep_raw) return B200_OK;
+    B200_CUDA_OK(cudaSetDevice(ix->device));
+    // searches enqueued on the callers' streams may still read the rows that are about to be freed
+    B200_CUDA_OK(cudaDeviceSynchronize());
+    const size_t row_b = (size_t)ix->d_pad * 4;
+    if (placement == 2 && ix->raw) {
+        B200_TRY(host_rows_reserve(ix, ix->n));
+        B200_CUDA_OK(cudaMemcpy(ix->h_rows, corpus_device_rows(ix->raw), (size_t)ix->n * row_b, cudaMemcpyDeviceToHost));
+        b200_corpus_free(ix->raw);
+        ix->raw = nullptr;
+    } else if (placement == 1 && ix->h_rows) {
+        const int raw_metric = ix->metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
+        b200_corpus *c = nullptr;
+        B200_TRY(b200_corpus_create(raw_metric, B200_DTYPE_F32, ix->d, ix->n, &c));
+        const int64_t chunk = std::max<int64_t>(1, kHostStageBytes / ((int64_t)ix->d * 4));
+        int rc = ix->w_rows.reserve((size_t)std::min(chunk, std::max<int64_t>(ix->n, 1)) * ix->d * 4);
+        for (int64_t off = 0; rc == B200_OK && off < ix->n; off += chunk) {   // unpadded [m][d] for the corpus append
+            const int64_t m = std::min(chunk, ix->n - off);
+            if (cudaMemcpy2DAsync(ix->w_rows.p, (size_t)ix->d * 4, ix->h_rows + off * ix->d_pad, row_b, (size_t)ix->d * 4, m, cudaMemcpyHostToDevice,
+                                  ix->stream) != cudaSuccess)
+                rc = fail(B200_ERR_CUDA, "host rows -> HBM copy failed");
+            else
+                rc = corpus_append_device(c, ix->w_rows.as<float>(), m, ix->stream);
+        }
+        ix->w_rows.release();
+        if (rc != B200_OK) {
+            b200_corpus_free(c);
+            return rc;
+        }
+        ix->raw = c;
+        cudaFreeHost(ix->h_rows);
+        ix->h_rows = nullptr;
+        ix->h_rows_dev = nullptr;
+        ix->h_rows_cap = 0;
+        ix->w_stage.release();
+    }
+    ix->keep_raw = placement;
+    return B200_OK;
+}
+
 extern "C" int b200_index_info(const b200_index *ix, int64_t *n, int *nlist, int *m, int *uses_ivf) {
     if (!ix) return fail(B200_ERR_INVALID, "null index");
     if (n) *n = ix->n;
@@ -1973,7 +2119,6 @@ static int refine_device(b200_index *ix, const float *d_q /*[nq][d_pad] prepared
                          int k, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
     RefineParams rp{};
     rp.queries = d_q;
-    rp.rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
     rp.cand = d_cand;
     rp.out_dis = d_out_dis;
     rp.out_ids = d_out_ids;
@@ -1985,9 +2130,33 @@ static int refine_device(b200_index *ix, const float *d_q /*[nq][d_pad] prepared
     rp.cosine = ix->metric == B200_METRIC_COSINE;
     rp.id_offset = id_offset;
     const size_t smem = (size_t)ix->d_pad * 4 + (size_t)9 * k * 8;
-    B200_CUDA_OK(cudaFuncSetAttribute(refine_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    refine_kernel<<<(unsigned)nq, 256, smem, s>>>(rp);
-    g_launches++;
+    if (!ix->h_rows) {
+        rp.rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
+        B200_CUDA_OK(cudaFuncSetAttribute(refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        refine_kernel<false><<<(unsigned)nq, 256, smem, s>>>(rp);
+        g_launches++;
+        B200_CUDA_OK(cudaGetLastError());
+        return B200_OK;
+    }
+    // rows in host memory: per chunk of queries, gather the candidates' rows over PCIe into the staging buffer (the grid is
+    // sized by candidate slots, so even one query's candidates spread over every SM), then re-rank from there
+    const int64_t per_q = (int64_t)ncand * ix->d_pad * 4;
+    const int64_t qchunk = std::max<int64_t>(1, std::min<int64_t>(nq, kHostStageBytes / per_q));
+    B200_TRY(ix->w_stage.reserve((size_t)qchunk * per_q));
+    B200_CUDA_OK(cudaFuncSetAttribute(refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    for (int64_t q0 = 0; q0 < nq; q0 += qchunk) {
+        const int64_t nqc = std::min(qchunk, nq - q0), slots = nqc * ncand;
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(slots, 8 * kGatherRows), (int64_t)ix->sms * 8));
+        gather_host_rows_kernel<<<grid, 256, 0, s>>>(ix->h_rows_dev, ix->n, ix->d_pad, d_cand + q0 * ncand, slots, ix->w_stage.as<float>());
+        RefineParams cp = rp;
+        cp.queries = d_q + q0 * ix->d_pad;
+        cp.rows = ix->w_stage.as<float>();
+        cp.cand = d_cand + q0 * ncand;
+        cp.out_dis = d_out_dis + q0 * k;
+        cp.out_ids = d_out_ids + q0 * k;
+        refine_kernel<true><<<(unsigned)nqc, 256, smem, s>>>(cp);
+        g_launches += 2;
+    }
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;
 }
@@ -2038,6 +2207,9 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     }
     const float *d_q = ix->w_q.as<float>();
     if (!ix->use_ivf || force_exact == 1) {
+        if (ix->keep_raw == 2)
+            return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available with the fp32 rows in host memory (keep_raw=2 placement): "
+                                              "the exact pass would stream every row over PCIe");
         if (!ix->raw) return fail(B200_ERR_INVALID, "exact search needs the fp32 rows (keep_raw=0 index)");
         // FLAT / fallback-to-flat: exact scan of the raw rows.  The raw corpus wants [nq][d] rows: strip the padding again.
         B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
@@ -2057,7 +2229,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     if (ix->binary && nprobe < nl && nprobe > 1024)
         return fail(B200_ERR_UNSUPPORTED, "binary indexes probe at most 1024 lists (the binary corpus k limit), or all of them (nprobe >= nlist)");
     const int refine_factor = std::max(1, parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", ix->refine_factor)));
-    const bool two_stage = ix->raw && refine_factor > 1 && !first_stage_only && !ix->binary;
+    const bool two_stage = has_rows(ix) && refine_factor > 1 && !first_stage_only && !ix->binary;
     const int k1 = two_stage ? std::min(1024, k * refine_factor) : k;
     if (out_num_candidates) *out_num_candidates = k1;
     const int64_t n_pairs = nq * nprobe;
@@ -2415,7 +2587,7 @@ extern "C" int b200_index_refine(b200_index *ix, const float *queries, int64_t n
         return fail(B200_ERR_INVALID, "bad arguments");
     if (!ix->built) return fail(B200_ERR_INVALID, "index not built");
     if (ix->binary) return fail(B200_ERR_UNSUPPORTED, "binary indexes have no second stage (their lists are exact)");
-    if (!ix->raw) return fail(B200_ERR_INVALID, "this index keeps no fp32 rows (keep_raw=0): no second stage");
+    if (!has_rows(ix)) return fail(B200_ERR_INVALID, "this index keeps no fp32 rows (keep_raw=0): no second stage");
     if (k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 in refine");
     if (nq == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ix->mu);
@@ -2476,7 +2648,8 @@ static int index_save_io(b200_index *ix, Io *f) {
     h.version = pq4 ? 3 : 2;
     h.reserved0 = pq4 ? 4 : 0;
     h.type = ix->type; h.metric = ix->metric; h.d = ix->d; h.nlist = ix->nlist; h.m = ix->m; h.dsub = ix->dsub;
-    h.default_nprobe = ix->default_nprobe; h.refine_factor = ix->refine_factor; h.payload = ix->payload; h.has_raw = ix->raw ? 1 : 0;
+    // has_raw 2: the same rows, to be loaded into host memory (keep_raw=2 placement)
+    h.default_nprobe = ix->default_nprobe; h.refine_factor = ix->refine_factor; h.payload = ix->payload; h.has_raw = ix->h_rows ? 2 : ix->raw ? 1 : 0;
     h.use_ivf = ix->use_ivf ? 1 : 0; h.code_bytes = ix->code_bytes; h.n = ix->n; h.pages_used = ix->pages_used;
     bool ok = wr(f, &h, sizeof(h));
     try {
@@ -2498,6 +2671,8 @@ static int index_save_io(b200_index *ix, Io *f) {
                 if (cudaMemcpy(buf.data(), rows + off * ix->d_pad, (size_t)mrows * ix->d_pad * 4, cudaMemcpyDeviceToHost) != cudaSuccess) ok = false;
                 for (int64_t r = 0; ok && r < mrows; r++) ok = wr(f, buf.data() + r * ix->d_pad, (size_t)ix->d * 4);
             }
+        } else if (ok && ix->h_rows) {   // the same bytes, straight from host memory
+            for (int64_t r = 0; ok && r < ix->n; r++) ok = wr(f, ix->h_rows + r * ix->d_pad, (size_t)ix->d * 4);
         }
         if (ok && ix->use_ivf) {
             std::vector<char> tmp;
@@ -2564,7 +2739,8 @@ static int index_load_io(Io *f, b200_index **out) {
                       h.n < (int64_t)0xffffffffll && h.payload >= 0 && h.payload <= 3 && (h.payload == IVF_PRODUCER_B1) == bin &&
                       (!h.use_ivf || (h.nlist > 0 && h.nlist <= (1 << 24) && (uint64_t)h.pages_used <= (uint64_t)h.n / kPageRows + (uint64_t)h.nlist + 1)) &&
                       (h.payload != IVF_PRODUCER_PQ || !h.use_ivf || (h.m > 0 && h.dsub > 0 && h.m * h.dsub == h.d && h.code_bytes >= (pq_bits == 4 ? (h.m + 1) / 2 : h.m) && h.code_bytes % 16 == 0)) &&
-                      (h.payload != IVF_PRODUCER_SQ8 || !h.use_ivf || (h.code_bytes >= h.d && h.code_bytes % 16 == 0)) && (h.has_raw || h.use_ivf);
+                      (h.payload != IVF_PRODUCER_SQ8 || !h.use_ivf || (h.code_bytes >= h.d && h.code_bytes % 16 == 0)) && (h.has_raw || h.use_ivf) &&
+                      h.has_raw >= 0 && h.has_raw <= 2 && (h.has_raw != 2 || (!bin && h.use_ivf));   // 2: host rows, float lists only
     if (!sane) return fail(B200_ERR_INVALID, "corrupt index header");
     b200_index *ix = nullptr;
     int rc = b200_index_create(kTypeNames[h.type], h.metric, h.d, "", &ix);
@@ -2586,6 +2762,15 @@ static int index_load_io(Io *f, b200_index **out) {
                 const int64_t mrows = std::min(chunk, h.n - off);
                 if (!rd(f, buf.data(), (size_t)mrows * rb)) return bail("truncated index file (rows)");
                 if (b200_corpus_append(ix->raw, buf.data(), mrows) != B200_OK) return bail(b200_last_error());
+            }
+        } else if (h.has_raw == 2) {   // straight into pinned host memory, never through HBM
+            if (host_rows_reserve(ix, h.n) != B200_OK) return bail(b200_last_error());
+            const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / ((int64_t)h.d * 4));
+            std::vector<float> buf((size_t)chunk * h.d);
+            for (int64_t off = 0; off < h.n; off += chunk) {
+                const int64_t mrows = std::min(chunk, h.n - off);
+                if (!rd(f, buf.data(), (size_t)mrows * h.d * 4)) return bail("truncated index file (rows)");
+                for (int64_t r = 0; r < mrows; r++) memcpy(ix->h_rows + (off + r) * ix->d_pad, buf.data() + r * h.d, (size_t)h.d * 4);
             }
         } else if (h.has_raw) {
             if (b200_corpus_create(raw_metric, B200_DTYPE_F32, h.d, h.n, &ix->raw) != B200_OK) return bail(b200_last_error());

@@ -474,6 +474,17 @@ class VectorIndex:
         _check(lib().b200_index_memory_bytes(self._h, C.byref(b)))
         return b.value
 
+    def host_memory_bytes(self):
+        """Pinned host bytes of the fp32 re-rank rows in host placement (keep_raw=2), else 0; memory_bytes() counts HBM only."""
+        b = C.c_uint64()
+        _check(lib().b200_index_host_memory_bytes(self._h, C.byref(b)))
+        return b.value
+
+    def set_raw_placement(self, placement: int):
+        """Move a finalized index's fp32 re-rank rows to HBM (1) or pinned host memory (2)."""
+        _check(lib().b200_index_set_raw_placement(self._h, C.c_int(placement)))
+        return self
+
     def info(self):
         n, nl, m, ivf = C.c_int64(), C.c_int(), C.c_int(), C.c_int()
         _check(lib().b200_index_info(self._h, C.byref(n), C.byref(nl), C.byref(m), C.byref(ivf)))

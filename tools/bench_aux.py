@@ -2,7 +2,7 @@
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
 workload; results are pasted into DESIGN.md section 7.
-Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter]"""
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows]"""
 import json
 import os
 import subprocess
@@ -404,6 +404,103 @@ def bench_pq4():
             print(json.dumps(pt), flush=True)
 
 
+def bench_host_rows():
+    """fp32 re-rank rows in HBM (keep_raw=1) against pinned host memory (keep_raw=2) on the pq_wide data (2 M clustered 768-d
+    rows, nlist 4096, k = 10, L2): SCANN (default M = 48, refine 16) and MSTG (refine 4), each built once and moved between
+    the placements with set_raw_placement, a round in each placement in turn after a warm-up round.  Per point and
+    placement: median call ms and refine-phase ms (phase_ms, CUDA events) with their spread; for the host placement the gather
+    rate (candidate rows gathered x d_pad x 4 B over the gather kernel's CUDA time, from torch.profiler in a separate
+    profiled pass); HBM bytes per row in both placements; and whether the outputs are byte-identical.  The same run times a
+    1 GB contiguous pinned -> device copy as the link's DMA figure."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    n, d, k, nlist = 2_000_000, 768, 10, 4096
+    y, qs = clustered(n, d, 10_000, seed=768, nq=1024)
+    ctx = gpu_context()
+    idx = {}
+    for name in ("SCANN", "MSTG"):
+        t0 = time.perf_counter()
+        idx[name] = b2.VectorIndex(name, b2.L2, d, f"ncentroids={nlist}, keep_raw=1").build(y)
+        idx[name].enable_timing(True)
+        print(json.dumps({"build": name, "m": idx[name].info()["m"], "build_s": round(time.perf_counter() - t0, 1)}), flush=True)
+    del y
+    hbm_row = {name: {} for name in idx}
+    for name, ix in idx.items():
+        hbm_row[name]["hbm"] = ix.memory_bytes() / n
+        ix.set_raw_placement(2)
+        hbm_row[name]["host"] = ix.memory_bytes() / n
+        hbm_row[name]["host_pinned"] = ix.host_memory_bytes() / n
+        ix.set_raw_placement(1)
+
+    # the link's DMA figure: 1 GB pinned -> device, CUDA events
+    h = torch.empty(1 << 28, dtype=torch.float32).pin_memory()
+    dv = torch.empty(1 << 28, dtype=torch.float32, device="cuda")
+    dma = []
+    for it in range(6):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        dv.copy_(h, non_blocking=True)
+        e1.record()
+        e1.synchronize()
+        if it:
+            dma.append(h.numel() * 4 / (e0.elapsed_time(e1) * 1e-3) / 1e9)
+    del h, dv
+    print(json.dumps({"dma_pinned_to_device_1GB_GB_per_s": round(float(np.median(dma)), 2), "spread": [round(min(dma), 2), round(max(dma), 2)], **ctx}),
+          flush=True)
+
+    def gather_ms(ix, q, prm, reps=3):
+        """CUDA time of gather_host_rows_kernel per search call (torch.profiler), None when the profiler sees none"""
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                ix.search(q, k, prm)
+            torch.cuda.synchronize()
+        us = [getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0) for e in prof.key_averages()
+              if "gather_host_rows_kernel" in e.key]
+        return sum(us) / reps / 1e3 if us else None
+
+    points = []
+    for nq in (1, 16, 256, 1024):
+        q = qs[:nq]
+        reps = 15 if nq <= 16 else 5
+        for nprobe in (4, 16):
+            prm = f"nprobe={nprobe}"
+            res = {}
+            for name, ix in idx.items():
+                call, ref, out = {1: [], 2: []}, {1: [], 2: []}, {}
+                for r in range(3):                      # round 0 warms both placements up and is not kept
+                    for pl in (1, 2):
+                        ix.set_raw_placement(pl)
+                        for it in range(reps if r else 2):
+                            t0 = time.perf_counter()
+                            out[pl] = ix.search(q, k, prm)
+                            t = time.perf_counter() - t0
+                            if r:
+                                call[pl].append(t * 1e3)
+                                ref[pl].append(ix.phase_ms()["refine"])
+                ncand = ix.last_num_candidates
+                _, cand = ix.search(q, ncand, prm, first_stage_only=True)   # the first stage the second one re-ranks
+                rows = int((cand >= 0).sum())
+                gms = gather_ms(ix, q, prm)
+                ix.set_raw_placement(1)
+                same = bool(np.array_equal(out[1][1], out[2][1]) and np.array_equal(out[1][0].view(np.uint32), out[2][0].view(np.uint32)))
+                e = dict(candidates=ncand, rows_gathered=rows, outputs_byte_identical=same,
+                         gather_kernel_ms=None if gms is None else round(gms, 4),
+                         gather_GB_per_s=None if not gms else round(rows * d * 4 / (gms * 1e-3) / 1e9, 2),
+                         hbm_bytes_per_row={"hbm": round(hbm_row[name]["hbm"], 1), "host": round(hbm_row[name]["host"], 1)},
+                         host_pinned_bytes_per_row=round(hbm_row[name]["host_pinned"], 1))
+                for pl, tag in ((1, "hbm"), (2, "host")):
+                    c, f = np.array(call[pl]), np.array(ref[pl])
+                    e[tag] = dict(call_ms=round(float(np.median(c)), 3), call_ms_spread=[round(float(c.min()), 3), round(float(c.max()), 3)],
+                                  refine_ms=round(float(np.median(f)), 4), refine_ms_spread=[round(float(f.min()), 4), round(float(f.max()), 4)])
+                res[name] = e
+            pt = dict(workload=f"host_rows {n} x {d} clustered, nlist={nlist}, k={k}, L2", nq=nq, nprobe=nprobe, reps=2 * reps, **ctx, **res)
+            points.append(pt)
+            print(json.dumps(pt), flush=True)
+    print(json.dumps({"workload": "host_rows summary", "all_outputs_byte_identical": all(p[nm]["outputs_byte_identical"] for p in points for nm in idx)}),
+          flush=True)
+
+
 def alive_bitmap(n, frac, clustered_runs, seed):
     """LSB-first bitmap keeping round(frac * n) rows (at least 1): uniformly random rows, or runs of up to 4096 contiguous
     rows at random starts (a tenant's rows are often contiguous)"""
@@ -510,4 +607,5 @@ if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
         {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
-         "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide, "pq4": bench_pq4, "prefilter": bench_prefilter}[w]()
+         "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide, "pq4": bench_pq4, "prefilter": bench_prefilter,
+         "host_rows": bench_host_rows}[w]()

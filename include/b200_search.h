@@ -261,7 +261,23 @@ int b200_index_info(const b200_index *ix, int64_t *n, int *nlist, int *m, int *u
  * item streams), "shared_bound=0" (do not share a per-query bound between the work items of a launch), "coarse_path=1|2|3" (centroid
  * probe by the scan kernel / the tensor-core top-k / score tiles + warp select; default 3 for nprobe > 8), "prefilter=0|1|2" (exact
  * paths of b200_index_search only -- FLAT, BINARYFLAT, the small-part fallback, exact_batch=1: as b200_corpus_set_prefilter;
- * the list scans of the IVF types are not affected). */
+ * the list scans of the IVF types are not affected).
+ * Filter-aware probing, float inverted-file types only (opt-in, because it changes answers): "filter_probe=1" with a filter
+ * given makes every query probe, in (coarse key, list id) order, the first
+ *   p_q = min(max_nprobe, max(nprobe, the fewest lists whose kept rows reach k1))
+ * lists (nlist when all of them do not reach it), k1 = min(1024, k x refine_factor) on two-stage searches, else k; of those
+ * it scans the lists that hold a kept row, and of each only the pages that hold one (leaving out the others changes no
+ * answer).  "max_nprobe=N" caps p_q (default nlist, clamped to [nprobe, nlist]; nprobe itself is unchanged).  With the
+ * default cap every query returns min(k, kept rows) rows.  Where p_q <= 1024, a query's answer is byte-identical to a
+ * filtered search of that query with "nprobe=p_q,coarse_path=3".
+ * The selection costs one device -> host read-back and ONE stream synchronise in mid-search per call, however large the
+ * batch (look-up-scan indexes included), in b200_index_search_device (and so b200_sharded_index_search) too.  When
+ * b200_index_search gets a host bitmap, the fp32 rows are in HBM and first_stage_only is 0, the exact pass over the kept
+ * rows answers instead (as "exact_batch=1") if the bitmap keeps at most 16 x nprobe x n / nlist rows AND that pass would
+ * score only the kept rows for this batch, i.e. within b200_corpus_set_prefilter's limit for the "prefilter" mode given (auto
+ * by default: a corpus of at least 512 MB and a share of at most 5 % / 12.5 %; 1 never; 2 up to n / 8 rows and 1 GiB of them).  nprobe >= nlist:
+ * only the page skipping.  Binary types: B200_ERR_UNSUPPORTED.
+ * Without a filter the key changes nothing. */
 int b200_index_search(b200_index *ix, const float *queries, int64_t nq, int k, const char *params, int first_stage_only,
                       const uint8_t *alive_bits /*nullable*/, float *out_dis, int64_t *out_ids, int64_t *out_num_candidates);
 /* same with device buffers, asynchronous on `stream` (NULL = the index's own stream, synchronised); id_offset is added to
@@ -276,6 +292,10 @@ int b200_index_list_sizes(const b200_index *ix, uint32_t *out_sizes /*[nlist]*/,
 int b200_index_enable_timing(b200_index *ix, int on);
 int b200_index_last_scan(b200_index *ix, int64_t *rows_streamed, int64_t *payload_row_bytes, int64_t *work_items,
                          double *kernel_ms_total, int64_t *kernel_launches, int reset);
+/* lists each query of the last search probed, out_lists[nq] (capacity >= nq, else B200_ERR_INVALID; null: skipped): p_q
+ * under filter_probe=1, nprobe on every other list search, 0 where an exact pass answered (FLAT, the small-part fallback,
+ * exact_batch=1, the filter_probe exact rule).  out_exact (nullable) = 1 when the filter_probe exact rule answered. */
+int b200_index_last_probe(b200_index *ix, int32_t *out_lists, int64_t capacity, int *out_exact);
 /* computeTopDistanceSubset: exact distances of candidate ids [nq][ncand] (negative = unused) -> top-k */
 int b200_index_refine(b200_index *ix, const float *queries, int64_t nq, const int64_t *cand_ids, int64_t ncand, int k,
                       float *out_dis, int64_t *out_ids);

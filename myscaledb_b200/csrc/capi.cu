@@ -867,6 +867,11 @@ int corpus_search_exact(b200_corpus *c, const void *d_queries, int64_t nq, int k
     if (alive >= 0 && alive <= limit) return search_gathered(c, d_queries, nq, k, d_alive, alive, id_offset, 0, d_out_dis, d_out_ids, s);
     return search_core(c, full_rows(c), d_queries, nq, k, d_alive, id_offset, 0, d_out_dis, d_out_ids, s);
 }
+
+// the host count above, for the index layer's filter_probe rule (stops past limit, as count_alive does)
+int64_t host_count_alive(const uint8_t *bits, int64_t n, int64_t limit) { return count_alive(bits, n, limit); }
+// the most kept rows for which corpus_search_exact takes the gathered path (-1: never), for the same filter_probe rule
+int64_t corpus_prefilter_limit(const b200_corpus *c, int mode, int64_t nq, int k) { return prefilter_limit(c, mode, nq, k); }
 }  // namespace b200
 
 extern "C" int b200_corpus_set_prefilter(b200_corpus *c, int mode) {

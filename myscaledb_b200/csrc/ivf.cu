@@ -1044,6 +1044,192 @@ __global__ void __launch_bounds__(256) gather_host_rows_kernel(const float *__re
     }
 }
 
+// ------------------------------------------------------------------------------------
+// filter_probe=1: per-search list state under the filter, and a probe depth per query that reaches k1 kept rows
+// ------------------------------------------------------------------------------------
+// One CTA per list walks its page chain, thread t on row t of every page: list_alive[l] = the list's rows the bitmap keeps;
+// f_pages[list_page_off[l] + j] = its pages with at least one kept row, in chain order; f_len[l] = the rows the plan and the
+// scan see through them (256 per kept page, and the original tail count if the list's last page is kept: only that page is
+// partial).  A dropped page holds no candidate, so the scan's answer does not change.
+__global__ void __launch_bounds__(256) list_alive_kernel(const uint32_t *list_len, const uint32_t *list_page_off, const uint32_t *list_pages,
+                                                         const uint32_t *row_ids, const uint8_t *alive, uint32_t *list_alive, uint32_t *f_len,
+                                                         uint32_t *f_pages) {
+    const int l = blockIdx.x;
+    const uint32_t len = list_len[l], pages = (len + kPageRows - 1) / kPageRows, off = list_page_off[l];
+    uint32_t kept_pages = 0, kept_rows = 0, flen = 0;
+    for (uint32_t j = 0; j < pages; j++) {
+        const uint32_t page = list_pages[off + j];
+        bool keep = false;
+        if (j * kPageRows + threadIdx.x < len) {
+            const uint32_t id = row_ids[(size_t)page * kPageRows + threadIdx.x];
+            keep = (alive[id >> 3] >> (id & 7)) & 1;
+        }
+        const uint32_t c = (uint32_t)__syncthreads_count(keep);
+        if (c) {
+            if (threadIdx.x == 0) f_pages[off + kept_pages] = page;
+            kept_pages++;
+            kept_rows += c;
+            flen = (kept_pages - 1) * kPageRows + min((uint32_t)kPageRows, len - j * kPageRows);
+        }
+    }
+    if (threadIdx.x == 0) {
+        list_alive[l] = kept_rows;
+        f_len[l] = flen;
+    }
+}
+
+// coarse keys as order-preserving u32 (-0 as +0, so that equal floats stay equal)
+__device__ __forceinline__ uint32_t coarse_key_u32(float f) {
+    const uint32_t u = __float_as_uint(f == 0.f ? 0.f : f);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+constexpr int kProbeThreads = 256;
+
+// The first `count` lists in (key, list id) order: every list with key < `key`, then the first `ties` lists with key == `key`
+// in list-id order.
+struct ProbeCut {
+    uint32_t key, ties, count;
+};
+
+// Shortest prefix of a query's lists in (key, id) order whose weight reaches `target`; weights min(w[l], target) (the test
+// W >= target is unchanged by the clamp, and the sums stay below 2^32), or 1 with w null.  count = nl when the whole row
+// does not reach it.  A radix select over the u32 keys (4 x 8 bits, histograms weighted), then the ties at the cut key in
+// list-id order (thread t owns a contiguous range of ids).  Called by every thread of the CTA.
+__device__ ProbeCut prefix_cut(const float *row, int nl, const uint32_t *w, uint32_t target) {
+    typedef cub::BlockScan<uint32_t, kProbeThreads> Scan;
+    typedef cub::BlockReduce<uint32_t, kProbeThreads> Reduce;
+    __shared__ union {
+        typename Scan::TempStorage scan;
+        typename Reduce::TempStorage red;
+    } tmp;
+    __shared__ uint32_t hist[256];
+    __shared__ uint32_t s_prefix, s_need, s_total, s_less, s_ties;
+    const int t = threadIdx.x;
+    uint32_t prefix = 0, mask = 0, need = target;
+    __syncthreads();   // a previous call's readers of the shared state are done
+    for (int shift = 24; shift >= 0; shift -= 8) {
+        for (int i = t; i < 256; i += kProbeThreads) hist[i] = 0;
+        __syncthreads();
+        for (int l = t; l < nl; l += kProbeThreads) {
+            const uint32_t u = coarse_key_u32(row[l]);
+            if ((u & mask) != prefix) continue;
+            const uint32_t wt = w ? min(w[l], target) : 1u;
+            if (wt) atomicAdd(&hist[(u >> shift) & 255], wt);
+        }
+        __syncthreads();
+        if (t == 0) {
+            if (shift == 24) {
+                uint32_t tot = 0;
+                for (int i = 0; i < 256; i++) tot += hist[i];
+                s_total = tot;
+            }
+            uint32_t acc = 0, b = 0;
+            for (; b < 255 && acc + hist[b] < need; b++) acc += hist[b];
+            s_prefix = prefix | (b << shift);
+            s_need = need - acc;
+        }
+        __syncthreads();
+        if (s_total < target) return {0xffffffffu, (uint32_t)nl, (uint32_t)nl};   // block-uniform
+        prefix = s_prefix;
+        need = s_need;
+        mask |= 255u << shift;
+    }
+    const int per = (nl + kProbeThreads - 1) / kProbeThreads;
+    const int l0 = min(nl, t * per), l1 = min(nl, l0 + per);
+    uint32_t less = 0, eq = 0, eq_w = 0;
+    for (int l = l0; l < l1; l++) {
+        const uint32_t u = coarse_key_u32(row[l]);
+        if (u < prefix) less++;
+        else if (u == prefix) {
+            eq++;
+            eq_w += w ? min(w[l], target) : 1u;
+        }
+    }
+    uint32_t eq_before, w_before;
+    Scan(tmp.scan).ExclusiveSum(eq, eq_before);
+    __syncthreads();
+    Scan(tmp.scan).ExclusiveSum(eq_w, w_before);
+    __syncthreads();
+    const uint32_t n_less = Reduce(tmp.red).Sum(less);
+    if (w_before < need && w_before + eq_w >= need) {   // the one thread whose range holds the cut
+        uint32_t acc = w_before, c = eq_before;
+        for (int l = l0; l < l1 && acc < need; l++) {
+            const uint32_t u = coarse_key_u32(row[l]);
+            if (u != prefix) continue;
+            c++;
+            acc += w ? min(w[l], target) : 1u;
+        }
+        s_ties = c;
+    }
+    if (t == 0) s_less = n_less;
+    __syncthreads();
+    return {prefix, s_ties, s_less + s_ties};
+}
+
+// The lists of a cut that hold a kept row, in list-id order: their count (every thread), and with out given, written to
+// out[0 ..).  A list without a kept row has a filtered length of 0: probing it adds no candidate, only a slot.  Called by
+// every thread of the CTA; thread t owns a contiguous range of list ids.
+__device__ uint32_t cut_live_lists(const float *row, int nl, const uint32_t *list_alive, uint32_t key, uint32_t ties, int64_t *out) {
+    typedef cub::BlockScan<uint32_t, kProbeThreads> Scan;
+    __shared__ typename Scan::TempStorage tmp;
+    const int t = threadIdx.x, per = (nl + kProbeThreads - 1) / kProbeThreads;
+    const int l0 = min(nl, t * per), l1 = min(nl, l0 + per);
+    uint32_t eq = 0;
+    for (int l = l0; l < l1; l++) eq += coarse_key_u32(row[l]) == key;
+    uint32_t eq_before, pos, total;
+    __syncthreads();   // a previous call's scan storage is free
+    Scan(tmp).ExclusiveSum(eq, eq_before);
+    uint32_t live = 0;
+    for (int l = l0, e = eq_before; l < l1; l++) {
+        const uint32_t u = coarse_key_u32(row[l]);
+        const bool in_cut = u < key || (u == key && (uint32_t)e++ < ties);
+        live += in_cut && list_alive[l] > 0;
+    }
+    __syncthreads();
+    Scan(tmp).ExclusiveSum(live, pos, total);
+    if (out)
+        for (int l = l0, e = eq_before; l < l1; l++) {
+            const uint32_t u = coarse_key_u32(row[l]);
+            const bool in_cut = u < key || (u == key && (uint32_t)e++ < ties);
+            if (in_cut && list_alive[l] > 0) out[pos++] = l;
+        }
+    return total;
+}
+
+// One CTA per query of a key chunk: p_q = min(max_nprobe, max(nprobe, the lists until W >= k1)), the cut of its first p_q
+// lists and live_out = how many of them hold a kept row (the lists it will probe).  totals[0] += live, totals[1] = max live.
+__global__ void __launch_bounds__(kProbeThreads) probe_select_kernel(const float *keys, int nl, const uint32_t *list_alive, uint32_t k1, int nprobe,
+                                                                     int max_nprobe, int *p_out, int *live_out, uint32_t *cut_key, uint32_t *cut_ties,
+                                                                     unsigned long long *totals) {
+    const int64_t q = blockIdx.x;
+    const float *row = keys + q * nl;
+    const ProbeCut wc = prefix_cut(row, nl, list_alive, k1);
+    const int p = min(max_nprobe, max(nprobe, (int)wc.count));
+    const ProbeCut c = p == (int)wc.count ? wc : prefix_cut(row, nl, nullptr, (uint32_t)p);
+    const uint32_t live = cut_live_lists(row, nl, list_alive, c.key, c.ties, nullptr);
+    if (threadIdx.x == 0) {
+        p_out[q] = p;
+        live_out[q] = (int)live;
+        cut_key[q] = c.key;
+        cut_ties[q] = c.ties;
+        atomicAdd(totals, (unsigned long long)live);
+        atomicMax(totals + 1, (unsigned long long)live);
+    }
+}
+
+// One CTA per query: its probe row [P] = the lists of its cut that hold a kept row, in list-id order, then -1 (an invalid
+// probe slot, which every later stage skips).
+__global__ void __launch_bounds__(kProbeThreads) probe_emit_kernel(const float *keys, int nl, const uint32_t *list_alive, const int *live_in,
+                                                                   const uint32_t *cut_key, const uint32_t *cut_ties, int P, int64_t *probe) {
+    const int64_t q = blockIdx.x;
+    int64_t *out = probe + q * P;
+    cut_live_lists(keys + q * nl, nl, list_alive, cut_key[q], cut_ties[q], out);
+    for (int j = live_in[q] + threadIdx.x; j < P; j += kProbeThreads) out[j] = -1;
+}
+
+__global__ void add_u64_kernel(const unsigned long long *src, unsigned long long *acc) { *acc += *src; }
+
 }  // namespace b200
 
 using namespace b200;
@@ -1126,6 +1312,14 @@ struct b200_index {
     DevArr w_rows, w_assign_i, w_assign_d, w_u32a, w_u32b, w_u32c, w_u32d, w_cnt, w_plan, w_sort, w_q, w_qraw, w_probe, w_pd, w_items,
         w_qbuf, w_inv, w_ppb, w_pconst, w_qconst, w_qb, w_cs, w_pk, w_pi, w_pw, w_lk, w_li, w_alive, w_od, w_oi, w_cand, w_host_q, w_ppopc, w_lut,
         w_stage;
+    // filter_probe=1 (per search): list_alive and the filtered lengths [2][nlist], the filtered page table [pages_used], the
+    // per-query selection (p_q, cut key, cut ties, then the Σ / max totals); pinned host copy of the totals and of every p_q
+    DevArr w_flist, w_fpages, w_fsel;
+    void *h_fsel = nullptr;
+    size_t h_fsel_cap = 0;
+    // lists each query of the last search probed (b200_index_last_probe), and whether the filter_probe exact rule answered it
+    std::vector<int32_t> last_probe;
+    bool last_probe_exact = false;
     // statistics of the last search (tests, bench roofline): rows x payload bytes the scan kernel was asked to stream
     int64_t last_scan_rows = 0, last_items = 0;
     bool timing = false, timed_pending = false;
@@ -1148,6 +1342,8 @@ int corpus_normalize_rows(b200_corpus *c);
 int corpus_append_device(b200_corpus *c, const float *d_rows, int64_t n, cudaStream_t s);
 int corpus_search_exact(b200_corpus *c, const void *d_queries, int64_t nq, int k, const uint8_t *d_alive, const uint8_t *h_alive,
                         int prefilter_mode, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s);
+int64_t host_count_alive(const uint8_t *bits, int64_t n, int64_t limit);
+int64_t corpus_prefilter_limit(const b200_corpus *c, int mode, int64_t nq, int k);
 }
 
 static int parse_int_param(const char *json, const char *key, int defv) {
@@ -1250,8 +1446,9 @@ extern "C" int b200_index_free(b200_index *ix) {
     for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_cnt, &ix->w_plan,
                       &ix->w_sort, &ix->w_q, &ix->w_qraw, &ix->w_probe, &ix->w_pd, &ix->w_items, &ix->w_qbuf, &ix->w_inv, &ix->w_ppb, &ix->w_pconst, &ix->w_qb, &ix->w_cs,
                       &ix->w_qconst, &ix->w_pk, &ix->w_pi, &ix->w_pw, &ix->w_lk, &ix->w_li, &ix->w_alive, &ix->w_od, &ix->w_oi, &ix->w_cand,
-                      &ix->w_host_q, &ix->w_ppopc, &ix->w_lut, &ix->w_stage})
+                      &ix->w_host_q, &ix->w_ppopc, &ix->w_lut, &ix->w_stage, &ix->w_flist, &ix->w_fpages, &ix->w_fsel})
         a->release();
+    if (ix->h_fsel) cudaFreeHost(ix->h_fsel);
     if (ix->ev0) cudaEventDestroy(ix->ev0);
     if (ix->ev1) cudaEventDestroy(ix->ev1);
     for (auto &e : ix->ev_ph)
@@ -2176,115 +2373,34 @@ __global__ void cosine_finish_kernel(const float *q, int64_t nq, int d, int d_pa
     dis[i] = ids[i] >= 0 ? 1.f - dis[i] : FLT_MAX;
 }
 
-// The whole search on the device, asynchronous on s.  d_queries: fp32 [nq][d]; outputs [nq][k].  h_alive: the host copy of
-// d_alive when the caller has one (the exact paths may then score only the rows it keeps), else null.
-static int search_device_locked(b200_index *ix, const float *d_queries, int64_t nq, int k, const char *params, int first_stage_only,
-                                const uint8_t *d_alive, const uint8_t *h_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids,
-                                int64_t *out_num_candidates, cudaStream_t s) {
-    if (out_num_candidates) *out_num_candidates = k;
-    if (nq == 0) return B200_OK;
-    const int force_exact = parse_int_param(params, "exact_batch", 0);
-    const int prefilter = parse_int_param(params, "prefilter", 0);   // A/B: 1 never, 2 whenever it fits (exact paths only)
-    if (prefilter < 0 || prefilter > 2) return fail(B200_ERR_INVALID, "prefilter must be 0 (auto), 1 (never) or 2 (always)");
-    if (pq_uses_lut(ix) && force_exact != 1 && k <= 1024) {
-        // the look-up scan's tables are nq x M KB (4-bit codes: nq x M x 64 B): a larger batch runs as consecutive query
-        // sub-batches through the whole search (every query's answer depends on that query alone, so the results are those of
-        // one batch)
-        const int64_t qmax = std::max<int64_t>(1, kPqLutScratchBytes / ((int64_t)ix->m * pq_codewords(ix->pq_bits) * 4));
-        if (nq > qmax) {
-            for (int64_t q0 = 0; q0 < nq; q0 += qmax)
-                B200_TRY(search_device_locked(ix, d_queries + q0 * ix->d, std::min(qmax, nq - q0), k, params, first_stage_only, d_alive, h_alive, id_offset,
-                                              d_out_dis + q0 * k, d_out_ids + q0 * k, out_num_candidates, s));
-            return B200_OK;
-        }
-    }
-    if (ix->binary) {
-        // binary queries are bytes [nq][d / 8]; list rows are exact, so refine_factor / keep_raw / first_stage_only change nothing
-        if (force_exact == 1) return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available on binary indexes (their lists are exact)");
-        if (!ix->use_ivf) return corpus_search_exact(ix->raw, d_queries, nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s);
-    } else {
-        B200_TRY(prepare_queries_device(ix, d_queries, nq, s));
-    }
-    const float *d_q = ix->w_q.as<float>();
-    if (!ix->use_ivf || force_exact == 1) {
-        if (ix->keep_raw == 2)
-            return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available with the fp32 rows in host memory (keep_raw=2 placement): "
-                                              "the exact pass would stream every row over PCIe");
-        if (!ix->raw) return fail(B200_ERR_INVALID, "exact search needs the fp32 rows (keep_raw=0 index)");
-        // FLAT / fallback-to-flat: exact scan of the raw rows.  The raw corpus wants [nq][d] rows: strip the padding again.
-        B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
-        if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
-        else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
-        B200_TRY(corpus_search_exact(ix->raw, ix->w_qraw.as<float>(), nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s));
-        if (ix->metric == B200_METRIC_COSINE) {
-            cosine_finish_kernel<<<(unsigned)ceil_div(nq * k, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, k, d_out_dis, d_out_ids);
-            g_launches++;
-        }
-        return B200_OK;
-    }
-    if (k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 on IVF indexes");
+// Pages of a list one work item streams for a scan of n_valid (query, list) pairs (see scan_probes); forced: the
+// "pages_per_chunk" A/B key, 0 = none.
+static uint32_t pages_per_chunk(const b200_index *ix, int64_t n_valid, int forced) {
+    const double avg_pages = std::max(1.0, (double)ix->pages_used / std::max(1, ix->nlist));
+    const double est_lists = std::min<double>((double)n_valid, (double)ix->nlist);
+    const double est_pages = est_lists * std::min<double>(ix->max_list_pages ? ix->max_list_pages : 1, 1.5 * avg_pages);
+    const double want_items = 4.0 * ix->sms;
+    // Lists probed by more than 16 queries run on per-lane top-k lists, whose cold start is paid per item: longer items pay;
+    // cooperative items (<= 16 queries) keep the 16-page cap.
+    const double q_per_list = (double)n_valid / std::max(1.0, est_lists);
+    const double cap = q_per_list > 16.0 ? 48.0 : 16.0;
+    uint32_t ppc = (uint32_t)std::min(cap, std::max(8.0, std::ceil(est_pages / want_items)));
+    if (est_lists * 2 < want_items) ppc = (uint32_t)std::max(2.0, std::min<double>(ppc, std::ceil(1.5 * avg_pages * est_lists / want_items)));   // a handful of queries
+    ppc = std::max<uint32_t>(ppc, (ix->max_list_pages + 63) / 64);   // at most 64 chunks per list
+    ppc = std::max<uint32_t>(ppc, 1);
+    if (forced) ppc = (uint32_t)forced;
+    return ppc;
+}
+
+// The steps of a list search after the coarse probe, asynchronous on s: pairs sorted by list, plan, query gather, grouped
+// scan, per-query merge, exact second stage.  probe: [nq][nprobe] list ids (negative = an invalid slot, skipped by every
+// step).  n_valid: the count of valid slots, sizing the gathered query rows, the work items and the partial lists.  list_len / list_pages: the index's own, or the filtered ones of filter_probe=1.
+static int scan_probes(b200_index *ix, const float *d_q, const float *d_queries, int64_t nq, int k, int k1, bool two_stage, const char *params,
+                       const int64_t *probe, int nprobe, int64_t n_valid, const uint32_t *list_len, const uint32_t *list_pages,
+                       const uint8_t *d_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
     const int nl = ix->nlist;
-    int nprobe = parse_int_param(params, "nprobe", ix->default_nprobe);
-    nprobe = std::max(1, std::min(nprobe, nl));
-    if (ix->binary && nprobe < nl && nprobe > 1024)
-        return fail(B200_ERR_UNSUPPORTED, "binary indexes probe at most 1024 lists (the binary corpus k limit), or all of them (nprobe >= nlist)");
-    const int refine_factor = std::max(1, parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", ix->refine_factor)));
-    const bool two_stage = has_rows(ix) && refine_factor > 1 && !first_stage_only && !ix->binary;
-    const int k1 = two_stage ? std::min(1024, k * refine_factor) : k;
-    if (out_num_candidates) *out_num_candidates = k1;
     const int64_t n_pairs = nq * nprobe;
     if (n_pairs >= (int64_t)1 << 31) return fail(B200_ERR_UNSUPPORTED, "nq * nprobe must stay below 2^31");
-
-    if (ix->timing) cudaEventRecord(ix->ev_ph[0], s);
-    // ---- coarse probe: nprobe nearest centroids per query (exact FLAT search of the centroid table)
-    B200_TRY(ix->w_probe.reserve((size_t)n_pairs * 8));
-    B200_TRY(ix->w_pd.reserve((size_t)n_pairs * 4));
-    if (ix->binary) {
-        if (nprobe >= nl) {
-            probe_all_kernel<<<(unsigned)ceil_div(n_pairs, 256), 256, 0, s>>>(ix->w_probe.as<int64_t>(), nq, nl);
-            g_launches++;
-        } else {
-            B200_TRY(pad_bin_rows(ix, d_queries, nq, ix->w_qraw, s));
-            B200_TRY(b200_corpus_search_device(ix->coarse, ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s));
-        }
-    } else {
-        B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
-        if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
-        else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
-        // The centroid table is small and nprobe is a large k for it: the tensor-core path keeps one k-list per query lane
-        // and never gets a selective threshold when k / nlist is a few percent.  The scan kernel's warp lists cost O(k / 32) per
-        // insert: use it when its estimated time (FMA-bound, ~1.4 TB/s of table bytes per 8-query pass) undercuts ~1 us per
-        // (query, 32 probes) of the tensor-core path.  Both rates of this model were taken on an earlier GPU and are
-        // not re-measured on the H100; they only pick between two exact paths.
-        const double t_scan = (double)ceil_div(nq, 8) * nl * ix->d_pad * 4.0 / 1.4e12;
-        const double t_gemm = 1e-6 * (double)nq * std::max(1.0, nprobe / 32.0) + 30e-6;
-        bool use_scan = nprobe > 8 && t_scan < t_gemm;
-        // nprobe > 8: full ranking keys + warp select (coarse_scores_kernel / coarse_select_kernel above)
-        int coarse_path = nprobe > 8 && nprobe <= 1024 ? 3 : use_scan ? 1 : 2;
-        if (const int forced = parse_int_param(params, "coarse_path", 0)) coarse_path = forced;   // A/B: 1 scan kernel, 2 tensor-core path, 3 select
-        if (coarse_path == 3) {
-            const int64_t chunk = std::max<int64_t>(64, std::min<int64_t>(nq, ((int64_t)64 << 20) / std::max(1, nl)));   // <= 256 MB of keys
-            B200_TRY(ix->w_cs.reserve((size_t)chunk * nl * 4));
-            const size_t sel_smem = (size_t)8 * nprobe * 8;
-            if (sel_smem > 48 * 1024) B200_CUDA_OK(cudaFuncSetAttribute(coarse_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
-            for (int64_t q0 = 0; q0 < nq; q0 += chunk) {
-                const int64_t nqc = std::min(chunk, nq - q0);
-                coarse_scores_kernel<<<dim3((unsigned)ceil_div(nl, kCoarseTile), (unsigned)ceil_div(nqc, kCoarseTile)), 256, 0, s>>>(
-                    d_q + q0 * ix->d_pad, ix->d_pad, ix->d_centroids, ix->d_cnorm, nqc, nl, ix->d, ix->w_cs.as<float>());
-                coarse_select_kernel<<<(unsigned)ceil_div(nqc, 8), 256, sel_smem, s>>>(ix->w_cs.as<float>(), nqc, nl, nprobe, ix->w_pd.as<float>() + q0 * nprobe,
-                                                                                       ix->w_probe.as<int64_t>() + q0 * nprobe);
-                g_launches += 2;
-            }
-            B200_CUDA_OK(cudaGetLastError());
-        } else {
-            b200_corpus_set_path(ix->coarse, coarse_path == 1 ? 1 : 0);
-            const int rc = b200_corpus_search_device(ix->coarse, ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s);
-            b200_corpus_set_path(ix->coarse, 0);
-            B200_TRY(rc);
-        }
-    }
-
-    if (ix->timing) cudaEventRecord(ix->ev_ph[1], s);
     // ---- pairs sorted by list
     B200_TRY(ix->w_u32a.reserve((size_t)n_pairs * 4));
     B200_TRY(ix->w_u32b.reserve((size_t)n_pairs * 4));
@@ -2292,7 +2408,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     B200_TRY(ix->w_u32d.reserve((size_t)n_pairs * 4));
     B200_TRY(ix->w_cnt.reserve((size_t)nl * 4));
     B200_CUDA_OK(cudaMemsetAsync(ix->w_cnt.p, 0, (size_t)nl * 4, s));
-    pairs_make_kernel<<<(unsigned)ceil_div(n_pairs, 256), 256, 0, s>>>(ix->w_probe.as<int64_t>(), n_pairs, nl, ix->w_u32a.as<uint32_t>(),
+    pairs_make_kernel<<<(unsigned)ceil_div(n_pairs, 256), 256, 0, s>>>(probe, n_pairs, nl, ix->w_u32a.as<uint32_t>(),
                                                                        ix->w_u32b.as<uint32_t>(), ix->w_cnt.as<uint32_t>());
     g_launches++;
     {
@@ -2313,25 +2429,10 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     // pays one cold start of its top-k lists.  The page counts (8 to 16, 48 below) were chosen on an earlier GPU and are
     // not re-measured on the H100.  The estimate uses host-side knowledge only (no device -> host round trip on the query path): probed
     // lists <= min(pairs, nlist), their length size-biased.
-    const double avg_pages = std::max(1.0, (double)ix->pages_used / std::max(1, nl));
-    const double est_lists = std::min<double>((double)n_pairs, (double)nl);
-    const double est_pages = est_lists * std::min<double>(ix->max_list_pages ? ix->max_list_pages : 1, 1.5 * avg_pages);
-    uint32_t ppc;
-    {
-        const double want_items = 4.0 * ix->sms;
-        // Lists probed by more than 16 queries run on per-lane top-k lists, whose cold start is paid per item: longer items pay;
-        // cooperative items (<= 16 queries) keep the 16-page cap.
-        const double q_per_list = (double)n_pairs / std::max(1.0, est_lists);
-        const double cap = q_per_list > 16.0 ? 48.0 : 16.0;
-        ppc = (uint32_t)std::min(cap, std::max(8.0, std::ceil(est_pages / want_items)));
-        if (est_lists * 2 < want_items) ppc = (uint32_t)std::max(2.0, std::min<double>(ppc, std::ceil(1.5 * avg_pages * est_lists / want_items)));   // a handful of queries
-        ppc = std::max<uint32_t>(ppc, (ix->max_list_pages + 63) / 64);   // at most 64 chunks per list
-        ppc = std::max<uint32_t>(ppc, 1);
-        if (const int forced = parse_int_param(params, "pages_per_chunk", 0)) ppc = (uint32_t)forced;
-    }
+    const uint32_t ppc = pages_per_chunk(ix, n_valid, parse_int_param(params, "pages_per_chunk", 0));
     const uint32_t max_chunks = (ix->max_list_pages + ppc - 1) / ppc;
-    const int64_t max_items = std::min<int64_t>((int64_t)n_pairs * max_chunks, (int64_t)(ceil_div(n_pairs, 128) + nl) * max_chunks);
-    const int64_t max_parts = n_pairs * max_chunks;
+    const int64_t max_items = std::min<int64_t>(n_valid * max_chunks, (int64_t)(ceil_div(n_valid, 128) + nl) * max_chunks);
+    const int64_t max_parts = n_valid * max_chunks;
     if (max_parts * k1 >= (int64_t)1 << 32) return fail(B200_ERR_UNSUPPORTED, "nq * nprobe * chunks * k too large for one batch; split the batch");
     B200_TRY(ix->w_items.reserve((size_t)max_items * sizeof(IvfGemmItem) + 64));
     B200_TRY(ix->w_plan.reserve((size_t)nl * 4 * 3));
@@ -2339,7 +2440,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     int *d_counts = ix->d_flag + 1;   // n_items, n_parts
     SearchPlan pl{};
     pl.cnt = ix->w_cnt.as<uint32_t>();
-    pl.list_len = ix->d_list_len;
+    pl.list_len = list_len;
     pl.list_page_off = ix->d_list_page_off;
     pl.list_order = ix->d_list_order;
     pl.pair_start = pair_start;
@@ -2358,9 +2459,9 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     const bool lut = pq_uses_lut(ix), pq4 = lut && ix->pq_bits == 4;
     const size_t qrow_bytes = ix->binary ? (size_t)ix->row_pad : (size_t)ix->d_pad64 * 2;
     if (!lut) {   // the table look-up scan reads no gathered query rows
-        B200_TRY(ix->w_qbuf.reserve(((size_t)n_pairs + 128) * qrow_bytes));
+        B200_TRY(ix->w_qbuf.reserve(((size_t)n_valid + 128) * qrow_bytes));
         // the 128 rows behind the last pair are read by the last items' A tiles (query slots without a query): keep them finite
-        B200_CUDA_OK(cudaMemsetAsync(ix->w_qbuf.as<char>() + (size_t)n_pairs * qrow_bytes, 0, (size_t)128 * qrow_bytes, s));
+        B200_CUDA_OK(cudaMemsetAsync(ix->w_qbuf.as<char>() + (size_t)n_valid * qrow_bytes, 0, (size_t)128 * qrow_bytes, s));
     }
     B200_TRY(ix->w_inv.reserve((size_t)n_pairs * 4));
     B200_TRY(ix->w_ppb.reserve((size_t)n_pairs * 4));
@@ -2418,7 +2519,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     IvfGemmParams gp{};
     gp.items = ix->w_items.as<IvfGemmItem>();
     gp.n_items_ptr = d_counts;
-    gp.list_pages = ix->d_list_pages;
+    gp.list_pages = list_pages;
     gp.row_bias = ix->d_row_bias;
     gp.row_ids = ix->d_row_ids;
     gp.alive = d_alive;
@@ -2470,7 +2571,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     }
     cudaError_t e = pq4   ? launch_ivf_pq4_topk(gp, grid, s, &detail)
                     : lut ? launch_ivf_pq_lut_topk(gp, grid, s, &detail)
-                          : launch_ivf_gemm_topk(gp, ix->w_qbuf.p, n_pairs + 128, ix->d_pool, (int64_t)ix->pool_pages * kPageRows, grid, s, &detail);
+                          : launch_ivf_gemm_topk(gp, ix->w_qbuf.p, n_valid + 128, ix->d_pool, (int64_t)ix->pool_pages * kPageRows, grid, s, &detail);
     if (ix->timing) {
         cudaEventRecord(ix->ev1, s);
         cudaEventRecord(ix->ev_ph[3], s);
@@ -2520,6 +2621,268 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     return B200_OK;
 }
 
+// Scratch budget of a filter_probe=1 batch after its selection: about kFilterProbeSlotBytes per probe slot [query][P] (the
+// probe row, the pair keys and their sort, the per-pair bookkeeping) plus, per valid slot, a gathered query row, work items
+// and partial lists.  A batch above it runs those steps on query sub-ranges: every query's answer depends on that query alone.
+constexpr int64_t kFilterProbeScratchBytes = 1ll << 30;
+constexpr int64_t kFilterProbeSlotBytes = 40;
+// The exact rule's limit in units of nprobe x n / nlist kept rows.  On 2 M x 768 rows (nprobe 16, nlist 4096, k 10, nq 1 -
+// 1024; H100 SXM at 700 W, DESIGN §7) the exact pass was faster than the lists at 1 % and 3 % of the rows (2.6 x and 7.7 x
+// nprobe x n / nlist) and slower at 10 % (25.6 x) for 3 of 4 batch sizes, so 1 (and 4) missed the faster path and 16 picks it.
+constexpr double kFilterProbeExactFactor = 16.0;
+
+// filter_probe=1 below nlist, after list_alive_kernel filtered the page table: the coarse keys of the batch (chunks of at most
+// 256 MB), one probe depth p_q per query and the number of its first p_q lists that hold a kept row, its live lists
+// (probe_select_kernel); ONE device -> host read-back (the 16-byte Σ / max of the live lists, with the nq values of p_q and of
+// the live lists) and a stream synchronise; then the probe rows [nq][P] of the live lists, P = max live lists, and the rest of
+// the search with nprobe := P, its buffers sized by the live lists.  Leaving out a list without a kept row changes no answer:
+// it holds no candidate and the merge does not depend on the order of its inputs.
+static int filter_probe_search(b200_index *ix, const float *d_q, int64_t nq, int k, int k1, bool two_stage, const char *params, int nprobe,
+                               const uint32_t *list_len, const uint32_t *list_pages, const uint8_t *d_alive, int64_t id_offset, float *d_out_dis,
+                               int64_t *d_out_ids, cudaStream_t s) {
+    const int nl = ix->nlist;
+    const int max_nprobe = std::max(nprobe, std::min(nl, parse_int_param(params, "max_nprobe", nl)));
+    const int64_t chunk = std::max<int64_t>(64, std::min<int64_t>(nq, ((int64_t)64 << 20) / std::max(1, nl)));   // <= 256 MB of keys
+    const bool one_chunk = nq <= chunk;
+    B200_TRY(ix->w_cs.reserve((size_t)chunk * nl * 4));
+    const size_t tot_off = round_up((size_t)nq * 16, 16);
+    B200_TRY(ix->w_fsel.reserve(tot_off + 24));
+    int *d_p = ix->w_fsel.as<int>(), *d_live = d_p + nq;
+    uint32_t *d_key = reinterpret_cast<uint32_t *>(d_live + nq), *d_ties = d_key + nq;
+    unsigned long long *d_tot = reinterpret_cast<unsigned long long *>(ix->w_fsel.as<char>() + tot_off);   // Σ live, max live, scan rows
+    B200_CUDA_OK(cudaMemsetAsync(d_tot, 0, 24, s));
+    auto coarse_keys = [&](int64_t q0, int64_t nqc) {
+        coarse_scores_kernel<<<dim3((unsigned)ceil_div(nl, kCoarseTile), (unsigned)ceil_div(nqc, kCoarseTile)), 256, 0, s>>>(
+            d_q + q0 * ix->d_pad, ix->d_pad, ix->d_centroids, ix->d_cnorm, nqc, nl, ix->d, ix->w_cs.as<float>());
+        g_launches++;
+    };
+    for (int64_t q0 = 0; q0 < nq; q0 += chunk) {
+        const int64_t nqc = std::min(chunk, nq - q0);
+        coarse_keys(q0, nqc);
+        probe_select_kernel<<<(unsigned)nqc, kProbeThreads, 0, s>>>(ix->w_cs.as<float>(), nl, ix->w_flist.as<uint32_t>(), (uint32_t)k1, nprobe,
+                                                                   max_nprobe, d_p + q0, d_live + q0, d_key + q0, d_ties + q0, d_tot);
+        g_launches++;
+    }
+    B200_CUDA_OK(cudaGetLastError());
+    const size_t hb = 16 + (size_t)nq * 8;
+    if (ix->h_fsel_cap < hb) {
+        if (ix->h_fsel) cudaFreeHost(ix->h_fsel);
+        ix->h_fsel = nullptr;
+        ix->h_fsel_cap = 0;
+        B200_CUDA_OK(cudaMallocHost(&ix->h_fsel, hb + hb / 4));
+        ix->h_fsel_cap = hb + hb / 4;
+    }
+    unsigned long long *h_tot = static_cast<unsigned long long *>(ix->h_fsel);
+    int32_t *h_p = reinterpret_cast<int32_t *>(h_tot + 2), *h_live = h_p + nq;
+    B200_CUDA_OK(cudaMemcpyAsync(h_tot, d_tot, 16, cudaMemcpyDeviceToHost, s));
+    B200_CUDA_OK(cudaMemcpyAsync(h_p, d_p, (size_t)nq * 8, cudaMemcpyDeviceToHost, s));   // p_q and live lists
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    const int64_t sum_live = (int64_t)h_tot[0];
+    const int P = std::max(1, (int)h_tot[1]);
+    ix->last_probe.insert(ix->last_probe.end(), h_p, h_p + nq);
+    if (ix->timing) cudaEventRecord(ix->ev_ph[1], s);
+
+    // Query ranges for the steps after the selection: the whole batch when its scratch, sized as scan_probes sizes it from
+    // its live lists, fits the budget; else consecutive ranges that each fit it (at least one query), each sized by its own.  On
+    // the look-up-scan indexes a range also keeps its per-query tables within kPqLutScratchBytes.
+    const int forced_ppc = parse_int_param(params, "pages_per_chunk", 0);
+    const int64_t qrow_bytes = pq_uses_lut(ix) ? 0 : (int64_t)ix->d_pad64 * 2;
+    auto scratch = [&](int64_t nqr, int64_t n_valid) {
+        const int64_t ppc = pages_per_chunk(ix, n_valid, forced_ppc);
+        const int64_t chunks = (ix->max_list_pages + ppc - 1) / ppc;
+        return nqr * P * kFilterProbeSlotBytes + n_valid * (qrow_bytes + chunks * ((int64_t)k1 * 8 + 4 + (int64_t)sizeof(IvfGemmItem)));
+    };
+    const int64_t qmax = pq_uses_lut(ix) ? std::max<int64_t>(1, kPqLutScratchBytes / ((int64_t)ix->m * pq_codewords(ix->pq_bits) * 4)) : nq;
+    std::vector<std::pair<int64_t, int64_t>> ranges;   // (end query, live lists of the range)
+    if (nq <= qmax && scratch(nq, sum_live) <= kFilterProbeScratchBytes) {
+        ranges.emplace_back(nq, sum_live);
+    } else {
+        for (int64_t a = 0; a < nq;) {
+            int64_t b = a + 1, v = h_live[a];
+            while (b < nq && b - a < qmax && scratch(b + 1 - a, v + h_live[b]) <= kFilterProbeScratchBytes) v += h_live[b++];
+            ranges.emplace_back(b, v);
+            a = b;
+        }
+    }
+    int64_t longest = 0;
+    for (size_t r = 0; r < ranges.size(); r++) longest = std::max(longest, ranges[r].first - (r ? ranges[r - 1].first : 0));
+    B200_TRY(ix->w_probe.reserve((size_t)longest * P * 8));
+    const bool split = ranges.size() > 1;
+    int64_t items = 0;
+    for (size_t r = 0; r < ranges.size(); r++) {
+        const int64_t a = r ? ranges[r - 1].first : 0, b = ranges[r].first;
+        // probe rows of queries [a, b): a one-chunk batch still has its keys, a larger one recomputes them (same kernel, same values)
+        for (int64_t q0 = a; q0 < b;) {
+            const int64_t q1 = one_chunk ? b : std::min(b, q0 + chunk);
+            if (!one_chunk) coarse_keys(q0, q1 - q0);
+            probe_emit_kernel<<<(unsigned)(q1 - q0), kProbeThreads, 0, s>>>(ix->w_cs.as<float>() + (one_chunk ? q0 * nl : 0), nl, ix->w_flist.as<uint32_t>(),
+                                                                           d_live + q0, d_key + q0, d_ties + q0, P, ix->w_probe.as<int64_t>() + (q0 - a) * P);
+            g_launches++;
+            q0 = q1;
+        }
+        B200_TRY(scan_probes(ix, d_q + a * ix->d_pad, nullptr, b - a, k, k1, two_stage, params, ix->w_probe.as<int64_t>(), P, ranges[r].second,
+                             list_len, list_pages, d_alive, id_offset, d_out_dis + a * k, d_out_ids + a * k, s));
+        items += ix->last_items;
+        if (split) {   // b200_index_last_scan reports the rows of the whole batch
+            add_u64_kernel<<<1, 1, 0, s>>>(reinterpret_cast<const unsigned long long *>(ix->d_flag + 4), d_tot + 2);
+            g_launches++;
+        }
+    }
+    if (split) B200_CUDA_OK(cudaMemcpyAsync(ix->d_flag + 4, d_tot + 2, 8, cudaMemcpyDeviceToDevice, s));
+    ix->last_items = items;
+    return B200_OK;
+}
+
+// The whole search on the device, asynchronous on s.  d_queries: fp32 [nq][d]; outputs [nq][k].  h_alive: the host copy of
+// d_alive when the caller has one (the exact paths may then score only the rows it keeps), else null.
+static int search_device_locked(b200_index *ix, const float *d_queries, int64_t nq, int k, const char *params, int first_stage_only,
+                                const uint8_t *d_alive, const uint8_t *h_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids,
+                                int64_t *out_num_candidates, cudaStream_t s) {
+    if (out_num_candidates) *out_num_candidates = k;
+    if (nq == 0) return B200_OK;
+    const int force_exact = parse_int_param(params, "exact_batch", 0);
+    const int prefilter = parse_int_param(params, "prefilter", 0);   // A/B: 1 never, 2 whenever it fits (exact paths only)
+    if (prefilter < 0 || prefilter > 2) return fail(B200_ERR_INVALID, "prefilter must be 0 (auto), 1 (never) or 2 (always)");
+    const int filter_probe = parse_int_param(params, "filter_probe", 0);
+    // filter_probe=1 below nlist keeps its look-up tables within the budget itself, under its one synchronise
+    const bool fselect_bounds_lut = filter_probe && d_alive && ix->use_ivf &&
+                                    std::max(1, parse_int_param(params, "nprobe", ix->default_nprobe)) < ix->nlist;
+    if (pq_uses_lut(ix) && force_exact != 1 && k <= 1024 && !fselect_bounds_lut) {
+        // the look-up scan's tables are nq x M KB (4-bit codes: nq x M x 64 B): a larger batch runs as consecutive query
+        // sub-batches through the whole search (every query's answer depends on that query alone, so the results are those of
+        // one batch)
+        const int64_t qmax = std::max<int64_t>(1, kPqLutScratchBytes / ((int64_t)ix->m * pq_codewords(ix->pq_bits) * 4));
+        if (nq > qmax) {
+            for (int64_t q0 = 0; q0 < nq; q0 += qmax)
+                B200_TRY(search_device_locked(ix, d_queries + q0 * ix->d, std::min(qmax, nq - q0), k, params, first_stage_only, d_alive, h_alive, id_offset,
+                                              d_out_dis + q0 * k, d_out_ids + q0 * k, out_num_candidates, s));
+            return B200_OK;
+        }
+    }
+    if (ix->binary) {
+        // binary queries are bytes [nq][d / 8]; list rows are exact, so refine_factor / keep_raw / first_stage_only change nothing
+        if (force_exact == 1) return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available on binary indexes (their lists are exact)");
+        if (filter_probe) return fail(B200_ERR_UNSUPPORTED, "filter_probe is not available on binary indexes (their coarse probe ranks at most 1024 lists)");
+        if (!ix->use_ivf) {
+            ix->last_probe.insert(ix->last_probe.end(), nq, 0);
+            return corpus_search_exact(ix->raw, d_queries, nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s);
+        }
+    } else {
+        B200_TRY(prepare_queries_device(ix, d_queries, nq, s));
+    }
+    const float *d_q = ix->w_q.as<float>();
+    bool exact = !ix->use_ivf || force_exact == 1;
+    if (!exact && filter_probe && d_alive && h_alive && ix->raw && !first_stage_only) {
+        // filter_probe exact rule: a filter that keeps at most kFilterProbeExactFactor x the rows one query's plain probe scans
+        // on average is answered by the exact pass over the kept rows (complete and exact) -- only when that pass takes its
+        // gathered path for this batch (prefilter mode, nq, k): past the gathered path's limit it would scan every row
+        const int np = std::max(1, std::min(parse_int_param(params, "nprobe", ix->default_nprobe), ix->nlist));
+        const int64_t limit = std::min<int64_t>((int64_t)(kFilterProbeExactFactor * np * (double)ix->n / (double)ix->nlist),
+                                                corpus_prefilter_limit(ix->raw, prefilter, nq, k));
+        exact = limit >= 0 && host_count_alive(h_alive, ix->n, limit) <= limit;
+        ix->last_probe_exact = exact;
+    }
+    if (exact) {
+        ix->last_probe.insert(ix->last_probe.end(), nq, 0);
+        if (ix->keep_raw == 2)
+            return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available with the fp32 rows in host memory (keep_raw=2 placement): "
+                                              "the exact pass would stream every row over PCIe");
+        if (!ix->raw) return fail(B200_ERR_INVALID, "exact search needs the fp32 rows (keep_raw=0 index)");
+        // FLAT / fallback-to-flat: exact scan of the raw rows.  The raw corpus wants [nq][d] rows: strip the padding again.
+        B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
+        if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
+        else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
+        B200_TRY(corpus_search_exact(ix->raw, ix->w_qraw.as<float>(), nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s));
+        if (ix->metric == B200_METRIC_COSINE) {
+            cosine_finish_kernel<<<(unsigned)ceil_div(nq * k, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, k, d_out_dis, d_out_ids);
+            g_launches++;
+        }
+        return B200_OK;
+    }
+    if (k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 on IVF indexes");
+    const int nl = ix->nlist;
+    int nprobe = parse_int_param(params, "nprobe", ix->default_nprobe);
+    nprobe = std::max(1, std::min(nprobe, nl));
+    if (ix->binary && nprobe < nl && nprobe > 1024)
+        return fail(B200_ERR_UNSUPPORTED, "binary indexes probe at most 1024 lists (the binary corpus k limit), or all of them (nprobe >= nlist)");
+    const int refine_factor = std::max(1, parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", ix->refine_factor)));
+    const bool two_stage = has_rows(ix) && refine_factor > 1 && !first_stage_only && !ix->binary;
+    const int k1 = two_stage ? std::min(1024, k * refine_factor) : k;
+    if (out_num_candidates) *out_num_candidates = k1;
+    // filter_probe=1 under a filter: the scan sees only the pages with kept rows, and below nlist every query probes as deep
+    // as its first k1 kept rows need
+    const bool fprobe = filter_probe && d_alive;
+    const bool fselect = fprobe && nprobe < nl;
+    const int64_t n_pairs = nq * nprobe;
+    if (!fselect && n_pairs >= (int64_t)1 << 31) return fail(B200_ERR_UNSUPPORTED, "nq * nprobe must stay below 2^31");
+    if (!fselect) ix->last_probe.insert(ix->last_probe.end(), nq, nprobe);
+
+    if (ix->timing) cudaEventRecord(ix->ev_ph[0], s);
+    const uint32_t *list_len = ix->d_list_len, *list_pages = ix->d_list_pages;
+    if (fprobe) {
+        B200_TRY(ix->w_flist.reserve((size_t)nl * 8));
+        B200_TRY(ix->w_fpages.reserve((size_t)std::max<uint32_t>(ix->pages_used, 1) * 4));
+        list_alive_kernel<<<(unsigned)nl, 256, 0, s>>>(ix->d_list_len, ix->d_list_page_off, ix->d_list_pages, ix->d_row_ids, d_alive,
+                                                       ix->w_flist.as<uint32_t>(), ix->w_flist.as<uint32_t>() + nl, ix->w_fpages.as<uint32_t>());
+        g_launches++;
+        list_len = ix->w_flist.as<uint32_t>() + nl;
+        list_pages = ix->w_fpages.as<uint32_t>();
+        if (fselect)
+            return filter_probe_search(ix, d_q, nq, k, k1, two_stage, params, nprobe, list_len, list_pages, d_alive, id_offset, d_out_dis, d_out_ids, s);
+    }
+    // ---- coarse probe: nprobe nearest centroids per query (exact FLAT search of the centroid table)
+    B200_TRY(ix->w_probe.reserve((size_t)n_pairs * 8));
+    B200_TRY(ix->w_pd.reserve((size_t)n_pairs * 4));
+    if (ix->binary) {
+        if (nprobe >= nl) {
+            probe_all_kernel<<<(unsigned)ceil_div(n_pairs, 256), 256, 0, s>>>(ix->w_probe.as<int64_t>(), nq, nl);
+            g_launches++;
+        } else {
+            B200_TRY(pad_bin_rows(ix, d_queries, nq, ix->w_qraw, s));
+            B200_TRY(b200_corpus_search_device(ix->coarse, ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s));
+        }
+    } else {
+        B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
+        if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
+        else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
+        // The centroid table is small and nprobe is a large k for it: the tensor-core path keeps one k-list per query lane
+        // and never gets a selective threshold when k / nlist is a few percent.  The scan kernel's warp lists cost O(k / 32) per
+        // insert: use it when its estimated time (FMA-bound, ~1.4 TB/s of table bytes per 8-query pass) undercuts ~1 us per
+        // (query, 32 probes) of the tensor-core path.  Both rates of this model were taken on an earlier GPU and are
+        // not re-measured on the H100; they only pick between two exact paths.
+        const double t_scan = (double)ceil_div(nq, 8) * nl * ix->d_pad * 4.0 / 1.4e12;
+        const double t_gemm = 1e-6 * (double)nq * std::max(1.0, nprobe / 32.0) + 30e-6;
+        bool use_scan = nprobe > 8 && t_scan < t_gemm;
+        // nprobe > 8: full ranking keys + warp select (coarse_scores_kernel / coarse_select_kernel above)
+        int coarse_path = nprobe > 8 && nprobe <= 1024 ? 3 : use_scan ? 1 : 2;
+        if (const int forced = parse_int_param(params, "coarse_path", 0)) coarse_path = forced;   // A/B: 1 scan kernel, 2 tensor-core path, 3 select
+        if (coarse_path == 3) {
+            const int64_t chunk = std::max<int64_t>(64, std::min<int64_t>(nq, ((int64_t)64 << 20) / std::max(1, nl)));   // <= 256 MB of keys
+            B200_TRY(ix->w_cs.reserve((size_t)chunk * nl * 4));
+            const size_t sel_smem = (size_t)8 * nprobe * 8;
+            if (sel_smem > 48 * 1024) B200_CUDA_OK(cudaFuncSetAttribute(coarse_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
+            for (int64_t q0 = 0; q0 < nq; q0 += chunk) {
+                const int64_t nqc = std::min(chunk, nq - q0);
+                coarse_scores_kernel<<<dim3((unsigned)ceil_div(nl, kCoarseTile), (unsigned)ceil_div(nqc, kCoarseTile)), 256, 0, s>>>(
+                    d_q + q0 * ix->d_pad, ix->d_pad, ix->d_centroids, ix->d_cnorm, nqc, nl, ix->d, ix->w_cs.as<float>());
+                coarse_select_kernel<<<(unsigned)ceil_div(nqc, 8), 256, sel_smem, s>>>(ix->w_cs.as<float>(), nqc, nl, nprobe, ix->w_pd.as<float>() + q0 * nprobe,
+                                                                                       ix->w_probe.as<int64_t>() + q0 * nprobe);
+                g_launches += 2;
+            }
+            B200_CUDA_OK(cudaGetLastError());
+        } else {
+            b200_corpus_set_path(ix->coarse, coarse_path == 1 ? 1 : 0);
+            const int rc = b200_corpus_search_device(ix->coarse, ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s);
+            b200_corpus_set_path(ix->coarse, 0);
+            B200_TRY(rc);
+        }
+    }
+
+    if (ix->timing) cudaEventRecord(ix->ev_ph[1], s);
+    return scan_probes(ix, d_q, d_queries, nq, k, k1, two_stage, params, ix->w_probe.as<int64_t>(), nprobe, n_pairs, list_len, list_pages, d_alive,
+                       id_offset, d_out_dis, d_out_ids, s);
+}
+
 static void timing_collect(b200_index *ix) {
     if (!ix->timing || !ix->timed_pending) return;
     float ms = 0;
@@ -2544,6 +2907,8 @@ extern "C" int b200_index_search_device(b200_index *ix, const float *d_queries, 
     B200_CUDA_OK(cudaSetDevice(ix->device));
     timing_collect(ix);
     cudaStream_t s = stream ? reinterpret_cast<cudaStream_t>(stream) : ix->stream;
+    ix->last_probe.clear();
+    ix->last_probe_exact = false;
     B200_TRY(search_device_locked(ix, d_queries, nq, k, params, first_stage_only, d_alive_bits, nullptr, id_offset, d_out_dis, d_out_ids, nullptr, s));
     if (!stream) B200_CUDA_OK(cudaStreamSynchronize(s));
     return B200_OK;
@@ -2560,6 +2925,8 @@ extern "C" int b200_index_search(b200_index *ix, const float *queries, int64_t n
     B200_CUDA_OK(cudaSetDevice(ix->device));
     timing_collect(ix);
     cudaStream_t s = ix->stream;
+    ix->last_probe.clear();
+    ix->last_probe_exact = false;
     B200_TRY(ix->w_host_q.reserve((size_t)nq * in_row_bytes(ix)));
     B200_TRY(ix->w_cand.reserve((size_t)nq * k * 12 + 16));
     B200_CUDA_OK(cudaMemcpyAsync(ix->w_host_q.p, queries, (size_t)nq * in_row_bytes(ix), cudaMemcpyHostToDevice, s));
@@ -2577,6 +2944,17 @@ extern "C" int b200_index_search(b200_index *ix, const float *queries, int64_t n
     B200_CUDA_OK(cudaMemcpyAsync(out_ids, r_i, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
     timing_collect(ix);
+    return B200_OK;
+}
+
+extern "C" int b200_index_last_probe(b200_index *ix, int32_t *out_lists, int64_t capacity, int *out_exact) {
+    if (!ix) return fail(B200_ERR_INVALID, "null index");
+    std::lock_guard<std::mutex> lk(ix->mu);
+    if (out_lists) {
+        if (capacity < (int64_t)ix->last_probe.size()) return fail(B200_ERR_INVALID, "buffer smaller than the last search's nq");
+        std::copy(ix->last_probe.begin(), ix->last_probe.end(), out_lists);
+    }
+    if (out_exact) *out_exact = ix->last_probe_exact ? 1 : 0;
     return B200_OK;
 }
 

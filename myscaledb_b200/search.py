@@ -406,6 +406,7 @@ class VectorIndex:
         self.d = d
         self._binary = metric in (HAMMING, JACCARD)
         _check(lib().b200_index_create(index_type.encode(), C.c_int(metric), C.c_int(d), params.encode(), C.byref(self._h)))
+        self._last_nq = 0
 
     def _rows(self, a):
         return np.ascontiguousarray(a, np.uint8 if self._binary else np.float32)
@@ -448,6 +449,7 @@ class VectorIndex:
                                               C.c_int(1 if first_stage_only else 0), C.c_void_p(alive_ptr or None),
                                               C.c_int64(id_offset), C.c_void_p(out_dis_ptr), C.c_void_p(out_ids_ptr),
                                               C.c_void_p(stream or None)))
+        self._last_nq = nq
 
     def enable_timing(self, on=True):
         _check(lib().b200_index_enable_timing(self._h, C.c_int(1 if on else 0)))
@@ -457,6 +459,15 @@ class VectorIndex:
         _check(lib().b200_index_last_scan(self._h, C.byref(rows), C.byref(rb), C.byref(items), C.byref(ms), C.byref(nl),
                                           C.c_int(1 if reset else 0)))
         return dict(rows_streamed=rows.value, payload_row_bytes=rb.value, work_items=items.value, kernel_ms=ms.value, launches=nl.value)
+
+    def last_probe(self):
+        """(lists each query of the last search probed, int32 [nq]; whether the filter_probe exact rule answered it).
+        filter_probe=1: p_q per query; other list searches: nprobe; exact passes: 0."""
+        n = self._last_nq
+        out = np.zeros(n, np.int32)
+        ex = C.c_int()
+        _check(lib().b200_index_last_probe(self._h, _p(out, C.c_int32), C.c_int64(n), C.byref(ex)))
+        return out, bool(ex.value)
 
     def phase_ms(self):
         a = (C.c_double * 5)()
@@ -501,6 +512,7 @@ class VectorIndex:
                                        C.c_int(1 if first_stage_only else 0), _p(ab, C.c_uint8), _p(dis, C.c_float),
                                        _p(ids, C.c_int64), C.byref(nc)))
         self.last_num_candidates = nc.value
+        self._last_nq = nq
         return dis, ids
 
     def save(self, path):
@@ -512,6 +524,7 @@ class VectorIndex:
         self._h = C.c_void_p()
         self.d = d
         self._binary = metric in (HAMMING, JACCARD)
+        self._last_nq = 0
         _check(lib().b200_index_load(str(path).encode(), C.byref(self._h)))
         return self
 

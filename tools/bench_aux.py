@@ -2,7 +2,7 @@
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
 workload; results are pasted into DESIGN.md section 7.
-Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows]"""
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows] [filtered]"""
 import json
 import os
 import subprocess
@@ -603,9 +603,100 @@ def bench_prefilter():
           flush=True)
 
 
+def bench_filtered():
+    """Filter-aware list probing: the pq_wide data (2 M clustered 768-d rows, nlist 4096), k = 10, nprobe = 16, MSTG
+    (keep_raw 1), SCANN and IVFFLAT under random filters (10 % to 0.001 %) and a correlated one (the rows of the centres
+    farthest from the queries), nq 1 / 16 / 256 / 1024.  The default search and filter_probe=1 alternate after a warm-up
+    round.  Per point and mode: short queries, recall@10 against the filtered FLAT answer, median call ms and its spread,
+    mean / max p_q, rows streamed and the path that answered.  For MSTG the two paths the exact rule picks between (the list
+    path through search_device, which has no host count, and exact_batch=1) are timed too."""
+    import torch
+
+    n, d, k, nlist, nprobe = 2_000_000, 768, 10, 4096, 16
+    rng = np.random.default_rng(768)
+    centres = rng.standard_normal((10_000, d)).astype(np.float32)
+    lab = np.empty(n, np.int64)
+    y = np.empty((n, d), np.float32)
+    for i in range(0, n, 500_000):   # the pq_wide rows, with their centres kept for the correlated filter
+        m = min(500_000, n - i)
+        lab[i:i + m] = rng.integers(0, 10_000, m)
+        y[i:i + m] = centres[lab[i:i + m]] + 0.3 * rng.standard_normal((m, d)).astype(np.float32)
+    qlab = rng.integers(0, 10_000, 1024)
+    qs = (centres[qlab] + 0.3 * rng.standard_normal((1024, d))).astype(np.float32)
+    ctx = gpu_context()
+    flat = b2.Corpus(b2.L2, d).append(y)
+    idx = {}
+    for name, typ in (("MSTG", "MSTG"), ("SCANN", "SCANN"), ("IVFFLAT", "IVFFLAT")):
+        t0 = time.perf_counter()
+        idx[name] = b2.VectorIndex(typ, b2.L2, d, f"ncentroids={nlist}" + (", keep_raw=1" if name == "MSTG" else "")).build(y)
+        print(json.dumps({"build": name, "build_s": round(time.perf_counter() - t0, 1)}), flush=True)
+    # correlated: the rows of the 20 centres farthest from the queries' mean (0.2 % of the rows, in lists no query probes)
+    far = np.argsort(-np.linalg.norm(centres - qs.mean(0), axis=1))[:20]
+    del y
+    filters = [(f"random {f:g}", f) for f in (0.1, 0.03, 0.01, 1e-3, 1e-4, 1e-5)] + [("correlated", None)]
+
+    def med(ts):
+        return round(1e3 * float(np.median(ts)), 3), round(1e3 * float(np.max(ts) - np.min(ts)), 3)
+
+    for fname, frac in filters:
+        if frac is None:
+            keep = np.isin(lab, far)
+            bits = np.packbits(keep, bitorder="little")
+        else:
+            bits, _ = alive_bitmap(n, frac, False, seed=int(frac * 1e6))
+            keep = np.unpackbits(bits, bitorder="little")[:n].astype(bool)
+        kept = int(keep.sum())
+        tbits = torch.from_numpy(bits).cuda()
+        for nq in (1, 16, 256, 1024):
+            q = qs[:nq]
+            _, truth = flat.search(q, k, alive_bits=bits)
+            tq = torch.from_numpy(q).cuda()
+            od = torch.empty((nq, k), dtype=torch.float32, device="cuda")
+            oi = torch.empty((nq, k), dtype=torch.int64, device="cuda")
+            reps = 5 if nq <= 16 else 3
+            for name, ix in idx.items():
+                modes = {"default": f"nprobe={nprobe}", "filter_probe": f"nprobe={nprobe}, filter_probe=1"}
+                if name == "MSTG":
+                    modes.update({"list_path": modes["filter_probe"], "exact_path": f"nprobe={nprobe}, exact_batch=1"})
+                ts = {m: [] for m in modes}
+                res, info = {}, {}
+                for it in range(reps + 1):          # round 0 warms every mode up and is not timed
+                    for m, prm in modes.items():
+                        t0 = time.perf_counter()
+                        if m == "list_path":
+                            ix.search_device(tq.data_ptr(), nq, k, od.data_ptr(), oi.data_ptr(), params=prm, alive_ptr=tbits.data_ptr())
+                            out = (od.cpu().numpy(), oi.cpu().numpy())
+                        else:
+                            out = ix.search(q, k, prm, alive_bits=bits)
+                        t = time.perf_counter() - t0
+                        if it:
+                            ts[m].append(t)
+                        else:
+                            p, ex = ix.last_probe()
+                            ls = ix.last_scan()
+                            res[m] = out
+                            path = "exact" if ex or m == "exact_path" else "lists"
+                            info[m] = dict(mean_p=round(float(p.mean()), 2), max_p=int(p.max()), path=path,
+                                           rows_streamed=ls["rows_streamed"] if path == "lists" else None)
+                pt = dict(workload=f"filtered pq_wide {n} x {d}, nlist={nlist}, nprobe={nprobe}, k={k}", index=name, filter=fname, kept=kept,
+                          nq=nq, **ctx)
+                for m in modes:
+                    ids = res[m][1]
+                    ms, spread = med(ts[m])
+                    pt[m] = dict(short_share=round(float(((ids >= 0).sum(1) < min(k, kept)).mean()), 4), recall=round(recall(ids, truth), 4),
+                                 call_ms=ms, call_ms_spread=spread, **info[m])
+                pt["identical_to_default"] = bool(np.array_equal(res["default"][1], res["filter_probe"][1])
+                                                  and res["default"][0].tobytes() == res["filter_probe"][0].tobytes())
+                if name == "MSTG":
+                    picked = pt["filter_probe"]["path"]
+                    faster = "exact" if pt["exact_path"]["call_ms"] < pt["list_path"]["call_ms"] else "lists"
+                    pt["rule_picked_faster"] = picked == faster
+                print(json.dumps(pt), flush=True)
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
         {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
          "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide, "pq4": bench_pq4, "prefilter": bench_prefilter,
-         "host_rows": bench_host_rows}[w]()
+         "host_rows": bench_host_rows, "filtered": bench_filtered}[w]()

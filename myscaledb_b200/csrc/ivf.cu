@@ -1567,8 +1567,9 @@ static int kmeans_device(const float *x, int64_t n, int64_t stride, int d, int n
                 if (h_cnt[i] == 0) empties.push_back(i);
             }
             if (!empties.empty()) {
+                // largest first, equal counts by the smaller cluster id: the pairing is a function of the counts alone
                 std::partial_sort(order.begin(), order.begin() + std::min<size_t>(nc, empties.size()), order.end(),
-                                  [&](int a, int b) { return h_cnt[a] > h_cnt[b]; });
+                                  [&](int a, int b) { return h_cnt[a] != h_cnt[b] ? h_cnt[a] > h_cnt[b] : a < b; });
                 std::vector<int> pairs;
                 for (size_t e = 0; e < empties.size() && e < (size_t)nc; e++) {
                     const int src = order[e];
@@ -1878,7 +1879,9 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
         B200_CUDA_OK(cudaMalloc(&d_l, (size_t)ns * 4));
         B200_CUDA_OK(cudaMalloc(&d_c32, (size_t)nl * 4));
         B200_CUDA_OK(cudaMalloc(&d_res, (size_t)ns * dsub * 4));
-        // the first ns rows of a strided view
+        // the first ns rows of a strided view.  Below 2 ns rows the stride is 1, so the codebooks are trained on the first 65536
+        // rows as given (tests/test_gpu_index_train.py pins this): one-shot build() already passes an even-strided sample, and
+        // a streamed train() of more rows than that should pass them in no particular order (not sorted by cluster)
         const int64_t step = std::max<int64_t>(1, n / ns);
         float *d_samp = nullptr;
         B200_CUDA_OK(cudaMalloc(&d_samp, (size_t)ns * d * 4));

@@ -22,7 +22,8 @@ constexpr int MAX_STAGES = 4;
 constexpr int SMEM_LIMIT = 232448;  // 227 KB of opt-in shared memory per block (sm_90)
 
 constexpr int SCRATCH_BYTES = 32 * EPI_THREADS * 4;  // IVF kernel: epilogue slow-path scratch [32][128] floats
-// Accumulator hand-off: the warpgroup's registers are written column-major into shared memory, 64 columns at a time
+// Accumulator hand-off of the IVF kernel (the flat kernel filters from the registers and stages only the groups of 32 columns that
+// can enter a list, ip_gemm_sm90.cu): the warpgroup's registers are written column-major into shared memory, 64 columns at a time
 // ([ACC_COLS][ACC_LD] floats; the padding of 4 makes both the fragment stores and the per-row reads of the epilogue
 // conflict-free).  It takes the place of tensor memory: the epilogue reads its query row in chunks of 32 columns.  Staging a
 // quarter of the tile rather than a half keeps 33 KB of shared memory for the operand ring, the lists and the PQ codebook.
@@ -178,16 +179,17 @@ __device__ __forceinline__ void wgmma_b1_n128(int32_t (&d)[64], uint64_t adesc, 
         : "l"(adesc), "l"(bdesc), "r"(accum));
 }
 
-// Store columns [COLS Q, COLS Q + COLS) of the warpgroup's two 64 x 128 accumulator fragments column-major into acc
-// ([COLS][ACC_LD]) as fp32 (s32 AND counts convert exactly: they are below 2^24).  Fragment layout of wgmma m64nN: warp w of
-// the warpgroup, lane l holds rows 16 w + l / 4 (+ 8) and columns 8 i + 2 (l % 4) (+ 1).
-template <int Q, int COLS = ACC_COLS, typename T>
+// Store columns [64 Q, 64 Q + 64) of the warpgroup's two 64 x 128 accumulator fragments column-major into acc
+// ([ACC_COLS][ACC_LD]) as fp32 (s32 AND counts convert exactly: they are below 2^24).  Fragment layout of wgmma m64nN: warp w
+// of the warpgroup, lane l holds rows 16 w + l / 4 (+ 8) and columns 8 i + 2 (l % 4) (+ 1), in d[4 i] (row, column),
+// d[4 i + 1] (row, column + 1), d[4 i + 2] (row + 8, column), d[4 i + 3] (row + 8, column + 1).
+template <int Q, typename T>
 __device__ __forceinline__ void acc_store(float *acc, const T (&d0)[64], const T (&d1)[64]) {
     const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
     const int r = warp * 16 + (lane >> 2), c = 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < COLS / 8; j++) {
-        const int i = Q * (COLS / 8) + j;
+    for (int j = 0; j < ACC_COLS / 8; j++) {
+        const int i = Q * (ACC_COLS / 8) + j;
         float *col = acc + (8 * j + c) * ACC_LD + r;
         col[0] = (float)d0[4 * i];
         col[ACC_LD] = (float)d0[4 * i + 1];
@@ -365,9 +367,17 @@ __device__ __forceinline__ void side_fma32(float (&v)[32], const float *scale, c
     }
 }
 
-// Jaccard keys of one chunk of 32 staged AND counts, with the integer expression and the IEEE division of binary_scan_kernel.
-// They are returned negated, for the max-tree form of epilogue_chunk.  scale / popc_y are the tile's side arrays in SHARED
-// memory; rows with side scale 0 (filtered, out of range) give -inf, i.e. key +inf, which never enters a list.
+// Jaccard key of one AND count (as fp32), with the integer expression and the IEEE division of binary_scan_kernel, returned
+// negated for the max-tree form of epilogue_chunk.  A row with side scale 0 (filtered, out of range) gives -inf, i.e. key +inf,
+// which never enters a list.
+__device__ __forceinline__ float jaccard_negkey(float v, int pq, float scale, float popc_y) {
+    const bool live = scale != 0.f;
+    const int x_and = (int)v, x_or = pq + (live ? (int)popc_y : 0) - x_and;
+    const float key = x_or == 0 ? 0.f : (float)(x_or - x_and) / (float)x_or;
+    return live ? -key : __int_as_float(0xff800000);
+}
+
+// jaccard_negkey of one chunk of 32 staged AND counts; scale / popc_y are the tile's side arrays in SHARED memory.
 __device__ __forceinline__ void jaccard_keys32(float (&v)[32], int pq, const float *scale, const float *popc_y) {
     const uint32_t sa = smem_u32(scale), ba = smem_u32(popc_y);
 #pragma unroll
@@ -376,12 +386,7 @@ __device__ __forceinline__ void jaccard_keys32(float (&v)[32], int pq, const flo
         asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(s[0]), "=f"(s[1]), "=f"(s[2]), "=f"(s[3]) : "r"(sa + j * 4));
         asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(b[0]), "=f"(b[1]), "=f"(b[2]), "=f"(b[3]) : "r"(ba + j * 4));
 #pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const bool live = s[i] != 0.f;
-            const int x_and = (int)v[j + i], x_or = pq + (live ? (int)b[i] : 0) - x_and;
-            const float key = x_or == 0 ? 0.f : (float)(x_or - x_and) / (float)x_or;
-            v[j + i] = live ? -key : __int_as_float(0xff800000);
-        }
+        for (int i = 0; i < 4; i++) v[j + i] = jaccard_negkey(v[j + i], pq, s[i], b[i]);
     }
 }
 

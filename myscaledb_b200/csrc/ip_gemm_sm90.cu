@@ -18,19 +18,20 @@
 //
 // One CTA = 128 queries (one query tile for its whole life) x corpus tiles of 256 rows (worker, worker + W, ...).  A tile is
 // computed as two N = 128 halves; per half, two wgmma m64n128 (query rows 0..63 / 64..127) per k-step accumulate in the
-// registers of one warpgroup, the result is staged column-major in shared memory and thread t of that warpgroup then filters
-// query row t in chunks of 32 columns into its private top-k list.
+// registers of one warpgroup.  Each warp of it holds 32 query rows of the fragment, and each lane of the warp owns the top-k
+// list of one of them; the warp tests every group of 32 columns from the registers and stages only a group that can enter a
+// list (see "hand-off" below).
 //   bf16 and binary rows: warps 0..3 and 4..7 are two consumer warpgroups, warpgroup w owns half w of every tile.  A stage of
 //               the ring holds the query k-block and the corpus k-block of all 256 rows, so the query k-block is fetched once
-//               per tile, not once per half.  The warpgroups share nothing but the ring: each has its own accumulator
-//               staging, side arrays, named barrier and per-query lists, and a CTA publishes two partial lists per query.
+//               per tile, not once per half.  The warpgroups share nothing but the ring: each has its own per-warp staging
+//               and per-query lists, and a CTA publishes two partial lists per query.
 //   fp32 rows:  warps 0..3 are the one consumer warpgroup; it walks both halves, a stage holds one half's corpus k-block
 //               (with the hi / lo planes a stage of both halves would leave no room for a ring).
 //   next warp   TMA producer (one lane), ring of full / empty mbarriers.
 // The key that is ranked is  acc * row_scale[j] + row_bias[j]  (smaller = better):
 //   IP: -acc | L2: ||y||^2 - 2 acc (+||q||^2 added at merge) | cosine: -acc / ||y|| | Hamming: popc(y) - 2 and (+popc(q) added
 //   at merge);  filtered / out-of-range rows: scale 0, bias +inf.
-//   Jaccard is not affine in the count: the thread maps its staged counts to keys itself (jaccard_keys32).
+//   Jaccard is not affine in the count: every group is staged, and the owner maps its counts to keys (jaccard_negkey).
 #include <cstdlib>
 #include <type_traits>
 
@@ -41,12 +42,9 @@ namespace gemm {
 
 // Shared-memory layout of gemm_topk_kernel per operand type, ring depth and list placement.
 //   [stage 0] .. [stage st - 1]   stage = [A hi][A lo][B (hi after the split) of WG halves][B lo]; lo planes: fp32 rows only
-//   per consumer warpgroup: accumulator staging [COLS][ACC_LD] floats (also the slow-path scratch of epilogue_chunk)
-//   per consumer warpgroup: side scale[SIDE_N], side bias[SIDE_N] of the tile rows the warpgroup owns
+//   per consumer warp: the staging buffer of the hand-off's slow path, [32 columns][32 query rows] floats, swizzled
 //   full / empty mbarriers
-//   per consumer warpgroup: the 128 per-thread lists, when they are kept in shared memory
-// Two warpgroups stage 32 accumulator columns at a time: 3 stages of 48 KB and two sets of 64-column staging and lists do not
-// fit in 227 KB.
+//   per consumer warpgroup: the 128 per-lane lists, when they are kept in shared memory
 template <Operand OP>
 struct Op {
     using L = Layout<OP>;   // operand geometry (k-block, planes); the offsets below are this kernel's own
@@ -63,14 +61,11 @@ struct Op {
     static constexpr int PASSES = BN / B_ROWS;               // halves a warpgroup walks per tile
     static constexpr int STAGE_BYTES = PLANES * (A_PLANE + WG * B_PLANE);
     static constexpr int TX_BYTES = PLANES * A_PLANE + WG * B_PLANE;   // what TMA writes (the B lo plane is computed)
-    static constexpr int COLS = WG == 1 ? ACC_COLS : 32;     // accumulator columns staged at a time
-    static constexpr int STAGING_BYTES = COLS * ACC_LD * 4;
-    static constexpr int SIDE_N = BN / WG;                   // side entries a warpgroup owns per tile
+    static constexpr int STAGING_BYTES = 32 * 32 * 4;        // per consumer warp
     static constexpr int MAX_ST = F32X3 ? 2 : 3;
     static_assert(MAX_ST <= MAX_STAGES, "barrier arrays");
-    __host__ __device__ static constexpr int off_acc(int st) { return st * STAGE_BYTES; }
-    __host__ __device__ static constexpr int off_side(int st) { return off_acc(st) + WG * STAGING_BYTES; }
-    __host__ __device__ static constexpr int off_bar(int st) { return off_side(st) + 2 * BN * 4; }
+    __host__ __device__ static constexpr int off_staging(int st) { return st * STAGE_BYTES; }
+    __host__ __device__ static constexpr int off_bar(int st) { return off_staging(st) + WG * 4 * STAGING_BYTES; }
     __host__ __device__ static constexpr int off_list(int st) { return off_bar(st) + 256; }
     static constexpr int list_bytes(int k_smem) { return k_smem * EPI_THREADS * 8; }   // one warpgroup's lists
     static size_t smem_bytes(int st, int k_smem) { return (size_t)off_list(st) + (size_t)WG * list_bytes(k_smem) + SMEM_ALIGN_SLACK; }
@@ -87,14 +82,68 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 template <int N>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
-// named barrier of one consumer warpgroup (ids 1 and 2; 0 is __syncthreads)
+// named barrier of the consumer warpgroup (id 1; 0 is __syncthreads): the fp32 corpus split before the MMAs read it
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
 
-// acc_store<q, COLS> for the q of an unrolled loop (the accumulator registers want compile-time indices)
-template <int COLS, int Q = 0, typename T>
-__device__ __forceinline__ void acc_store_cols(float *acc, const T (&d0)[64], const T (&d1)[64], int q) {
-    if (q == Q) acc_store<Q, COLS>(acc, d0, d1);
-    else if constexpr ((Q + 1) * COLS < HN) acc_store_cols<COLS, Q + 1>(acc, d0, d1, q);
+// ---- hand-off from the accumulator registers to the per-lane lists ----
+// Fragment layout of wgmma m64nN (acc_store): warp w of the warpgroup, lane l holds rows r = 16 w + l / 4 and r + 8 of the
+// M = 64 half in d0 (rows 0..63 of the query tile) and the same rows + 64 in d1, columns 8 i + 2 (l % 4) (+ 1).  So warp w
+// holds 32 query rows of the tile, and lane L of that warp owns the list of one of them ("slot" L):
+//   slot s < 16: row 16 w + s,   slot s >= 16: row 64 + 16 w + (s - 16).
+// A lane's four fragment rows r, r + 8, 64 + r, 72 + r ("rho" 0..3) are slots l / 4 + 8 rho.
+__device__ __forceinline__ int slot_row(int warp, int slot) { return (slot < 16 ? 0 : 48) + 16 * warp + slot; }
+
+// Group G of 32 columns of the half as negated keys (larger = better, the max-tree form of epilogue_chunk):
+// u[8 rho + 2 i + e] = column 8 i + 2 (l % 4) + e of the group, fragment row rho.
+//   plain IP (and the AND counts of Jaccard): the score;  side keys: -(acc * scale + bias).
+// sc / bi: the side entries of column 32 G + lane of the half (fetched by SHFL).  s32 accumulators (AND counts) hold the bits of
+// their fp32 value by now (acc_to_f32).
+__device__ __forceinline__ float acc_f32(float x) { return x; }
+__device__ __forceinline__ float acc_f32(int32_t x) { return __int_as_float(x); }
+template <int G, typename T>
+__device__ __forceinline__ void group_keys(float (&u)[32], const T (&d0)[64], const T (&d1)[64], bool side, float sc, float bi, int lane) {
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const int x = 4 * (4 * G + i);
+        u[2 * i] = acc_f32(d0[x]);
+        u[2 * i + 1] = acc_f32(d0[x + 1]);
+        u[8 + 2 * i] = acc_f32(d0[x + 2]);
+        u[8 + 2 * i + 1] = acc_f32(d0[x + 3]);
+        u[16 + 2 * i] = acc_f32(d1[x]);
+        u[16 + 2 * i + 1] = acc_f32(d1[x + 1]);
+        u[24 + 2 * i] = acc_f32(d1[x + 2]);
+        u[24 + 2 * i + 1] = acc_f32(d1[x + 3]);
+    }
+    if (!side) return;
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const int col = 8 * (j >> 1) + 2 * (lane & 3) + (j & 1);
+        const float s = __shfl_sync(0xffffffffu, sc, col), b = __shfl_sync(0xffffffffu, bi, col);
+#pragma unroll
+        for (int rho = 0; rho < 4; rho++) {
+            float &x = u[8 * rho + j];
+            x = -fmaf(x, s, b);
+        }
+    }
+}
+
+// group_keys for the g of a loop that is not unrolled (the accumulator registers want compile-time indices)
+template <int G = 0, typename T>
+__device__ __forceinline__ void group_keys_at(int g, float (&u)[32], const T (&d0)[64], const T (&d1)[64], bool side, const float (&sc)[4],
+                                              const float (&bi)[4], int lane) {
+    if (g == G) group_keys<G>(u, d0, d1, side, sc[G], bi[G], lane);
+    else if constexpr (G + 1 < HN / 32) group_keys_at<G + 1>(g, u, d0, d1, side, sc, bi, lane);
+}
+
+// Max over the quad of the lane's four fragment-row maxima m[rho], one row per lane (a reduce-scatter in three SHFL): lane l
+// ends with the row rho = 2 (l & 1) + (l & 2) / 2, i.e. owner slot l / 4 + 8 rho.
+__device__ __forceinline__ float quad_rows_max(const float (&m)[4], int lane) {
+    const bool b0 = lane & 1, b1 = lane & 2;
+    const float s0 = __shfl_xor_sync(0xffffffffu, b0 ? m[0] : m[2], 1);
+    const float s1 = __shfl_xor_sync(0xffffffffu, b0 ? m[1] : m[3], 1);
+    const float k0 = fmaxf(b0 ? m[2] : m[0], s0), k1 = fmaxf(b0 ? m[3] : m[1], s1);
+    const float s = __shfl_xor_sync(0xffffffffu, b1 ? k0 : k1, 2);
+    return fmaxf(b1 ? k1 : k0, s);
 }
 
 // x = hi + lo with both parts exactly representable in TF32 (so the result does not depend on how the tensor core
@@ -125,7 +174,8 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
     using O = Op<OP>;
     const int STAGES = p.stages;
     extern __shared__ unsigned char smem_dyn[];
-    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
+    // 1024-byte aligned, derived from smem_dyn by an offset so that the compiler keeps the shared address space
+    unsigned char *smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
     uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + O::off_bar(STAGES));
     uint64_t *empty_bar = full_bar + MAX_STAGES;
 
@@ -199,51 +249,53 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
         // ===================== consumer warpgroup: MMAs, then the fused top-k =====================
         if constexpr (O::WG == 2) setmaxnreg_inc<O::CONSUMER_REGS>();
         const int wg = threadIdx.x / EPI_THREADS;   // with two warpgroups: the half of every tile this one owns
-        const int row = threadIdx.x % EPI_THREADS;  // query row inside the tile
+        const int tid = threadIdx.x % EPI_THREADS;  // thread of the warpgroup = slot of its list in the interleaved lists
+        const int wwarp = tid >> 5;                 // warp of the warpgroup
+        const int qrow = slot_row(wwarp, lane);     // query row (inside the tile) of this lane's list
         const bool use_side = p.row_scale || p.row_bias || p.alive || p.scale_const != -1.f;
-        // everything the epilogue writes is private to the warpgroup: the two drift apart by up to the ring's depth
-        float *acc = reinterpret_cast<float *>(smem + O::off_acc(STAGES) + wg * O::STAGING_BYTES);
-        float *side_scale = reinterpret_cast<float *>(smem + O::off_side(STAGES)) + wg * 2 * O::SIDE_N;
-        float *side_bias = side_scale + O::SIDE_N;
+        const bool jaccard = OP == Operand::B1 && p.jaccard;
+        // everything the epilogue writes is private to the warp: the two warpgroups drift apart by up to the ring's depth
+        float *staging = reinterpret_cast<float *>(smem + O::off_staging(STAGES) + (wg * 4 + wwarp) * O::STAGING_BYTES);
+        const uint32_t staging_s = smem_u32(staging);
         // partial list  worker * WG + wg  of query tile qt (the merge reads [list][nq_pad][k])
         const size_t producer = ((size_t)worker * O::WG + wg) * p.q_tiles + qt;
         ThreadTopK list;
         list.n = 0;
         list.worst = 0;
         // rows past the batch (zero padding up to the tile size) must never pay for the slow path: nothing beats -FLT_MAX
-        list.thr_key = (qt * BM + row < p.nq_valid) ? FLT_MAX : -FLT_MAX;
+        list.thr_key = (qt * BM + qrow < p.nq_valid) ? FLT_MAX : -FLT_MAX;
         list.thr_id = 0;
         const int list_cap = list_cap_for(p.k);
         if (p.lists_in_smem) {
             unsigned char *lists = smem + O::off_list(STAGES) + wg * O::list_bytes(list_cap);
-            list_bind(list, reinterpret_cast<float *>(lists), reinterpret_cast<uint32_t *>(lists + O::list_bytes(list_cap) / 2), row, p.k);
+            list_bind(list, reinterpret_cast<float *>(lists), reinterpret_cast<uint32_t *>(lists + O::list_bytes(list_cap) / 2), tid, p.k);
         } else {
             list_bind(list, p.list_keys_gmem + producer * list_cap * EPI_THREADS, p.list_ids_gmem + producer * list_cap * EPI_THREADS,
-                      row, p.k);
+                      tid, p.k);
         }
-        // binary Jaccard: popc(q) of this thread's query row (0 for padding rows)
-        const int pq = (OP == Operand::B1 && p.jaccard && qt * BM + row < p.nq_valid) ? (int)p.q_popc[qt * BM + row] : 0;
+        // binary Jaccard: popc(q) of this lane's query row (0 for padding rows)
+        const int pq = (jaccard && qt * BM + qrow < p.nq_valid) ? (int)p.q_popc[qt * BM + qrow] : 0;
         const uint32_t smem0 = smem_u32(smem);
         int stage = 0;
         uint32_t phase = 0;
         typename O::Acc d0[64], d1[64];
         for (int64_t t = worker; t < n_tiles; t += W) {
             const int64_t n0 = t * BN;
-            // the side entries of this warpgroup's rows of the tile (in flight during the MMAs; written after the barrier below)
-            float sc[O::SIDE_N / EPI_THREADS], bi[O::SIDE_N / EPI_THREADS];
-            if (use_side) {
-#pragma unroll
-                for (int i = 0; i < O::SIDE_N / EPI_THREADS; i++) {
-                    const int64_t r = n0 + wg * O::SIDE_N + row + i * EPI_THREADS;
-                    bool ok = r < p.n;
-                    if (ok && p.alive) ok = (p.alive[r >> 3] >> (r & 7)) & 1;
-                    sc[i] = ok ? (p.row_scale ? p.row_scale[r] : p.scale_const) : 0.f;
-                    bi[i] = ok ? (p.row_bias ? p.row_bias[r] : 0.f) : __int_as_float(0x7f800000);
-                }
-            }
             const bool tail = n0 + BN > p.n;
             for (int pass = 0; pass < O::PASSES; pass++) {
                 const int h = O::WG == 1 ? pass : wg;   // the half of the tile
+                // side entries of columns 32 g + lane of the half (in flight during the MMAs)
+                float sc[HN / 32] = {}, bi[HN / 32] = {};
+                if (use_side) {
+#pragma unroll
+                    for (int g = 0; g < HN / 32; g++) {
+                        const int64_t r = n0 + h * HN + 32 * g + lane;
+                        bool ok = r < p.n;
+                        if (ok && p.alive) ok = (p.alive[r >> 3] >> (r & 7)) & 1;
+                        sc[g] = ok ? (p.row_scale ? p.row_scale[r] : p.scale_const) : 0.f;
+                        bi[g] = ok ? (p.row_bias ? p.row_bias[r] : 0.f) : __int_as_float(0x7f800000);
+                    }
+                }
                 int prev = -1;
                 for (int kb = 0; kb < kb_count; kb++) {
                     mbar_wait(&full_bar[stage], phase);
@@ -254,14 +306,14 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                         uint4 *bl = b + O::B_PLANE / 16;
 #pragma unroll
                         for (int i = 0; i < O::B_PLANE / 16 / EPI_THREADS; i++) {
-                            const uint4 raw = b[row + i * EPI_THREADS];
+                            const uint4 raw = b[tid + i * EPI_THREADS];
                             uint4 hi, lo;
                             split_tf32(raw.x, hi.x, lo.x);
                             split_tf32(raw.y, hi.y, lo.y);
                             split_tf32(raw.z, hi.z, lo.z);
                             split_tf32(raw.w, hi.w, lo.w);
-                            b[row + i * EPI_THREADS] = hi;
-                            bl[row + i * EPI_THREADS] = lo;
+                            b[tid + i * EPI_THREADS] = hi;
+                            bl[tid + i * EPI_THREADS] = lo;
                         }
                         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic stores -> wgmma operand reads
                         wg_bar(wg);
@@ -319,40 +371,74 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                 wgmma_wait<0>();
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                if constexpr (OP == Operand::B1) {
+                    // AND counts -> fp32 (exact: below 2^24), once, in place: the hand-off reads them as floats
 #pragma unroll
-                for (int q = 0; q < HN / O::COLS; q++) {
-                    wg_bar(wg);  // every row's reads of the previous staging (and of the previous tile's side arrays) are done
-                    if (pass == 0 && q == 0 && use_side) {
-#pragma unroll
-                        for (int i = 0; i < O::SIDE_N / EPI_THREADS; i++) {
-                            side_scale[row + i * EPI_THREADS] = sc[i];
-                            side_bias[row + i * EPI_THREADS] = bi[i];
-                        }
+                    for (int i = 0; i < 64; i++) {
+                        d0[i] = __float_as_int((float)d0[i]);
+                        d1[i] = __float_as_int((float)d1[i]);
                     }
-                    acc_store_cols<O::COLS>(acc, d0, d1, q);
-                    wg_bar(wg);
-                    // Chunks of 32 columns.  A chunk is first reduced to its best key (31 FMNMX); the per-element test only
-                    // runs for the rare chunk that can beat the current k-th key, and parks its keys where the chunk was staged.
+                }
+                // Fast path, from the registers: per group of 32 columns each lane reduces its fragment to the best negated
+                // key of each of its four rows (28 FMNMX), the quad to one row per lane (3 SHFL), which is tested against the
+                // owner's threshold with the non-strict test of epilogue_chunk, and one vote.  Thresholds only tighten, so the
+                // ones read before the four tests admit at least what epilogue_chunk will.
+                const float thr = __shfl_sync(0xffffffffu, fminf(list.thr_key, FLT_MAX), (lane >> 2) + 8 * (2 * (lane & 1) + ((lane >> 1) & 1)));
+                // Jaccard keys are not affine in the count: every group takes the slow path, where the owners key it.
+                uint32_t slow = jaccard ? (1u << HN / 32) - 1 : 0;   // groups where some owner of the warp may insert
+                if (!jaccard) {
+#pragma unroll
+                    for (int g = 0; g < HN / 32; g++) {
+                        float u[32], m[4];
+                        group_keys_at(g, u, d0, d1, use_side, sc, bi, lane);   // g is a constant here
+#pragma unroll
+                        for (int rho = 0; rho < 4; rho++) {
+                            const float *x = u + 8 * rho;
+                            m[rho] = fmaxf(fmaxf(fmaxf(x[0], x[1]), fmaxf(x[2], x[3])), fmaxf(fmaxf(x[4], x[5]), fmaxf(x[6], x[7])));
+                        }
+                        if (__any_sync(0xffffffffu, quad_rows_max(m, lane) >= -thr)) slow |= 1u << g;
+                    }
+                }
+                // Slow path: the warp stages such a group in its buffer, [column j][slot s] at j * 32 + (s ^ 8 ((j / 2) % 4))
+                // (conflict-free both for the fragment stores and for the owners' column reads), and each owner runs
+                // epilogue_chunk on its 32 columns, parking its keys over the buffer.
 #pragma unroll 1
-                    for (int cc = 0; cc < O::COLS / 32; cc++) {
-                        float v[32];
-                        acc_load32(acc, row, cc * 32, v);
-                        float *scratch = acc + cc * 32 * ACC_LD + row;
-                        const int c0 = h * HN + q * O::COLS + cc * 32;   // column of the tile
-                        const int s0 = c0 - wg * O::SIDE_N;               // ... and of this warpgroup's side arrays
-                        if (OP == Operand::B1 && p.jaccard) {
-                            jaccard_keys32(v, pq, side_scale + s0, side_bias + s0);
-                            epilogue_chunk<ACC_LD>(list, v, false, side_scale + s0, side_bias + s0, (uint32_t)(n0 + c0), tail, p.n, scratch);
-                        } else {
-                            epilogue_chunk<ACC_LD>(list, v, use_side, side_scale + s0, side_bias + s0, (uint32_t)(n0 + c0), tail, p.n, scratch);
+                while (slow) {
+                    const int g = __ffs(slow) - 1;
+                    slow &= slow - 1;
+                    float u[32];
+                    group_keys_at(g, u, d0, d1, use_side && !jaccard, sc, bi, lane);
+#pragma unroll
+                    for (int j = 0; j < 8; j++) {
+                        const int col = 8 * (j >> 1) + 2 * (lane & 3) + (j & 1);
+#pragma unroll
+                        for (int rho = 0; rho < 4; rho++) {
+                            const uint32_t a = staging_s + 4 * (col * 32 + (((lane >> 2) + 8 * rho) ^ (8 * (lane & 3))));
+                            asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(u[8 * rho + j]) : "memory");
                         }
                     }
+                    __syncwarp();
+                    float v[32];
+#pragma unroll
+                    for (int j = 0; j < 32; j++) {
+                        const uint32_t a = staging_s + 4 * (j * 32 + (lane ^ (8 * ((j >> 1) & 3))));
+                        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[j]) : "r"(a) : "memory");
+                    }
+                    __syncwarp();   // every owner holds its row before any parks keys over the buffer
+                    if (jaccard) {   // AND counts -> negated keys; column j's side entries are lane j's
+                        const float s = g == 0 ? sc[0] : g == 1 ? sc[1] : g == 2 ? sc[2] : sc[3];
+                        const float b = g == 0 ? bi[0] : g == 1 ? bi[1] : g == 2 ? bi[2] : bi[3];
+#pragma unroll
+                        for (int j = 0; j < 32; j++) v[j] = jaccard_negkey(v[j], pq, __shfl_sync(0xffffffffu, s, j), __shfl_sync(0xffffffffu, b, j));
+                    }
+                    epilogue_chunk<32>(list, v, false, nullptr, nullptr, (uint32_t)(n0 + h * HN + 32 * g), tail, p.n, staging + lane);
+                    __syncwarp();   // ... and the parked keys are read before the next group is staged
                 }
             }
         }
-        // publish this warpgroup's per-query partial list
-        float *ok = p.part_keys + (producer * BM + row) * p.k;
-        uint32_t *oi = p.part_ids + (producer * BM + row) * p.k;
+        // publish this lane's per-query partial list
+        float *ok = p.part_keys + (producer * BM + qrow) * p.k;
+        uint32_t *oi = p.part_ids + (producer * BM + qrow) * p.k;
         list_publish(list, ok, oi);
     }
 }

@@ -207,12 +207,24 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *                               the 8-bit default M when that default's sub-vector length is even (M = 96 at d = 768, 24 at
  *                               d = 96), else the 8-bit default (M = 10 at d = 250).  bit_size=8, or no bit_size, is the
  *                               8-bit index; any other value is refused at create with B200_ERR_UNSUPPORTED.  4-bit indexes
- *                               are saved as B2IX v3 (below);
+ *                               are saved as B2IX v3 (below).
+ *                               "aq_threshold=T" (IVFPQ, SCANN and HNSWPQ; other types ignore the key; 0 < T < 1, ScaNN
+ *                               recommends 0.2 for normalised data) trains and encodes with ScaNN's anisotropic loss
+ *                               ||r||^2 + w <r, x>^2 (r = x - x^ the row's reconstruction error, w = (eta - 1) / ||x||^2,
+ *                               eta = (d - 1) T^2 / (1 - T^2)), which weights the error along the row, the part that moves
+ *                               inner products, above the error across it: the codebooks take kAqIters coordinate-descent /
+ *                               least-squares iterations after k-means, and every added row takes the codes that lower its
+ *                               loss from the nearest-codeword ones (csrc/ivf_aq.cu).  Codes, scans and file are those of
+ *                               plain PQ (8 or 4 bits; an AQ index is an ordinary B2IX v2 / v3 file), and it composes with
+ *                               keep_raw, refine_factor, filter_probe and both build styles.  Absent or 0: plain PQ, file byte
+ *                               for byte.  A negative, >= 1 or non-numeric value is refused at create with B200_ERR_INVALID,
+ *                               a non-zero one under L2 with B200_ERR_UNSUPPORTED (the loss is defined for inner-product
+ *                               ranking), and d / M > 64 at train with B200_ERR_UNSUPPORTED;
  *   "MSTG"                      closed source upstream; here the two-stage index of SURVEY 2.5 K6: bf16 lists + exact
  *                               fp32 second stage (supportTwoStageSearch, first_stage_only, computeTopDistanceSubset);
  *   "SCANN", "HNSWFLAT", "HNSWSQ", "HNSWPQ"   accepted and SERVED BY THE INVERTED-FILE ENGINE with the payload their
- *                               name implies (PQ + re-rank, bf16, 8-bit, PQ): there is no graph traversal and no
- *                               anisotropic quantiser in this library; the contract for every ANN type is recall against
+ *                               name implies (PQ + re-rank, bf16, 8-bit, PQ): there is no graph traversal in this
+ *                               library (ScaNN's anisotropic PQ loss is the opt-in aq_threshold above); the contract for every ANN type is recall against
  *                               FLAT, not traversal order (SURVEY 8c: parity unpinned for ANN at large N);
  *   "BINARYFLAT"                binary rows (metric HAMMING or JACCARD, d in bits: a multiple of 8, at most 65536), exact
  *                               resident binary corpus (scan or b1 tensor-core kernel, chosen as for a binary corpus);
@@ -296,6 +308,10 @@ int b200_index_last_scan(b200_index *ix, int64_t *rows_streamed, int64_t *payloa
  * under filter_probe=1, nprobe on every other list search, 0 where an exact pass answered (FLAT, the small-part fallback,
  * exact_batch=1, the filter_probe exact rule).  out_exact (nullable) = 1 when the filter_probe exact rule answered. */
 int b200_index_last_probe(b200_index *ix, int32_t *out_lists, int64_t capacity, int *out_exact);
+/* aq_threshold indexes (tests, benchmarks): eta and the training sample's mean anisotropic loss after the k-means codebooks,
+ * then after each anisotropic iteration, out_loss[*out_n] (capacity >= *out_n, else B200_ERR_INVALID; null: skipped).
+ * B200_ERR_INVALID for an index not trained with the key here (plain PQ, other types, an index loaded from a file). */
+int b200_index_train_loss(const b200_index *ix, double *out_eta, double *out_loss, int capacity, int *out_n);
 /* computeTopDistanceSubset: exact distances of candidate ids [nq][ncand] (negative = unused) -> top-k */
 int b200_index_refine(b200_index *ix, const float *queries, int64_t nq, const int64_t *cand_ids, int64_t ncand, int k,
                       float *out_dis, int64_t *out_ids);

@@ -32,12 +32,11 @@
 #include <cub/cub.cuh>
 
 #include "common.cuh"
+#include "ivf_aq.h"
 #include "ivf_gemm.h"
 #include "kernels.h"
 
 namespace b200 {
-
-constexpr int kPageRows = 256;
 
 // ------------------------------------------------------------------------------------
 // k-means assignment: for every point the nearest centroid under L2 (argmin ||c||^2 - 2 x.c).
@@ -267,43 +266,6 @@ __global__ void __launch_bounds__(1024) add_plan_kernel(const AddPlan p) {
         if (fits) *p.pages_used = used + tot_pages;
         else *p.overflow = 1;
     }
-}
-
-// One warp per row of the list-sorted chunk: convert / encode the row into its pool slot, record its id and norm term.
-struct ScatterParams {
-    const float *rows;          // chunk rows fp32 [n][stride] (cosine: already unit length)
-    int64_t stride;
-    const uint32_t *sorted_list;  // [n] list of sorted element i
-    const uint32_t *sorted_row;   // [n] chunk row of sorted element i
-    const uint32_t *seg_start, *new_base, *first_new_seq, *list_len, *tail_page;
-    uint32_t id_base;
-    int64_t n;
-    int d, d_pad64;
-    int l2;
-    // bf16 payload
-    __nv_bfloat16 *pool;
-    // SQ8 payload
-    const float *sq_lo, *sq_inv_step, *sq_step;   // per dimension
-    // PQ payload
-    const float *centroids;     // [nlist][d]
-    const float *pq;            // [m][256][dsub] fp32 (nearest-centroid search)
-    const __nv_bfloat16 *pq_bf16;  // values the scan kernel will see (null: the fp32 ones, table look-up scan)
-    int m, dsub, pq_bits;          // pq_bits 4: pq is [m][16][dsub], codes two per byte (code j in byte j / 2, even j low)
-    uint8_t *codes;
-    int code_bytes;
-    float *row_bias;
-    uint32_t *row_ids;
-    int payload;
-    // binary payload: rows [n][stride] bytes -> pool bytes [page][row_pad / kb_w][256][kb_w]
-    const uint8_t *brows;
-    uint8_t *bpool;
-    int row_bytes, row_pad, kb_w;
-};
-
-__device__ __forceinline__ uint32_t pool_row_of(const ScatterParams &p, uint32_t l, uint32_t pos) {
-    const uint32_t seq = pos / kPageRows;
-    const uint32_t page = seq < p.first_new_seq[l] ? p.tail_page[l] : p.new_base[l] + (seq - p.first_new_seq[l]);
-    return page * kPageRows + (pos % kPageRows);
 }
 
 __global__ void __launch_bounds__(256) scatter_rows_kernel(const ScatterParams p) {
@@ -1272,6 +1234,10 @@ struct b200_index {
     int type = IDX_FLAT, metric = B200_METRIC_L2, d = 0, d_pad = 0, d_pad64 = 0;
     int nlist = 0, m = 0, dsub = 0;
     int pq_bits = 8;                // PQ code width: 8 (256 codewords, one byte per code) or 4 (16 codewords, two codes per byte)
+    // aq_threshold=T (PQ types, IP / cosine): anisotropic codebooks and codes (ivf_aq.cu) with eta = (d - 1) T^2 / (1 - T^2);
+    // 0: plain PQ.  aq_loss: the training sample's mean loss after the k-means codebooks, then after each iteration.
+    double aq_threshold = 0, aq_eta = 0;
+    std::vector<double> aq_loss;
     int default_nprobe = 32, refine_factor = 4;
     int payload = IVF_PRODUCER_TMA;
     int keep_raw = -1;              // -1 auto (yes), 0 no fp32 rows (first-stage distances only), 1 yes, 2 yes, in host memory
@@ -1362,6 +1328,27 @@ static int parse_int_param(const char *json, const char *key, int defv) {
     return defv;
 }
 
+// float value of a key, whole-word matched as parse_int_param: 0 with *out = defv when the key is absent, -1 when its value is
+// not a number (the value runs to the next ',', '"', '\'', '}', ' ' or the end)
+static int parse_float_param(const char *json, const char *key, double defv, double *out) {
+    *out = defv;
+    if (!json) return 0;
+    const size_t kl = strlen(key);
+    for (const char *p = strstr(json, key); p; p = strstr(p + 1, key)) {
+        const bool left_ok = p == json || !(isalnum((unsigned char)p[-1]) || p[-1] == '_');
+        const char *e = p + kl;
+        const bool right_ok = !(isalnum((unsigned char)*e) || *e == '_');
+        if (!left_ok || !right_ok) continue;
+        while (*e && (*e == '"' || *e == ':' || *e == '=' || *e == ' ' || *e == '\'')) e++;
+        char *end = nullptr;
+        const double v = (*e >= '0' && *e <= '9') || *e == '.' || *e == '-' || *e == '+' ? strtod(e, &end) : 0.0;
+        if (!end || end == e || !(*end == 0 || strchr(",\"'} ", *end)) || !std::isfinite(v)) return -1;
+        *out = v;
+        return 0;
+    }
+    return 0;
+}
+
 extern "C" int b200_index_create(const char *type, int metric, int d, const char *params, b200_index **out) {
     if (!type || !out || d <= 0) return fail(B200_ERR_INVALID, "bad arguments");
     *out = nullptr;
@@ -1384,6 +1371,14 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
     const bool pq_type = ty == IDX_IVFPQ || ty == IDX_SCANN || ty == IDX_HNSWPQ;
     const int pq_bits = pq_type ? parse_int_param(params, "bit_size", 8) : 8;
     if (pq_bits != 8 && pq_bits != 4) return fail(B200_ERR_UNSUPPORTED, "PQ bit_size must be 8 or 4, got " + std::to_string(pq_bits));
+    // anisotropic PQ (the PQ types only; the others ignore the key): 0 < T < 1, or 0 / absent for plain PQ
+    double aq_t = 0;
+    if (pq_type) {
+        if (parse_float_param(params, "aq_threshold", 0.0, &aq_t) != 0 || aq_t < 0 || aq_t >= 1)
+            return fail(B200_ERR_INVALID, "aq_threshold must be a number with 0 < T < 1 (or 0: plain PQ)");
+        if (aq_t > 0 && metric == B200_METRIC_L2)
+            return fail(B200_ERR_UNSUPPORTED, "aq_threshold: the anisotropic loss is defined for inner-product ranking (IP, COSINE), not L2");
+    }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
@@ -1398,9 +1393,12 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
     ix->nlist = parse_int_param(params, "ncentroids", parse_int_param(params, "nlist", 0));
     ix->m = parse_int_param(params, "M", parse_int_param(params, "m", 0));
     ix->pq_bits = pq_bits;
+    ix->aq_threshold = aq_t;
+    ix->aq_eta = (d - 1) * aq_t * aq_t / (1 - aq_t * aq_t);
     ix->default_nprobe = parse_int_param(params, "nprobe", 32);
-    // payload of a list row.  The graph types of the reference (hnswlib) and ScaNN have no graph / anisotropic quantiser
-    // here: they are SERVED by the inverted-file engine with the payload their suffix names (recall contract, SURVEY 8c).
+    // payload of a list row.  The graph types of the reference (hnswlib) and ScaNN have no graph here (ScaNN's anisotropic
+    // loss is the opt-in aq_threshold): they are SERVED by the inverted-file engine with the payload their suffix names
+    // (recall contract, SURVEY 8c).
     switch (ty) {
         case IDX_IVFPQ: case IDX_SCANN: case IDX_HNSWPQ: ix->payload = IVF_PRODUCER_PQ; break;
         case IDX_IVFSQ: case IDX_HNSWSQ: ix->payload = IVF_PRODUCER_SQ8; break;
@@ -1810,6 +1808,11 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
         }
         if (d % ix->m) return fail(B200_ERR_INVALID, "PQ M must divide the dimension");
         const int dsub = d / ix->m;
+        if (ix->aq_threshold > 0 && dsub > kAqMaxDsub)
+            return fail(B200_ERR_UNSUPPORTED, "aq_threshold: the codebook update solves for sub-vectors of at most " + std::to_string(kAqMaxDsub) +
+                                                  " dims (d / M <= " + std::to_string(kAqMaxDsub) + "), got d / M = " + std::to_string(dsub));
+        if (ix->aq_threshold > 0 && !aq_encoder_smem(d, ix->m))
+            return fail(B200_ERR_UNSUPPORTED, "aq_threshold: a row of d = " + std::to_string(d) + " does not fit the encoder's shared memory");
         if (ix->pq_bits == 4) {
             // the 4-bit look-up scan keeps one query's M x 64 B table in shared memory, at any d / M
             if (!ivf_pq4_fits(ix->m))
@@ -1896,6 +1899,12 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
                 g_launches++;
                 rc = kmeans_device(d_res, ns, dsub, dsub, ncw, 8, ix->d_pq + (size_t)j * ncw * dsub, s);
             }
+        }
+        if (rc == B200_OK && ix->aq_threshold > 0) {
+            // anisotropic iterations on the same sample, from the k-means codebooks (ivf_aq.cu)
+            const AqTrain at{d_samp, ns, d, m, dsub, ncw, d_l, ix->d_centroids, ix->d_pq, ix->aq_eta};
+            ix->aq_loss.clear();
+            rc = aq_train_codebooks(at, &ix->aq_loss, s);
         }
         if (rc == B200_OK && ix->d_pq_bf16) {
             cudaError_t e = launch_f32_to_bf16_rows(ix->d_pq, dsub, ix->d_pq_bf16, dsub, (int64_t)m * 256, s);
@@ -2058,6 +2067,7 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     if (over) return fail(B200_ERR_NOMEM, "page pool exhausted: more rows added than b200_index_reserve() announced");
     if (ix->binary) scatter_bin_rows_kernel<<<gridsz(n * 32), 256, 0, s>>>(sp);
     else scatter_rows_kernel<<<gridsz(n * 32), 256, 0, s>>>(sp);
+    if (ix->payload == IVF_PRODUCER_PQ && ix->aq_threshold > 0) B200_TRY(aq_encode_chunk(sp, ix->aq_eta, s));   // from the nearest codes
     add_commit_kernel<<<(unsigned)ceil_div(nl, 256), 256, 0, s>>>(ix->w_cnt.as<uint32_t>(), new_base, first_new, ix->d_list_len, ix->d_tail_page, nl);
     g_launches += 2;
     B200_CUDA_OK(cudaGetLastError());
@@ -2947,6 +2957,17 @@ extern "C" int b200_index_search(b200_index *ix, const float *queries, int64_t n
     B200_CUDA_OK(cudaMemcpyAsync(out_ids, r_i, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
     timing_collect(ix);
+    return B200_OK;
+}
+
+extern "C" int b200_index_train_loss(const b200_index *ix, double *out_eta, double *out_loss, int capacity, int *out_n) {
+    if (!ix) return fail(B200_ERR_INVALID, "bad arguments");
+    if (ix->aq_loss.empty()) return fail(B200_ERR_INVALID, "this index was not trained with aq_threshold (or is a loaded one)");
+    const int n = (int)ix->aq_loss.size();
+    if (out_loss && capacity < n) return fail(B200_ERR_INVALID, "train_loss: capacity " + std::to_string(capacity) + " < " + std::to_string(n));
+    if (out_eta) *out_eta = ix->aq_eta;
+    if (out_loss) std::copy(ix->aq_loss.begin(), ix->aq_loss.end(), out_loss);
+    if (out_n) *out_n = n;
     return B200_OK;
 }
 

@@ -469,6 +469,15 @@ class VectorIndex:
         _check(lib().b200_index_last_probe(self._h, _p(out, C.c_int32), C.c_int64(n), C.byref(ex)))
         return out, bool(ex.value)
 
+    def train_loss(self):
+        """aq_threshold indexes: (eta, float64 [1 + iterations] mean anisotropic loss of the training sample after the k-means
+        codebooks, then after each iteration).  B200Error for an index not trained with the key."""
+        eta, n = C.c_double(), C.c_int()
+        _check(lib().b200_index_train_loss(self._h, C.byref(eta), None, C.c_int(0), C.byref(n)))
+        out = np.zeros(n.value, np.float64)
+        _check(lib().b200_index_train_loss(self._h, C.byref(eta), _p(out, C.c_double), C.c_int(n.value), C.byref(n)))
+        return eta.value, out
+
     def phase_ms(self):
         a = (C.c_double * 5)()
         _check(lib().b200_index_phase_ms(self._h, a))

@@ -2,7 +2,7 @@
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
 workload; results are pasted into DESIGN.md section 7.
-Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows] [filtered]"""
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows] [filtered] [aq]"""
 import json
 import os
 import subprocess
@@ -694,9 +694,110 @@ def bench_filtered():
                 print(json.dumps(pt), flush=True)
 
 
+def bench_aq():
+    """Anisotropic PQ (aq_threshold=0.2) against plain PQ on the pq_wide data (2 M clustered 768-d rows, nlist 4096, k = 10),
+    normalised under COSINE and as given under IP, truth = FLAT: SCANN 8-bit (M = 48), SCANN 4-bit (M = 96) and IVFPQ's first
+    stage (M = 48), each built with and without the key.  Per build: train ms (on the sample build() would take) and add ms,
+    and the AQ sample-loss trajectory.  Per nq x nprobe and index pair: recall@10 at refine_factor 1, 2, 4, 8, 16 (IVFPQ: its
+    first stage), median call ms and list-scan kernel ms with their spread (plain and AQ alternating within every repeat after
+    a warm-up round), and with the re-rank rows in host memory (keep_raw=2 placement) the call time at the smallest refine
+    factor whose recall reaches the plain index's recall at 16.  BENCH_AQ_N overrides the row count (a rehearsal size),
+    BENCH_AQ_METRICS (cosine,ip) the metrics run."""
+    n = int(os.environ.get("BENCH_AQ_N", 2_000_000))
+    d, k, T = 768, 10, 0.2
+    nlist = 4096 if n >= 1_000_000 else max(16, int(4 * np.sqrt(n)))
+    rfs = (1, 2, 4, 8, 16)
+    y0, qs0 = clustered(n, d, 10_000 if n >= 1_000_000 else 64, seed=768, nq=1024)
+    ctx = gpu_context()
+    ns = min(n, max(256 * nlist, 65536))
+    sample = (np.arange(ns, dtype=np.float64) * float(n) / float(ns)).astype(np.int64)   # the rows build() trains on
+    kinds = (("SCANN8", "SCANN", f"ncentroids={nlist}, M=48"), ("SCANN4", "SCANN", f"ncentroids={nlist}, M=96, bit_size=4"),
+             ("IVFPQ8", "IVFPQ", f"ncentroids={nlist}, M=48, keep_raw=0"))
+    print(json.dumps({"workload": f"aq {n} x {d} clustered, nlist={nlist}, k={k}, aq_threshold={T}", **ctx}), flush=True)
+
+    def med(v):
+        v = np.array(v)
+        return dict(ms=round(float(np.median(v)), 3), spread=[round(float(v.min()), 3), round(float(v.max()), 3)])
+
+    want = os.environ.get("BENCH_AQ_METRICS", "cosine,ip").split(",")
+    for metric, mname in ((b2.COSINE, "cosine"), (b2.IP, "ip")):
+        if mname not in want:
+            continue
+        y, qs = y0, qs0
+        if metric == b2.COSINE:
+            y = y0 / np.linalg.norm(y0, axis=1, keepdims=True)
+            qs = qs0 / np.linalg.norm(qs0, axis=1, keepdims=True)
+        flat = b2.Corpus(metric, d).append(y)
+        idx = {}
+        for kind, typ, params in kinds:
+            for aq in (False, True):
+                name = kind + ("_aq" if aq else "")
+                ix = b2.VectorIndex(typ, metric, d, params + (f", aq_threshold={T}" if aq else ""))
+                ix.reserve(n)
+                t0 = time.perf_counter()
+                ix.train(y[sample])
+                t1 = time.perf_counter()
+                ix.add(y).finalize()
+                t2 = time.perf_counter()
+                ix.enable_timing(True)
+                idx[name] = ix
+                e = {"metric": mname, "build": name, "m": ix.info()["m"], "train_ms": round((t1 - t0) * 1e3, 1), "add_ms": round((t2 - t1) * 1e3, 1)}
+                if aq:
+                    eta, traj = ix.train_loss()
+                    e.update(eta=round(eta, 4), loss=[round(float(v), 6) for v in traj])
+                print(json.dumps(e), flush=True)
+        for nq in (1, 16, 256, 1024):
+            q = qs[:nq]
+            _, truth = flat.search(q, k)
+            reps = 7 if nq <= 16 else 3
+            for nprobe in (4, 16):
+                pt = dict(metric=mname, nq=nq, nprobe=nprobe, reps=reps)
+                for kind, _, _ in kinds:
+                    pair = (kind, kind + "_aq")
+                    fso = kind.startswith("IVFPQ")
+                    res = {name: {} for name in pair}
+                    for rf in ((1,) if fso else rfs):
+                        prm = f"nprobe={nprobe}, refine_factor={rf}"
+                        call, kern, out = {nm: [] for nm in pair}, {nm: [] for nm in pair}, {}
+                        for r in range(reps + 1):   # round 0 warms both up and is not kept
+                            for nm in pair:
+                                idx[nm].last_scan(reset=True)
+                                t0 = time.perf_counter()
+                                out[nm] = idx[nm].search(q, k, prm, first_stage_only=fso)
+                                t = time.perf_counter() - t0
+                                ls = idx[nm].last_scan(reset=True)
+                                if r:
+                                    call[nm].append(t * 1e3)
+                                    kern[nm].append(ls["kernel_ms"] / max(1, ls["launches"]))
+                        for nm in pair:
+                            res[nm][f"rf{rf}"] = dict(recall=round(recall(out[nm][1], truth), 4), call=med(call[nm]), scan=med(kern[nm]))
+                    if not fso:
+                        # rows in host memory: the call at the smallest refine factor reaching the plain index's recall at 16
+                        target = res[kind]["rf16"]["recall"]
+                        pick = {nm: next((rf for rf in rfs if res[nm][f"rf{rf}"]["recall"] >= target), 16) for nm in pair}
+                        host = {nm: [] for nm in pair}
+                        for nm in pair:
+                            idx[nm].set_raw_placement(2)
+                        for r in range(reps + 1):
+                            for nm in pair:
+                                t0 = time.perf_counter()
+                                idx[nm].search(q, k, f"nprobe={nprobe}, refine_factor={pick[nm]}")
+                                if r:
+                                    host[nm].append((time.perf_counter() - t0) * 1e3)
+                        for nm in pair:
+                            idx[nm].set_raw_placement(1)
+                            res[nm]["host_rows"] = dict(target_recall=target, refine_factor=pick[nm], call=med(host[nm]))
+                    pt.update(res)
+                print(json.dumps(pt), flush=True)
+        for ix in idx.values():
+            ix.close()
+        flat.close()
+        del idx, flat
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
         {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
          "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide, "pq4": bench_pq4, "prefilter": bench_prefilter,
-         "host_rows": bench_host_rows, "filtered": bench_filtered}[w]()
+         "host_rows": bench_host_rows, "filtered": bench_filtered, "aq": bench_aq}[w]()

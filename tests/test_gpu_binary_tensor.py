@@ -60,12 +60,18 @@ COMBOS = [(1, 1, b2.HAMMING, False), (129, 10, b2.JACCARD, True), (1024, 100, b2
 
 
 @pytest.mark.parametrize("n", [1, 255, 256, 257, 513, 70_000])
-@pytest.mark.parametrize("nbytes", [16, 48, 128, 144, 256])   # < one k-block, < one, exactly one, a partial second, two
+# < one k-block, < one, exactly one, a partial second, two; 4096 bits (4 k-blocks) and the widest rows, 65536 bits (64)
+@pytest.mark.parametrize("nbytes", [16, 48, 128, 144, 256, 512, 8192])
 def test_oracle_parity_at_tile_and_kblock_boundaries(n, nbytes):
     rng = np.random.default_rng(n * 1000 + nbytes)
-    y = rows(rng, n, nbytes)
     combos = COMBOS if n < 70_000 else COMBOS[:3]
+    wide = nbytes > 256                     # the oracle's time: at most 4 MB of rows and 2^29 row bytes x queries per call
+    if wide:
+        n = min(n, (1 << 22) // nbytes - 1)
+    y = rows(rng, n, nbytes)
     for nq, k, metric, with_alive in combos:
+        if wide:
+            nq = min(nq, max(1, (1 << 29) // (n * nbytes)))
         x = rows(rng, nq, nbytes)
         alive = orc.pack_bits(rng.random(n) < 0.7) if with_alive else None
         check_paths(metric, y, x, k, alive)

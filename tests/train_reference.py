@@ -331,14 +331,8 @@ def bin_list_lengths(xbytes, t):
 
 
 def read_binary_coarse(path):
-    """(header fields, centroid bytes u8 [nlist][cent_pad], list lengths int64 [nlist]) of a binary inverted-file index
-    file: the B2IX header, [n][d / 8] rows when has_raw, then the centroids and the list lengths (index_save_io)."""
-    raw = open(path, "rb").read()
-    h = np.frombuffer(raw, R.HEADER, count=1)[0]
-    assert h["magic"] == b"B2IX" and h["version"] == 2 and h["use_ivf"], "not a B2IX v2 inverted-file index"
-    rb, nl, n = int(h["d"]) // 8, int(h["nlist"]), int(h["n"])
-    off = R.HEADER.itemsize + (n * rb if h["has_raw"] else 0)
-    cp = cent_pad(rb)
-    cent = np.frombuffer(raw, np.uint8, count=nl * cp, offset=off).reshape(nl, cp)
-    lens = np.frombuffer(raw, "<u4", count=nl, offset=off + nl * cp).astype(np.int64)
-    return h, cent, lens
+    """(decoded index, centroid bytes u8 [nlist][cent_pad], list lengths int64 [nlist]) of a binary inverted-file index file,
+    decoded whole by tests/binary_ivf_reference.read_binary_index."""
+    from tests import binary_ivf_reference as B   # that module builds on this one
+    s = B.read_binary_index(path)
+    return s, s.centroids, s.list_len

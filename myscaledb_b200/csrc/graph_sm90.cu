@@ -1,0 +1,446 @@
+// graph_sm90.cu -- the neighbour graph of an HNSWFLAT index (graph_degree=D): candidate lists -> rank-based pruning ->
+// reverse edges and merge at build, and the one-CTA-per-query graph search (DESIGN §3).
+#include <cub/cub.cuh>
+
+#include "common.cuh"
+#include "graph.h"
+
+namespace b200 {
+
+// ------------------------------------------------------------------------------------
+// build
+// ------------------------------------------------------------------------------------
+__global__ void graph_candidates_kernel(const int64_t *__restrict__ ids, int64_t m, int64_t row0, int K, uint32_t *__restrict__ cand) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const int64_t *row = ids + i * (K + 1);
+    int self = K;   // absent (duplicate rows): drop the last entry
+    for (int j = 0; j < K + 1; j++)
+        if (row[j] == row0 + i) {
+            self = j;
+            break;
+        }
+    uint32_t *out = cand + i * K;
+    for (int j = 0, o = 0; j < K + 1; j++) {
+        if (j == self) continue;
+        out[o++] = row[j] >= 0 ? (uint32_t)row[j] : kNoId;
+    }
+}
+
+int graph_candidates(const int64_t *d_ids, int64_t m, int64_t row0, int K, uint32_t *d_cand, cudaStream_t s) {
+    if (m == 0) return B200_OK;
+    graph_candidates_kernel<<<(unsigned)ceil_div(m, 256), 256, 0, s>>>(d_ids, m, row0, K, d_cand);
+    g_launches++;
+    B200_CUDA_OK(cudaGetLastError());
+    return B200_OK;
+}
+
+// One block per node A, cand(A) = c[0..K) in shared memory, also sorted by id for membership.  Thread pair (i, p) looks up
+// v = cand(c[i])[p]: when v = c[j] with i < j and p < j, c[i] is a detour to c[j] (c[j] ranks ahead of position j in the list of
+// a closer candidate).  The detour counts are integer sums, so the result does not depend on the order of the additions.
+__global__ void __launch_bounds__(256) graph_prune_kernel(const uint32_t *__restrict__ cand, int64_t n, int K, int D, uint32_t *__restrict__ pruned) {
+    __shared__ uint32_t c[2 * kGraphMaxDegree], sid[2 * kGraphMaxDegree];
+    __shared__ int spos[2 * kGraphMaxDegree], det[2 * kGraphMaxDegree];
+    const int64_t a = blockIdx.x;
+    const int tid = threadIdx.x;
+    if (tid < K) {
+        const uint32_t v = cand[a * K + tid];
+        c[tid] = v < (uint64_t)n ? v : kNoId;
+        det[tid] = 0;
+    }
+    __syncthreads();
+    if (tid < K) {   // rank by (id, position): ids are distinct, the position only orders the padding
+        const uint32_t v = c[tid];
+        int r = 0;
+        for (int j = 0; j < K; j++) r += c[j] < v || (c[j] == v && j < tid);
+        sid[r] = v;
+        spos[r] = tid;
+    }
+    __syncthreads();
+    for (int e = tid; e < K * K; e += blockDim.x) {
+        const int i = e / K, pp = e - i * K;
+        const uint32_t u = c[i];
+        if (u == kNoId) continue;
+        const uint32_t v = cand[(int64_t)u * K + pp];
+        if (v == kNoId) continue;
+        int lo = 0, hi = K;   // first sorted entry >= v
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (sid[mid] < v) lo = mid + 1;
+            else hi = mid;
+        }
+        if (lo < K && sid[lo] == v) {
+            const int j = spos[lo];
+            if (j > i && pp < j) atomicAdd(&det[j], 1);
+        }
+    }
+    __syncthreads();
+    __shared__ int nvalid;
+    if (tid == 0) {
+        int nv = 0;
+        for (int j = 0; j < K; j++) nv += c[j] != kNoId;
+        nvalid = nv;
+    }
+    if (tid < K && c[tid] != kNoId) {
+        const int key = det[tid] * K + tid;
+        int r = 0;
+        for (int j = 0; j < K; j++) r += c[j] != kNoId && det[j] * K + j < key;
+        if (r < D) pruned[a * D + r] = c[tid];
+    }
+    __syncthreads();
+    for (int r = nvalid + tid; r < D; r += blockDim.x) pruned[a * D + r] = kNoId;
+}
+
+int graph_prune(const uint32_t *d_cand, int64_t n, int D, uint32_t *d_pruned, cudaStream_t s) {
+    if (n == 0) return B200_OK;
+    graph_prune_kernel<<<(unsigned)n, 256, 0, s>>>(d_cand, n, 2 * D, D, d_pruned);
+    g_launches++;
+    B200_CUDA_OK(cudaGetLastError());
+    return B200_OK;
+}
+
+// triple (B, r, A) of edge A -> B at rank r as key B * D + r, value A, in A-major order; empty slots get the key n * D
+__global__ void graph_triples_kernel(const uint32_t *__restrict__ pruned, int64_t n, int D, uint64_t *__restrict__ keys, uint32_t *__restrict__ vals) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n * D) return;
+    const uint32_t b = pruned[e];
+    const int64_t a = e / D, r = e - a * D;
+    keys[e] = b != kNoId ? (uint64_t)b * D + r : (uint64_t)n * D;
+    vals[e] = (uint32_t)a;
+}
+
+__device__ __forceinline__ bool graph_row_has(const uint32_t *row, int cnt, uint32_t v) {
+    for (int t = 0; t < cnt; t++)
+        if (row[t] == v) return true;
+    return false;
+}
+
+// graph(B): the first D / 2 pruned forward edges, then at most D / 2 reverse sources in (rank, source) order, then the rest of
+// the forward edges; duplicates skipped, at most D entries, empty slots 0xFFFFFFFF
+__global__ void graph_merge_kernel(const uint32_t *__restrict__ pruned, const uint64_t *__restrict__ keys, const uint32_t *__restrict__ vals,
+                                   int64_t n, int D, uint32_t *__restrict__ graph) {
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= n) return;
+    const uint32_t *fwd = pruned + b * D;
+    uint32_t *row = graph + b * D;
+    int cnt = 0;
+    for (int r = 0; r < D / 2; r++) {
+        const uint32_t v = fwd[r];
+        if (v != kNoId && !graph_row_has(row, cnt, v)) row[cnt++] = v;
+    }
+    const int64_t total = n * D;
+    int64_t lo = 0, hi = total;   // first key >= b * D
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (keys[mid] < (uint64_t)b * D) lo = mid + 1;
+        else hi = mid;
+    }
+    for (int added = 0; lo < total && keys[lo] < (uint64_t)(b + 1) * D && added < D / 2 && cnt < D; lo++) {
+        const uint32_t v = vals[lo];
+        if (!graph_row_has(row, cnt, v)) {
+            row[cnt++] = v;
+            added++;
+        }
+    }
+    for (int r = D / 2; r < D && cnt < D; r++) {
+        const uint32_t v = fwd[r];
+        if (v != kNoId && !graph_row_has(row, cnt, v)) row[cnt++] = v;
+    }
+    for (; cnt < D; cnt++) row[cnt] = kNoId;
+}
+
+int graph_merge(const uint32_t *d_pruned, int64_t n, int D, uint32_t *d_graph, cudaStream_t s) {
+    if (n == 0) return B200_OK;
+    const int64_t e = n * D;
+    if (e >= (int64_t)1 << 31) return fail(B200_ERR_UNSUPPORTED, "graph build: n x graph_degree must stay below 2^31");
+    uint64_t *keys = nullptr, *keys_out = nullptr;
+    uint32_t *vals = nullptr, *vals_out = nullptr;
+    void *tmp = nullptr;
+    size_t tb = 0;
+    int end_bit = 1;
+    while (end_bit < 64 && ((uint64_t)e >> end_bit) != 0) end_bit++;
+    cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, keys_out, vals, vals_out, (int)e, 0, end_bit, s);
+    int rc = B200_OK;
+    if (cudaMalloc(&keys, (size_t)e * 8) != cudaSuccess || cudaMalloc(&keys_out, (size_t)e * 8) != cudaSuccess ||
+        cudaMalloc(&vals, (size_t)e * 4) != cudaSuccess || cudaMalloc(&vals_out, (size_t)e * 4) != cudaSuccess ||
+        cudaMalloc(&tmp, tb + 256) != cudaSuccess) {
+        cudaGetLastError();
+        rc = fail(B200_ERR_NOMEM, "graph build: cudaMalloc of the reverse-edge scratch failed (" + std::to_string(e * 24) + " bytes)");
+    }
+    if (rc == B200_OK) {
+        graph_triples_kernel<<<(unsigned)ceil_div(e, 256), 256, 0, s>>>(d_pruned, n, D, keys, vals);
+        // stable: equal (B, r) keys keep the A-ascending order of the triples
+        cub::DeviceRadixSort::SortPairs(tmp, tb, keys, keys_out, vals, vals_out, (int)e, 0, end_bit, s);
+        graph_merge_kernel<<<(unsigned)ceil_div(n, 128), 128, 0, s>>>(d_pruned, keys_out, vals_out, n, D, d_graph);
+        g_launches += 3;
+        const cudaError_t err = cudaStreamSynchronize(s);
+        if (err != cudaSuccess) rc = fail(B200_ERR_CUDA, std::string("graph merge: ") + cudaGetErrorString(err));
+    }
+    for (void *p : {(void *)keys, (void *)keys_out, (void *)vals, (void *)vals_out, tmp})
+        if (p) cudaFree(p);
+    return rc;
+}
+
+// ------------------------------------------------------------------------------------
+// search: one CTA per query
+// ------------------------------------------------------------------------------------
+namespace {
+constexpr int kBatch = kGraphMaxDegree * kGraphWidth;   // ids one step filters and scores (>= kGraphMaxSeeds)
+static_assert(kBatch >= kGraphMaxSeeds, "a step takes the seeds");
+
+struct GraphSmem {
+    int64_t qs, vis, ek0, ei0, ek1, ei1, ck, ci, sk, si, nb, ak0, ai0, ak1, ai1, sh, ef0, ef1, total;
+};
+
+__host__ __device__ inline GraphSmem graph_smem_layout(int d_pad, int ef, int k, bool filtered) {
+    GraphSmem L{};
+    const int ka = filtered ? k : 0;
+    int64_t o = 0;
+    L.qs = o; o += (int64_t)d_pad * 4;
+    L.vis = o; o += (int64_t)kGraphVisitedSlots * 4;
+    L.ek0 = o; o += (int64_t)ef * 4;
+    L.ei0 = o; o += (int64_t)ef * 4;
+    L.ek1 = o; o += (int64_t)ef * 4;
+    L.ei1 = o; o += (int64_t)ef * 4;
+    L.ck = o; o += kBatch * 4;
+    L.ci = o; o += kBatch * 4;
+    L.sk = o; o += kBatch * 4;
+    L.si = o; o += kBatch * 4;
+    L.nb = o; o += kBatch * 4;
+    L.ak0 = o; o += (int64_t)ka * 4;
+    L.ai0 = o; o += (int64_t)ka * 4;
+    L.ak1 = o; o += (int64_t)ka * 4;
+    L.ai1 = o; o += (int64_t)ka * 4;
+    L.sh = o; o += 32 * 4;
+    L.ef0 = o; o += ef;
+    L.ef1 = o; o += ef;
+    L.total = (o + 15) / 16 * 16;
+    return L;
+}
+
+__device__ __forceinline__ uint32_t vis_slot(uint32_t id) { return (id * 0x9E3779B1u) >> (32 - kGraphVisitedLog2); }
+
+__device__ __forceinline__ bool vis_contains(const uint32_t *vis, uint32_t id) {
+    for (uint32_t s = vis_slot(id);; s = (s + 1) & (kGraphVisitedSlots - 1)) {
+        const uint32_t v = vis[s];
+        if (v == id) return true;
+        if (v == kNoId) return false;
+    }
+}
+
+// distinct ids only; the slot an id lands in depends on the order of the inserts, membership does not
+__device__ __forceinline__ void vis_insert(uint32_t *vis, uint32_t id) {
+    for (uint32_t s = vis_slot(id);; s = (s + 1) & (kGraphVisitedSlots - 1)) {
+        const uint32_t old = atomicCAS(&vis[s], kNoId, id);
+        if (old == kNoId || old == id) return;
+    }
+}
+
+// entries of the sorted a[0..len) better than (key, id)
+__device__ __forceinline__ int count_better(const float *ak, const uint32_t *ai, int len, float key, uint32_t id) {
+    int lo = 0, hi = len;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (better(ak[mid], ai[mid], key, id)) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// out[0..min(cap, cnt + nc)) = the best of the sorted list (cnt entries) and the sorted candidates (nc, disjoint ids); new
+// candidates unexpanded.  Every thread of the CTA calls it.
+__device__ __forceinline__ void merge_lists(const float *lk, const uint32_t *li, const uint8_t *lf, int cnt, const float *ck, const uint32_t *ci,
+                                            int nc, int cap, float *ok, uint32_t *oi, uint8_t *of) {
+    for (int p = threadIdx.x; p < cnt; p += blockDim.x) {
+        const int np = p + count_better(ck, ci, nc, lk[p], li[p]);
+        if (np < cap) {
+            ok[np] = lk[p];
+            oi[np] = li[p];
+            if (of) of[np] = lf[p];
+        }
+    }
+    for (int r = threadIdx.x; r < nc; r += blockDim.x) {
+        const int np = r + count_better(lk, li, cnt, ck[r], ci[r]);
+        if (np < cap) {
+            ok[np] = ck[r];
+            oi[np] = ci[r];
+            if (of) of[np] = 0;
+        }
+    }
+}
+}  // namespace
+
+// Shared memory: the query, the visited table, two ef-entry lists (keys, ids, expanded flags) used in turn, the step's
+// candidates (adjacency order, then sorted), the neighbour row, two k-entry lists of alive rows (filtered searches only).
+// A step: warp 0 drops empty slots, repeats within the row and visited ids, compacts the rest in row order and inserts them
+// into the visited table; a warp per row scores them (128-bit loads, fp32, fixed lane order); they are sorted by (key, id) and
+// rank-merged into the ef list (and, those the bitmap keeps, into the alive list).  Every answer-bearing step is a sort or a
+// merge by (key, id): the result does not depend on thread timing.
+__global__ void __launch_bounds__(kGraphThreads) graph_search_kernel(const GraphSearchParams p) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const bool filtered = p.alive != nullptr;
+    const GraphSmem L = graph_smem_layout(p.d_pad, p.ef, p.k, filtered);
+    float *qs = reinterpret_cast<float *>(smem_raw + L.qs);
+    uint32_t *vis = reinterpret_cast<uint32_t *>(smem_raw + L.vis);
+    // the two lists of each kind are at a fixed byte distance: list `b` of a kind is its list 0 plus b x that distance
+    float *ek0 = reinterpret_cast<float *>(smem_raw + L.ek0);
+    uint32_t *ei0 = reinterpret_cast<uint32_t *>(smem_raw + L.ei0);
+    uint8_t *ef0 = smem_raw + L.ef0;
+    const int64_t dek = L.ek1 - L.ek0, dei = L.ei1 - L.ei0, def = L.ef1 - L.ef0, dak = L.ak1 - L.ak0, dai = L.ai1 - L.ai0;
+    float *ck = reinterpret_cast<float *>(smem_raw + L.ck), *sk = reinterpret_cast<float *>(smem_raw + L.sk);
+    uint32_t *ci = reinterpret_cast<uint32_t *>(smem_raw + L.ci), *si = reinterpret_cast<uint32_t *>(smem_raw + L.si);
+    uint32_t *nb = reinterpret_cast<uint32_t *>(smem_raw + L.nb);
+    float *ak0 = reinterpret_cast<float *>(smem_raw + L.ak0);
+    uint32_t *ai0 = reinterpret_cast<uint32_t *>(smem_raw + L.ai0);
+    auto ek = [&](int b) { return reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(ek0) + b * dek); };
+    auto ei = [&](int b) { return reinterpret_cast<uint32_t *>(reinterpret_cast<unsigned char *>(ei0) + b * dei); };
+    auto ef = [&](int b) { return ef0 + b * def; };
+    auto ak = [&](int b) { return reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(ak0) + b * dak); };
+    auto ai = [&](int b) { return reinterpret_cast<uint32_t *>(reinterpret_cast<unsigned char *>(ai0) + b * dai); };
+    int *sh = reinterpret_cast<int *>(smem_raw + L.sh);
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int64_t q = blockIdx.x;
+    const int nwarps = kGraphThreads / 32;
+    for (int i = tid; i < p.d_pad; i += kGraphThreads) qs[i] = p.queries[q * p.d_pad + i];
+    for (int i = tid; i < kGraphVisitedSlots; i += kGraphThreads) vis[i] = kNoId;
+    for (int j = tid; j < p.nseeds; j += kGraphThreads) {
+        const int64_t v = p.seeds[q * p.nseeds + j];
+        nb[j] = v >= 0 && v < p.n ? (uint32_t)v : kNoId;
+    }
+    __syncthreads();
+    int cur = 0, cnt = 0, acur = 0, acnt = 0;
+    unsigned long long scored = 0;
+
+    // one step over nb[0..m)
+    auto step = [&](int m) {
+        if (warp == 0) {
+            int nc = 0;
+            for (int b = 0; b < m; b += 32) {
+                const int j = b + lane;
+                const uint32_t v = j < m ? nb[j] : kNoId;
+                bool fresh = v < (uint64_t)p.n;
+                for (int t = 0; fresh && t < j; t++) fresh = nb[t] != v;
+                if (fresh) fresh = !vis_contains(vis, v);
+                const unsigned bal = __ballot_sync(0xffffffffu, fresh);
+                if (fresh) ci[nc + __popc(bal & ((1u << lane) - 1))] = v;
+                nc += __popc(bal);
+            }
+            __syncwarp();
+            for (int c = lane; c < nc; c += 32) vis_insert(vis, ci[c]);
+            if (lane == 0) sh[0] = nc;
+        }
+        __syncthreads();
+        const int nc = sh[0];
+        for (int c = warp; c < nc; c += nwarps) {
+            const float4 *row = reinterpret_cast<const float4 *>(p.rows + (size_t)ci[c] * p.d_pad);
+            const float4 *x4 = reinterpret_cast<const float4 *>(qs);
+            float acc = 0.f;
+            for (int cc = lane; cc < p.d_pad / 4; cc += 32) {
+                const float4 y = __ldg(row + cc);
+                const float4 x = x4[cc];
+                if (p.l2) {
+                    float t = x.x - y.x; acc = fmaf(t, t, acc);
+                    t = x.y - y.y; acc = fmaf(t, t, acc);
+                    t = x.z - y.z; acc = fmaf(t, t, acc);
+                    t = x.w - y.w; acc = fmaf(t, t, acc);
+                } else {
+                    acc = fmaf(x.x, y.x, acc); acc = fmaf(x.y, y.y, acc);
+                    acc = fmaf(x.z, y.z, acc); acc = fmaf(x.w, y.w, acc);
+                }
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+            if (lane == 0) ck[c] = p.l2 ? acc : -acc;
+        }
+        scored += (unsigned long long)nc;
+        __syncthreads();
+        if (tid < nc) {   // sort by (key, id)
+            const float key = ck[tid];
+            const uint32_t id = ci[tid];
+            int r = 0;
+            for (int c = 0; c < nc; c++) r += better(ck[c], ci[c], key, id);
+            sk[r] = key;
+            si[r] = id;
+        }
+        __syncthreads();
+        merge_lists(ek(cur), ei(cur), ef(cur), cnt, sk, si, nc, p.ef, ek(cur ^ 1), ei(cur ^ 1), ef(cur ^ 1));
+        cur ^= 1;
+        cnt = min(p.ef, cnt + nc);
+        if (filtered) {   // the kept ones, still sorted, into ck / ci (free after the sort)
+            if (tid < nc) {
+                const uint32_t id = si[tid];
+                if ((p.alive[id >> 3] >> (id & 7)) & 1) {
+                    int r = 0;
+                    for (int c = 0; c < tid; c++) r += (p.alive[si[c] >> 3] >> (si[c] & 7)) & 1;
+                    ck[r] = sk[tid];
+                    ci[r] = id;
+                }
+            }
+            if (tid == 0) {
+                int na = 0;
+                for (int c = 0; c < nc; c++) na += (p.alive[si[c] >> 3] >> (si[c] & 7)) & 1;
+                sh[1] = na;
+            }
+            __syncthreads();
+            const int na = sh[1];
+            merge_lists(ak(acur), ai(acur), nullptr, acnt, ck, ci, na, p.k, ak(acur ^ 1), ai(acur ^ 1), nullptr);
+            acur ^= 1;
+            acnt = min(p.k, acnt + na);
+        }
+        __syncthreads();
+    };
+
+    step(p.nseeds);
+    for (int it = 0; it < p.max_iters; it++) {
+        // parent: the first unexpanded entry of the list
+        int first = INT_MAX;
+        for (int e = tid; e < cnt; e += kGraphThreads)
+            if (!ef(cur)[e]) {
+                first = e;
+                break;
+            }
+        first = __reduce_min_sync(0xffffffffu, first);
+        if (lane == 0) sh[8 + warp] = first;
+        __syncthreads();
+        if (tid == 0) {
+            int f = INT_MAX;
+            for (int w = 0; w < nwarps; w++) f = min(f, sh[8 + w]);
+            sh[2] = f;
+            if (f != INT_MAX) {
+                ef(cur)[f] = 1;
+                sh[3] = (int)ei(cur)[f];
+            }
+        }
+        __syncthreads();
+        if (sh[2] == INT_MAX) break;
+        const uint32_t parent = (uint32_t)sh[3];
+        for (int j = tid; j < p.degree; j += kGraphThreads) nb[j] = p.graph[(size_t)parent * p.degree + j];
+        __syncthreads();
+        step(p.degree);
+    }
+
+    const float *fk = filtered ? ak(acur) : ek(cur);
+    const uint32_t *fi = filtered ? ai(acur) : ei(cur);
+    const int have_n = filtered ? acnt : min(cnt, p.k);
+    for (int j = tid; j < p.k; j += kGraphThreads) {
+        const bool have = j < have_n;
+        p.out_ids[q * p.k + j] = have ? (int64_t)fi[j] + p.id_offset : -1;
+        p.out_dis[q * p.k + j] = have ? (p.l2 ? fk[j] : -fk[j]) : (p.l2 ? FLT_MAX : -FLT_MAX);
+    }
+    if (tid == 0) atomicAdd(p.rows_scored, scored);
+}
+
+size_t graph_search_smem(int d_pad, int ef, int k, bool filtered) { return (size_t)graph_smem_layout(d_pad, ef, k, filtered).total; }
+
+int graph_search(const GraphSearchParams &p, int64_t nq, cudaStream_t s) {
+    if (nq == 0) return B200_OK;
+    const size_t smem = graph_search_smem(p.d_pad, p.ef, p.k, p.alive != nullptr);
+    B200_CUDA_OK(cudaFuncSetAttribute(graph_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    graph_search_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
+    g_launches++;
+    B200_CUDA_OK(cudaGetLastError());
+    return B200_OK;
+}
+
+}  // namespace b200

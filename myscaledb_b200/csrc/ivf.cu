@@ -22,6 +22,7 @@
 // quantiser is trained by k-majority (Hamming assignment, per-bit majority; integer work, so deterministic), a page holds the
 // row bytes k-block-major, and the list rows are exact, so there is no second stage.
 #include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -32,6 +33,7 @@
 #include <cub/cub.cuh>
 
 #include "common.cuh"
+#include "graph.h"
 #include "ivf_aq.h"
 #include "ivf_gemm.h"
 #include "kernels.h"
@@ -1288,6 +1290,14 @@ struct b200_index {
     bool last_probe_exact = false;
     // statistics of the last search (tests, bench roofline): rows x payload bytes the scan kernel was asked to stream
     int64_t last_scan_rows = 0, last_items = 0;
+    // graph_degree=D (HNSWFLAT): neighbour graph [n][D] u32 built at finalize, 0xFFFFFFFF = empty slot (graph_sm90.cu)
+    int graph_degree = 0;
+    uint32_t *d_graph = nullptr;
+    // seed ids [last_seed_nq][last_seed_s] of the last graph search (b200_index_last_seeds), and their first-stage distances
+    DevArr w_seeds, w_seedd;
+    int64_t last_seed_nq = 0;
+    int last_seed_s = 0;
+    bool last_graph = false;        // the last search walked the graph: last_scan reports rows scored x d_pad x 4 bytes
     bool timing = false, timed_pending = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaEvent_t ev_ph[6] = {};      // phase boundaries of the last search: start | coarse | pairs+plan+gather | scan | merge | refine
@@ -1420,6 +1430,23 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
     const int dflt_refine = (ty == IDX_IVFPQ || ty == IDX_IVFSQ || bin) ? 1 : (ix->payload == IVF_PRODUCER_PQ ? 16 : 4);
     ix->refine_factor = parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", dflt_refine));
     ix->keep_raw = parse_int_param(params, "keep_raw", -1);
+    // graph_degree=D: HNSWFLAT only, over its fp32 rows in HBM (the reference's m is PQ M here and keeps that meaning)
+    ix->graph_degree = parse_int_param(params, "graph_degree", 0);
+    if (ix->graph_degree > 0) {
+        if (ty != IDX_HNSWFLAT) {
+            delete ix;
+            return fail(B200_ERR_UNSUPPORTED, "graph_degree: a neighbour graph is built on HNSWFLAT only (the other types keep quantised or binary rows)");
+        }
+        if (!graph_degree_ok(ix->graph_degree)) {
+            const int gd = ix->graph_degree;
+            delete ix;
+            return fail(B200_ERR_INVALID, "graph_degree must be 16, 32 or 64 (or 0: no graph), got " + std::to_string(gd));
+        }
+        if (ix->keep_raw == 0 || ix->keep_raw == 2) {
+            delete ix;
+            return fail(B200_ERR_UNSUPPORTED, "graph_degree: the graph search reads the fp32 rows in HBM (keep_raw=1)");
+        }
+    }
     cudaGetDevice(&ix->device);
     cudaDeviceGetAttribute(&ix->sms, cudaDevAttrMultiProcessorCount, ix->device);
     if (cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking) != cudaSuccess) {
@@ -1439,12 +1466,13 @@ extern "C" int b200_index_free(b200_index *ix) {
     if (ix->coarse) b200_corpus_free(ix->coarse);
     for (void *p : {(void *)ix->d_centroids, (void *)ix->d_bcent, (void *)ix->d_cnorm, (void *)ix->d_pq, (void *)ix->d_pq_bf16, (void *)ix->d_sq, ix->d_pool, (void *)ix->d_row_bias,
                     (void *)ix->d_row_ids, (void *)ix->d_list_len, (void *)ix->d_tail_page, (void *)ix->d_page_owner, (void *)ix->d_page_seq,
-                    (void *)ix->d_pages_used, (void *)ix->d_flag, (void *)ix->d_list_page_off, (void *)ix->d_list_pages, (void *)ix->d_list_order})
+                    (void *)ix->d_pages_used, (void *)ix->d_flag, (void *)ix->d_list_page_off, (void *)ix->d_list_pages, (void *)ix->d_list_order, (void *)ix->d_graph})
         if (p) cudaFree(p);
     for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_cnt, &ix->w_plan,
                       &ix->w_sort, &ix->w_q, &ix->w_qraw, &ix->w_probe, &ix->w_pd, &ix->w_items, &ix->w_qbuf, &ix->w_inv, &ix->w_ppb, &ix->w_pconst, &ix->w_qb, &ix->w_cs,
                       &ix->w_qconst, &ix->w_pk, &ix->w_pi, &ix->w_pw, &ix->w_lk, &ix->w_li, &ix->w_alive, &ix->w_od, &ix->w_oi, &ix->w_cand,
-                      &ix->w_host_q, &ix->w_ppopc, &ix->w_lut, &ix->w_stage, &ix->w_flist, &ix->w_fpages, &ix->w_fsel})
+                      &ix->w_host_q, &ix->w_ppopc, &ix->w_lut, &ix->w_stage, &ix->w_flist, &ix->w_fpages, &ix->w_fsel,
+                      &ix->w_seeds, &ix->w_seedd})
         a->release();
     if (ix->h_fsel) cudaFreeHost(ix->h_fsel);
     if (ix->ev0) cudaEventDestroy(ix->ev0);
@@ -2102,6 +2130,80 @@ extern "C" int b200_index_add(b200_index *ix, const float *rows, int64_t n) {
     return B200_OK;
 }
 
+static int search_device_locked(b200_index *ix, const float *d_queries, int64_t nq, int k, const char *params, int first_stage_only,
+                                const uint8_t *d_alive, const uint8_t *h_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids,
+                                int64_t *out_num_candidates, cudaStream_t s);
+
+// scratch of one chunk of the graph build's list searches (their pairs, partial lists and candidates); sizes the chunk
+constexpr int64_t kGraphBuildSearchBytes = (int64_t)512 << 20;
+
+namespace {
+struct DevScratch {   // freed on every return path of the graph build
+    void *p = nullptr;
+    ~DevScratch() {
+        if (p) cudaFree(p);
+    }
+    int alloc(size_t bytes) {
+        if (cudaMalloc(&p, std::max<size_t>(bytes, 16)) != cudaSuccess) {
+            cudaGetLastError();
+            p = nullptr;
+            return fail(B200_ERR_NOMEM, "graph build: cudaMalloc(" + std::to_string(bytes) + ") failed");
+        }
+        return B200_OK;
+    }
+};
+}  // namespace
+
+// graph_degree=D: every row searches the index's own lists with its defaults (nprobe, exact re-rank with refine_factor) for
+// k = 2D + 1, exactly ix.search(rows, 2D + 1, "graph=0"); its own id dropped, the 2D candidates are pruned by rank (CAGRA) and
+// merged with the reverse edges (graph_sm90.cu).  phase_ms then holds candidates | prune | merge in milliseconds.
+static int build_graph_locked(b200_index *ix) {
+    using clk = std::chrono::steady_clock;
+    const auto ms_since = [](clk::time_point t) { return std::chrono::duration<double, std::milli>(clk::now() - t).count(); };
+    cudaStream_t s = ix->stream;
+    const int D = ix->graph_degree, K = 2 * D, d = ix->d;
+    const int64_t n = ix->n;
+    const int np = std::max(1, std::min(ix->default_nprobe, ix->nlist));
+    const int k1 = std::min(1024, (K + 1) * std::max(1, ix->refine_factor));
+    const int64_t chunk = std::max<int64_t>(256, std::min<int64_t>(n, kGraphBuildSearchBytes / ((int64_t)np * k1 * 8)));
+    DevScratch cand, pruned, q, dis, ids;
+    B200_TRY(cand.alloc((size_t)n * K * 4));
+    B200_TRY(q.alloc((size_t)chunk * d * 4));
+    B200_TRY(dis.alloc((size_t)chunk * (K + 1) * 4));
+    B200_TRY(ids.alloc((size_t)chunk * (K + 1) * 8));
+    auto t = clk::now();
+    const float *rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
+    for (int64_t off = 0; off < n; off += chunk) {
+        const int64_t m = std::min(chunk, n - off);
+        B200_CUDA_OK(cudaMemcpy2DAsync(q.p, (size_t)d * 4, rows + off * ix->d_pad, (size_t)ix->d_pad * 4, (size_t)d * 4, m, cudaMemcpyDeviceToDevice, s));
+        B200_TRY(search_device_locked(ix, static_cast<float *>(q.p), m, K + 1, nullptr, 0, nullptr, nullptr, 0, static_cast<float *>(dis.p),
+                                      static_cast<int64_t *>(ids.p), nullptr, s));
+        B200_TRY(graph_candidates(static_cast<int64_t *>(ids.p), m, off, K, static_cast<uint32_t *>(cand.p) + off * K, s));
+    }
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    for (DevScratch *b : {&q, &dis, &ids}) {
+        cudaFree(b->p);
+        b->p = nullptr;
+    }
+    const double t_cand = ms_since(t);
+    t = clk::now();
+    B200_TRY(pruned.alloc((size_t)n * D * 4));
+    B200_TRY(graph_prune(static_cast<uint32_t *>(cand.p), n, D, static_cast<uint32_t *>(pruned.p), s));
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    cudaFree(cand.p);
+    cand.p = nullptr;
+    const double t_prune = ms_since(t);
+    t = clk::now();
+    DevScratch graph;
+    B200_TRY(graph.alloc((size_t)n * D * 4));
+    B200_TRY(graph_merge(static_cast<uint32_t *>(pruned.p), n, D, static_cast<uint32_t *>(graph.p), s));
+    ix->d_graph = static_cast<uint32_t *>(graph.p);
+    graph.p = nullptr;
+    const double ph[5] = {t_cand, t_prune, ms_since(t), 0, 0};
+    std::copy(ph, ph + 5, ix->phase_ms);
+    return B200_OK;
+}
+
 static int finalize_locked(b200_index *ix) {
     if (ix->built) return B200_OK;
     if (!ix->trained) return fail(B200_ERR_INVALID, "index not trained");
@@ -2152,6 +2254,8 @@ static int finalize_locked(b200_index *ix) {
         const int raw_metric = ix->metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
         if (!ix->use_ivf) B200_TRY(b200_corpus_create(ix->binary ? ix->metric : raw_metric, ix->binary ? B200_DTYPE_BIN : B200_DTYPE_F32, ix->d, 0, &ix->raw));
     }
+    // a part below the inverted-file threshold is FLAT and gets no graph
+    if (ix->graph_degree > 0 && ix->use_ivf && ix->n > 0 && !ix->d_graph) B200_TRY(build_graph_locked(ix));
     ix->built = true;
     return B200_OK;
 }
@@ -2202,6 +2306,7 @@ extern "C" int b200_index_memory_bytes(const b200_index *ix, uint64_t *out_bytes
              (uint64_t)ix->pool_pages * 12;
         if (ix->d_pq) b += (uint64_t)ix->m * pq_codewords(ix->pq_bits) * ix->dsub * (ix->d_pq_bf16 ? 6 : 4);   // fp32 codebook (+ the decoder's bf16 copy)
     }
+    if (ix->d_graph) b += (uint64_t)ix->n * ix->graph_degree * 4;
     *out_bytes = b;
     return B200_OK;
 }
@@ -2221,6 +2326,7 @@ extern "C" int b200_index_set_raw_placement(b200_index *ix, int placement) {
     if (ix->binary || !ix->use_ivf)
         return fail(B200_ERR_UNSUPPORTED, "the rows are the index here (FLAT, a part below the inverted-file threshold or a binary index): they stay in HBM");
     if (ix->keep_raw != 1 && ix->keep_raw != 2) return fail(B200_ERR_INVALID, "this index keeps no fp32 rows (keep_raw=0)");
+    if (placement == 2 && ix->d_graph) return fail(B200_ERR_UNSUPPORTED, "graph_degree: the graph search reads the fp32 rows in HBM");
     if (placement == ix->keep_raw) return B200_OK;
     B200_CUDA_OK(cudaSetDevice(ix->device));
     // searches enqueued on the callers' streams may still read the rows that are about to be freed
@@ -2281,7 +2387,7 @@ extern "C" int b200_index_last_scan(b200_index *ix, int64_t *rows_streamed, int6
         if (cudaMemcpy(&r, ix->d_flag + 4, 8, cudaMemcpyDeviceToHost) == cudaSuccess) ix->last_scan_rows = (int64_t)r;
     }
     if (rows_streamed) *rows_streamed = ix->last_scan_rows;
-    if (payload_row_bytes_out) *payload_row_bytes_out = (int64_t)payload_row_bytes(ix);
+    if (payload_row_bytes_out) *payload_row_bytes_out = ix->last_graph ? (int64_t)ix->d_pad * 4 : (int64_t)payload_row_bytes(ix);
     if (work_items) *work_items = ix->last_items;
     if (kernel_ms_total) *kernel_ms_total = ix->timed_ms;
     if (kernel_launches) *kernel_launches = ix->timed_launches;
@@ -2746,6 +2852,62 @@ static int filter_probe_search(b200_index *ix, const float *d_q, int64_t nq, int
     return B200_OK;
 }
 
+// Graph search under a filter on the host entry: a filter that keeps fewer than kGraphExactFactor x k of the rows one query
+// scores at the iteration cap (kept share x rows scored < 2k) would leave the alive list short, so the gathered exact pass over
+// the kept rows answers instead.  Not measured: 2 only asks for room to fill k from the kept rows met on the walk.
+constexpr double kGraphExactFactor = 2.0;
+
+// rows one graph query scores at most: its seeds, then D per expanded parent up to the iteration cap
+static int64_t graph_rows_at_cap(const b200_index *ix, int nseeds) {
+    return nseeds + (int64_t)graph_iteration_cap(ix->graph_degree) * kGraphWidth * ix->graph_degree;
+}
+
+static int graph_ef(const char *params, int k) {
+    return std::max(k, parse_int_param(params, "ef_s", 64));
+}
+
+// The graph search, asynchronous on s (d_q: the prepared queries [nq][d_pad]): seeds from the list path's first stage at
+// nprobe 1 (the best min(ef_s, 32) ids per query), then graph_search_kernel, one CTA per query, over the fp32 rows in HBM.
+static int graph_search_locked(b200_index *ix, const float *d_queries, const float *d_q, int64_t nq, int k, const char *params, const uint8_t *d_alive,
+                               int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
+    const int ef = graph_ef(params, k);
+    const int S = std::min(ef, kGraphMaxSeeds);
+    B200_TRY(ix->w_seeds.reserve((size_t)nq * S * 8));
+    B200_TRY(ix->w_seedd.reserve((size_t)nq * S * 4));
+    B200_TRY(search_device_locked(ix, d_queries, nq, S, "graph=0 nprobe=1", 1, nullptr, nullptr, 0, ix->w_seedd.as<float>(), ix->w_seeds.as<int64_t>(),
+                                  nullptr, s));
+    ix->last_seed_nq = nq;
+    ix->last_seed_s = S;
+    unsigned long long *scored = reinterpret_cast<unsigned long long *>(ix->d_flag + 4);
+    B200_CUDA_OK(cudaMemsetAsync(scored, 0, 8, s));
+    GraphSearchParams gp{};
+    gp.queries = d_q;
+    gp.rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
+    gp.graph = ix->d_graph;
+    gp.seeds = ix->w_seeds.as<int64_t>();
+    gp.alive = d_alive;
+    gp.out_dis = d_out_dis;
+    gp.out_ids = d_out_ids;
+    gp.rows_scored = scored;
+    gp.n = ix->n;
+    gp.id_offset = id_offset;
+    gp.d_pad = ix->d_pad;
+    gp.degree = ix->graph_degree;
+    gp.nseeds = S;
+    gp.ef = ef;
+    gp.k = k;
+    gp.max_iters = graph_iteration_cap(ix->graph_degree);
+    gp.l2 = ix->metric == B200_METRIC_L2;
+    B200_TRY(graph_search(gp, nq, s));
+    if (ix->metric == B200_METRIC_COSINE) {
+        cosine_finish_kernel<<<(unsigned)ceil_div(nq * k, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, k, d_out_dis, d_out_ids);
+        g_launches++;
+    }
+    ix->last_items = nq;
+    ix->last_graph = true;
+    return B200_OK;
+}
+
 // The whole search on the device, asynchronous on s.  d_queries: fp32 [nq][d]; outputs [nq][k].  h_alive: the host copy of
 // d_alive when the caller has one (the exact paths may then score only the rows it keeps), else null.
 static int search_device_locked(b200_index *ix, const float *d_queries, int64_t nq, int k, const char *params, int first_stage_only,
@@ -2785,7 +2947,20 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     }
     const float *d_q = ix->w_q.as<float>();
     bool exact = !ix->use_ivf || force_exact == 1;
-    if (!exact && filter_probe && d_alive && h_alive && ix->raw && !first_stage_only) {
+    // graph_degree indexes walk their graph unless asked for the lists (graph=0) or the exact pass (exact_batch=1)
+    const bool graph = ix->d_graph && !exact && parse_int_param(params, "graph", 1) != 0;
+    if (graph) {
+        if (k > kGraphMaxEf) return fail(B200_ERR_UNSUPPORTED, "k > 1024 on the graph search");
+        const int ef_s = parse_int_param(params, "ef_s", 64);
+        if (ef_s > kGraphMaxEf) return fail(B200_ERR_INVALID, "ef_s must be at most 1024, got " + std::to_string(ef_s));
+        if (d_alive && h_alive) {
+            const int64_t rows_cap = graph_rows_at_cap(ix, std::min(graph_ef(params, k), kGraphMaxSeeds));
+            const int64_t limit = std::min<int64_t>((int64_t)std::ceil(kGraphExactFactor * k * (double)ix->n / (double)rows_cap) - 1,
+                                                    corpus_prefilter_limit(ix->raw, prefilter, nq, k));
+            exact = limit >= 0 && host_count_alive(h_alive, ix->n, limit) <= limit;
+            ix->last_probe_exact = exact;
+        }
+    } else if (!exact && filter_probe && d_alive && h_alive && ix->raw && !first_stage_only) {
         // filter_probe exact rule: a filter that keeps at most kFilterProbeExactFactor x the rows one query's plain probe scans
         // on average is answered by the exact pass over the kept rows (complete and exact) -- only when that pass takes its
         // gathered path for this batch (prefilter mode, nq, k): past the gathered path's limit it would scan every row
@@ -2812,6 +2987,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         }
         return B200_OK;
     }
+    if (graph) return graph_search_locked(ix, d_queries, d_q, nq, k, params, d_alive, id_offset, d_out_dis, d_out_ids, s);
     if (k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 on IVF indexes");
     const int nl = ix->nlist;
     int nprobe = parse_int_param(params, "nprobe", ix->default_nprobe);
@@ -2922,6 +3098,7 @@ extern "C" int b200_index_search_device(b200_index *ix, const float *d_queries, 
     cudaStream_t s = stream ? reinterpret_cast<cudaStream_t>(stream) : ix->stream;
     ix->last_probe.clear();
     ix->last_probe_exact = false;
+    ix->last_graph = false;
     B200_TRY(search_device_locked(ix, d_queries, nq, k, params, first_stage_only, d_alive_bits, nullptr, id_offset, d_out_dis, d_out_ids, nullptr, s));
     if (!stream) B200_CUDA_OK(cudaStreamSynchronize(s));
     return B200_OK;
@@ -2940,6 +3117,7 @@ extern "C" int b200_index_search(b200_index *ix, const float *queries, int64_t n
     cudaStream_t s = ix->stream;
     ix->last_probe.clear();
     ix->last_probe_exact = false;
+    ix->last_graph = false;
     B200_TRY(ix->w_host_q.reserve((size_t)nq * in_row_bytes(ix)));
     B200_TRY(ix->w_cand.reserve((size_t)nq * k * 12 + 16));
     B200_CUDA_OK(cudaMemcpyAsync(ix->w_host_q.p, queries, (size_t)nq * in_row_bytes(ix), cudaMemcpyHostToDevice, s));
@@ -2979,6 +3157,32 @@ extern "C" int b200_index_last_probe(b200_index *ix, int32_t *out_lists, int64_t
         std::copy(ix->last_probe.begin(), ix->last_probe.end(), out_lists);
     }
     if (out_exact) *out_exact = ix->last_probe_exact ? 1 : 0;
+    return B200_OK;
+}
+
+extern "C" int b200_index_graph(const b200_index *ix, uint32_t *out, int64_t capacity_rows, int *out_degree) {
+    if (!ix) return fail(B200_ERR_INVALID, "null index");
+    const int D = ix->d_graph ? ix->graph_degree : 0;
+    if (out_degree) *out_degree = D;
+    if (out && D) {
+        if (capacity_rows < ix->n) return fail(B200_ERR_INVALID, "buffer smaller than the index's rows");
+        B200_CUDA_OK(cudaSetDevice(ix->device));
+        B200_CUDA_OK(cudaMemcpy(out, ix->d_graph, (size_t)ix->n * D * 4, cudaMemcpyDeviceToHost));
+    }
+    return B200_OK;
+}
+
+extern "C" int b200_index_last_seeds(b200_index *ix, int64_t *out, int64_t capacity, int *out_per_query) {
+    if (!ix) return fail(B200_ERR_INVALID, "null index");
+    std::lock_guard<std::mutex> lk(ix->mu);
+    const int S = ix->last_graph ? ix->last_seed_s : 0;
+    if (out_per_query) *out_per_query = S;
+    if (out && S) {
+        if (capacity < ix->last_seed_nq * S) return fail(B200_ERR_INVALID, "buffer smaller than the last search's nq x seeds");
+        B200_CUDA_OK(cudaSetDevice(ix->device));
+        B200_CUDA_OK(cudaDeviceSynchronize());   // the search may still run on the caller's stream
+        B200_CUDA_OK(cudaMemcpy(out, ix->w_seeds.p, (size_t)ix->last_seed_nq * S * 8, cudaMemcpyDeviceToHost));
+    }
     return B200_OK;
 }
 
@@ -3046,9 +3250,10 @@ static int index_save_io(b200_index *ix, Io *f) {
     IxHeader h{};
     memcpy(h.magic, "B2IX", 4);
     // v3: the v2 layout with reserved0 = the PQ code width (4) and a [m][16][dsub] codebook; every other index stays v2
+    // v4: the v2 layout with reserved0 = the graph degree D, followed by the graph [n][D] u32 (graph_degree indexes)
     const bool pq4 = pq_uses_lut(ix) && ix->pq_bits == 4;
-    h.version = pq4 ? 3 : 2;
-    h.reserved0 = pq4 ? 4 : 0;
+    h.version = pq4 ? 3 : ix->d_graph ? 4 : 2;
+    h.reserved0 = pq4 ? 4 : ix->d_graph ? (uint32_t)ix->graph_degree : 0;
     h.type = ix->type; h.metric = ix->metric; h.d = ix->d; h.nlist = ix->nlist; h.m = ix->m; h.dsub = ix->dsub;
     // has_raw 2: the same rows, to be loaded into host memory (keep_raw=2 placement)
     h.default_nprobe = ix->default_nprobe; h.refine_factor = ix->refine_factor; h.payload = ix->payload; h.has_raw = ix->h_rows ? 2 : ix->raw ? 1 : 0;
@@ -3097,6 +3302,16 @@ static int index_save_io(b200_index *ix, Io *f) {
                 if (ok && ix->d_row_bias) ok = dump(ix->d_row_bias + row0, kPageRows * 4);
             }
         }
+        if (ok && ix->d_graph) {
+            const size_t rb = (size_t)ix->graph_degree * 4;
+            const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / (int64_t)rb);
+            std::vector<char> buf((size_t)chunk * rb);
+            for (int64_t off = 0; ok && off < ix->n; off += chunk) {
+                const int64_t mrows = std::min(chunk, ix->n - off);
+                ok = cudaMemcpy(buf.data(), ix->d_graph + off * ix->graph_degree, (size_t)mrows * rb, cudaMemcpyDeviceToHost) == cudaSuccess &&
+                     wr(f, buf.data(), (size_t)mrows * rb);
+            }
+        }
     } catch (const std::bad_alloc &) {
         ok = false;
     }
@@ -3126,8 +3341,8 @@ extern "C" int b200_index_save_cb(b200_index *ix, int (*write)(void *ctx, const 
 static int index_load_io(Io *f, b200_index **out) {
     *out = nullptr;
     IxHeader h{};
-    if (!rd(f, &h, sizeof(h)) || memcmp(h.magic, "B2IX", 4) != 0 || (h.version != 2 && h.version != 3))
-        return fail(B200_ERR_INVALID, "not a B2IX v2 / v3 index file");
+    if (!rd(f, &h, sizeof(h)) || memcmp(h.magic, "B2IX", 4) != 0 || (h.version != 2 && h.version != 3 && h.version != 4))
+        return fail(B200_ERR_INVALID, "not a B2IX v2 / v3 / v4 index file");
     // a truncated or corrupt file must fail here, not in a kernel: every size below is derived from these fields
     const bool bin = h.type >= IDX_BINFLAT;
     // v3: an inverted-file PQ index with 4-bit codes (reserved0 = 4), nibble-packed code rows and a [m][16][dsub] codebook
@@ -3136,6 +3351,9 @@ static int index_load_io(Io *f, b200_index **out) {
         !(h.reserved0 == 4 && h.payload == IVF_PRODUCER_PQ && h.use_ivf && h.m > 0 && h.dsub > 0 && (int64_t)h.m * h.dsub == h.d &&
           h.code_bytes >= pq_code_bytes(h.m, 4) && h.code_bytes % 16 == 0 && ivf_pq4_fits(h.m)))
         return fail(B200_ERR_INVALID, "corrupt index header (v3: 4-bit PQ with M <= " + std::to_string(ivf_pq4_max_m()) + " expected)");
+    // v4: an HNSWFLAT inverted-file index with its fp32 rows in HBM and a graph of degree reserved0
+    if (h.version == 4 && !(graph_degree_ok((int)h.reserved0) && h.type == IDX_HNSWFLAT && h.use_ivf && h.has_raw == 1))
+        return fail(B200_ERR_INVALID, "corrupt index header (v4: an HNSWFLAT graph of degree 16, 32 or 64 over HBM rows expected)");
     const bool sane = h.type >= 0 && h.type < IDX_NUM_TYPES && h.metric >= 0 && h.metric <= 4 && (h.metric >= B200_METRIC_HAMMING) == bin &&
                       h.d > 0 && h.d <= (1 << 16) && (!bin || h.d % 8 == 0) && h.n >= 0 &&
                       h.n < (int64_t)0xffffffffll && h.payload >= 0 && h.payload <= 3 && (h.payload == IVF_PRODUCER_B1) == bin &&
@@ -3259,6 +3477,21 @@ static int index_load_io(Io *f, b200_index **out) {
             cudaMemset(ix->d_flag, 0, 32);
             if ((bin ? upload_coarse_bin(ix, ix->stream) : upload_coarse(ix, ix->stream)) != B200_OK) return bail(b200_last_error());
             if (cudaStreamSynchronize(ix->stream) != cudaSuccess) return bail("upload failed");
+        }
+        if (h.version == 4) {   // every id < n or 0xFFFFFFFF before a kernel walks the graph
+            const int D = (int)h.reserved0;
+            const size_t rb = (size_t)D * 4;
+            const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / (int64_t)rb);
+            std::vector<uint32_t> buf((size_t)chunk * D);
+            if (cudaMalloc(&ix->d_graph, std::max<size_t>((size_t)h.n * rb, 16)) != cudaSuccess) return bail("cudaMalloc of the graph failed");
+            ix->graph_degree = D;
+            for (int64_t off = 0; off < h.n; off += chunk) {
+                const int64_t mrows = std::min(chunk, h.n - off);
+                if (!rd(f, buf.data(), (size_t)mrows * rb)) return bail("truncated index file (graph)");
+                for (int64_t e = 0; e < mrows * D; e++)
+                    if (buf[e] != kNoId && buf[e] >= (uint64_t)h.n) return bail("corrupt index file (graph id out of range)");
+                if (cudaMemcpy(ix->d_graph + off * D, buf.data(), (size_t)mrows * rb, cudaMemcpyHostToDevice) != cudaSuccess) return bail("H2D failed");
+            }
         }
     } catch (const std::bad_alloc &) {
         return bail("out of host memory while loading the index");

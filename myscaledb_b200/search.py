@@ -469,6 +469,27 @@ class VectorIndex:
         _check(lib().b200_index_last_probe(self._h, _p(out, C.c_int32), C.c_int64(n), C.byref(ex)))
         return out, bool(ex.value)
 
+    def graph(self):
+        """graph_degree indexes: the neighbour graph, uint32 [n][D] (0xFFFFFFFF = empty slot); None without a graph."""
+        deg = C.c_int()
+        _check(lib().b200_index_graph(self._h, None, C.c_int64(0), C.byref(deg)))
+        if deg.value == 0:
+            return None
+        n = self.info()["n"]
+        out = np.zeros((n, deg.value), np.uint32)
+        _check(lib().b200_index_graph(self._h, _p(out, C.c_uint32), C.c_int64(n), C.byref(deg)))
+        return out
+
+    def last_seeds(self):
+        """Seed ids of the last search when it walked the graph, int64 [nq][S] (negative = none); None otherwise."""
+        s = C.c_int()
+        _check(lib().b200_index_last_seeds(self._h, None, C.c_int64(0), C.byref(s)))
+        if s.value == 0:
+            return None
+        out = np.zeros((self._last_nq, s.value), np.int64)
+        _check(lib().b200_index_last_seeds(self._h, _p(out, C.c_int64), C.c_int64(out.size), C.byref(s)))
+        return out
+
     def train_loss(self):
         """aq_threshold indexes: (eta, float64 [1 + iterations] mean anisotropic loss of the training sample after the k-means
         codebooks, then after each iteration).  B200Error for an index not trained with the key."""

@@ -2,7 +2,7 @@
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
 workload; results are pasted into DESIGN.md section 7.
-Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows] [filtered] [aq]"""
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows] [filtered] [aq] [graph]"""
 import json
 import os
 import subprocess
@@ -795,9 +795,81 @@ def bench_aq():
         del idx, flat
 
 
+def bench_graph():
+    """HNSWFLAT graph search (graph_degree=32) against the same index's list path.  Shapes: the pq_wide data (clustered
+    768-d rows, 10 000 centres, spread 0.3) and a less clustered one (spread 1.0); rows from GRAPH_ROWS (default 2 M).  Per
+    shape: build time split into candidates / prune / merge and memory_bytes; per ef_s: recall@10 at nq = 1024, QPS at batch
+    1024, the nq = 1 call (median, p10-p90), rows scored per query, and the graph kernel's gathered bytes (rows scored x d x 4)
+    over its CUDA time (torch.profiler) against the 3.35 TB/s data sheet; then the list path (graph=0) over nprobe and the
+    QPS of the cheapest nprobe that reaches recall 0.90 / 0.95 / 0.99."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    n, d, k, D = int(os.environ.get("GRAPH_ROWS", 2_000_000)), 768, 10, 32
+    ctx = gpu_context()
+
+    def calls(fn, reps):
+        fn()
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            out = fn()
+            ts.append(time.perf_counter() - t0)
+        return np.array(ts), out
+
+    def kernel_ms(fn):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        for e in prof.key_averages():
+            if "graph_search_kernel" in e.key:
+                return getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / 1e3 / max(1, e.count)
+        return None
+
+    for spread in (0.3, 1.0):
+        y, qs = clustered(n, d, 10_000, seed=768, spread=spread, nq=1024)
+        flat = b2.Corpus(b2.L2, d).append(y)
+        _, truth = flat.search(qs, k)
+        flat.close()
+        t0 = time.perf_counter()
+        ix = b2.VectorIndex("HNSWFLAT", b2.L2, d, f"graph_degree={D}").build(y)
+        build_s = time.perf_counter() - t0
+        ph = ix.phase_ms()
+        del y
+        print(json.dumps(dict(workload=f"graph {n} x {d} clustered spread {spread}", D=D, **ctx, build_s=round(build_s, 2),
+                              graph_candidates_s=round(ph["coarse"] / 1e3, 2), graph_prune_s=round(ph["plan"] / 1e3, 3),
+                              graph_merge_s=round(ph["scan"] / 1e3, 3), memory_bytes=ix.memory_bytes(), nlist=ix.info()["nlist"])), flush=True)
+        for ef in (32, 64, 128, 256, 512):
+            prm = f"ef_s={ef}"
+            tb, (_, ids) = calls(lambda: ix.search(qs, k, prm), 5)
+            rows = ix.last_scan()["rows_streamed"] / len(qs)
+            t1, _ = calls(lambda: ix.search(qs[:1], k, prm), 50)
+            kms = kernel_ms(lambda: ix.search(qs, k, prm))
+            gb = rows * len(qs) * d * 4
+            print(json.dumps(dict(workload=f"graph spread {spread}", ef_s=ef, recall=round(recall(ids, truth), 4),
+                                  qps_1024=round(len(qs) / np.median(tb), 1), nq1_ms_median=round(1e3 * np.median(t1), 3),
+                                  nq1_ms_p10_p90=[round(1e3 * np.percentile(t1, 10), 3), round(1e3 * np.percentile(t1, 90), 3)],
+                                  rows_scored_per_query=round(rows, 1), kernel_ms=None if kms is None else round(kms, 3),
+                                  gathered_TBps=None if not kms else round(gb / (kms * 1e-3) / 1e12, 3),
+                                  share_of_3_35TBps=None if not kms else round(gb / (kms * 1e-3) / 3.35e12, 3))), flush=True)
+        pts = []
+        for nprobe in (1, 2, 4, 8, 16, 32, 64, 128, 256):
+            prm = f"graph=0,nprobe={nprobe}"
+            tb, (_, ids) = calls(lambda: ix.search(qs, k, prm), 5)
+            pts.append((nprobe, recall(ids, truth), len(qs) / float(np.median(tb))))
+            print(json.dumps(dict(workload=f"lists spread {spread}", nprobe=nprobe, recall=round(pts[-1][1], 4), qps_1024=round(pts[-1][2], 1))),
+                  flush=True)
+        at = {}
+        for target in (0.90, 0.95, 0.99):
+            ok = [p for p in pts if p[1] >= target]
+            at[str(target)] = None if not ok else dict(nprobe=ok[0][0], qps_1024=round(ok[0][2], 1))
+        print(json.dumps(dict(workload=f"lists spread {spread}", qps_at_recall=at)), flush=True)
+        ix.close()
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
         {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
          "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide, "pq4": bench_pq4, "prefilter": bench_prefilter,
-         "host_rows": bench_host_rows, "filtered": bench_filtered, "aq": bench_aq}[w]()
+         "host_rows": bench_host_rows, "filtered": bench_filtered, "aq": bench_aq, "graph": bench_graph}[w]()

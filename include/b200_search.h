@@ -364,7 +364,9 @@ int b200_comm_unique_id(const char *nccl_lib_path /*nullable*/, void *out_id_128
 int b200_comm_create(const char *nccl_lib_path /*nullable*/, const void *unique_id_128_bytes, int rank, int world, b200_comm **out);
 int b200_comm_info(const b200_comm *c, int *rank, int *world);
 int b200_comm_free(b200_comm *c);
-/* building blocks: device buffers a shard search writes its [nq][k] result to, then all-gather + merge on `stream` */
+/* building blocks: device buffers a shard search writes its [nq][k] result to, then all-gather + merge on `stream`.
+ * The two are one packed record: dis [nq * k] fp32, padded to a multiple of 8 bytes, then ids [nq * k] int64, so *d_ids is
+ * 8-byte aligned for every nq * k.  gather_merge refuses k > 2048 before it issues the all-gather. */
 int b200_comm_local_buffers(b200_comm *c, int64_t nq, int k, float **d_dis, int64_t **d_ids);
 int b200_comm_gather_merge(b200_comm *c, int64_t nq, int k, int descending, float *d_out_dis, int64_t *d_out_ids, void *stream);
 /* the same for lists produced on the host (per-shard BM25 top-k: scores descending, unused slots score -inf / id -1);
@@ -375,13 +377,20 @@ int b200_comm_gather_merge_host(b200_comm *c, const float *h_dis, const int64_t 
 int b200_comm_allreduce_sum_u64(b200_comm *c, uint64_t *host_counters, int64_t n);
 /* whole steps.  Every rank passes its own shard and the same queries; every rank receives the global top-k.
  * id_offset = first global row id of this rank's shard.  `stream` must be a real stream.  use_graph != 0 replays the step
- * (query conversion, tensor-core scan, all-gather, merge) as ONE CUDA graph from the second call with the same arguments. */
+ * (query conversion, tensor-core scan, all-gather, merge) as ONE CUDA graph from the second call with the same arguments.
+ * A replay answers as an eager call would: the graph is captured again when the corpus changed since the capture (an
+ * append, set_path, a workspace that grew for another search) or is another corpus at a reused address. */
 int b200_sharded_corpus_search(b200_comm *cm, b200_corpus *corpus, const float *d_queries, int64_t nq, int k,
                                const uint8_t *d_alive_bits /*nullable*/, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids,
                                void *stream, int use_graph);
-/* host queries in, host results out (H2D, scan, all-gather, merge, D2H, synchronise inside) */
+/* graphs the sharded corpus search captured and replays it launched, over the communicator's life */
+int b200_comm_graph_stats(b200_comm *c, int64_t *captures, int64_t *replays);
+/* host queries in, host results out (H2D, scan, all-gather, merge, D2H, synchronise inside).  d must equal the corpus'
+ * dimension (B200_ERR_INVALID otherwise).  Query rows are what the device entry reads: fp32 [nq][d], or for a binary corpus
+ * bytes [nq][d / 8] passed through `queries`. */
 int b200_sharded_corpus_search_host(b200_comm *cm, b200_corpus *corpus, const float *queries, int64_t nq, int d, int k,
                                     int64_t id_offset, float *out_dis, int64_t *out_ids, void *stream, int use_graph);
+/* metric must be the index' own (B200_ERR_INVALID otherwise): it sets the merge direction */
 int b200_sharded_index_search(b200_comm *cm, b200_index *ix, int metric, const float *d_queries, int64_t nq, int k, const char *params,
                               const uint8_t *d_alive_bits /*nullable*/, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids,
                               void *stream);

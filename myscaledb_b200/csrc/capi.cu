@@ -5,6 +5,8 @@
 // There is deliberately no CPU compute path in this file: every entry point either runs
 // CUDA kernels on an sm_90 device or fails with B200_ERR_NO_DEVICE / B200_ERR_CUDA.
 #include <algorithm>
+#include <array>
+#include <atomic>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
@@ -55,11 +57,13 @@ static int num_sms() {
 struct DevBuf {
     void *p = nullptr;
     size_t cap = 0;
+    uint64_t reallocs = 0;   // times p changed: a CUDA graph that baked p in is stale once this moves (corpus_state_epoch)
     int reserve(size_t bytes) {
         if (bytes <= cap) return B200_OK;
         if (p) cudaFree(p);
         p = nullptr;
         cap = 0;
+        reallocs++;
         size_t want = bytes + bytes / 4 + 256;
         cudaError_t e = cudaMalloc(&p, want);
         if (e != cudaSuccess) {
@@ -73,6 +77,7 @@ struct DevBuf {
         if (p) cudaFree(p);
         p = nullptr;
         cap = 0;
+        reallocs++;
     }
     template <typename T>
     T *as() {
@@ -99,10 +104,19 @@ struct b200_corpus {
     int sms = 132;
     cudaStream_t stream = nullptr;
     std::mutex mu;
+    // CUDA graphs of sharded steps (comm.cu) bake in the rows, the row count, the side arrays, the path and the workspace
+    // pointers: `serial` names this corpus for the whole process (an address can be reused after a free), `epoch` moves
+    // whenever one of those changes except the workspaces, whose reallocations corpus_state_epoch adds
+    uint64_t serial = 0;
+    uint64_t epoch = 0;
     // workspaces
     DevBuf w_raw, w_q32, w_qbf, w_qlo, w_qnorm, w_pk, w_pi, w_lk, w_li, w_alive, w_odis, w_oids, w_stage, w_prog;
     // pre-filtered search (prefilter.cu): kept row ids, compaction scratch, compact rows (+ a row of slack), their side arrays
     DevBuf w_pf_ids, w_pf_tmp, w_pf_rows, w_pf_side;
+    std::array<DevBuf *, 18> workspaces() {
+        return {&w_raw, &w_q32, &w_qbf, &w_qlo, &w_qnorm, &w_pk, &w_pi, &w_lk, &w_li, &w_alive, &w_odis, &w_oids, &w_stage, &w_prog,
+                &w_pf_ids, &w_pf_tmp, &w_pf_rows, &w_pf_side};
+    }
     int prefilter = 0;             // b200_corpus_set_prefilter: 0 auto | 1 never | 2 whenever the compact copy fits the budget
     int64_t last_rows_scored = 0;  // rows the last search scored: n after a full scan, the kept rows after a gathered one
     // fused single-launch path of the host entry point (small batches, scan kernel): mapped pinned staging + counters
@@ -159,6 +173,17 @@ namespace b200 {
 // hooks for comm.cu
 int corpus_metric(const b200_corpus *c) { return c->metric; }
 bool corpus_timing_enabled(const b200_corpus *c) { return c->timing; }
+int corpus_dim(const b200_corpus *c) { return c->d; }
+// bytes of one query row as the device entry points read it: fp32 [d], binary corpora [d / 8]
+int64_t corpus_query_row_bytes(const b200_corpus *c) { return c->dtype == B200_DTYPE_BIN ? c->d_pad : (int64_t)c->d * 4; }
+uint64_t corpus_serial(const b200_corpus *c) { return c->serial; }
+// changes whenever something a captured search baked in changes: rows, row count, side arrays, path, workspace pointers
+uint64_t corpus_state_epoch(b200_corpus *c) {
+    std::lock_guard<std::mutex> lk(c->mu);
+    uint64_t e = c->epoch;
+    for (DevBuf *b : c->workspaces()) e += b->reallocs;
+    return e;
+}
 // hooks for the index layer (ivf.cu): device view of the rows / in-place row normalisation
 const void *corpus_device_rows(const b200_corpus *c) { return c->data; }
 // append fp32 rows [n][d] (binary corpora: bytes [n][d / 8]) that already live on the device (index build, centroid tables);
@@ -177,6 +202,7 @@ int corpus_append_device(b200_corpus *c, const float *d_rows, int64_t n, cudaStr
     B200_TRY(corpus_norms(c, c->n, n));
     B200_CUDA_OK(cudaStreamSynchronize(c->stream));
     c->n += n;
+    c->epoch++;
     return B200_OK;
 }
 int corpus_normalize_rows(b200_corpus *c) {
@@ -243,6 +269,8 @@ extern "C" int b200_corpus_create(int metric, int dtype, int d, int64_t capacity
     c->d_pad = pad_for(dtype, d);
     c->row_bytes = dtype == B200_DTYPE_BIN ? c->d_pad : (int64_t)c->d_pad * (dtype == B200_DTYPE_BF16 ? 2 : 4);
     c->cap = capacity_rows;
+    static std::atomic<uint64_t> next_serial{0};
+    c->serial = ++next_serial;
     cudaGetDevice(&c->device);
     c->sms = num_sms();
     if (const char *ev = getenv("B200_GEMM_RESCORE_L2")) c->rescore_l2 = atoi(ev);
@@ -293,6 +321,7 @@ static int corpus_alloc(b200_corpus *c, int64_t rows) {
     }
     c->cap = std::max(c->cap, rows);
     c->owns = true;
+    c->epoch++;
     return B200_OK;
 }
 
@@ -336,6 +365,7 @@ extern "C" int b200_corpus_append(b200_corpus *c, const void *rows, int64_t n) {
     B200_TRY(corpus_norms(c, c->n, n));
     B200_CUDA_OK(cudaStreamSynchronize(c->stream));
     c->n += n;
+    c->epoch++;
     return B200_OK;
 }
 
@@ -363,6 +393,7 @@ extern "C" int b200_corpus_adopt_device(b200_corpus *c, const void *device_rows,
     if (c->metric == B200_METRIC_COSINE) B200_CUDA_OK(cudaMalloc(&c->row_scale, (size_t)n * 4 + 256));
     if (c->metric == B200_METRIC_L2 || c->dtype == B200_DTYPE_BIN) B200_CUDA_OK(cudaMalloc(&c->row_bias, (size_t)n * 4 + 256));
     c->side_cap_rows = n;
+    c->epoch++;
     B200_TRY(corpus_norms(c, 0, n));
     B200_CUDA_OK(cudaStreamSynchronize(c->stream));
     return B200_OK;
@@ -381,6 +412,7 @@ extern "C" int b200_corpus_set_path(b200_corpus *c, int path) {
     // earlier target (CTA pairs, multicast clusters, queries in tensor memory); sm_90 has one tensor-core kernel per operand
     // type, so they select it.
     c->path = path >= 2 ? 2 : path;
+    c->epoch++;
     return B200_OK;
 }
 
@@ -424,9 +456,7 @@ extern "C" int b200_corpus_free(b200_corpus *c) {
     if (c->row_bias) cudaFree(c->row_bias);
     if (c->h_pin) cudaFreeHost(c->h_pin);
     if (c->d_tickets) cudaFree(c->d_tickets);
-    for (DevBuf *b : {&c->w_raw, &c->w_q32, &c->w_qbf, &c->w_qlo, &c->w_qnorm, &c->w_pk, &c->w_pi, &c->w_lk, &c->w_li, &c->w_alive,
-                      &c->w_odis, &c->w_oids, &c->w_stage, &c->w_prog, &c->w_pf_ids, &c->w_pf_tmp, &c->w_pf_rows, &c->w_pf_side})
-        b->release();
+    for (DevBuf *b : c->workspaces()) b->release();
     for (auto *v : {&c->ev_used, &c->ev_free})
         for (auto &ev : *v) {
             cudaEventDestroy(ev.first);
@@ -1109,6 +1139,7 @@ static int scratch_corpus(int metric, int dtype, int d, int64_t rows, b200_corpu
     c->n = 0;
     c->cap = 0;
     c->path = 0;
+    c->epoch++;
     (void)rows;
     *out = c;
     return B200_OK;

@@ -5,7 +5,7 @@
 // src/VectorIndex/Storages/MergeTreeBaseSearchManager.cpp:207-299) and the table-wide statistics sum of
 // ReadWithHybridSearch::getStatisticForTextSearch (src/VectorIndex/Processors/ReadWithHybridSearch.cpp:89-209).
 // The only data-path collective of the vector side is ONE ncclAllGather of the packed record
-// {float dis[nq * k]; int64 id[nq * k]} per rank and batch (122 KB at nq = 1024, k = 10: latency-bound over NVSwitch),
+// {float dis[nq * k]; padding to 8 bytes; int64 id[nq * k]} per rank and batch (122 KB at nq = 1024, k = 10: latency-bound over NVSwitch),
 // followed by the merge kernel (b200_topk_merge_device_ex); BM25 adds one ncclAllReduce(sum) of a few uint64 counters.
 // NCCL is resolved at run time (dlopen of the libnccl.so.2 the process already carries, e.g. PyTorch's): the library has no
 // link-time dependency on it and single-GPU users never touch it.
@@ -85,12 +85,31 @@ struct b200_comm {
     void *d_host_out = nullptr;              // merged result of the host-buffer gather
     size_t host_out_cap = 0;
     std::mutex mu;
-    // CUDA graphs of whole sharded search steps, keyed by everything that is baked into the nodes
-    std::map<std::tuple<const void *, const void *, int64_t, int, const void *, int64_t, void *, void *, void *>, cudaGraphExec_t> graphs;
-    std::map<cudaGraphExec_t, int64_t> graph_launches;   // kernels / collectives one replay stands for (launch accounting)
+    // CUDA graphs of whole sharded search steps, keyed by the corpus' serial number and the call's arguments; the corpus'
+    // state epoch at capture says whether the rows, side arrays, path and workspaces the nodes point at are still current
+    struct Graph {
+        cudaGraphExec_t exec = nullptr;
+        uint64_t epoch = 0;
+        int64_t launches = 0;   // kernels / collectives one replay stands for (launch accounting)
+    };
+    std::map<std::tuple<uint64_t, const void *, int64_t, int, const void *, int64_t, void *, void *, void *>, Graph> graphs;
+    int64_t graph_captures = 0, graph_replays = 0;
     void *host_stage = nullptr;                          // device staging of the host-buffer entry point
     size_t host_stage_cap = 0;
 };
+
+// The packed record of one rank: dis [nq * k] fp32, padded to a multiple of 8 bytes, then ids [nq * k] int64.  The record
+// size is a multiple of 8, so the ids of every gathered record are 8-byte aligned.
+static size_t record_dis_bytes(int64_t nq, int k) { return round_up((size_t)nq * k * 4, 8); }
+static size_t record_bytes(int64_t nq, int k) { return record_dis_bytes(nq, k) + (size_t)nq * k * 8; }
+static int64_t *record_ids(void *rec, int64_t nq, int k) {
+    return reinterpret_cast<int64_t *>(reinterpret_cast<char *>(rec) + record_dis_bytes(nq, k));
+}
+
+static void drop_graphs(b200_comm *c) {
+    for (auto &kv : c->graphs) cudaGraphExecDestroy(kv.second.exec);
+    c->graphs.clear();
+}
 
 #define B200_NCCL_OK(c, expr)                                                                                              \
     do {                                                                                                                   \
@@ -135,7 +154,7 @@ extern "C" int b200_comm_free(b200_comm *c) {
     if (!c) return B200_OK;
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
-    for (auto &kv : c->graphs) cudaGraphExecDestroy(kv.second);
+    drop_graphs(c);
     if (c->comm) c->api->CommDestroy(c->comm);
     for (void *p : {c->send, c->recv, (void *)c->d_counters, c->host_stage, c->d_host_out})
         if (p) cudaFree(p);
@@ -151,14 +170,13 @@ extern "C" int b200_comm_info(const b200_comm *c, int *rank, int *world) {
 }
 
 static int comm_reserve(b200_comm *c, int64_t nq, int k) {
-    const size_t rec = (size_t)nq * k * 12;
+    const size_t rec = record_bytes(nq, k);
     if (rec > c->send_cap) {
         if (c->send) cudaFree(c->send);
         if (c->recv) cudaFree(c->recv);
         c->send = c->recv = nullptr;
         c->send_cap = c->recv_cap = 0;
-        for (auto &kv : c->graphs) cudaGraphExecDestroy(kv.second);   // captured pointers are gone
-        c->graphs.clear();
+        drop_graphs(c);   // captured pointers are gone
         const size_t want = rec + rec / 4 + 256;
         if (cudaMalloc(&c->send, want) != cudaSuccess || cudaMalloc(&c->recv, want * c->world) != cudaSuccess) {
             cudaGetLastError();
@@ -177,31 +195,30 @@ extern "C" int b200_comm_local_buffers(b200_comm *c, int64_t nq, int k, float **
     B200_CUDA_OK(cudaSetDevice(c->device));
     B200_TRY(comm_reserve(c, std::max<int64_t>(nq, 1), k));
     *d_dis = reinterpret_cast<float *>(c->send);
-    *d_ids = reinterpret_cast<int64_t *>(reinterpret_cast<char *>(c->send) + (size_t)nq * k * 4);
+    *d_ids = record_ids(c->send, nq, k);
     return B200_OK;
 }
 
 // all-gather of the records written at b200_comm_local_buffers(nq, k) + merge -> the global top-k on every rank
 extern "C" int b200_comm_gather_merge(b200_comm *c, int64_t nq, int k, int descending, float *d_out_dis, int64_t *d_out_ids, void *stream) {
     if (!c || !d_out_dis || !d_out_ids || nq < 0 || k <= 0) return fail(B200_ERR_INVALID, "bad arguments");
+    // every refusal comes before the collective: a rank that returns early must not leave the others inside the all-gather
+    if (k > 2048) return fail(B200_ERR_UNSUPPORTED, "k > 2048 not supported by the merge kernel");
     if (nq == 0) return B200_OK;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    const size_t rec = (size_t)nq * k * 12;
+    const size_t rec = record_bytes(nq, k);
     if (rec > c->send_cap) return fail(B200_ERR_INVALID, "call b200_comm_local_buffers(nq, k) first");
     if (c->world == 1) {
         B200_CUDA_OK(cudaMemcpyAsync(d_out_dis, c->send, (size_t)nq * k * 4, cudaMemcpyDeviceToDevice, s));
-        B200_CUDA_OK(cudaMemcpyAsync(d_out_ids, reinterpret_cast<char *>(c->send) + (size_t)nq * k * 4, (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, s));
+        B200_CUDA_OK(cudaMemcpyAsync(d_out_ids, record_ids(c->send, nq, k), (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, s));
         return B200_OK;
     }
     B200_NCCL_OK(c, c->api->AllGather(c->send, c->recv, rec, ncclUint8, c->comm, s));
     g_launches++;
-    // list l of the gathered buffer: dis at recv + l * rec, ids 4 nq k bytes further (rec is a multiple of 8 when nq * k is even;
-    // the strides are passed in elements of the respective type, so rec must be divisible by 8)
-    if (rec % 8) return fail(B200_ERR_UNSUPPORTED, "nq * k must be even for the packed all-gather record");
-    return b200_topk_merge_device_ex(reinterpret_cast<const float *>(c->recv),
-                                     reinterpret_cast<const int64_t *>(reinterpret_cast<const char *>(c->recv) + (size_t)nq * k * 4), c->world,
-                                     (int64_t)(rec / 4), (int64_t)(rec / 8), nq, k, k, descending, 0, d_out_dis, d_out_ids, nullptr,
-                                     stream ? stream : nullptr);
+    // list l of the gathered buffer: dis at recv + l * rec, ids record_dis_bytes further; rec is a multiple of 8, so the
+    // strides are whole elements of both types
+    return b200_topk_merge_device_ex(reinterpret_cast<const float *>(c->recv), record_ids(c->recv, nq, k), c->world, (int64_t)(rec / 4),
+                                     (int64_t)(rec / 8), nq, k, k, descending, 0, d_out_dis, d_out_ids, nullptr, stream ? stream : nullptr);
 }
 
 // Host-buffer form for lists that are produced on the host (the per-shard BM25 top-k of b200_bm25_search_batch): uploads
@@ -270,12 +287,17 @@ extern "C" int b200_index_search_device(b200_index *ix, const float *d_queries, 
 namespace b200 {
 int corpus_metric(const b200_corpus *c);
 bool corpus_timing_enabled(const b200_corpus *c);
+int corpus_dim(const b200_corpus *c);
+int64_t corpus_query_row_bytes(const b200_corpus *c);
+uint64_t corpus_serial(const b200_corpus *c);
+uint64_t corpus_state_epoch(b200_corpus *c);
+int index_metric(const b200_index *ix);
 }
 
 static int sharded_corpus_step(b200_comm *cm, b200_corpus *corpus, const float *d_queries, int64_t nq, int k, const uint8_t *d_alive,
                                int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
     float *l_dis = reinterpret_cast<float *>(cm->send);
-    int64_t *l_ids = reinterpret_cast<int64_t *>(reinterpret_cast<char *>(cm->send) + (size_t)nq * k * 4);
+    int64_t *l_ids = record_ids(cm->send, nq, k);
     B200_TRY(b200_corpus_search_device(corpus, d_queries, nq, k, d_alive, id_offset, l_dis, l_ids, s));
     return b200_comm_gather_merge(cm, nq, k, corpus_metric(corpus) == B200_METRIC_IP ? 1 : 0, d_out_dis, d_out_ids, s);
 }
@@ -296,9 +318,16 @@ extern "C" int b200_sharded_corpus_search(b200_comm *cm, b200_corpus *corpus, co
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     if (!use_graph || corpus_timing_enabled(corpus))
         return sharded_corpus_step(cm, corpus, d_queries, nq, k, d_alive_bits, id_offset, d_out_dis, d_out_ids, s);
-    const auto key = std::make_tuple((const void *)corpus, (const void *)d_queries, nq, k, (const void *)d_alive_bits, id_offset, (void *)d_out_dis,
-                                     (void *)d_out_ids, (void *)s);
+    const auto key = std::make_tuple(corpus_serial(corpus), (const void *)d_queries, nq, k, (const void *)d_alive_bits, id_offset,
+                                     (void *)d_out_dis, (void *)d_out_ids, (void *)s);
     auto it = cm->graphs.find(key);
+    if (it != cm->graphs.end() && it->second.epoch != corpus_state_epoch(corpus)) {
+        // the corpus grew, moved, changed path or reallocated a workspace since the capture: the nodes point at old state
+        B200_CUDA_OK(cudaStreamSynchronize(s));
+        cudaGraphExecDestroy(it->second.exec);
+        cm->graphs.erase(it);
+        it = cm->graphs.end();
+    }
     if (it == cm->graphs.end()) {
         // first call: run eagerly once (sizes every workspace), then capture the identical sequence
         B200_TRY(sharded_corpus_step(cm, corpus, d_queries, nq, k, d_alive_bits, id_offset, d_out_dis, d_out_ids, s));
@@ -319,12 +348,26 @@ extern "C" int b200_sharded_corpus_search(b200_comm *cm, b200_corpus *corpus, co
         e = cudaGraphInstantiate(&exec, g, 0);
         cudaGraphDestroy(g);
         if (e != cudaSuccess) return fail(B200_ERR_CUDA, std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e));
-        it = cm->graphs.emplace(key, exec).first;
-        cm->graph_launches[exec] = per_step;
+        b200_comm::Graph gr;
+        gr.exec = exec;
+        gr.epoch = corpus_state_epoch(corpus);
+        gr.launches = per_step;
+        it = cm->graphs.emplace(key, gr).first;
+        cm->graph_captures++;
         g_launches = launches_before;   // the captured pass launched nothing
     }
-    B200_CUDA_OK(cudaGraphLaunch(it->second, s));
-    g_launches += cm->graph_launches[it->second];
+    B200_CUDA_OK(cudaGraphLaunch(it->second.exec, s));
+    cm->graph_replays++;
+    g_launches += it->second.launches;
+    return B200_OK;
+}
+
+// CUDA graphs this communicator captured and replayed (b200_sharded_corpus_search with use_graph)
+extern "C" int b200_comm_graph_stats(b200_comm *c, int64_t *captures, int64_t *replays) {
+    if (!c) return fail(B200_ERR_INVALID, "null communicator");
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (captures) *captures = c->graph_captures;
+    if (replays) *replays = c->graph_replays;
     return B200_OK;
 }
 
@@ -334,25 +377,27 @@ extern "C" int b200_sharded_corpus_search_host(b200_comm *cm, b200_corpus *corpu
                                                int64_t id_offset, float *out_dis, int64_t *out_ids, void *stream, int use_graph) {
     if (!cm || !corpus || (!queries && nq > 0) || !out_dis || !out_ids || nq < 0 || k <= 0 || d <= 0 || !stream)
         return fail(B200_ERR_INVALID, "bad arguments (a non-NULL stream is required)");
+    if (d != corpus_dim(corpus)) return fail(B200_ERR_INVALID, "d differs from the corpus' dimension");
     if (nq == 0) return B200_OK;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const size_t q_bytes = (size_t)nq * corpus_query_row_bytes(corpus);   // binary corpora: d / 8 bytes per query
     {
         std::lock_guard<std::mutex> lk(cm->mu);
         B200_CUDA_OK(cudaSetDevice(cm->device));
-        const size_t need = (size_t)nq * d * 4 + (size_t)nq * k * 12 + 64;
+        const size_t need = round_up(q_bytes, 16) + round_up((size_t)nq * k * 4, 16) + (size_t)nq * k * 8;
         if (need > cm->host_stage_cap) {
             if (cm->host_stage) cudaFree(cm->host_stage);
             cm->host_stage = nullptr;
-            for (auto &kv : cm->graphs) cudaGraphExecDestroy(kv.second);
-            cm->graphs.clear();
+            cm->host_stage_cap = 0;
+            drop_graphs(cm);
             B200_CUDA_OK(cudaMalloc(&cm->host_stage, need + need / 4));
             cm->host_stage_cap = need + need / 4;
         }
     }
     float *d_q = reinterpret_cast<float *>(cm->host_stage);
-    float *d_od = reinterpret_cast<float *>(reinterpret_cast<char *>(cm->host_stage) + round_up((size_t)nq * d * 4, 16));
+    float *d_od = reinterpret_cast<float *>(reinterpret_cast<char *>(cm->host_stage) + round_up(q_bytes, 16));
     int64_t *d_oi = reinterpret_cast<int64_t *>(reinterpret_cast<char *>(d_od) + round_up((size_t)nq * k * 4, 16));
-    B200_CUDA_OK(cudaMemcpyAsync(d_q, queries, (size_t)nq * d * 4, cudaMemcpyHostToDevice, s));
+    B200_CUDA_OK(cudaMemcpyAsync(d_q, queries, q_bytes, cudaMemcpyHostToDevice, s));
     B200_TRY(b200_sharded_corpus_search(cm, corpus, d_q, nq, k, nullptr, id_offset, d_od, d_oi, stream, use_graph));
     B200_CUDA_OK(cudaMemcpyAsync(out_dis, d_od, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaMemcpyAsync(out_ids, d_oi, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
@@ -365,12 +410,13 @@ extern "C" int b200_sharded_index_search(b200_comm *cm, b200_index *ix, int metr
                                          const uint8_t *d_alive_bits, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, void *stream) {
     if (!cm || !ix || (!d_queries && nq > 0) || !d_out_dis || !d_out_ids || nq < 0 || k <= 0 || !stream)
         return fail(B200_ERR_INVALID, "bad arguments (a non-NULL stream is required)");
+    if (metric != index_metric(ix)) return fail(B200_ERR_INVALID, "metric differs from the index' metric");
     if (nq == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(cm->mu);
     B200_CUDA_OK(cudaSetDevice(cm->device));
     B200_TRY(comm_reserve(cm, nq, k));
     float *l_dis = reinterpret_cast<float *>(cm->send);
-    int64_t *l_ids = reinterpret_cast<int64_t *>(reinterpret_cast<char *>(cm->send) + (size_t)nq * k * 4);
+    int64_t *l_ids = record_ids(cm->send, nq, k);
     B200_TRY(b200_index_search_device(ix, d_queries, nq, k, params, 0, d_alive_bits, id_offset, l_dis, l_ids, stream));
     return b200_comm_gather_merge(cm, nq, k, metric == B200_METRIC_IP ? 1 : 0, d_out_dis, d_out_ids, stream);
 }

@@ -1320,6 +1320,8 @@ int corpus_search_exact(b200_corpus *c, const void *d_queries, int64_t nq, int k
                         int prefilter_mode, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s);
 int64_t host_count_alive(const uint8_t *bits, int64_t n, int64_t limit);
 int64_t corpus_prefilter_limit(const b200_corpus *c, int mode, int64_t nq, int k);
+// hook for comm.cu: b200_sharded_index_search refuses a metric other than the index's
+int index_metric(const b200_index *ix) { return ix->metric; }
 }
 
 static int parse_int_param(const char *json, const char *key, int defv) {

@@ -119,9 +119,10 @@ class Comm:
     def sharded_corpus_search_host(self, corpus, queries, k: int, id_offset: int, stream: int, use_graph: bool = True, out=None):
         import numpy as np
         from ._lib import lib
-        from .search import _check
-        q = np.ascontiguousarray(queries, np.float32)
-        nq, d = q.shape
+        from .search import BIN, _check
+        binary = corpus.dtype == BIN   # query rows are bytes [nq][d / 8]
+        q = np.ascontiguousarray(queries, np.uint8 if binary else np.float32)
+        nq, d = q.shape[0], q.shape[1] * (8 if binary else 1)
         dis, ids = out if out is not None else (np.empty((nq, k), np.float32), np.empty((nq, k), np.int64))
         _check(lib().b200_sharded_corpus_search_host(self._h, corpus._h, q.ctypes.data_as(C.c_void_p), C.c_int64(nq), C.c_int(d), C.c_int(k),
                                                      C.c_int64(id_offset), dis.ctypes.data_as(C.c_void_p), ids.ctypes.data_as(C.c_void_p),
@@ -135,6 +136,14 @@ class Comm:
         _check(lib().b200_sharded_index_search(self._h, index._h, C.c_int(metric), C.c_void_p(q_ptr), C.c_int64(nq), C.c_int(k), params.encode(),
                                                C.c_void_p(alive_ptr or None), C.c_int64(id_offset), C.c_void_p(out_dis_ptr),
                                                C.c_void_p(out_ids_ptr), C.c_void_p(stream)))
+
+    def graph_stats(self):
+        """(captures, replays) of the sharded corpus search's CUDA graphs on this communicator."""
+        from ._lib import lib
+        from .search import _check
+        cap, rep = C.c_int64(), C.c_int64()
+        _check(lib().b200_comm_graph_stats(self._h, C.byref(cap), C.byref(rep)))
+        return cap.value, rep.value
 
     def gather_merge_host(self, dis, ids, descending: bool):
         """Per-shard [nq][k] lists held on the host (BM25 top-k) -> the table-wide top-k on every rank."""

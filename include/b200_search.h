@@ -221,18 +221,24 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *                               a non-zero one under L2 with B200_ERR_UNSUPPORTED (the loss is defined for inner-product
  *                               ranking), and d / M > 64 at train with B200_ERR_UNSUPPORTED;
  *   "MSTG"                      closed source upstream; here the two-stage index of SURVEY 2.5 K6: bf16 lists + exact
- *                               fp32 second stage (supportTwoStageSearch, first_stage_only, computeTopDistanceSubset);
+ *                               fp32 second stage (supportTwoStageSearch, first_stage_only, computeTopDistanceSubset).
+ *                               With "graph_degree=D" it also builds a neighbour graph (as HNSWFLAT below, from each row's
+ *                               2D + 1 nearest by its own list search's FIRST stage) and walks it over its bf16 list rows in
+ *                               HBM; with fp32 rows (keep_raw=1, or 2: in host memory) and refine_factor > 1 the walk's best
+ *                               min(1024, k x refine_factor) rows (out_num_candidates) are re-ranked exactly, otherwise
+ *                               it returns first-stage distances.  Every keep_raw is accepted with it;
  *   "SCANN", "HNSWFLAT", "HNSWSQ", "HNSWPQ"   accepted and SERVED BY THE INVERTED-FILE ENGINE with the payload their
  *                               name implies (PQ + re-rank, bf16, 8-bit, PQ): they traverse no graph unless HNSWFLAT
- *                               has graph_degree below (ScaNN's anisotropic PQ loss is the opt-in aq_threshold above); the contract for every ANN type is recall against
+ *                               has graph_degree below (MSTG's graph is above; ScaNN's anisotropic PQ loss is the opt-in aq_threshold above); the contract for every ANN type is recall against
  *                               FLAT, not traversal order (SURVEY 8c: parity unpinned for ANN at large N).
  *                               HNSWFLAT with "graph_degree=D" (D = 16, 32 or 64; absent or 0: the lists only) also builds a
  *                               neighbour graph [n][D] at finalize (each row's 2D nearest by its own list search, pruned by
  *                               rank, merged with reverse edges) and searches it by default: one CTA per query walks the graph
  *                               from the best min(ef_s, 32) ids of an nprobe=1 first stage, scoring each row once, exactly in
  *                               fp32.  Search keys: "ef_s=N" (list width, default 64, raised to k, at most 1024), "graph=0" (the
- *                               list search instead).  Any other type with graph_degree > 0, or keep_raw=0 / 2 with it:
- *                               B200_ERR_UNSUPPORTED; another D: B200_ERR_INVALID.  A part below the threshold has no graph;
+ *                               list search instead).  Any type but HNSWFLAT / MSTG with graph_degree > 0, or HNSWFLAT
+ *                               with keep_raw=0 / 2 and it: B200_ERR_UNSUPPORTED; another D: B200_ERR_INVALID.  A part
+ *                               below the threshold has no graph;
  *   "BINARYFLAT"                binary rows (metric HAMMING or JACCARD, d in bits: a multiple of 8, at most 65536), exact
  *                               resident binary corpus (scan or b1 tensor-core kernel, chosen as for a binary corpus);
  *   "BINARYIVF"                 inverted lists of the row bytes, coarse quantiser trained by k-majority (Hamming, for
@@ -305,7 +311,8 @@ int b200_index_search_device(b200_index *ix, const float *d_queries, int64_t nq,
                              const uint8_t *d_alive_bits /*nullable*/, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids,
                              void *stream);
 /* roofline inputs of the list scan: CUDA-event time of the grouped scan kernel since the last reset, bytes per list row,
- * and an upper bound of the work items of the last search.  After a graph search: the rows it scored, d_pad x 4 and nq.
+ * and an upper bound of the work items of the last search.  After a graph search: the rows it scored, the bytes of one
+ * row it read (HNSWFLAT: d_pad x 4, MSTG: the bf16 list row, d_pad64 x 2) and nq.
  * After the finalize of a graph_degree index, b200_index_phase_ms holds the graph build's candidates | prune | merge. */
 int b200_index_phase_ms(b200_index *ix, double out_ms[5]);   /* last search: coarse | pairs+plan+gather | scan | merge | refine */
 int b200_index_list_sizes(const b200_index *ix, uint32_t *out_sizes /*[nlist]*/, int capacity);
@@ -326,7 +333,8 @@ int b200_index_refine(b200_index *ix, const float *queries, int64_t nq, const in
 /* moves the fp32 rows of a finalized index between HBM (placement 1) and pinned host memory (2), the keep_raw values, under
  * the index mutex (waits for the device first); the move to host frees the HBM rows and their side arrays.  An index loaded
  * from an older file can so be demoted without a rebuild.  B200_ERR_INVALID for an index without rows (keep_raw=0) or not
- * finalized; B200_ERR_UNSUPPORTED where the rows are the index (FLAT, small parts, binary types). */
+ * finalized; B200_ERR_UNSUPPORTED where the rows are the index (FLAT, small parts, binary types) and for an HNSWFLAT graph
+ * (its walk reads them; an MSTG graph walks its bf16 list rows and moves in both directions). */
 int b200_index_set_raw_placement(b200_index *ix, int placement);
 /* graph_degree indexes: the neighbour graph, out[n][D] u32 (0xFFFFFFFF = empty slot; capacity_rows >= n, else
  * B200_ERR_INVALID; null: skipped), *out_degree = D, or 0 when the index has no graph (then nothing is copied) */
@@ -340,7 +348,8 @@ int b200_index_last_seeds(b200_index *ix, int64_t *out, int64_t capacity, int *o
  * index is written as v2.  load accepts both and validates every size it derives.  An index with its fp32 rows in host
  * memory writes the header's has_raw as 2 (every other byte as in HBM placement) and loads them straight into pinned host
  * memory again.  An index with a graph (graph_degree) is written as v4: the v2 layout with the reserved word holding D,
- * followed by the graph [n][D] u32; load checks every graph id (< n or 0xFFFFFFFF) before any kernel reads it. */
+ * followed by the graph [n][D] u32 (HNSWFLAT with has_raw 1, MSTG with has_raw 0, 1 or 2); load checks every graph id
+ * (< n or 0xFFFFFFFF) before any kernel reads it. */
 int b200_index_save(b200_index *ix, const char *path);
 int b200_index_load(const char *path, b200_index **out);
 /* the same through the host's own streams (Search::IndexDataFileWriter / Reader over ClickHouse disks,

@@ -1,4 +1,4 @@
-// graph.h -- fixed-degree neighbour graph of an HNSWFLAT index (graph_degree=D): build steps and the one-CTA-per-query
+// graph.h -- fixed-degree neighbour graph of an HNSWFLAT or MSTG index (graph_degree=D): build steps and the one-CTA-per-query
 // search (graph_sm90.cu).  The host side (candidates from the index's own list search, persistence, the search entry)
 // lives in ivf.cu.
 #pragma once
@@ -33,9 +33,17 @@ int graph_prune(const uint32_t *d_cand, int64_t n, int D, uint32_t *d_pruned, cu
 // reverse edges and merge: pruned [n][D] -> graph [n][D].  Allocates and frees its own scratch (2 x n x D x 12 B + the sort's).
 int graph_merge(const uint32_t *d_pruned, int64_t n, int D, uint32_t *d_graph, cudaStream_t s);
 
+// id -> pool slot map row_slot[n] of a finalized bf16 inverted-file index, from its page chains (one CTA per list)
+int graph_row_slots(const uint32_t *d_list_len, const uint32_t *d_list_page_off, const uint32_t *d_list_pages, const uint32_t *d_row_ids, int nlist,
+                    uint32_t *d_row_slot, cudaStream_t s);
+// out [m][d] fp32 = the bf16 page rows of ids row0 .. row0 + m - 1 (pool: [page][d_pad64 / 64][256][64] bf16)
+int graph_page_rows(const void *d_pool, const uint32_t *d_row_slot, int64_t row0, int64_t m, int d, int d_pad64, float *d_out, cudaStream_t s);
+
 struct GraphSearchParams {
     const float *queries;      // [nq][d_pad], prepared (cosine: unit)
-    const float *rows;         // [n][d_pad] fp32
+    const float *rows;         // [n][d_pad] fp32 (HNSWFLAT)
+    const void *pages;         // MSTG, else null: the bf16 list pool [page][d_pad64 / 64][256][64] (cosine: unit rows) ...
+    const uint32_t *row_slot;  // ... and row v's slot in it
     const uint32_t *graph;     // [n][degree], 0xFFFFFFFF = empty slot
     const int64_t *seeds;      // [nq][nseeds], negative = none
     const uint8_t *alive;      // nullable: bit r of byte r / 8 keeps row r
@@ -43,11 +51,13 @@ struct GraphSearchParams {
     int64_t *out_ids;
     unsigned long long *rows_scored;   // += rows scored by every query
     int64_t n, id_offset;
-    int d_pad, degree, nseeds, ef, k, max_iters;
+    int d_pad, d_pad64, degree, nseeds, ef, k, max_iters;   // k: entries returned per query
     int l2;                    // else inner product (distance -key)
 };
 
-size_t graph_search_smem(int d_pad, int ef, int k, bool filtered);
+// dynamic shared memory of one query's CTA; q_len = d_pad (fp32 rows) or d_pad64 (bf16 pages)
+size_t graph_search_smem(int q_len, int ef, int k, bool filtered);
+// graph_search_kernel over the fp32 rows, or graph_search_bf16_kernel when p.pages is set
 int graph_search(const GraphSearchParams &p, int64_t nq, cudaStream_t s);
 
 }  // namespace b200

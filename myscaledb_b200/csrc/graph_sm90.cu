@@ -1,9 +1,11 @@
-// graph_sm90.cu -- the neighbour graph of an HNSWFLAT index (graph_degree=D): candidate lists -> rank-based pruning ->
-// reverse edges and merge at build, and the one-CTA-per-query graph search (DESIGN §3).
+// graph_sm90.cu -- the neighbour graph of an HNSWFLAT or MSTG index (graph_degree=D): candidate lists -> rank-based pruning ->
+// reverse edges and merge at build, and the one-CTA-per-query graph search over fp32 rows (HNSWFLAT) or the bf16 list pages
+// (MSTG) (DESIGN §3).
 #include <cub/cub.cuh>
 
 #include "common.cuh"
 #include "graph.h"
+#include "ivf_aq.h"
 
 namespace b200 {
 
@@ -181,6 +183,48 @@ int graph_merge(const uint32_t *d_pruned, int64_t n, int D, uint32_t *d_graph, c
     return rc;
 }
 
+// One CTA per list walks its page chain, thread t on row t of every page (as list_alive_kernel in ivf.cu): the list's valid
+// rows record their pool slot under their id.  Slots past the list's length are never read.
+__global__ void __launch_bounds__(kPageRows) row_slot_kernel(const uint32_t *__restrict__ list_len, const uint32_t *__restrict__ list_page_off,
+                                                             const uint32_t *__restrict__ list_pages, const uint32_t *__restrict__ row_ids,
+                                                             uint32_t *__restrict__ row_slot) {
+    const int l = blockIdx.x;
+    const uint32_t len = list_len[l], off = list_page_off[l];
+    for (uint32_t j = 0; j * kPageRows < len; j++) {
+        if (j * kPageRows + threadIdx.x >= len) break;
+        const uint32_t slot = list_pages[off + j] * kPageRows + threadIdx.x;
+        row_slot[row_ids[slot]] = slot;
+    }
+}
+
+int graph_row_slots(const uint32_t *d_list_len, const uint32_t *d_list_page_off, const uint32_t *d_list_pages, const uint32_t *d_row_ids, int nlist,
+                    uint32_t *d_row_slot, cudaStream_t s) {
+    if (nlist == 0) return B200_OK;
+    row_slot_kernel<<<(unsigned)nlist, kPageRows, 0, s>>>(d_list_len, d_list_page_off, d_list_pages, d_row_ids, d_row_slot);
+    g_launches++;
+    B200_CUDA_OK(cudaGetLastError());
+    return B200_OK;
+}
+
+// rows [m][d] fp32 = the bf16 page rows of ids row0 .. row0 + m - 1 (the graph build's queries of an index without fp32 rows)
+__global__ void page_rows_kernel(const __nv_bfloat16 *__restrict__ pool, const uint32_t *__restrict__ row_slot, int64_t row0, int64_t m, int d, int d_pad64,
+                                 float *__restrict__ out) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= m * d) return;
+    const int64_t i = e / d;
+    const int j = (int)(e - i * d);
+    const uint32_t slot = row_slot[row0 + i];
+    out[e] = __bfloat162float(pool[(((size_t)(slot / kPageRows) * (d_pad64 / 64) + j / 64) * kPageRows + slot % kPageRows) * 64 + j % 64]);
+}
+
+int graph_page_rows(const void *d_pool, const uint32_t *d_row_slot, int64_t row0, int64_t m, int d, int d_pad64, float *d_out, cudaStream_t s) {
+    if (m == 0) return B200_OK;
+    page_rows_kernel<<<(unsigned)ceil_div(m * d, 256), 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16 *>(d_pool), d_row_slot, row0, m, d, d_pad64, d_out);
+    g_launches++;
+    B200_CUDA_OK(cudaGetLastError());
+    return B200_OK;
+}
+
 // ------------------------------------------------------------------------------------
 // search: one CTA per query
 // ------------------------------------------------------------------------------------
@@ -268,18 +312,20 @@ __device__ __forceinline__ void merge_lists(const float *lk, const uint32_t *li,
         }
     }
 }
-}  // namespace
 
 // Shared memory: the query, the visited table, two ef-entry lists (keys, ids, expanded flags) used in turn, the step's
 // candidates (adjacency order, then sorted), the neighbour row, two k-entry lists of alive rows (filtered searches only).
 // A step: warp 0 drops empty slots, repeats within the row and visited ids, compacts the rest in row order and inserts them
-// into the visited table; a warp per row scores them (128-bit loads, fp32, fixed lane order); they are sorted by (key, id) and
-// rank-merged into the ef list (and, those the bitmap keeps, into the alive list).  Every answer-bearing step is a sort or a
-// merge by (key, id): the result does not depend on thread timing.
-__global__ void __launch_bounds__(kGraphThreads) graph_search_kernel(const GraphSearchParams p) {
+// into the visited table; a warp per row scores them (`score`: 128-bit loads, fp32, fixed lane order); they are sorted by
+// (key, id) and rank-merged into the ef list (and, those the bitmap keeps, into the alive list).  Every answer-bearing step is
+// a sort or a merge by (key, id): the result does not depend on thread timing.  q_len: the query's floats in shared memory
+// (>= d_pad, zero beyond it), dim i at qs[qpos(i)]; score(id, qs, lane) returns, on every lane, the warp's L2 distance or inner
+// product of row id.
+template <class QPos, class Score>
+__device__ __forceinline__ void graph_walk(const GraphSearchParams &p, int q_len, QPos qpos, Score score) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const bool filtered = p.alive != nullptr;
-    const GraphSmem L = graph_smem_layout(p.d_pad, p.ef, p.k, filtered);
+    const GraphSmem L = graph_smem_layout(q_len, p.ef, p.k, filtered);
     float *qs = reinterpret_cast<float *>(smem_raw + L.qs);
     uint32_t *vis = reinterpret_cast<uint32_t *>(smem_raw + L.vis);
     // the two lists of each kind are at a fixed byte distance: list `b` of a kind is its list 0 plus b x that distance
@@ -302,7 +348,7 @@ __global__ void __launch_bounds__(kGraphThreads) graph_search_kernel(const Graph
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int64_t q = blockIdx.x;
     const int nwarps = kGraphThreads / 32;
-    for (int i = tid; i < p.d_pad; i += kGraphThreads) qs[i] = p.queries[q * p.d_pad + i];
+    for (int i = tid; i < q_len; i += kGraphThreads) qs[qpos(i)] = i < p.d_pad ? p.queries[q * p.d_pad + i] : 0.f;
     for (int i = tid; i < kGraphVisitedSlots; i += kGraphThreads) vis[i] = kNoId;
     for (int j = tid; j < p.nseeds; j += kGraphThreads) {
         const int64_t v = p.seeds[q * p.nseeds + j];
@@ -333,24 +379,7 @@ __global__ void __launch_bounds__(kGraphThreads) graph_search_kernel(const Graph
         __syncthreads();
         const int nc = sh[0];
         for (int c = warp; c < nc; c += nwarps) {
-            const float4 *row = reinterpret_cast<const float4 *>(p.rows + (size_t)ci[c] * p.d_pad);
-            const float4 *x4 = reinterpret_cast<const float4 *>(qs);
-            float acc = 0.f;
-            for (int cc = lane; cc < p.d_pad / 4; cc += 32) {
-                const float4 y = __ldg(row + cc);
-                const float4 x = x4[cc];
-                if (p.l2) {
-                    float t = x.x - y.x; acc = fmaf(t, t, acc);
-                    t = x.y - y.y; acc = fmaf(t, t, acc);
-                    t = x.z - y.z; acc = fmaf(t, t, acc);
-                    t = x.w - y.w; acc = fmaf(t, t, acc);
-                } else {
-                    acc = fmaf(x.x, y.x, acc); acc = fmaf(x.y, y.y, acc);
-                    acc = fmaf(x.z, y.z, acc); acc = fmaf(x.w, y.w, acc);
-                }
-            }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+            const float acc = score(ci[c], qs, lane);
             if (lane == 0) ck[c] = p.l2 ? acc : -acc;
         }
         scored += (unsigned long long)nc;
@@ -430,14 +459,84 @@ __global__ void __launch_bounds__(kGraphThreads) graph_search_kernel(const Graph
     }
     if (tid == 0) atomicAdd(p.rows_scored, scored);
 }
+}  // namespace
 
-size_t graph_search_smem(int d_pad, int ef, int k, bool filtered) { return (size_t)graph_smem_layout(d_pad, ef, k, filtered).total; }
+// HNSWFLAT: rows scored from the fp32 rows in HBM
+__global__ void __launch_bounds__(kGraphThreads) graph_search_kernel(const GraphSearchParams p) {
+    graph_walk(p, p.d_pad, [](int i) { return i; }, [&](uint32_t v, const float *qs, int lane) {
+        const float4 *row = reinterpret_cast<const float4 *>(p.rows + (size_t)v * p.d_pad);
+        const float4 *x4 = reinterpret_cast<const float4 *>(qs);
+        float acc = 0.f;
+        for (int cc = lane; cc < p.d_pad / 4; cc += 32) {
+            const float4 y = __ldg(row + cc);
+            const float4 x = x4[cc];
+            if (p.l2) {
+                float t = x.x - y.x; acc = fmaf(t, t, acc);
+                t = x.y - y.y; acc = fmaf(t, t, acc);
+                t = x.z - y.z; acc = fmaf(t, t, acc);
+                t = x.w - y.w; acc = fmaf(t, t, acc);
+            } else {
+                acc = fmaf(x.x, y.x, acc); acc = fmaf(x.y, y.y, acc);
+                acc = fmaf(x.z, y.z, acc); acc = fmaf(x.w, y.w, acc);
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        return acc;
+    });
+}
+
+// MSTG: rows scored in place from the bf16 list pages, row v at pool slot row_slot[v] ([page][d_pad64 / 64][256][64] bf16).
+// Lane l reads 16 bytes (8 dims) of the 128-byte segment of k-block l / 8 + 4j, widens them to fp32 and accumulates against
+// the query in its fixed order; the lane tree below is fixed, so a key depends on the row and the query alone.  The query's
+// dims of a k-block sit in shared memory as [half][part][4]: dim 8 part + 4 half + e at 32 half + 4 part + e, so that the 8
+// lanes of a quarter-warp read its two float4 of each k-block from 128 contiguous bytes each (no bank conflict).
+// acc plus the terms of the two dims of a bf16 pair (low half first) against the query's x0, x1
+__device__ __forceinline__ float bf16x2_term(int l2, uint32_t u, float x0, float x1, float acc) {
+    const float y0 = __uint_as_float(u << 16), y1 = __uint_as_float(u & 0xffff0000u);
+    if (l2) {
+        float t = x0 - y0; acc = fmaf(t, t, acc);
+        t = x1 - y1; return fmaf(t, t, acc);
+    }
+    acc = fmaf(x0, y0, acc);
+    return fmaf(x1, y1, acc);
+}
+
+// (kGraphThreads, 2): without the occupancy hint ptxas keeps this walk to 32 registers and spills; two CTAs per SM is what its
+// shared memory allows at the largest lists anyway
+__global__ void __launch_bounds__(kGraphThreads, 2) graph_search_bf16_kernel(const GraphSearchParams p) {
+    const auto qpos = [](int i) { return (i & ~63) | ((i >> 2) & 1) << 5 | ((i >> 3) & 7) << 2 | (i & 3); };
+    graph_walk(p, p.d_pad64, qpos, [&](uint32_t v, const float *qs, int lane) {
+        const uint32_t slot = p.row_slot[v];
+        const int kbs = p.d_pad64 / 64, seg = lane >> 3, part = lane & 7;
+        const __nv_bfloat16 *pool = static_cast<const __nv_bfloat16 *>(p.pages);
+        const uint4 *row = reinterpret_cast<const uint4 *>(pool + ((size_t)(slot / kPageRows) * kbs * kPageRows + slot % kPageRows) * 64) + part;
+        const float4 *x4 = reinterpret_cast<const float4 *>(qs) + part;
+        float acc = 0.f;
+        for (int kb = seg; kb < kbs; kb += 4) {
+            const uint4 u = __ldg(row + (size_t)kb * kPageRows * 8);
+            const float4 xa = x4[kb * 16], xb = x4[kb * 16 + 8];
+            acc = bf16x2_term(p.l2, u.x, xa.x, xa.y, acc);
+            acc = bf16x2_term(p.l2, u.y, xa.z, xa.w, acc);
+            acc = bf16x2_term(p.l2, u.z, xb.x, xb.y, acc);
+            acc = bf16x2_term(p.l2, u.w, xb.z, xb.w, acc);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        return acc;
+    });
+}
+
+size_t graph_search_smem(int q_len, int ef, int k, bool filtered) { return (size_t)graph_smem_layout(q_len, ef, k, filtered).total; }
 
 int graph_search(const GraphSearchParams &p, int64_t nq, cudaStream_t s) {
     if (nq == 0) return B200_OK;
-    const size_t smem = graph_search_smem(p.d_pad, p.ef, p.k, p.alive != nullptr);
-    B200_CUDA_OK(cudaFuncSetAttribute(graph_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    graph_search_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
+    const bool bf16 = p.pages != nullptr;
+    const size_t smem = graph_search_smem(bf16 ? p.d_pad64 : p.d_pad, p.ef, p.k, p.alive != nullptr);
+    const void *fn = bf16 ? (const void *)graph_search_bf16_kernel : (const void *)graph_search_kernel;
+    B200_CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (bf16) graph_search_bf16_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
+    else graph_search_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
     g_launches++;
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;

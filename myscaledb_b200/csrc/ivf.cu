@@ -1290,14 +1290,16 @@ struct b200_index {
     bool last_probe_exact = false;
     // statistics of the last search (tests, bench roofline): rows x payload bytes the scan kernel was asked to stream
     int64_t last_scan_rows = 0, last_items = 0;
-    // graph_degree=D (HNSWFLAT): neighbour graph [n][D] u32 built at finalize, 0xFFFFFFFF = empty slot (graph_sm90.cu)
+    // graph_degree=D (HNSWFLAT, MSTG): neighbour graph [n][D] u32 built at finalize, 0xFFFFFFFF = empty slot (graph_sm90.cu);
+    // MSTG walks its bf16 list rows in place: d_row_slot[n] = row id -> pool slot, derived from the page chains at finalize
+    // and at load (never saved: a load may place the pages elsewhere)
     int graph_degree = 0;
-    uint32_t *d_graph = nullptr;
+    uint32_t *d_graph = nullptr, *d_row_slot = nullptr;
     // seed ids [last_seed_nq][last_seed_s] of the last graph search (b200_index_last_seeds), and their first-stage distances
     DevArr w_seeds, w_seedd;
     int64_t last_seed_nq = 0;
     int last_seed_s = 0;
-    bool last_graph = false;        // the last search walked the graph: last_scan reports rows scored x d_pad x 4 bytes
+    bool last_graph = false;        // the last search walked the graph: last_scan reports the rows it scored
     bool timing = false, timed_pending = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaEvent_t ev_ph[6] = {};      // phase boundaries of the last search: start | coarse | pairs+plan+gather | scan | merge | refine
@@ -1432,19 +1434,20 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
     const int dflt_refine = (ty == IDX_IVFPQ || ty == IDX_IVFSQ || bin) ? 1 : (ix->payload == IVF_PRODUCER_PQ ? 16 : 4);
     ix->refine_factor = parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", dflt_refine));
     ix->keep_raw = parse_int_param(params, "keep_raw", -1);
-    // graph_degree=D: HNSWFLAT only, over its fp32 rows in HBM (the reference's m is PQ M here and keeps that meaning)
+    // graph_degree=D: HNSWFLAT, walked over its fp32 rows in HBM, or MSTG, walked over its bf16 list rows with any keep_raw
+    // (the reference's m is PQ M here and keeps that meaning)
     ix->graph_degree = parse_int_param(params, "graph_degree", 0);
     if (ix->graph_degree > 0) {
-        if (ty != IDX_HNSWFLAT) {
+        if (ty != IDX_HNSWFLAT && ty != IDX_MSTG) {
             delete ix;
-            return fail(B200_ERR_UNSUPPORTED, "graph_degree: a neighbour graph is built on HNSWFLAT only (the other types keep quantised or binary rows)");
+            return fail(B200_ERR_UNSUPPORTED, "graph_degree: a neighbour graph is built on HNSWFLAT and MSTG only (the other types keep quantised or binary rows)");
         }
         if (!graph_degree_ok(ix->graph_degree)) {
             const int gd = ix->graph_degree;
             delete ix;
             return fail(B200_ERR_INVALID, "graph_degree must be 16, 32 or 64 (or 0: no graph), got " + std::to_string(gd));
         }
-        if (ix->keep_raw == 0 || ix->keep_raw == 2) {
+        if (ty == IDX_HNSWFLAT && (ix->keep_raw == 0 || ix->keep_raw == 2)) {
             delete ix;
             return fail(B200_ERR_UNSUPPORTED, "graph_degree: the graph search reads the fp32 rows in HBM (keep_raw=1)");
         }
@@ -1468,7 +1471,8 @@ extern "C" int b200_index_free(b200_index *ix) {
     if (ix->coarse) b200_corpus_free(ix->coarse);
     for (void *p : {(void *)ix->d_centroids, (void *)ix->d_bcent, (void *)ix->d_cnorm, (void *)ix->d_pq, (void *)ix->d_pq_bf16, (void *)ix->d_sq, ix->d_pool, (void *)ix->d_row_bias,
                     (void *)ix->d_row_ids, (void *)ix->d_list_len, (void *)ix->d_tail_page, (void *)ix->d_page_owner, (void *)ix->d_page_seq,
-                    (void *)ix->d_pages_used, (void *)ix->d_flag, (void *)ix->d_list_page_off, (void *)ix->d_list_pages, (void *)ix->d_list_order, (void *)ix->d_graph})
+                    (void *)ix->d_pages_used, (void *)ix->d_flag, (void *)ix->d_list_page_off, (void *)ix->d_list_pages, (void *)ix->d_list_order, (void *)ix->d_graph,
+                    (void *)ix->d_row_slot})
         if (p) cudaFree(p);
     for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_cnt, &ix->w_plan,
                       &ix->w_sort, &ix->w_q, &ix->w_qraw, &ix->w_probe, &ix->w_pd, &ix->w_items, &ix->w_qbuf, &ix->w_inv, &ix->w_ppb, &ix->w_pconst, &ix->w_qb, &ix->w_cs,
@@ -2156,17 +2160,32 @@ struct DevScratch {   // freed on every return path of the graph build
 };
 }  // namespace
 
-// graph_degree=D: every row searches the index's own lists with its defaults (nprobe, exact re-rank with refine_factor) for
-// k = 2D + 1, exactly ix.search(rows, 2D + 1, "graph=0"); its own id dropped, the 2D candidates are pruned by rank (CAGRA) and
-// merged with the reverse edges (graph_sm90.cu).  phase_ms then holds candidates | prune | merge in milliseconds.
+// MSTG graph: d_row_slot[n] from the page chains of the finalized (or loaded) lists
+static int build_row_slot(b200_index *ix) {
+    if (!ix->d_row_slot && cudaMalloc(&ix->d_row_slot, std::max<size_t>((size_t)ix->n * 4, 16)) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(B200_ERR_NOMEM, "cudaMalloc of the graph's row slot map failed");
+    }
+    // a loaded file whose row ids repeat would leave ids unmapped: they read slot 0, never a slot outside the pool
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_row_slot, 0, (size_t)ix->n * 4, ix->stream));
+    return graph_row_slots(ix->d_list_len, ix->d_list_page_off, ix->d_list_pages, ix->d_row_ids, ix->nlist, ix->d_row_slot, ix->stream);
+}
+
+// graph_degree=D: every row searches the index's own lists with its defaults for k = 2D + 1.  HNSWFLAT: nprobe and the exact
+// re-rank with refine_factor, exactly ix.search(rows, 2D + 1, "graph=0").  MSTG: the first stage only, exactly
+// ix.search(rows, 2D + 1, "graph=0", first_stage_only=True): the graph is built in the metric its walk scores, the same way for
+// either placement of the fp32 rows, and never reads a row over PCIe.  The queries are the fp32 rows (HBM or host memory), or,
+// in an index without them (MSTG keep_raw=0), the bf16 list rows.  Its own id dropped, a row's 2D candidates are pruned by rank
+// (CAGRA) and merged with the reverse edges (graph_sm90.cu).  phase_ms then holds candidates | prune | merge in milliseconds.
 static int build_graph_locked(b200_index *ix) {
     using clk = std::chrono::steady_clock;
     const auto ms_since = [](clk::time_point t) { return std::chrono::duration<double, std::milli>(clk::now() - t).count(); };
     cudaStream_t s = ix->stream;
     const int D = ix->graph_degree, K = 2 * D, d = ix->d;
     const int64_t n = ix->n;
+    const bool mstg = ix->type == IDX_MSTG;
     const int np = std::max(1, std::min(ix->default_nprobe, ix->nlist));
-    const int k1 = std::min(1024, (K + 1) * std::max(1, ix->refine_factor));
+    const int k1 = mstg ? K + 1 : std::min(1024, (K + 1) * std::max(1, ix->refine_factor));
     const int64_t chunk = std::max<int64_t>(256, std::min<int64_t>(n, kGraphBuildSearchBytes / ((int64_t)np * k1 * 8)));
     DevScratch cand, pruned, q, dis, ids;
     B200_TRY(cand.alloc((size_t)n * K * 4));
@@ -2174,11 +2193,15 @@ static int build_graph_locked(b200_index *ix) {
     B200_TRY(dis.alloc((size_t)chunk * (K + 1) * 4));
     B200_TRY(ids.alloc((size_t)chunk * (K + 1) * 8));
     auto t = clk::now();
-    const float *rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
+    const float *rows = ix->raw ? reinterpret_cast<const float *>(corpus_device_rows(ix->raw)) : ix->h_rows;
     for (int64_t off = 0; off < n; off += chunk) {
         const int64_t m = std::min(chunk, n - off);
-        B200_CUDA_OK(cudaMemcpy2DAsync(q.p, (size_t)d * 4, rows + off * ix->d_pad, (size_t)ix->d_pad * 4, (size_t)d * 4, m, cudaMemcpyDeviceToDevice, s));
-        B200_TRY(search_device_locked(ix, static_cast<float *>(q.p), m, K + 1, nullptr, 0, nullptr, nullptr, 0, static_cast<float *>(dis.p),
+        if (rows)
+            B200_CUDA_OK(cudaMemcpy2DAsync(q.p, (size_t)d * 4, rows + off * ix->d_pad, (size_t)ix->d_pad * 4, (size_t)d * 4, m,
+                                           ix->raw ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
+        else
+            B200_TRY(graph_page_rows(ix->d_pool, ix->d_row_slot, off, m, d, ix->d_pad64, static_cast<float *>(q.p), s));
+        B200_TRY(search_device_locked(ix, static_cast<float *>(q.p), m, K + 1, nullptr, mstg ? 1 : 0, nullptr, nullptr, 0, static_cast<float *>(dis.p),
                                       static_cast<int64_t *>(ids.p), nullptr, s));
         B200_TRY(graph_candidates(static_cast<int64_t *>(ids.p), m, off, K, static_cast<uint32_t *>(cand.p) + off * K, s));
     }
@@ -2257,7 +2280,10 @@ static int finalize_locked(b200_index *ix) {
         if (!ix->use_ivf) B200_TRY(b200_corpus_create(ix->binary ? ix->metric : raw_metric, ix->binary ? B200_DTYPE_BIN : B200_DTYPE_F32, ix->d, 0, &ix->raw));
     }
     // a part below the inverted-file threshold is FLAT and gets no graph
-    if (ix->graph_degree > 0 && ix->use_ivf && ix->n > 0 && !ix->d_graph) B200_TRY(build_graph_locked(ix));
+    if (ix->graph_degree > 0 && ix->use_ivf && ix->n > 0 && !ix->d_graph) {
+        if (ix->type == IDX_MSTG) B200_TRY(build_row_slot(ix));
+        B200_TRY(build_graph_locked(ix));
+    }
     ix->built = true;
     return B200_OK;
 }
@@ -2309,6 +2335,7 @@ extern "C" int b200_index_memory_bytes(const b200_index *ix, uint64_t *out_bytes
         if (ix->d_pq) b += (uint64_t)ix->m * pq_codewords(ix->pq_bits) * ix->dsub * (ix->d_pq_bf16 ? 6 : 4);   // fp32 codebook (+ the decoder's bf16 copy)
     }
     if (ix->d_graph) b += (uint64_t)ix->n * ix->graph_degree * 4;
+    if (ix->d_row_slot) b += (uint64_t)ix->n * 4;
     *out_bytes = b;
     return B200_OK;
 }
@@ -2328,7 +2355,8 @@ extern "C" int b200_index_set_raw_placement(b200_index *ix, int placement) {
     if (ix->binary || !ix->use_ivf)
         return fail(B200_ERR_UNSUPPORTED, "the rows are the index here (FLAT, a part below the inverted-file threshold or a binary index): they stay in HBM");
     if (ix->keep_raw != 1 && ix->keep_raw != 2) return fail(B200_ERR_INVALID, "this index keeps no fp32 rows (keep_raw=0)");
-    if (placement == 2 && ix->d_graph) return fail(B200_ERR_UNSUPPORTED, "graph_degree: the graph search reads the fp32 rows in HBM");
+    if (placement == 2 && ix->d_graph && ix->type == IDX_HNSWFLAT)
+        return fail(B200_ERR_UNSUPPORTED, "graph_degree: the HNSWFLAT graph search reads the fp32 rows in HBM");
     if (placement == ix->keep_raw) return B200_OK;
     B200_CUDA_OK(cudaSetDevice(ix->device));
     // searches enqueued on the callers' streams may still read the rows that are about to be freed
@@ -2389,7 +2417,8 @@ extern "C" int b200_index_last_scan(b200_index *ix, int64_t *rows_streamed, int6
         if (cudaMemcpy(&r, ix->d_flag + 4, 8, cudaMemcpyDeviceToHost) == cudaSuccess) ix->last_scan_rows = (int64_t)r;
     }
     if (rows_streamed) *rows_streamed = ix->last_scan_rows;
-    if (payload_row_bytes_out) *payload_row_bytes_out = ix->last_graph ? (int64_t)ix->d_pad * 4 : (int64_t)payload_row_bytes(ix);
+    // the graph walk reads fp32 rows (HNSWFLAT) or the bf16 list rows (MSTG)
+    if (payload_row_bytes_out) *payload_row_bytes_out = ix->last_graph && !ix->d_row_slot ? (int64_t)ix->d_pad * 4 : (int64_t)payload_row_bytes(ix);
     if (work_items) *work_items = ix->last_items;
     if (kernel_ms_total) *kernel_ms_total = ix->timed_ms;
     if (kernel_launches) *kernel_launches = ix->timed_launches;
@@ -2869,10 +2898,13 @@ static int graph_ef(const char *params, int k) {
 }
 
 // The graph search, asynchronous on s (d_q: the prepared queries [nq][d_pad]): seeds from the list path's first stage at
-// nprobe 1 (the best min(ef_s, 32) ids per query), then graph_search_kernel, one CTA per query, over the fp32 rows in HBM.
-static int graph_search_locked(b200_index *ix, const float *d_queries, const float *d_q, int64_t nq, int k, const char *params, const uint8_t *d_alive,
-                               int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
-    const int ef = graph_ef(params, k);
+// nprobe 1 (the best min(ef_s, 32) ids per query), then one CTA per query walks the graph: graph_search_kernel over the fp32
+// rows in HBM (HNSWFLAT, kc = k), or graph_search_bf16_kernel over the bf16 list rows (MSTG).  With a second stage
+// (two_stage, MSTG only; kc may equal k, at k = 1024) the walk's best kc rows are re-ranked exactly by refine_device, from HBM
+// or from host memory.
+static int graph_search_locked(b200_index *ix, const float *d_queries, const float *d_q, int64_t nq, int k, int kc, bool two_stage, const char *params,
+                               const uint8_t *d_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
+    const int ef = graph_ef(params, kc);
     const int S = std::min(ef, kGraphMaxSeeds);
     B200_TRY(ix->w_seeds.reserve((size_t)nq * S * 8));
     B200_TRY(ix->w_seedd.reserve((size_t)nq * S * 4));
@@ -2882,26 +2914,38 @@ static int graph_search_locked(b200_index *ix, const float *d_queries, const flo
     ix->last_seed_s = S;
     unsigned long long *scored = reinterpret_cast<unsigned long long *>(ix->d_flag + 4);
     B200_CUDA_OK(cudaMemsetAsync(scored, 0, 8, s));
+    if (two_stage) {
+        B200_TRY(ix->w_od.reserve((size_t)nq * kc * 4));
+        B200_TRY(ix->w_oi.reserve((size_t)nq * kc * 8));
+    }
     GraphSearchParams gp{};
     gp.queries = d_q;
-    gp.rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
+    if (ix->d_row_slot) {
+        gp.pages = ix->d_pool;
+        gp.row_slot = ix->d_row_slot;
+    } else {
+        gp.rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
+    }
     gp.graph = ix->d_graph;
     gp.seeds = ix->w_seeds.as<int64_t>();
     gp.alive = d_alive;
-    gp.out_dis = d_out_dis;
-    gp.out_ids = d_out_ids;
+    gp.out_dis = two_stage ? ix->w_od.as<float>() : d_out_dis;
+    gp.out_ids = two_stage ? ix->w_oi.as<int64_t>() : d_out_ids;
     gp.rows_scored = scored;
     gp.n = ix->n;
-    gp.id_offset = id_offset;
+    gp.id_offset = two_stage ? 0 : id_offset;
     gp.d_pad = ix->d_pad;
+    gp.d_pad64 = ix->d_pad64;
     gp.degree = ix->graph_degree;
     gp.nseeds = S;
     gp.ef = ef;
-    gp.k = k;
+    gp.k = kc;
     gp.max_iters = graph_iteration_cap(ix->graph_degree);
     gp.l2 = ix->metric == B200_METRIC_L2;
     B200_TRY(graph_search(gp, nq, s));
-    if (ix->metric == B200_METRIC_COSINE) {
+    if (two_stage) {
+        B200_TRY(refine_device(ix, d_q, nq, ix->w_oi.as<int64_t>(), kc, k, id_offset, d_out_dis, d_out_ids, s));
+    } else if (ix->metric == B200_METRIC_COSINE) {
         cosine_finish_kernel<<<(unsigned)ceil_div(nq * k, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, k, d_out_dis, d_out_ids);
         g_launches++;
     }
@@ -2951,13 +2995,24 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     bool exact = !ix->use_ivf || force_exact == 1;
     // graph_degree indexes walk their graph unless asked for the lists (graph=0) or the exact pass (exact_batch=1)
     const bool graph = ix->d_graph && !exact && parse_int_param(params, "graph", 1) != 0;
+    // the walk returns kc rows per query: HNSWFLAT's are exact (kc = k); MSTG's are re-ranked from the fp32 rows when it has a
+    // second stage (graph_two_stage, the list path's two_stage; kc = min(1024, k x refine_factor), its k1)
+    int kc = k;
+    bool graph_two_stage = false;
     if (graph) {
         if (k > kGraphMaxEf) return fail(B200_ERR_UNSUPPORTED, "k > 1024 on the graph search");
         const int ef_s = parse_int_param(params, "ef_s", 64);
         if (ef_s > kGraphMaxEf) return fail(B200_ERR_INVALID, "ef_s must be at most 1024, got " + std::to_string(ef_s));
-        if (d_alive && h_alive) {
-            const int64_t rows_cap = graph_rows_at_cap(ix, std::min(graph_ef(params, k), kGraphMaxSeeds));
-            const int64_t limit = std::min<int64_t>((int64_t)std::ceil(kGraphExactFactor * k * (double)ix->n / (double)rows_cap) - 1,
+        if (ix->d_row_slot) {
+            const int refine_factor = std::max(1, parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", ix->refine_factor)));
+            graph_two_stage = has_rows(ix) && refine_factor > 1 && !first_stage_only;
+            if (graph_two_stage) kc = std::min(kGraphMaxEf, k * refine_factor);
+        }
+        if (out_num_candidates) *out_num_candidates = kc;
+        // the exact rule scans the fp32 rows in HBM: without them (MSTG keep_raw=0 | 2) the walk always answers
+        if (d_alive && h_alive && ix->raw) {
+            const int64_t rows_cap = graph_rows_at_cap(ix, std::min(graph_ef(params, kc), kGraphMaxSeeds));
+            const int64_t limit = std::min<int64_t>((int64_t)std::ceil(kGraphExactFactor * kc * (double)ix->n / (double)rows_cap) - 1,
                                                     corpus_prefilter_limit(ix->raw, prefilter, nq, k));
             exact = limit >= 0 && host_count_alive(h_alive, ix->n, limit) <= limit;
             ix->last_probe_exact = exact;
@@ -2973,6 +3028,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         ix->last_probe_exact = exact;
     }
     if (exact) {
+        if (out_num_candidates) *out_num_candidates = k;
         ix->last_probe.insert(ix->last_probe.end(), nq, 0);
         if (ix->keep_raw == 2)
             return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available with the fp32 rows in host memory (keep_raw=2 placement): "
@@ -2989,7 +3045,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         }
         return B200_OK;
     }
-    if (graph) return graph_search_locked(ix, d_queries, d_q, nq, k, params, d_alive, id_offset, d_out_dis, d_out_ids, s);
+    if (graph) return graph_search_locked(ix, d_queries, d_q, nq, k, kc, graph_two_stage, params, d_alive, id_offset, d_out_dis, d_out_ids, s);
     if (k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 on IVF indexes");
     const int nl = ix->nlist;
     int nprobe = parse_int_param(params, "nprobe", ix->default_nprobe);
@@ -3353,9 +3409,10 @@ static int index_load_io(Io *f, b200_index **out) {
         !(h.reserved0 == 4 && h.payload == IVF_PRODUCER_PQ && h.use_ivf && h.m > 0 && h.dsub > 0 && (int64_t)h.m * h.dsub == h.d &&
           h.code_bytes >= pq_code_bytes(h.m, 4) && h.code_bytes % 16 == 0 && ivf_pq4_fits(h.m)))
         return fail(B200_ERR_INVALID, "corrupt index header (v3: 4-bit PQ with M <= " + std::to_string(ivf_pq4_max_m()) + " expected)");
-    // v4: an HNSWFLAT inverted-file index with its fp32 rows in HBM and a graph of degree reserved0
-    if (h.version == 4 && !(graph_degree_ok((int)h.reserved0) && h.type == IDX_HNSWFLAT && h.use_ivf && h.has_raw == 1))
-        return fail(B200_ERR_INVALID, "corrupt index header (v4: an HNSWFLAT graph of degree 16, 32 or 64 over HBM rows expected)");
+    // v4: an inverted-file index with a graph of degree reserved0: HNSWFLAT with its fp32 rows in HBM, or MSTG with any rows
+    if (h.version == 4 && !(graph_degree_ok((int)h.reserved0) && h.use_ivf &&
+                            ((h.type == IDX_HNSWFLAT && h.has_raw == 1) || (h.type == IDX_MSTG && h.payload == IVF_PRODUCER_TMA))))
+        return fail(B200_ERR_INVALID, "corrupt index header (v4: an HNSWFLAT graph of degree 16, 32 or 64 over HBM rows, or an MSTG graph, expected)");
     const bool sane = h.type >= 0 && h.type < IDX_NUM_TYPES && h.metric >= 0 && h.metric <= 4 && (h.metric >= B200_METRIC_HAMMING) == bin &&
                       h.d > 0 && h.d <= (1 << 16) && (!bin || h.d % 8 == 0) && h.n >= 0 &&
                       h.n < (int64_t)0xffffffffll && h.payload >= 0 && h.payload <= 3 && (h.payload == IVF_PRODUCER_B1) == bin &&
@@ -3494,6 +3551,9 @@ static int index_load_io(Io *f, b200_index **out) {
                     if (buf[e] != kNoId && buf[e] >= (uint64_t)h.n) return bail("corrupt index file (graph id out of range)");
                 if (cudaMemcpy(ix->d_graph + off * D, buf.data(), (size_t)mrows * rb, cudaMemcpyHostToDevice) != cudaSuccess) return bail("H2D failed");
             }
+            // MSTG: the slot map of the pages as loaded here
+            if (h.type == IDX_MSTG && (build_row_slot(ix) != B200_OK || cudaStreamSynchronize(ix->stream) != cudaSuccess))
+                return bail(std::string("graph row slot map: ") + b200_last_error());
         }
     } catch (const std::bad_alloc &) {
         return bail("out of host memory while loading the index");

@@ -118,7 +118,7 @@ static const char * const MYSCALE_VALID_INDEX_PARAMETER = R"({
  "HNSWSQ": {"m": {"type": "int", "range": [8, 128]}, "ef_c": {"type": "int", "range": [16, 1024]}, "ef_s": {"type": "int", "range": [16, 1024]}, "nprobe": {"type": "int", "range": [1, 1048576]}},
  "HNSWPQ": {"m": {"type": "int", "range": [8, 128]}, "M": {"type": "int", "range": [1, 4096]}, "aq_threshold": {"type": "float", "range": [0, 1]}, "nprobe": {"type": "int", "range": [1, 1048576]}},
  "SCANN": {"ncentroids": {"type": "int", "range": [1, 1048576]}, "M": {"type": "int", "range": [1, 4096]}, "aq_threshold": {"type": "float", "range": [0, 1]}, "nprobe": {"type": "int", "range": [1, 1048576]}, "reorder_k_factor": {"type": "int", "range": [1, 100]}},
- "MSTG": {"ncentroids": {"type": "int", "range": [1, 1048576]}, "alpha": {"type": "float", "range": [1, 4]}, "nprobe": {"type": "int", "range": [1, 1048576]}, "refine_factor": {"type": "int", "range": [1, 100]}, "disk_mode": {"type": "int", "range": [0, 2]}},
+ "MSTG": {"ncentroids": {"type": "int", "range": [1, 1048576]}, "alpha": {"type": "float", "range": [1, 4]}, "nprobe": {"type": "int", "range": [1, 1048576]}, "refine_factor": {"type": "int", "range": [1, 100]}, "disk_mode": {"type": "int", "range": [0, 2]}, "graph_degree": {"type": "int", "range": [0, 64]}, "ef_s": {"type": "int", "range": [16, 1024]}},
  "BinaryIVF": {}, "BinaryHNSW": {}, "BinaryMSTG": {}
 })";
 

@@ -2,7 +2,7 @@
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
 workload; results are pasted into DESIGN.md section 7.
-Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows] [filtered] [aq] [graph]"""
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows] [filtered] [aq] [graph] [mstg_graph]"""
 import json
 import os
 import subprocess
@@ -867,9 +867,79 @@ def bench_graph():
         ix.close()
 
 
+def bench_mstg_graph():
+    """MSTG graph search (graph_degree=32): the walk over the bf16 list rows, then the exact re-rank of k x refine_factor = 40
+    rows from HBM (keep_raw=1) or from pinned host memory over PCIe (keep_raw=2), against the HNSWFLAT graph and MSTG's own
+    lists (graph=0) on the same data: the graph mode's generator (768-d, 10 000 centres, spreads 0.3 and 1.0).  Rows from
+    MSTG_GRAPH_ROWS (default "500000,2000000"; the larger shape runs keep_raw=2 only, the configuration whose HBM it is meant
+    to fit), spreads from MSTG_GRAPH_SPREADS (default "0.3,1.0").  Per index: build phases, memory_bytes / host_memory_bytes; per ef_s: recall@10 at nq = 1024, QPS at batch 1024,
+    the nq = 1 call (median, p10-p90), rows scored per query, and the walk / gather / re-rank kernels' CUDA times per batch
+    (torch.profiler, a separate call)."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    d, k, D = 768, 10, 32
+    ctx = gpu_context()
+
+    def calls(fn, reps):
+        fn()
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            out = fn()
+            ts.append(time.perf_counter() - t0)
+        return np.array(ts), out
+
+    def kernel_ms(fn):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        out = {}
+        for e in prof.key_averages():
+            for name in ("graph_search_bf16_kernel", "graph_search_kernel", "gather_host_rows_kernel", "refine_kernel"):
+                if name in e.key and not (name == "graph_search_kernel" and "bf16" in e.key):
+                    out[name] = round(out.get(name, 0.0) + getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / 1e3, 3)
+        return out
+
+    for n in [int(v) for v in os.environ.get("MSTG_GRAPH_ROWS", "500000,2000000").split(",")]:
+        for spread in [float(v) for v in os.environ.get("MSTG_GRAPH_SPREADS", "0.3,1.0").split(",")]:
+            y, qs = clustered(n, d, 10_000, seed=768, spread=spread, nq=1024)
+            flat = b2.Corpus(b2.L2, d).append(y)
+            _, truth = flat.search(qs, k)
+            flat.close()
+            kinds = [("MSTG", 2), ("MSTG", 1), ("HNSWFLAT", 1)] if n <= 500_000 else [("MSTG", 2)]
+            for kind, keep_raw in kinds:
+                t0 = time.perf_counter()
+                ix = b2.VectorIndex(kind, b2.L2, d, f"graph_degree={D},keep_raw={keep_raw}").build(y)
+                build_s = time.perf_counter() - t0
+                ph = ix.phase_ms()
+                tag = f"{kind} keep_raw={keep_raw} {n} x {d} spread {spread}"
+                print(json.dumps(dict(workload=tag, D=D, **ctx, build_s=round(build_s, 2), graph_candidates_s=round(ph["coarse"] / 1e3, 2),
+                                      graph_prune_s=round(ph["plan"] / 1e3, 3), graph_merge_s=round(ph["scan"] / 1e3, 3),
+                                      memory_bytes=ix.memory_bytes(), host_memory_bytes=ix.host_memory_bytes(), nlist=ix.info()["nlist"])), flush=True)
+                for ef in (32, 64, 128, 256):
+                    prm = f"ef_s={ef}"
+                    tb, (_, ids) = calls(lambda: ix.search(qs, k, prm), 5)
+                    rows = ix.last_scan()["rows_streamed"] / len(qs)
+                    t1, _ = calls(lambda: ix.search(qs[:1], k, prm), 50)
+                    print(json.dumps(dict(workload=tag, ef_s=ef, recall=round(recall(ids, truth), 4), qps_1024=round(len(qs) / np.median(tb), 1),
+                                          nq1_ms_median=round(1e3 * np.median(t1), 3),
+                                          nq1_ms_p10_p90=[round(1e3 * np.percentile(t1, 10), 3), round(1e3 * np.percentile(t1, 90), 3)],
+                                          rows_scored_per_query=round(rows, 1), kernel_ms_per_batch=kernel_ms(lambda: ix.search(qs, k, prm)))), flush=True)
+                if kind == "MSTG" and keep_raw == 1:
+                    for nprobe in (8, 16, 32, 64, 128):
+                        prm = f"graph=0,nprobe={nprobe}"
+                        tb, (_, ids) = calls(lambda: ix.search(qs, k, prm), 5)
+                        print(json.dumps(dict(workload=f"MSTG lists {n} x {d} spread {spread}", nprobe=nprobe, recall=round(recall(ids, truth), 4),
+                                              qps_1024=round(len(qs) / np.median(tb), 1))), flush=True)
+                ix.close()
+            del y
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
         {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
          "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide, "pq4": bench_pq4, "prefilter": bench_prefilter,
-         "host_rows": bench_host_rows, "filtered": bench_filtered, "aq": bench_aq, "graph": bench_graph}[w]()
+         "host_rows": bench_host_rows, "filtered": bench_filtered, "aq": bench_aq, "graph": bench_graph,
+         "mstg_graph": bench_mstg_graph}[w]()

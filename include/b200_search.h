@@ -269,6 +269,15 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *   b200_index_finalize()
  * b200_index_build(rows, n) does all four from one host array.  *_device variants take fp32 rows already in HBM.
  * ---------------------------------------------------------------------------------- */
+/* Widest float index with inverted lists (every float type but FLAT, which keeps no limit below the loader's 65536;
+ * binary types take up to 65536 bits): create refuses a wider d with B200_ERR_UNSUPPORTED, and so does load for a wider
+ * file.  The bound is the largest block of shared memory a search of these types needs: the graph walk over MSTG's bf16 list
+ * rows at ef_s = k = 1024 under a filter holds the query (d_pad64 floats) and 101760 bytes of lists and visited table in the
+ * 227 KB a block may use, so d_pad64 <= 32640.  Every other configuration fits wider: the fp32 graph walk (HNSWFLAT) up to
+ * d_pad 32672, the exact second stage at k = 1024 (d_pad x 4 + 73728 bytes) up to d_pad 39680; the bf16 and SQ8 list scans
+ * stream k-blocks and need no more shared memory at any width. */
+#define B200_MAX_FLOAT_DIM 32640
+
 typedef struct b200_index b200_index;
 int b200_index_create(const char *type, int metric, int d, const char *params, b200_index **out);
 int b200_index_build(b200_index *ix, const float *rows, int64_t n);
@@ -323,6 +332,9 @@ int b200_index_last_scan(b200_index *ix, int64_t *rows_streamed, int64_t *payloa
  * under filter_probe=1, nprobe on every other list search, 0 where an exact pass answered (FLAT, the small-part fallback,
  * exact_batch=1, the filter_probe exact rule).  out_exact (nullable) = 1 when the filter_probe exact rule answered. */
 int b200_index_last_probe(b200_index *ix, int32_t *out_lists, int64_t capacity, int *out_exact);
+/* coarse-probe path of the last search of a float inverted-file index (tests): 1 the FMA scan of the centroid table, 2 the
+ * tensor-core (3xTF32) path, 3 the ranking keys + select kernels, 0 none ran (every list probed, an exact pass, binary). */
+int b200_index_last_coarse(b200_index *ix, int *path);
 /* aq_threshold indexes (tests, benchmarks): eta and the training sample's mean anisotropic loss after the k-means codebooks,
  * then after each anisotropic iteration, out_loss[*out_n] (capacity >= *out_n, else B200_ERR_INVALID; null: skipped).
  * B200_ERR_INVALID for an index not trained with the key here (plain PQ, other types, an index loaded from a file). */

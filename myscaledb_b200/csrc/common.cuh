@@ -33,6 +33,9 @@ extern thread_local int64_t g_launches;
 __host__ __device__ static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 __host__ __device__ static inline int64_t round_up(int64_t a, int64_t b) { return ceil_div(a, b) * b; }
 
+// opt-in dynamic shared memory of one block on sm_90 (227 KB)
+constexpr int kSmemOptinBytes = 232448;
+
 constexpr uint32_t kNoId = 0xffffffffu;
 constexpr uint64_t kNoId64 = ~0ull;
 template <typename IdT> struct NoId;

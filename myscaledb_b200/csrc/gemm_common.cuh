@@ -19,7 +19,7 @@ constexpr int EPI_THREADS = 128;   // the consumer warpgroup: MMAs, then the top
 constexpr int NUM_THREADS = EPI_THREADS + 32;  // IVF kernel: + one TMA producer warp (warp 4)
 constexpr int SMEM_ALIGN_SLACK = 1024;
 constexpr int MAX_STAGES = 4;
-constexpr int SMEM_LIMIT = 232448;  // 227 KB of opt-in shared memory per block (sm_90)
+constexpr int SMEM_LIMIT = kSmemOptinBytes;
 
 constexpr int SCRATCH_BYTES = 32 * EPI_THREADS * 4;  // IVF kernel: epilogue slow-path scratch [32][128] floats
 // Accumulator hand-off of the IVF kernel (the flat kernel filters from the registers and stages only the groups of 32 columns that

@@ -534,6 +534,9 @@ int graph_search(const GraphSearchParams &p, int64_t nq, cudaStream_t s) {
     const bool bf16 = p.pages != nullptr;
     const size_t smem = graph_search_smem(bf16 ? p.d_pad64 : p.d_pad, p.ef, p.k, p.alive != nullptr);
     const void *fn = bf16 ? (const void *)graph_search_bf16_kernel : (const void *)graph_search_kernel;
+    if (smem > (size_t)kSmemOptinBytes)   // d <= B200_MAX_FLOAT_DIM keeps this far below the limit at ef = k = 1024 with a filter
+        return fail(B200_ERR_UNSUPPORTED, "graph search: d_pad " + std::to_string(bf16 ? p.d_pad64 : p.d_pad) + " at ef " + std::to_string(p.ef) +
+                                              " needs " + std::to_string(smem) + " bytes of shared memory, more than " + std::to_string(kSmemOptinBytes));
     B200_CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (bf16) graph_search_bf16_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
     else graph_search_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);

@@ -1288,6 +1288,7 @@ struct b200_index {
     // lists each query of the last search probed (b200_index_last_probe), and whether the filter_probe exact rule answered it
     std::vector<int32_t> last_probe;
     bool last_probe_exact = false;
+    int last_coarse = 0;   // coarse-probe path of the last float list search (b200_index_last_coarse), 0 = none
     // statistics of the last search (tests, bench roofline): rows x payload bytes the scan kernel was asked to stream
     int64_t last_scan_rows = 0, last_items = 0;
     // graph_degree=D (HNSWFLAT, MSTG): neighbour graph [n][D] u32 built at finalize, 0xFFFFFFFF = empty slot (graph_sm90.cu);
@@ -1381,6 +1382,9 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
     if (bin && !bin_metric) return fail(B200_ERR_INVALID, "binary indexes take HAMMING or JACCARD");
     if (!bin && !float_metric) return fail(B200_ERR_INVALID, "float indexes take L2, IP or COSINE");
     if (bin && (d % 8 != 0 || d > (1 << 16))) return fail(B200_ERR_INVALID, "binary dimension must be a multiple of 8 bits, at most 65536");
+    if (!bin && ty != IDX_FLAT && d > B200_MAX_FLOAT_DIM)
+        return fail(B200_ERR_UNSUPPORTED, "index type " + t + ": d must be at most B200_MAX_FLOAT_DIM = " + std::to_string(B200_MAX_FLOAT_DIM) + ", got " +
+                                              std::to_string(d));
     // PQ code width (IVFPQ, SCANN, HNSWPQ only; the other types ignore the key)
     const bool pq_type = ty == IDX_IVFPQ || ty == IDX_SCANN || ty == IDX_HNSWPQ;
     const int pq_bits = pq_type ? parse_int_param(params, "bit_size", 8) : 8;
@@ -2477,6 +2481,9 @@ static int refine_device(b200_index *ix, const float *d_q /*[nq][d_pad] prepared
     rp.cosine = ix->metric == B200_METRIC_COSINE;
     rp.id_offset = id_offset;
     const size_t smem = (size_t)ix->d_pad * 4 + (size_t)9 * k * 8;
+    if (smem > (size_t)kSmemOptinBytes)   // d <= B200_MAX_FLOAT_DIM keeps this far below the limit at k = 1024
+        return fail(B200_ERR_UNSUPPORTED, "exact second stage: d_pad " + std::to_string(ix->d_pad) + " at k " + std::to_string(k) + " needs " +
+                                              std::to_string(smem) + " bytes of shared memory, more than " + std::to_string(kSmemOptinBytes));
     if (!ix->h_rows) {
         rp.rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
         B200_CUDA_OK(cudaFuncSetAttribute(refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -3102,7 +3109,8 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         bool use_scan = nprobe > 8 && t_scan < t_gemm;
         // nprobe > 8: full ranking keys + warp select (coarse_scores_kernel / coarse_select_kernel above)
         int coarse_path = nprobe > 8 && nprobe <= 1024 ? 3 : use_scan ? 1 : 2;
-        if (const int forced = parse_int_param(params, "coarse_path", 0)) coarse_path = forced;   // A/B: 1 scan kernel, 2 tensor-core path, 3 select
+        const int forced = parse_int_param(params, "coarse_path", 0);   // A/B: 1 scan kernel, 2 tensor-core path, 3 select
+        if (forced) coarse_path = forced;
         if (coarse_path == 3) {
             const int64_t chunk = std::max<int64_t>(64, std::min<int64_t>(nq, ((int64_t)64 << 20) / std::max(1, nl)));   // <= 256 MB of keys
             B200_TRY(ix->w_cs.reserve((size_t)chunk * nl * 4));
@@ -3117,11 +3125,16 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
                 g_launches += 2;
             }
             B200_CUDA_OK(cudaGetLastError());
+            ix->last_coarse = 3;
         } else {
-            b200_corpus_set_path(ix->coarse, coarse_path == 1 ? 1 : 0);
+            // chosen 2: the corpus' own choice by batch size; forced 2: the tensor-core path whatever the batch
+            b200_corpus_set_path(ix->coarse, coarse_path == 1 ? 1 : forced == 2 ? 2 : 0);
             const int rc = b200_corpus_search_device(ix->coarse, ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s);
             b200_corpus_set_path(ix->coarse, 0);
             B200_TRY(rc);
+            int kernel = 0;
+            B200_TRY(b200_corpus_last_variant(ix->coarse, &kernel, nullptr, nullptr, nullptr));
+            ix->last_coarse = kernel == B200_KERNEL_SCAN ? 1 : 2;
         }
     }
 
@@ -3156,6 +3169,7 @@ extern "C" int b200_index_search_device(b200_index *ix, const float *d_queries, 
     cudaStream_t s = stream ? reinterpret_cast<cudaStream_t>(stream) : ix->stream;
     ix->last_probe.clear();
     ix->last_probe_exact = false;
+    ix->last_coarse = 0;
     ix->last_graph = false;
     B200_TRY(search_device_locked(ix, d_queries, nq, k, params, first_stage_only, d_alive_bits, nullptr, id_offset, d_out_dis, d_out_ids, nullptr, s));
     if (!stream) B200_CUDA_OK(cudaStreamSynchronize(s));
@@ -3175,6 +3189,7 @@ extern "C" int b200_index_search(b200_index *ix, const float *queries, int64_t n
     cudaStream_t s = ix->stream;
     ix->last_probe.clear();
     ix->last_probe_exact = false;
+    ix->last_coarse = 0;
     ix->last_graph = false;
     B200_TRY(ix->w_host_q.reserve((size_t)nq * in_row_bytes(ix)));
     B200_TRY(ix->w_cand.reserve((size_t)nq * k * 12 + 16));
@@ -3215,6 +3230,13 @@ extern "C" int b200_index_last_probe(b200_index *ix, int32_t *out_lists, int64_t
         std::copy(ix->last_probe.begin(), ix->last_probe.end(), out_lists);
     }
     if (out_exact) *out_exact = ix->last_probe_exact ? 1 : 0;
+    return B200_OK;
+}
+
+extern "C" int b200_index_last_coarse(b200_index *ix, int *path) {
+    if (!ix || !path) return fail(B200_ERR_INVALID, "bad arguments");
+    std::lock_guard<std::mutex> lk(ix->mu);
+    *path = ix->last_coarse;
     return B200_OK;
 }
 

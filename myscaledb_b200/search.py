@@ -469,6 +469,12 @@ class VectorIndex:
         _check(lib().b200_index_last_probe(self._h, _p(out, C.c_int32), C.c_int64(n), C.byref(ex)))
         return out, bool(ex.value)
 
+    def last_coarse(self):
+        """Coarse-probe path of the last search: 1 FMA scan, 2 tensor cores (3xTF32), 3 keys + select, 0 none ran."""
+        p = C.c_int()
+        _check(lib().b200_index_last_coarse(self._h, C.byref(p)))
+        return p.value
+
     def graph(self):
         """graph_degree indexes: the neighbour graph, uint32 [n][D] (0xFFFFFFFF = empty slot); None without a graph."""
         deg = C.c_int()

@@ -1,6 +1,7 @@
 """Float64 reference of a stored float inverted-file index and of its first-stage search.
 
 `read_index` decodes a B2IX v2 file written by `VectorIndex.save` (layout: `index_save_io` in csrc/ivf.cu).
+`check_build` asserts the build invariants of a stored index.
 `reference_search` ranks every row of the probed lists by the key the list scan defines for its payload, computed in
 float64 from the stored payload, with the device's roundings reproduced where they change a value (bf16 queries, bf16
 codebooks, the SQ8 query scaling, the cosine normalisation).  `compare` checks a library answer against it.
@@ -14,8 +15,24 @@ L2, IP, COSINE = 0, 1, 2
 PAYLOAD_BF16, PAYLOAD_PQ, PAYLOAD_SQ8 = 0, 1, 2
 PAGE = 256
 FLT_MAX = float(np.finfo(np.float32).max)
-# tolerance of a key: TOL_REL x the sum of the absolute values of its terms (fp32 accumulation over d)
+# tolerance of a key: TOL_REL x the sum of the absolute values of its terms (fp32 accumulation over d); bf16 / SQ8 rows
+# wider than TC_WIDE add the tensor-core truncation bound (tc_weights).  PQ decodes at most 220 dims, so never does.
 TOL_REL = 3e-5
+
+
+U = 2.0 ** -24
+TC_WIDE = 768     # widest bf16 row (d_pad64) of the narrower checks, held to TOL_REL alone
+
+
+def tc_weights(d):
+    """Per-column weights w_i of the tensor-core truncation bound (tests/flat_reference.py): a wgmma K-step adds K = 16
+    products to the fp32 accumulator after aligning them to the largest exponent and truncating, so each of the K + 1 addends
+    can lose 2 u of the step's largest magnitude, at most the sum of |t_i| over the columns added so far.  Summed over the
+    steps, the product part of a key is off by at most 2 (K + 1) u sum_i w_i |t_i|, with w_i = d_pad64 / 16 - i // 16 the
+    K-steps from the one that adds column i to the last.  The scan adds k-blocks in column order."""
+    d_pad64 = -(-d // 64) * 64
+    return (d_pad64 // 16 - np.arange(d) // 16).astype(np.float64)
+
 
 HEADER = np.dtype([("magic", "S4"), ("version", "<u4"), ("type", "<i4"), ("metric", "<i4"), ("d", "<i4"), ("nlist", "<i4"),
                    ("m", "<i4"), ("dsub", "<i4"), ("default_nprobe", "<i4"), ("refine_factor", "<i4"), ("payload", "<i4"),
@@ -160,33 +177,35 @@ def row_keys(s, Q, rows=None):
     Q = np.asarray(Q, np.float32)
     Q64 = Q.astype(np.float64)
     d = s.d
+    # rows wider than the narrower checks: + the truncation bound of the tensor-core product (tc_weights), over its terms
+    trunc = (lambda a, b: 2 * 17 * U * ((np.abs(a) * tc_weights(d)) @ np.abs(b).T)) if s.d_pad64 > TC_WIDE else (lambda a, b: 0.0)
     if s.payload == PAYLOAD_BF16:
         qt = to_bf16_values(Q).astype(np.float64)
         Y = pay[:, :d].astype(np.float64)
-        ip, aip = qt @ Y.T, np.abs(qt) @ np.abs(Y).T
+        ip, aip, w = qt @ Y.T, np.abs(qt) @ np.abs(Y).T, trunc(qt, Y)
         if s.metric == L2:
             qq, yy = (qt * qt).sum(1)[:, None], (Y * Y).sum(1)[None, :]
             key = qq + yy - 2 * ip
-            return key, np.maximum(key, 0.0), TOL_REL * (qq + yy + 2 * aip)
+            return key, np.maximum(key, 0.0), TOL_REL * (qq + yy + 2 * aip) + 2 * w
         if s.metric == IP:
-            return -ip, ip, TOL_REL * aip
-        return 1 - ip, 1 - ip, TOL_REL * (1 + aip)
+            return -ip, ip, TOL_REL * aip + w
+        return 1 - ip, 1 - ip, TOL_REL * (1 + aip) + w
     if s.payload == PAYLOAD_SQ8:
         lo, step, _, mid = (s.sq[i].astype(np.float64) for i in range(4))
         cm = pay[:, :d].astype(np.float64) - 128.0
         qs = to_bf16_values(Q * s.sq[1][None, :]).astype(np.float64)     # fp32 product, bf16 RNE (pair_fill_kernel)
-        t, at = qs @ cm.T, np.abs(qs) @ np.abs(cm).T
+        t, at, w = qs @ cm.T, np.abs(qs) @ np.abs(cm).T, trunc(qs, cm)
         qm, aqm = (Q64 @ mid)[:, None], (np.abs(Q64) @ np.abs(mid))[:, None]
         if s.metric == L2:
             v = lo[None, :] + pay[:, :d].astype(np.float64) * step[None, :]
             vv = (v * v).sum(1)[None, :]
             qq = (Q64 * Q64).sum(1)[:, None]
             key = qq - 2 * qm + vv - 2 * t
-            return key, np.maximum(key, 0.0), TOL_REL * (qq + 2 * aqm + vv + 2 * at)
+            return key, np.maximum(key, 0.0), TOL_REL * (qq + 2 * aqm + vv + 2 * at) + 2 * w
         sc = qm + t
         if s.metric == IP:
-            return -sc, sc, TOL_REL * (aqm + at)
-        return 1 - sc, 1 - sc, TOL_REL * (1 + aqm + at)
+            return -sc, sc, TOL_REL * (aqm + at) + w
+        return 1 - sc, 1 - sc, TOL_REL * (1 + aqm + at) + w
     # PQ on the residual: r^ = bf16 codebook entries, c = the row's list centroid
     R = pq_decode(s, pay).astype(np.float64)
     C = s.centroids.astype(np.float64)
@@ -213,8 +232,9 @@ def coarse_probe(s, Q, nprobe):
     distances are within tolerance, so the probe set itself is ambiguous)."""
     Q64 = np.asarray(Q, np.float64)
     C = s.centroids.astype(np.float64)
-    dist = ((Q64[:, None, :] - C[None, :, :]) ** 2).sum(2)
-    ptol = 1e-5 * ((Q64 * Q64).sum(1)[:, None] + (C * C).sum(1)[None, :] + 2 * np.abs(Q64) @ np.abs(C).T)
+    qq, cc = (Q64 * Q64).sum(1)[:, None], (C * C).sum(1)[None, :]
+    dist = qq + cc - 2 * Q64 @ C.T        # expanded: no nq x nlist x d temporary; fp64 rounding << ptol
+    ptol = 1e-5 * (qq + cc + 2 * np.abs(Q64) @ np.abs(C).T)
     order = np.argsort(dist, axis=1, kind="stable")
     npr = max(1, min(nprobe, s.nlist))
     probed = order[:, :npr]
@@ -308,3 +328,77 @@ def compare(r, dis_g, ids_g):
             if missing:
                 bad.append(f"q{q}: rows {sorted(missing)[:5]} below the k-th key are missing")
     return bad
+
+
+def check_build(s, ix, y):
+    """Build invariants of a stored float inverted-file index s (read_index) of ix built from the rows y: every row in its
+    nearest list exactly once, the stored fp32 rows, the payload (bf16 RNE, SQ codes and padding, nearest PQ codewords) and
+    row_bias."""
+    n, d = len(y), s.d
+    ids, lst, pay = s.flat()
+    assert np.array_equal(np.sort(ids), np.arange(n)), "the lists do not hold every row exactly once"
+    assert np.array_equal(s.list_len, ix.list_sizes().astype(np.int64))
+    assert s.has_raw
+    x = s.rows.astype(np.float32)
+    if s.metric == COSINE:   # rows are stored unit length; the payload is encoded from the same vectors
+        np.testing.assert_allclose(x, y / np.linalg.norm(y.astype(np.float64), axis=1, keepdims=True), rtol=0, atol=1e-6)
+    else:
+        assert np.array_equal(x, y)
+    X = x[ids].astype(np.float64)
+    C = s.centroids.astype(np.float64)
+    # ||x - c||^2 expanded (no n x nlist x d temporary at wide d): fp64 rounding stays far below the 1e-5 tolerance
+    xx, cc = (X * X).sum(1)[:, None], (C * C).sum(1)[None, :]
+    dist = xx + cc - 2 * X @ C.T
+    tol = 1e-5 * (xx + cc + 2 * np.abs(X) @ np.abs(C).T)
+    own = dist[np.arange(n), lst]
+    assert (own <= dist.min(1) + tol[np.arange(n), lst]).all(), "a row is not in its nearest list"
+    if s.payload == PAYLOAD_BF16:
+        assert np.array_equal(pay[:, :d], to_bf16_values(x[ids])), "bf16 payload is not RNE of the row"
+        assert (pay[:, d:] == 0).all()
+        Y = pay[:, :d].astype(np.float64)
+        bias, S = (Y * Y).sum(1), (Y * Y).sum(1)
+    elif s.payload == PAYLOAD_SQ8:
+        lo, step, inv = s.sq[0], s.sq[1], s.sq[2]
+        want = np.clip(np.rint((x[ids] - lo) * inv), 0, 255)                     # the device's fp32 arithmetic
+        got = pay[:, :d].astype(np.float64)
+        t = (X - lo.astype(np.float64)) * inv.astype(np.float64)
+        near_half = np.abs(t - np.floor(t) - 0.5) < 1e-5 * np.maximum(1.0, np.abs(t))
+        assert ((got == want) | ((np.abs(got - want) == 1) & near_half)).all(), "SQ codes differ from rint((x - lo) / step)"
+        assert (pay[:, d:] == 128).all(), "SQ padding bytes must decode to 0"
+        v = lo.astype(np.float64) + got * step.astype(np.float64)
+        bias, S = (v * v).sum(1), (v * v).sum(1)
+    else:
+        res = X - C[lst]
+        cb = s.codebook.astype(np.float64)
+        for j in range(s.m):
+            r = res[:, j * s.dsub:(j + 1) * s.dsub]
+            dd = ((r[:, None, :] - cb[j][None, :, :]) ** 2).sum(2)
+            got = dd[np.arange(n), pay[:, j]]
+            assert (got <= dd.min(1) + 1e-5 * ((r * r).sum(1) + (cb[j] ** 2).sum(1).max()) + 1e-12).all(), f"PQ code {j} is not the nearest codeword"
+        assert (pay[:, s.m:] == 0).all(), "PQ padding bytes must be 0"
+        Rh = pq_decode(s, pay).astype(np.float64)
+        bias = (Rh * (Rh + 2 * C[lst])).sum(1)
+        S = (np.abs(Rh) * np.abs(Rh + 2 * C[lst])).sum(1)
+    if s.metric == L2:
+        b = np.concatenate(s.bias).astype(np.float64)
+        assert (np.abs(b - bias) <= TOL_REL * S + 1e-30).all(), "row_bias differs from its formula"
+    else:
+        assert all(a is None for a in s.bias)
+
+
+def rerank(rows, q, cand, k, metric):
+    """Exact second stage: candidates [nq][kc] (-1 = none) of the prepared queries q against the stored fp32 rows -> the top k
+    by (fp32 key, id), (dis float32 [nq][k], ids int64 [nq][k]).  The key is the float64 value rounded once to fp32: the
+    library's key wherever its fp32 sum is exact (small integers), else within its rounding (see the callers' bounds)."""
+    nq = len(q)
+    empty = -FLT_MAX if metric == IP else FLT_MAX
+    dis = np.full((nq, k), empty, np.float32)
+    ids = np.full((nq, k), -1, np.int64)
+    for i in range(nq):
+        c = cand[i][cand[i] >= 0]
+        yy, qq = rows[c].astype(np.float64), np.asarray(q[i], np.float64)
+        key = (((yy - qq) ** 2).sum(1) if metric == L2 else -(yy @ qq)).astype(np.float32)
+        order = np.lexsort((c, key))[:k]
+        ids[i, :len(order)] = c[order]
+        dis[i, :len(order)] = key[order] if metric == L2 else (-key[order] if metric == IP else 1 - (-key[order]))
+    return dis, ids

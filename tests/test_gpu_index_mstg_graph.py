@@ -12,6 +12,7 @@ import oracle as orc
 from myscaledb_b200.search import B200Error
 from oracle import pack_bits
 from tests import graph_reference as G
+from tests import ivf_reference as R
 from tests.util import check_topk, to_bf16_values
 
 pytestmark = pytest.mark.gpu
@@ -54,21 +55,6 @@ def _check_graph(ix, y, D):
     assert np.array_equal(got, want), f"{int((got != want).any(1).sum())} of {len(y)} graph rows differ from the reference"
 
 
-def _rerank(y, q, cand, k, metric):
-    """exact second stage of the reference: candidates [nq][kc] (-1 = none) -> top k by (fp32 distance, id)"""
-    nq = len(q)
-    dis = np.full((nq, k), -np.finfo(F32).max if metric == b2.IP else np.finfo(F32).max, F32)
-    ids = np.full((nq, k), -1, np.int64)
-    for i in range(nq):
-        c = cand[i][cand[i] >= 0]
-        yy, qq = y[c].astype(np.float64), q[i].astype(np.float64)
-        key = (((yy - qq) ** 2).sum(1) if metric == b2.L2 else -(yy @ qq)).astype(F32)
-        order = np.lexsort((c, key))[:k]
-        ids[i, :len(order)] = c[order]
-        dis[i, :len(order)] = key[order] if metric == b2.L2 else -key[order]
-    return dis, ids
-
-
 @pytest.mark.parametrize("metric", [b2.L2, b2.IP])
 @pytest.mark.parametrize("D", [16, 32])
 def test_graph_is_the_reference(metric, D):
@@ -109,7 +95,7 @@ def test_search_is_the_reference(d, metric, filtered):
         seeds = ix.last_seeds()
         assert seeds is not None and seeds.shape == (len(q), min(max(ef, kc), G.MAX_SEEDS))
         _, wi, scored = G.search(g, y, q, seeds, max(ef, kc), kc, G.iteration_cap(D), _metric_name(metric), alive)
-        rd, ri = _rerank(y, q, wi, k, metric)
+        rd, ri = R.rerank(y, q, wi, k, metric)
         assert np.array_equal(ids, ri), f"ef_s={ef}: ids differ from the reference"
         assert dis.tobytes() == rd.tobytes(), f"ef_s={ef}: distances differ from the reference"
         assert ix.last_scan()["rows_streamed"] == int(scored.sum())

@@ -206,20 +206,6 @@ def test_coarse_kmeans_tensor_core_assignment(tmp_path):
 # ---------------------------------------------------------------------------------------------------------------------------
 # SQ8 ranges, bit for bit
 # ---------------------------------------------------------------------------------------------------------------------------
-def _sq_problems(got, want_rows):
-    want = T.sq_ranges(want_rows)
-    fused = T.sq_ranges(want_rows, fused_mid=True)
-    bad = []
-    for i, name in enumerate(("lo", "step", "1/step", "mid")):
-        ok = got[i] == want[i]
-        if i == 3:
-            ok |= got[i] == fused[i]
-        if not ok.all():
-            j = int(np.argmin(ok))
-            bad.append(f"{name}[{j}]: device {got[i][j]!r}, reference {want[i][j]!r}")
-    return bad
-
-
 def sq_rows(rng, n, d, nl):
     y, _ = separated(rng, n, d, nl)
     y[:, 3] = -2.5            # a constant column: step 1
@@ -237,14 +223,14 @@ def test_sq_ranges_bit_for_bit(metric, tmp_path):
     ix.reserve(n).train(y).add(y).finalize()
     s = _stored(ix, tmp_path / "ix.b2ix")
     x = T.train_rows(y, metric)
-    assert not _sq_problems(s.sq, x), _sq_problems(s.sq, x)
+    assert not T.sq_problems(s.sq, x), T.sq_problems(s.sq, x)
     if metric != b2.COSINE:
         assert s.sq[1][3] == 1 and s.sq[1][5] == 1 and (s.sq[0][6] < 0) and (s.sq[3][6] < 0)
     _match(s.centroids, T.kmeans(x, nl, 10), "IVFSQ centroids")
     # negative control: one ulp off in one step
     got = s.sq.copy()
     got[1][0] = np.nextafter(got[1][0], F32(np.inf))
-    assert _sq_problems(got, x), "negative control: a step one ulp off is accepted"
+    assert T.sq_problems(got, x), "negative control: a step one ulp off is accepted"
 
 
 def test_sq_ranges_of_build_sample(tmp_path):
@@ -255,8 +241,8 @@ def test_sq_ranges_of_build_sample(tmp_path):
     y[out[:5], 0] = 1e3       # extremes build() does not train on
     y[out[5:9], 1] = -1e3
     s = _stored(b2.VectorIndex("IVFSQ", b2.L2, d, f"ncentroids={nl}").build(y), tmp_path / "ix.b2ix")
-    assert not _sq_problems(s.sq, T.build_sample(y, nl)), _sq_problems(s.sq, T.build_sample(y, nl))
-    assert _sq_problems(s.sq, y), "negative control: the ranges of every row are accepted"
+    assert not T.sq_problems(s.sq, T.build_sample(y, nl)), T.sq_problems(s.sq, T.build_sample(y, nl))
+    assert T.sq_problems(s.sq, y), "negative control: the ranges of every row are accepted"
 
 
 # ---------------------------------------------------------------------------------------------------------------------------

@@ -83,64 +83,13 @@ def cache(tmp_path_factory):
 # ---------------------------------------------------------------------------------------------------------------------------
 # a. build invariants
 # ---------------------------------------------------------------------------------------------------------------------------
-def _check_build(s, ix, y):
-    n, d = len(y), s.d
-    ids, lst, pay = s.flat()
-    assert np.array_equal(np.sort(ids), np.arange(n)), "the lists do not hold every row exactly once"
-    assert np.array_equal(s.list_len, ix.list_sizes().astype(np.int64))
-    assert s.has_raw
-    x = s.rows.astype(F32)
-    if s.metric == R.COSINE:   # rows are stored unit length; the payload is encoded from the same vectors
-        np.testing.assert_allclose(x, y / np.linalg.norm(y.astype(np.float64), axis=1, keepdims=True), rtol=0, atol=1e-6)
-    else:
-        assert np.array_equal(x, y)
-    X = x[ids].astype(np.float64)
-    C = s.centroids.astype(np.float64)
-    dist = ((X[:, None, :] - C[None, :, :]) ** 2).sum(2)
-    tol = 1e-5 * ((X * X).sum(1)[:, None] + (C * C).sum(1)[None, :] + 2 * np.abs(X) @ np.abs(C).T)
-    own = dist[np.arange(n), lst]
-    assert (own <= dist.min(1) + tol[np.arange(n), lst]).all(), "a row is not in its nearest list"
-    if s.payload == R.PAYLOAD_BF16:
-        assert np.array_equal(pay[:, :d], to_bf16_values(x[ids])), "bf16 payload is not RNE of the row"
-        assert (pay[:, d:] == 0).all()
-        Y = pay[:, :d].astype(np.float64)
-        bias, S = (Y * Y).sum(1), (Y * Y).sum(1)
-    elif s.payload == R.PAYLOAD_SQ8:
-        lo, step, inv = s.sq[0], s.sq[1], s.sq[2]
-        want = np.clip(np.rint((x[ids] - lo) * inv), 0, 255)                     # the device's fp32 arithmetic
-        got = pay[:, :d].astype(np.float64)
-        t = (X - lo.astype(np.float64)) * inv.astype(np.float64)
-        near_half = np.abs(t - np.floor(t) - 0.5) < 1e-5 * np.maximum(1.0, np.abs(t))
-        assert ((got == want) | ((np.abs(got - want) == 1) & near_half)).all(), "SQ codes differ from rint((x - lo) / step)"
-        assert (pay[:, d:] == 128).all(), "SQ padding bytes must decode to 0"
-        v = lo.astype(np.float64) + got * step.astype(np.float64)
-        bias, S = (v * v).sum(1), (v * v).sum(1)
-    else:
-        res = X - C[lst]
-        cb = s.codebook.astype(np.float64)
-        for j in range(s.m):
-            r = res[:, j * s.dsub:(j + 1) * s.dsub]
-            dd = ((r[:, None, :] - cb[j][None, :, :]) ** 2).sum(2)
-            got = dd[np.arange(n), pay[:, j]]
-            assert (got <= dd.min(1) + 1e-5 * ((r * r).sum(1) + (cb[j] ** 2).sum(1).max()) + 1e-12).all(), f"PQ code {j} is not the nearest codeword"
-        assert (pay[:, s.m:] == 0).all(), "PQ padding bytes must be 0"
-        Rh = R.pq_decode(s, pay).astype(np.float64)
-        bias = (Rh * (Rh + 2 * C[lst])).sum(1)
-        S = (np.abs(Rh) * np.abs(Rh + 2 * C[lst])).sum(1)
-    if s.metric == R.L2:
-        b = np.concatenate(s.bias).astype(np.float64)
-        assert (np.abs(b - bias) <= R.TOL_REL * S + 1e-30).all(), "row_bias differs from its formula"
-    else:
-        assert all(a is None for a in s.bias)
-
-
 @pytest.mark.parametrize("payload", ["bf16", "sq8", "pq2"])
 @pytest.mark.parametrize("metric", METRICS)
 def test_build_invariants_one_shot_and_streamed(payload, metric, tmp_path):
     d = 100
     y, _ = _data(N, d, seed=7 + metric)
     a = b2.VectorIndex(PAYLOADS[payload][0], metric, d, _params(payload, d)).build(y)
-    _check_build(_saved(a, tmp_path / "a.b2ix"), a, y)
+    R.check_build(_saved(a, tmp_path / "a.b2ix"), a, y)
     # streamed: chunks of 1, 255, 257 and 1000 rows split list tails across add() calls
     b = b2.VectorIndex(PAYLOADS[payload][0], metric, d, _params(payload, d)).reserve(N).train(y)
     off, sizes = 0, [1, 255, 257, 1000]
@@ -150,7 +99,7 @@ def test_build_invariants_one_shot_and_streamed(payload, metric, tmp_path):
         b.add(y[off:off + sizes[i % 4]])
         off += sizes[i % 4]
     b.finalize()
-    _check_build(_saved(b, tmp_path / "b.b2ix"), b, y)
+    R.check_build(_saved(b, tmp_path / "b.b2ix"), b, y)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------

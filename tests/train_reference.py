@@ -218,6 +218,22 @@ def sq_ranges(x, fused_mid=False):
     return np.stack([lo, step, inv, mid])
 
 
+def sq_problems(got, want_rows):
+    """Differences of a stored SQ8 range table got [4][d] (lo, step, 1 / step, mid) from the reference of the rows, bit for
+    bit (mid may also be the fused form)."""
+    want = sq_ranges(want_rows)
+    fused = sq_ranges(want_rows, fused_mid=True)
+    bad = []
+    for i, name in enumerate(("lo", "step", "1/step", "mid")):
+        ok = got[i] == want[i]
+        if i == 3:
+            ok |= got[i] == fused[i]
+        if not ok.all():
+            j = int(np.argmin(ok))
+            bad.append(f"{name}[{j}]: device {got[i][j]!r}, reference {want[i][j]!r}")
+    return bad
+
+
 def pq_sample(x, stride_rule="first"):
     """The PQ training sample: the first ns = min(n, 65536) rows of the view strided by max(1, n // ns).  stride_rule="even"
     takes rows floor(i n / ns) instead (a perturbation for negative controls)."""

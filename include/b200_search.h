@@ -268,6 +268,30 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *   b200_index_add(chunk) ...       -- any number of chunks, row ids continue from the rows already added
  *   b200_index_finalize()
  * b200_index_build(rows, n) does all four from one host array.  *_device variants take fp32 rows already in HBM.
+ *
+ * Unusable rows and queries (float indexes; a ClickHouse Float32 column can hold NaN and inf).  A row or query is unusable
+ * when the fp32 sum of the squares of its coordinates is not finite: a NaN or infinite coordinate, or one whose square
+ * overflows (about 1e19 and up).  One device helper (warp_row_usable) decides it for training and add alike.
+ *   Training: the coarse k-means, the SQ ranges, the PQ codebooks and the anisotropic iterations use only the usable rows of
+ *     the sample, in their order, judged as given (before the cosine normalisation); the FLAT fallback below counts only
+ *     those rows.  This holds for train, train_device and build's strided sample.
+ *   Add: an unusable row keeps its row id (info's n counts it) and its fp32 row under keep_raw 1 and 2, but goes to no list,
+ *     nor does a row for which the centroid search finds no list: the list sizes add up to the rows that are in a list.
+ *   Search: the list scans, the exact second stage and both graph walks never return a row that is in no list;
+ *     filter_probe's promise is min(k, kept rows that are in a list).  The exact paths (FLAT, the small-part fallback,
+ *     exact_batch=1, the filter_probe exact rule) keep the FLAT rule instead: a row whose distance is not finite is never
+ *     returned and never displaces a finite one (under IP, a row with an infinite coordinate is outside that rule).  They
+ *     judge the distance, not the row, so they CAN return an unusable row whose distance is finite: one whose square
+ *     overflows is a zero row after the cosine normalisation (distance 1), and under IP its inner product is finite (and
+ *     may rank first).  Where the filter_probe exact rule answers, its promise is FLAT's: min(k, kept rows with a finite
+ *     distance).
+ *   Queries: one with a NaN coordinate returns no rows on every path and metric; one with an infinite coordinate returns no
+ *     rows under L2 and cosine (under IP it is outside the contract, as for FLAT).  A non-finite query never changes the
+ *     answer of another query of the batch.
+ *   Cosine: rows and queries whose sum of squares is below FLT_EPSILON are usable and stay as given (no normalisation); their
+ *     key is 1 - <q, x>.
+ *   Files: the format is unchanged; the list lengths may add up to less than n (load refuses more than n).  A row in no list
+ *     has an empty adjacency row in a v4 graph, and load refuses an MSTG graph edge to such a row.
  * ---------------------------------------------------------------------------------- */
 /* Widest float index with inverted lists (every float type but FLAT, which keeps no limit below the loader's 65536;
  * binary types take up to 65536 bits): create refuses a wider d with B200_ERR_UNSUPPORTED, and so does load for a wider
@@ -361,7 +385,7 @@ int b200_index_last_seeds(b200_index *ix, int64_t *out, int64_t capacity, int *o
  * memory writes the header's has_raw as 2 (every other byte as in HBM placement) and loads them straight into pinned host
  * memory again.  An index with a graph (graph_degree) is written as v4: the v2 layout with the reserved word holding D,
  * followed by the graph [n][D] u32 (HNSWFLAT with has_raw 1, MSTG with has_raw 0, 1 or 2); load checks every graph id
- * (< n or 0xFFFFFFFF) before any kernel reads it. */
+ * (< n or 0xFFFFFFFF; MSTG: a row that is in a list) before any kernel reads it. */
 int b200_index_save(b200_index *ix, const char *path);
 int b200_index_load(const char *path, b200_index **out);
 /* the same through the host's own streams (Search::IndexDataFileWriter / Reader over ClickHouse disks,

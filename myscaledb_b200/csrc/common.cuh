@@ -62,6 +62,17 @@ __device__ __forceinline__ int warp_sum(int v) {
     return v;
 }
 
+// The one rule for an unusable row or query (include/b200_search.h, "Unusable rows"): the fp32 sum of the squares of its d
+// coordinates is not finite (a NaN or infinite coordinate, or one whose square overflows).  Every lane of the warp calls it
+// and gets the answer.
+__device__ __forceinline__ bool warp_row_usable(const float *x, int d) {
+    float s = 0.f;
+    for (int j = lane_id(); j < d; j += 32) s = fmaf(x[j], x[j], s);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    return isfinite(s);
+}
+
 // Warp-cooperative sorted top-k list living in shared (or global) memory.
 // keys/ids: k slots, sorted best-first, `n` valid.  All 32 lanes call with the same
 // (key,id); n/thr are warp-uniform registers.

@@ -26,17 +26,20 @@ __host__ __device__ constexpr int graph_iteration_cap(int degree) {
 inline bool graph_degree_ok(int d) { return d == 16 || d == 32 || d == 64; }
 
 // ids [m][K + 1] of the list search of rows row0 .. row0 + m - 1 (negative = none) -> cand [m][K] u32: the row's own id
-// dropped (or, when it is absent, the last entry), negative ids as 0xFFFFFFFF
-int graph_candidates(const int64_t *d_ids, int64_t m, int64_t row0, int K, uint32_t *d_cand, cudaStream_t s);
+// dropped (or, when it is absent, the last entry), negative ids as 0xFFFFFFFF.  A row in no list (row_slot 0xFFFFFFFF) gets
+// none, so no edge leaves it; the list searches never return it, so none reaches it.
+int graph_candidates(const int64_t *d_ids, const uint32_t *d_row_slot, int64_t m, int64_t row0, int K, uint32_t *d_cand, cudaStream_t s);
 // rank-based pruning (CAGRA): cand [n][2D] -> pruned [n][D], per node the D candidates with the smallest (detour count, rank)
 int graph_prune(const uint32_t *d_cand, int64_t n, int D, uint32_t *d_pruned, cudaStream_t s);
 // reverse edges and merge: pruned [n][D] -> graph [n][D].  Allocates and frees its own scratch (2 x n x D x 12 B + the sort's).
 int graph_merge(const uint32_t *d_pruned, int64_t n, int D, uint32_t *d_graph, cudaStream_t s);
 
-// id -> pool slot map row_slot[n] of a finalized bf16 inverted-file index, from its page chains (one CTA per list)
+// id -> pool slot map row_slot[n] of a finalized inverted-file index, from its page chains (one CTA per list); the caller fills
+// it with 0xFFFFFFFF first, which stays the slot of a row in no list
 int graph_row_slots(const uint32_t *d_list_len, const uint32_t *d_list_page_off, const uint32_t *d_list_pages, const uint32_t *d_row_ids, int nlist,
                     uint32_t *d_row_slot, cudaStream_t s);
-// out [m][d] fp32 = the bf16 page rows of ids row0 .. row0 + m - 1 (pool: [page][d_pad64 / 64][256][64] bf16)
+// out [m][d] fp32 = the bf16 page rows of ids row0 .. row0 + m - 1 (pool: [page][d_pad64 / 64][256][64] bf16); zeros for a row
+// in no list
 int graph_page_rows(const void *d_pool, const uint32_t *d_row_slot, int64_t row0, int64_t m, int d, int d_pad64, float *d_out, cudaStream_t s);
 
 struct GraphSearchParams {

@@ -12,26 +12,31 @@ namespace b200 {
 // ------------------------------------------------------------------------------------
 // build
 // ------------------------------------------------------------------------------------
-__global__ void graph_candidates_kernel(const int64_t *__restrict__ ids, int64_t m, int64_t row0, int K, uint32_t *__restrict__ cand) {
+__global__ void graph_candidates_kernel(const int64_t *__restrict__ ids, const uint32_t *__restrict__ row_slot, int64_t m, int64_t row0, int K,
+                                        uint32_t *__restrict__ cand) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
     const int64_t *row = ids + i * (K + 1);
+    uint32_t *out = cand + i * K;
+    if (row_slot[row0 + i] == kNoId) {
+        for (int j = 0; j < K; j++) out[j] = kNoId;
+        return;
+    }
     int self = K;   // absent (duplicate rows): drop the last entry
     for (int j = 0; j < K + 1; j++)
         if (row[j] == row0 + i) {
             self = j;
             break;
         }
-    uint32_t *out = cand + i * K;
     for (int j = 0, o = 0; j < K + 1; j++) {
         if (j == self) continue;
         out[o++] = row[j] >= 0 ? (uint32_t)row[j] : kNoId;
     }
 }
 
-int graph_candidates(const int64_t *d_ids, int64_t m, int64_t row0, int K, uint32_t *d_cand, cudaStream_t s) {
+int graph_candidates(const int64_t *d_ids, const uint32_t *d_row_slot, int64_t m, int64_t row0, int K, uint32_t *d_cand, cudaStream_t s) {
     if (m == 0) return B200_OK;
-    graph_candidates_kernel<<<(unsigned)ceil_div(m, 256), 256, 0, s>>>(d_ids, m, row0, K, d_cand);
+    graph_candidates_kernel<<<(unsigned)ceil_div(m, 256), 256, 0, s>>>(d_ids, d_row_slot, m, row0, K, d_cand);
     g_launches++;
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;
@@ -184,7 +189,8 @@ int graph_merge(const uint32_t *d_pruned, int64_t n, int D, uint32_t *d_graph, c
 }
 
 // One CTA per list walks its page chain, thread t on row t of every page (as list_alive_kernel in ivf.cu): the list's valid
-// rows record their pool slot under their id.  Slots past the list's length are never read.
+// rows record their pool slot under their id.  Slots past the list's length are never read; a row in no list keeps the
+// caller's 0xFFFFFFFF.
 __global__ void __launch_bounds__(kPageRows) row_slot_kernel(const uint32_t *__restrict__ list_len, const uint32_t *__restrict__ list_page_off,
                                                              const uint32_t *__restrict__ list_pages, const uint32_t *__restrict__ row_ids,
                                                              uint32_t *__restrict__ row_slot) {
@@ -214,7 +220,7 @@ __global__ void page_rows_kernel(const __nv_bfloat16 *__restrict__ pool, const u
     const int64_t i = e / d;
     const int j = (int)(e - i * d);
     const uint32_t slot = row_slot[row0 + i];
-    out[e] = __bfloat162float(pool[(((size_t)(slot / kPageRows) * (d_pad64 / 64) + j / 64) * kPageRows + slot % kPageRows) * 64 + j % 64]);
+    out[e] = slot == kNoId ? 0.f : __bfloat162float(pool[(((size_t)(slot / kPageRows) * (d_pad64 / 64) + j / 64) * kPageRows + slot % kPageRows) * 64 + j % 64]);
 }
 
 int graph_page_rows(const void *d_pool, const uint32_t *d_row_slot, int64_t row0, int64_t m, int d, int d_pad64, float *d_out, cudaStream_t s) {

@@ -200,12 +200,25 @@ static inline int gridsz(int64_t work, int threads = 256) {
 // ------------------------------------------------------------------------------------
 // build: chunk -> paged lists
 // ------------------------------------------------------------------------------------
-__global__ void assign_to_u32_kernel(const int64_t *ids, int64_t n, uint32_t *out, uint32_t *cnt) {
+// nearest centroid ids -> u32 lists and per-list counts.  A row without one (id -1: no finite distance to any centroid) or
+// flagged unusable gets `none`: 0 for the k-means of usable training rows, nlist for added rows (in no list; counted in
+// cnt[nlist]).
+__global__ void assign_to_u32_kernel(const int64_t *ids, int64_t n, const uint8_t *usable, uint32_t none, uint32_t *out, uint32_t *cnt) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const uint32_t l = ids[i] < 0 ? 0u : (uint32_t)ids[i];
+    const uint32_t l = ids[i] < 0 || (usable && !usable[i]) ? none : (uint32_t)ids[i];
     out[i] = l;
     atomicAdd(&cnt[l], 1u);
+}
+
+// usable[r] = 1 when row r of x [n][d] is usable (warp_row_usable), else 0; one warp per row
+__global__ void __launch_bounds__(256) row_usable_kernel(const float *x, int64_t n, int d, uint8_t *usable) {
+    const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = warp_global; r < n; r += nwarps) {
+        const bool ok = warp_row_usable(x + r * d, d);
+        if (lane_id() == 0) usable[r] = ok ? 1 : 0;
+    }
 }
 
 // Exclusive scan of per-thread partial sums across one 1024-thread CTA.
@@ -1280,6 +1293,8 @@ struct b200_index {
     DevArr w_rows, w_assign_i, w_assign_d, w_u32a, w_u32b, w_u32c, w_u32d, w_cnt, w_plan, w_sort, w_q, w_qraw, w_probe, w_pd, w_items,
         w_qbuf, w_inv, w_ppb, w_pconst, w_qconst, w_qb, w_cs, w_pk, w_pi, w_pw, w_lk, w_li, w_alive, w_od, w_oi, w_cand, w_host_q, w_ppopc, w_lut,
         w_stage;
+    // build: one flag per row of the chunk or training sample, 1 = usable (row_usable_kernel)
+    DevArr w_usable;
     // filter_probe=1 (per search): list_alive and the filtered lengths [2][nlist], the filtered page table [pages_used], the
     // per-query selection (p_q, cut key, cut ties, then the Σ / max totals); pinned host copy of the totals and of every p_q
     DevArr w_flist, w_fpages, w_fsel;
@@ -1482,7 +1497,7 @@ extern "C" int b200_index_free(b200_index *ix) {
                       &ix->w_sort, &ix->w_q, &ix->w_qraw, &ix->w_probe, &ix->w_pd, &ix->w_items, &ix->w_qbuf, &ix->w_inv, &ix->w_ppb, &ix->w_pconst, &ix->w_qb, &ix->w_cs,
                       &ix->w_qconst, &ix->w_pk, &ix->w_pi, &ix->w_pw, &ix->w_lk, &ix->w_li, &ix->w_alive, &ix->w_od, &ix->w_oi, &ix->w_cand,
                       &ix->w_host_q, &ix->w_ppopc, &ix->w_lut, &ix->w_stage, &ix->w_flist, &ix->w_fpages, &ix->w_fsel,
-                      &ix->w_seeds, &ix->w_seedd})
+                      &ix->w_seeds, &ix->w_seedd, &ix->w_usable})
         a->release();
     if (ix->h_fsel) cudaFreeHost(ix->h_fsel);
     if (ix->ev0) cudaEventDestroy(ix->ev0);
@@ -1579,7 +1594,7 @@ static int kmeans_device(const float *x, int64_t n, int64_t stride, int d, int n
             if (rc == B200_OK) rc = b200_corpus_search_device(table, x, n, 1, nullptr, 0, d_dis, d_idx64, s);
             if (rc != B200_OK) break;
             B200_CUDA_OK(cudaMemsetAsync(d_cnt, 0, (size_t)nc * 4, s));
-            assign_to_u32_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(d_idx64, n, d_idx, d_cnt);
+            assign_to_u32_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(d_idx64, n, nullptr, 0u, d_idx, d_cnt);
             g_launches++;
         } else {
             rows_sqnorm_kernel<<<(unsigned)ceil_div(nc, 256), 256, 0, s>>>(d_c, nc, d, d_cn);
@@ -1709,7 +1724,7 @@ static int kmajority_device(const uint8_t *x, int64_t n, int stride, int rb, int
         if (rc != B200_OK) break;
         B200_CUDA_OK(cudaMemsetAsync(d_cnt, 0, (size_t)nc * 4, s));
         B200_CUDA_OK(cudaMemsetAsync(d_changed, 0, 4, s));
-        assign_to_u32_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(d_idx64, n, d_idx, d_cnt);
+        assign_to_u32_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(d_idx64, n, nullptr, 0u, d_idx, d_cnt);
         count_changes_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(d_idx, d_prev, n, d_changed);
         g_launches += 2;
         uint32_t changed = 0;
@@ -1823,6 +1838,32 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
     if (ix->binary) return train_binary_locked(ix, d_rows, n);
     cudaStream_t s = ix->stream;
     const int d = ix->d;
+    // only the usable rows of the sample train, in their order and as given (before the cosine normalisation, which would
+    // turn a row whose square overflows into a zero row); a sample without an unusable row is used in place
+    const float *x = d_rows;
+    if (n > 0) {
+        B200_TRY(ix->w_usable.reserve((size_t)n));
+        B200_TRY(ix->w_assign_i.reserve((size_t)(n + 1) * 8));
+        uint8_t *usable = ix->w_usable.as<uint8_t>();
+        int64_t *pick = ix->w_assign_i.as<int64_t>(), *d_kept = pick + n;
+        row_usable_kernel<<<gridsz(n * 32), 256, 0, s>>>(d_rows, n, d, usable);
+        g_launches++;
+        size_t tb = 0;
+        const cub::CountingInputIterator<int64_t> iota(0);
+        B200_CUDA_OK(cub::DeviceSelect::Flagged(nullptr, tb, iota, usable, pick, d_kept, n, s));
+        B200_TRY(ix->w_sort.reserve(tb + 256));
+        B200_CUDA_OK(cub::DeviceSelect::Flagged(ix->w_sort.p, tb, iota, usable, pick, d_kept, n, s));
+        int64_t kept = 0;
+        B200_CUDA_OK(cudaMemcpyAsync(&kept, d_kept, 8, cudaMemcpyDeviceToHost, s));
+        B200_CUDA_OK(cudaStreamSynchronize(s));
+        if (kept < n) {
+            B200_TRY(ix->w_rows.reserve((size_t)std::max<int64_t>(kept, 1) * d * 4));
+            if (kept) gather_rows_kernel<<<gridsz(kept * d), 256, 0, s>>>(d_rows, d, pick, kept, d, ix->w_rows.as<float>());
+            g_launches++;
+            x = ix->w_rows.as<float>();
+            n = kept;
+        }
+    }
     const int64_t total = ix->reserved > 0 ? ix->reserved : n;
     decide_ivf(ix, total, n);
     if (!ix->use_ivf) {
@@ -1875,10 +1916,11 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
     if (ix->keep_raw < 0) ix->keep_raw = 1;
     const int nl = ix->nlist;
     // training rows: unit length under cosine
-    const float *x = d_rows;
     if (ix->metric == B200_METRIC_COSINE) {
-        B200_TRY(ix->w_rows.reserve((size_t)n * d * 4));
-        B200_CUDA_OK(cudaMemcpyAsync(ix->w_rows.p, d_rows, (size_t)n * d * 4, cudaMemcpyDeviceToDevice, s));
+        if (x != ix->w_rows.p) {
+            B200_TRY(ix->w_rows.reserve((size_t)n * d * 4));
+            B200_CUDA_OK(cudaMemcpyAsync(ix->w_rows.p, x, (size_t)n * d * 4, cudaMemcpyDeviceToDevice, s));
+        }
         B200_CUDA_OK(launch_normalize_rows_f32(ix->w_rows.as<float>(), d, n, s));
         x = ix->w_rows.as<float>();
     }
@@ -1930,7 +1972,7 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
         int rc = b200_corpus_search_device(ix->coarse, d_samp, ns, 1, nullptr, 0, d_ad, d_a, s);
         if (rc == B200_OK) {
             cudaMemsetAsync(d_c32, 0, (size_t)nl * 4, s);
-            assign_to_u32_kernel<<<(unsigned)ceil_div(ns, 256), 256, 0, s>>>(d_a, ns, d_l, d_c32);
+            assign_to_u32_kernel<<<(unsigned)ceil_div(ns, 256), 256, 0, s>>>(d_a, ns, nullptr, 0u, d_l, d_c32);
             g_launches++;
             for (int j = 0; j < m && rc == B200_OK; j++) {
                 residual_sub_kernel<<<gridsz(ns * dsub), 256, 0, s>>>(d_samp, ns, d, ix->d_centroids, d_l, d, j, dsub, d_res);
@@ -2022,20 +2064,30 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     B200_TRY(ix->w_u32b.reserve((size_t)n * 4));
     B200_TRY(ix->w_u32c.reserve((size_t)n * 4));
     B200_TRY(ix->w_u32d.reserve((size_t)n * 4));
-    B200_TRY(ix->w_cnt.reserve((size_t)nl * 4));
+    B200_TRY(ix->w_cnt.reserve((size_t)(nl + 1) * 4));
     B200_TRY(ix->w_plan.reserve((size_t)nl * 4 * 3));
     if (ix->binary) {
         B200_TRY(pad_bin_rows(ix, d_rows, n, ix->w_rows, s));
         x = ix->w_rows.as<float>();
     }
     B200_TRY(b200_corpus_search_device(ix->coarse, x, n, 1, nullptr, 0, ix->w_assign_d.as<float>(), ix->w_assign_i.as<int64_t>(), s));
-    B200_CUDA_OK(cudaMemsetAsync(ix->w_cnt.p, 0, (size_t)nl * 4, s));
-    assign_to_u32_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(ix->w_assign_i.as<int64_t>(), n, ix->w_u32a.as<uint32_t>(), ix->w_cnt.as<uint32_t>());
+    // unusable rows (judged as given, before the cosine normalisation) and rows without a nearest centroid get the key nlist:
+    // they sort behind every list, are counted in w_cnt[nl] and go to no list
+    const uint8_t *usable = nullptr;
+    if (!ix->binary) {
+        B200_TRY(ix->w_usable.reserve((size_t)n));
+        row_usable_kernel<<<gridsz(n * 32), 256, 0, s>>>(d_rows, n, d, ix->w_usable.as<uint8_t>());
+        g_launches++;
+        usable = ix->w_usable.as<uint8_t>();
+    }
+    B200_CUDA_OK(cudaMemsetAsync(ix->w_cnt.p, 0, (size_t)(nl + 1) * 4, s));
+    assign_to_u32_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(ix->w_assign_i.as<int64_t>(), n, usable, (uint32_t)nl, ix->w_u32a.as<uint32_t>(),
+                                                                     ix->w_cnt.as<uint32_t>());
     iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(ix->w_u32b.as<uint32_t>(), n);
     g_launches += 2;
     {
         int bits = 1;
-        while ((1 << bits) < nl) bits++;
+        while ((1 << bits) <= nl) bits++;   // keys 0 .. nlist
         size_t tmp_bytes = 0;
         cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, ix->w_u32a.as<uint32_t>(), ix->w_u32c.as<uint32_t>(), ix->w_u32b.as<uint32_t>(),
                                         ix->w_u32d.as<uint32_t>(), (int)n, 0, bits, s);
@@ -2070,7 +2122,6 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     sp.list_len = ix->d_list_len;
     sp.tail_page = ix->d_tail_page;
     sp.id_base = (uint32_t)ix->n;
-    sp.n = n;
     sp.d = d;
     sp.d_pad64 = ix->d_pad64;
     sp.l2 = ix->metric == B200_METRIC_L2;
@@ -2100,11 +2151,14 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
         sp.kb_w = ix->kb_w;
     }
     int over = 0;
+    uint32_t in_no_list = 0;
     B200_CUDA_OK(cudaMemcpyAsync(&over, ix->d_flag, 4, cudaMemcpyDeviceToHost, s));
+    B200_CUDA_OK(cudaMemcpyAsync(&in_no_list, ix->w_cnt.as<uint32_t>() + nl, 4, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
     if (over) return fail(B200_ERR_NOMEM, "page pool exhausted: more rows added than b200_index_reserve() announced");
-    if (ix->binary) scatter_bin_rows_kernel<<<gridsz(n * 32), 256, 0, s>>>(sp);
-    else scatter_rows_kernel<<<gridsz(n * 32), 256, 0, s>>>(sp);
+    sp.n = n - in_no_list;   // the list-sorted rows that go to a list; the rest sort behind them
+    if (ix->binary) scatter_bin_rows_kernel<<<gridsz(sp.n * 32), 256, 0, s>>>(sp);
+    else scatter_rows_kernel<<<gridsz(sp.n * 32), 256, 0, s>>>(sp);
     if (ix->payload == IVF_PRODUCER_PQ && ix->aq_threshold > 0) B200_TRY(aq_encode_chunk(sp, ix->aq_eta, s));   // from the nearest codes
     add_commit_kernel<<<(unsigned)ceil_div(nl, 256), 256, 0, s>>>(ix->w_cnt.as<uint32_t>(), new_base, first_new, ix->d_list_len, ix->d_tail_page, nl);
     g_launches += 2;
@@ -2164,15 +2218,21 @@ struct DevScratch {   // freed on every return path of the graph build
 };
 }  // namespace
 
-// MSTG graph: d_row_slot[n] from the page chains of the finalized (or loaded) lists
+// row_slot[n] from the page chains of the finalized (or loaded) lists; 0xFFFFFFFF for a row in no list (an unusable row, or
+// an id a loaded file repeats in place of it).  No kernel reads a pool slot through it without that check: the graph build
+// gives such rows no edges, and a load refuses an MSTG graph edge to one.
+static int fill_row_slot(const b200_index *ix, uint32_t *d_row_slot) {
+    B200_CUDA_OK(cudaMemsetAsync(d_row_slot, 0xff, (size_t)ix->n * 4, ix->stream));
+    return graph_row_slots(ix->d_list_len, ix->d_list_page_off, ix->d_list_pages, ix->d_row_ids, ix->nlist, d_row_slot, ix->stream);
+}
+
+// MSTG graph: the walk reads its bf16 list rows through d_row_slot
 static int build_row_slot(b200_index *ix) {
     if (!ix->d_row_slot && cudaMalloc(&ix->d_row_slot, std::max<size_t>((size_t)ix->n * 4, 16)) != cudaSuccess) {
         cudaGetLastError();
         return fail(B200_ERR_NOMEM, "cudaMalloc of the graph's row slot map failed");
     }
-    // a loaded file whose row ids repeat would leave ids unmapped: they read slot 0, never a slot outside the pool
-    B200_CUDA_OK(cudaMemsetAsync(ix->d_row_slot, 0, (size_t)ix->n * 4, ix->stream));
-    return graph_row_slots(ix->d_list_len, ix->d_list_page_off, ix->d_list_pages, ix->d_row_ids, ix->nlist, ix->d_row_slot, ix->stream);
+    return fill_row_slot(ix, ix->d_row_slot);
 }
 
 // graph_degree=D: every row searches the index's own lists with its defaults for k = 2D + 1.  HNSWFLAT: nprobe and the exact
@@ -2191,7 +2251,14 @@ static int build_graph_locked(b200_index *ix) {
     const int np = std::max(1, std::min(ix->default_nprobe, ix->nlist));
     const int k1 = mstg ? K + 1 : std::min(1024, (K + 1) * std::max(1, ix->refine_factor));
     const int64_t chunk = std::max<int64_t>(256, std::min<int64_t>(n, kGraphBuildSearchBytes / ((int64_t)np * k1 * 8)));
-    DevScratch cand, pruned, q, dis, ids;
+    DevScratch cand, pruned, q, dis, ids, slots;
+    // which rows are in a list: MSTG's slot map, a scratch one for HNSWFLAT
+    const uint32_t *row_slot = ix->d_row_slot;
+    if (!row_slot) {
+        B200_TRY(slots.alloc((size_t)n * 4));
+        B200_TRY(fill_row_slot(ix, static_cast<uint32_t *>(slots.p)));
+        row_slot = static_cast<const uint32_t *>(slots.p);
+    }
     B200_TRY(cand.alloc((size_t)n * K * 4));
     B200_TRY(q.alloc((size_t)chunk * d * 4));
     B200_TRY(dis.alloc((size_t)chunk * (K + 1) * 4));
@@ -2207,10 +2274,10 @@ static int build_graph_locked(b200_index *ix) {
             B200_TRY(graph_page_rows(ix->d_pool, ix->d_row_slot, off, m, d, ix->d_pad64, static_cast<float *>(q.p), s));
         B200_TRY(search_device_locked(ix, static_cast<float *>(q.p), m, K + 1, nullptr, mstg ? 1 : 0, nullptr, nullptr, 0, static_cast<float *>(dis.p),
                                       static_cast<int64_t *>(ids.p), nullptr, s));
-        B200_TRY(graph_candidates(static_cast<int64_t *>(ids.p), m, off, K, static_cast<uint32_t *>(cand.p) + off * K, s));
+        B200_TRY(graph_candidates(static_cast<int64_t *>(ids.p), row_slot, m, off, K, static_cast<uint32_t *>(cand.p) + off * K, s));
     }
     B200_CUDA_OK(cudaStreamSynchronize(s));
-    for (DevScratch *b : {&q, &dis, &ids}) {
+    for (DevScratch *b : {&q, &dis, &ids, &slots}) {
         cudaFree(b->p);
         b->p = nullptr;
     }
@@ -2277,7 +2344,7 @@ static int finalize_locked(b200_index *ix) {
         for (int l = 0; l < nl; l++) ix->max_list_pages = std::max<uint32_t>(ix->max_list_pages, (ix->list_len[l] + kPageRows - 1) / kPageRows);
     }
     // build scratch is not needed any more
-    for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_plan, &ix->w_host_q})
+    for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_plan, &ix->w_host_q, &ix->w_usable})
         a->release();
     if (!ix->raw) {  // an index without a single row still answers (empty results)
         const int raw_metric = ix->metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
@@ -2516,9 +2583,24 @@ static int refine_device(b200_index *ix, const float *d_q /*[nq][d_pad] prepared
 }
 
 // d_queries_raw: device fp32 [nq][d] -> ix->w_q [nq][d_pad] (cosine: unit length)
+// an unusable query (warp_row_usable) becomes all NaN: a distance to it is never finite, on any path; one warp per query
+__global__ void __launch_bounds__(256) nan_unusable_queries_kernel(float *q, int64_t nq, int d_pad) {
+    const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = warp_global; r < nq; r += nwarps)
+        if (!warp_row_usable(q + r * d_pad, d_pad))
+            for (int j = lane_id(); j < d_pad; j += 32) q[r * d_pad + j] = __int_as_float(0x7fffffff);
+}
+
 static int prepare_queries_device(b200_index *ix, const float *d_queries_raw, int64_t nq, cudaStream_t s) {
     B200_TRY(ix->w_q.reserve((size_t)nq * ix->d_pad * 4));
     B200_CUDA_OK(launch_pad_rows_f32(d_queries_raw, ix->d, ix->w_q.as<float>(), ix->d_pad, nq, s));
+    // L2 and cosine: a query with an infinite coordinate (or one whose square overflows) returns no rows, as a NaN one does.
+    // Under IP such a query is outside the contract (include/b200_search.h) and is scored as given.
+    if (ix->metric != B200_METRIC_IP && nq) {
+        nan_unusable_queries_kernel<<<gridsz(nq * 32), 256, 0, s>>>(ix->w_q.as<float>(), nq, ix->d_pad);
+        g_launches++;
+    }
     if (ix->metric == B200_METRIC_COSINE) B200_CUDA_OK(launch_normalize_rows_f32(ix->w_q.as<float>(), ix->d_pad, nq, s));
     return B200_OK;
 }
@@ -3484,6 +3566,7 @@ static int index_load_io(Io *f, b200_index **out) {
             }
         }
         ix->n = h.n;
+        std::vector<uint8_t> in_list;   // row id -> it is in a list
         if (ix->use_ivf) {
             std::vector<char> tmp;
             auto slurp = [&](void **dptr, size_t bytes) {
@@ -3506,7 +3589,8 @@ static int index_load_io(Io *f, b200_index **out) {
                 ix->max_list_pages = std::max<uint32_t>(ix->max_list_pages, (ix->list_len[l] + kPageRows - 1) / kPageRows);
             }
             page_off[nl] = (uint32_t)pages;
-            if (total != (uint64_t)h.n || pages != h.pages_used) return bail("corrupt index file (list lengths do not add up)");
+            // unusable rows are in no list: the lists hold at most n rows
+            if (total > (uint64_t)h.n || pages != h.pages_used) return bail("corrupt index file (list lengths do not add up)");
             if (h.payload == IVF_PRODUCER_PQ) {
                 if (!slurp((void **)&ix->d_pq, (size_t)h.m * pq_codewords(pq_bits) * h.dsub * 4)) return bail("truncated index file (codebook)");
                 if (pq_bits == 4) {
@@ -3528,6 +3612,7 @@ static int index_load_io(Io *f, b200_index **out) {
             std::vector<char> page(pb);
             std::vector<uint32_t> ids(kPageRows);
             std::vector<float> bias(kPageRows);
+            in_list.assign((size_t)h.n, 0);
             uint32_t pg = 0;
             for (int l = 0; l < nl; l++) {
                 const uint32_t np = (ix->list_len[l] + kPageRows - 1) / kPageRows;
@@ -3535,8 +3620,10 @@ static int index_load_io(Io *f, b200_index **out) {
                     if (!rd(f, page.data(), pb) || !rd(f, ids.data(), kPageRows * 4) || (ix->d_row_bias && !rd(f, bias.data(), kPageRows * 4)))
                         return bail("truncated index file (pages)");
                     const uint32_t valid = std::min<uint32_t>(kPageRows, ix->list_len[l] - t * kPageRows);
-                    for (uint32_t r = 0; r < valid; r++)
+                    for (uint32_t r = 0; r < valid; r++) {
                         if (ids[r] >= (uint64_t)h.n) return bail("corrupt index file (row id out of range)");
+                        in_list[ids[r]] = 1;
+                    }
                     const size_t row0 = (size_t)pg * kPageRows;
                     if (cudaMemcpy(reinterpret_cast<char *>(ix->d_pool) + (size_t)pg * pb, page.data(), pb, cudaMemcpyHostToDevice) != cudaSuccess ||
                         cudaMemcpy(ix->d_row_ids + row0, ids.data(), kPageRows * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
@@ -3559,7 +3646,7 @@ static int index_load_io(Io *f, b200_index **out) {
             if ((bin ? upload_coarse_bin(ix, ix->stream) : upload_coarse(ix, ix->stream)) != B200_OK) return bail(b200_last_error());
             if (cudaStreamSynchronize(ix->stream) != cudaSuccess) return bail("upload failed");
         }
-        if (h.version == 4) {   // every id < n or 0xFFFFFFFF before a kernel walks the graph
+        if (h.version == 4) {   // every id < n or 0xFFFFFFFF before a kernel walks the graph; MSTG: every id in a list (it has a pool slot)
             const int D = (int)h.reserved0;
             const size_t rb = (size_t)D * 4;
             const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / (int64_t)rb);
@@ -3569,8 +3656,11 @@ static int index_load_io(Io *f, b200_index **out) {
             for (int64_t off = 0; off < h.n; off += chunk) {
                 const int64_t mrows = std::min(chunk, h.n - off);
                 if (!rd(f, buf.data(), (size_t)mrows * rb)) return bail("truncated index file (graph)");
-                for (int64_t e = 0; e < mrows * D; e++)
-                    if (buf[e] != kNoId && buf[e] >= (uint64_t)h.n) return bail("corrupt index file (graph id out of range)");
+                for (int64_t e = 0; e < mrows * D; e++) {
+                    if (buf[e] == kNoId) continue;
+                    if (buf[e] >= (uint64_t)h.n) return bail("corrupt index file (graph id out of range)");
+                    if (h.type == IDX_MSTG && !in_list[buf[e]]) return bail("corrupt index file (graph edge to a row in no list)");
+                }
                 if (cudaMemcpy(ix->d_graph + off * D, buf.data(), (size_t)mrows * rb, cudaMemcpyHostToDevice) != cudaSuccess) return bail("H2D failed");
             }
             // MSTG: the slot map of the pages as loaded here

@@ -330,28 +330,51 @@ def compare(r, dis_g, ids_g):
     return bad
 
 
-def check_build(s, ix, y):
-    """Build invariants of a stored float inverted-file index s (read_index) of ix built from the rows y: every row in its
-    nearest list exactly once, the stored fp32 rows, the payload (bf16 RNE, SQ codes and padding, nearest PQ codewords) and
-    row_bias."""
-    n, d = len(y), s.d
+def usable(y):
+    """Rows the library may index: the fp32 sum of the squares of the coordinates is finite (no NaN or infinite coordinate,
+    no square that overflows), include/b200_search.h "Unusable rows"."""
+    y = np.asarray(y, np.float32)
+    with np.errstate(over="ignore", invalid="ignore"):
+        return np.isfinite(np.square(y).sum(1, dtype=np.float32))
+
+
+def check_lists(s, ix, y):
+    """List invariants of a stored float inverted-file index s of ix built from the rows y, for every payload: every usable
+    row in its nearest list exactly once and every unusable one in none, the list sizes, the stored fp32 rows (NaN bits
+    included) and finite centroids.  Returns (ids, lists, payload rows) of s.flat() and the stored rows x."""
+    y = np.asarray(y, np.float32)
     ids, lst, pay = s.flat()
-    assert np.array_equal(np.sort(ids), np.arange(n)), "the lists do not hold every row exactly once"
+    ok = usable(y)
+    assert np.isfinite(s.centroids).all(), "a centroid is not finite"
+    assert np.array_equal(np.sort(ids), np.nonzero(ok)[0]), "the lists do not hold every usable row, and no other, exactly once"
     assert np.array_equal(s.list_len, ix.list_sizes().astype(np.int64))
+    assert int(s.list_len.sum()) == int(ok.sum())
     assert s.has_raw
     x = s.rows.astype(np.float32)
-    if s.metric == COSINE:   # rows are stored unit length; the payload is encoded from the same vectors
-        np.testing.assert_allclose(x, y / np.linalg.norm(y.astype(np.float64), axis=1, keepdims=True), rtol=0, atol=1e-6)
+    if s.metric == COSINE:   # rows are stored unit length (those below FLT_EPSILON as given); the payload is encoded from them
+        np.testing.assert_allclose(x[ok], normalize_rows_f32(y[ok]), rtol=0, atol=1e-6)
     else:
-        assert np.array_equal(x, y)
+        assert x.tobytes() == y.tobytes(), "the stored fp32 rows differ from the input"
     X = x[ids].astype(np.float64)
     C = s.centroids.astype(np.float64)
     # ||x - c||^2 expanded (no n x nlist x d temporary at wide d): fp64 rounding stays far below the 1e-5 tolerance
     xx, cc = (X * X).sum(1)[:, None], (C * C).sum(1)[None, :]
     dist = xx + cc - 2 * X @ C.T
     tol = 1e-5 * (xx + cc + 2 * np.abs(X) @ np.abs(C).T)
-    own = dist[np.arange(n), lst]
-    assert (own <= dist.min(1) + tol[np.arange(n), lst]).all(), "a row is not in its nearest list"
+    at = np.arange(len(ids))
+    own = dist[at, lst]
+    assert (own <= dist.min(1) + tol[at, lst]).all(), "a row is not in its nearest list"
+    return ids, lst, pay, x
+
+
+def check_build(s, ix, y):
+    """Build invariants of a stored float inverted-file index s (read_index) of ix built from the rows y: check_lists, then
+    the payload (bf16 RNE, SQ codes and padding, nearest bf16-decoded PQ codewords) and row_bias."""
+    d = s.d
+    ids, lst, pay, x = check_lists(s, ix, y)
+    X = x[ids].astype(np.float64)
+    C = s.centroids.astype(np.float64)
+    n = len(ids)
     if s.payload == PAYLOAD_BF16:
         assert np.array_equal(pay[:, :d], to_bf16_values(x[ids])), "bf16 payload is not RNE of the row"
         assert (pay[:, d:] == 0).all()

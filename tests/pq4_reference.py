@@ -147,3 +147,30 @@ def reference_search(s, queries, k, nprobe, alive=None, table_round=None):
         r.out_dis[q, :len(top)] = dis[q, top]
     r.alive_row = alive_row
     return r
+
+
+def check_build(s, ix, y):
+    """Build invariants of a stored 4-bit PQ index s (read_index4) of ix built from the rows y: ivf_reference.check_lists, a
+    finite codebook, zero padding nibbles and bytes, every code the nearest fp32 codeword of the row's residual and row_bias
+    from the fp32 codewords."""
+    ids, lst, pay, x = R.check_lists(s, ix, y)
+    assert np.isfinite(s.codebook).all(), "a codeword is not finite"
+    n = len(ids)
+    codes = unpack(pay, s.m)
+    assert (pack(codes, s.code_bytes) == pay).all(), "padding nibbles and bytes must be 0"
+    X, C = x[ids].astype(np.float64), s.centroids.astype(np.float64)
+    res = X - C[lst]
+    cb = s.codebook.astype(np.float64)
+    for j in range(s.m):
+        r = res[:, j * s.dsub:(j + 1) * s.dsub]
+        dd = ((r[:, None, :] - cb[j][None, :, :]) ** 2).sum(2)
+        got = dd[np.arange(n), codes[:, j]]
+        assert (got <= dd.min(1) + 1e-5 * ((r * r).sum(1) + (cb[j] ** 2).sum(1).max()) + 1e-12).all(), f"code {j} is not the nearest fp32 codeword"
+    if s.metric == R.L2:
+        Rf = decode(s, pay).astype(np.float64)
+        bias = (Rf * (Rf + 2 * C[lst])).sum(1)
+        S = (np.abs(Rf) * np.abs(Rf + 2 * C[lst])).sum(1)
+        b = np.concatenate(s.bias).astype(np.float64)
+        assert (np.abs(b - bias) <= R.TOL_REL * S + 1e-30).all(), "row_bias differs from its fp32 formula"
+    else:
+        assert all(a is None for a in s.bias)

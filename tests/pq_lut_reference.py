@@ -86,3 +86,30 @@ def reference_search(s, queries, k, nprobe, alive=None, table_round=None):
         r.out_dis[q, :len(top)] = dis[q, top]
     r.alive_row = alive_row
     return r
+
+
+def check_build(s, ix, y):
+    """Build invariants of a stored table look-up PQ index s (ivf_reference.read_index) of ix built from the rows y:
+    ivf_reference.check_lists, a finite codebook, every code the nearest fp32 codeword of the row's residual, zero padding
+    bytes and row_bias from the fp32 codewords."""
+    ids, lst, pay, x = R.check_lists(s, ix, y)
+    assert np.isfinite(s.codebook).all(), "a codeword is not finite"
+    n = len(ids)
+    X, C = x[ids].astype(np.float64), s.centroids.astype(np.float64)
+    res = X - C[lst]
+    cb = s.codebook.astype(np.float64)
+    for j in range(s.m):
+        r = res[:, j * s.dsub:(j + 1) * s.dsub]
+        dd = ((r[:, None, :] - cb[j][None, :, :]) ** 2).sum(2)
+        got = dd[np.arange(n), pay[:, j]]
+        assert (got <= dd.min(1) + 1e-5 * ((r * r).sum(1) + (cb[j] ** 2).sum(1).max()) + 1e-12).all(), f"PQ code {j} is not the nearest fp32 codeword"
+    assert (pay[:, s.m:] == 0).all(), "PQ padding bytes must be 0"
+    if s.metric == R.L2:
+        Rf = pq_decode(s, pay).astype(np.float64)
+        np.testing.assert_array_equal(Rf, cb[np.arange(s.m)[None, :], pay[:, :s.m].astype(np.int64)].reshape(n, s.d))
+        bias = (Rf * (Rf + 2 * C[lst])).sum(1)
+        S = (np.abs(Rf) * np.abs(Rf + 2 * C[lst])).sum(1)
+        b = np.concatenate(s.bias).astype(np.float64)
+        assert (np.abs(b - bias) <= R.TOL_REL * S + 1e-30).all(), "row_bias differs from its fp32 formula"
+    else:
+        assert all(a is None for a in s.bias)

@@ -260,29 +260,6 @@ def test_table_sub_batches_at_m_2048(cache):
 # ---------------------------------------------------------------------------------------------------------------------------
 # build invariants
 # ---------------------------------------------------------------------------------------------------------------------------
-def _check_build(s, ix, y):
-    n = len(y)
-    ids, lst, pay = s.flat()
-    assert np.array_equal(np.sort(ids), np.arange(n))
-    assert np.array_equal(s.list_len, ix.list_sizes().astype(np.int64))
-    codes = P.unpack(pay, s.m)
-    assert (P.pack(codes, s.code_bytes) == pay).all(), "padding nibbles and bytes must be 0"
-    X, C = s.rows.astype(np.float64)[ids], s.centroids.astype(np.float64)
-    res = X - C[lst]
-    cb = s.codebook.astype(np.float64)
-    for j in range(s.m):
-        r = res[:, j * s.dsub:(j + 1) * s.dsub]
-        dd = ((r[:, None, :] - cb[j][None, :, :]) ** 2).sum(2)
-        got = dd[np.arange(n), codes[:, j]]
-        assert (got <= dd.min(1) + 1e-5 * ((r * r).sum(1) + (cb[j] ** 2).sum(1).max()) + 1e-12).all(), f"code {j} is not the nearest fp32 codeword"
-    if s.metric == R.L2:
-        Rf = P.decode(s, pay).astype(np.float64)
-        bias = (Rf * (Rf + 2 * C[lst])).sum(1)
-        S = (np.abs(Rf) * np.abs(Rf + 2 * C[lst])).sum(1)
-        b = np.concatenate(s.bias).astype(np.float64)
-        assert (np.abs(b - bias) <= R.TOL_REL * S + 1e-30).all(), "row_bias differs from its fp32 formula"
-    else:
-        assert all(a is None for a in s.bias)
 
 
 @pytest.mark.parametrize("metric", METRICS)
@@ -291,7 +268,7 @@ def test_build_invariants_one_shot_and_streamed(metric, d, m, tmp_path):
     y, _ = _data(N, d, seed=7 + metric)
     a = b2.VectorIndex("IVFPQ", metric, d, _params(m)).build(y)
     sa = _saved(a, tmp_path / "a.b2ix")
-    _check_build(sa, a, y)
+    P.check_build(sa, a, y)
     b = b2.VectorIndex("IVFPQ", metric, d, _params(m)).reserve(N).train(y)
     off, sizes, i = 0, [1, 255, 257, 1000], 0
     while off < N:
@@ -302,7 +279,7 @@ def test_build_invariants_one_shot_and_streamed(metric, d, m, tmp_path):
     # k-means training is not bitwise reproducible from run to run (8-bit indexes neither), so the two builds are held to the
     # same invariants and the same stored shape rather than compared byte for byte
     sb = _saved(b, tmp_path / "b.b2ix")
-    _check_build(sb, b, y)
+    P.check_build(sb, b, y)
     assert (sa.version, sa.m, sa.dsub, sa.code_bytes, sa.n) == (sb.version, sb.m, sb.dsub, sb.code_bytes, sb.n)
 
 

@@ -210,30 +210,6 @@ def test_query_sub_batches_at_m_128(cache):
 # ---------------------------------------------------------------------------------------------------------------------------
 # build invariants
 # ---------------------------------------------------------------------------------------------------------------------------
-def _check_build(s, ix, y):
-    n = len(y)
-    ids, lst, pay = s.flat()
-    assert np.array_equal(np.sort(ids), np.arange(n))
-    assert np.array_equal(s.list_len, ix.list_sizes().astype(np.int64))
-    x = s.rows.astype(np.float64)
-    X, C = x[ids], s.centroids.astype(np.float64)
-    res = X - C[lst]
-    cb = s.codebook.astype(np.float64)
-    for j in range(s.m):
-        r = res[:, j * s.dsub:(j + 1) * s.dsub]
-        dd = ((r[:, None, :] - cb[j][None, :, :]) ** 2).sum(2)
-        got = dd[np.arange(n), pay[:, j]]
-        assert (got <= dd.min(1) + 1e-5 * ((r * r).sum(1) + (cb[j] ** 2).sum(1).max()) + 1e-12).all(), f"PQ code {j} is not the nearest fp32 codeword"
-    assert (pay[:, s.m:] == 0).all(), "PQ padding bytes must be 0"
-    if s.metric == R.L2:
-        Rf = L.pq_decode(s, pay).astype(np.float64)
-        np.testing.assert_array_equal(Rf, cb[np.arange(s.m)[None, :], pay[:, :s.m].astype(np.int64)].reshape(n, s.d))
-        bias = (Rf * (Rf + 2 * C[lst])).sum(1)
-        S = (np.abs(Rf) * np.abs(Rf + 2 * C[lst])).sum(1)
-        b = np.concatenate(s.bias).astype(np.float64)
-        assert (np.abs(b - bias) <= R.TOL_REL * S + 1e-30).all(), "row_bias differs from its fp32 formula"
-    else:
-        assert all(a is None for a in s.bias)
 
 
 @pytest.mark.parametrize("metric", METRICS)
@@ -242,7 +218,7 @@ def test_build_invariants_one_shot_and_streamed(metric, tmp_path):
     y, _ = _data(N, d, seed=7 + metric)
     a = b2.VectorIndex("IVFPQ", metric, d, f"ncentroids={NLIST}, M={m}").build(y)
     sa = _saved(a, tmp_path / "a.b2ix")
-    _check_build(sa, a, y)
+    L.check_build(sa, a, y)
     b = b2.VectorIndex("IVFPQ", metric, d, f"ncentroids={NLIST}, M={m}").reserve(N).train(y)
     off, sizes, i = 0, [1, 255, 257, 1000], 0
     while off < N:
@@ -250,7 +226,7 @@ def test_build_invariants_one_shot_and_streamed(metric, tmp_path):
         off += sizes[i % 4]
         i += 1
     b.finalize()
-    _check_build(_saved(b, tmp_path / "b.b2ix"), b, y)
+    L.check_build(_saved(b, tmp_path / "b.b2ix"), b, y)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------

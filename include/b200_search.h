@@ -236,7 +236,11 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *                               rank, merged with reverse edges) and searches it by default: one CTA per query walks the graph
  *                               from the best min(ef_s, 32) ids of an nprobe=1 first stage, scoring each row once, exactly in
  *                               fp32.  Search keys: "ef_s=N" (list width, default 64, raised to k, at most 1024), "graph=0" (the
- *                               list search instead).  Any type but HNSWFLAT / MSTG with graph_degree > 0, or HNSWFLAT
+ *                               list search instead), "search_width=W" (W = 1, 2, 4 or 8, default 1: W parents expanded
+ *                               per iteration by a cluster of W CTAs per query, for single queries and small batches; the
+ *                               same scores, so the answer of W = 1 is the default's byte for byte; another W on a search
+ *                               that would walk the graph: B200_ERR_INVALID, checked before the filtered exact rule as
+ *                               ef_s is; ignored with graph=0, exact_batch=1 or no graph; it applies to MSTG's walk too).  Any type but HNSWFLAT / MSTG with graph_degree > 0, or HNSWFLAT
  *                               with keep_raw=0 / 2 and it: B200_ERR_UNSUPPORTED; another D: B200_ERR_INVALID.  A part
  *                               below the threshold has no graph;
  *   "BINARYFLAT"                binary rows (metric HAMMING or JACCARD, d in bits: a multiple of 8, at most 65536), exact
@@ -299,7 +303,9 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  * rows at ef_s = k = 1024 under a filter holds the query (d_pad64 floats) and 101760 bytes of lists and visited table in the
  * 227 KB a block may use, so d_pad64 <= 32640.  Every other configuration fits wider: the fp32 graph walk (HNSWFLAT) up to
  * d_pad 32672, the exact second stage at k = 1024 (d_pad x 4 + 73728 bytes) up to d_pad 39680; the bf16 and SQ8 list scans
- * stream k-blocks and need no more shared memory at any width. */
+ * stream k-blocks and need no more shared memory at any width.  The graph walks at search_width=W > 1 hold (W - 1) KB + 512
+ * bytes more: at ef_s = k = 1024 under a filter they are refused with B200_ERR_UNSUPPORTED above d_pad64 32256 / 31744 /
+ * 30720 (MSTG) and d_pad 32288 / 31776 / 30752 (HNSWFLAT) for W = 2 / 4 / 8; create and load accept the same widths. */
 #define B200_MAX_FLOAT_DIM 32640
 
 typedef struct b200_index b200_index;

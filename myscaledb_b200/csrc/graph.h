@@ -1,6 +1,6 @@
-// graph.h -- fixed-degree neighbour graph of an HNSWFLAT or MSTG index (graph_degree=D): build steps and the one-CTA-per-query
-// search (graph_sm90.cu).  The host side (candidates from the index's own list search, persistence, the search entry)
-// lives in ivf.cu.
+// graph.h -- fixed-degree neighbour graph of an HNSWFLAT or MSTG index (graph_degree=D): build steps and the graph search, one
+// CTA per query or one W-CTA cluster per query (search_width=W) (graph_sm90.cu).  The host side (candidates from the index's
+// own list search, persistence, the search entry) lives in ivf.cu.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -13,17 +13,19 @@ constexpr int kGraphThreads = 256;
 constexpr int kGraphVisitedLog2 = 14;
 constexpr int kGraphVisitedSlots = 1 << kGraphVisitedLog2;
 constexpr int kGraphMaxSeeds = 32;     // seeds per query: the best min(ef_s, 32) ids of the list path's first stage at nprobe 1
-constexpr int kGraphWidth = 1;         // parents expanded per iteration
+constexpr int kGraphMaxWidth = 8;      // parents expanded per iteration (search_width=W): 1, 2, 4 or 8, one CTA of a cluster each
 constexpr int kGraphMaxDegree = 64;
 constexpr int kGraphMaxEf = 1024;
 
-// Iterations one query may run: every iteration inserts at most kGraphWidth x D ids into the visited table and the seeds at
-// most kGraphMaxSeeds, so the table never holds more than kGraphVisitedSlots / 2 ids.  D = 16 / 32 / 64: 510 / 255 / 127.
-__host__ __device__ constexpr int graph_iteration_cap(int degree) {
-    return (kGraphVisitedSlots / 2 - kGraphMaxSeeds) / (kGraphWidth * degree);
+// Iterations one query may run: every iteration inserts at most width x D ids into the visited table and the seeds at most
+// kGraphMaxSeeds, so the table never holds more than kGraphVisitedSlots / 2 ids.  W = 1, D = 16 / 32 / 64: 510 / 255 / 127;
+// W = 8, D = 64: 15.
+__host__ __device__ constexpr int graph_iteration_cap(int degree, int width = 1) {
+    return (kGraphVisitedSlots / 2 - kGraphMaxSeeds) / (width * degree);
 }
 
 inline bool graph_degree_ok(int d) { return d == 16 || d == 32 || d == 64; }
+inline bool graph_width_ok(int w) { return w == 1 || w == 2 || w == 4 || w == 8; }
 
 // ids [m][K + 1] of the list search of rows row0 .. row0 + m - 1 (negative = none) -> cand [m][K] u32: the row's own id
 // dropped (or, when it is absent, the last entry), negative ids as 0xFFFFFFFF.  A row in no list (row_slot 0xFFFFFFFF) gets
@@ -58,9 +60,11 @@ struct GraphSearchParams {
     int l2;                    // else inner product (distance -key)
 };
 
-// dynamic shared memory of one query's CTA; q_len = d_pad (fp32 rows) or d_pad64 (bf16 pages)
-size_t graph_search_smem(int q_len, int ef, int k, bool filtered);
-// graph_search_kernel over the fp32 rows, or graph_search_bf16_kernel when p.pages is set
-int graph_search(const GraphSearchParams &p, int64_t nq, cudaStream_t s);
+// dynamic shared memory of each CTA of a query; q_len = d_pad (fp32 rows) or d_pad64 (bf16 pages)
+size_t graph_search_smem(int q_len, int ef, int k, bool filtered, int width);
+// graph_search_kernel over the fp32 rows, or graph_search_bf16_kernel when p.pages is set; at width = W > 1 (W parents per
+// iteration, graph_width_ok) their cluster forms, nq x W CTAs in clusters of W.  B200_ERR_UNSUPPORTED when the shared memory
+// does not fit or a cluster cannot be resident.
+int graph_search(const GraphSearchParams &p, int64_t nq, int width, cudaStream_t s);
 
 }  // namespace b200

@@ -1,7 +1,12 @@
 // graph_sm90.cu -- the neighbour graph of an HNSWFLAT or MSTG index (graph_degree=D): candidate lists -> rank-based pruning ->
-// reverse edges and merge at build, and the one-CTA-per-query graph search over fp32 rows (HNSWFLAT) or the bf16 list pages
-// (MSTG) (DESIGN §3).
+// reverse edges and merge at build, and the graph search over fp32 rows (HNSWFLAT) or the bf16 list pages (MSTG), one CTA per
+// query or, at search_width=W > 1, one cluster of W CTAs per query that expands W parents per iteration (DESIGN §3).
+#include <cooperative_groups.h>
 #include <cub/cub.cuh>
+
+#include <map>
+#include <mutex>
+#include <tuple>
 
 #include "common.cuh"
 #include "graph.h"
@@ -232,19 +237,23 @@ int graph_page_rows(const void *d_pool, const uint32_t *d_row_slot, int64_t row0
 }
 
 // ------------------------------------------------------------------------------------
-// search: one CTA per query
+// search: one CTA per query (W = 1), or one cluster of W CTAs per query (search_width=W)
 // ------------------------------------------------------------------------------------
 namespace {
-constexpr int kBatch = kGraphMaxDegree * kGraphWidth;   // ids one step filters and scores (>= kGraphMaxSeeds)
-static_assert(kBatch >= kGraphMaxSeeds, "a step takes the seeds");
+namespace cg = cooperative_groups;
+static_assert(kGraphMaxDegree >= kGraphMaxSeeds, "a step takes the seeds");
+static_assert(kGraphMaxWidth <= 8, "sh[16 ..) and sh[24 ..) hold one int per rank of a cluster");
 
 struct GraphSmem {
-    int64_t qs, vis, ek0, ei0, ek1, ei1, ck, ci, sk, si, nb, ak0, ai0, ak1, ai1, sh, ef0, ef1, total;
+    int64_t qs, vis, ek0, ei0, ek1, ei1, ck, ci, sk, si, nb, pk, pi, ak0, ai0, ak1, ai1, sh, ef0, ef1, total;
 };
 
-__host__ __device__ inline GraphSmem graph_smem_layout(int d_pad, int ef, int k, bool filtered) {
+// ck / ci / sk / si: the candidates of a step (W rows of at most kGraphMaxDegree); nb: this CTA's neighbour row; pk / pi
+// (W > 1 only): this CTA's sorted candidates, which the other CTAs of its cluster read
+__host__ __device__ inline GraphSmem graph_smem_layout(int d_pad, int ef, int k, bool filtered, int width) {
     GraphSmem L{};
     const int ka = filtered ? k : 0;
+    const int64_t batch = (int64_t)kGraphMaxDegree * width, pub = width > 1 ? kGraphMaxDegree : 0;
     int64_t o = 0;
     L.qs = o; o += (int64_t)d_pad * 4;
     L.vis = o; o += (int64_t)kGraphVisitedSlots * 4;
@@ -252,11 +261,13 @@ __host__ __device__ inline GraphSmem graph_smem_layout(int d_pad, int ef, int k,
     L.ei0 = o; o += (int64_t)ef * 4;
     L.ek1 = o; o += (int64_t)ef * 4;
     L.ei1 = o; o += (int64_t)ef * 4;
-    L.ck = o; o += kBatch * 4;
-    L.ci = o; o += kBatch * 4;
-    L.sk = o; o += kBatch * 4;
-    L.si = o; o += kBatch * 4;
-    L.nb = o; o += kBatch * 4;
+    L.ck = o; o += batch * 4;
+    L.ci = o; o += batch * 4;
+    L.sk = o; o += batch * 4;
+    L.si = o; o += batch * 4;
+    L.nb = o; o += kGraphMaxDegree * 4;
+    L.pk = o; o += pub * 4;
+    L.pi = o; o += pub * 4;
     L.ak0 = o; o += (int64_t)ka * 4;
     L.ai0 = o; o += (int64_t)ka * 4;
     L.ak1 = o; o += (int64_t)ka * 4;
@@ -319,6 +330,24 @@ __device__ __forceinline__ void merge_lists(const float *lk, const uint32_t *li,
     }
 }
 
+// Every thread of the CTA calls it with a flag: *below = the set flags of the threads below it; returns the set flags of the
+// CTA.  scratch: one int per warp, free again when it returns.
+__device__ __forceinline__ int cta_count_flags(bool flag, int *scratch, int *below) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const unsigned bal = __ballot_sync(0xffffffffu, flag);
+    if (lane == 0) scratch[warp] = __popc(bal);
+    __syncthreads();
+    int b = __popc(bal & ((1u << lane) - 1)), all = 0;
+    for (int w = 0; w < kGraphThreads / 32; w++) {
+        const int c = scratch[w];
+        b += w < warp ? c : 0;
+        all += c;
+    }
+    *below = b;
+    __syncthreads();
+    return all;
+}
+
 // Shared memory: the query, the visited table, two ef-entry lists (keys, ids, expanded flags) used in turn, the step's
 // candidates (adjacency order, then sorted), the neighbour row, two k-entry lists of alive rows (filtered searches only).
 // A step: warp 0 drops empty slots, repeats within the row and visited ids, compacts the rest in row order and inserts them
@@ -327,11 +356,22 @@ __device__ __forceinline__ void merge_lists(const float *lk, const uint32_t *li,
 // a sort or a merge by (key, id): the result does not depend on thread timing.  q_len: the query's floats in shared memory
 // (>= d_pad, zero beyond it), dim i at qs[qpos(i)]; score(id, qs, lane) returns, on every lane, the warp's L2 distance or inner
 // product of row id.
-template <class QPos, class Score>
+//
+// W > 1 (search_width=W): the W CTAs of a cluster walk one query, each holding the same copy of the lists and the visited
+// table.  An iteration takes the first W unexpanded entries; CTA r loads the row of parent r into its nb (phase A), cluster
+// barrier 1.  Phase B: CTA r puts the valid ids of the rows of ranks below r (read from their nb) into its visited table, so
+// the step above keeps the ids of its own row that are valid, unvisited, and not earlier in the concatenation of the W rows;
+// it scores and sorts them into pk / pi, their count in sh[0]; cluster barrier 2.  Phase C: every CTA copies the W sorted
+// runs in rank order, puts the ids of higher ranks into its visited table and rank-merges the runs: each CTA then applies the
+// same candidates, and every copy of the state stays the same (the visited tables hold the same ids).  A CTA writes nb only
+// in phase A (read by others in phase B, before barrier 2) and pk / pi / sh[0] only in phase B (read in phase C, before the
+// next barrier 1).  Every barrier sits on control flow that depends on the shared state alone, so all CTAs reach it; a last
+// one keeps every CTA's shared memory until no other reads it.  CTA 0 writes the answer.
+template <int W, class QPos, class Score>
 __device__ __forceinline__ void graph_walk(const GraphSearchParams &p, int q_len, QPos qpos, Score score) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const bool filtered = p.alive != nullptr;
-    const GraphSmem L = graph_smem_layout(q_len, p.ef, p.k, filtered);
+    const GraphSmem L = graph_smem_layout(q_len, p.ef, p.k, filtered, W);
     float *qs = reinterpret_cast<float *>(smem_raw + L.qs);
     uint32_t *vis = reinterpret_cast<uint32_t *>(smem_raw + L.vis);
     // the two lists of each kind are at a fixed byte distance: list `b` of a kind is its list 0 plus b x that distance
@@ -342,6 +382,9 @@ __device__ __forceinline__ void graph_walk(const GraphSearchParams &p, int q_len
     float *ck = reinterpret_cast<float *>(smem_raw + L.ck), *sk = reinterpret_cast<float *>(smem_raw + L.sk);
     uint32_t *ci = reinterpret_cast<uint32_t *>(smem_raw + L.ci), *si = reinterpret_cast<uint32_t *>(smem_raw + L.si);
     uint32_t *nb = reinterpret_cast<uint32_t *>(smem_raw + L.nb);
+    // where a step sorts this CTA's candidates: the step's sorted candidates (W = 1), or the run the cluster reads (W > 1)
+    float *rk = W == 1 ? sk : reinterpret_cast<float *>(smem_raw + L.pk);
+    uint32_t *ri = W == 1 ? si : reinterpret_cast<uint32_t *>(smem_raw + L.pi);
     float *ak0 = reinterpret_cast<float *>(smem_raw + L.ak0);
     uint32_t *ai0 = reinterpret_cast<uint32_t *>(smem_raw + L.ai0);
     auto ek = [&](int b) { return reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(ek0) + b * dek); };
@@ -352,20 +395,34 @@ __device__ __forceinline__ void graph_walk(const GraphSearchParams &p, int q_len
     int *sh = reinterpret_cast<int *>(smem_raw + L.sh);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int64_t q = blockIdx.x;
+    const int64_t q = blockIdx.x / W;
+    int rank = 0;
+    if constexpr (W > 1) rank = (int)cg::this_cluster().block_rank();
     const int nwarps = kGraphThreads / 32;
     for (int i = tid; i < q_len; i += kGraphThreads) qs[qpos(i)] = i < p.d_pad ? p.queries[q * p.d_pad + i] : 0.f;
     for (int i = tid; i < kGraphVisitedSlots; i += kGraphThreads) vis[i] = kNoId;
-    for (int j = tid; j < p.nseeds; j += kGraphThreads) {
-        const int64_t v = p.seeds[q * p.nseeds + j];
-        nb[j] = v >= 0 && v < p.n ? (uint32_t)v : kNoId;
-    }
+    if (rank == 0)   // the seeds are the row of rank 0 in the first step
+        for (int j = tid; j < p.nseeds; j += kGraphThreads) {
+            const int64_t v = p.seeds[q * p.nseeds + j];
+            nb[j] = v >= 0 && v < p.n ? (uint32_t)v : kNoId;
+        }
     __syncthreads();
     int cur = 0, cnt = 0, acur = 0, acnt = 0;
     unsigned long long scored = 0;
 
-    // one step over nb[0..m)
-    auto step = [&](int m) {
+    // one step over the rows of ranks 0 .. np - 1, m ids each (W = 1: over nb[0..m))
+    auto step = [&](int m, int np) {
+        if constexpr (W > 1) {
+            cg::cluster_group cluster = cg::this_cluster();
+            cluster.sync();   // barrier 1: the rows are in the nb of ranks 0 .. np - 1
+            const int pre = min(rank, np) * m;
+            for (int e = tid; e < pre; e += kGraphThreads) {
+                const uint32_t v = cluster.map_shared_rank(nb, e / m)[e % m];
+                if (v < (uint64_t)p.n) vis_insert(vis, v);
+            }
+            __syncthreads();
+            if (rank >= np) m = 0;
+        }
         if (warp == 0) {
             int nc = 0;
             for (int b = 0; b < m; b += 32) {
@@ -388,37 +445,92 @@ __device__ __forceinline__ void graph_walk(const GraphSearchParams &p, int q_len
             const float acc = score(ci[c], qs, lane);
             if (lane == 0) ck[c] = p.l2 ? acc : -acc;
         }
-        scored += (unsigned long long)nc;
+        if constexpr (W == 1) scored += (unsigned long long)nc;
         __syncthreads();
-        if (tid < nc) {   // sort by (key, id)
+        if (tid < nc) {   // sort by (key, id); nc <= kGraphMaxDegree < kGraphThreads
             const float key = ck[tid];
             const uint32_t id = ci[tid];
             int r = 0;
             for (int c = 0; c < nc; c++) r += better(ck[c], ci[c], key, id);
-            sk[r] = key;
-            si[r] = id;
+            rk[r] = key;
+            ri[r] = id;
         }
         __syncthreads();
-        merge_lists(ek(cur), ei(cur), ef(cur), cnt, sk, si, nc, p.ef, ek(cur ^ 1), ei(cur ^ 1), ef(cur ^ 1));
-        cur ^= 1;
-        cnt = min(p.ef, cnt + nc);
-        if (filtered) {   // the kept ones, still sorted, into ck / ci (free after the sort)
-            if (tid < nc) {
-                const uint32_t id = si[tid];
-                if ((p.alive[id >> 3] >> (id & 7)) & 1) {
-                    int r = 0;
-                    for (int c = 0; c < tid; c++) r += (p.alive[si[c] >> 3] >> (si[c] & 7)) & 1;
-                    ck[r] = sk[tid];
-                    ci[r] = id;
-                }
-            }
-            if (tid == 0) {
-                int na = 0;
-                for (int c = 0; c < nc; c++) na += (p.alive[si[c] >> 3] >> (si[c] & 7)) & 1;
-                sh[1] = na;
+        int total = nc;   // the step's candidates, sorted in sk / si
+        if constexpr (W > 1) {
+            cg::cluster_group cluster = cg::this_cluster();
+            cluster.sync();   // barrier 2: every rank's sorted run is in its pk / pi, its length in its sh[0]
+            int *runs = sh + 24;
+            if (tid < W) runs[tid] = *cluster.map_shared_rank(sh, tid);
+            __syncthreads();
+            total = 0;
+            for (int r = 0; r < W; r++) total += runs[r];
+            // run r at ck / ci [off, off + runs[r]), in rank order
+            for (int e = tid; e < W * kGraphMaxDegree; e += kGraphThreads) {
+                const int r = e / kGraphMaxDegree, j = e % kGraphMaxDegree;
+                if (j >= runs[r]) continue;
+                int off = 0;
+                for (int t = 0; t < r; t++) off += runs[t];
+                const uint32_t id = cluster.map_shared_rank(ri, r)[j];
+                ck[off + j] = cluster.map_shared_rank(rk, r)[j];
+                ci[off + j] = id;
+                if (r > rank) vis_insert(vis, id);
             }
             __syncthreads();
-            const int na = sh[1];
+            // rank-merge: an entry's place is its place in its run plus the entries of the other runs better than it
+            for (int e = tid; e < W * kGraphMaxDegree; e += kGraphThreads) {
+                const int r = e / kGraphMaxDegree, j = e % kGraphMaxDegree;
+                if (j >= runs[r]) continue;
+                int off = 0;
+                for (int t = 0; t < r; t++) off += runs[t];
+                const float key = ck[off + j];
+                const uint32_t id = ci[off + j];
+                int pos = j;
+                for (int t = 0, o = 0; t < W; o += runs[t], t++)
+                    if (t != r) pos += count_better(ck + o, ci + o, runs[t], key, id);
+                sk[pos] = key;
+                si[pos] = id;
+            }
+            scored += (unsigned long long)total;
+            __syncthreads();
+        }
+        merge_lists(ek(cur), ei(cur), ef(cur), cnt, sk, si, total, p.ef, ek(cur ^ 1), ei(cur ^ 1), ef(cur ^ 1));
+        cur ^= 1;
+        cnt = min(p.ef, cnt + total);
+        if (filtered) {   // the kept ones, still sorted, into ck / ci (free after the sort)
+            int na = 0;
+            if constexpr (W == 1) {
+                if (tid < nc) {
+                    const uint32_t id = si[tid];
+                    if ((p.alive[id >> 3] >> (id & 7)) & 1) {
+                        int r = 0;
+                        for (int c = 0; c < tid; c++) r += (p.alive[si[c] >> 3] >> (si[c] & 7)) & 1;
+                        ck[r] = sk[tid];
+                        ci[r] = id;
+                    }
+                }
+                if (tid == 0) {
+                    int kept = 0;
+                    for (int c = 0; c < nc; c++) kept += (p.alive[si[c] >> 3] >> (si[c] & 7)) & 1;
+                    sh[1] = kept;
+                }
+                __syncthreads();
+                na = sh[1];
+            } else {   // up to W x kGraphMaxDegree candidates: compacted a CTA-width at a time
+                for (int b = 0; b < total; b += kGraphThreads) {
+                    const int t = b + tid;
+                    const uint32_t id = t < total ? si[t] : 0;
+                    const bool keep = t < total && ((p.alive[id >> 3] >> (id & 7)) & 1);
+                    int below;
+                    const int all = cta_count_flags(keep, sh + 8, &below);
+                    if (keep) {
+                        ck[na + below] = sk[t];
+                        ci[na + below] = id;
+                    }
+                    na += all;
+                }
+                __syncthreads();
+            }
             merge_lists(ak(acur), ai(acur), nullptr, acnt, ck, ci, na, p.k, ak(acur ^ 1), ai(acur ^ 1), nullptr);
             acur ^= 1;
             acnt = min(p.k, acnt + na);
@@ -426,50 +538,78 @@ __device__ __forceinline__ void graph_walk(const GraphSearchParams &p, int q_len
         __syncthreads();
     };
 
-    step(p.nseeds);
+    step(p.nseeds, 1);
     for (int it = 0; it < p.max_iters; it++) {
-        // parent: the first unexpanded entry of the list
-        int first = INT_MAX;
-        for (int e = tid; e < cnt; e += kGraphThreads)
-            if (!ef(cur)[e]) {
-                first = e;
-                break;
+        if constexpr (W == 1) {
+            // parent: the first unexpanded entry of the list
+            int first = INT_MAX;
+            for (int e = tid; e < cnt; e += kGraphThreads)
+                if (!ef(cur)[e]) {
+                    first = e;
+                    break;
+                }
+            first = __reduce_min_sync(0xffffffffu, first);
+            if (lane == 0) sh[8 + warp] = first;
+            __syncthreads();
+            if (tid == 0) {
+                int f = INT_MAX;
+                for (int w = 0; w < nwarps; w++) f = min(f, sh[8 + w]);
+                sh[2] = f;
+                if (f != INT_MAX) {
+                    ef(cur)[f] = 1;
+                    sh[3] = (int)ei(cur)[f];
+                }
             }
-        first = __reduce_min_sync(0xffffffffu, first);
-        if (lane == 0) sh[8 + warp] = first;
-        __syncthreads();
-        if (tid == 0) {
-            int f = INT_MAX;
-            for (int w = 0; w < nwarps; w++) f = min(f, sh[8 + w]);
-            sh[2] = f;
-            if (f != INT_MAX) {
-                ef(cur)[f] = 1;
-                sh[3] = (int)ei(cur)[f];
+            __syncthreads();
+            if (sh[2] == INT_MAX) break;
+            const uint32_t parent = (uint32_t)sh[3];
+            for (int j = tid; j < p.degree; j += kGraphThreads) nb[j] = p.graph[(size_t)parent * p.degree + j];
+            __syncthreads();
+            step(p.degree, 1);
+        } else {
+            // parents: the first W unexpanded entries of the list (fewer when fewer remain) into sh[16 ..), a CTA-width at a time.
+            // np and the list are the same in every CTA of the cluster, so all of them break together.
+            int np = 0;
+            for (int b = 0; b < cnt && np < W; b += kGraphThreads) {
+                const int e = b + tid;
+                const bool un = e < cnt && !ef(cur)[e];
+                int below;
+                const int all = cta_count_flags(un, sh + 8, &below);
+                if (un && np + below < W) {
+                    sh[16 + np + below] = (int)ei(cur)[e];
+                    ef(cur)[e] = 1;
+                }
+                np = min(W, np + all);
             }
+            __syncthreads();
+            if (np == 0) break;
+            if (rank < np) {
+                const uint32_t parent = (uint32_t)sh[16 + rank];
+                for (int j = tid; j < p.degree; j += kGraphThreads) nb[j] = p.graph[(size_t)parent * p.degree + j];
+            }
+            __syncthreads();
+            step(p.degree, np);
         }
-        __syncthreads();
-        if (sh[2] == INT_MAX) break;
-        const uint32_t parent = (uint32_t)sh[3];
-        for (int j = tid; j < p.degree; j += kGraphThreads) nb[j] = p.graph[(size_t)parent * p.degree + j];
-        __syncthreads();
-        step(p.degree);
     }
+    if constexpr (W > 1) cg::this_cluster().sync();   // no CTA leaves while another may still read its shared memory
 
-    const float *fk = filtered ? ak(acur) : ek(cur);
-    const uint32_t *fi = filtered ? ai(acur) : ei(cur);
-    const int have_n = filtered ? acnt : min(cnt, p.k);
-    for (int j = tid; j < p.k; j += kGraphThreads) {
-        const bool have = j < have_n;
-        p.out_ids[q * p.k + j] = have ? (int64_t)fi[j] + p.id_offset : -1;
-        p.out_dis[q * p.k + j] = have ? (p.l2 ? fk[j] : -fk[j]) : (p.l2 ? FLT_MAX : -FLT_MAX);
+    if (rank == 0) {
+        const float *fk = filtered ? ak(acur) : ek(cur);
+        const uint32_t *fi = filtered ? ai(acur) : ei(cur);
+        const int have_n = filtered ? acnt : min(cnt, p.k);
+        for (int j = tid; j < p.k; j += kGraphThreads) {
+            const bool have = j < have_n;
+            p.out_ids[q * p.k + j] = have ? (int64_t)fi[j] + p.id_offset : -1;
+            p.out_dis[q * p.k + j] = have ? (p.l2 ? fk[j] : -fk[j]) : (p.l2 ? FLT_MAX : -FLT_MAX);
+        }
+        if (tid == 0) atomicAdd(p.rows_scored, scored);
     }
-    if (tid == 0) atomicAdd(p.rows_scored, scored);
 }
-}  // namespace
 
 // HNSWFLAT: rows scored from the fp32 rows in HBM
-__global__ void __launch_bounds__(kGraphThreads) graph_search_kernel(const GraphSearchParams p) {
-    graph_walk(p, p.d_pad, [](int i) { return i; }, [&](uint32_t v, const float *qs, int lane) {
+template <int W>
+__device__ __forceinline__ void graph_walk_fp32(const GraphSearchParams &p) {
+    graph_walk<W>(p, p.d_pad, [](int i) { return i; }, [&](uint32_t v, const float *qs, int lane) {
         const float4 *row = reinterpret_cast<const float4 *>(p.rows + (size_t)v * p.d_pad);
         const float4 *x4 = reinterpret_cast<const float4 *>(qs);
         float acc = 0.f;
@@ -508,11 +648,10 @@ __device__ __forceinline__ float bf16x2_term(int l2, uint32_t u, float x0, float
     return fmaf(x1, y1, acc);
 }
 
-// (kGraphThreads, 2): without the occupancy hint ptxas keeps this walk to 32 registers and spills; two CTAs per SM is what its
-// shared memory allows at the largest lists anyway
-__global__ void __launch_bounds__(kGraphThreads, 2) graph_search_bf16_kernel(const GraphSearchParams p) {
+template <int W>
+__device__ __forceinline__ void graph_walk_bf16(const GraphSearchParams &p) {
     const auto qpos = [](int i) { return (i & ~63) | ((i >> 2) & 1) << 5 | ((i >> 3) & 7) << 2 | (i & 3); };
-    graph_walk(p, p.d_pad64, qpos, [&](uint32_t v, const float *qs, int lane) {
+    graph_walk<W>(p, p.d_pad64, qpos, [&](uint32_t v, const float *qs, int lane) {
         const uint32_t slot = p.row_slot[v];
         const int kbs = p.d_pad64 / 64, seg = lane >> 3, part = lane & 7;
         const __nv_bfloat16 *pool = static_cast<const __nv_bfloat16 *>(p.pages);
@@ -532,20 +671,92 @@ __global__ void __launch_bounds__(kGraphThreads, 2) graph_search_bf16_kernel(con
         return acc;
     });
 }
+}  // namespace
 
-size_t graph_search_smem(int q_len, int ef, int k, bool filtered) { return (size_t)graph_smem_layout(q_len, ef, k, filtered).total; }
+__global__ void __launch_bounds__(kGraphThreads) graph_search_kernel(const GraphSearchParams p) { graph_walk_fp32<1>(p); }
 
-int graph_search(const GraphSearchParams &p, int64_t nq, cudaStream_t s) {
+// (kGraphThreads, 2): without the occupancy hint ptxas keeps this walk to 32 registers and spills; two CTAs per SM is what its
+// shared memory allows at the largest lists anyway
+__global__ void __launch_bounds__(kGraphThreads, 2) graph_search_bf16_kernel(const GraphSearchParams p) { graph_walk_bf16<1>(p); }
+
+// the walks at search_width = W > 1: one cluster of W CTAs per query (grid nq x W, cluster (W, 1, 1)).  (kGraphThreads, 2) on
+// both: without it ptxas keeps the fp32 walk to 40 registers and spills
+template <int W>
+__global__ void __launch_bounds__(kGraphThreads, 2) graph_search_cluster_kernel(const GraphSearchParams p) { graph_walk_fp32<W>(p); }
+template <int W>
+__global__ void __launch_bounds__(kGraphThreads, 2) graph_search_bf16_cluster_kernel(const GraphSearchParams p) { graph_walk_bf16<W>(p); }
+
+size_t graph_search_smem(int q_len, int ef, int k, bool filtered, int width) {
+    return (size_t)graph_smem_layout(q_len, ef, k, filtered, width).total;
+}
+
+namespace {
+template <int W>
+const void *graph_cluster_kernel(bool bf16) {
+    return bf16 ? (const void *)graph_search_bf16_cluster_kernel<W> : (const void *)graph_search_cluster_kernel<W>;
+}
+
+// cudaOccupancyMaxActiveClusters of (device, kernel, dynamic shared memory), asked once per key
+int graph_max_active_clusters(const void *fn, const cudaLaunchConfig_t &cfg, int *clusters) {
+    static std::mutex mu;
+    static std::map<std::tuple<int, const void *, size_t>, int> known;
+    int dev = 0;
+    B200_CUDA_OK(cudaGetDevice(&dev));
+    const auto key = std::make_tuple(dev, fn, cfg.dynamicSmemBytes);
+    std::lock_guard<std::mutex> lock(mu);
+    const auto it = known.find(key);
+    if (it != known.end()) {
+        *clusters = it->second;
+        return B200_OK;
+    }
+    B200_CUDA_OK(cudaOccupancyMaxActiveClusters(clusters, fn, &cfg));
+    known[key] = *clusters;
+    return B200_OK;
+}
+}  // namespace
+
+int graph_search(const GraphSearchParams &p, int64_t nq, int width, cudaStream_t s) {
     if (nq == 0) return B200_OK;
+    const int W = width;
+    if (!graph_width_ok(W)) return fail(B200_ERR_INVALID, "search_width must be 1, 2, 4 or 8, got " + std::to_string(W));
     const bool bf16 = p.pages != nullptr;
-    const size_t smem = graph_search_smem(bf16 ? p.d_pad64 : p.d_pad, p.ef, p.k, p.alive != nullptr);
-    const void *fn = bf16 ? (const void *)graph_search_bf16_kernel : (const void *)graph_search_kernel;
-    if (smem > (size_t)kSmemOptinBytes)   // d <= B200_MAX_FLOAT_DIM keeps this far below the limit at ef = k = 1024 with a filter
+    const size_t smem = graph_search_smem(bf16 ? p.d_pad64 : p.d_pad, p.ef, p.k, p.alive != nullptr, W);
+    const void *fn = W == 1   ? (bf16 ? (const void *)graph_search_bf16_kernel : (const void *)graph_search_kernel)
+                     : W == 2 ? graph_cluster_kernel<2>(bf16)
+                     : W == 4 ? graph_cluster_kernel<4>(bf16)
+                              : graph_cluster_kernel<8>(bf16);
+    // d <= B200_MAX_FLOAT_DIM keeps this below the limit at W = 1; W > 1 adds (W - 1) KB for the step's candidates and 512 B
+    // for the published run, refused at the widest d_pad at ef = k = 1024 with a filter (include/b200_search.h)
+    if (smem > (size_t)kSmemOptinBytes)
         return fail(B200_ERR_UNSUPPORTED, "graph search: d_pad " + std::to_string(bf16 ? p.d_pad64 : p.d_pad) + " at ef " + std::to_string(p.ef) +
-                                              " needs " + std::to_string(smem) + " bytes of shared memory, more than " + std::to_string(kSmemOptinBytes));
+                                              (W > 1 ? " and search_width " + std::to_string(W) : std::string()) + " needs " + std::to_string(smem) +
+                                              " bytes of shared memory, more than " + std::to_string(kSmemOptinBytes));
     B200_CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (bf16) graph_search_bf16_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
-    else graph_search_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
+    if (W == 1) {
+        if (bf16) graph_search_bf16_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
+        else graph_search_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
+    } else {
+        if (nq > INT32_MAX / W) return fail(B200_ERR_UNSUPPORTED, "graph search: nq x search_width must stay below 2^31");
+        cudaLaunchConfig_t cfg{};
+        cudaLaunchAttribute attr{};
+        attr.id = cudaLaunchAttributeClusterDimension;
+        attr.val.clusterDim.x = (unsigned)W;
+        attr.val.clusterDim.y = 1;
+        attr.val.clusterDim.z = 1;
+        cfg.gridDim = dim3((unsigned)(nq * W));
+        cfg.blockDim = dim3(kGraphThreads);
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = s;
+        cfg.attrs = &attr;
+        cfg.numAttrs = 1;
+        int clusters = 0;
+        B200_TRY(graph_max_active_clusters(fn, cfg, &clusters));
+        if (clusters < 1)
+            return fail(B200_ERR_UNSUPPORTED, "graph search: a cluster of " + std::to_string(W) + " CTAs with " + std::to_string(smem) +
+                                                  " bytes of shared memory each cannot be resident on this device");
+        void *args[] = {const_cast<GraphSearchParams *>(&p)};
+        B200_CUDA_OK(cudaLaunchKernelExC(&cfg, fn, args));
+    }
     g_launches++;
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;

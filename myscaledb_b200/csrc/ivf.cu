@@ -1342,7 +1342,8 @@ int64_t corpus_prefilter_limit(const b200_corpus *c, int mode, int64_t nq, int k
 int index_metric(const b200_index *ix) { return ix->metric; }
 }
 
-static int parse_int_param(const char *json, const char *key, int defv) {
+// signed: a value with a leading '-' is read too (else such a key reads as absent)
+static int parse_int_param(const char *json, const char *key, int defv, bool signed_value = false) {
     if (!json) return defv;
     const size_t kl = strlen(key);
     for (const char *p = strstr(json, key); p; p = strstr(p + 1, key)) {
@@ -1352,6 +1353,7 @@ static int parse_int_param(const char *json, const char *key, int defv) {
         const bool right_ok = !(isalnum((unsigned char)*e) || *e == '_');
         if (!left_ok || !right_ok) continue;
         while (*e && (*e == '"' || *e == ':' || *e == '=' || *e == ' ' || *e == '\'')) e++;
+        if (signed_value && *e == '-' && e[1] >= '0' && e[1] <= '9') return atoi(e);
         if (!(*e >= '0' && *e <= '9')) continue;
         return atoi(e);
     }
@@ -2977,23 +2979,28 @@ static int filter_probe_search(b200_index *ix, const float *d_q, int64_t nq, int
 // the kept rows answers instead.  Not measured: 2 only asks for room to fill k from the kept rows met on the walk.
 constexpr double kGraphExactFactor = 2.0;
 
-// rows one graph query scores at most: its seeds, then D per expanded parent up to the iteration cap
-static int64_t graph_rows_at_cap(const b200_index *ix, int nseeds) {
-    return nseeds + (int64_t)graph_iteration_cap(ix->graph_degree) * kGraphWidth * ix->graph_degree;
+// rows one graph query scores at most: its seeds, then D per expanded parent, W parents per iteration up to the iteration cap
+static int64_t graph_rows_at_cap(const b200_index *ix, int nseeds, int width) {
+    return nseeds + (int64_t)graph_iteration_cap(ix->graph_degree, width) * width * ix->graph_degree;
 }
 
 static int graph_ef(const char *params, int k) {
     return std::max(k, parse_int_param(params, "ef_s", 64));
 }
 
+// search_width=W: parents expanded per iteration, one CTA of a cluster each (1, 2, 4 or 8; default 1, one CTA per query)
+static int graph_width(const char *params) { return parse_int_param(params, "search_width", 1, true); }
+
 // The graph search, asynchronous on s (d_q: the prepared queries [nq][d_pad]): seeds from the list path's first stage at
-// nprobe 1 (the best min(ef_s, 32) ids per query), then one CTA per query walks the graph: graph_search_kernel over the fp32
-// rows in HBM (HNSWFLAT, kc = k), or graph_search_bf16_kernel over the bf16 list rows (MSTG).  With a second stage
+// nprobe 1 (the best min(ef_s, 32) ids per query), then one CTA per query (search_width=W > 1: one cluster of W CTAs, W
+// parents per iteration) walks the graph: graph_search_kernel over the fp32 rows in HBM (HNSWFLAT, kc = k), or
+// graph_search_bf16_kernel over the bf16 list rows (MSTG).  With a second stage
 // (two_stage, MSTG only; kc may equal k, at k = 1024) the walk's best kc rows are re-ranked exactly by refine_device, from HBM
 // or from host memory.
 static int graph_search_locked(b200_index *ix, const float *d_queries, const float *d_q, int64_t nq, int k, int kc, bool two_stage, const char *params,
                                const uint8_t *d_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
     const int ef = graph_ef(params, kc);
+    const int width = graph_width(params);   // validated by search_device_locked
     const int S = std::min(ef, kGraphMaxSeeds);
     B200_TRY(ix->w_seeds.reserve((size_t)nq * S * 8));
     B200_TRY(ix->w_seedd.reserve((size_t)nq * S * 4));
@@ -3029,16 +3036,16 @@ static int graph_search_locked(b200_index *ix, const float *d_queries, const flo
     gp.nseeds = S;
     gp.ef = ef;
     gp.k = kc;
-    gp.max_iters = graph_iteration_cap(ix->graph_degree);
+    gp.max_iters = graph_iteration_cap(ix->graph_degree, width);
     gp.l2 = ix->metric == B200_METRIC_L2;
-    B200_TRY(graph_search(gp, nq, s));
+    B200_TRY(graph_search(gp, nq, width, s));
     if (two_stage) {
         B200_TRY(refine_device(ix, d_q, nq, ix->w_oi.as<int64_t>(), kc, k, id_offset, d_out_dis, d_out_ids, s));
     } else if (ix->metric == B200_METRIC_COSINE) {
         cosine_finish_kernel<<<(unsigned)ceil_div(nq * k, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, k, d_out_dis, d_out_ids);
         g_launches++;
     }
-    ix->last_items = nq;
+    ix->last_items = nq * width;   // CTAs launched
     ix->last_graph = true;
     return B200_OK;
 }
@@ -3092,6 +3099,8 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         if (k > kGraphMaxEf) return fail(B200_ERR_UNSUPPORTED, "k > 1024 on the graph search");
         const int ef_s = parse_int_param(params, "ef_s", 64);
         if (ef_s > kGraphMaxEf) return fail(B200_ERR_INVALID, "ef_s must be at most 1024, got " + std::to_string(ef_s));
+        const int width = graph_width(params);
+        if (!graph_width_ok(width)) return fail(B200_ERR_INVALID, "search_width must be 1, 2, 4 or 8, got " + std::to_string(width));
         if (ix->d_row_slot) {
             const int refine_factor = std::max(1, parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", ix->refine_factor)));
             graph_two_stage = has_rows(ix) && refine_factor > 1 && !first_stage_only;
@@ -3100,7 +3109,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         if (out_num_candidates) *out_num_candidates = kc;
         // the exact rule scans the fp32 rows in HBM: without them (MSTG keep_raw=0 | 2) the walk always answers
         if (d_alive && h_alive && ix->raw) {
-            const int64_t rows_cap = graph_rows_at_cap(ix, std::min(graph_ef(params, kc), kGraphMaxSeeds));
+            const int64_t rows_cap = graph_rows_at_cap(ix, std::min(graph_ef(params, kc), kGraphMaxSeeds), width);
             const int64_t limit = std::min<int64_t>((int64_t)std::ceil(kGraphExactFactor * kc * (double)ix->n / (double)rows_cap) - 1,
                                                     corpus_prefilter_limit(ix->raw, prefilter, nq, k));
             exact = limit >= 0 && host_count_alive(h_alive, ix->n, limit) <= limit;

@@ -110,12 +110,12 @@ struct b200_corpus {
     uint64_t serial = 0;
     uint64_t epoch = 0;
     // workspaces
-    DevBuf w_raw, w_q32, w_qbf, w_qlo, w_qnorm, w_pk, w_pi, w_lk, w_li, w_alive, w_odis, w_oids, w_stage, w_prog;
+    DevBuf w_raw, w_q32, w_qbf, w_qlo, w_qnorm, w_pk, w_pi, w_lk, w_li, w_alive, w_odis, w_oids, w_stage, w_prog, w_qb;
     // pre-filtered search (prefilter.cu): kept row ids, compaction scratch, compact rows (+ a row of slack), their side arrays
     DevBuf w_pf_ids, w_pf_tmp, w_pf_rows, w_pf_side;
-    std::array<DevBuf *, 18> workspaces() {
+    std::array<DevBuf *, 19> workspaces() {
         return {&w_raw, &w_q32, &w_qbf, &w_qlo, &w_qnorm, &w_pk, &w_pi, &w_lk, &w_li, &w_alive, &w_odis, &w_oids, &w_stage, &w_prog,
-                &w_pf_ids, &w_pf_tmp, &w_pf_rows, &w_pf_side};
+                &w_qb, &w_pf_ids, &w_pf_tmp, &w_pf_rows, &w_pf_side};
     }
     int prefilter = 0;             // b200_corpus_set_prefilter: 0 auto | 1 never | 2 whenever the compact copy fits the budget
     int64_t last_rows_scored = 0;  // rows the last search scored: n after a full scan, the kept rows after a gathered one
@@ -504,6 +504,9 @@ static int gemm_chunk(b200_corpus *c, GemmTopkParams &gp, int64_t nq_c, int k, i
     gp.nq_valid = (int)nq_c;
     gp.k = k;
     gp.q_tiles = q_tiles;
+    B200_TRY(c->w_qb.reserve((size_t)nq_pad * 4));
+    B200_CUDA_OK(cudaMemsetAsync(c->w_qb.p, 0xff, (size_t)nq_pad * 4, s));   // no bound yet
+    gp.query_bound = c->w_qb.as<uint32_t>();
     if (q_tiles > 1) {
         B200_TRY(c->w_prog.reserve((size_t)grid * 4));
         B200_CUDA_OK(cudaMemsetAsync(c->w_prog.p, 0, (size_t)grid * 4, s));

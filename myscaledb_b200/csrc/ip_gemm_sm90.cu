@@ -209,22 +209,25 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
             // Pacing: the CTAs that stream the SAME corpus tiles for different query tiles stay within `sync_slack`
             // tiles of each other, so a tile is fetched from HBM once and served to the others from L2.  Only pacing, no
             // data dependency: plain volatile counters.  Bounded wait (~50 us): if the sharers are not co-resident
-            // (another kernel holds SMs) pacing is dropped instead of risking a co-residency deadlock.
+            // (another kernel holds SMs) pacing is dropped instead of risking a co-residency deadlock.  Lane g reads sharer g's
+            // counter, so a check is one L2 round trip rather than one per sharer: a tile's check has to end within the few
+            // k-blocks the ring holds ahead of the consumers.
             if (pacing) {
-                int ok = 1;
-                if (lane == 0) {
-                    volatile int *prog = p.progress + (size_t)worker * p.q_tiles;
-                    prog[qt] = ordinal + 1;
-                    int spins = 0;
-                    for (int g = 0; g < p.q_tiles; g++)
-                        while (prog[g] < ordinal + 1 - p.sync_slack && spins < 256) {
-                            __nanosleep(200);
-                            spins++;
-                        }
-                    if (spins >= 256) prog[qt] = 0x7fffffff;  // never hold anybody back again
-                    ok = spins < 256;
+                volatile int *prog = p.progress + (size_t)worker * p.q_tiles;
+                if (lane == 0) prog[qt] = ordinal + 1;
+                __syncwarp();
+                int spins = 0;
+                while (spins < 256) {
+                    bool behind = false;
+                    for (int g = lane; g < p.q_tiles; g += 32) behind |= prog[g] < ordinal + 1 - p.sync_slack;
+                    if (!__any_sync(0xffffffffu, behind)) break;
+                    __nanosleep(200);
+                    spins++;
                 }
-                pacing = __shfl_sync(0xffffffffu, ok, 0) != 0;
+                if (spins >= 256) {
+                    if (lane == 0) prog[qt] = 0x7fffffff;  // never hold anybody back again
+                    pacing = false;
+                }
             }
             __syncwarp();
             for (int h = 0; h < O::PASSES; h++) {
@@ -273,8 +276,10 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
             list_bind(list, p.list_keys_gmem + producer * list_cap * EPI_THREADS, p.list_ids_gmem + producer * list_cap * EPI_THREADS,
                       tid, p.k);
         }
+        const int q = qt * BM + qrow;   // this lane's query in the batch
+        const bool live = q < p.nq_valid;
         // binary Jaccard: popc(q) of this lane's query row (0 for padding rows)
-        const int pq = (jaccard && qt * BM + qrow < p.nq_valid) ? (int)p.q_popc[qt * BM + qrow] : 0;
+        const int pq = (jaccard && live) ? (int)p.q_popc[q] : 0;
         const uint32_t smem0 = smem_u32(smem);
         int stage = 0;
         uint32_t phase = 0;
@@ -284,6 +289,8 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
             const bool tail = n0 + BN > p.n;
             for (int pass = 0; pass < O::PASSES; pass++) {
                 const int h = O::WG == 1 ? pass : wg;   // the half of the tile
+                // the query's shared bound: the best k-th key any of its lists has published (in flight during the MMAs)
+                const uint32_t bound_u = live ? __ldcg(p.query_bound + q) : 0xffffffffu;
                 // side entries of columns 32 g + lane of the half (in flight during the MMAs)
                 float sc[HN / 32] = {}, bi[HN / 32] = {};
                 if (use_side) {
@@ -382,8 +389,12 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
                 // Fast path, from the registers: per group of 32 columns each lane reduces its fragment to the best negated
                 // key of each of its four rows (28 FMNMX), the quad to one row per lane (3 SHFL), which is tested against the
                 // owner's threshold with the non-strict test of epilogue_chunk, and one vote.  Thresholds only tighten, so the
-                // ones read before the four tests admit at least what epilogue_chunk will.
-                const float thr = __shfl_sync(0xffffffffu, fminf(list.thr_key, FLT_MAX), (lane >> 2) + 8 * (2 * (lane & 1) + ((lane >> 1) & 1)));
+                // ones read before the four tests admit at least what epilogue_chunk will.  The threshold is the smaller of the
+                // list's own k-th key and the query's shared bound.  Keys here are absolute per query (the per-query constant is
+                // added at the merge), so the bound is exact; a key equal to it is still admitted, so ties keep their
+                // smallest-id winner.
+                const float bound = bound_u == 0xffffffffu ? FLT_MAX : bound_decode(bound_u);
+                const float thr = __shfl_sync(0xffffffffu, fminf(list.thr_key, bound), (lane >> 2) + 8 * (2 * (lane & 1) + ((lane >> 1) & 1)));
                 // Jaccard keys are not affine in the count: every group takes the slow path, where the owners key it.
                 uint32_t slow = jaccard ? (1u << HN / 32) - 1 : 0;   // groups where some owner of the warp may insert
                 if (!jaccard) {
@@ -431,9 +442,13 @@ gemm_topk_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
 #pragma unroll
                         for (int j = 0; j < 32; j++) v[j] = jaccard_negkey(v[j], pq, __shfl_sync(0xffffffffu, s, j), __shfl_sync(0xffffffffu, b, j));
                     }
-                    epilogue_chunk<32>(list, v, false, nullptr, nullptr, (uint32_t)(n0 + h * HN + 32 * g), tail, p.n, staging + lane);
+                    epilogue_chunk<32>(list, v, false, nullptr, nullptr, (uint32_t)(n0 + h * HN + 32 * g), tail, p.n, staging + lane,
+                                       bound);
                     __syncwarp();   // ... and the parked keys are read before the next group is staged
                 }
+                // a full list's k-th key bounds the query's k-th key over all its lists; only finite keys (NaN / inf rows)
+                if (live && list.n == list.k && list.thr_key < bound && fabsf(list.thr_key) <= FLT_MAX)
+                    atomicMin(p.query_bound + q, bound_encode(list.thr_key));
             }
         }
         // publish this lane's per-query partial list

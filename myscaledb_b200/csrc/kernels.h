@@ -90,6 +90,7 @@ struct GemmTopkParams {
     uint32_t *part_ids;
     float *list_keys_gmem;     // scratch for lists that do not fit in shared memory: [W * q_tiles][list_cap_for(k)][128]
     uint32_t *list_ids_gmem;
+    uint32_t *query_bound;     // [nq_pad] 0xffffffff-filled: the best k-th key any list of the query has reached (bound_encode)
     int64_t n;
     int nq_pad, d_pad, k;
     int nq_valid;              // queries actually in the batch (rows past it are padding)

@@ -220,6 +220,19 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *                               for byte.  A negative, >= 1 or non-numeric value is refused at create with B200_ERR_INVALID,
  *                               a non-zero one under L2 with B200_ERR_UNSUPPORTED (the loss is defined for inner-product
  *                               ranking), and d / M > 64 at train with B200_ERR_UNSUPPORTED;
+ *                               "opq=1" (IVFPQ, SCANN and HNSWPQ; other types ignore the key) learns an orthonormal rotation
+ *                               R [d][d] fp32 (y = x.R; Ge et al., optimised PQ) at train, in "opq_iters=N" alternations
+ *                               (default 20, not tuned) of the PQ codebooks of the rotated residuals with an orthogonal
+ *                               Procrustes step, and quantises x.R instead of x: the centroids, codebooks, codes and norm
+ *                               terms live in the rotated space, and the coarse probe and the list scan take the prepared
+ *                               query rotated.  The fp32 rows and every exact path (the second stage, exact_batch=1, the
+ *                               pre-filter, filter_probe's exact rule, small parts) stay unrotated.  R does not change L2,
+ *                               IP or cosine; each query batch pays one d x d product.  It composes with bit_size=4,
+ *                               aq_threshold, keep_raw, refine_factor, filter_probe and both build styles.  opq_iters=0 keeps
+ *                               R = I (still stored and applied).  A part below the inverted-file threshold stays FLAT with
+ *                               no R.  Absent or 0: plain PQ, file byte for byte.  Another value of opq, or opq_iters < 0, is
+ *                               refused at create with B200_ERR_INVALID, opq=1 with d > 4096 (R <= 64 MB) with
+ *                               B200_ERR_UNSUPPORTED.  Saved as B2IX v5 (below);
  *   "MSTG"                      closed source upstream; here the two-stage index of SURVEY 2.5 K6: bf16 lists + exact
  *                               fp32 second stage (supportTwoStageSearch, first_stage_only, computeTopDistanceSubset).
  *                               With "graph_degree=D" it also builds a neighbour graph (as HNSWFLAT below, from each row's
@@ -369,6 +382,12 @@ int b200_index_last_coarse(b200_index *ix, int *path);
  * then after each anisotropic iteration, out_loss[*out_n] (capacity >= *out_n, else B200_ERR_INVALID; null: skipped).
  * B200_ERR_INVALID for an index not trained with the key here (plain PQ, other types, an index loaded from a file). */
 int b200_index_train_loss(const b200_index *ix, double *out_eta, double *out_loss, int capacity, int *out_n);
+/* opq=1 indexes (tests, benchmarks): the rotation R, out_r[d][d] fp32 row-major with y = x.R (null: skipped), and the
+ * training sample's mean PQ loss (mean ||r - r^||^2 of its residuals) at R = I, then after each alternation,
+ * out_loss[*out_n] (capacity >= *out_n, else B200_ERR_INVALID; null: skipped).  An index loaded from a file returns its R
+ * with *out_n = 0.  B200_ERR_INVALID for an index without the key, or one that holds no rotation (not trained, or a part
+ * below the inverted-file threshold, which is FLAT). */
+int b200_index_opq(const b200_index *ix, float *out_r, double *out_loss, int capacity, int *out_n);
 /* computeTopDistanceSubset: exact distances of candidate ids [nq][ncand] (negative = unused) -> top-k */
 int b200_index_refine(b200_index *ix, const float *queries, int64_t nq, const int64_t *cand_ids, int64_t ncand, int k,
                       float *out_dis, int64_t *out_ids);
@@ -391,7 +410,9 @@ int b200_index_last_seeds(b200_index *ix, int64_t *out, int64_t capacity, int *o
  * memory writes the header's has_raw as 2 (every other byte as in HBM placement) and loads them straight into pinned host
  * memory again.  An index with a graph (graph_degree) is written as v4: the v2 layout with the reserved word holding D,
  * followed by the graph [n][D] u32 (HNSWFLAT with has_raw 1, MSTG with has_raw 0, 1 or 2); load checks every graph id
- * (< n or 0xFFFFFFFF; MSTG: a row that is in a list) before any kernel reads it. */
+ * (< n or 0xFFFFFFFF; MSTG: a row that is in a list) before any kernel reads it.  An opq=1 index is written as v5: the v2
+ * layout (reserved word 0) or the v3 one (4-bit codes, reserved word 4), followed by R [d][d] fp32; load accepts it for an
+ * inverted-file IVFPQ / SCANN / HNSWPQ index with d <= 4096 and a finite R orthonormal within 1e-4 (max |R^T R - I|). */
 int b200_index_save(b200_index *ix, const char *path);
 int b200_index_load(const char *path, b200_index **out);
 /* the same through the host's own streams (Search::IndexDataFileWriter / Reader over ClickHouse disks,

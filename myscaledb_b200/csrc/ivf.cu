@@ -36,6 +36,7 @@
 #include "graph.h"
 #include "ivf_aq.h"
 #include "ivf_gemm.h"
+#include "ivf_opq.h"
 #include "kernels.h"
 
 namespace b200 {
@@ -1253,6 +1254,12 @@ struct b200_index {
     // 0: plain PQ.  aq_loss: the training sample's mean loss after the k-means codebooks, then after each iteration.
     double aq_threshold = 0, aq_eta = 0;
     std::vector<double> aq_loss;
+    // opq=1 (PQ types): the rotation R [d][d] fp32, y = x.R (ivf_opq.h).  The centroids, codebooks, codes and norm terms live
+    // in the rotated space, the fp32 rows do not.  opq_loss: the sample's mean PQ loss at R = I, then after each of the
+    // opq_iters alternations (empty on a loaded index).  A part below the inverted-file threshold keeps no R.
+    int opq = 0, opq_iters = 20;
+    float *d_opq = nullptr;
+    std::vector<double> opq_loss;
     int default_nprobe = 32, refine_factor = 4;
     int payload = IVF_PRODUCER_TMA;
     int keep_raw = -1;              // -1 auto (yes), 0 no fp32 rows (first-stage distances only), 1 yes, 2 yes, in host memory
@@ -1292,7 +1299,7 @@ struct b200_index {
     // workspaces (grow-only)
     DevArr w_rows, w_assign_i, w_assign_d, w_u32a, w_u32b, w_u32c, w_u32d, w_cnt, w_plan, w_sort, w_q, w_qraw, w_probe, w_pd, w_items,
         w_qbuf, w_inv, w_ppb, w_pconst, w_qconst, w_qb, w_cs, w_pk, w_pi, w_pw, w_lk, w_li, w_alive, w_od, w_oi, w_cand, w_host_q, w_ppopc, w_lut,
-        w_stage;
+        w_stage, w_qrot;
     // build: one flag per row of the chunk or training sample, 1 = usable (row_usable_kernel)
     DevArr w_usable;
     // filter_probe=1 (per search): list_alive and the filtered lengths [2][nlist], the filtered page table [pages_used], the
@@ -1414,6 +1421,13 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
         if (aq_t > 0 && metric == B200_METRIC_L2)
             return fail(B200_ERR_UNSUPPORTED, "aq_threshold: the anisotropic loss is defined for inner-product ranking (IP, COSINE), not L2");
     }
+    // optimised PQ (the PQ types only; the others ignore the keys): opq=1 learns a rotation in opq_iters alternations
+    const int opq = pq_type ? parse_int_param(params, "opq", 0, true) : 0;
+    const int opq_iters = pq_type ? parse_int_param(params, "opq_iters", 20, true) : 20;
+    if (opq != 0 && opq != 1) return fail(B200_ERR_INVALID, "opq must be 0 (plain PQ) or 1 (optimised PQ), got " + std::to_string(opq));
+    if (opq_iters < 0) return fail(B200_ERR_INVALID, "opq_iters must be >= 0, got " + std::to_string(opq_iters));
+    if (opq && d > kOpqMaxDim)
+        return fail(B200_ERR_UNSUPPORTED, "opq=1: the rotation is d x d fp32, d must be at most " + std::to_string(kOpqMaxDim) + ", got " + std::to_string(d));
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
@@ -1430,6 +1444,8 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
     ix->pq_bits = pq_bits;
     ix->aq_threshold = aq_t;
     ix->aq_eta = (d - 1) * aq_t * aq_t / (1 - aq_t * aq_t);
+    ix->opq = opq;
+    ix->opq_iters = opq_iters;
     ix->default_nprobe = parse_int_param(params, "nprobe", 32);
     // payload of a list row.  The graph types of the reference (hnswlib) and ScaNN have no graph here (ScaNN's anisotropic
     // loss is the opt-in aq_threshold): they are SERVED by the inverted-file engine with the payload their suffix names
@@ -1493,13 +1509,13 @@ extern "C" int b200_index_free(b200_index *ix) {
     for (void *p : {(void *)ix->d_centroids, (void *)ix->d_bcent, (void *)ix->d_cnorm, (void *)ix->d_pq, (void *)ix->d_pq_bf16, (void *)ix->d_sq, ix->d_pool, (void *)ix->d_row_bias,
                     (void *)ix->d_row_ids, (void *)ix->d_list_len, (void *)ix->d_tail_page, (void *)ix->d_page_owner, (void *)ix->d_page_seq,
                     (void *)ix->d_pages_used, (void *)ix->d_flag, (void *)ix->d_list_page_off, (void *)ix->d_list_pages, (void *)ix->d_list_order, (void *)ix->d_graph,
-                    (void *)ix->d_row_slot})
+                    (void *)ix->d_row_slot, (void *)ix->d_opq})
         if (p) cudaFree(p);
     for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_cnt, &ix->w_plan,
                       &ix->w_sort, &ix->w_q, &ix->w_qraw, &ix->w_probe, &ix->w_pd, &ix->w_items, &ix->w_qbuf, &ix->w_inv, &ix->w_ppb, &ix->w_pconst, &ix->w_qb, &ix->w_cs,
                       &ix->w_qconst, &ix->w_pk, &ix->w_pi, &ix->w_pw, &ix->w_lk, &ix->w_li, &ix->w_alive, &ix->w_od, &ix->w_oi, &ix->w_cand,
                       &ix->w_host_q, &ix->w_ppopc, &ix->w_lut, &ix->w_stage, &ix->w_flist, &ix->w_fpages, &ix->w_fsel,
-                      &ix->w_seeds, &ix->w_seedd, &ix->w_usable})
+                      &ix->w_seeds, &ix->w_seedd, &ix->w_usable, &ix->w_qrot})
         a->release();
     if (ix->h_fsel) cudaFreeHost(ix->h_fsel);
     if (ix->ev0) cudaEventDestroy(ix->ev0);
@@ -1565,7 +1581,8 @@ static int host_rows_reserve(b200_index *ix, int64_t rows) {
 
 // k-means on device rows x [n][stride]; centroids written to d_c [nc][d].  Assignment: exact top-1 search of the centroid
 // table with the FLAT engine (tensor cores from 20 rows up) when the table is large, the tiled fp32 kernel otherwise.
-static int kmeans_device(const float *x, int64_t n, int64_t stride, int d, int nc, int iters, float *d_c, cudaStream_t s) {
+// warm: start from the centroids already in d_c (OPQ's alternations) instead of nc evenly strided rows.
+static int kmeans_device(const float *x, int64_t n, int64_t stride, int d, int nc, int iters, float *d_c, cudaStream_t s, bool warm = false) {
     std::vector<int64_t> pick(nc);
     for (int i = 0; i < nc; i++) pick[i] = (int64_t)((double)i * (double)n / (double)nc);
     int64_t *d_pick = nullptr;
@@ -1577,9 +1594,11 @@ static int kmeans_device(const float *x, int64_t n, int64_t stride, int d, int n
     B200_CUDA_OK(cudaMalloc(&d_cn, (size_t)nc * 4));
     B200_CUDA_OK(cudaMalloc(&d_cnt, (size_t)nc * 4));
     B200_CUDA_OK(cudaMalloc(&d_idx, (size_t)n * 4));
-    B200_CUDA_OK(cudaMemcpyAsync(d_pick, pick.data(), (size_t)nc * 8, cudaMemcpyHostToDevice, s));
-    gather_rows_kernel<<<gridsz((int64_t)nc * d), 256, 0, s>>>(x, stride, d_pick, nc, d, d_c);
-    g_launches++;
+    if (!warm) {
+        B200_CUDA_OK(cudaMemcpyAsync(d_pick, pick.data(), (size_t)nc * 8, cudaMemcpyHostToDevice, s));
+        gather_rows_kernel<<<gridsz((int64_t)nc * d), 256, 0, s>>>(x, stride, d_pick, nc, d, d_c);
+        g_launches++;
+    }
     const bool big = (double)n * nc * d > 2e11 && stride == d;   // tensor-core assignment pays from ~0.2 TFLOP per iteration
     b200_corpus *table = nullptr;
     if (big) {
@@ -1832,6 +1851,64 @@ static int train_binary_locked(b200_index *ix, const void *d_rows, int64_t n) {
     return B200_OK;
 }
 
+// opq=1: from the PQ training sample samp [ns][d] (as indexed) and its lists, the OPQ alternations (Ge et al. 2014, the
+// non-parametric solution).  Res = samp - c.  Start: R = I, codebooks by k-means on Res.R (8 iterations, as plain PQ).  Then
+// opq_iters times: R = polar(Res^T Res^) for the decoded codes Res^ of Res.R (the Procrustes step), and a warm-started k-means
+// of 4 iterations per sub-quantiser on the new Res.R (Faiss's count).  ix->opq_loss: the mean ||Res.R - Res^||^2 of the
+// sample at R = I, then after each alternation.  The codebooks of the last alternation are the index's.  Finally the
+// centroids (and the coarse table) and samp are rotated in place: the AQ iterations and the lists work in the rotated space.
+static int opq_train_locked(b200_index *ix, float *samp, int64_t ns, const uint32_t *d_l) {
+    cudaStream_t s = ix->stream;
+    const int d = ix->d, m = ix->m, dsub = ix->dsub, ncw = pq_codewords(ix->pq_bits), nl = ix->nlist;
+    const size_t rows_b = (size_t)ns * d * 4;
+    float *res = nullptr, *resr = nullptr, *xhat = nullptr;
+    double *err = nullptr;
+    int rc = B200_OK;
+    auto cuda_ok = [&](cudaError_t e) {
+        if (e != cudaSuccess && rc == B200_OK) rc = fail(B200_ERR_CUDA, std::string("OPQ training: ") + cudaGetErrorString(e));
+        return rc == B200_OK;
+    };
+    std::vector<double> h_err(ns);
+    auto loss = [&]() {   // encode Res.R with the current codebooks (-> xhat) and append the sample's mean loss
+        if (!cuda_ok(launch_opq_encode(resr, ns, d, m, dsub, ncw, ix->d_pq, xhat, err, s)) ||
+            !cuda_ok(cudaMemcpyAsync(h_err.data(), err, (size_t)ns * 8, cudaMemcpyDeviceToHost, s)) || !cuda_ok(cudaStreamSynchronize(s)))
+            return;
+        double t = 0;
+        for (int64_t r = 0; r < ns; r++) t += h_err[r];
+        ix->opq_loss.push_back(t / (double)std::max<int64_t>(ns, 1));
+    };
+    auto codebooks = [&](int iters, bool warm) {
+        for (int j = 0; j < m && rc == B200_OK; j++) rc = kmeans_device(resr + (size_t)j * dsub, ns, d, dsub, ncw, iters, ix->d_pq + (size_t)j * ncw * dsub, s, warm);
+    };
+    ix->opq_loss.clear();
+    std::vector<float> eye((size_t)d * d, 0.f);
+    for (int i = 0; i < d; i++) eye[(size_t)i * d + i] = 1.f;
+    // resr also takes the rotated centroids at the end: nlist may exceed the sample (ncentroids > 65 536)
+    if (cuda_ok(cudaMalloc(&ix->d_opq, (size_t)d * d * 4)) && cuda_ok(cudaMalloc(&res, rows_b)) &&
+        cuda_ok(cudaMalloc(&resr, (size_t)std::max<int64_t>(ns, nl) * d * 4)) &&
+        cuda_ok(cudaMalloc(&xhat, rows_b)) && cuda_ok(cudaMalloc(&err, (size_t)std::max<int64_t>(ns, 1) * 8)) &&
+        cuda_ok(cudaMemcpyAsync(ix->d_opq, eye.data(), (size_t)d * d * 4, cudaMemcpyHostToDevice, s))) {
+        residual_sub_kernel<<<gridsz(ns * d), 256, 0, s>>>(samp, ns, d, ix->d_centroids, d_l, d, 0, d, res);
+        g_launches++;
+        if (cuda_ok(launch_opq_rotate(res, d, ns, d, ix->d_opq, resr, d, s))) codebooks(8, false);
+        if (rc == B200_OK) loss();
+        for (int it = 0; it < ix->opq_iters && rc == B200_OK; it++) {
+            rc = opq_procrustes(res, xhat, ns, d, ix->d_opq, s);
+            if (rc == B200_OK && cuda_ok(launch_opq_rotate(res, d, ns, d, ix->d_opq, resr, d, s))) codebooks(4, true);
+            if (rc == B200_OK) loss();
+        }
+        // the centroids and the sample into the rotated space (resr and res are free now)
+        if (rc == B200_OK && cuda_ok(launch_opq_rotate(ix->d_centroids, d, nl, d, ix->d_opq, resr, d, s)) &&
+            cuda_ok(cudaMemcpyAsync(ix->d_centroids, resr, (size_t)nl * d * 4, cudaMemcpyDeviceToDevice, s)) &&
+            cuda_ok(launch_opq_rotate(samp, d, ns, d, ix->d_opq, res, d, s)) && cuda_ok(cudaMemcpyAsync(samp, res, rows_b, cudaMemcpyDeviceToDevice, s)))
+            rc = upload_coarse(ix, s);
+        cuda_ok(cudaStreamSynchronize(s));
+    }
+    for (void *p : {(void *)res, (void *)resr, (void *)xhat, (void *)err})
+        if (p) cudaFree(p);
+    return rc;
+}
+
 // Search::VectorIndex::train: coarse quantiser (+ PQ codebooks / SQ ranges) from a sample already on the device,
 // rows fp32 [n][d] contiguous.  Decides FLAT fallback for small parts (the reference's fallback_to_flat, test 00029).
 static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
@@ -1976,14 +2053,19 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
             cudaMemsetAsync(d_c32, 0, (size_t)nl * 4, s);
             assign_to_u32_kernel<<<(unsigned)ceil_div(ns, 256), 256, 0, s>>>(d_a, ns, nullptr, 0u, d_l, d_c32);
             g_launches++;
-            for (int j = 0; j < m && rc == B200_OK; j++) {
-                residual_sub_kernel<<<gridsz(ns * dsub), 256, 0, s>>>(d_samp, ns, d, ix->d_centroids, d_l, d, j, dsub, d_res);
-                g_launches++;
-                rc = kmeans_device(d_res, ns, dsub, dsub, ncw, 8, ix->d_pq + (size_t)j * ncw * dsub, s);
+            if (ix->opq) {
+                rc = opq_train_locked(ix, d_samp, ns, d_l);   // R, the rotated centroids and sample, the codebooks
+            } else {
+                for (int j = 0; j < m && rc == B200_OK; j++) {
+                    residual_sub_kernel<<<gridsz(ns * dsub), 256, 0, s>>>(d_samp, ns, d, ix->d_centroids, d_l, d, j, dsub, d_res);
+                    g_launches++;
+                    rc = kmeans_device(d_res, ns, dsub, dsub, ncw, 8, ix->d_pq + (size_t)j * ncw * dsub, s);
+                }
             }
         }
         if (rc == B200_OK && ix->aq_threshold > 0) {
-            // anisotropic iterations on the same sample, from the k-means codebooks (ivf_aq.cu)
+            // anisotropic iterations on the same sample, from the k-means codebooks (ivf_aq.cu); with opq=1 the sample and the
+            // centroids are the rotated ones (the loss does not change under a rotation)
             const AqTrain at{d_samp, ns, d, m, dsub, ncw, d_l, ix->d_centroids, ix->d_pq, ix->aq_eta};
             ix->aq_loss.clear();
             rc = aq_train_codebooks(at, &ix->aq_loss, s);
@@ -2058,6 +2140,11 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     if (!ix->use_ivf) {
         ix->n += n;
         return B200_OK;
+    }
+    if (ix->d_opq) {   // opq=1: the assignment, the codes and the norm terms come from x.R; the fp32 rows above stay as given
+        B200_TRY(ix->w_qrot.reserve((size_t)n * d * 4));
+        B200_CUDA_OK(launch_opq_rotate(x, d, n, d, ix->d_opq, ix->w_qrot.as<float>(), d, s));
+        x = ix->w_qrot.as<float>();
     }
     // ---- assign -> (list, row) sorted by list
     B200_TRY(ix->w_assign_i.reserve((size_t)n * 8));
@@ -2346,7 +2433,7 @@ static int finalize_locked(b200_index *ix) {
         for (int l = 0; l < nl; l++) ix->max_list_pages = std::max<uint32_t>(ix->max_list_pages, (ix->list_len[l] + kPageRows - 1) / kPageRows);
     }
     // build scratch is not needed any more
-    for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_plan, &ix->w_host_q, &ix->w_usable})
+    for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_plan, &ix->w_host_q, &ix->w_usable, &ix->w_qrot})
         a->release();
     if (!ix->raw) {  // an index without a single row still answers (empty results)
         const int raw_metric = ix->metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
@@ -2407,6 +2494,7 @@ extern "C" int b200_index_memory_bytes(const b200_index *ix, uint64_t *out_bytes
              (uint64_t)ix->pool_pages * 12;
         if (ix->d_pq) b += (uint64_t)ix->m * pq_codewords(ix->pq_bits) * ix->dsub * (ix->d_pq_bf16 ? 6 : 4);   // fp32 codebook (+ the decoder's bf16 copy)
     }
+    if (ix->d_opq) b += (uint64_t)ix->d * ix->d * 4;
     if (ix->d_graph) b += (uint64_t)ix->n * ix->graph_degree * 4;
     if (ix->d_row_slot) b += (uint64_t)ix->n * 4;
     *out_bytes = b;
@@ -2634,9 +2722,10 @@ static uint32_t pages_per_chunk(const b200_index *ix, int64_t n_valid, int force
 }
 
 // The steps of a list search after the coarse probe, asynchronous on s: pairs sorted by list, plan, query gather, grouped
-// scan, per-query merge, exact second stage.  probe: [nq][nprobe] list ids (negative = an invalid slot, skipped by every
+// scan, per-query merge, exact second stage.  d_q: the first stage's queries [nq][d_pad] (opq=1: rotated), d_qx: the
+// prepared queries of the exact second stage.  probe: [nq][nprobe] list ids (negative = an invalid slot, skipped by every
 // step).  n_valid: the count of valid slots, sizing the gathered query rows, the work items and the partial lists.  list_len / list_pages: the index's own, or the filtered ones of filter_probe=1.
-static int scan_probes(b200_index *ix, const float *d_q, const float *d_queries, int64_t nq, int k, int k1, bool two_stage, const char *params,
+static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, const float *d_queries, int64_t nq, int k, int k1, bool two_stage, const char *params,
                        const int64_t *probe, int nprobe, int64_t n_valid, const uint32_t *list_len, const uint32_t *list_pages,
                        const uint8_t *d_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
     const int nl = ix->nlist;
@@ -2857,7 +2946,7 @@ static int scan_probes(b200_index *ix, const float *d_q, const float *d_queries,
         B200_CUDA_OK(cudaGetLastError());
     }
     if (ix->timing) cudaEventRecord(ix->ev_ph[4], s);
-    if (two_stage) B200_TRY(refine_device(ix, d_q, nq, m_ids, k1, k, id_offset, d_out_dis, d_out_ids, s));
+    if (two_stage) B200_TRY(refine_device(ix, d_qx, nq, m_ids, k1, k, id_offset, d_out_dis, d_out_ids, s));
     if (ix->timing) cudaEventRecord(ix->ev_ph[5], s);
     return B200_OK;
 }
@@ -2878,7 +2967,7 @@ constexpr double kFilterProbeExactFactor = 16.0;
 // the live lists) and a stream synchronise; then the probe rows [nq][P] of the live lists, P = max live lists, and the rest of
 // the search with nprobe := P, its buffers sized by the live lists.  Leaving out a list without a kept row changes no answer:
 // it holds no candidate and the merge does not depend on the order of its inputs.
-static int filter_probe_search(b200_index *ix, const float *d_q, int64_t nq, int k, int k1, bool two_stage, const char *params, int nprobe,
+static int filter_probe_search(b200_index *ix, const float *d_q, const float *d_qx, int64_t nq, int k, int k1, bool two_stage, const char *params, int nprobe,
                                const uint32_t *list_len, const uint32_t *list_pages, const uint8_t *d_alive, int64_t id_offset, float *d_out_dis,
                                int64_t *d_out_ids, cudaStream_t s) {
     const int nl = ix->nlist;
@@ -2961,7 +3050,7 @@ static int filter_probe_search(b200_index *ix, const float *d_q, int64_t nq, int
             g_launches++;
             q0 = q1;
         }
-        B200_TRY(scan_probes(ix, d_q + a * ix->d_pad, nullptr, b - a, k, k1, two_stage, params, ix->w_probe.as<int64_t>(), P, ranges[r].second,
+        B200_TRY(scan_probes(ix, d_q + a * ix->d_pad, d_qx + a * ix->d_pad, nullptr, b - a, k, k1, two_stage, params, ix->w_probe.as<int64_t>(), P, ranges[r].second,
                              list_len, list_pages, d_alive, id_offset, d_out_dis + a * k, d_out_ids + a * k, s));
         items += ix->last_items;
         if (split) {   // b200_index_last_scan reports the rows of the whole batch
@@ -3163,6 +3252,13 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     if (!fselect) ix->last_probe.insert(ix->last_probe.end(), nq, nprobe);
 
     if (ix->timing) cudaEventRecord(ix->ev_ph[0], s);
+    // opq=1: the coarse probe and the list scan take the rotated queries; the exact second stage keeps the prepared ones
+    const float *d_qx = d_q;
+    if (ix->d_opq) {
+        B200_TRY(ix->w_qrot.reserve((size_t)nq * ix->d_pad * 4));
+        B200_CUDA_OK(launch_opq_rotate(d_qx, ix->d_pad, nq, ix->d, ix->d_opq, ix->w_qrot.as<float>(), ix->d_pad, s));
+        d_q = ix->w_qrot.as<float>();
+    }
     const uint32_t *list_len = ix->d_list_len, *list_pages = ix->d_list_pages;
     if (fprobe) {
         B200_TRY(ix->w_flist.reserve((size_t)nl * 8));
@@ -3173,7 +3269,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         list_len = ix->w_flist.as<uint32_t>() + nl;
         list_pages = ix->w_fpages.as<uint32_t>();
         if (fselect)
-            return filter_probe_search(ix, d_q, nq, k, k1, two_stage, params, nprobe, list_len, list_pages, d_alive, id_offset, d_out_dis, d_out_ids, s);
+            return filter_probe_search(ix, d_q, d_qx, nq, k, k1, two_stage, params, nprobe, list_len, list_pages, d_alive, id_offset, d_out_dis, d_out_ids, s);
     }
     // ---- coarse probe: nprobe nearest centroids per query (exact FLAT search of the centroid table)
     B200_TRY(ix->w_probe.reserve((size_t)n_pairs * 8));
@@ -3230,7 +3326,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     }
 
     if (ix->timing) cudaEventRecord(ix->ev_ph[1], s);
-    return scan_probes(ix, d_q, d_queries, nq, k, k1, two_stage, params, ix->w_probe.as<int64_t>(), nprobe, n_pairs, list_len, list_pages, d_alive,
+    return scan_probes(ix, d_q, d_qx, d_queries, nq, k, k1, two_stage, params, ix->w_probe.as<int64_t>(), nprobe, n_pairs, list_len, list_pages, d_alive,
                        id_offset, d_out_dis, d_out_ids, s);
 }
 
@@ -3309,6 +3405,21 @@ extern "C" int b200_index_train_loss(const b200_index *ix, double *out_eta, doub
     if (out_loss && capacity < n) return fail(B200_ERR_INVALID, "train_loss: capacity " + std::to_string(capacity) + " < " + std::to_string(n));
     if (out_eta) *out_eta = ix->aq_eta;
     if (out_loss) std::copy(ix->aq_loss.begin(), ix->aq_loss.end(), out_loss);
+    if (out_n) *out_n = n;
+    return B200_OK;
+}
+
+extern "C" int b200_index_opq(const b200_index *ix, float *out_r, double *out_loss, int capacity, int *out_n) {
+    if (!ix) return fail(B200_ERR_INVALID, "bad arguments");
+    if (!ix->opq) return fail(B200_ERR_INVALID, "this index was not created with opq=1");
+    if (!ix->d_opq) return fail(B200_ERR_INVALID, "this index holds no rotation (not trained yet, or a part below the inverted-file threshold: FLAT)");
+    const int n = (int)ix->opq_loss.size();
+    if (out_loss && capacity < n) return fail(B200_ERR_INVALID, "opq: capacity " + std::to_string(capacity) + " < " + std::to_string(n));
+    if (out_r) {
+        B200_CUDA_OK(cudaSetDevice(ix->device));
+        B200_CUDA_OK(cudaMemcpy(out_r, ix->d_opq, (size_t)ix->d * ix->d * 4, cudaMemcpyDeviceToHost));
+    }
+    if (out_loss) std::copy(ix->opq_loss.begin(), ix->opq_loss.end(), out_loss);
     if (out_n) *out_n = n;
     return B200_OK;
 }
@@ -3422,8 +3533,9 @@ static int index_save_io(b200_index *ix, Io *f) {
     memcpy(h.magic, "B2IX", 4);
     // v3: the v2 layout with reserved0 = the PQ code width (4) and a [m][16][dsub] codebook; every other index stays v2
     // v4: the v2 layout with reserved0 = the graph degree D, followed by the graph [n][D] u32 (graph_degree indexes)
+    // v5: an opq=1 index: the v2 layout (reserved0 = 0) or the v3 one (reserved0 = 4), followed by R [d][d] fp32
     const bool pq4 = pq_uses_lut(ix) && ix->pq_bits == 4;
-    h.version = pq4 ? 3 : ix->d_graph ? 4 : 2;
+    h.version = ix->d_opq ? 5 : pq4 ? 3 : ix->d_graph ? 4 : 2;
     h.reserved0 = pq4 ? 4 : ix->d_graph ? (uint32_t)ix->graph_degree : 0;
     h.type = ix->type; h.metric = ix->metric; h.d = ix->d; h.nlist = ix->nlist; h.m = ix->m; h.dsub = ix->dsub;
     // has_raw 2: the same rows, to be loaded into host memory (keep_raw=2 placement)
@@ -3473,6 +3585,10 @@ static int index_save_io(b200_index *ix, Io *f) {
                 if (ok && ix->d_row_bias) ok = dump(ix->d_row_bias + row0, kPageRows * 4);
             }
         }
+        if (ok && ix->d_opq) {
+            std::vector<float> r((size_t)ix->d * ix->d);
+            ok = cudaMemcpy(r.data(), ix->d_opq, r.size() * 4, cudaMemcpyDeviceToHost) == cudaSuccess && wr(f, r.data(), r.size() * 4);
+        }
         if (ok && ix->d_graph) {
             const size_t rb = (size_t)ix->graph_degree * 4;
             const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / (int64_t)rb);
@@ -3512,16 +3628,21 @@ extern "C" int b200_index_save_cb(b200_index *ix, int (*write)(void *ctx, const 
 static int index_load_io(Io *f, b200_index **out) {
     *out = nullptr;
     IxHeader h{};
-    if (!rd(f, &h, sizeof(h)) || memcmp(h.magic, "B2IX", 4) != 0 || (h.version != 2 && h.version != 3 && h.version != 4))
-        return fail(B200_ERR_INVALID, "not a B2IX v2 / v3 / v4 index file");
+    if (!rd(f, &h, sizeof(h)) || memcmp(h.magic, "B2IX", 4) != 0 || h.version < 2 || h.version > 5)
+        return fail(B200_ERR_INVALID, "not a B2IX v2 / v3 / v4 / v5 index file");
     // a truncated or corrupt file must fail here, not in a kernel: every size below is derived from these fields
     const bool bin = h.type >= IDX_BINFLAT;
     // v3: an inverted-file PQ index with 4-bit codes (reserved0 = 4), nibble-packed code rows and a [m][16][dsub] codebook
-    const int pq_bits = h.version == 3 ? 4 : 8;
-    if (h.version == 3 &&
+    // v5: an opq=1 PQ index (IVFPQ, SCANN, HNSWPQ; d <= kOpqMaxDim) with v3's reserved0 (4: 4-bit codes, 0: 8-bit)
+    if (h.version == 5 && !(h.payload == IVF_PRODUCER_PQ && h.use_ivf && (h.type == IDX_IVFPQ || h.type == IDX_SCANN || h.type == IDX_HNSWPQ) &&
+                            h.d > 0 && h.d <= kOpqMaxDim && (h.reserved0 == 0 || h.reserved0 == 4)))
+        return fail(B200_ERR_INVALID, "corrupt index header (v5: an inverted-file IVFPQ / SCANN / HNSWPQ index with d <= " + std::to_string(kOpqMaxDim) +
+                                          " and reserved0 0 or 4 expected)");
+    const int pq_bits = h.version == 3 || (h.version == 5 && h.reserved0 == 4) ? 4 : 8;
+    if (pq_bits == 4 &&
         !(h.reserved0 == 4 && h.payload == IVF_PRODUCER_PQ && h.use_ivf && h.m > 0 && h.dsub > 0 && (int64_t)h.m * h.dsub == h.d &&
           h.code_bytes >= pq_code_bytes(h.m, 4) && h.code_bytes % 16 == 0 && ivf_pq4_fits(h.m)))
-        return fail(B200_ERR_INVALID, "corrupt index header (v3: 4-bit PQ with M <= " + std::to_string(ivf_pq4_max_m()) + " expected)");
+        return fail(B200_ERR_INVALID, "corrupt index header (4-bit PQ with M <= " + std::to_string(ivf_pq4_max_m()) + " expected)");
     // v4: an inverted-file index with a graph of degree reserved0: HNSWFLAT with its fp32 rows in HBM, or MSTG with any rows
     if (h.version == 4 && !(graph_degree_ok((int)h.reserved0) && h.use_ivf &&
                             ((h.type == IDX_HNSWFLAT && h.has_raw == 1) || (h.type == IDX_MSTG && h.payload == IVF_PRODUCER_TMA))))
@@ -3654,6 +3775,19 @@ static int index_load_io(Io *f, b200_index **out) {
             cudaMemset(ix->d_flag, 0, 32);
             if ((bin ? upload_coarse_bin(ix, ix->stream) : upload_coarse(ix, ix->stream)) != B200_OK) return bail(b200_last_error());
             if (cudaStreamSynchronize(ix->stream) != cudaSuccess) return bail("upload failed");
+        }
+        if (h.version == 5) {   // R: finite and orthonormal before any row or query is rotated by it
+            std::vector<float> r((size_t)h.d * h.d);
+            if (!rd(f, r.data(), r.size() * 4)) return bail("truncated index file (OPQ rotation)");
+            for (float v : r)
+                if (!std::isfinite(v)) return bail("corrupt index file (OPQ rotation not finite)");
+            double err = 0;
+            if (cudaMalloc(&ix->d_opq, r.size() * 4) != cudaSuccess ||
+                cudaMemcpy(ix->d_opq, r.data(), r.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+                opq_orthonormal_error(ix->d_opq, h.d, &err, ix->stream) != B200_OK)
+                return bail(std::string("OPQ rotation upload: ") + b200_last_error());
+            if (!(err <= kOpqLoadTol)) return bail("corrupt index file (OPQ rotation not orthonormal: max |R^T R - I| = " + std::to_string(err) + ")");
+            ix->opq = 1;
         }
         if (h.version == 4) {   // every id < n or 0xFFFFFFFF before a kernel walks the graph; MSTG: every id in a list (it has a pool slot)
             const int D = (int)h.reserved0;

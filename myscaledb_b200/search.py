@@ -505,6 +505,16 @@ class VectorIndex:
         _check(lib().b200_index_train_loss(self._h, C.byref(eta), _p(out, C.c_double), C.c_int(n.value), C.byref(n)))
         return eta.value, out
 
+    def opq(self):
+        """opq=1 indexes: (R float32 [d][d], y = x.R; float64 [1 + opq_iters] mean PQ loss of the training sample at R = I,
+        then after each alternation; empty for a loaded index).  B200Error for an index without the key or without a rotation."""
+        n = C.c_int()
+        _check(lib().b200_index_opq(self._h, None, None, C.c_int(0), C.byref(n)))
+        r = np.zeros((self.d, self.d), np.float32)
+        loss = np.zeros(n.value, np.float64)
+        _check(lib().b200_index_opq(self._h, _p(r, C.c_float), _p(loss, C.c_double), C.c_int(n.value), C.byref(n)))
+        return r, loss
+
     def phase_ms(self):
         a = (C.c_double * 5)()
         _check(lib().b200_index_phase_ms(self._h, a))

@@ -253,7 +253,8 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *                               per iteration by a cluster of W CTAs per query, for single queries and small batches; the
  *                               same scores, so the answer of W = 1 is the default's byte for byte; another W on a search
  *                               that would walk the graph: B200_ERR_INVALID, checked before the filtered exact rule as
- *                               ef_s is; ignored with graph=0, exact_batch=1 or no graph; it applies to MSTG's walk too).  Any type but HNSWFLAT / MSTG with graph_degree > 0, or HNSWFLAT
+ *                               ef_s is; ignored with graph=0, exact_batch=1 or no graph; it applies to MSTG's and
+ *                               BINARYMSTG's walks too).  Any type but HNSWFLAT / MSTG / BINARYMSTG with graph_degree > 0, or HNSWFLAT
  *                               with keep_raw=0 / 2 and it: B200_ERR_UNSUPPORTED; another D: B200_ERR_INVALID.  A part
  *                               below the threshold has no graph;
  *   "BINARYFLAT"                binary rows (metric HAMMING or JACCARD, d in bits: a multiple of 8, at most 65536), exact
@@ -262,7 +263,16 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *                               Jaccard too), scanned on the tensor cores (wgmma .b1 AND + popcount); list rows are exact,
  *                               so every returned distance is exact and nprobe >= nlist returns the BINARYFLAT answer
  *                               byte for byte.  nprobe must be <= 1024 unless it is >= nlist (B200_ERR_UNSUPPORTED);
- *   "BINARYHNSW", "BINARYMSTG"  accepted and served by the BINARYIVF engine (no graph; same recall contract as HNSW*).
+ *   "BINARYHNSW", "BINARYMSTG"  accepted and served by the BINARYIVF engine (same recall contract as HNSW*).  BINARYHNSW has
+ *                               no graph.  BINARYMSTG with "graph_degree=D" (16, 32 or 64; another D: B200_ERR_INVALID)
+ *                               also builds a neighbour graph as MSTG does, from each row's 2D + 1 nearest by its own list
+ *                               search (exact, "graph=0" at the default nprobe, queried with the row bytes read back from
+ *                               the pages), and walks it by default over its binary list rows in HBM with ef_s,
+ *                               search_width, graph=0 and the k <= 1024 limit as HNSWFLAT.  Every key of the walk is the
+ *                               exact Hamming / Jaccard distance BINARYFLAT returns for that (query, row), so there is no
+ *                               second stage (out_num_candidates = k).  Under a filter the walk always answers (a binary
+ *                               inverted-file index keeps no exact corpus) and may return fewer than k rows;
+ *                               "graph=0,nprobe=<nlist>" is the exact complete answer.
  * Binary types take only HAMMING / JACCARD and float types only L2 / IP / COSINE (else B200_ERR_INVALID).  For a binary
  * index every `rows` / `queries` pointer below (build, train, add, search and their _device forms) carries bytes
  * [n][d / 8] behind the `const float *` type, the convention of the binary corpora.  Binary indexes have no second stage:
@@ -308,7 +318,7 @@ int b200_topk_merge_device_ex(const float *d_dis, const int64_t *d_ids, int n_li
  *   Cosine: rows and queries whose sum of squares is below FLT_EPSILON are usable and stay as given (no normalisation); their
  *     key is 1 - <q, x>.
  *   Files: the format is unchanged; the list lengths may add up to less than n (load refuses more than n).  A row in no list
- *     has an empty adjacency row in a v4 graph, and load refuses an MSTG graph edge to such a row.
+ *     has an empty adjacency row in a v4 graph, and load refuses an MSTG or BINARYMSTG graph edge to such a row.
  * ---------------------------------------------------------------------------------- */
 /* Widest float index with inverted lists (every float type but FLAT, which keeps no limit below the loader's 65536;
  * binary types take up to 65536 bits): create refuses a wider d with B200_ERR_UNSUPPORTED, and so does load for a wider
@@ -409,8 +419,8 @@ int b200_index_last_seeds(b200_index *ix, int64_t *out, int64_t capacity, int *o
  * index is written as v2.  load accepts both and validates every size it derives.  An index with its fp32 rows in host
  * memory writes the header's has_raw as 2 (every other byte as in HBM placement) and loads them straight into pinned host
  * memory again.  An index with a graph (graph_degree) is written as v4: the v2 layout with the reserved word holding D,
- * followed by the graph [n][D] u32 (HNSWFLAT with has_raw 1, MSTG with has_raw 0, 1 or 2); load checks every graph id
- * (< n or 0xFFFFFFFF; MSTG: a row that is in a list) before any kernel reads it.  An opq=1 index is written as v5: the v2
+ * followed by the graph [n][D] u32 (HNSWFLAT with has_raw 1, MSTG with has_raw 0, 1 or 2, BINARYMSTG); load checks every
+ * graph id (< n or 0xFFFFFFFF; MSTG, BINARYMSTG: a row that is in a list) before any kernel reads it.  An opq=1 index is written as v5: the v2
  * layout (reserved word 0) or the v3 one (4-bit codes, reserved word 4), followed by R [d][d] fp32; load accepts it for an
  * inverted-file IVFPQ / SCANN / HNSWPQ index with d <= 4096 and a finite R orthonormal within 1e-4 (max |R^T R - I|). */
 int b200_index_save(b200_index *ix, const char *path);

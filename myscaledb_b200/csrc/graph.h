@@ -1,6 +1,6 @@
-// graph.h -- fixed-degree neighbour graph of an HNSWFLAT or MSTG index (graph_degree=D): build steps and the graph search, one
-// CTA per query or one W-CTA cluster per query (search_width=W) (graph_sm90.cu).  The host side (candidates from the index's
-// own list search, persistence, the search entry) lives in ivf.cu.
+// graph.h -- fixed-degree neighbour graph of an HNSWFLAT, MSTG or BINARYMSTG index (graph_degree=D): build steps and the graph
+// search, one CTA per query or one W-CTA cluster per query (search_width=W) (graph_sm90.cu).  The host side (candidates from
+// the index's own list search, persistence, the search entry) lives in ivf.cu.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,6 +43,10 @@ int graph_row_slots(const uint32_t *d_list_len, const uint32_t *d_list_page_off,
 // out [m][d] fp32 = the bf16 page rows of ids row0 .. row0 + m - 1 (pool: [page][d_pad64 / 64][256][64] bf16); zeros for a row
 // in no list
 int graph_page_rows(const void *d_pool, const uint32_t *d_row_slot, int64_t row0, int64_t m, int d, int d_pad64, float *d_out, cudaStream_t s);
+// out [m][row_bytes] bytes = the binary page rows of ids row0 .. row0 + m - 1 (pool: [page][row_pad / kb_w][256][kb_w] bytes);
+// zeros for a row in no list
+int graph_bin_page_rows(const void *d_pool, const uint32_t *d_row_slot, int64_t row0, int64_t m, int row_bytes, int row_pad, int kb_w, uint8_t *d_out,
+                        cudaStream_t s);
 
 struct GraphSearchParams {
     const float *queries;      // [nq][d_pad], prepared (cosine: unit)
@@ -60,11 +64,23 @@ struct GraphSearchParams {
     int l2;                    // else inner product (distance -key)
 };
 
-// dynamic shared memory of each CTA of a query; q_len = d_pad (fp32 rows) or d_pad64 (bf16 pages)
+// BINARYMSTG: the walk over the binary list pages.  g.pages is the pool [page][row_pad / kb_w][256][kb_w] bytes, g.row_slot
+// row v's slot in it, g.queries unused, g.l2 = 1 (the key is the distance), g.d_pad / g.d_pad64 unused.
+struct GraphB1Params {
+    GraphSearchParams g;
+    const uint8_t *queries;    // [nq][row_bytes]
+    const float *row_popc;     // [pool rows] popcount of the row at a slot (an exact float)
+    int row_bytes, row_pad, kb_w;
+    int jaccard;               // else Hamming
+};
+
+// dynamic shared memory of each CTA of a query; q_len = d_pad (fp32 rows), d_pad64 (bf16 pages) or row_pad / 4 (binary pages)
 size_t graph_search_smem(int q_len, int ef, int k, bool filtered, int width);
 // graph_search_kernel over the fp32 rows, or graph_search_bf16_kernel when p.pages is set; at width = W > 1 (W parents per
 // iteration, graph_width_ok) their cluster forms, nq x W CTAs in clusters of W.  B200_ERR_UNSUPPORTED when the shared memory
 // does not fit or a cluster cannot be resident.
 int graph_search(const GraphSearchParams &p, int64_t nq, int width, cudaStream_t s);
+// graph_search_b1_kernel over the binary list pages (BINARYMSTG), or its cluster forms at width = W > 1; errors as graph_search
+int graph_search_b1(const GraphB1Params &p, int64_t nq, int width, cudaStream_t s);
 
 }  // namespace b200

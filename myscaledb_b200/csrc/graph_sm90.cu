@@ -1,6 +1,7 @@
-// graph_sm90.cu -- the neighbour graph of an HNSWFLAT or MSTG index (graph_degree=D): candidate lists -> rank-based pruning ->
-// reverse edges and merge at build, and the graph search over fp32 rows (HNSWFLAT) or the bf16 list pages (MSTG), one CTA per
-// query or, at search_width=W > 1, one cluster of W CTAs per query that expands W parents per iteration (DESIGN §3).
+// graph_sm90.cu -- the neighbour graph of an HNSWFLAT, MSTG or BINARYMSTG index (graph_degree=D): candidate lists -> rank-based
+// pruning -> reverse edges and merge at build, and the graph search over fp32 rows (HNSWFLAT), the bf16 list pages (MSTG) or the
+// binary list pages (BINARYMSTG), one CTA per query or, at search_width=W > 1, one cluster of W CTAs per query that expands W
+// parents per iteration (DESIGN §3).
 #include <cooperative_groups.h>
 #include <cub/cub.cuh>
 
@@ -236,6 +237,27 @@ int graph_page_rows(const void *d_pool, const uint32_t *d_row_slot, int64_t row0
     return B200_OK;
 }
 
+// rows [m][row_bytes] = the binary page rows of ids row0 .. row0 + m - 1 (the graph build's queries of a BINARYMSTG index)
+__global__ void bin_page_rows_kernel(const uint8_t *__restrict__ pool, const uint32_t *__restrict__ row_slot, int64_t row0, int64_t m, int row_bytes,
+                                     int row_pad, int kb_w, uint8_t *__restrict__ out) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= m * row_bytes) return;
+    const int64_t i = e / row_bytes;
+    const int j = (int)(e - i * row_bytes);
+    const uint32_t slot = row_slot[row0 + i];
+    out[e] = slot == kNoId ? 0 : pool[(((size_t)(slot / kPageRows) * (row_pad / kb_w) + j / kb_w) * kPageRows + slot % kPageRows) * kb_w + j % kb_w];
+}
+
+int graph_bin_page_rows(const void *d_pool, const uint32_t *d_row_slot, int64_t row0, int64_t m, int row_bytes, int row_pad, int kb_w, uint8_t *d_out,
+                        cudaStream_t s) {
+    if (m == 0) return B200_OK;
+    bin_page_rows_kernel<<<(unsigned)ceil_div(m * row_bytes, 256), 256, 0, s>>>(static_cast<const uint8_t *>(d_pool), d_row_slot, row0, m, row_bytes,
+                                                                                 row_pad, kb_w, d_out);
+    g_launches++;
+    B200_CUDA_OK(cudaGetLastError());
+    return B200_OK;
+}
+
 // ------------------------------------------------------------------------------------
 // search: one CTA per query (W = 1), or one cluster of W CTAs per query (search_width=W)
 // ------------------------------------------------------------------------------------
@@ -354,8 +376,8 @@ __device__ __forceinline__ int cta_count_flags(bool flag, int *scratch, int *bel
 // into the visited table; a warp per row scores them (`score`: 128-bit loads, fp32, fixed lane order); they are sorted by
 // (key, id) and rank-merged into the ef list (and, those the bitmap keeps, into the alive list).  Every answer-bearing step is
 // a sort or a merge by (key, id): the result does not depend on thread timing.  q_len: the query's floats in shared memory
-// (>= d_pad, zero beyond it), dim i at qs[qpos(i)]; score(id, qs, lane) returns, on every lane, the warp's L2 distance or inner
-// product of row id.
+// (>= d_pad, zero beyond it) as stage(qs, q, i) writes them, one 4-byte word i per call; score(id, qs, lane) returns, on every
+// lane, the warp's L2 distance or inner product of row id (binary rows: their distance).
 //
 // W > 1 (search_width=W): the W CTAs of a cluster walk one query, each holding the same copy of the lists and the visited
 // table.  An iteration takes the first W unexpanded entries; CTA r loads the row of parent r into its nb (phase A), cluster
@@ -367,8 +389,8 @@ __device__ __forceinline__ int cta_count_flags(bool flag, int *scratch, int *bel
 // in phase A (read by others in phase B, before barrier 2) and pk / pi / sh[0] only in phase B (read in phase C, before the
 // next barrier 1).  Every barrier sits on control flow that depends on the shared state alone, so all CTAs reach it; a last
 // one keeps every CTA's shared memory until no other reads it.  CTA 0 writes the answer.
-template <int W, class QPos, class Score>
-__device__ __forceinline__ void graph_walk(const GraphSearchParams &p, int q_len, QPos qpos, Score score) {
+template <int W, class Stage, class Score>
+__device__ __forceinline__ void graph_walk(const GraphSearchParams &p, int q_len, Stage stage, Score score) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const bool filtered = p.alive != nullptr;
     const GraphSmem L = graph_smem_layout(q_len, p.ef, p.k, filtered, W);
@@ -399,7 +421,7 @@ __device__ __forceinline__ void graph_walk(const GraphSearchParams &p, int q_len
     int rank = 0;
     if constexpr (W > 1) rank = (int)cg::this_cluster().block_rank();
     const int nwarps = kGraphThreads / 32;
-    for (int i = tid; i < q_len; i += kGraphThreads) qs[qpos(i)] = i < p.d_pad ? p.queries[q * p.d_pad + i] : 0.f;
+    for (int i = tid; i < q_len; i += kGraphThreads) stage(qs, q, i);
     for (int i = tid; i < kGraphVisitedSlots; i += kGraphThreads) vis[i] = kNoId;
     if (rank == 0)   // the seeds are the row of rank 0 in the first step
         for (int j = tid; j < p.nseeds; j += kGraphThreads) {
@@ -609,7 +631,8 @@ __device__ __forceinline__ void graph_walk(const GraphSearchParams &p, int q_len
 // HNSWFLAT: rows scored from the fp32 rows in HBM
 template <int W>
 __device__ __forceinline__ void graph_walk_fp32(const GraphSearchParams &p) {
-    graph_walk<W>(p, p.d_pad, [](int i) { return i; }, [&](uint32_t v, const float *qs, int lane) {
+    const auto stage = [&](float *qs, int64_t q, int i) { qs[i] = i < p.d_pad ? p.queries[q * p.d_pad + i] : 0.f; };
+    graph_walk<W>(p, p.d_pad, stage, [&](uint32_t v, const float *qs, int lane) {
         const float4 *row = reinterpret_cast<const float4 *>(p.rows + (size_t)v * p.d_pad);
         const float4 *x4 = reinterpret_cast<const float4 *>(qs);
         float acc = 0.f;
@@ -651,7 +674,8 @@ __device__ __forceinline__ float bf16x2_term(int l2, uint32_t u, float x0, float
 template <int W>
 __device__ __forceinline__ void graph_walk_bf16(const GraphSearchParams &p) {
     const auto qpos = [](int i) { return (i & ~63) | ((i >> 2) & 1) << 5 | ((i >> 3) & 7) << 2 | (i & 3); };
-    graph_walk<W>(p, p.d_pad64, qpos, [&](uint32_t v, const float *qs, int lane) {
+    const auto stage = [&](float *qs, int64_t q, int i) { qs[qpos(i)] = i < p.d_pad ? p.queries[q * p.d_pad + i] : 0.f; };
+    graph_walk<W>(p, p.d_pad64, stage, [&](uint32_t v, const float *qs, int lane) {
         const uint32_t slot = p.row_slot[v];
         const int kbs = p.d_pad64 / 64, seg = lane >> 3, part = lane & 7;
         const __nv_bfloat16 *pool = static_cast<const __nv_bfloat16 *>(p.pages);
@@ -671,6 +695,47 @@ __device__ __forceinline__ void graph_walk_bf16(const GraphSearchParams &p) {
         return acc;
     });
 }
+
+// BINARYMSTG: rows scored in place from the binary list pages ([page][row_pad / kb_w][256][kb_w] bytes), row v at pool slot
+// row_slot[v].  The query's bytes sit in shared memory as row_pad / 4 words, zero beyond row_bytes.  Lane l ANDs the 16-byte
+// chunks l, l + 32, ... of the row with the query and counts the set bits; the shuffle tree sums the lanes' counts.  With
+// popc(q) (summed once by every warp) and the stored popc(y), the key is BINARYFLAT's distance: Hamming popc(q) + popc(y) - 2
+// and; Jaccard (or - and) / or with or = popc(q) + popc(y) - and (0 when or = 0), one IEEE division.  Every count is an exact
+// integer, so a key equals the exact scan's distance of that (query, row) to the bit.
+template <int W>
+__device__ __forceinline__ void graph_walk_b1(const GraphB1Params &b) {
+    const GraphSearchParams &p = b.g;
+    const uint8_t *qb = b.queries + (int64_t)(blockIdx.x / W) * b.row_bytes;
+    int qpop = 0;
+    for (int j = threadIdx.x & 31; j < b.row_bytes; j += 32) qpop += __popc((uint32_t)qb[j]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) qpop += __shfl_xor_sync(0xffffffffu, qpop, o);
+    const auto stage = [&](float *qs, int64_t, int i) {
+        uint32_t w = 0;
+        for (int e = 0; e < 4; e++)
+            if (4 * i + e < b.row_bytes) w |= (uint32_t)qb[4 * i + e] << (8 * e);
+        reinterpret_cast<uint32_t *>(qs)[i] = w;
+    };
+    graph_walk<W>(p, b.row_pad / 4, stage, [&](uint32_t v, const float *qs, int lane) {
+        const uint32_t slot = p.row_slot[v];
+        const int cpk = b.kb_w / 16;   // 16-byte chunks per k-block
+        const uint8_t *row = static_cast<const uint8_t *>(p.pages) + (size_t)(slot / kPageRows) * kPageRows * b.row_pad + (size_t)(slot % kPageRows) * b.kb_w;
+        const uint4 *x4 = reinterpret_cast<const uint4 *>(qs);
+        int a = 0;
+        for (int c = lane; c < b.row_pad / 16; c += 32) {
+            const int kb = c / cpk;
+            const uint4 y = __ldg(reinterpret_cast<const uint4 *>(row + (size_t)kb * kPageRows * b.kb_w) + (c - kb * cpk));
+            const uint4 x = x4[c];
+            a += __popc(x.x & y.x) + __popc(x.y & y.y) + __popc(x.z & y.z) + __popc(x.w & y.w);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+        const int yp = (int)b.row_popc[slot];
+        if (!b.jaccard) return (float)(qpop + yp - 2 * a);
+        const int x_or = qpop + yp - a;
+        return x_or == 0 ? 0.f : (float)(x_or - a) / (float)x_or;
+    });
+}
 }  // namespace
 
 __global__ void __launch_bounds__(kGraphThreads) graph_search_kernel(const GraphSearchParams p) { graph_walk_fp32<1>(p); }
@@ -685,6 +750,11 @@ template <int W>
 __global__ void __launch_bounds__(kGraphThreads, 2) graph_search_cluster_kernel(const GraphSearchParams p) { graph_walk_fp32<W>(p); }
 template <int W>
 __global__ void __launch_bounds__(kGraphThreads, 2) graph_search_bf16_cluster_kernel(const GraphSearchParams p) { graph_walk_bf16<W>(p); }
+
+// BINARYMSTG's walk over the binary list pages, and its cluster forms; (kGraphThreads, 2) as the bf16 walk
+__global__ void __launch_bounds__(kGraphThreads, 2) graph_search_b1_kernel(const GraphB1Params p) { graph_walk_b1<1>(p); }
+template <int W>
+__global__ void __launch_bounds__(kGraphThreads, 2) graph_search_b1_cluster_kernel(const GraphB1Params p) { graph_walk_b1<W>(p); }
 
 size_t graph_search_smem(int q_len, int ef, int k, bool filtered, int width) {
     return (size_t)graph_smem_layout(q_len, ef, k, filtered, width).total;
@@ -713,6 +783,31 @@ int graph_max_active_clusters(const void *fn, const cudaLaunchConfig_t &cfg, int
     known[key] = *clusters;
     return B200_OK;
 }
+
+// nq clusters of W CTAs (W > 1) of the walk fn, its one parameter at arg
+int graph_launch_clusters(const void *fn, void *arg, size_t smem, int64_t nq, int W, cudaStream_t s) {
+    if (nq > INT32_MAX / W) return fail(B200_ERR_UNSUPPORTED, "graph search: nq x search_width must stay below 2^31");
+    cudaLaunchConfig_t cfg{};
+    cudaLaunchAttribute attr{};
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = (unsigned)W;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.gridDim = dim3((unsigned)(nq * W));
+    cfg.blockDim = dim3(kGraphThreads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = s;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    int clusters = 0;
+    B200_TRY(graph_max_active_clusters(fn, cfg, &clusters));
+    if (clusters < 1)
+        return fail(B200_ERR_UNSUPPORTED, "graph search: a cluster of " + std::to_string(W) + " CTAs with " + std::to_string(smem) +
+                                              " bytes of shared memory each cannot be resident on this device");
+    void *args[] = {arg};
+    B200_CUDA_OK(cudaLaunchKernelExC(&cfg, fn, args));
+    return B200_OK;
+}
 }  // namespace
 
 int graph_search(const GraphSearchParams &p, int64_t nq, int width, cudaStream_t s) {
@@ -736,27 +831,29 @@ int graph_search(const GraphSearchParams &p, int64_t nq, int width, cudaStream_t
         if (bf16) graph_search_bf16_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
         else graph_search_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
     } else {
-        if (nq > INT32_MAX / W) return fail(B200_ERR_UNSUPPORTED, "graph search: nq x search_width must stay below 2^31");
-        cudaLaunchConfig_t cfg{};
-        cudaLaunchAttribute attr{};
-        attr.id = cudaLaunchAttributeClusterDimension;
-        attr.val.clusterDim.x = (unsigned)W;
-        attr.val.clusterDim.y = 1;
-        attr.val.clusterDim.z = 1;
-        cfg.gridDim = dim3((unsigned)(nq * W));
-        cfg.blockDim = dim3(kGraphThreads);
-        cfg.dynamicSmemBytes = smem;
-        cfg.stream = s;
-        cfg.attrs = &attr;
-        cfg.numAttrs = 1;
-        int clusters = 0;
-        B200_TRY(graph_max_active_clusters(fn, cfg, &clusters));
-        if (clusters < 1)
-            return fail(B200_ERR_UNSUPPORTED, "graph search: a cluster of " + std::to_string(W) + " CTAs with " + std::to_string(smem) +
-                                                  " bytes of shared memory each cannot be resident on this device");
-        void *args[] = {const_cast<GraphSearchParams *>(&p)};
-        B200_CUDA_OK(cudaLaunchKernelExC(&cfg, fn, args));
+        B200_TRY(graph_launch_clusters(fn, const_cast<GraphSearchParams *>(&p), smem, nq, W, s));
     }
+    g_launches++;
+    B200_CUDA_OK(cudaGetLastError());
+    return B200_OK;
+}
+
+int graph_search_b1(const GraphB1Params &p, int64_t nq, int width, cudaStream_t s) {
+    if (nq == 0) return B200_OK;
+    const int W = width;
+    if (!graph_width_ok(W)) return fail(B200_ERR_INVALID, "search_width must be 1, 2, 4 or 8, got " + std::to_string(W));
+    // the query is at most 8 KB (65536 bits): every ef, k and W fits
+    const size_t smem = graph_search_smem(p.row_pad / 4, p.g.ef, p.g.k, p.g.alive != nullptr, W);
+    if (smem > (size_t)kSmemOptinBytes)
+        return fail(B200_ERR_UNSUPPORTED, "graph search: a " + std::to_string(p.row_pad) + "-byte binary query at ef " + std::to_string(p.g.ef) +
+                                              " needs " + std::to_string(smem) + " bytes of shared memory, more than " + std::to_string(kSmemOptinBytes));
+    const void *fn = W == 1   ? (const void *)graph_search_b1_kernel
+                     : W == 2 ? (const void *)graph_search_b1_cluster_kernel<2>
+                     : W == 4 ? (const void *)graph_search_b1_cluster_kernel<4>
+                              : (const void *)graph_search_b1_cluster_kernel<8>;
+    B200_CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (W == 1) graph_search_b1_kernel<<<(unsigned)nq, kGraphThreads, smem, s>>>(p);
+    else B200_TRY(graph_launch_clusters(fn, const_cast<GraphB1Params *>(&p), smem, nq, W, s));
     g_launches++;
     B200_CUDA_OK(cudaGetLastError());
     return B200_OK;

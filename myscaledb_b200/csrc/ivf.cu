@@ -1313,9 +1313,9 @@ struct b200_index {
     int last_coarse = 0;   // coarse-probe path of the last float list search (b200_index_last_coarse), 0 = none
     // statistics of the last search (tests, bench roofline): rows x payload bytes the scan kernel was asked to stream
     int64_t last_scan_rows = 0, last_items = 0;
-    // graph_degree=D (HNSWFLAT, MSTG): neighbour graph [n][D] u32 built at finalize, 0xFFFFFFFF = empty slot (graph_sm90.cu);
-    // MSTG walks its bf16 list rows in place: d_row_slot[n] = row id -> pool slot, derived from the page chains at finalize
-    // and at load (never saved: a load may place the pages elsewhere)
+    // graph_degree=D (HNSWFLAT, MSTG, BINARYMSTG): neighbour graph [n][D] u32 built at finalize, 0xFFFFFFFF = empty slot
+    // (graph_sm90.cu); MSTG and BINARYMSTG walk their bf16 / binary list rows in place: d_row_slot[n] = row id -> pool slot,
+    // derived from the page chains at finalize and at load (never saved: a load may place the pages elsewhere)
     int graph_degree = 0;
     uint32_t *d_graph = nullptr, *d_row_slot = nullptr;
     // seed ids [last_seed_nq][last_seed_s] of the last graph search (b200_index_last_seeds), and their first-stage distances
@@ -1457,9 +1457,9 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
         default: ix->payload = IVF_PRODUCER_TMA;
     }
     if (bin) {
-        // Binary types: BINARYHNSW / BINARYMSTG are served by the binary inverted-file engine (no graph); list rows are exact,
-        // so there is no second stage.  k-block width kb_w = the row rounded up to 16 bytes, at most 128 (one 1024-bit wgmma
-        // k-block); TMA zero-fills the rest of the 128-byte box.
+        // Binary types: BINARYHNSW / BINARYMSTG are served by the binary inverted-file engine (BINARYMSTG walks a graph over its
+        // list rows with graph_degree); list rows are exact, so there is no second stage.  k-block width kb_w = the row rounded
+        // up to 16 bytes, at most 128 (one 1024-bit wgmma k-block); TMA zero-fills the rest of the 128-byte box.
         ix->binary = true;
         ix->row_bytes = d / 8;
         ix->kb_w = (int)std::min<int64_t>(128, round_up(ix->row_bytes, 16));
@@ -1471,13 +1471,14 @@ extern "C" int b200_index_create(const char *type, int metric, int d, const char
     const int dflt_refine = (ty == IDX_IVFPQ || ty == IDX_IVFSQ || bin) ? 1 : (ix->payload == IVF_PRODUCER_PQ ? 16 : 4);
     ix->refine_factor = parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", dflt_refine));
     ix->keep_raw = parse_int_param(params, "keep_raw", -1);
-    // graph_degree=D: HNSWFLAT, walked over its fp32 rows in HBM, or MSTG, walked over its bf16 list rows with any keep_raw
-    // (the reference's m is PQ M here and keeps that meaning)
+    // graph_degree=D: HNSWFLAT, walked over its fp32 rows in HBM, MSTG, walked over its bf16 list rows with any keep_raw, or
+    // BINARYMSTG, walked over its binary list rows (the reference's m is PQ M here and keeps that meaning)
     ix->graph_degree = parse_int_param(params, "graph_degree", 0);
     if (ix->graph_degree > 0) {
-        if (ty != IDX_HNSWFLAT && ty != IDX_MSTG) {
+        if (ty != IDX_HNSWFLAT && ty != IDX_MSTG && ty != IDX_BINMSTG) {
             delete ix;
-            return fail(B200_ERR_UNSUPPORTED, "graph_degree: a neighbour graph is built on HNSWFLAT and MSTG only (the other types keep quantised or binary rows)");
+            return fail(B200_ERR_UNSUPPORTED,
+                        "graph_degree: a neighbour graph is built on HNSWFLAT, MSTG and BINARYMSTG only (the other types keep quantised rows, or are BINARYHNSW / BINARYIVF)");
         }
         if (!graph_degree_ok(ix->graph_degree)) {
             const int gd = ix->graph_degree;
@@ -2315,7 +2316,7 @@ static int fill_row_slot(const b200_index *ix, uint32_t *d_row_slot) {
     return graph_row_slots(ix->d_list_len, ix->d_list_page_off, ix->d_list_pages, ix->d_row_ids, ix->nlist, d_row_slot, ix->stream);
 }
 
-// MSTG graph: the walk reads its bf16 list rows through d_row_slot
+// MSTG / BINARYMSTG graph: the walk reads its bf16 / binary list rows through d_row_slot
 static int build_row_slot(b200_index *ix) {
     if (!ix->d_row_slot && cudaMalloc(&ix->d_row_slot, std::max<size_t>((size_t)ix->n * 4, 16)) != cudaSuccess) {
         cudaGetLastError();
@@ -2328,8 +2329,10 @@ static int build_row_slot(b200_index *ix) {
 // re-rank with refine_factor, exactly ix.search(rows, 2D + 1, "graph=0").  MSTG: the first stage only, exactly
 // ix.search(rows, 2D + 1, "graph=0", first_stage_only=True): the graph is built in the metric its walk scores, the same way for
 // either placement of the fp32 rows, and never reads a row over PCIe.  The queries are the fp32 rows (HBM or host memory), or,
-// in an index without them (MSTG keep_raw=0), the bf16 list rows.  Its own id dropped, a row's 2D candidates are pruned by rank
-// (CAGRA) and merged with the reverse edges (graph_sm90.cu).  phase_ms then holds candidates | prune | merge in milliseconds.
+// in an index without them (MSTG keep_raw=0), the bf16 list rows.  BINARYMSTG: its lists are exact, so the search is exactly
+// ix.search(rows, 2D + 1, "graph=0"), its queries the row bytes read back from the binary pages (it keeps no other copy).  Its
+// own id dropped, a row's 2D candidates are pruned by rank (CAGRA) and merged with the reverse edges (graph_sm90.cu).  phase_ms
+// then holds candidates | prune | merge in milliseconds.
 static int build_graph_locked(b200_index *ix) {
     using clk = std::chrono::steady_clock;
     const auto ms_since = [](clk::time_point t) { return std::chrono::duration<double, std::milli>(clk::now() - t).count(); };
@@ -2338,10 +2341,13 @@ static int build_graph_locked(b200_index *ix) {
     const int64_t n = ix->n;
     const bool mstg = ix->type == IDX_MSTG;
     const int np = std::max(1, std::min(ix->default_nprobe, ix->nlist));
-    const int k1 = mstg ? K + 1 : std::min(1024, (K + 1) * std::max(1, ix->refine_factor));
-    const int64_t chunk = std::max<int64_t>(256, std::min<int64_t>(n, kGraphBuildSearchBytes / ((int64_t)np * k1 * 8)));
+    const int k1 = mstg || ix->binary ? K + 1 : std::min(1024, (K + 1) * std::max(1, ix->refine_factor));
+    // BINARYMSTG: the chunk's query rows (up to 8 KB each, about a row's list-search scratch) count against the budget too.  The
+    // float builds keep their chunk: its size picks the list search's coarse path, so a new one could move their graphs.
+    const int64_t q_row_bytes = ix->binary ? ix->row_bytes : (int64_t)d * 4;
+    const int64_t chunk = std::max<int64_t>(256, std::min<int64_t>(n, kGraphBuildSearchBytes / ((int64_t)np * k1 * 8 + (ix->binary ? q_row_bytes : 0))));
     DevScratch cand, pruned, q, dis, ids, slots;
-    // which rows are in a list: MSTG's slot map, a scratch one for HNSWFLAT
+    // which rows are in a list: the slot map of MSTG / BINARYMSTG, a scratch one for HNSWFLAT
     const uint32_t *row_slot = ix->d_row_slot;
     if (!row_slot) {
         B200_TRY(slots.alloc((size_t)n * 4));
@@ -2349,14 +2355,16 @@ static int build_graph_locked(b200_index *ix) {
         row_slot = static_cast<const uint32_t *>(slots.p);
     }
     B200_TRY(cand.alloc((size_t)n * K * 4));
-    B200_TRY(q.alloc((size_t)chunk * d * 4));
+    B200_TRY(q.alloc((size_t)chunk * q_row_bytes));   // fp32 rows, or binary rows of d / 8 bytes
     B200_TRY(dis.alloc((size_t)chunk * (K + 1) * 4));
     B200_TRY(ids.alloc((size_t)chunk * (K + 1) * 8));
     auto t = clk::now();
     const float *rows = ix->raw ? reinterpret_cast<const float *>(corpus_device_rows(ix->raw)) : ix->h_rows;
     for (int64_t off = 0; off < n; off += chunk) {
         const int64_t m = std::min(chunk, n - off);
-        if (rows)
+        if (ix->binary)
+            B200_TRY(graph_bin_page_rows(ix->d_pool, ix->d_row_slot, off, m, ix->row_bytes, ix->row_pad, ix->kb_w, static_cast<uint8_t *>(q.p), s));
+        else if (rows)
             B200_CUDA_OK(cudaMemcpy2DAsync(q.p, (size_t)d * 4, rows + off * ix->d_pad, (size_t)ix->d_pad * 4, (size_t)d * 4, m,
                                            ix->raw ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
         else
@@ -2441,7 +2449,7 @@ static int finalize_locked(b200_index *ix) {
     }
     // a part below the inverted-file threshold is FLAT and gets no graph
     if (ix->graph_degree > 0 && ix->use_ivf && ix->n > 0 && !ix->d_graph) {
-        if (ix->type == IDX_MSTG) B200_TRY(build_row_slot(ix));
+        if (ix->type == IDX_MSTG || ix->type == IDX_BINMSTG) B200_TRY(build_row_slot(ix));
         B200_TRY(build_graph_locked(ix));
     }
     ix->built = true;
@@ -2578,7 +2586,7 @@ extern "C" int b200_index_last_scan(b200_index *ix, int64_t *rows_streamed, int6
         if (cudaMemcpy(&r, ix->d_flag + 4, 8, cudaMemcpyDeviceToHost) == cudaSuccess) ix->last_scan_rows = (int64_t)r;
     }
     if (rows_streamed) *rows_streamed = ix->last_scan_rows;
-    // the graph walk reads fp32 rows (HNSWFLAT) or the bf16 list rows (MSTG)
+    // the graph walk reads fp32 rows (HNSWFLAT), the bf16 list rows (MSTG) or the binary list rows (BINARYMSTG)
     if (payload_row_bytes_out) *payload_row_bytes_out = ix->last_graph && !ix->d_row_slot ? (int64_t)ix->d_pad * 4 : (int64_t)payload_row_bytes(ix);
     if (work_items) *work_items = ix->last_items;
     if (kernel_ms_total) *kernel_ms_total = ix->timed_ms;
@@ -3082,8 +3090,9 @@ static int graph_width(const char *params) { return parse_int_param(params, "sea
 
 // The graph search, asynchronous on s (d_q: the prepared queries [nq][d_pad]): seeds from the list path's first stage at
 // nprobe 1 (the best min(ef_s, 32) ids per query), then one CTA per query (search_width=W > 1: one cluster of W CTAs, W
-// parents per iteration) walks the graph: graph_search_kernel over the fp32 rows in HBM (HNSWFLAT, kc = k), or
-// graph_search_bf16_kernel over the bf16 list rows (MSTG).  With a second stage
+// parents per iteration) walks the graph: graph_search_kernel over the fp32 rows in HBM (HNSWFLAT, kc = k),
+// graph_search_bf16_kernel over the bf16 list rows (MSTG), or graph_search_b1_kernel over the binary list rows (BINARYMSTG, kc =
+// k: its keys are the exact distances; d_queries are its query bytes).  With a second stage
 // (two_stage, MSTG only; kc may equal k, at k = 1024) the walk's best kc rows are re-ranked exactly by refine_device, from HBM
 // or from host memory.
 static int graph_search_locked(b200_index *ix, const float *d_queries, const float *d_q, int64_t nq, int k, int kc, bool two_stage, const char *params,
@@ -3103,8 +3112,9 @@ static int graph_search_locked(b200_index *ix, const float *d_queries, const flo
         B200_TRY(ix->w_od.reserve((size_t)nq * kc * 4));
         B200_TRY(ix->w_oi.reserve((size_t)nq * kc * 8));
     }
-    GraphSearchParams gp{};
-    gp.queries = d_q;
+    GraphB1Params bp{};
+    GraphSearchParams &gp = bp.g;
+    gp.queries = ix->binary ? nullptr : d_q;
     if (ix->d_row_slot) {
         gp.pages = ix->d_pool;
         gp.row_slot = ix->d_row_slot;
@@ -3126,8 +3136,18 @@ static int graph_search_locked(b200_index *ix, const float *d_queries, const flo
     gp.ef = ef;
     gp.k = kc;
     gp.max_iters = graph_iteration_cap(ix->graph_degree, width);
-    gp.l2 = ix->metric == B200_METRIC_L2;
-    B200_TRY(graph_search(gp, nq, width, s));
+    gp.l2 = ix->metric == B200_METRIC_L2 || ix->binary;
+    if (ix->binary) {
+        bp.queries = reinterpret_cast<const uint8_t *>(d_queries);
+        bp.row_popc = ix->d_row_bias;
+        bp.row_bytes = ix->row_bytes;
+        bp.row_pad = ix->row_pad;
+        bp.kb_w = ix->kb_w;
+        bp.jaccard = ix->metric == B200_METRIC_JACCARD;
+        B200_TRY(graph_search_b1(bp, nq, width, s));
+    } else {
+        B200_TRY(graph_search(gp, nq, width, s));
+    }
     if (two_stage) {
         B200_TRY(refine_device(ix, d_q, nq, ix->w_oi.as<int64_t>(), kc, k, id_offset, d_out_dis, d_out_ids, s));
     } else if (ix->metric == B200_METRIC_COSINE) {
@@ -3190,14 +3210,15 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         if (ef_s > kGraphMaxEf) return fail(B200_ERR_INVALID, "ef_s must be at most 1024, got " + std::to_string(ef_s));
         const int width = graph_width(params);
         if (!graph_width_ok(width)) return fail(B200_ERR_INVALID, "search_width must be 1, 2, 4 or 8, got " + std::to_string(width));
-        if (ix->d_row_slot) {
+        if (ix->d_row_slot && !ix->binary) {   // BINARYMSTG: the walk's keys are the exact distances
             const int refine_factor = std::max(1, parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", ix->refine_factor)));
             graph_two_stage = has_rows(ix) && refine_factor > 1 && !first_stage_only;
             if (graph_two_stage) kc = std::min(kGraphMaxEf, k * refine_factor);
         }
         if (out_num_candidates) *out_num_candidates = kc;
-        // the exact rule scans the fp32 rows in HBM: without them (MSTG keep_raw=0 | 2) the walk always answers
-        if (d_alive && h_alive && ix->raw) {
+        // the exact rule scans the fp32 rows in HBM: without them (MSTG keep_raw=0 | 2) the walk always answers, and so does
+        // BINARYMSTG's (its lists are the only copy of its rows; a load refuses a v4 binary file with rows)
+        if (d_alive && h_alive && ix->raw && !ix->binary) {
             const int64_t rows_cap = graph_rows_at_cap(ix, std::min(graph_ef(params, kc), kGraphMaxSeeds), width);
             const int64_t limit = std::min<int64_t>((int64_t)std::ceil(kGraphExactFactor * kc * (double)ix->n / (double)rows_cap) - 1,
                                                     corpus_prefilter_limit(ix->raw, prefilter, nq, k));
@@ -3643,10 +3664,14 @@ static int index_load_io(Io *f, b200_index **out) {
         !(h.reserved0 == 4 && h.payload == IVF_PRODUCER_PQ && h.use_ivf && h.m > 0 && h.dsub > 0 && (int64_t)h.m * h.dsub == h.d &&
           h.code_bytes >= pq_code_bytes(h.m, 4) && h.code_bytes % 16 == 0 && ivf_pq4_fits(h.m)))
         return fail(B200_ERR_INVALID, "corrupt index header (4-bit PQ with M <= " + std::to_string(ivf_pq4_max_m()) + " expected)");
-    // v4: an inverted-file index with a graph of degree reserved0: HNSWFLAT with its fp32 rows in HBM, or MSTG with any rows
+    // v4: an inverted-file index with a graph of degree reserved0: HNSWFLAT with its fp32 rows in HBM, MSTG with any rows, or
+    // BINARYMSTG without rows (its inverted lists hold the only copy)
+    const bool walks_pages = h.type == IDX_MSTG || h.type == IDX_BINMSTG;   // the graph walk reads the list rows through the slot map
     if (h.version == 4 && !(graph_degree_ok((int)h.reserved0) && h.use_ivf &&
-                            ((h.type == IDX_HNSWFLAT && h.has_raw == 1) || (h.type == IDX_MSTG && h.payload == IVF_PRODUCER_TMA))))
-        return fail(B200_ERR_INVALID, "corrupt index header (v4: an HNSWFLAT graph of degree 16, 32 or 64 over HBM rows, or an MSTG graph, expected)");
+                            ((h.type == IDX_HNSWFLAT && h.has_raw == 1) || (h.type == IDX_MSTG && h.payload == IVF_PRODUCER_TMA) ||
+                             (h.type == IDX_BINMSTG && h.payload == IVF_PRODUCER_B1 && h.has_raw == 0))))
+        return fail(B200_ERR_INVALID, "corrupt index header (v4: an HNSWFLAT graph of degree 16, 32 or 64 over HBM rows, an MSTG graph, or a "
+                                      "BINARYMSTG graph without rows, expected)");
     const bool sane = h.type >= 0 && h.type < IDX_NUM_TYPES && h.metric >= 0 && h.metric <= 4 && (h.metric >= B200_METRIC_HAMMING) == bin &&
                       h.d > 0 && h.d <= (1 << 16) && (!bin || h.d % 8 == 0) && h.n >= 0 &&
                       h.n < (int64_t)0xffffffffll && h.payload >= 0 && h.payload <= 3 && (h.payload == IVF_PRODUCER_B1) == bin &&
@@ -3789,7 +3814,7 @@ static int index_load_io(Io *f, b200_index **out) {
             if (!(err <= kOpqLoadTol)) return bail("corrupt index file (OPQ rotation not orthonormal: max |R^T R - I| = " + std::to_string(err) + ")");
             ix->opq = 1;
         }
-        if (h.version == 4) {   // every id < n or 0xFFFFFFFF before a kernel walks the graph; MSTG: every id in a list (it has a pool slot)
+        if (h.version == 4) {   // every id < n or 0xFFFFFFFF before a kernel walks the graph; (BINARY)MSTG: every id in a list (it has a pool slot)
             const int D = (int)h.reserved0;
             const size_t rb = (size_t)D * 4;
             const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / (int64_t)rb);
@@ -3802,12 +3827,12 @@ static int index_load_io(Io *f, b200_index **out) {
                 for (int64_t e = 0; e < mrows * D; e++) {
                     if (buf[e] == kNoId) continue;
                     if (buf[e] >= (uint64_t)h.n) return bail("corrupt index file (graph id out of range)");
-                    if (h.type == IDX_MSTG && !in_list[buf[e]]) return bail("corrupt index file (graph edge to a row in no list)");
+                    if (walks_pages && !in_list[buf[e]]) return bail("corrupt index file (graph edge to a row in no list)");
                 }
                 if (cudaMemcpy(ix->d_graph + off * D, buf.data(), (size_t)mrows * rb, cudaMemcpyHostToDevice) != cudaSuccess) return bail("H2D failed");
             }
-            // MSTG: the slot map of the pages as loaded here
-            if (h.type == IDX_MSTG && (build_row_slot(ix) != B200_OK || cudaStreamSynchronize(ix->stream) != cudaSuccess))
+            // MSTG / BINARYMSTG: the slot map of the pages as loaded here
+            if (walks_pages && (build_row_slot(ix) != B200_OK || cudaStreamSynchronize(ix->stream) != cudaSuccess))
                 return bail(std::string("graph row slot map: ") + b200_last_error());
         }
     } catch (const std::bad_alloc &) {

@@ -119,7 +119,8 @@ static const char * const MYSCALE_VALID_INDEX_PARAMETER = R"({
  "HNSWPQ": {"m": {"type": "int", "range": [8, 128]}, "M": {"type": "int", "range": [1, 4096]}, "aq_threshold": {"type": "float", "range": [0, 1]}, "opq": {"type": "int", "range": [0, 1]}, "opq_iters": {"type": "int", "range": [0, 1000]}, "nprobe": {"type": "int", "range": [1, 1048576]}},
  "SCANN": {"ncentroids": {"type": "int", "range": [1, 1048576]}, "M": {"type": "int", "range": [1, 4096]}, "aq_threshold": {"type": "float", "range": [0, 1]}, "opq": {"type": "int", "range": [0, 1]}, "opq_iters": {"type": "int", "range": [0, 1000]}, "nprobe": {"type": "int", "range": [1, 1048576]}, "reorder_k_factor": {"type": "int", "range": [1, 100]}},
  "MSTG": {"ncentroids": {"type": "int", "range": [1, 1048576]}, "alpha": {"type": "float", "range": [1, 4]}, "nprobe": {"type": "int", "range": [1, 1048576]}, "refine_factor": {"type": "int", "range": [1, 100]}, "disk_mode": {"type": "int", "range": [0, 2]}, "graph_degree": {"type": "int", "range": [0, 64]}, "ef_s": {"type": "int", "range": [16, 1024]}, "search_width": {"type": "int", "range": [1, 8]}},
- "BinaryIVF": {}, "BinaryHNSW": {}, "BinaryMSTG": {}
+ "BinaryIVF": {}, "BinaryHNSW": {},
+ "BinaryMSTG": {"graph_degree": {"type": "int", "range": [0, 64]}, "ef_s": {"type": "int", "range": [16, 1024]}, "search_width": {"type": "int", "range": [1, 8]}}
 })";
 
 // MergeTreeVSManager.cpp:361-366, VIWithDataPart.cpp:405-407 (erase_if over {key, value}), :645

@@ -2,7 +2,7 @@
 """Secondary measurements (not the driver's bench line): IVFPQ, the two-stage (MSTG-type) index and
 BM25 at moderate single-GPU scale, shaped after BASELINE.json configs 3-5.  Prints one JSON line per
 workload; results are pasted into DESIGN.md section 7.
-Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows] [filtered] [aq] [graph] [mstg_graph]"""
+Usage: python tools/bench_aux.py [ivfpq] [mstg] [bm25] [flat10k] [ingest] [binary] [binary_ivf] [pq_wide] [pq4] [prefilter] [host_rows] [filtered] [aq] [graph] [mstg_graph] [binary_graph]"""
 import json
 import os
 import subprocess
@@ -936,10 +936,75 @@ def bench_mstg_graph():
             del y
 
 
+def bench_binary_graph():
+    """BINARYMSTG graph search (graph_degree=32) against the same index's lists (graph=0), Hamming and Jaccard, on 1 M
+    clustered rows of 1024 bits (BINARY_GRAPH_BITS; binary_clustered: 10 000 centres, each bit flipped with probability 1/16).  Per metric: build
+    time with the graph's candidates / prune / merge phases, memory_bytes per row; per ef_s: recall@10 against BINARYFLAT at
+    nq = 1024 (tie-aware: returned rows within the 10th exact distance, since Hamming ties are common), QPS at batch 1024
+    (median of 5), the nq = 1 call (median, p10-p90) at search_width 1 and 8, rows scored per query; then the lists over
+    nprobe and, per ef_s, the cheapest nprobe whose recall reaches the walk's, with its batch QPS."""
+    n, bits, k, D = int(os.environ.get("BINARY_GRAPH_ROWS", 1_000_000)), int(os.environ.get("BINARY_GRAPH_BITS", 1024)), 10, 32
+    ctx = gpu_context()
+    y, qs = binary_clustered(n, bits // 8, 10_000, seed=bits)
+
+    def calls(fn, reps):
+        fn()
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            out = fn()
+            ts.append(time.perf_counter() - t0)
+        return np.array(ts), out
+
+    def tie_recall(dis, ids, td):
+        return float(((ids >= 0) & (dis <= td[:, k - 1:k])).sum()) / (len(ids) * k)
+
+    for metric, name in ((b2.HAMMING, "Hamming"), (b2.JACCARD, "Jaccard")):
+        flat = b2.Corpus(metric, bits, dtype=S.BIN).append(y)
+        td, _ = flat.search(qs, k)
+        flat.close()
+        t0 = time.perf_counter()
+        ix = b2.VectorIndex("BINARYMSTG", metric, bits, f"graph_degree={D}").build(y)
+        build_s = time.perf_counter() - t0
+        ph = ix.phase_ms()
+        plain = b2.VectorIndex("BINARYMSTG", metric, bits).build(y)
+        tag = f"BINARYMSTG {name} {n} x {bits} bits"
+        print(json.dumps(dict(workload=tag, D=D, **ctx, build_s=round(build_s, 2), graph_candidates_s=round(ph["coarse"] / 1e3, 2),
+                              graph_prune_s=round(ph["plan"] / 1e3, 3), graph_merge_s=round(ph["scan"] / 1e3, 3),
+                              memory_bytes_per_row=round(ix.memory_bytes() / n, 1), lists_only_memory_bytes_per_row=round(plain.memory_bytes() / n, 1),
+                              nlist=ix.info()["nlist"])), flush=True)
+        plain.close()
+        walk = []
+        for ef in (32, 64, 128, 256):
+            prm = f"ef_s={ef}"
+            tb, (dis, ids) = calls(lambda: ix.search(qs, k, prm), 5)
+            rows = ix.last_scan()["rows_streamed"] / len(qs)
+            pt = dict(workload=tag, ef_s=ef, recall=round(tie_recall(dis, ids, td), 4), qps_1024=round(len(qs) / np.median(tb), 1),
+                      rows_scored_per_query=round(rows, 1))
+            for w in (1, 8):
+                t1, _ = calls(lambda: ix.search(qs[:1], k, f"{prm},search_width={w}"), 50)
+                pt[f"nq1_W{w}_ms_median"] = round(1e3 * np.median(t1), 3)
+                pt[f"nq1_W{w}_ms_p10_p90"] = [round(1e3 * np.percentile(t1, 10), 3), round(1e3 * np.percentile(t1, 90), 3)]
+            walk.append(pt)
+            print(json.dumps(pt), flush=True)
+        pts = []
+        for nprobe in (1, 2, 4, 8, 16, 32, 64, 128, 256):
+            prm = f"graph=0,nprobe={nprobe}"
+            tb, (dis, ids) = calls(lambda: ix.search(qs, k, prm), 5)
+            pts.append((nprobe, tie_recall(dis, ids, td), len(qs) / float(np.median(tb))))
+            print(json.dumps(dict(workload=f"{tag} lists", nprobe=nprobe, recall=round(pts[-1][1], 4), qps_1024=round(pts[-1][2], 1))), flush=True)
+        for pt in walk:
+            ok = [p for p in pts if p[1] >= pt["recall"]]
+            print(json.dumps(dict(workload=f"{tag} lists at the walk's recall", ef_s=pt["ef_s"], walk_recall=pt["recall"],
+                                  walk_qps_1024=pt["qps_1024"], lists=None if not ok else dict(nprobe=ok[0][0], recall=round(ok[0][1], 4),
+                                                                                               qps_1024=round(ok[0][2], 1)))), flush=True)
+        ix.close()
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["ivfpq", "mstg", "bm25"]
     for w in which:
         {"ivfpq": bench_ivfpq, "mstg": bench_mstg, "bm25": bench_bm25, "flat10k": bench_flat10k, "ingest": bench_ingest,
          "binary": bench_binary, "binary_ivf": bench_binary_ivf, "pq_wide": bench_pq_wide, "pq4": bench_pq4, "prefilter": bench_prefilter,
          "host_rows": bench_host_rows, "filtered": bench_filtered, "aq": bench_aq, "graph": bench_graph,
-         "mstg_graph": bench_mstg_graph}[w]()
+         "mstg_graph": bench_mstg_graph, "binary_graph": bench_binary_graph}[w]()

@@ -112,7 +112,10 @@ int b200_corpus_free(b200_corpus *c);
  * Pre-filtered exact search: with alive_bits given, this call (and b200_flat_knn, b200_binary_knn, b200_part_scan, and
  * b200_index_search on FLAT / BINARYFLAT / small-part fallback / exact_batch=1) counts the bitmap's set bits on the host.
  * When the filter keeps few enough rows (see b200_corpus_set_prefilter) only those rows are copied into a compact scratch
- * corpus and scored; the result is byte for byte the full scan's, and the cost follows the rows kept, not the corpus size. */
+ * corpus and scored; the result is byte for byte the full scan's, and the cost follows the rows kept, not the corpus size.
+ * Batch size: this call, b200_corpus_search_device, b200_flat_knn, b200_binary_knn and b200_part_scan take any nq whose
+ * queries, results and per-query scratch fit in device memory; the scan and tensor-core kernels split a large batch into
+ * as many launches as the grid limits need. */
 int b200_corpus_search(b200_corpus *c, const float *queries, int64_t nq, int k, const uint8_t *alive_bits /*nullable*/,
                        float *out_dis, int64_t *out_ids);
 /* same, queries and results in device memory, asynchronous on `stream` (a cudaStream_t
@@ -344,6 +347,10 @@ int b200_index_info(const b200_index *ix, int64_t *n, int *nlist, int *m, int *u
 /* first_stage_only (two-stage types): return the first-stage candidates with first-stage distances;
  * out_num_candidates receives the width the first stage ran with (SearchResult::getNumCandidates).
  * "exact_batch=1" in `params` answers by an exact pass over the fp32 rows instead (recall 1).
+ * Batch size: the exact paths (FLAT, BINARYFLAT, the small-part fallback, exact_batch=1) take any batch that fits in device
+ * memory, as b200_corpus_search does.  The list scans of the inverted-file types refuse, with B200_ERR_UNSUPPORTED, a batch with nq x nprobe >= 2^31 probe pairs or with nq x nprobe x chunks x k1 >= 2^32 candidate slots
+ * (chunks: the pieces a long list is cut into, k1 = min(1024, k x refine_factor) on two-stage searches, else k); split such
+ * a batch.  The index stays usable after a refusal.
  * Tuning / A-B switches, also in `params` (defaults are chosen from the batch shape): "pages_per_chunk=N" (pages of a list one work
  * item streams), "shared_bound=0" (do not share a per-query bound between the work items of a launch), "coarse_path=1|2|3" (centroid
  * probe by the scan kernel / the tensor-core top-k / score tiles + warp select; default 3 for nprobe > 8), "prefilter=0|1|2" (exact

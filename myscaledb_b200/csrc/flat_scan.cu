@@ -748,14 +748,27 @@ cudaError_t launch_rescore_l2(const void *corpus, int bf16, int64_t row_bytes, i
 // ------------------------------------------------------------------------------------
 // host launchers
 // ------------------------------------------------------------------------------------
+// Query tiles ride on gridDim.y, at most 65535 of them per launch: a larger batch launches slice after slice, each with its
+// queries and partial lists offset to the slice's first query.  The fused form (<= 8 queries) is always one slice.
+constexpr int64_t kMaxGridY = 65535;
+
 template <int QT, int U, int CU>
-static cudaError_t launch_scan_qt(const ScanParams &p, dim3 grid, size_t smem, cudaStream_t s) {
+static cudaError_t launch_scan_qt(const ScanParams &p, int blocks_x, size_t smem, cudaStream_t s) {
     auto go = [&](auto kern) -> cudaError_t {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        kern<<<grid, kScanThreads, smem, s>>>(p);
-        g_launches++;
-        return cudaGetLastError();
+        const int64_t slice = p.fused ? p.nq : kMaxGridY * QT;
+        for (int64_t q0 = 0; q0 < p.nq; q0 += slice) {
+            ScanParams ps = p;
+            ps.nq = std::min(slice, p.nq - q0);
+            ps.queries += q0 * p.d_pad;
+            ps.part_keys += q0 * blocks_x * p.k;
+            ps.part_ids += q0 * blocks_x * p.k;
+            kern<<<dim3(blocks_x, (unsigned)ceil_div(ps.nq, QT)), kScanThreads, smem, s>>>(ps);
+            g_launches++;
+            if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        }
+        return cudaSuccess;
     };
     if (p.l2) return p.bf16 ? go(flat_scan_kernel<QT, U, CU, true, true>) : go(flat_scan_kernel<QT, U, CU, true, false>);
     return p.bf16 ? go(flat_scan_kernel<QT, U, CU, false, true>) : go(flat_scan_kernel<QT, U, CU, false, false>);
@@ -768,7 +781,6 @@ size_t scan_smem_bytes(int qt, int d_pad, int k) {
 
 cudaError_t launch_flat_scan(const ScanParams &p_in, int qt, int blocks_x, cudaStream_t s) {
     ScanParams p = p_in;
-    const dim3 grid(blocks_x, (unsigned)ceil_div(p.nq, qt));
     size_t smem = scan_smem_bytes(qt, p.d_pad, p.k);
     p.stage_cap = 0;
     if (p.fused && (size_t)blocks_x * p.k <= 8192) {
@@ -782,26 +794,34 @@ cudaError_t launch_flat_scan(const ScanParams &p_in, int qt, int blocks_x, cudaS
     // loads in flight per lane: short rows -> 4 rows x 1 chunk; long rows -> 4 chunks x (4 | 2) rows
     if (cpl <= 2) {
         switch (qt) {
-            case 1: return launch_scan_qt<1, 4, 1>(p, grid, smem, s);
-            case 4: return launch_scan_qt<4, 4, 1>(p, grid, smem, s);
-            default: return launch_scan_qt<8, 4, 1>(p, grid, smem, s);
+            case 1: return launch_scan_qt<1, 4, 1>(p, blocks_x, smem, s);
+            case 4: return launch_scan_qt<4, 4, 1>(p, blocks_x, smem, s);
+            default: return launch_scan_qt<8, 4, 1>(p, blocks_x, smem, s);
         }
     }
     switch (qt) {
-        case 1: return launch_scan_qt<1, 4, 4>(p, grid, smem, s);
-        case 4: return launch_scan_qt<4, 2, 4>(p, grid, smem, s);
-        default: return launch_scan_qt<8, 2, 4>(p, grid, smem, s);
+        case 1: return launch_scan_qt<1, 4, 4>(p, blocks_x, smem, s);
+        case 4: return launch_scan_qt<4, 2, 4>(p, blocks_x, smem, s);
+        default: return launch_scan_qt<8, 2, 4>(p, blocks_x, smem, s);
     }
 }
 
 cudaError_t launch_binary_scan(const BinaryScanParams &p, int blocks_x, cudaStream_t s) {
-    const dim3 grid(blocks_x, (unsigned)p.nq);
     const size_t smem = round_up(p.nbytes, 16) + (size_t)kScanWarps * p.k * 8;
     cudaError_t e = cudaFuncSetAttribute(binary_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    binary_scan_kernel<<<grid, kScanThreads, smem, s>>>(p);
-    g_launches++;
-    return cudaGetLastError();
+    // one query per y-block: slices of at most kMaxGridY queries, as in launch_scan_qt
+    for (int64_t q0 = 0; q0 < p.nq; q0 += kMaxGridY) {
+        BinaryScanParams ps = p;
+        ps.nq = std::min(kMaxGridY, p.nq - q0);
+        ps.queries += q0 * p.nbytes;
+        ps.part_keys += q0 * blocks_x * p.k;
+        ps.part_ids += q0 * blocks_x * p.k;
+        binary_scan_kernel<<<dim3(blocks_x, (unsigned)ps.nq), kScanThreads, smem, s>>>(ps);
+        g_launches++;
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 cudaError_t launch_topk_merge(const MergeParams &p, bool external, cudaStream_t s) {

@@ -627,6 +627,12 @@ __global__ void __launch_bounds__(1024) search_plan_kernel(const SearchPlan p) {
 // ------------------------------------------------------------------------------------
 constexpr int kCoarseTile = 64, kCoarseTK = 16;
 
+// Queries per coarse_scores_kernel launch: <= 256 MB of keys, and at most 65535 query tiles (gridDim.y).
+static int64_t coarse_chunk(int64_t nq, int nl) {
+    const int64_t by_bytes = std::max<int64_t>(64, std::min<int64_t>(nq, ((int64_t)64 << 20) / std::max(1, nl)));
+    return std::min<int64_t>(by_bytes, (int64_t)65535 * kCoarseTile);
+}
+
 __global__ void __launch_bounds__(256) coarse_scores_kernel(const float *x, int64_t ldx, const float *cent, const float *cnorm, int64_t nq,
                                                             int nl, int d, float *out /*[nq][nl]*/) {
     __shared__ float sx[kCoarseTK][kCoarseTile + 4], sc[kCoarseTK][kCoarseTile + 4];
@@ -2980,7 +2986,7 @@ static int filter_probe_search(b200_index *ix, const float *d_q, const float *d_
                                int64_t *d_out_ids, cudaStream_t s) {
     const int nl = ix->nlist;
     const int max_nprobe = std::max(nprobe, std::min(nl, parse_int_param(params, "max_nprobe", nl)));
-    const int64_t chunk = std::max<int64_t>(64, std::min<int64_t>(nq, ((int64_t)64 << 20) / std::max(1, nl)));   // <= 256 MB of keys
+    const int64_t chunk = coarse_chunk(nq, nl);
     const bool one_chunk = nq <= chunk;
     B200_TRY(ix->w_cs.reserve((size_t)chunk * nl * 4));
     const size_t tot_off = round_up((size_t)nq * 16, 16);
@@ -3320,7 +3326,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         const int forced = parse_int_param(params, "coarse_path", 0);   // A/B: 1 scan kernel, 2 tensor-core path, 3 select
         if (forced) coarse_path = forced;
         if (coarse_path == 3) {
-            const int64_t chunk = std::max<int64_t>(64, std::min<int64_t>(nq, ((int64_t)64 << 20) / std::max(1, nl)));   // <= 256 MB of keys
+            const int64_t chunk = coarse_chunk(nq, nl);
             B200_TRY(ix->w_cs.reserve((size_t)chunk * nl * 4));
             const size_t sel_smem = (size_t)8 * nprobe * 8;
             if (sel_smem > 48 * 1024) B200_CUDA_OK(cudaFuncSetAttribute(coarse_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));

@@ -157,6 +157,9 @@ int b200_corpus_enable_timing(b200_corpus *c, int on);
 int b200_corpus_kernel_time(b200_corpus *c, int reset, double *out_total_ms, int64_t *out_launches);
 /* number of kernels this library launched on the calling thread since the last reset */
 int64_t b200_launch_count(int reset);
+/* bytes of device memory the library holds, over every device and thread (a diagnostic: what the library allocated
+ * itself, unlike cudaMemGetInfo, which also moves with every other user of the device) */
+int64_t b200_device_bytes(void);
 /* b200_flat_knn / b200_binary_knn / b200_part_scan keep one grow-only scratch corpus per calling thread (device rows,
  * workspaces, stream), sized for the largest part that thread has scanned; this frees it (it is also freed at thread
  * exit).  A ClickHouse worker calls it when it goes idle. */

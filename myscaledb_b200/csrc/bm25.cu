@@ -487,28 +487,6 @@ __global__ void bm25_finish_kernel(const float *dis, const int64_t *docs, const 
     if (d >= 0) atomicAdd(&out_count[i / k], 1u);
 }
 
-struct DevVec {
-    void *p = nullptr;
-    size_t cap = 0;
-    int reserve(size_t bytes) {
-        if (bytes <= cap) return B200_OK;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        if (cudaMalloc(&p, bytes + 256) != cudaSuccess) {
-            cudaGetLastError();
-            return fail(B200_ERR_NOMEM, "cudaMalloc failed in bm25");
-        }
-        cap = bytes;
-        return B200_OK;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-};
-
 }  // namespace b200
 
 using namespace b200;
@@ -527,7 +505,7 @@ struct b200_bm25 {
     int device = 0;
     cudaStream_t stream = nullptr;
     std::mutex mu;
-    DevVec d_docs, d_tfs, d_fn, d_rows, d_clauses, d_begin, d_caches, d_pk, d_pi, d_alive, d_odis, d_oids, d_score, d_row64, d_cnt, d_masks, d_ranges;
+    DevMem d_docs, d_tfs, d_fn, d_rows, d_clauses, d_begin, d_caches, d_pk, d_pi, d_alive, d_odis, d_oids, d_score, d_row64, d_cnt, d_masks, d_ranges;
 };
 
 static int bm25_device_ok() {
@@ -561,9 +539,6 @@ extern "C" int b200_bm25_create(uint32_t n_fields, b200_bm25 **out) {
 extern "C" int b200_bm25_free(b200_bm25 *ix) {
     if (!ix) return B200_OK;
     cudaSetDevice(ix->device);
-    for (DevVec *v : {&ix->d_docs, &ix->d_tfs, &ix->d_fn, &ix->d_rows, &ix->d_clauses, &ix->d_begin, &ix->d_caches, &ix->d_pk,
-                      &ix->d_pi, &ix->d_alive, &ix->d_odis, &ix->d_oids, &ix->d_score, &ix->d_row64, &ix->d_cnt, &ix->d_masks, &ix->d_ranges})
-        v->release();
     if (ix->ev0) cudaEventDestroy(ix->ev0);
     if (ix->ev1) cudaEventDestroy(ix->ev1);
     if (ix->stream) cudaStreamDestroy(ix->stream);
@@ -645,10 +620,10 @@ extern "C" int b200_bm25_commit(b200_bm25 *ix) {
         for (size_t d = 0; d < nd; d++) fn[(size_t)f * nd + d] = fieldnorm_to_id(ix->doc_len[f][d]);
     std::vector<uint32_t> rows(nd ? nd : 1);
     for (size_t d = 0; d < nd; d++) rows[d] = (uint32_t)ix->row_ids[d];
-    B200_TRY(ix->d_docs.reserve(docs.size() * 4));
-    B200_TRY(ix->d_tfs.reserve(tfs.size() * 4));
-    B200_TRY(ix->d_fn.reserve(fn.size()));
-    B200_TRY(ix->d_rows.reserve(rows.size() * 4));
+    B200_TRY(ix->d_docs.alloc(docs.size() * 4 + 256));
+    B200_TRY(ix->d_tfs.alloc(tfs.size() * 4 + 256));
+    B200_TRY(ix->d_fn.alloc(fn.size() + 256));
+    B200_TRY(ix->d_rows.alloc(rows.size() * 4 + 256));
     B200_CUDA_OK(cudaMemcpyAsync(ix->d_docs.p, docs.data(), docs.size() * 4, cudaMemcpyHostToDevice, ix->stream));
     B200_CUDA_OK(cudaMemcpyAsync(ix->d_tfs.p, tfs.data(), tfs.size() * 4, cudaMemcpyHostToDevice, ix->stream));
     B200_CUDA_OK(cudaMemcpyAsync(ix->d_fn.p, fn.data(), fn.size(), cudaMemcpyHostToDevice, ix->stream));

@@ -53,38 +53,6 @@ static int num_sms() {
     return n;
 }
 
-// grow-only device buffer
-struct DevBuf {
-    void *p = nullptr;
-    size_t cap = 0;
-    uint64_t reallocs = 0;   // times p changed: a CUDA graph that baked p in is stale once this moves (corpus_state_epoch)
-    int reserve(size_t bytes) {
-        if (bytes <= cap) return B200_OK;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        reallocs++;
-        size_t want = bytes + bytes / 4 + 256;
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            return fail(B200_ERR_NOMEM, "cudaMalloc(" + std::to_string(want) + ") failed: " + cudaGetErrorString(e));
-        }
-        cap = want;
-        return B200_OK;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        reallocs++;
-    }
-    template <typename T>
-    T *as() {
-        return reinterpret_cast<T *>(p);
-    }
-};
-
 }  // namespace b200
 
 using namespace b200;
@@ -93,12 +61,11 @@ struct b200_corpus {
     int metric = 0, dtype = 0, d = 0, d_pad = 0;
     int64_t cap = 0, n = 0;
     int64_t row_bytes = 0;
-    void *data = nullptr;
-    size_t data_cap_bytes = 0;   // allocation size of `data` (owned corpora)
+    DevMem owned_rows;           // the rows, when the corpus allocated them
+    void *data = nullptr;        // the rows: owned_rows, or device rows the caller adopted in and still owns
     int64_t side_cap_rows = 0;   // rows the row_scale / row_bias arrays can hold
-    bool owns = true;
-    float *row_scale = nullptr;  // cosine: -1/||y||
-    float *row_bias = nullptr;   // L2: ||y||^2 (GEMM path); binary: popcount of the row (tensor-core path)
+    DevMem row_scale;            // float [rows]; cosine: -1/||y||
+    DevMem row_bias;             // float [rows]; L2: ||y||^2 (GEMM path); binary: popcount of the row (tensor-core path)
     int device = 0;
     int path = 0;
     int sms = 132;
@@ -110,10 +77,10 @@ struct b200_corpus {
     uint64_t serial = 0;
     uint64_t epoch = 0;
     // workspaces
-    DevBuf w_raw, w_q32, w_qbf, w_qlo, w_qnorm, w_pk, w_pi, w_lk, w_li, w_alive, w_odis, w_oids, w_stage, w_prog, w_qb;
+    DevMem w_raw, w_q32, w_qbf, w_qlo, w_qnorm, w_pk, w_pi, w_lk, w_li, w_alive, w_odis, w_oids, w_stage, w_prog, w_qb;
     // pre-filtered search (prefilter.cu): kept row ids, compaction scratch, compact rows (+ a row of slack), their side arrays
-    DevBuf w_pf_ids, w_pf_tmp, w_pf_rows, w_pf_side;
-    std::array<DevBuf *, 19> workspaces() {
+    DevMem w_pf_ids, w_pf_tmp, w_pf_rows, w_pf_side;
+    std::array<DevMem *, 19> workspaces() {
         return {&w_raw, &w_q32, &w_qbf, &w_qlo, &w_qnorm, &w_pk, &w_pi, &w_lk, &w_li, &w_alive, &w_odis, &w_oids, &w_stage, &w_prog,
                 &w_qb, &w_pf_ids, &w_pf_tmp, &w_pf_rows, &w_pf_side};
     }
@@ -122,7 +89,7 @@ struct b200_corpus {
     // fused single-launch path of the host entry point (small batches, scan kernel): mapped pinned staging + counters
     void *h_pin = nullptr;         // [queries 8 * d fp32 | dis 8 * k | ids 8 * k | flag]
     size_t h_pin_bytes = 0;
-    unsigned int *d_tickets = nullptr;   // [8] + tiles_done, then (at +64 bytes) the device copy of the staged queries
+    DevMem d_tickets;              // uint32 [8] + tiles_done, then (at +64 bytes) the device copy of the staged queries
     unsigned int fused_seq = 0;
     int d_tickets_d = 0;           // row length the query staging behind d_tickets was sized for
     int fused_enabled = 1;         // B200_FUSED_SCAN=0 disables (A/B)
@@ -181,7 +148,7 @@ uint64_t corpus_serial(const b200_corpus *c) { return c->serial; }
 uint64_t corpus_state_epoch(b200_corpus *c) {
     std::lock_guard<std::mutex> lk(c->mu);
     uint64_t e = c->epoch;
-    for (DevBuf *b : c->workspaces()) e += b->reallocs;
+    for (DevMem *b : c->workspaces()) e += b->reallocs;
     return e;
 }
 // hooks for the index layer (ivf.cu): device view of the rows / in-place row normalisation
@@ -243,6 +210,8 @@ extern "C" int b200_set_device(int device) {
     return B200_OK;
 }
 
+extern "C" int64_t b200_device_bytes(void) { return g_device_bytes; }
+
 extern "C" int64_t b200_launch_count(int reset) {
     int64_t v = g_launches;
     if (reset) g_launches = 0;
@@ -285,42 +254,34 @@ extern "C" int b200_corpus_create(int metric, int dtype, int d, int64_t capacity
 }
 
 static int corpus_alloc(b200_corpus *c, int64_t rows) {
-    if (c->data && !c->owns) return fail(B200_ERR_INVALID, "corpus adopted device memory; cannot append");
+    if (c->data && !c->owned_rows) return fail(B200_ERR_INVALID, "corpus adopted device memory; cannot append");
     // +1 row of slack so that 16-byte vector loads of the last row never leave the allocation
     const size_t need = (size_t)(rows + 1) * c->row_bytes + 256;
     const bool want_scale = c->metric == B200_METRIC_COSINE, want_bias = c->metric == B200_METRIC_L2 || is_bin_metric(c->metric);
-    if (!c->data || c->data_cap_bytes < need) {
-        void *nd = nullptr;
-        cudaError_t e = cudaMalloc(&nd, need);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            return fail(B200_ERR_NOMEM, std::string("cudaMalloc corpus: ") + cudaGetErrorString(e));
-        }
+    if (!c->data || c->owned_rows.size() < need) {
+        DevMem nd;   // the rows held so far are copied over before the old allocation goes
+        B200_TRY(nd.alloc(need));
         if (c->data && c->n) {
-            cudaMemcpyAsync(nd, c->data, (size_t)c->n * c->row_bytes, cudaMemcpyDeviceToDevice, c->stream);
+            cudaMemcpyAsync(nd.p, c->data, (size_t)c->n * c->row_bytes, cudaMemcpyDeviceToDevice, c->stream);
             cudaStreamSynchronize(c->stream);
         }
-        if (c->data) cudaFree(c->data);
-        c->data = nd;
-        c->data_cap_bytes = need;
+        c->owned_rows = std::move(nd);
+        c->data = c->owned_rows.p;
     }
     if ((want_scale && (!c->row_scale || c->side_cap_rows < rows)) || (want_bias && (!c->row_bias || c->side_cap_rows < rows))) {
-        float *ns = nullptr, *nb = nullptr;
-        if (want_scale && cudaMalloc(&ns, (size_t)rows * 4 + 256) != cudaSuccess) return fail(B200_ERR_NOMEM, "cudaMalloc row_scale");
-        if (want_bias && cudaMalloc(&nb, (size_t)rows * 4 + 256) != cudaSuccess) return fail(B200_ERR_NOMEM, "cudaMalloc row_bias");
+        DevMem ns, nb;
+        if (want_scale) B200_TRY(ns.alloc((size_t)rows * 4 + 256));
+        if (want_bias) B200_TRY(nb.alloc((size_t)rows * 4 + 256));
         if (c->n) {
-            if (ns && c->row_scale) cudaMemcpyAsync(ns, c->row_scale, (size_t)c->n * 4, cudaMemcpyDeviceToDevice, c->stream);
-            if (nb && c->row_bias) cudaMemcpyAsync(nb, c->row_bias, (size_t)c->n * 4, cudaMemcpyDeviceToDevice, c->stream);
+            if (ns && c->row_scale) cudaMemcpyAsync(ns.p, c->row_scale.p, (size_t)c->n * 4, cudaMemcpyDeviceToDevice, c->stream);
+            if (nb && c->row_bias) cudaMemcpyAsync(nb.p, c->row_bias.p, (size_t)c->n * 4, cudaMemcpyDeviceToDevice, c->stream);
             cudaStreamSynchronize(c->stream);
         }
-        if (c->row_scale) cudaFree(c->row_scale);
-        if (c->row_bias) cudaFree(c->row_bias);
-        c->row_scale = ns;
-        c->row_bias = nb;
+        c->row_scale = std::move(ns);
+        c->row_bias = std::move(nb);
         c->side_cap_rows = rows;
     }
     c->cap = std::max(c->cap, rows);
-    c->owns = true;
     c->epoch++;
     return B200_OK;
 }
@@ -328,11 +289,11 @@ static int corpus_alloc(b200_corpus *c, int64_t rows) {
 static int corpus_norms(b200_corpus *c, int64_t first, int64_t n) {
     const char *rows = reinterpret_cast<const char *>(c->data) + first * c->row_bytes;
     if (c->dtype == B200_DTYPE_BIN)
-        B200_CUDA_OK(launch_popc_rows(reinterpret_cast<const uint8_t *>(rows), c->row_bytes, n, c->row_bias + first, c->stream));
+        B200_CUDA_OK(launch_popc_rows(reinterpret_cast<const uint8_t *>(rows), c->row_bytes, n, c->row_bias.as<float>() + first, c->stream));
     if (c->metric == B200_METRIC_COSINE)
-        B200_CUDA_OK(launch_row_norms(rows, c->dtype == B200_DTYPE_BF16, c->d_pad, n, 1, c->row_scale + first, c->stream));
+        B200_CUDA_OK(launch_row_norms(rows, c->dtype == B200_DTYPE_BF16, c->d_pad, n, 1, c->row_scale.as<float>() + first, c->stream));
     if (c->metric == B200_METRIC_L2)
-        B200_CUDA_OK(launch_row_norms(rows, c->dtype == B200_DTYPE_BF16, c->d_pad, n, 0, c->row_bias + first, c->stream));
+        B200_CUDA_OK(launch_row_norms(rows, c->dtype == B200_DTYPE_BF16, c->d_pad, n, 0, c->row_bias.as<float>() + first, c->stream));
     return B200_OK;
 }
 
@@ -372,7 +333,7 @@ extern "C" int b200_corpus_append(b200_corpus *c, const void *rows, int64_t n) {
 extern "C" int b200_corpus_memory_bytes(const b200_corpus *c, uint64_t *out_bytes) {
     if (!c || !out_bytes) return fail(B200_ERR_INVALID, "bad arguments");
     // rows (as allocated; adopted rows belong to the caller but still occupy HBM) + per-row side arrays
-    uint64_t b = c->owns ? (uint64_t)c->data_cap_bytes : (uint64_t)c->n * (uint64_t)c->row_bytes;
+    uint64_t b = c->owned_rows ? (uint64_t)c->owned_rows.size() : (uint64_t)c->n * (uint64_t)c->row_bytes;
     if (c->row_scale) b += (uint64_t)std::max(c->side_cap_rows, c->n) * 4;
     if (c->row_bias) b += (uint64_t)std::max(c->side_cap_rows, c->n) * 4;
     *out_bytes = b;
@@ -386,12 +347,11 @@ extern "C" int b200_corpus_adopt_device(b200_corpus *c, const void *device_rows,
     if (c->dtype != B200_DTYPE_BIN && c->d != c->d_pad)
         return fail(B200_ERR_INVALID, "adopted rows must already be padded (d % 64 == 0 for bf16, d % 4 == 0 for f32)");
     B200_CUDA_OK(cudaSetDevice(c->device));
+    if (c->metric == B200_METRIC_COSINE) B200_TRY(c->row_scale.alloc((size_t)n * 4 + 256));
+    if (c->metric == B200_METRIC_L2 || c->dtype == B200_DTYPE_BIN) B200_TRY(c->row_bias.alloc((size_t)n * 4 + 256));
     c->data = const_cast<void *>(device_rows);
-    c->owns = false;
     c->n = n;
     c->cap = n;
-    if (c->metric == B200_METRIC_COSINE) B200_CUDA_OK(cudaMalloc(&c->row_scale, (size_t)n * 4 + 256));
-    if (c->metric == B200_METRIC_L2 || c->dtype == B200_DTYPE_BIN) B200_CUDA_OK(cudaMalloc(&c->row_bias, (size_t)n * 4 + 256));
     c->side_cap_rows = n;
     c->epoch++;
     B200_TRY(corpus_norms(c, 0, n));
@@ -451,12 +411,7 @@ extern "C" int b200_corpus_free(b200_corpus *c) {
     if (!c) return B200_OK;
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
-    if (c->data && c->owns) cudaFree(c->data);
-    if (c->row_scale) cudaFree(c->row_scale);
-    if (c->row_bias) cudaFree(c->row_bias);
     if (c->h_pin) cudaFreeHost(c->h_pin);
-    if (c->d_tickets) cudaFree(c->d_tickets);
-    for (DevBuf *b : c->workspaces()) b->release();
     for (auto *v : {&c->ev_used, &c->ev_free})
         for (auto &ev : *v) {
             cudaEventDestroy(ev.first);
@@ -570,7 +525,7 @@ struct RowsView {
     int64_t n;
     const float *row_scale, *row_bias;
 };
-static RowsView full_rows(const b200_corpus *c) { return {c->data, c->n, c->row_scale, c->row_bias}; }
+static RowsView full_rows(const b200_corpus *c) { return {c->data, c->n, c->row_scale.as<float>(), c->row_bias.as<float>()}; }
 
 // ------------------------------------------------------------------------------------
 // search core: everything on device, asynchronous on `s`
@@ -876,8 +831,8 @@ static int search_gathered(b200_corpus *c, const void *d_queries, int64_t nq, in
     B200_TRY(c->w_pf_side.reserve((size_t)side_stride * 2 * 4));
     // only the side arrays search_core reads for this metric: a re-dimensioned per-thread scratch corpus may still hold
     // arrays of another metric, sized for an earlier, smaller part
-    const float *scale = c->metric == B200_METRIC_COSINE ? c->row_scale : nullptr;
-    const float *bias = c->metric == B200_METRIC_L2 || c->dtype == B200_DTYPE_BIN ? c->row_bias : nullptr;
+    const float *scale = c->metric == B200_METRIC_COSINE ? c->row_scale.as<float>() : nullptr;
+    const float *bias = c->metric == B200_METRIC_L2 || c->dtype == B200_DTYPE_BIN ? c->row_bias.as<float>() : nullptr;
     float *cscale = scale ? c->w_pf_side.as<float>() : nullptr, *cbias = bias ? c->w_pf_side.as<float>() + side_stride : nullptr;
     B200_CUDA_OK(launch_prefilter_gather(c->data, c->row_bytes, scale, bias, c->w_pf_ids.as<uint32_t>(), alive, c->w_pf_rows.p,
                                          cscale, cbias, s));
@@ -958,13 +913,11 @@ static int search_host_fused(b200_corpus *c, const float *queries, int64_t nq, i
         c->h_pin_bytes = need;
     }
     if (!c->d_tickets || c->d_tickets_d != c->d) {
-        if (c->d_tickets) cudaFree(c->d_tickets);
-        c->d_tickets = nullptr;
-        B200_CUDA_OK(cudaMalloc(&c->d_tickets, 64 + (size_t)8 * c->d * 4));
-        B200_CUDA_OK(cudaMemsetAsync(c->d_tickets, 0, 64, s));
+        B200_TRY(c->d_tickets.alloc(64 + (size_t)8 * c->d * 4));
+        B200_CUDA_OK(cudaMemsetAsync(c->d_tickets.p, 0, 64, s));
         c->d_tickets_d = c->d;
     }
-    float *d_q = reinterpret_cast<float *>(reinterpret_cast<char *>(c->d_tickets) + 64);
+    float *d_q = reinterpret_cast<float *>(c->d_tickets.as<char>() + 64);
     char *hp = reinterpret_cast<char *>(c->h_pin);
     float *h_q = reinterpret_cast<float *>(hp);
     float *h_dis = reinterpret_cast<float *>(hp + (size_t)8 * c->d * 4);
@@ -1001,7 +954,7 @@ static int search_host_fused(b200_corpus *c, const float *queries, int64_t nq, i
     ScanParams sp{};
     sp.corpus = c->data;
     sp.queries = d_q;
-    sp.row_scale = c->metric == B200_METRIC_COSINE ? c->row_scale : nullptr;
+    sp.row_scale = c->metric == B200_METRIC_COSINE ? c->row_scale.as<float>() : nullptr;
     sp.alive = d_alive;
     sp.part_keys = c->w_pk.as<float>();
     sp.part_ids = c->w_pi.as<uint32_t>();
@@ -1019,8 +972,8 @@ static int search_host_fused(b200_corpus *c, const float *queries, int64_t nq, i
     sp.out_mode = c->metric == B200_METRIC_L2 ? kOutKey : c->metric == B200_METRIC_IP ? kOutNeg : kOutOnePlus;
     sp.ip_min_quirk = ip_min_quirk && c->metric == B200_METRIC_IP;
     sp.id_offset = 0;
-    sp.tickets = c->d_tickets;
-    sp.tiles_done = c->d_tickets + 8;
+    sp.tickets = c->d_tickets.as<unsigned int>();
+    sp.tiles_done = c->d_tickets.as<unsigned int>() + 8;
     sp.out_dis = reinterpret_cast<float *>(dpc + (reinterpret_cast<char *>(h_dis) - hp));
     sp.out_ids = reinterpret_cast<int64_t *>(dpc + (reinterpret_cast<char *>(h_ids) - hp));
     sp.done_flag = reinterpret_cast<volatile unsigned int *>(dpc + need - 16);
@@ -1102,34 +1055,22 @@ extern "C" int b200_corpus_search(b200_corpus *c, const float *queries, int64_t 
 // The host-buffer entry points (b200_flat_knn / b200_binary_knn / b200_part_scan) are called once per part or per
 // mark by each ClickHouse worker thread: they reuse one scratch corpus per thread (device buffers, stream and
 // workspaces grow-only) instead of paying cudaMalloc / cudaStreamCreate on every call.
-struct ScratchCorpus {
-    b200_corpus *c = nullptr;
-    ~ScratchCorpus() {
-        if (c) b200_corpus_free(c);
-    }
-};
-static thread_local ScratchCorpus t_scratch;
+static thread_local CorpusPtr t_scratch;
 
 // gives this thread's scratch corpus (device buffers sized for the largest part it has scanned) back to the driver
 extern "C" int b200_thread_release(void) {
-    if (t_scratch.c) {
-        b200_corpus_free(t_scratch.c);
-        t_scratch.c = nullptr;
-    }
+    t_scratch.reset();
     return B200_OK;
 }
 
 static int scratch_corpus(int metric, int dtype, int d, int64_t rows, b200_corpus **out) {
-    b200_corpus *c = t_scratch.c;
     int dev = 0;
     cudaGetDevice(&dev);
-    if (c && (c->device != dev || !c->owns)) {
-        b200_corpus_free(c);
-        c = t_scratch.c = nullptr;
-    }
+    if (t_scratch && (t_scratch->device != dev || (t_scratch->data && !t_scratch->owned_rows))) t_scratch.reset();
+    b200_corpus *c = t_scratch.get();
     if (!c) {
         B200_TRY(b200_corpus_create(metric, dtype, d, rows, &c));
-        t_scratch.c = c;
+        t_scratch.reset(c);
         *out = c;
         return B200_OK;
     }

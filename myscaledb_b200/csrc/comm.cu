@@ -78,12 +78,9 @@ struct b200_comm {
     ncclComm_t comm = nullptr;
     NcclApi *api = nullptr;
     int rank = 0, world = 1, device = 0;
-    void *send = nullptr, *recv = nullptr;   // packed records: one / world of them
-    size_t send_cap = 0, recv_cap = 0;
-    uint64_t *d_counters = nullptr;          // all-reduce scratch
-    size_t counters_cap = 0;
-    void *d_host_out = nullptr;              // merged result of the host-buffer gather
-    size_t host_out_cap = 0;
+    DevMem send, recv;                       // packed records: one / world of them
+    DevMem d_counters;                       // uint64 all-reduce scratch
+    DevMem d_host_out;                       // merged result of the host-buffer gather
     std::mutex mu;
     // CUDA graphs of whole sharded search steps, keyed by the corpus' serial number and the call's arguments; the corpus'
     // state epoch at capture says whether the rows, side arrays, path and workspaces the nodes point at are still current
@@ -94,8 +91,7 @@ struct b200_comm {
     };
     std::map<std::tuple<uint64_t, const void *, int64_t, int, const void *, int64_t, void *, void *, void *>, Graph> graphs;
     int64_t graph_captures = 0, graph_replays = 0;
-    void *host_stage = nullptr;                          // device staging of the host-buffer entry point
-    size_t host_stage_cap = 0;
+    DevMem host_stage;                                   // device staging of the host-buffer entry point
 };
 
 // The packed record of one rank: dis [nq * k] fp32, padded to a multiple of 8 bytes, then ids [nq * k] int64.  The record
@@ -156,8 +152,6 @@ extern "C" int b200_comm_free(b200_comm *c) {
     cudaDeviceSynchronize();
     drop_graphs(c);
     if (c->comm) c->api->CommDestroy(c->comm);
-    for (void *p : {c->send, c->recv, (void *)c->d_counters, c->host_stage, c->d_host_out})
-        if (p) cudaFree(p);
     delete c;
     return B200_OK;
 }
@@ -171,19 +165,14 @@ extern "C" int b200_comm_info(const b200_comm *c, int *rank, int *world) {
 
 static int comm_reserve(b200_comm *c, int64_t nq, int k) {
     const size_t rec = record_bytes(nq, k);
-    if (rec > c->send_cap) {
-        if (c->send) cudaFree(c->send);
-        if (c->recv) cudaFree(c->recv);
-        c->send = c->recv = nullptr;
-        c->send_cap = c->recv_cap = 0;
+    if (rec > c->send.size()) {
+        c->send.reset();
+        c->recv.reset();
         drop_graphs(c);   // captured pointers are gone
-        const size_t want = rec + rec / 4 + 256;
-        if (cudaMalloc(&c->send, want) != cudaSuccess || cudaMalloc(&c->recv, want * c->world) != cudaSuccess) {
-            cudaGetLastError();
+        if (c->send.reserve(rec) != B200_OK || c->recv.alloc(c->send.size() * c->world) != B200_OK) {
+            c->send.reset();
             return fail(B200_ERR_NOMEM, "cudaMalloc of the all-gather buffers failed");
         }
-        c->send_cap = want;
-        c->recv_cap = want * c->world;
     }
     return B200_OK;
 }
@@ -194,8 +183,8 @@ extern "C" int b200_comm_local_buffers(b200_comm *c, int64_t nq, int k, float **
     std::lock_guard<std::mutex> lk(c->mu);
     B200_CUDA_OK(cudaSetDevice(c->device));
     B200_TRY(comm_reserve(c, std::max<int64_t>(nq, 1), k));
-    *d_dis = reinterpret_cast<float *>(c->send);
-    *d_ids = record_ids(c->send, nq, k);
+    *d_dis = c->send.as<float>();
+    *d_ids = record_ids(c->send.p, nq, k);
     return B200_OK;
 }
 
@@ -207,17 +196,17 @@ extern "C" int b200_comm_gather_merge(b200_comm *c, int64_t nq, int k, int desce
     if (nq == 0) return B200_OK;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     const size_t rec = record_bytes(nq, k);
-    if (rec > c->send_cap) return fail(B200_ERR_INVALID, "call b200_comm_local_buffers(nq, k) first");
+    if (rec > c->send.size()) return fail(B200_ERR_INVALID, "call b200_comm_local_buffers(nq, k) first");
     if (c->world == 1) {
-        B200_CUDA_OK(cudaMemcpyAsync(d_out_dis, c->send, (size_t)nq * k * 4, cudaMemcpyDeviceToDevice, s));
-        B200_CUDA_OK(cudaMemcpyAsync(d_out_ids, record_ids(c->send, nq, k), (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, s));
+        B200_CUDA_OK(cudaMemcpyAsync(d_out_dis, c->send.p, (size_t)nq * k * 4, cudaMemcpyDeviceToDevice, s));
+        B200_CUDA_OK(cudaMemcpyAsync(d_out_ids, record_ids(c->send.p, nq, k), (size_t)nq * k * 8, cudaMemcpyDeviceToDevice, s));
         return B200_OK;
     }
-    B200_NCCL_OK(c, c->api->AllGather(c->send, c->recv, rec, ncclUint8, c->comm, s));
+    B200_NCCL_OK(c, c->api->AllGather(c->send.p, c->recv.p, rec, ncclUint8, c->comm, s));
     g_launches++;
     // list l of the gathered buffer: dis at recv + l * rec, ids record_dis_bytes further; rec is a multiple of 8, so the
     // strides are whole elements of both types
-    return b200_topk_merge_device_ex(reinterpret_cast<const float *>(c->recv), record_ids(c->recv, nq, k), c->world, (int64_t)(rec / 4),
+    return b200_topk_merge_device_ex(c->recv.as<const float>(), record_ids(c->recv.p, nq, k), c->world, (int64_t)(rec / 4),
                                      (int64_t)(rec / 8), nq, k, k, descending, 0, d_out_dis, d_out_ids, nullptr, stream ? stream : nullptr);
 }
 
@@ -238,15 +227,9 @@ extern "C" int b200_comm_gather_merge_host(b200_comm *c, const float *h_dis, con
     B200_TRY(b200_comm_local_buffers(c, nq, k, &d_dis, &d_ids));
     std::lock_guard<std::mutex> lk(c->mu);
     const size_t nd = (size_t)nq * k * 4, ni = (size_t)nq * k * 8;
-    if (nd + ni > c->host_out_cap) {
-        if (c->d_host_out) cudaFree(c->d_host_out);
-        c->d_host_out = nullptr;
-        c->host_out_cap = 0;
-        B200_CUDA_OK(cudaMalloc(&c->d_host_out, nd + ni + 256));
-        c->host_out_cap = nd + ni + 256;
-    }
-    float *o_dis = reinterpret_cast<float *>(c->d_host_out);
-    int64_t *o_ids = reinterpret_cast<int64_t *>(reinterpret_cast<char *>(c->d_host_out) + ((nd + 7) & ~(size_t)7));
+    if (nd + ni > c->d_host_out.size()) B200_TRY(c->d_host_out.alloc(nd + ni + 256));
+    float *o_dis = c->d_host_out.as<float>();
+    int64_t *o_ids = reinterpret_cast<int64_t *>(c->d_host_out.as<char>() + ((nd + 7) & ~(size_t)7));
     B200_CUDA_OK(cudaMemcpyAsync(d_dis, h_dis, nd, cudaMemcpyHostToDevice, nullptr));
     B200_CUDA_OK(cudaMemcpyAsync(d_ids, h_ids, ni, cudaMemcpyHostToDevice, nullptr));
     B200_TRY(b200_comm_gather_merge(c, nq, k, descending, o_dis, o_ids, nullptr));
@@ -263,17 +246,12 @@ extern "C" int b200_comm_allreduce_sum_u64(b200_comm *c, uint64_t *host_counters
     if (n == 0 || c->world == 1) return B200_OK;
     std::lock_guard<std::mutex> lk(c->mu);
     B200_CUDA_OK(cudaSetDevice(c->device));
-    if ((size_t)n * 8 > c->counters_cap) {
-        if (c->d_counters) cudaFree(c->d_counters);
-        c->d_counters = nullptr;
-        B200_CUDA_OK(cudaMalloc(&c->d_counters, (size_t)n * 8 + 256));
-        c->counters_cap = (size_t)n * 8 + 256;
-    }
-    B200_CUDA_OK(cudaMemcpy(c->d_counters, host_counters, (size_t)n * 8, cudaMemcpyHostToDevice));
-    B200_NCCL_OK(c, c->api->AllReduce(c->d_counters, c->d_counters, (size_t)n, ncclUint64, ncclSum, c->comm, nullptr));
+    if ((size_t)n * 8 > c->d_counters.size()) B200_TRY(c->d_counters.alloc((size_t)n * 8 + 256));
+    B200_CUDA_OK(cudaMemcpy(c->d_counters.p, host_counters, (size_t)n * 8, cudaMemcpyHostToDevice));
+    B200_NCCL_OK(c, c->api->AllReduce(c->d_counters.p, c->d_counters.p, (size_t)n, ncclUint64, ncclSum, c->comm, nullptr));
     g_launches++;
     B200_CUDA_OK(cudaStreamSynchronize(nullptr));
-    B200_CUDA_OK(cudaMemcpy(host_counters, c->d_counters, (size_t)n * 8, cudaMemcpyDeviceToHost));
+    B200_CUDA_OK(cudaMemcpy(host_counters, c->d_counters.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
     return B200_OK;
 }
 
@@ -296,8 +274,8 @@ int index_metric(const b200_index *ix);
 
 static int sharded_corpus_step(b200_comm *cm, b200_corpus *corpus, const float *d_queries, int64_t nq, int k, const uint8_t *d_alive,
                                int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
-    float *l_dis = reinterpret_cast<float *>(cm->send);
-    int64_t *l_ids = record_ids(cm->send, nq, k);
+    float *l_dis = cm->send.as<float>();
+    int64_t *l_ids = record_ids(cm->send.p, nq, k);
     B200_TRY(b200_corpus_search_device(corpus, d_queries, nq, k, d_alive, id_offset, l_dis, l_ids, s));
     return b200_comm_gather_merge(cm, nq, k, corpus_metric(corpus) == B200_METRIC_IP ? 1 : 0, d_out_dis, d_out_ids, s);
 }
@@ -385,17 +363,13 @@ extern "C" int b200_sharded_corpus_search_host(b200_comm *cm, b200_corpus *corpu
         std::lock_guard<std::mutex> lk(cm->mu);
         B200_CUDA_OK(cudaSetDevice(cm->device));
         const size_t need = round_up(q_bytes, 16) + round_up((size_t)nq * k * 4, 16) + (size_t)nq * k * 8;
-        if (need > cm->host_stage_cap) {
-            if (cm->host_stage) cudaFree(cm->host_stage);
-            cm->host_stage = nullptr;
-            cm->host_stage_cap = 0;
-            drop_graphs(cm);
-            B200_CUDA_OK(cudaMalloc(&cm->host_stage, need + need / 4));
-            cm->host_stage_cap = need + need / 4;
+        if (need > cm->host_stage.size()) {
+            drop_graphs(cm);   // captured pointers are about to go
+            B200_TRY(cm->host_stage.alloc(need + need / 4));
         }
     }
-    float *d_q = reinterpret_cast<float *>(cm->host_stage);
-    float *d_od = reinterpret_cast<float *>(reinterpret_cast<char *>(cm->host_stage) + round_up(q_bytes, 16));
+    float *d_q = cm->host_stage.as<float>();
+    float *d_od = reinterpret_cast<float *>(cm->host_stage.as<char>() + round_up(q_bytes, 16));
     int64_t *d_oi = reinterpret_cast<int64_t *>(reinterpret_cast<char *>(d_od) + round_up((size_t)nq * k * 4, 16));
     B200_CUDA_OK(cudaMemcpyAsync(d_q, queries, q_bytes, cudaMemcpyHostToDevice, s));
     B200_TRY(b200_sharded_corpus_search(cm, corpus, d_q, nq, k, nullptr, id_offset, d_od, d_oi, stream, use_graph));
@@ -415,8 +389,8 @@ extern "C" int b200_sharded_index_search(b200_comm *cm, b200_index *ix, int metr
     std::lock_guard<std::mutex> lk(cm->mu);
     B200_CUDA_OK(cudaSetDevice(cm->device));
     B200_TRY(comm_reserve(cm, nq, k));
-    float *l_dis = reinterpret_cast<float *>(cm->send);
-    int64_t *l_ids = record_ids(cm->send, nq, k);
+    float *l_dis = cm->send.as<float>();
+    int64_t *l_ids = record_ids(cm->send.p, nq, k);
     B200_TRY(b200_index_search_device(ix, d_queries, nq, k, params, 0, d_alive_bits, id_offset, l_dis, l_ids, stream));
     return b200_comm_gather_merge(cm, nq, k, metric == B200_METRIC_IP ? 1 : 0, d_out_dis, d_out_ids, stream);
 }

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include <atomic>
+#include <memory>
 #include <float.h>
 #include <string>
 
@@ -29,6 +31,70 @@ extern thread_local int64_t g_launches;
         int _rc = (expr);          \
         if (_rc != B200_OK) return _rc; \
     } while (0)
+
+// bytes the DevMem buffers of the process hold (b200_device_bytes)
+inline std::atomic<int64_t> g_device_bytes{0};
+
+// The one owner of device memory: every cudaMalloc and cudaFree of the library is here.  Move-only; the destructor frees.
+// cudaFree waits for the device, so a buffer dropped on an error path is never freed under a kernel still reading it.
+struct DevMem {
+    void *p = nullptr;
+    size_t cap = 0;
+    uint64_t reallocs = 0;   // times p changed: a CUDA graph that baked p in is stale once this moves (corpus_state_epoch)
+
+    DevMem() = default;
+    DevMem(const DevMem &) = delete;
+    DevMem &operator=(const DevMem &) = delete;
+    DevMem(DevMem &&o) noexcept : p(o.p), cap(o.cap) {
+        o.p = nullptr;
+        o.cap = 0;
+    }
+    DevMem &operator=(DevMem &&o) noexcept {
+        if (this != &o) {
+            reset();
+            p = o.p;
+            cap = o.cap;
+            o.p = nullptr;
+            o.cap = 0;
+        }
+        return *this;
+    }
+    ~DevMem() { reset(); }
+
+    // exactly `bytes`, in place of what the buffer held
+    int alloc(size_t bytes) {
+        reset();
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            p = nullptr;
+            return fail(B200_ERR_NOMEM, "cudaMalloc(" + std::to_string(bytes) + ") failed: " + cudaGetErrorString(e));
+        }
+        cap = bytes;
+        g_device_bytes += (int64_t)bytes;
+        return B200_OK;
+    }
+    // grow-only workspace: at least `bytes`, with a quarter of slack so that slowly growing batches rarely reallocate
+    int reserve(size_t bytes) { return bytes <= cap ? B200_OK : alloc(bytes + bytes / 4 + 256); }
+    void reset() {
+        reallocs++;
+        if (!p) return;
+        cudaFree(p);
+        g_device_bytes -= (int64_t)cap;
+        p = nullptr;
+        cap = 0;
+    }
+    template <typename T>
+    T *as() const { return reinterpret_cast<T *>(p); }
+    size_t size() const { return cap; }
+    explicit operator bool() const { return p != nullptr; }
+};
+
+// a corpus the library created for itself, freed with b200_corpus_free
+struct CorpusFree {
+    void operator()(b200_corpus *c) const { b200_corpus_free(c); }
+};
+using CorpusPtr = std::unique_ptr<b200_corpus, CorpusFree>;
 
 __host__ __device__ static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 __host__ __device__ static inline int64_t round_up(int64_t a, int64_t b) { return ceil_div(a, b) * b; }

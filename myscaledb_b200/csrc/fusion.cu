@@ -164,31 +164,27 @@ extern "C" int b200_hybrid_fusion_batch(int fusion_type, int64_t nq, const uint3
     int dev = 0;
     B200_CUDA_OK(cudaGetDevice(&dev));
     static std::mutex g_mu;
-    struct Scratch {
-        char *d = nullptr, *h = nullptr;
-        size_t cap = 0;
+    struct PerDevice {
+        DevMem d;
+        char *h = nullptr;
         cudaStream_t s = nullptr;
     };
-    static Scratch g_scratch[64];
+    static PerDevice g_scratch[64];
     if (dev < 0 || dev >= 64) return fail(B200_ERR_UNSUPPORTED, "device ordinal above 63");
     std::lock_guard<std::mutex> lk(g_mu);
-    Scratch &sc = g_scratch[dev];
+    PerDevice &sc = g_scratch[dev];
     if (!sc.s) B200_CUDA_OK(cudaStreamCreateWithFlags(&sc.s, cudaStreamNonBlocking));
-    if (off + 256 > sc.cap) {
-        if (sc.d) cudaFree(sc.d);
+    if (off + 256 > sc.d.size()) {
         if (sc.h) cudaFreeHost(sc.h);
-        sc.d = sc.h = nullptr;
-        sc.cap = 0;
+        sc.h = nullptr;
         const size_t want = (off + 256) * 2;
-        B200_CUDA_OK(cudaMalloc(&sc.d, want));
+        B200_TRY(sc.d.alloc(want));
         if (cudaMallocHost(&sc.h, want) != cudaSuccess) {
-            cudaFree(sc.d);
-            sc.d = nullptr;
+            sc.d.reset();
             return fail(B200_ERR_NOMEM, "cudaMallocHost failed in fusion");
         }
-        sc.cap = want;
     }
-    char *d = sc.d;
+    char *d = sc.d.as<char>();
     cudaStream_t s = sc.s;
     int rc = B200_OK;
     // inputs: packed into the pinned mirror at their carved offsets, then ONE copy (o_vs .. end of o_tc is contiguous)

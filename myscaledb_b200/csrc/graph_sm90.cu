@@ -166,32 +166,24 @@ int graph_merge(const uint32_t *d_pruned, int64_t n, int D, uint32_t *d_graph, c
     if (n == 0) return B200_OK;
     const int64_t e = n * D;
     if (e >= (int64_t)1 << 31) return fail(B200_ERR_UNSUPPORTED, "graph build: n x graph_degree must stay below 2^31");
-    uint64_t *keys = nullptr, *keys_out = nullptr;
-    uint32_t *vals = nullptr, *vals_out = nullptr;
-    void *tmp = nullptr;
+    DevMem keys, keys_out, vals, vals_out, tmp;
     size_t tb = 0;
     int end_bit = 1;
     while (end_bit < 64 && ((uint64_t)e >> end_bit) != 0) end_bit++;
-    cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, keys_out, vals, vals_out, (int)e, 0, end_bit, s);
-    int rc = B200_OK;
-    if (cudaMalloc(&keys, (size_t)e * 8) != cudaSuccess || cudaMalloc(&keys_out, (size_t)e * 8) != cudaSuccess ||
-        cudaMalloc(&vals, (size_t)e * 4) != cudaSuccess || cudaMalloc(&vals_out, (size_t)e * 4) != cudaSuccess ||
-        cudaMalloc(&tmp, tb + 256) != cudaSuccess) {
-        cudaGetLastError();
-        rc = fail(B200_ERR_NOMEM, "graph build: cudaMalloc of the reverse-edge scratch failed (" + std::to_string(e * 24) + " bytes)");
-    }
-    if (rc == B200_OK) {
-        graph_triples_kernel<<<(unsigned)ceil_div(e, 256), 256, 0, s>>>(d_pruned, n, D, keys, vals);
-        // stable: equal (B, r) keys keep the A-ascending order of the triples
-        cub::DeviceRadixSort::SortPairs(tmp, tb, keys, keys_out, vals, vals_out, (int)e, 0, end_bit, s);
-        graph_merge_kernel<<<(unsigned)ceil_div(n, 128), 128, 0, s>>>(d_pruned, keys_out, vals_out, n, D, d_graph);
-        g_launches += 3;
-        const cudaError_t err = cudaStreamSynchronize(s);
-        if (err != cudaSuccess) rc = fail(B200_ERR_CUDA, std::string("graph merge: ") + cudaGetErrorString(err));
-    }
-    for (void *p : {(void *)keys, (void *)keys_out, (void *)vals, (void *)vals_out, tmp})
-        if (p) cudaFree(p);
-    return rc;
+    cub::DeviceRadixSort::SortPairs(nullptr, tb, keys.as<uint64_t>(), keys_out.as<uint64_t>(), vals.as<uint32_t>(), vals_out.as<uint32_t>(), (int)e, 0,
+                                    end_bit, s);
+    if (keys.alloc((size_t)e * 8) != B200_OK || keys_out.alloc((size_t)e * 8) != B200_OK || vals.alloc((size_t)e * 4) != B200_OK ||
+        vals_out.alloc((size_t)e * 4) != B200_OK || tmp.alloc(tb + 256) != B200_OK)
+        return fail(B200_ERR_NOMEM, "graph build: cudaMalloc of the reverse-edge scratch failed (" + std::to_string(e * 24) + " bytes)");
+    graph_triples_kernel<<<(unsigned)ceil_div(e, 256), 256, 0, s>>>(d_pruned, n, D, keys.as<uint64_t>(), vals.as<uint32_t>());
+    // stable: equal (B, r) keys keep the A-ascending order of the triples
+    cub::DeviceRadixSort::SortPairs(tmp.p, tb, keys.as<uint64_t>(), keys_out.as<uint64_t>(), vals.as<uint32_t>(), vals_out.as<uint32_t>(), (int)e, 0, end_bit,
+                                    s);
+    graph_merge_kernel<<<(unsigned)ceil_div(n, 128), 128, 0, s>>>(d_pruned, keys_out.as<uint64_t>(), vals_out.as<uint32_t>(), n, D, d_graph);
+    g_launches += 3;
+    const cudaError_t err = cudaStreamSynchronize(s);
+    if (err != cudaSuccess) return fail(B200_ERR_CUDA, std::string("graph merge: ") + cudaGetErrorString(err));
+    return B200_OK;
 }
 
 // One CTA per list walks its page chain, thread t on row t of every page (as list_alive_kernel in ivf.cu): the list's valid

@@ -1227,31 +1227,6 @@ static const char *kTypeNames[] = {"FLAT", "IVFFLAT", "IVFPQ", "MSTG", "IVFSQ", 
                                    "BINARYFLAT", "BINARYIVF", "BINARYHNSW", "BINARYMSTG"};
 static bool is_flat_type(int t) { return t == IDX_FLAT || t == IDX_BINFLAT; }
 
-struct DevArr {
-    void *p = nullptr;
-    size_t cap = 0;
-    int reserve(size_t bytes) {
-        if (bytes <= cap) return B200_OK;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        const size_t want = bytes + bytes / 4 + 256;
-        if (cudaMalloc(&p, want) != cudaSuccess) {
-            cudaGetLastError();
-            return fail(B200_ERR_NOMEM, "cudaMalloc(" + std::to_string(want) + ") failed (index workspace)");
-        }
-        cap = want;
-        return B200_OK;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-    template <typename T>
-    T *as() const { return reinterpret_cast<T *>(p); }
-};
-
 struct b200_index {
     int type = IDX_FLAT, metric = B200_METRIC_L2, d = 0, d_pad = 0, d_pad64 = 0;
     int nlist = 0, m = 0, dsub = 0;
@@ -1264,7 +1239,7 @@ struct b200_index {
     // in the rotated space, the fp32 rows do not.  opq_loss: the sample's mean PQ loss at R = I, then after each of the
     // opq_iters alternations (empty on a loaded index).  A part below the inverted-file threshold keeps no R.
     int opq = 0, opq_iters = 20;
-    float *d_opq = nullptr;
+    DevMem d_opq;                   // float [d][d]
     std::vector<double> opq_loss;
     int default_nprobe = 32, refine_factor = 4;
     int payload = IVF_PRODUCER_TMA;
@@ -1272,45 +1247,45 @@ struct b200_index {
     int code_bytes = 0;
     int64_t n = 0, reserved = 0;
     bool trained = false, built = false, use_ivf = false;
-    b200_corpus *raw = nullptr;     // fp32 rows in id order (cosine: unit vectors), metric L2 or IP
+    CorpusPtr raw;                  // fp32 rows in id order (cosine: unit vectors), metric L2 or IP
     // keep_raw=2 on an inverted-file float index: raw's rows [h_rows_cap][d_pad] (same values, zero padding) in pinned,
     // mapped host memory instead; the second stage gathers its candidates over PCIe
     float *h_rows = nullptr;
     const float *h_rows_dev = nullptr;   // the device's address of h_rows
     int64_t h_rows_cap = 0;
-    b200_corpus *coarse = nullptr;  // centroid table as a FLAT corpus (L2)
-    float *d_centroids = nullptr;   // [nlist][d]
-    float *d_cnorm = nullptr;       // [nlist] ||c||^2 (coarse probe)
-    float *d_pq = nullptr;          // [m][256][dsub] fp32
-    __nv_bfloat16 *d_pq_bf16 = nullptr;
-    float *d_sq = nullptr;          // [4][d]: lo, step, 1/step, mid
+    CorpusPtr coarse;               // centroid table as a FLAT corpus (L2)
+    DevMem d_centroids;             // float [nlist][d]
+    DevMem d_cnorm;                 // float [nlist] ||c||^2 (coarse probe)
+    DevMem d_pq;                    // float [m][256][dsub]
+    DevMem d_pq_bf16;               // bf16 [m][256][dsub]
+    DevMem d_sq;                    // float [4][d]: lo, step, 1/step, mid
     // paged lists
     uint32_t pool_pages = 0, pages_used = 0;
-    void *d_pool = nullptr;         // bf16 [pool_pages * 256][d_pad64]  |  codes [pool_pages * 256][code_bytes]
-    float *d_row_bias = nullptr;
-    uint32_t *d_row_ids = nullptr;
-    uint32_t *d_list_len = nullptr, *d_tail_page = nullptr, *d_page_owner = nullptr, *d_page_seq = nullptr, *d_pages_used = nullptr;
-    int *d_flag = nullptr;
-    uint32_t *d_list_page_off = nullptr, *d_list_pages = nullptr, *d_list_order = nullptr;   // after finalize
+    DevMem d_pool;                  // bf16 [pool_pages * 256][d_pad64]  |  codes [pool_pages * 256][code_bytes]
+    DevMem d_row_bias;              // float [pool rows]
+    DevMem d_row_ids;               // uint32 [pool rows]; the uint32 arrays below: [nlist], [nlist], [pages], [pages], [1]
+    DevMem d_list_len, d_tail_page, d_page_owner, d_page_seq, d_pages_used;
+    DevMem d_flag;                  // int [8]
+    DevMem d_list_page_off, d_list_pages, d_list_order;   // uint32, after finalize
     std::vector<uint32_t> list_len;  // host copy after finalize
     // binary indexes: rows are bytes [n][row_bytes]; pages [page][row_pad / kb_w][256 rows][kb_w bytes]; the coarse table is
     // d_bcent zero-padded to cent_pad (16-byte) rows, searched as a Hamming corpus (zero bits change no distance)
     bool binary = false;
     int row_bytes = 0, kb_w = 0, row_pad = 0, cent_pad = 0;
-    uint8_t *d_bcent = nullptr;     // [nlist][cent_pad]
+    DevMem d_bcent;                 // uint8 [nlist][cent_pad]
     uint32_t max_list_pages = 0;
     int device = 0, sms = 132;
     cudaStream_t stream = nullptr;
     std::mutex mu;
     // workspaces (grow-only)
-    DevArr w_rows, w_assign_i, w_assign_d, w_u32a, w_u32b, w_u32c, w_u32d, w_cnt, w_plan, w_sort, w_q, w_qraw, w_probe, w_pd, w_items,
+    DevMem w_rows, w_assign_i, w_assign_d, w_u32a, w_u32b, w_u32c, w_u32d, w_cnt, w_plan, w_sort, w_q, w_qraw, w_probe, w_pd, w_items,
         w_qbuf, w_inv, w_ppb, w_pconst, w_qconst, w_qb, w_cs, w_pk, w_pi, w_pw, w_lk, w_li, w_alive, w_od, w_oi, w_cand, w_host_q, w_ppopc, w_lut,
         w_stage, w_qrot;
     // build: one flag per row of the chunk or training sample, 1 = usable (row_usable_kernel)
-    DevArr w_usable;
+    DevMem w_usable;
     // filter_probe=1 (per search): list_alive and the filtered lengths [2][nlist], the filtered page table [pages_used], the
     // per-query selection (p_q, cut key, cut ties, then the Σ / max totals); pinned host copy of the totals and of every p_q
-    DevArr w_flist, w_fpages, w_fsel;
+    DevMem w_flist, w_fpages, w_fsel;
     void *h_fsel = nullptr;
     size_t h_fsel_cap = 0;
     // lists each query of the last search probed (b200_index_last_probe), and whether the filter_probe exact rule answered it
@@ -1323,9 +1298,9 @@ struct b200_index {
     // (graph_sm90.cu); MSTG and BINARYMSTG walk their bf16 / binary list rows in place: d_row_slot[n] = row id -> pool slot,
     // derived from the page chains at finalize and at load (never saved: a load may place the pages elsewhere)
     int graph_degree = 0;
-    uint32_t *d_graph = nullptr, *d_row_slot = nullptr;
+    DevMem d_graph, d_row_slot;     // uint32
     // seed ids [last_seed_nq][last_seed_s] of the last graph search (b200_index_last_seeds), and their first-stage distances
-    DevArr w_seeds, w_seedd;
+    DevMem w_seeds, w_seedd;
     int64_t last_seed_nq = 0;
     int last_seed_s = 0;
     bool last_graph = false;        // the last search walked the graph: last_scan reports the rows it scored
@@ -1510,20 +1485,7 @@ extern "C" int b200_index_free(b200_index *ix) {
     if (!ix) return B200_OK;
     cudaSetDevice(ix->device);
     if (ix->stream) cudaStreamSynchronize(ix->stream);
-    if (ix->raw) b200_corpus_free(ix->raw);
     if (ix->h_rows) cudaFreeHost(ix->h_rows);
-    if (ix->coarse) b200_corpus_free(ix->coarse);
-    for (void *p : {(void *)ix->d_centroids, (void *)ix->d_bcent, (void *)ix->d_cnorm, (void *)ix->d_pq, (void *)ix->d_pq_bf16, (void *)ix->d_sq, ix->d_pool, (void *)ix->d_row_bias,
-                    (void *)ix->d_row_ids, (void *)ix->d_list_len, (void *)ix->d_tail_page, (void *)ix->d_page_owner, (void *)ix->d_page_seq,
-                    (void *)ix->d_pages_used, (void *)ix->d_flag, (void *)ix->d_list_page_off, (void *)ix->d_list_pages, (void *)ix->d_list_order, (void *)ix->d_graph,
-                    (void *)ix->d_row_slot, (void *)ix->d_opq})
-        if (p) cudaFree(p);
-    for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_cnt, &ix->w_plan,
-                      &ix->w_sort, &ix->w_q, &ix->w_qraw, &ix->w_probe, &ix->w_pd, &ix->w_items, &ix->w_qbuf, &ix->w_inv, &ix->w_ppb, &ix->w_pconst, &ix->w_qb, &ix->w_cs,
-                      &ix->w_qconst, &ix->w_pk, &ix->w_pi, &ix->w_pw, &ix->w_lk, &ix->w_li, &ix->w_alive, &ix->w_od, &ix->w_oi, &ix->w_cand,
-                      &ix->w_host_q, &ix->w_ppopc, &ix->w_lut, &ix->w_stage, &ix->w_flist, &ix->w_fpages, &ix->w_fsel,
-                      &ix->w_seeds, &ix->w_seedd, &ix->w_usable, &ix->w_qrot})
-        a->release();
     if (ix->h_fsel) cudaFreeHost(ix->h_fsel);
     if (ix->ev0) cudaEventDestroy(ix->ev0);
     if (ix->ev1) cudaEventDestroy(ix->ev1);
@@ -1586,41 +1548,48 @@ static int host_rows_reserve(b200_index *ix, int64_t rows) {
     return B200_OK;
 }
 
+// a new empty corpus in `out`, whose old one is freed first
+static int corpus_create(int metric, int dtype, int d, int64_t capacity_rows, CorpusPtr &out) {
+    out.reset();
+    b200_corpus *c = nullptr;
+    B200_TRY(b200_corpus_create(metric, dtype, d, capacity_rows, &c));
+    out.reset(c);
+    return B200_OK;
+}
+
 // k-means on device rows x [n][stride]; centroids written to d_c [nc][d].  Assignment: exact top-1 search of the centroid
 // table with the FLAT engine (tensor cores from 20 rows up) when the table is large, the tiled fp32 kernel otherwise.
 // warm: start from the centroids already in d_c (OPQ's alternations) instead of nc evenly strided rows.
 static int kmeans_device(const float *x, int64_t n, int64_t stride, int d, int nc, int iters, float *d_c, cudaStream_t s, bool warm = false) {
     std::vector<int64_t> pick(nc);
     for (int i = 0; i < nc; i++) pick[i] = (int64_t)((double)i * (double)n / (double)nc);
-    int64_t *d_pick = nullptr;
-    float *d_sums = nullptr, *d_cn = nullptr, *d_dis = nullptr;
-    uint32_t *d_cnt = nullptr, *d_idx = nullptr;
-    int64_t *d_idx64 = nullptr;
-    B200_CUDA_OK(cudaMalloc(&d_pick, (size_t)nc * 8));
-    B200_CUDA_OK(cudaMalloc(&d_sums, (size_t)nc * d * 4));
-    B200_CUDA_OK(cudaMalloc(&d_cn, (size_t)nc * 4));
-    B200_CUDA_OK(cudaMalloc(&d_cnt, (size_t)nc * 4));
-    B200_CUDA_OK(cudaMalloc(&d_idx, (size_t)n * 4));
+    DevMem pick_b, sums_b, cn_b, cnt_b, idx_b, idx64_b, dis_b;
+    B200_TRY(pick_b.alloc((size_t)nc * 8));
+    B200_TRY(sums_b.alloc((size_t)nc * d * 4));
+    B200_TRY(cn_b.alloc((size_t)nc * 4));
+    B200_TRY(cnt_b.alloc((size_t)nc * 4));
+    B200_TRY(idx_b.alloc((size_t)n * 4));
+    int64_t *d_pick = pick_b.as<int64_t>();
+    float *d_sums = sums_b.as<float>(), *d_cn = cn_b.as<float>();
+    uint32_t *d_cnt = cnt_b.as<uint32_t>(), *d_idx = idx_b.as<uint32_t>();
     if (!warm) {
         B200_CUDA_OK(cudaMemcpyAsync(d_pick, pick.data(), (size_t)nc * 8, cudaMemcpyHostToDevice, s));
         gather_rows_kernel<<<gridsz((int64_t)nc * d), 256, 0, s>>>(x, stride, d_pick, nc, d, d_c);
         g_launches++;
     }
     const bool big = (double)n * nc * d > 2e11 && stride == d;   // tensor-core assignment pays from ~0.2 TFLOP per iteration
-    b200_corpus *table = nullptr;
     if (big) {
-        B200_CUDA_OK(cudaMalloc(&d_idx64, (size_t)n * 8));
-        B200_CUDA_OK(cudaMalloc(&d_dis, (size_t)n * 4));
+        B200_TRY(idx64_b.alloc((size_t)n * 8));
+        B200_TRY(dis_b.alloc((size_t)n * 4));
     }
-    int rc = B200_OK;
-    for (int it = 0; it < iters && rc == B200_OK; it++) {
+    int64_t *d_idx64 = idx64_b.as<int64_t>();
+    float *d_dis = dis_b.as<float>();
+    CorpusPtr table;
+    for (int it = 0; it < iters; it++) {
         if (big) {
-            if (table) b200_corpus_free(table);
-            table = nullptr;
-            rc = b200_corpus_create(B200_METRIC_L2, B200_DTYPE_F32, d, nc, &table);
-            if (rc == B200_OK) rc = corpus_append_device(table, d_c, nc, s);
-            if (rc == B200_OK) rc = b200_corpus_search_device(table, x, n, 1, nullptr, 0, d_dis, d_idx64, s);
-            if (rc != B200_OK) break;
+            B200_TRY(corpus_create(B200_METRIC_L2, B200_DTYPE_F32, d, nc, table));
+            B200_TRY(corpus_append_device(table.get(), d_c, nc, s));
+            B200_TRY(b200_corpus_search_device(table.get(), x, n, 1, nullptr, 0, d_dis, d_idx64, s));
             B200_CUDA_OK(cudaMemsetAsync(d_cnt, 0, (size_t)nc * 4, s));
             assign_to_u32_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(d_idx64, n, nullptr, 0u, d_idx, d_cnt);
             g_launches++;
@@ -1657,25 +1626,19 @@ static int kmeans_device(const float *x, int64_t n, int64_t stride, int d, int n
                     pairs.push_back(src);
                 }
                 if (!pairs.empty()) {
-                    int *d_pairs = nullptr;
-                    B200_CUDA_OK(cudaMalloc(&d_pairs, pairs.size() * 4));
-                    B200_CUDA_OK(cudaMemcpyAsync(d_pairs, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s));
-                    kmeans_split_kernel<<<(unsigned)(pairs.size() / 2), 128, 0, s>>>(d_c, d_pairs, d);
+                    DevMem d_pairs;
+                    B200_TRY(d_pairs.alloc(pairs.size() * 4));
+                    B200_CUDA_OK(cudaMemcpyAsync(d_pairs.p, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s));
+                    kmeans_split_kernel<<<(unsigned)(pairs.size() / 2), 128, 0, s>>>(d_c, d_pairs.as<int>(), d);
                     g_launches++;
                     B200_CUDA_OK(cudaStreamSynchronize(s));
-                    cudaFree(d_pairs);
                 }
             }
         }
     }
-    if (rc == B200_OK) {
-        B200_CUDA_OK(cudaGetLastError());
-        B200_CUDA_OK(cudaStreamSynchronize(s));
-    }
-    if (table) b200_corpus_free(table);
-    for (void *p : {(void *)d_pick, (void *)d_sums, (void *)d_cn, (void *)d_cnt, (void *)d_idx, (void *)d_idx64, (void *)d_dis})
-        if (p) cudaFree(p);
-    return rc;
+    B200_CUDA_OK(cudaGetLastError());
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    return B200_OK;
 }
 
 // total rows the index will hold (Search::createVectorIndex's total_vec, VIWithDataPart.cpp:416-430): sizes the page pool
@@ -1688,27 +1651,21 @@ extern "C" int b200_index_reserve(b200_index *ix, int64_t total_rows) {
 }
 
 static int upload_coarse(b200_index *ix, cudaStream_t s) {
-    if (ix->coarse) b200_corpus_free(ix->coarse);
-    ix->coarse = nullptr;
     // L2 for every metric (unit vectors under cosine; IP indexes probe by L2 too, like Faiss's default quantiser)
-    B200_TRY(b200_corpus_create(B200_METRIC_L2, B200_DTYPE_F32, ix->d, ix->nlist, &ix->coarse));
-    if (ix->d_cnorm) cudaFree(ix->d_cnorm);
-    ix->d_cnorm = nullptr;
-    B200_CUDA_OK(cudaMalloc(&ix->d_cnorm, (size_t)ix->nlist * 4));
-    B200_CUDA_OK(launch_row_norms(ix->d_centroids, 0, ix->d, ix->nlist, 0, ix->d_cnorm, s));
-    return corpus_append_device(ix->coarse, ix->d_centroids, ix->nlist, s);
+    B200_TRY(corpus_create(B200_METRIC_L2, B200_DTYPE_F32, ix->d, ix->nlist, ix->coarse));
+    B200_TRY(ix->d_cnorm.alloc((size_t)ix->nlist * 4));
+    B200_CUDA_OK(launch_row_norms(ix->d_centroids.as<float>(), 0, ix->d, ix->nlist, 0, ix->d_cnorm.as<float>(), s));
+    return corpus_append_device(ix->coarse.get(), ix->d_centroids.as<float>(), ix->nlist, s);
 }
 
 // binary centroid table as a Hamming corpus of cent_pad-byte rows (a multiple of 16 bytes: always on the b1 tensor path)
 static int upload_coarse_bin(b200_index *ix, cudaStream_t s) {
-    if (ix->coarse) b200_corpus_free(ix->coarse);
-    ix->coarse = nullptr;
-    B200_TRY(b200_corpus_create(B200_METRIC_HAMMING, B200_DTYPE_BIN, ix->cent_pad * 8, ix->nlist, &ix->coarse));
-    return corpus_append_device(ix->coarse, reinterpret_cast<const float *>(ix->d_bcent), ix->nlist, s);
+    B200_TRY(corpus_create(B200_METRIC_HAMMING, B200_DTYPE_BIN, ix->cent_pad * 8, ix->nlist, ix->coarse));
+    return corpus_append_device(ix->coarse.get(), reinterpret_cast<const float *>(ix->d_bcent.as<uint8_t>()), ix->nlist, s);
 }
 
 // binary rows [n][row_bytes] (device) -> dst [n][cent_pad], zero-padded: the form the coarse table is searched with
-static int pad_bin_rows(const b200_index *ix, const void *d_rows, int64_t n, DevArr &dst, cudaStream_t s) {
+static int pad_bin_rows(const b200_index *ix, const void *d_rows, int64_t n, DevMem &dst, cudaStream_t s) {
     B200_TRY(dst.reserve((size_t)std::max<int64_t>(n, 1) * ix->cent_pad));
     if (n == 0) return B200_OK;
     B200_CUDA_OK(cudaMemsetAsync(dst.p, 0, (size_t)n * ix->cent_pad, s));
@@ -1725,31 +1682,29 @@ static int kmajority_device(const uint8_t *x, int64_t n, int stride, int rb, int
     for (int i = 0; i < nc; i++) pick[i] = (int64_t)((double)i * (double)n / (double)nc);
     // per-(cluster, bit) counts for <= 64 M counters (256 MB) at a time
     const int chunk = (int)std::max<int64_t>(1, std::min<int64_t>(nc, ((int64_t)64 << 20) / ((int64_t)rb * 8)));
-    int64_t *d_pick = nullptr, *d_idx64 = nullptr;
-    float *d_dis = nullptr;
-    uint32_t *d_idx = nullptr, *d_prev = nullptr, *d_cnt = nullptr, *d_changed = nullptr, *d_bits = nullptr;
-    B200_CUDA_OK(cudaMalloc(&d_pick, (size_t)nc * 8));
-    B200_CUDA_OK(cudaMalloc(&d_idx64, (size_t)n * 8));
-    B200_CUDA_OK(cudaMalloc(&d_dis, (size_t)n * 4));
-    B200_CUDA_OK(cudaMalloc(&d_idx, (size_t)n * 4));
-    B200_CUDA_OK(cudaMalloc(&d_prev, (size_t)n * 4));
-    B200_CUDA_OK(cudaMalloc(&d_cnt, (size_t)nc * 4));
-    B200_CUDA_OK(cudaMalloc(&d_changed, 4));
-    B200_CUDA_OK(cudaMalloc(&d_bits, (size_t)chunk * rb * 8 * 4));
+    DevMem pick_b, idx64_b, dis_b, idx_b, prev_b, cnt_b, changed_b, bits_b;
+    B200_TRY(pick_b.alloc((size_t)nc * 8));
+    B200_TRY(idx64_b.alloc((size_t)n * 8));
+    B200_TRY(dis_b.alloc((size_t)n * 4));
+    B200_TRY(idx_b.alloc((size_t)n * 4));
+    B200_TRY(prev_b.alloc((size_t)n * 4));
+    B200_TRY(cnt_b.alloc((size_t)nc * 4));
+    B200_TRY(changed_b.alloc(4));
+    B200_TRY(bits_b.alloc((size_t)chunk * rb * 8 * 4));
+    int64_t *d_pick = pick_b.as<int64_t>(), *d_idx64 = idx64_b.as<int64_t>();
+    float *d_dis = dis_b.as<float>();
+    uint32_t *d_idx = idx_b.as<uint32_t>(), *d_prev = prev_b.as<uint32_t>(), *d_cnt = cnt_b.as<uint32_t>(), *d_changed = changed_b.as<uint32_t>(),
+             *d_bits = bits_b.as<uint32_t>();
     B200_CUDA_OK(cudaMemcpyAsync(d_pick, pick.data(), (size_t)nc * 8, cudaMemcpyHostToDevice, s));
     gather_bytes_kernel<<<gridsz((int64_t)nc * stride), 256, 0, s>>>(x, stride, d_pick, nc, d_c);
     B200_CUDA_OK(cudaMemsetAsync(d_prev, 0xff, (size_t)n * 4, s));
     g_launches++;
     std::vector<uint32_t> h_cnt(nc), h_idx;
-    b200_corpus *table = nullptr;
-    int rc = B200_OK;
-    for (int it = 0; it < iters && rc == B200_OK; it++) {
-        if (table) b200_corpus_free(table);
-        table = nullptr;
-        rc = b200_corpus_create(B200_METRIC_HAMMING, B200_DTYPE_BIN, stride * 8, nc, &table);
-        if (rc == B200_OK) rc = corpus_append_device(table, reinterpret_cast<const float *>(d_c), nc, s);
-        if (rc == B200_OK) rc = b200_corpus_search_device(table, reinterpret_cast<const float *>(x), n, 1, nullptr, 0, d_dis, d_idx64, s);
-        if (rc != B200_OK) break;
+    CorpusPtr table;
+    for (int it = 0; it < iters; it++) {
+        B200_TRY(corpus_create(B200_METRIC_HAMMING, B200_DTYPE_BIN, stride * 8, nc, table));
+        B200_TRY(corpus_append_device(table.get(), reinterpret_cast<const float *>(d_c), nc, s));
+        B200_TRY(b200_corpus_search_device(table.get(), reinterpret_cast<const float *>(x), n, 1, nullptr, 0, d_dis, d_idx64, s));
         B200_CUDA_OK(cudaMemsetAsync(d_cnt, 0, (size_t)nc * 4, s));
         B200_CUDA_OK(cudaMemsetAsync(d_changed, 0, 4, s));
         assign_to_u32_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(d_idx64, n, nullptr, 0u, d_idx, d_cnt);
@@ -1792,14 +1747,9 @@ static int kmajority_device(const uint8_t *x, int64_t n, int stride, int rb, int
             }
         }
     }
-    if (rc == B200_OK) {
-        B200_CUDA_OK(cudaGetLastError());
-        B200_CUDA_OK(cudaStreamSynchronize(s));
-    }
-    if (table) b200_corpus_free(table);
-    for (void *p : {(void *)d_pick, (void *)d_idx64, (void *)d_dis, (void *)d_idx, (void *)d_prev, (void *)d_cnt, (void *)d_changed, (void *)d_bits})
-        if (p) cudaFree(p);
-    return rc;
+    B200_CUDA_OK(cudaGetLastError());
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    return B200_OK;
 }
 
 // FLAT fallback for small parts (the reference's fallback_to_flat, test 00029) and the default nlist
@@ -1817,23 +1767,21 @@ static int alloc_pool(b200_index *ix, int64_t total, cudaStream_t s) {
     if (pages * kPageRows >= (int64_t)0xffffffffll) return fail(B200_ERR_UNSUPPORTED, "an index shard is limited to 2^32 - 1 pool rows");
     ix->pool_pages = (uint32_t)pages;
     const size_t rows = (size_t)pages * kPageRows;
-    if (cudaMalloc(&ix->d_pool, rows * payload_row_bytes(ix) + 256) != cudaSuccess) {
-        cudaGetLastError();
+    if (ix->d_pool.alloc(rows * payload_row_bytes(ix) + 256) != B200_OK)
         return fail(B200_ERR_NOMEM, "cudaMalloc of the page pool failed (" + std::to_string(rows * payload_row_bytes(ix)) + " bytes)");
-    }
-    B200_CUDA_OK(cudaMemsetAsync(ix->d_pool, 0, rows * payload_row_bytes(ix), s));
-    B200_CUDA_OK(cudaMalloc(&ix->d_row_ids, rows * 4));
-    if (ix->metric == B200_METRIC_L2 || ix->binary) B200_CUDA_OK(cudaMalloc(&ix->d_row_bias, rows * 4));
-    B200_CUDA_OK(cudaMalloc(&ix->d_list_len, (size_t)nl * 4));
-    B200_CUDA_OK(cudaMalloc(&ix->d_tail_page, (size_t)nl * 4));
-    B200_CUDA_OK(cudaMalloc(&ix->d_page_owner, (size_t)pages * 4));
-    B200_CUDA_OK(cudaMalloc(&ix->d_page_seq, (size_t)pages * 4));
-    B200_CUDA_OK(cudaMalloc(&ix->d_pages_used, 4));
-    B200_CUDA_OK(cudaMalloc(&ix->d_flag, 32));
-    B200_CUDA_OK(cudaMemsetAsync(ix->d_list_len, 0, (size_t)nl * 4, s));
-    B200_CUDA_OK(cudaMemsetAsync(ix->d_tail_page, 0, (size_t)nl * 4, s));
-    B200_CUDA_OK(cudaMemsetAsync(ix->d_pages_used, 0, 4, s));
-    B200_CUDA_OK(cudaMemsetAsync(ix->d_flag, 0, 32, s));
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_pool.p, 0, rows * payload_row_bytes(ix), s));
+    B200_TRY(ix->d_row_ids.alloc(rows * 4));
+    if (ix->metric == B200_METRIC_L2 || ix->binary) B200_TRY(ix->d_row_bias.alloc(rows * 4));
+    B200_TRY(ix->d_list_len.alloc((size_t)nl * 4));
+    B200_TRY(ix->d_tail_page.alloc((size_t)nl * 4));
+    B200_TRY(ix->d_page_owner.alloc((size_t)pages * 4));
+    B200_TRY(ix->d_page_seq.alloc((size_t)pages * 4));
+    B200_TRY(ix->d_pages_used.alloc(4));
+    B200_TRY(ix->d_flag.alloc(32));
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_list_len.as<uint32_t>(), 0, (size_t)nl * 4, s));
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_tail_page.as<uint32_t>(), 0, (size_t)nl * 4, s));
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_pages_used.as<uint32_t>(), 0, 4, s));
+    B200_CUDA_OK(cudaMemsetAsync(ix->d_flag.as<int>(), 0, 32, s));
     return B200_OK;
 }
 
@@ -1849,8 +1797,8 @@ static int train_binary_locked(b200_index *ix, const void *d_rows, int64_t n) {
     }
     ix->keep_raw = 0;   // list rows are exact: nothing to re-rank
     B200_TRY(pad_bin_rows(ix, d_rows, n, ix->w_rows, s));
-    B200_CUDA_OK(cudaMalloc(&ix->d_bcent, (size_t)ix->nlist * ix->cent_pad));
-    B200_TRY(kmajority_device(ix->w_rows.as<uint8_t>(), n, ix->cent_pad, ix->row_bytes, ix->nlist, 10, ix->d_bcent, s));
+    B200_TRY(ix->d_bcent.alloc((size_t)ix->nlist * ix->cent_pad));
+    B200_TRY(kmajority_device(ix->w_rows.as<uint8_t>(), n, ix->cent_pad, ix->row_bytes, ix->nlist, 10, ix->d_bcent.as<uint8_t>(), s));
     B200_TRY(upload_coarse_bin(ix, s));
     B200_TRY(alloc_pool(ix, total, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
@@ -1868,52 +1816,52 @@ static int opq_train_locked(b200_index *ix, float *samp, int64_t ns, const uint3
     cudaStream_t s = ix->stream;
     const int d = ix->d, m = ix->m, dsub = ix->dsub, ncw = pq_codewords(ix->pq_bits), nl = ix->nlist;
     const size_t rows_b = (size_t)ns * d * 4;
-    float *res = nullptr, *resr = nullptr, *xhat = nullptr;
-    double *err = nullptr;
-    int rc = B200_OK;
-    auto cuda_ok = [&](cudaError_t e) {
-        if (e != cudaSuccess && rc == B200_OK) rc = fail(B200_ERR_CUDA, std::string("OPQ training: ") + cudaGetErrorString(e));
-        return rc == B200_OK;
-    };
+    // resr also takes the rotated centroids at the end: nlist may exceed the sample (ncentroids > 65 536)
+    DevMem res_b, resr_b, xhat_b, err_b;
+    B200_TRY(ix->d_opq.alloc((size_t)d * d * 4));
+    B200_TRY(res_b.alloc(rows_b));
+    B200_TRY(resr_b.alloc((size_t)std::max<int64_t>(ns, nl) * d * 4));
+    B200_TRY(xhat_b.alloc(rows_b));
+    B200_TRY(err_b.alloc((size_t)std::max<int64_t>(ns, 1) * 8));
+    float *R = ix->d_opq.as<float>(), *centroids = ix->d_centroids.as<float>(), *pq = ix->d_pq.as<float>();
+    float *res = res_b.as<float>(), *resr = resr_b.as<float>(), *xhat = xhat_b.as<float>();
+    double *err = err_b.as<double>();
     std::vector<double> h_err(ns);
     auto loss = [&]() {   // encode Res.R with the current codebooks (-> xhat) and append the sample's mean loss
-        if (!cuda_ok(launch_opq_encode(resr, ns, d, m, dsub, ncw, ix->d_pq, xhat, err, s)) ||
-            !cuda_ok(cudaMemcpyAsync(h_err.data(), err, (size_t)ns * 8, cudaMemcpyDeviceToHost, s)) || !cuda_ok(cudaStreamSynchronize(s)))
-            return;
+        B200_CUDA_OK(launch_opq_encode(resr, ns, d, m, dsub, ncw, pq, xhat, err, s));
+        B200_CUDA_OK(cudaMemcpyAsync(h_err.data(), err, (size_t)ns * 8, cudaMemcpyDeviceToHost, s));
+        B200_CUDA_OK(cudaStreamSynchronize(s));
         double t = 0;
         for (int64_t r = 0; r < ns; r++) t += h_err[r];
         ix->opq_loss.push_back(t / (double)std::max<int64_t>(ns, 1));
+        return B200_OK;
     };
-    auto codebooks = [&](int iters, bool warm) {
-        for (int j = 0; j < m && rc == B200_OK; j++) rc = kmeans_device(resr + (size_t)j * dsub, ns, d, dsub, ncw, iters, ix->d_pq + (size_t)j * ncw * dsub, s, warm);
+    auto codebooks = [&](int iters, bool warm) {   // Res.R (-> resr), then its k-means per sub-quantiser
+        B200_CUDA_OK(launch_opq_rotate(res, d, ns, d, R, resr, d, s));
+        for (int j = 0; j < m; j++) B200_TRY(kmeans_device(resr + (size_t)j * dsub, ns, d, dsub, ncw, iters, pq + (size_t)j * ncw * dsub, s, warm));
+        return B200_OK;
     };
     ix->opq_loss.clear();
     std::vector<float> eye((size_t)d * d, 0.f);
     for (int i = 0; i < d; i++) eye[(size_t)i * d + i] = 1.f;
-    // resr also takes the rotated centroids at the end: nlist may exceed the sample (ncentroids > 65 536)
-    if (cuda_ok(cudaMalloc(&ix->d_opq, (size_t)d * d * 4)) && cuda_ok(cudaMalloc(&res, rows_b)) &&
-        cuda_ok(cudaMalloc(&resr, (size_t)std::max<int64_t>(ns, nl) * d * 4)) &&
-        cuda_ok(cudaMalloc(&xhat, rows_b)) && cuda_ok(cudaMalloc(&err, (size_t)std::max<int64_t>(ns, 1) * 8)) &&
-        cuda_ok(cudaMemcpyAsync(ix->d_opq, eye.data(), (size_t)d * d * 4, cudaMemcpyHostToDevice, s))) {
-        residual_sub_kernel<<<gridsz(ns * d), 256, 0, s>>>(samp, ns, d, ix->d_centroids, d_l, d, 0, d, res);
-        g_launches++;
-        if (cuda_ok(launch_opq_rotate(res, d, ns, d, ix->d_opq, resr, d, s))) codebooks(8, false);
-        if (rc == B200_OK) loss();
-        for (int it = 0; it < ix->opq_iters && rc == B200_OK; it++) {
-            rc = opq_procrustes(res, xhat, ns, d, ix->d_opq, s);
-            if (rc == B200_OK && cuda_ok(launch_opq_rotate(res, d, ns, d, ix->d_opq, resr, d, s))) codebooks(4, true);
-            if (rc == B200_OK) loss();
-        }
-        // the centroids and the sample into the rotated space (resr and res are free now)
-        if (rc == B200_OK && cuda_ok(launch_opq_rotate(ix->d_centroids, d, nl, d, ix->d_opq, resr, d, s)) &&
-            cuda_ok(cudaMemcpyAsync(ix->d_centroids, resr, (size_t)nl * d * 4, cudaMemcpyDeviceToDevice, s)) &&
-            cuda_ok(launch_opq_rotate(samp, d, ns, d, ix->d_opq, res, d, s)) && cuda_ok(cudaMemcpyAsync(samp, res, rows_b, cudaMemcpyDeviceToDevice, s)))
-            rc = upload_coarse(ix, s);
-        cuda_ok(cudaStreamSynchronize(s));
+    B200_CUDA_OK(cudaMemcpyAsync(R, eye.data(), (size_t)d * d * 4, cudaMemcpyHostToDevice, s));
+    residual_sub_kernel<<<gridsz(ns * d), 256, 0, s>>>(samp, ns, d, centroids, d_l, d, 0, d, res);
+    g_launches++;
+    B200_TRY(codebooks(8, false));
+    B200_TRY(loss());
+    for (int it = 0; it < ix->opq_iters; it++) {
+        B200_TRY(opq_procrustes(res, xhat, ns, d, R, s));
+        B200_TRY(codebooks(4, true));
+        B200_TRY(loss());
     }
-    for (void *p : {(void *)res, (void *)resr, (void *)xhat, (void *)err})
-        if (p) cudaFree(p);
-    return rc;
+    // the centroids and the sample into the rotated space (resr and res are free now)
+    B200_CUDA_OK(launch_opq_rotate(centroids, d, nl, d, R, resr, d, s));
+    B200_CUDA_OK(cudaMemcpyAsync(centroids, resr, (size_t)nl * d * 4, cudaMemcpyDeviceToDevice, s));
+    B200_CUDA_OK(launch_opq_rotate(samp, d, ns, d, R, res, d, s));
+    B200_CUDA_OK(cudaMemcpyAsync(samp, res, rows_b, cudaMemcpyDeviceToDevice, s));
+    B200_TRY(upload_coarse(ix, s));
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    return B200_OK;
 }
 
 // Search::VectorIndex::train: coarse quantiser (+ PQ codebooks / SQ ranges) from a sample already on the device,
@@ -2010,17 +1958,17 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
         B200_CUDA_OK(launch_normalize_rows_f32(ix->w_rows.as<float>(), d, n, s));
         x = ix->w_rows.as<float>();
     }
-    B200_CUDA_OK(cudaMalloc(&ix->d_centroids, (size_t)nl * d * 4));
-    B200_TRY(kmeans_device(x, n, d, d, nl, 10, ix->d_centroids, s));
+    B200_TRY(ix->d_centroids.alloc((size_t)nl * d * 4));
+    B200_TRY(kmeans_device(x, n, d, d, nl, 10, ix->d_centroids.as<float>(), s));
     B200_TRY(upload_coarse(ix, s));
     if (ix->payload == IVF_PRODUCER_SQ8) {
         ix->code_bytes = (int)round_up(d, 16);
-        B200_CUDA_OK(cudaMalloc(&ix->d_sq, (size_t)4 * d * 4));
-        float *lo = ix->d_sq, *hi = ix->d_sq + d;
+        B200_TRY(ix->d_sq.alloc((size_t)4 * d * 4));
+        float *lo = ix->d_sq.as<float>(), *hi = ix->d_sq.as<float>() + d;
         dim_minmax_kernel<<<d, 256, 0, s>>>(x, n, d, d, lo, hi);
         g_launches++;
         std::vector<float> h((size_t)4 * d);
-        B200_CUDA_OK(cudaMemcpyAsync(h.data(), ix->d_sq, (size_t)2 * d * 4, cudaMemcpyDeviceToHost, s));
+        B200_CUDA_OK(cudaMemcpyAsync(h.data(), ix->d_sq.as<float>(), (size_t)2 * d * 4, cudaMemcpyDeviceToHost, s));
         B200_CUDA_OK(cudaStreamSynchronize(s));
         for (int j = 0; j < d; j++) {
             const float l = h[j], u = h[d + j];
@@ -2029,61 +1977,53 @@ static int train_device_locked(b200_index *ix, const float *d_rows, int64_t n) {
             h[2 * d + j] = 1.f / step;
             h[3 * d + j] = l + 128.f * step;   // value of code 128 = the zero of the offset-binary code the scan decodes
         }
-        B200_CUDA_OK(cudaMemcpyAsync(ix->d_sq, h.data(), (size_t)4 * d * 4, cudaMemcpyHostToDevice, s));
+        B200_CUDA_OK(cudaMemcpyAsync(ix->d_sq.as<float>(), h.data(), (size_t)4 * d * 4, cudaMemcpyHostToDevice, s));
     }
     if (ix->payload == IVF_PRODUCER_PQ) {
         const int m = ix->m, dsub = d / m;   // validated above
         const int ncw = pq_codewords(ix->pq_bits);
         ix->dsub = dsub;
         ix->code_bytes = pq_code_bytes(m, ix->pq_bits);
-        B200_CUDA_OK(cudaMalloc(&ix->d_pq, (size_t)m * ncw * dsub * 4));
-        if (!pq_uses_lut(ix)) B200_CUDA_OK(cudaMalloc(&ix->d_pq_bf16, (size_t)m * 256 * dsub * 2));   // the decoder's copy
+        B200_TRY(ix->d_pq.alloc((size_t)m * ncw * dsub * 4));
+        if (!pq_uses_lut(ix)) B200_TRY(ix->d_pq_bf16.alloc((size_t)m * 256 * dsub * 2));   // the decoder's copy
         // residuals of (a sample of) the training rows, one sub-quantiser at a time
         const int64_t ns = std::min<int64_t>(n, 65536);
-        int64_t *d_a = nullptr;
-        float *d_ad = nullptr, *d_res = nullptr;
-        uint32_t *d_l = nullptr, *d_c32 = nullptr;
-        B200_CUDA_OK(cudaMalloc(&d_a, (size_t)ns * 8));
-        B200_CUDA_OK(cudaMalloc(&d_ad, (size_t)ns * 4));
-        B200_CUDA_OK(cudaMalloc(&d_l, (size_t)ns * 4));
-        B200_CUDA_OK(cudaMalloc(&d_c32, (size_t)nl * 4));
-        B200_CUDA_OK(cudaMalloc(&d_res, (size_t)ns * dsub * 4));
+        DevMem a_b, ad_b, l_b, c32_b, res_b, samp_b;
+        B200_TRY(a_b.alloc((size_t)ns * 8));
+        B200_TRY(ad_b.alloc((size_t)ns * 4));
+        B200_TRY(l_b.alloc((size_t)ns * 4));
+        B200_TRY(c32_b.alloc((size_t)nl * 4));
+        B200_TRY(res_b.alloc((size_t)ns * dsub * 4));
         // the first ns rows of a strided view.  Below 2 ns rows the stride is 1, so the codebooks are trained on the first 65536
         // rows as given (tests/test_gpu_index_train.py pins this): one-shot build() already passes an even-strided sample, and
         // a streamed train() of more rows than that should pass them in no particular order (not sorted by cluster)
         const int64_t step = std::max<int64_t>(1, n / ns);
-        float *d_samp = nullptr;
-        B200_CUDA_OK(cudaMalloc(&d_samp, (size_t)ns * d * 4));
+        B200_TRY(samp_b.alloc((size_t)ns * d * 4));
+        float *d_samp = samp_b.as<float>(), *d_res = res_b.as<float>();
+        uint32_t *d_l = l_b.as<uint32_t>();
         B200_CUDA_OK(cudaMemcpy2DAsync(d_samp, (size_t)d * 4, x, (size_t)step * d * 4, (size_t)d * 4, ns, cudaMemcpyDeviceToDevice, s));
-        int rc = b200_corpus_search_device(ix->coarse, d_samp, ns, 1, nullptr, 0, d_ad, d_a, s);
-        if (rc == B200_OK) {
-            cudaMemsetAsync(d_c32, 0, (size_t)nl * 4, s);
-            assign_to_u32_kernel<<<(unsigned)ceil_div(ns, 256), 256, 0, s>>>(d_a, ns, nullptr, 0u, d_l, d_c32);
-            g_launches++;
-            if (ix->opq) {
-                rc = opq_train_locked(ix, d_samp, ns, d_l);   // R, the rotated centroids and sample, the codebooks
-            } else {
-                for (int j = 0; j < m && rc == B200_OK; j++) {
-                    residual_sub_kernel<<<gridsz(ns * dsub), 256, 0, s>>>(d_samp, ns, d, ix->d_centroids, d_l, d, j, dsub, d_res);
-                    g_launches++;
-                    rc = kmeans_device(d_res, ns, dsub, dsub, ncw, 8, ix->d_pq + (size_t)j * ncw * dsub, s);
-                }
+        B200_TRY(b200_corpus_search_device(ix->coarse.get(), d_samp, ns, 1, nullptr, 0, ad_b.as<float>(), a_b.as<int64_t>(), s));
+        cudaMemsetAsync(c32_b.p, 0, (size_t)nl * 4, s);
+        assign_to_u32_kernel<<<(unsigned)ceil_div(ns, 256), 256, 0, s>>>(a_b.as<int64_t>(), ns, nullptr, 0u, d_l, c32_b.as<uint32_t>());
+        g_launches++;
+        if (ix->opq) {
+            B200_TRY(opq_train_locked(ix, d_samp, ns, d_l));   // R, the rotated centroids and sample, the codebooks
+        } else {
+            for (int j = 0; j < m; j++) {
+                residual_sub_kernel<<<gridsz(ns * dsub), 256, 0, s>>>(d_samp, ns, d, ix->d_centroids.as<float>(), d_l, d, j, dsub, d_res);
+                g_launches++;
+                B200_TRY(kmeans_device(d_res, ns, dsub, dsub, ncw, 8, ix->d_pq.as<float>() + (size_t)j * ncw * dsub, s));
             }
         }
-        if (rc == B200_OK && ix->aq_threshold > 0) {
+        if (ix->aq_threshold > 0) {
             // anisotropic iterations on the same sample, from the k-means codebooks (ivf_aq.cu); with opq=1 the sample and the
             // centroids are the rotated ones (the loss does not change under a rotation)
-            const AqTrain at{d_samp, ns, d, m, dsub, ncw, d_l, ix->d_centroids, ix->d_pq, ix->aq_eta};
+            const AqTrain at{d_samp, ns, d, m, dsub, ncw, d_l, ix->d_centroids.as<float>(), ix->d_pq.as<float>(), ix->aq_eta};
             ix->aq_loss.clear();
-            rc = aq_train_codebooks(at, &ix->aq_loss, s);
+            B200_TRY(aq_train_codebooks(at, &ix->aq_loss, s));
         }
-        if (rc == B200_OK && ix->d_pq_bf16) {
-            cudaError_t e = launch_f32_to_bf16_rows(ix->d_pq, dsub, ix->d_pq_bf16, dsub, (int64_t)m * 256, s);
-            if (e != cudaSuccess) rc = fail(B200_ERR_CUDA, cudaGetErrorString(e));
-        }
-        cudaStreamSynchronize(s);
-        for (void *p : {(void *)d_a, (void *)d_ad, (void *)d_l, (void *)d_c32, (void *)d_res, (void *)d_samp}) cudaFree(p);
-        B200_TRY(rc);
+        if (ix->d_pq_bf16) B200_CUDA_OK(launch_f32_to_bf16_rows(ix->d_pq.as<float>(), dsub, ix->d_pq_bf16.as<__nv_bfloat16>(), dsub, (int64_t)m * 256, s));
+        B200_CUDA_OK(cudaStreamSynchronize(s));
     }
     B200_TRY(alloc_pool(ix, total, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
@@ -2106,7 +2046,7 @@ extern "C" int b200_index_train(b200_index *ix, const float *rows, int64_t n) {
     B200_TRY(staged_h2d(ix->w_host_q.p, rows, (size_t)n * in_row_bytes(ix), ix->device, ix->stream));
     B200_CUDA_OK(cudaStreamSynchronize(ix->stream));
     int rc = train_device_locked(ix, ix->w_host_q.as<float>(), n);
-    ix->w_host_q.release();
+    ix->w_host_q.reset();
     return rc;
 }
 
@@ -2122,8 +2062,8 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     if (ix->n + n >= (int64_t)0xffffffffll) return fail(B200_ERR_UNSUPPORTED, "an index shard is limited to 2^32 - 1 rows");
     const float *x = d_rows;
     if (ix->binary && !ix->use_ivf) {   // BINARYFLAT / small part: an exact binary corpus
-        if (!ix->raw) B200_TRY(b200_corpus_create(ix->metric, B200_DTYPE_BIN, d, std::max<int64_t>(ix->reserved, n), &ix->raw));
-        B200_TRY(corpus_append_device(ix->raw, d_rows, n, s));
+        if (!ix->raw) B200_TRY(corpus_create(ix->metric, B200_DTYPE_BIN, d, std::max<int64_t>(ix->reserved, n), ix->raw));
+        B200_TRY(corpus_append_device(ix->raw.get(), d_rows, n, s));
         ix->n += n;
         return B200_OK;
     }
@@ -2136,9 +2076,9 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     if (ix->keep_raw == 1 && !ix->binary) {
         if (!ix->raw) {
             const int raw_metric = ix->metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
-            B200_TRY(b200_corpus_create(raw_metric, B200_DTYPE_F32, d, std::max<int64_t>(ix->reserved, n), &ix->raw));
+            B200_TRY(corpus_create(raw_metric, B200_DTYPE_F32, d, std::max<int64_t>(ix->reserved, n), ix->raw));
         }
-        B200_TRY(corpus_append_device(ix->raw, x, n, s));
+        B200_TRY(corpus_append_device(ix->raw.get(), x, n, s));
     } else if (ix->keep_raw == 2 && !ix->binary) {   // train resolved keep_raw=2 to 1 where the rows are the index
         B200_TRY(host_rows_reserve(ix, std::max(ix->n + n, ix->reserved)));
         B200_CUDA_OK(cudaMemcpy2DAsync(ix->h_rows + ix->n * ix->d_pad, (size_t)ix->d_pad * 4, x, (size_t)d * 4, (size_t)d * 4, n,
@@ -2150,7 +2090,7 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     }
     if (ix->d_opq) {   // opq=1: the assignment, the codes and the norm terms come from x.R; the fp32 rows above stay as given
         B200_TRY(ix->w_qrot.reserve((size_t)n * d * 4));
-        B200_CUDA_OK(launch_opq_rotate(x, d, n, d, ix->d_opq, ix->w_qrot.as<float>(), d, s));
+        B200_CUDA_OK(launch_opq_rotate(x, d, n, d, ix->d_opq.as<float>(), ix->w_qrot.as<float>(), d, s));
         x = ix->w_qrot.as<float>();
     }
     // ---- assign -> (list, row) sorted by list
@@ -2166,7 +2106,7 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
         B200_TRY(pad_bin_rows(ix, d_rows, n, ix->w_rows, s));
         x = ix->w_rows.as<float>();
     }
-    B200_TRY(b200_corpus_search_device(ix->coarse, x, n, 1, nullptr, 0, ix->w_assign_d.as<float>(), ix->w_assign_i.as<int64_t>(), s));
+    B200_TRY(b200_corpus_search_device(ix->coarse.get(), x, n, 1, nullptr, 0, ix->w_assign_d.as<float>(), ix->w_assign_i.as<int64_t>(), s));
     // unusable rows (judged as given, before the cosine normalisation) and rows without a nearest centroid get the key nlist:
     // they sort behind every list, are counted in w_cnt[nl] and go to no list
     const uint8_t *usable = nullptr;
@@ -2198,13 +2138,13 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     ap.seg_start = seg_start;
     ap.new_base = new_base;
     ap.first_new_seq = first_new;
-    ap.list_len = ix->d_list_len;
-    ap.page_owner = ix->d_page_owner;
-    ap.page_seq = ix->d_page_seq;
-    ap.pages_used = ix->d_pages_used;
+    ap.list_len = ix->d_list_len.as<uint32_t>();
+    ap.page_owner = ix->d_page_owner.as<uint32_t>();
+    ap.page_seq = ix->d_page_seq.as<uint32_t>();
+    ap.pages_used = ix->d_pages_used.as<uint32_t>();
     ap.pool_pages = ix->pool_pages;
     ap.nlist = nl;
-    ap.overflow = ix->d_flag;
+    ap.overflow = ix->d_flag.as<int>();
     add_plan_kernel<<<1, 1024, 0, s>>>(ap);
     g_launches++;
     ScatterParams sp{};
@@ -2215,40 +2155,40 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     sp.seg_start = seg_start;
     sp.new_base = new_base;
     sp.first_new_seq = first_new;
-    sp.list_len = ix->d_list_len;
-    sp.tail_page = ix->d_tail_page;
+    sp.list_len = ix->d_list_len.as<uint32_t>();
+    sp.tail_page = ix->d_tail_page.as<uint32_t>();
     sp.id_base = (uint32_t)ix->n;
     sp.d = d;
     sp.d_pad64 = ix->d_pad64;
     sp.l2 = ix->metric == B200_METRIC_L2;
-    sp.pool = reinterpret_cast<__nv_bfloat16 *>(ix->d_pool);
+    sp.pool = reinterpret_cast<__nv_bfloat16 *>(ix->d_pool.p);
     if (ix->d_sq) {
-        sp.sq_lo = ix->d_sq;
-        sp.sq_step = ix->d_sq + d;
-        sp.sq_inv_step = ix->d_sq + 2 * d;
+        sp.sq_lo = ix->d_sq.as<float>();
+        sp.sq_step = ix->d_sq.as<float>() + d;
+        sp.sq_inv_step = ix->d_sq.as<float>() + 2 * d;
     }
-    sp.centroids = ix->d_centroids;
-    sp.pq = ix->d_pq;
-    sp.pq_bf16 = ix->d_pq_bf16;
+    sp.centroids = ix->d_centroids.as<float>();
+    sp.pq = ix->d_pq.as<float>();
+    sp.pq_bf16 = ix->d_pq_bf16.as<__nv_bfloat16>();
     sp.m = ix->m;
     sp.dsub = ix->dsub;
     sp.pq_bits = ix->pq_bits;
-    sp.codes = reinterpret_cast<uint8_t *>(ix->d_pool);
+    sp.codes = reinterpret_cast<uint8_t *>(ix->d_pool.p);
     sp.code_bytes = ix->code_bytes;
-    sp.row_bias = ix->d_row_bias;
-    sp.row_ids = ix->d_row_ids;
+    sp.row_bias = ix->d_row_bias.as<float>();
+    sp.row_ids = ix->d_row_ids.as<uint32_t>();
     sp.payload = ix->payload;
     if (ix->binary) {
         sp.brows = reinterpret_cast<const uint8_t *>(d_rows);
         sp.stride = ix->row_bytes;
-        sp.bpool = reinterpret_cast<uint8_t *>(ix->d_pool);
+        sp.bpool = reinterpret_cast<uint8_t *>(ix->d_pool.p);
         sp.row_bytes = ix->row_bytes;
         sp.row_pad = ix->row_pad;
         sp.kb_w = ix->kb_w;
     }
     int over = 0;
     uint32_t in_no_list = 0;
-    B200_CUDA_OK(cudaMemcpyAsync(&over, ix->d_flag, 4, cudaMemcpyDeviceToHost, s));
+    B200_CUDA_OK(cudaMemcpyAsync(&over, ix->d_flag.as<int>(), 4, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaMemcpyAsync(&in_no_list, ix->w_cnt.as<uint32_t>() + nl, 4, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
     if (over) return fail(B200_ERR_NOMEM, "page pool exhausted: more rows added than b200_index_reserve() announced");
@@ -2256,7 +2196,7 @@ static int add_device_locked(b200_index *ix, const void *d_rows_v, int64_t n) {
     if (ix->binary) scatter_bin_rows_kernel<<<gridsz(sp.n * 32), 256, 0, s>>>(sp);
     else scatter_rows_kernel<<<gridsz(sp.n * 32), 256, 0, s>>>(sp);
     if (ix->payload == IVF_PRODUCER_PQ && ix->aq_threshold > 0) B200_TRY(aq_encode_chunk(sp, ix->aq_eta, s));   // from the nearest codes
-    add_commit_kernel<<<(unsigned)ceil_div(nl, 256), 256, 0, s>>>(ix->w_cnt.as<uint32_t>(), new_base, first_new, ix->d_list_len, ix->d_tail_page, nl);
+    add_commit_kernel<<<(unsigned)ceil_div(nl, 256), 256, 0, s>>>(ix->w_cnt.as<uint32_t>(), new_base, first_new, ix->d_list_len.as<uint32_t>(), ix->d_tail_page.as<uint32_t>(), nl);
     g_launches += 2;
     B200_CUDA_OK(cudaGetLastError());
     B200_CUDA_OK(cudaStreamSynchronize(s));
@@ -2297,38 +2237,18 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
 // scratch of one chunk of the graph build's list searches (their pairs, partial lists and candidates); sizes the chunk
 constexpr int64_t kGraphBuildSearchBytes = (int64_t)512 << 20;
 
-namespace {
-struct DevScratch {   // freed on every return path of the graph build
-    void *p = nullptr;
-    ~DevScratch() {
-        if (p) cudaFree(p);
-    }
-    int alloc(size_t bytes) {
-        if (cudaMalloc(&p, std::max<size_t>(bytes, 16)) != cudaSuccess) {
-            cudaGetLastError();
-            p = nullptr;
-            return fail(B200_ERR_NOMEM, "graph build: cudaMalloc(" + std::to_string(bytes) + ") failed");
-        }
-        return B200_OK;
-    }
-};
-}  // namespace
-
 // row_slot[n] from the page chains of the finalized (or loaded) lists; 0xFFFFFFFF for a row in no list (an unusable row, or
 // an id a loaded file repeats in place of it).  No kernel reads a pool slot through it without that check: the graph build
 // gives such rows no edges, and a load refuses an MSTG graph edge to one.
 static int fill_row_slot(const b200_index *ix, uint32_t *d_row_slot) {
     B200_CUDA_OK(cudaMemsetAsync(d_row_slot, 0xff, (size_t)ix->n * 4, ix->stream));
-    return graph_row_slots(ix->d_list_len, ix->d_list_page_off, ix->d_list_pages, ix->d_row_ids, ix->nlist, d_row_slot, ix->stream);
+    return graph_row_slots(ix->d_list_len.as<uint32_t>(), ix->d_list_page_off.as<uint32_t>(), ix->d_list_pages.as<uint32_t>(), ix->d_row_ids.as<uint32_t>(), ix->nlist, d_row_slot, ix->stream);
 }
 
 // MSTG / BINARYMSTG graph: the walk reads its bf16 / binary list rows through d_row_slot
 static int build_row_slot(b200_index *ix) {
-    if (!ix->d_row_slot && cudaMalloc(&ix->d_row_slot, std::max<size_t>((size_t)ix->n * 4, 16)) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(B200_ERR_NOMEM, "cudaMalloc of the graph's row slot map failed");
-    }
-    return fill_row_slot(ix, ix->d_row_slot);
+    if (!ix->d_row_slot) B200_TRY(ix->d_row_slot.alloc(std::max<size_t>((size_t)ix->n * 4, 16)));
+    return fill_row_slot(ix, ix->d_row_slot.as<uint32_t>());
 }
 
 // graph_degree=D: every row searches the index's own lists with its defaults for k = 2D + 1.  HNSWFLAT: nprobe and the exact
@@ -2352,52 +2272,47 @@ static int build_graph_locked(b200_index *ix) {
     // float builds keep their chunk: its size picks the list search's coarse path, so a new one could move their graphs.
     const int64_t q_row_bytes = ix->binary ? ix->row_bytes : (int64_t)d * 4;
     const int64_t chunk = std::max<int64_t>(256, std::min<int64_t>(n, kGraphBuildSearchBytes / ((int64_t)np * k1 * 8 + (ix->binary ? q_row_bytes : 0))));
-    DevScratch cand, pruned, q, dis, ids, slots;
+    DevMem cand, pruned, q, dis, ids, slots;
     // which rows are in a list: the slot map of MSTG / BINARYMSTG, a scratch one for HNSWFLAT
-    const uint32_t *row_slot = ix->d_row_slot;
+    const uint32_t *row_slot = ix->d_row_slot.as<uint32_t>();
     if (!row_slot) {
-        B200_TRY(slots.alloc((size_t)n * 4));
+        B200_TRY(slots.alloc(std::max<size_t>((size_t)n * 4, 16)));
         B200_TRY(fill_row_slot(ix, static_cast<uint32_t *>(slots.p)));
         row_slot = static_cast<const uint32_t *>(slots.p);
     }
-    B200_TRY(cand.alloc((size_t)n * K * 4));
-    B200_TRY(q.alloc((size_t)chunk * q_row_bytes));   // fp32 rows, or binary rows of d / 8 bytes
-    B200_TRY(dis.alloc((size_t)chunk * (K + 1) * 4));
-    B200_TRY(ids.alloc((size_t)chunk * (K + 1) * 8));
+    B200_TRY(cand.alloc(std::max<size_t>((size_t)n * K * 4, 16)));
+    B200_TRY(q.alloc(std::max<size_t>((size_t)chunk * q_row_bytes, 16)));   // fp32 rows, or binary rows of d / 8 bytes
+    B200_TRY(dis.alloc(std::max<size_t>((size_t)chunk * (K + 1) * 4, 16)));
+    B200_TRY(ids.alloc(std::max<size_t>((size_t)chunk * (K + 1) * 8, 16)));
     auto t = clk::now();
-    const float *rows = ix->raw ? reinterpret_cast<const float *>(corpus_device_rows(ix->raw)) : ix->h_rows;
+    const float *rows = ix->raw ? reinterpret_cast<const float *>(corpus_device_rows(ix->raw.get())) : ix->h_rows;
     for (int64_t off = 0; off < n; off += chunk) {
         const int64_t m = std::min(chunk, n - off);
         if (ix->binary)
-            B200_TRY(graph_bin_page_rows(ix->d_pool, ix->d_row_slot, off, m, ix->row_bytes, ix->row_pad, ix->kb_w, static_cast<uint8_t *>(q.p), s));
+            B200_TRY(graph_bin_page_rows(ix->d_pool.p, ix->d_row_slot.as<uint32_t>(), off, m, ix->row_bytes, ix->row_pad, ix->kb_w, static_cast<uint8_t *>(q.p), s));
         else if (rows)
             B200_CUDA_OK(cudaMemcpy2DAsync(q.p, (size_t)d * 4, rows + off * ix->d_pad, (size_t)ix->d_pad * 4, (size_t)d * 4, m,
                                            ix->raw ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
         else
-            B200_TRY(graph_page_rows(ix->d_pool, ix->d_row_slot, off, m, d, ix->d_pad64, static_cast<float *>(q.p), s));
+            B200_TRY(graph_page_rows(ix->d_pool.p, ix->d_row_slot.as<uint32_t>(), off, m, d, ix->d_pad64, static_cast<float *>(q.p), s));
         B200_TRY(search_device_locked(ix, static_cast<float *>(q.p), m, K + 1, nullptr, mstg ? 1 : 0, nullptr, nullptr, 0, static_cast<float *>(dis.p),
                                       static_cast<int64_t *>(ids.p), nullptr, s));
         B200_TRY(graph_candidates(static_cast<int64_t *>(ids.p), row_slot, m, off, K, static_cast<uint32_t *>(cand.p) + off * K, s));
     }
     B200_CUDA_OK(cudaStreamSynchronize(s));
-    for (DevScratch *b : {&q, &dis, &ids, &slots}) {
-        cudaFree(b->p);
-        b->p = nullptr;
-    }
+    for (DevMem *b : {&q, &dis, &ids, &slots}) b->reset();
     const double t_cand = ms_since(t);
     t = clk::now();
-    B200_TRY(pruned.alloc((size_t)n * D * 4));
+    B200_TRY(pruned.alloc(std::max<size_t>((size_t)n * D * 4, 16)));
     B200_TRY(graph_prune(static_cast<uint32_t *>(cand.p), n, D, static_cast<uint32_t *>(pruned.p), s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
-    cudaFree(cand.p);
-    cand.p = nullptr;
+    cand.reset();
     const double t_prune = ms_since(t);
     t = clk::now();
-    DevScratch graph;
-    B200_TRY(graph.alloc((size_t)n * D * 4));
-    B200_TRY(graph_merge(static_cast<uint32_t *>(pruned.p), n, D, static_cast<uint32_t *>(graph.p), s));
-    ix->d_graph = static_cast<uint32_t *>(graph.p);
-    graph.p = nullptr;
+    DevMem graph;
+    B200_TRY(graph.alloc(std::max<size_t>((size_t)n * D * 4, 16)));
+    B200_TRY(graph_merge(pruned.as<uint32_t>(), n, D, graph.as<uint32_t>(), s));
+    ix->d_graph = std::move(graph);
     const double ph[5] = {t_cand, t_prune, ms_since(t), 0, 0};
     std::copy(ph, ph + 5, ix->phase_ms);
     return B200_OK;
@@ -2409,49 +2324,49 @@ static int finalize_locked(b200_index *ix) {
     cudaStream_t s = ix->stream;
     if (ix->use_ivf) {
         const int nl = ix->nlist;
-        B200_CUDA_OK(cudaMemcpy(&ix->pages_used, ix->d_pages_used, 4, cudaMemcpyDeviceToHost));
+        B200_CUDA_OK(cudaMemcpy(&ix->pages_used, ix->d_pages_used.as<uint32_t>(), 4, cudaMemcpyDeviceToHost));
         const uint32_t np = ix->pages_used;
-        B200_CUDA_OK(cudaMalloc(&ix->d_list_page_off, (size_t)(nl + 1) * 4));
-        B200_CUDA_OK(cudaMalloc(&ix->d_list_pages, (size_t)std::max<uint32_t>(np, 1) * 4));
-        B200_CUDA_OK(cudaMalloc(&ix->d_list_order, (size_t)nl * 4));
-        uint64_t *keys = nullptr, *keys_out = nullptr;
-        uint32_t *vals = nullptr, *neg = nullptr, *neg_out = nullptr, *iota = nullptr;
-        B200_CUDA_OK(cudaMalloc(&keys, (size_t)std::max<uint32_t>(np, 1) * 8));
-        B200_CUDA_OK(cudaMalloc(&keys_out, (size_t)std::max<uint32_t>(np, 1) * 8));
-        B200_CUDA_OK(cudaMalloc(&vals, (size_t)std::max<uint32_t>(np, 1) * 4));
-        B200_CUDA_OK(cudaMalloc(&neg, (size_t)nl * 4));
-        B200_CUDA_OK(cudaMalloc(&neg_out, (size_t)nl * 4));
-        B200_CUDA_OK(cudaMalloc(&iota, (size_t)nl * 4));
+        B200_TRY(ix->d_list_page_off.alloc((size_t)(nl + 1) * 4));
+        B200_TRY(ix->d_list_pages.alloc((size_t)std::max<uint32_t>(np, 1) * 4));
+        B200_TRY(ix->d_list_order.alloc((size_t)nl * 4));
+        DevMem keys_b, keys_out_b, vals_b, neg_b, neg_out_b, iota_b;
+        B200_TRY(keys_b.alloc((size_t)std::max<uint32_t>(np, 1) * 8));
+        B200_TRY(keys_out_b.alloc((size_t)std::max<uint32_t>(np, 1) * 8));
+        B200_TRY(vals_b.alloc((size_t)std::max<uint32_t>(np, 1) * 4));
+        B200_TRY(neg_b.alloc((size_t)nl * 4));
+        B200_TRY(neg_out_b.alloc((size_t)nl * 4));
+        B200_TRY(iota_b.alloc((size_t)nl * 4));
+        uint64_t *keys = keys_b.as<uint64_t>(), *keys_out = keys_out_b.as<uint64_t>();
+        uint32_t *vals = vals_b.as<uint32_t>(), *neg = neg_b.as<uint32_t>(), *neg_out = neg_out_b.as<uint32_t>(), *iota = iota_b.as<uint32_t>();
         if (np) {
-            page_keys_kernel<<<(unsigned)ceil_div(np, 256), 256, 0, s>>>(ix->d_page_owner, ix->d_page_seq, np, keys, vals);
+            page_keys_kernel<<<(unsigned)ceil_div(np, 256), 256, 0, s>>>(ix->d_page_owner.as<uint32_t>(), ix->d_page_seq.as<uint32_t>(), np, keys, vals);
             size_t tb = 0;
-            cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, keys_out, vals, ix->d_list_pages, (int)np, 0, 64, s);
+            cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, keys_out, vals, ix->d_list_pages.as<uint32_t>(), (int)np, 0, 64, s);
             B200_TRY(ix->w_sort.reserve(tb + 256));
-            cub::DeviceRadixSort::SortPairs(ix->w_sort.p, tb, keys, keys_out, vals, ix->d_list_pages, (int)np, 0, 64, s);
+            cub::DeviceRadixSort::SortPairs(ix->w_sort.p, tb, keys, keys_out, vals, ix->d_list_pages.as<uint32_t>(), (int)np, 0, 64, s);
             g_launches += 2;
         }
-        list_pages_scan_kernel<<<1, 1024, 0, s>>>(ix->d_list_len, nl, ix->d_list_page_off, neg);
+        list_pages_scan_kernel<<<1, 1024, 0, s>>>(ix->d_list_len.as<uint32_t>(), nl, ix->d_list_page_off.as<uint32_t>(), neg);
         iota_kernel<<<(unsigned)ceil_div(nl, 256), 256, 0, s>>>(iota, nl);
         {
             size_t tb = 0;
-            cub::DeviceRadixSort::SortPairs(nullptr, tb, neg, neg_out, iota, ix->d_list_order, nl, 0, 32, s);
+            cub::DeviceRadixSort::SortPairs(nullptr, tb, neg, neg_out, iota, ix->d_list_order.as<uint32_t>(), nl, 0, 32, s);
             B200_TRY(ix->w_sort.reserve(tb + 256));
-            cub::DeviceRadixSort::SortPairs(ix->w_sort.p, tb, neg, neg_out, iota, ix->d_list_order, nl, 0, 32, s);
+            cub::DeviceRadixSort::SortPairs(ix->w_sort.p, tb, neg, neg_out, iota, ix->d_list_order.as<uint32_t>(), nl, 0, 32, s);
         }
         g_launches += 3;
         ix->list_len.resize(nl);
-        B200_CUDA_OK(cudaMemcpyAsync(ix->list_len.data(), ix->d_list_len, (size_t)nl * 4, cudaMemcpyDeviceToHost, s));
+        B200_CUDA_OK(cudaMemcpyAsync(ix->list_len.data(), ix->d_list_len.as<uint32_t>(), (size_t)nl * 4, cudaMemcpyDeviceToHost, s));
         B200_CUDA_OK(cudaStreamSynchronize(s));
-        for (void *p : {(void *)keys, (void *)keys_out, (void *)vals, (void *)neg, (void *)neg_out, (void *)iota}) cudaFree(p);
         ix->max_list_pages = 0;
         for (int l = 0; l < nl; l++) ix->max_list_pages = std::max<uint32_t>(ix->max_list_pages, (ix->list_len[l] + kPageRows - 1) / kPageRows);
     }
     // build scratch is not needed any more
-    for (DevArr *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_plan, &ix->w_host_q, &ix->w_usable, &ix->w_qrot})
-        a->release();
+    for (DevMem *a : {&ix->w_rows, &ix->w_assign_i, &ix->w_assign_d, &ix->w_u32a, &ix->w_u32b, &ix->w_u32c, &ix->w_u32d, &ix->w_plan, &ix->w_host_q, &ix->w_usable, &ix->w_qrot})
+        a->reset();
     if (!ix->raw) {  // an index without a single row still answers (empty results)
         const int raw_metric = ix->metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
-        if (!ix->use_ivf) B200_TRY(b200_corpus_create(ix->binary ? ix->metric : raw_metric, ix->binary ? B200_DTYPE_BIN : B200_DTYPE_F32, ix->d, 0, &ix->raw));
+        if (!ix->use_ivf) B200_TRY(corpus_create(ix->binary ? ix->metric : raw_metric, ix->binary ? B200_DTYPE_BIN : B200_DTYPE_F32, ix->d, 0, ix->raw));
     }
     // a part below the inverted-file threshold is FLAT and gets no graph
     if (ix->graph_degree > 0 && ix->use_ivf && ix->n > 0 && !ix->d_graph) {
@@ -2500,8 +2415,8 @@ extern "C" int b200_index_build(b200_index *ix, const float *rows, int64_t n) {
 extern "C" int b200_index_memory_bytes(const b200_index *ix, uint64_t *out_bytes) {
     if (!ix || !out_bytes) return fail(B200_ERR_INVALID, "bad arguments");
     uint64_t b = 0, t = 0;
-    if (ix->raw && b200_corpus_memory_bytes(ix->raw, &t) == B200_OK) b += t;
-    if (ix->coarse && b200_corpus_memory_bytes(ix->coarse, &t) == B200_OK) b += t;
+    if (ix->raw && b200_corpus_memory_bytes(ix->raw.get(), &t) == B200_OK) b += t;
+    if (ix->coarse && b200_corpus_memory_bytes(ix->coarse.get(), &t) == B200_OK) b += t;
     if (ix->use_ivf) {
         const uint64_t rows = (uint64_t)ix->pool_pages * kPageRows;
         b += (uint64_t)ix->nlist * (ix->binary ? (uint64_t)ix->cent_pad : (uint64_t)ix->d * 4) + rows * (payload_row_bytes(ix) + 4 + (ix->d_row_bias ? 4 : 0)) +
@@ -2539,13 +2454,12 @@ extern "C" int b200_index_set_raw_placement(b200_index *ix, int placement) {
     const size_t row_b = (size_t)ix->d_pad * 4;
     if (placement == 2 && ix->raw) {
         B200_TRY(host_rows_reserve(ix, ix->n));
-        B200_CUDA_OK(cudaMemcpy(ix->h_rows, corpus_device_rows(ix->raw), (size_t)ix->n * row_b, cudaMemcpyDeviceToHost));
-        b200_corpus_free(ix->raw);
-        ix->raw = nullptr;
+        B200_CUDA_OK(cudaMemcpy(ix->h_rows, corpus_device_rows(ix->raw.get()), (size_t)ix->n * row_b, cudaMemcpyDeviceToHost));
+        ix->raw.reset();
     } else if (placement == 1 && ix->h_rows) {
         const int raw_metric = ix->metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
-        b200_corpus *c = nullptr;
-        B200_TRY(b200_corpus_create(raw_metric, B200_DTYPE_F32, ix->d, ix->n, &c));
+        CorpusPtr c;
+        B200_TRY(corpus_create(raw_metric, B200_DTYPE_F32, ix->d, ix->n, c));
         const int64_t chunk = std::max<int64_t>(1, kHostStageBytes / ((int64_t)ix->d * 4));
         int rc = ix->w_rows.reserve((size_t)std::min(chunk, std::max<int64_t>(ix->n, 1)) * ix->d * 4);
         for (int64_t off = 0; rc == B200_OK && off < ix->n; off += chunk) {   // unpadded [m][d] for the corpus append
@@ -2554,19 +2468,16 @@ extern "C" int b200_index_set_raw_placement(b200_index *ix, int placement) {
                                   ix->stream) != cudaSuccess)
                 rc = fail(B200_ERR_CUDA, "host rows -> HBM copy failed");
             else
-                rc = corpus_append_device(c, ix->w_rows.as<float>(), m, ix->stream);
+                rc = corpus_append_device(c.get(), ix->w_rows.as<float>(), m, ix->stream);
         }
-        ix->w_rows.release();
-        if (rc != B200_OK) {
-            b200_corpus_free(c);
-            return rc;
-        }
-        ix->raw = c;
+        ix->w_rows.reset();
+        B200_TRY(rc);
+        ix->raw = std::move(c);
         cudaFreeHost(ix->h_rows);
         ix->h_rows = nullptr;
         ix->h_rows_dev = nullptr;
         ix->h_rows_cap = 0;
-        ix->w_stage.release();
+        ix->w_stage.reset();
     }
     ix->keep_raw = placement;
     return B200_OK;
@@ -2589,7 +2500,7 @@ extern "C" int b200_index_last_scan(b200_index *ix, int64_t *rows_streamed, int6
     timing_collect(ix);
     if (ix->d_flag && ix->use_ivf) {
         unsigned long long r = 0;
-        if (cudaMemcpy(&r, ix->d_flag + 4, 8, cudaMemcpyDeviceToHost) == cudaSuccess) ix->last_scan_rows = (int64_t)r;
+        if (cudaMemcpy(&r, ix->d_flag.as<int>() + 4, 8, cudaMemcpyDeviceToHost) == cudaSuccess) ix->last_scan_rows = (int64_t)r;
     }
     if (rows_streamed) *rows_streamed = ix->last_scan_rows;
     // the graph walk reads fp32 rows (HNSWFLAT), the bf16 list rows (MSTG) or the binary list rows (BINARYMSTG)
@@ -2656,7 +2567,7 @@ static int refine_device(b200_index *ix, const float *d_q /*[nq][d_pad] prepared
         return fail(B200_ERR_UNSUPPORTED, "exact second stage: d_pad " + std::to_string(ix->d_pad) + " at k " + std::to_string(k) + " needs " +
                                               std::to_string(smem) + " bytes of shared memory, more than " + std::to_string(kSmemOptinBytes));
     if (!ix->h_rows) {
-        rp.rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
+        rp.rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw.get()));
         B200_CUDA_OK(cudaFuncSetAttribute(refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         refine_kernel<false><<<(unsigned)nq, 256, smem, s>>>(rp);
         g_launches++;
@@ -2781,19 +2692,19 @@ static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, cons
     B200_TRY(ix->w_items.reserve((size_t)max_items * sizeof(IvfGemmItem) + 64));
     B200_TRY(ix->w_plan.reserve((size_t)nl * 4 * 3));
     uint32_t *pair_start = ix->w_plan.as<uint32_t>(), *part_off = pair_start + nl, *n_chunks = part_off + nl;
-    int *d_counts = ix->d_flag + 1;   // n_items, n_parts
+    int *d_counts = ix->d_flag.as<int>() + 1;   // n_items, n_parts
     SearchPlan pl{};
     pl.cnt = ix->w_cnt.as<uint32_t>();
     pl.list_len = list_len;
-    pl.list_page_off = ix->d_list_page_off;
-    pl.list_order = ix->d_list_order;
+    pl.list_page_off = ix->d_list_page_off.as<uint32_t>();
+    pl.list_order = ix->d_list_order.as<uint32_t>();
     pl.pair_start = pair_start;
     pl.part_off = part_off;
     pl.n_chunks = n_chunks;
     pl.items = ix->w_items.as<IvfGemmItem>();
     pl.n_items = d_counts;
     pl.n_parts = d_counts + 1;
-    pl.scan_rows = reinterpret_cast<unsigned long long *>(ix->d_flag + 4);
+    pl.scan_rows = reinterpret_cast<unsigned long long *>(ix->d_flag.as<int>() + 4);
     pl.nlist = nl;
     pl.max_items = (int)std::min<int64_t>(max_items, INT32_MAX);
     pl.pages_per_chunk = ppc;
@@ -2818,8 +2729,8 @@ static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, cons
     pf.part_off = part_off;
     pf.n_chunks = n_chunks;
     pf.queries = d_q;
-    pf.sq_step = ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq + ix->d : nullptr;
-    pf.centroids = ix->payload == IVF_PRODUCER_PQ ? ix->d_centroids : nullptr;
+    pf.sq_step = ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq.as<float>() + ix->d : nullptr;
+    pf.centroids = ix->payload == IVF_PRODUCER_PQ ? ix->d_centroids.as<float>() : nullptr;
     pf.qbuf = lut ? nullptr : ix->w_qbuf.as<__nv_bfloat16>();
     pf.inv = ix->w_inv.as<uint32_t>();
     pf.pair_part_base = ix->w_ppb.as<uint32_t>();
@@ -2846,11 +2757,11 @@ static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, cons
         g_launches++;
         if (lut) {   // the per-query tables T[q][j][e] = <q_j, codebook_j[e]> (fp32)
             B200_TRY(ix->w_lut.reserve((size_t)nq * ix->m * pq_codewords(ix->pq_bits) * 4));
-            B200_CUDA_OK(pq4 ? launch_pq4_lut(d_q, nq, ix->d_pad, ix->d_pq, ix->m, ix->dsub, ix->w_lut.as<float>(), s)
-                             : launch_pq_lut(d_q, nq, ix->d_pad, ix->d_pq, ix->m, ix->dsub, ix->w_lut.as<float>(), s));
+            B200_CUDA_OK(pq4 ? launch_pq4_lut(d_q, nq, ix->d_pad, ix->d_pq.as<float>(), ix->m, ix->dsub, ix->w_lut.as<float>(), s)
+                             : launch_pq_lut(d_q, nq, ix->d_pad, ix->d_pq.as<float>(), ix->m, ix->dsub, ix->w_lut.as<float>(), s));
         }
         if (ix->payload != IVF_PRODUCER_PQ) {   // PQ: the pair constant (||q - c||^2 or -<q, c>) is the whole query term
-            query_const_kernel<<<(unsigned)ceil_div(nq * 32, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq + 3 * ix->d : nullptr,
+            query_const_kernel<<<(unsigned)ceil_div(nq * 32, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, ix->payload == IVF_PRODUCER_SQ8 ? ix->d_sq.as<float>() + 3 * ix->d : nullptr,
                                                                                 ix->metric == B200_METRIC_L2, ix->payload == IVF_PRODUCER_TMA, ix->w_qconst.as<float>());
             g_launches++;
         }
@@ -2864,8 +2775,8 @@ static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, cons
     gp.items = ix->w_items.as<IvfGemmItem>();
     gp.n_items_ptr = d_counts;
     gp.list_pages = list_pages;
-    gp.row_bias = ix->d_row_bias;
-    gp.row_ids = ix->d_row_ids;
+    gp.row_bias = ix->d_row_bias.as<float>();
+    gp.row_ids = ix->d_row_ids.as<uint32_t>();
     gp.alive = d_alive;
     gp.pair_part_base = ix->w_ppb.as<uint32_t>();
     gp.part_keys = ix->w_pk.as<float>();
@@ -2892,8 +2803,8 @@ static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, cons
     }
     gp.k = k1;
     gp.producer = ix->payload;
-    gp.codes = reinterpret_cast<const uint8_t *>(ix->d_pool);
-    gp.codebook_bf16 = ix->d_pq_bf16;
+    gp.codes = reinterpret_cast<const uint8_t *>(ix->d_pool.p);
+    gp.codebook_bf16 = ix->d_pq_bf16.as<__nv_bfloat16>();
     gp.code_bytes = ix->code_bytes;
     gp.m = ix->m;
     gp.dsub = ix->dsub;
@@ -2915,7 +2826,7 @@ static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, cons
     }
     cudaError_t e = pq4   ? launch_ivf_pq4_topk(gp, grid, s, &detail)
                     : lut ? launch_ivf_pq_lut_topk(gp, grid, s, &detail)
-                          : launch_ivf_gemm_topk(gp, ix->w_qbuf.p, n_valid + 128, ix->d_pool, (int64_t)ix->pool_pages * kPageRows, grid, s, &detail);
+                          : launch_ivf_gemm_topk(gp, ix->w_qbuf.p, n_valid + 128, ix->d_pool.p, (int64_t)ix->pool_pages * kPageRows, grid, s, &detail);
     if (ix->timing) {
         cudaEventRecord(ix->ev1, s);
         cudaEventRecord(ix->ev_ph[3], s);
@@ -2997,7 +2908,7 @@ static int filter_probe_search(b200_index *ix, const float *d_q, const float *d_
     B200_CUDA_OK(cudaMemsetAsync(d_tot, 0, 24, s));
     auto coarse_keys = [&](int64_t q0, int64_t nqc) {
         coarse_scores_kernel<<<dim3((unsigned)ceil_div(nl, kCoarseTile), (unsigned)ceil_div(nqc, kCoarseTile)), 256, 0, s>>>(
-            d_q + q0 * ix->d_pad, ix->d_pad, ix->d_centroids, ix->d_cnorm, nqc, nl, ix->d, ix->w_cs.as<float>());
+            d_q + q0 * ix->d_pad, ix->d_pad, ix->d_centroids.as<float>(), ix->d_cnorm.as<float>(), nqc, nl, ix->d, ix->w_cs.as<float>());
         g_launches++;
     };
     for (int64_t q0 = 0; q0 < nq; q0 += chunk) {
@@ -3068,11 +2979,11 @@ static int filter_probe_search(b200_index *ix, const float *d_q, const float *d_
                              list_len, list_pages, d_alive, id_offset, d_out_dis + a * k, d_out_ids + a * k, s));
         items += ix->last_items;
         if (split) {   // b200_index_last_scan reports the rows of the whole batch
-            add_u64_kernel<<<1, 1, 0, s>>>(reinterpret_cast<const unsigned long long *>(ix->d_flag + 4), d_tot + 2);
+            add_u64_kernel<<<1, 1, 0, s>>>(reinterpret_cast<const unsigned long long *>(ix->d_flag.as<int>() + 4), d_tot + 2);
             g_launches++;
         }
     }
-    if (split) B200_CUDA_OK(cudaMemcpyAsync(ix->d_flag + 4, d_tot + 2, 8, cudaMemcpyDeviceToDevice, s));
+    if (split) B200_CUDA_OK(cudaMemcpyAsync(ix->d_flag.as<int>() + 4, d_tot + 2, 8, cudaMemcpyDeviceToDevice, s));
     ix->last_items = items;
     return B200_OK;
 }
@@ -3112,7 +3023,7 @@ static int graph_search_locked(b200_index *ix, const float *d_queries, const flo
                                   nullptr, s));
     ix->last_seed_nq = nq;
     ix->last_seed_s = S;
-    unsigned long long *scored = reinterpret_cast<unsigned long long *>(ix->d_flag + 4);
+    unsigned long long *scored = reinterpret_cast<unsigned long long *>(ix->d_flag.as<int>() + 4);
     B200_CUDA_OK(cudaMemsetAsync(scored, 0, 8, s));
     if (two_stage) {
         B200_TRY(ix->w_od.reserve((size_t)nq * kc * 4));
@@ -3122,12 +3033,12 @@ static int graph_search_locked(b200_index *ix, const float *d_queries, const flo
     GraphSearchParams &gp = bp.g;
     gp.queries = ix->binary ? nullptr : d_q;
     if (ix->d_row_slot) {
-        gp.pages = ix->d_pool;
-        gp.row_slot = ix->d_row_slot;
+        gp.pages = ix->d_pool.p;
+        gp.row_slot = ix->d_row_slot.as<uint32_t>();
     } else {
-        gp.rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
+        gp.rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw.get()));
     }
-    gp.graph = ix->d_graph;
+    gp.graph = ix->d_graph.as<uint32_t>();
     gp.seeds = ix->w_seeds.as<int64_t>();
     gp.alive = d_alive;
     gp.out_dis = two_stage ? ix->w_od.as<float>() : d_out_dis;
@@ -3145,7 +3056,7 @@ static int graph_search_locked(b200_index *ix, const float *d_queries, const flo
     gp.l2 = ix->metric == B200_METRIC_L2 || ix->binary;
     if (ix->binary) {
         bp.queries = reinterpret_cast<const uint8_t *>(d_queries);
-        bp.row_popc = ix->d_row_bias;
+        bp.row_popc = ix->d_row_bias.as<float>();
         bp.row_bytes = ix->row_bytes;
         bp.row_pad = ix->row_pad;
         bp.kb_w = ix->kb_w;
@@ -3197,7 +3108,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         if (filter_probe) return fail(B200_ERR_UNSUPPORTED, "filter_probe is not available on binary indexes (their coarse probe ranks at most 1024 lists)");
         if (!ix->use_ivf) {
             ix->last_probe.insert(ix->last_probe.end(), nq, 0);
-            return corpus_search_exact(ix->raw, d_queries, nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s);
+            return corpus_search_exact(ix->raw.get(), d_queries, nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s);
         }
     } else {
         B200_TRY(prepare_queries_device(ix, d_queries, nq, s));
@@ -3227,7 +3138,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         if (d_alive && h_alive && ix->raw && !ix->binary) {
             const int64_t rows_cap = graph_rows_at_cap(ix, std::min(graph_ef(params, kc), kGraphMaxSeeds), width);
             const int64_t limit = std::min<int64_t>((int64_t)std::ceil(kGraphExactFactor * kc * (double)ix->n / (double)rows_cap) - 1,
-                                                    corpus_prefilter_limit(ix->raw, prefilter, nq, k));
+                                                    corpus_prefilter_limit(ix->raw.get(), prefilter, nq, k));
             exact = limit >= 0 && host_count_alive(h_alive, ix->n, limit) <= limit;
             ix->last_probe_exact = exact;
         }
@@ -3237,7 +3148,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         // gathered path for this batch (prefilter mode, nq, k): past the gathered path's limit it would scan every row
         const int np = std::max(1, std::min(parse_int_param(params, "nprobe", ix->default_nprobe), ix->nlist));
         const int64_t limit = std::min<int64_t>((int64_t)(kFilterProbeExactFactor * np * (double)ix->n / (double)ix->nlist),
-                                                corpus_prefilter_limit(ix->raw, prefilter, nq, k));
+                                                corpus_prefilter_limit(ix->raw.get(), prefilter, nq, k));
         exact = limit >= 0 && host_count_alive(h_alive, ix->n, limit) <= limit;
         ix->last_probe_exact = exact;
     }
@@ -3252,7 +3163,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
         if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
         else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
-        B200_TRY(corpus_search_exact(ix->raw, ix->w_qraw.as<float>(), nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s));
+        B200_TRY(corpus_search_exact(ix->raw.get(), ix->w_qraw.as<float>(), nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s));
         if (ix->metric == B200_METRIC_COSINE) {
             cosine_finish_kernel<<<(unsigned)ceil_div(nq * k, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, k, d_out_dis, d_out_ids);
             g_launches++;
@@ -3283,14 +3194,14 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     const float *d_qx = d_q;
     if (ix->d_opq) {
         B200_TRY(ix->w_qrot.reserve((size_t)nq * ix->d_pad * 4));
-        B200_CUDA_OK(launch_opq_rotate(d_qx, ix->d_pad, nq, ix->d, ix->d_opq, ix->w_qrot.as<float>(), ix->d_pad, s));
+        B200_CUDA_OK(launch_opq_rotate(d_qx, ix->d_pad, nq, ix->d, ix->d_opq.as<float>(), ix->w_qrot.as<float>(), ix->d_pad, s));
         d_q = ix->w_qrot.as<float>();
     }
-    const uint32_t *list_len = ix->d_list_len, *list_pages = ix->d_list_pages;
+    const uint32_t *list_len = ix->d_list_len.as<uint32_t>(), *list_pages = ix->d_list_pages.as<uint32_t>();
     if (fprobe) {
         B200_TRY(ix->w_flist.reserve((size_t)nl * 8));
         B200_TRY(ix->w_fpages.reserve((size_t)std::max<uint32_t>(ix->pages_used, 1) * 4));
-        list_alive_kernel<<<(unsigned)nl, 256, 0, s>>>(ix->d_list_len, ix->d_list_page_off, ix->d_list_pages, ix->d_row_ids, d_alive,
+        list_alive_kernel<<<(unsigned)nl, 256, 0, s>>>(ix->d_list_len.as<uint32_t>(), ix->d_list_page_off.as<uint32_t>(), ix->d_list_pages.as<uint32_t>(), ix->d_row_ids.as<uint32_t>(), d_alive,
                                                        ix->w_flist.as<uint32_t>(), ix->w_flist.as<uint32_t>() + nl, ix->w_fpages.as<uint32_t>());
         g_launches++;
         list_len = ix->w_flist.as<uint32_t>() + nl;
@@ -3307,7 +3218,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
             g_launches++;
         } else {
             B200_TRY(pad_bin_rows(ix, d_queries, nq, ix->w_qraw, s));
-            B200_TRY(b200_corpus_search_device(ix->coarse, ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s));
+            B200_TRY(b200_corpus_search_device(ix->coarse.get(), ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s));
         }
     } else {
         B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
@@ -3333,7 +3244,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
             for (int64_t q0 = 0; q0 < nq; q0 += chunk) {
                 const int64_t nqc = std::min(chunk, nq - q0);
                 coarse_scores_kernel<<<dim3((unsigned)ceil_div(nl, kCoarseTile), (unsigned)ceil_div(nqc, kCoarseTile)), 256, 0, s>>>(
-                    d_q + q0 * ix->d_pad, ix->d_pad, ix->d_centroids, ix->d_cnorm, nqc, nl, ix->d, ix->w_cs.as<float>());
+                    d_q + q0 * ix->d_pad, ix->d_pad, ix->d_centroids.as<float>(), ix->d_cnorm.as<float>(), nqc, nl, ix->d, ix->w_cs.as<float>());
                 coarse_select_kernel<<<(unsigned)ceil_div(nqc, 8), 256, sel_smem, s>>>(ix->w_cs.as<float>(), nqc, nl, nprobe, ix->w_pd.as<float>() + q0 * nprobe,
                                                                                        ix->w_probe.as<int64_t>() + q0 * nprobe);
                 g_launches += 2;
@@ -3342,12 +3253,12 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
             ix->last_coarse = 3;
         } else {
             // chosen 2: the corpus' own choice by batch size; forced 2: the tensor-core path whatever the batch
-            b200_corpus_set_path(ix->coarse, coarse_path == 1 ? 1 : forced == 2 ? 2 : 0);
-            const int rc = b200_corpus_search_device(ix->coarse, ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s);
-            b200_corpus_set_path(ix->coarse, 0);
+            b200_corpus_set_path(ix->coarse.get(), coarse_path == 1 ? 1 : forced == 2 ? 2 : 0);
+            const int rc = b200_corpus_search_device(ix->coarse.get(), ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s);
+            b200_corpus_set_path(ix->coarse.get(), 0);
             B200_TRY(rc);
             int kernel = 0;
-            B200_TRY(b200_corpus_last_variant(ix->coarse, &kernel, nullptr, nullptr, nullptr));
+            B200_TRY(b200_corpus_last_variant(ix->coarse.get(), &kernel, nullptr, nullptr, nullptr));
             ix->last_coarse = kernel == B200_KERNEL_SCAN ? 1 : 2;
         }
     }
@@ -3444,7 +3355,7 @@ extern "C" int b200_index_opq(const b200_index *ix, float *out_r, double *out_lo
     if (out_loss && capacity < n) return fail(B200_ERR_INVALID, "opq: capacity " + std::to_string(capacity) + " < " + std::to_string(n));
     if (out_r) {
         B200_CUDA_OK(cudaSetDevice(ix->device));
-        B200_CUDA_OK(cudaMemcpy(out_r, ix->d_opq, (size_t)ix->d * ix->d * 4, cudaMemcpyDeviceToHost));
+        B200_CUDA_OK(cudaMemcpy(out_r, ix->d_opq.as<float>(), (size_t)ix->d * ix->d * 4, cudaMemcpyDeviceToHost));
     }
     if (out_loss) std::copy(ix->opq_loss.begin(), ix->opq_loss.end(), out_loss);
     if (out_n) *out_n = n;
@@ -3476,7 +3387,7 @@ extern "C" int b200_index_graph(const b200_index *ix, uint32_t *out, int64_t cap
     if (out && D) {
         if (capacity_rows < ix->n) return fail(B200_ERR_INVALID, "buffer smaller than the index's rows");
         B200_CUDA_OK(cudaSetDevice(ix->device));
-        B200_CUDA_OK(cudaMemcpy(out, ix->d_graph, (size_t)ix->n * D * 4, cudaMemcpyDeviceToHost));
+        B200_CUDA_OK(cudaMemcpy(out, ix->d_graph.as<uint32_t>(), (size_t)ix->n * D * 4, cudaMemcpyDeviceToHost));
     }
     return B200_OK;
 }
@@ -3574,7 +3485,7 @@ static int index_save_io(b200_index *ix, Io *f) {
             const size_t rb = (size_t)ix->row_bytes;
             const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / (int64_t)rb);
             std::vector<char> buf((size_t)chunk * rb);
-            const char *rows = reinterpret_cast<const char *>(corpus_device_rows(ix->raw));
+            const char *rows = reinterpret_cast<const char *>(corpus_device_rows(ix->raw.get()));
             for (int64_t off = 0; ok && off < ix->n; off += chunk) {
                 const int64_t mrows = std::min(chunk, ix->n - off);
                 ok = cudaMemcpy(buf.data(), rows + off * rb, (size_t)mrows * rb, cudaMemcpyDeviceToHost) == cudaSuccess && wr(f, buf.data(), (size_t)mrows * rb);
@@ -3582,7 +3493,7 @@ static int index_save_io(b200_index *ix, Io *f) {
         } else if (ok && ix->raw) {  // fp32 rows, unpadded (cosine indexes hold unit vectors; they are written as stored)
             const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / ((int64_t)ix->d_pad * 4));
             std::vector<float> buf((size_t)chunk * ix->d_pad);
-            const float *rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw));
+            const float *rows = reinterpret_cast<const float *>(corpus_device_rows(ix->raw.get()));
             for (int64_t off = 0; ok && off < ix->n; off += chunk) {
                 const int64_t mrows = std::min(chunk, ix->n - off);
                 if (cudaMemcpy(buf.data(), rows + off * ix->d_pad, (size_t)mrows * ix->d_pad * 4, cudaMemcpyDeviceToHost) != cudaSuccess) ok = false;
@@ -3598,23 +3509,23 @@ static int index_save_io(b200_index *ix, Io *f) {
                 if (bytes && cudaMemcpy(tmp.data(), dptr, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return false;
                 return wr(f, tmp.data(), bytes);
             };
-            ok = (ix->binary ? dump(ix->d_bcent, (size_t)ix->nlist * ix->cent_pad) : dump(ix->d_centroids, (size_t)ix->nlist * ix->d * 4)) &&
+            ok = (ix->binary ? dump(ix->d_bcent.as<uint8_t>(), (size_t)ix->nlist * ix->cent_pad) : dump(ix->d_centroids.as<float>(), (size_t)ix->nlist * ix->d * 4)) &&
                  wr(f, ix->list_len.data(), (size_t)ix->nlist * 4);
-            if (ok && ix->d_pq) ok = dump(ix->d_pq, (size_t)ix->m * pq_codewords(ix->pq_bits) * ix->dsub * 4);
-            if (ok && ix->d_sq) ok = dump(ix->d_sq, (size_t)4 * ix->d * 4);
+            if (ok && ix->d_pq) ok = dump(ix->d_pq.as<float>(), (size_t)ix->m * pq_codewords(ix->pq_bits) * ix->dsub * 4);
+            if (ok && ix->d_sq) ok = dump(ix->d_sq.as<float>(), (size_t)4 * ix->d * 4);
             std::vector<uint32_t> pages(ix->pages_used);
             if (ok && ix->pages_used)
-                ok = cudaMemcpy(pages.data(), ix->d_list_pages, (size_t)ix->pages_used * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
+                ok = cudaMemcpy(pages.data(), ix->d_list_pages.as<uint32_t>(), (size_t)ix->pages_used * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
             const size_t pb = (size_t)kPageRows * payload_row_bytes(ix);
             for (uint32_t i = 0; ok && i < ix->pages_used; i++) {
                 const size_t row0 = (size_t)pages[i] * kPageRows;
-                ok = dump(reinterpret_cast<const char *>(ix->d_pool) + (size_t)pages[i] * pb, pb) && dump(ix->d_row_ids + row0, kPageRows * 4);
-                if (ok && ix->d_row_bias) ok = dump(ix->d_row_bias + row0, kPageRows * 4);
+                ok = dump(reinterpret_cast<const char *>(ix->d_pool.p) + (size_t)pages[i] * pb, pb) && dump(ix->d_row_ids.as<uint32_t>() + row0, kPageRows * 4);
+                if (ok && ix->d_row_bias) ok = dump(ix->d_row_bias.as<float>() + row0, kPageRows * 4);
             }
         }
         if (ok && ix->d_opq) {
             std::vector<float> r((size_t)ix->d * ix->d);
-            ok = cudaMemcpy(r.data(), ix->d_opq, r.size() * 4, cudaMemcpyDeviceToHost) == cudaSuccess && wr(f, r.data(), r.size() * 4);
+            ok = cudaMemcpy(r.data(), ix->d_opq.as<float>(), r.size() * 4, cudaMemcpyDeviceToHost) == cudaSuccess && wr(f, r.data(), r.size() * 4);
         }
         if (ok && ix->d_graph) {
             const size_t rb = (size_t)ix->graph_degree * 4;
@@ -3622,7 +3533,7 @@ static int index_save_io(b200_index *ix, Io *f) {
             std::vector<char> buf((size_t)chunk * rb);
             for (int64_t off = 0; ok && off < ix->n; off += chunk) {
                 const int64_t mrows = std::min(chunk, ix->n - off);
-                ok = cudaMemcpy(buf.data(), ix->d_graph + off * ix->graph_degree, (size_t)mrows * rb, cudaMemcpyDeviceToHost) == cudaSuccess &&
+                ok = cudaMemcpy(buf.data(), ix->d_graph.as<uint32_t>() + off * ix->graph_degree, (size_t)mrows * rb, cudaMemcpyDeviceToHost) == cudaSuccess &&
                      wr(f, buf.data(), (size_t)mrows * rb);
             }
         }
@@ -3698,14 +3609,14 @@ static int index_load_io(Io *f, b200_index **out) {
         ix->payload = h.payload; ix->use_ivf = h.use_ivf != 0; ix->code_bytes = h.code_bytes; ix->keep_raw = h.has_raw;
         const int raw_metric = h.metric == B200_METRIC_L2 ? B200_METRIC_L2 : B200_METRIC_IP;
         if (h.has_raw && bin) {
-            if (b200_corpus_create(h.metric, B200_DTYPE_BIN, h.d, h.n, &ix->raw) != B200_OK) return bail(b200_last_error());
+            if (corpus_create(h.metric, B200_DTYPE_BIN, h.d, h.n, ix->raw) != B200_OK) return bail(b200_last_error());
             const size_t rb = (size_t)ix->row_bytes;
             const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / (int64_t)rb);
             std::vector<char> buf((size_t)chunk * rb);
             for (int64_t off = 0; off < h.n; off += chunk) {
                 const int64_t mrows = std::min(chunk, h.n - off);
                 if (!rd(f, buf.data(), (size_t)mrows * rb)) return bail("truncated index file (rows)");
-                if (b200_corpus_append(ix->raw, buf.data(), mrows) != B200_OK) return bail(b200_last_error());
+                if (b200_corpus_append(ix->raw.get(), buf.data(), mrows) != B200_OK) return bail(b200_last_error());
             }
         } else if (h.has_raw == 2) {   // straight into pinned host memory, never through HBM
             if (host_rows_reserve(ix, h.n) != B200_OK) return bail(b200_last_error());
@@ -3717,28 +3628,27 @@ static int index_load_io(Io *f, b200_index **out) {
                 for (int64_t r = 0; r < mrows; r++) memcpy(ix->h_rows + (off + r) * ix->d_pad, buf.data() + r * h.d, (size_t)h.d * 4);
             }
         } else if (h.has_raw) {
-            if (b200_corpus_create(raw_metric, B200_DTYPE_F32, h.d, h.n, &ix->raw) != B200_OK) return bail(b200_last_error());
+            if (corpus_create(raw_metric, B200_DTYPE_F32, h.d, h.n, ix->raw) != B200_OK) return bail(b200_last_error());
             const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / ((int64_t)h.d * 4));
             std::vector<float> buf((size_t)chunk * h.d);
             for (int64_t off = 0; off < h.n; off += chunk) {
                 const int64_t mrows = std::min(chunk, h.n - off);
                 if (!rd(f, buf.data(), (size_t)mrows * h.d * 4)) return bail("truncated index file (rows)");
-                if (b200_corpus_append(ix->raw, buf.data(), mrows) != B200_OK) return bail(b200_last_error());
+                if (b200_corpus_append(ix->raw.get(), buf.data(), mrows) != B200_OK) return bail(b200_last_error());
             }
         }
         ix->n = h.n;
         std::vector<uint8_t> in_list;   // row id -> it is in a list
         if (ix->use_ivf) {
             std::vector<char> tmp;
-            auto slurp = [&](void **dptr, size_t bytes) {
+            auto slurp = [&](DevMem &dst, size_t bytes) {
                 tmp.resize(bytes);
                 if (!rd(f, tmp.data(), bytes)) return false;
-                if (cudaMalloc(dptr, bytes + 256) != cudaSuccess) return false;
-                return cudaMemcpy(*dptr, tmp.data(), bytes, cudaMemcpyHostToDevice) == cudaSuccess;
+                return dst.alloc(bytes + 256) == B200_OK && cudaMemcpy(dst.p, tmp.data(), bytes, cudaMemcpyHostToDevice) == cudaSuccess;
             };
             const int nl = h.nlist;
             ix->list_len.resize(nl);
-            if (!(bin ? slurp((void **)&ix->d_bcent, (size_t)nl * ix->cent_pad) : slurp((void **)&ix->d_centroids, (size_t)nl * h.d * 4)) ||
+            if (!(bin ? slurp(ix->d_bcent, (size_t)nl * ix->cent_pad) : slurp(ix->d_centroids, (size_t)nl * h.d * 4)) ||
                 !rd(f, ix->list_len.data(), (size_t)nl * 4))
                 return bail("truncated index file (quantiser)");
             uint64_t total = 0, pages = 0;
@@ -3753,22 +3663,22 @@ static int index_load_io(Io *f, b200_index **out) {
             // unusable rows are in no list: the lists hold at most n rows
             if (total > (uint64_t)h.n || pages != h.pages_used) return bail("corrupt index file (list lengths do not add up)");
             if (h.payload == IVF_PRODUCER_PQ) {
-                if (!slurp((void **)&ix->d_pq, (size_t)h.m * pq_codewords(pq_bits) * h.dsub * 4)) return bail("truncated index file (codebook)");
+                if (!slurp(ix->d_pq, (size_t)h.m * pq_codewords(pq_bits) * h.dsub * 4)) return bail("truncated index file (codebook)");
                 if (pq_bits == 4) {
                     // validated with the header: the 4-bit look-up scan reads the fp32 codebook
                 } else if (pq_dsub_decodable(h.dsub)) {   // the tensor-core decoder's bf16 copy; the table look-up scan reads the fp32 codebook
-                    if (cudaMalloc(&ix->d_pq_bf16, (size_t)h.m * 256 * h.dsub * 2) != cudaSuccess) return bail("cudaMalloc failed");
-                    if (launch_f32_to_bf16_rows(ix->d_pq, h.dsub, ix->d_pq_bf16, h.dsub, (int64_t)h.m * 256, ix->stream) != cudaSuccess)
+                    if (ix->d_pq_bf16.alloc((size_t)h.m * 256 * h.dsub * 2) != B200_OK) return bail("cudaMalloc failed");
+                    if (launch_f32_to_bf16_rows(ix->d_pq.as<float>(), h.dsub, ix->d_pq_bf16.as<__nv_bfloat16>(), h.dsub, (int64_t)h.m * 256, ix->stream) != cudaSuccess)
                         return bail("codebook conversion failed");
                 } else if (!ivf_pq_lut_fits(h.m)) {
                     return bail("corrupt index header (PQ M too large for the table look-up scan)");
                 }
             }
-            if (h.payload == IVF_PRODUCER_SQ8 && !slurp((void **)&ix->d_sq, (size_t)4 * h.d * 4)) return bail("truncated index file (SQ ranges)");
+            if (h.payload == IVF_PRODUCER_SQ8 && !slurp(ix->d_sq, (size_t)4 * h.d * 4)) return bail("truncated index file (SQ ranges)");
             ix->pool_pages = ix->pages_used = h.pages_used;
             const size_t pb = (size_t)kPageRows * payload_row_bytes(ix), rows = (size_t)std::max<uint32_t>(h.pages_used, 1) * kPageRows;
-            if (cudaMalloc(&ix->d_pool, rows * payload_row_bytes(ix) + 256) != cudaSuccess || cudaMalloc(&ix->d_row_ids, rows * 4) != cudaSuccess ||
-                ((h.metric == B200_METRIC_L2 || bin) && cudaMalloc(&ix->d_row_bias, rows * 4) != cudaSuccess))
+            if (ix->d_pool.alloc(rows * payload_row_bytes(ix) + 256) != B200_OK || ix->d_row_ids.alloc(rows * 4) != B200_OK ||
+                ((h.metric == B200_METRIC_L2 || bin) && ix->d_row_bias.alloc(rows * 4) != B200_OK))
                 return bail("cudaMalloc of the page pool failed");
             std::vector<char> page(pb);
             std::vector<uint32_t> ids(kPageRows);
@@ -3786,9 +3696,9 @@ static int index_load_io(Io *f, b200_index **out) {
                         in_list[ids[r]] = 1;
                     }
                     const size_t row0 = (size_t)pg * kPageRows;
-                    if (cudaMemcpy(reinterpret_cast<char *>(ix->d_pool) + (size_t)pg * pb, page.data(), pb, cudaMemcpyHostToDevice) != cudaSuccess ||
-                        cudaMemcpy(ix->d_row_ids + row0, ids.data(), kPageRows * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
-                        (ix->d_row_bias && cudaMemcpy(ix->d_row_bias + row0, bias.data(), kPageRows * 4, cudaMemcpyHostToDevice) != cudaSuccess))
+                    if (cudaMemcpy(reinterpret_cast<char *>(ix->d_pool.p) + (size_t)pg * pb, page.data(), pb, cudaMemcpyHostToDevice) != cudaSuccess ||
+                        cudaMemcpy(ix->d_row_ids.as<uint32_t>() + row0, ids.data(), kPageRows * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+                        (ix->d_row_bias && cudaMemcpy(ix->d_row_bias.as<float>() + row0, bias.data(), kPageRows * 4, cudaMemcpyHostToDevice) != cudaSuccess))
                         return bail("H2D failed");
                 }
             }
@@ -3796,14 +3706,13 @@ static int index_load_io(Io *f, b200_index **out) {
             for (uint32_t i = 0; i < h.pages_used; i++) iota_pages[i] = i;
             for (int l = 0; l < nl; l++) order[l] = (uint32_t)l;
             std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return ix->list_len[a] > ix->list_len[b]; });
-            auto up = [&](uint32_t **dptr, const std::vector<uint32_t> &v, size_t count) {
-                return cudaMalloc(dptr, std::max<size_t>(count, 1) * 4) == cudaSuccess &&
-                       cudaMemcpy(*dptr, v.data(), count * 4, cudaMemcpyHostToDevice) == cudaSuccess;
+            auto up = [&](DevMem &dst, const std::vector<uint32_t> &v, size_t count) {
+                return dst.alloc(std::max<size_t>(count, 1) * 4) == B200_OK && cudaMemcpy(dst.p, v.data(), count * 4, cudaMemcpyHostToDevice) == cudaSuccess;
             };
-            if (!up(&ix->d_list_pages, iota_pages, h.pages_used) || !up(&ix->d_list_page_off, page_off, (size_t)nl + 1) ||
-                !up(&ix->d_list_order, order, nl) || !up(&ix->d_list_len, ix->list_len, nl) || cudaMalloc(&ix->d_flag, 32) != cudaSuccess)
+            if (!up(ix->d_list_pages, iota_pages, h.pages_used) || !up(ix->d_list_page_off, page_off, (size_t)nl + 1) || !up(ix->d_list_order, order, nl) ||
+                !up(ix->d_list_len, ix->list_len, nl) || ix->d_flag.alloc(32) != B200_OK)
                 return bail("cudaMalloc failed");
-            cudaMemset(ix->d_flag, 0, 32);
+            cudaMemset(ix->d_flag.as<int>(), 0, 32);
             if ((bin ? upload_coarse_bin(ix, ix->stream) : upload_coarse(ix, ix->stream)) != B200_OK) return bail(b200_last_error());
             if (cudaStreamSynchronize(ix->stream) != cudaSuccess) return bail("upload failed");
         }
@@ -3813,9 +3722,9 @@ static int index_load_io(Io *f, b200_index **out) {
             for (float v : r)
                 if (!std::isfinite(v)) return bail("corrupt index file (OPQ rotation not finite)");
             double err = 0;
-            if (cudaMalloc(&ix->d_opq, r.size() * 4) != cudaSuccess ||
-                cudaMemcpy(ix->d_opq, r.data(), r.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
-                opq_orthonormal_error(ix->d_opq, h.d, &err, ix->stream) != B200_OK)
+            if (ix->d_opq.alloc(r.size() * 4) != B200_OK ||
+                cudaMemcpy(ix->d_opq.as<float>(), r.data(), r.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+                opq_orthonormal_error(ix->d_opq.as<float>(), h.d, &err, ix->stream) != B200_OK)
                 return bail(std::string("OPQ rotation upload: ") + b200_last_error());
             if (!(err <= kOpqLoadTol)) return bail("corrupt index file (OPQ rotation not orthonormal: max |R^T R - I| = " + std::to_string(err) + ")");
             ix->opq = 1;
@@ -3825,7 +3734,7 @@ static int index_load_io(Io *f, b200_index **out) {
             const size_t rb = (size_t)D * 4;
             const int64_t chunk = std::max<int64_t>(1, (64ll << 20) / (int64_t)rb);
             std::vector<uint32_t> buf((size_t)chunk * D);
-            if (cudaMalloc(&ix->d_graph, std::max<size_t>((size_t)h.n * rb, 16)) != cudaSuccess) return bail("cudaMalloc of the graph failed");
+            if (ix->d_graph.alloc(std::max<size_t>((size_t)h.n * rb, 16)) != B200_OK) return bail("cudaMalloc of the graph failed");
             ix->graph_degree = D;
             for (int64_t off = 0; off < h.n; off += chunk) {
                 const int64_t mrows = std::min(chunk, h.n - off);
@@ -3835,7 +3744,7 @@ static int index_load_io(Io *f, b200_index **out) {
                     if (buf[e] >= (uint64_t)h.n) return bail("corrupt index file (graph id out of range)");
                     if (walks_pages && !in_list[buf[e]]) return bail("corrupt index file (graph edge to a row in no list)");
                 }
-                if (cudaMemcpy(ix->d_graph + off * D, buf.data(), (size_t)mrows * rb, cudaMemcpyHostToDevice) != cudaSuccess) return bail("H2D failed");
+                if (cudaMemcpy(ix->d_graph.as<uint32_t>() + off * D, buf.data(), (size_t)mrows * rb, cudaMemcpyHostToDevice) != cudaSuccess) return bail("H2D failed");
             }
             // MSTG / BINARYMSTG: the slot map of the pages as loaded here
             if (walks_pages && (build_row_slot(ix) != B200_OK || cudaStreamSynchronize(ix->stream) != cudaSuccess))

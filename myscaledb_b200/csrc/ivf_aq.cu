@@ -376,57 +376,57 @@ int aq_train_codebooks(const AqTrain &t, std::vector<double> *loss, cudaStream_t
     if (!smem) return fail(B200_ERR_UNSUPPORTED, "aq_threshold: a row of d = " + std::to_string(t.d) + " does not fit the encoder's shared memory");
     B200_CUDA_OK(cudaFuncSetAttribute(aq_encode_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int64_t n = t.n;
-    uint8_t *codes = nullptr, *key = nullptr, *key_s = nullptr;
-    uint32_t *row = nullptr, *member = nullptr, *cnt = nullptr;
-    double *p = nullptr, *w = nullptr, *dl = nullptr;
-    float *old_cb = nullptr;
-    void *tmp = nullptr;
+    const int bits = t.ncw == 16 ? 4 : 8;
+    DevMem codes_b, key_b, key_s_b, row_b, member_b, cnt_b, p_b, w_b, dl_b, old_cb_b, tmp;
     size_t tmp_bytes = 0;
-    int bits = t.ncw == 16 ? 4 : 8;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, key, key_s, row, member, (int)n, 0, bits, s);
-    int rc = B200_OK;
-    auto ok = [&](cudaError_t e) {
-        if (e != cudaSuccess && rc == B200_OK) rc = fail(B200_ERR_CUDA, std::string("anisotropic PQ training: ") + cudaGetErrorString(e));
-        return rc == B200_OK;
-    };
-    ok(cudaMalloc(&codes, (size_t)n * t.m)) && ok(cudaMalloc(&key, (size_t)n)) && ok(cudaMalloc(&key_s, (size_t)n)) &&
-        ok(cudaMalloc(&row, (size_t)n * 4)) && ok(cudaMalloc(&member, (size_t)n * 4)) && ok(cudaMalloc(&cnt, (size_t)t.ncw * 4)) &&
-        ok(cudaMalloc(&p, (size_t)n * 8)) && ok(cudaMalloc(&w, (size_t)n * 8)) && ok(cudaMalloc(&dl, (size_t)n * 8)) &&
-        ok(cudaMalloc(&old_cb, (size_t)t.ncw * t.dsub * 4)) && ok(cudaMalloc(&tmp, tmp_bytes + 256));
+    cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, key_b.as<uint8_t>(), key_s_b.as<uint8_t>(), row_b.as<uint32_t>(), member_b.as<uint32_t>(), (int)n, 0,
+                                    bits, s);
+    B200_TRY(codes_b.alloc((size_t)n * t.m));
+    B200_TRY(key_b.alloc((size_t)n));
+    B200_TRY(key_s_b.alloc((size_t)n));
+    B200_TRY(row_b.alloc((size_t)n * 4));
+    B200_TRY(member_b.alloc((size_t)n * 4));
+    B200_TRY(cnt_b.alloc((size_t)t.ncw * 4));
+    B200_TRY(p_b.alloc((size_t)n * 8));
+    B200_TRY(w_b.alloc((size_t)n * 8));
+    B200_TRY(dl_b.alloc((size_t)n * 8));
+    B200_TRY(old_cb_b.alloc((size_t)t.ncw * t.dsub * 4));
+    B200_TRY(tmp.alloc(tmp_bytes + 256));
+    uint8_t *codes = codes_b.as<uint8_t>(), *key = key_b.as<uint8_t>(), *key_s = key_s_b.as<uint8_t>();
+    uint32_t *row = row_b.as<uint32_t>(), *member = member_b.as<uint32_t>(), *cnt = cnt_b.as<uint32_t>();
+    double *p = p_b.as<double>(), *w = w_b.as<double>(), *dl = dl_b.as<double>();
+    float *old_cb = old_cb_b.as<float>();
     std::vector<double> h;
     const int rows_grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n * 32, 256), 132 * 32));
-    for (int it = 0; it < kAqIters && rc == B200_OK; it++) {
+    for (int it = 0; it < kAqIters; it++) {
         aq_encode_sample_kernel<<<aq_grid(n), kAqWarps * 32, smem, s>>>(t, (float)t.eta, codes);
         aq_state_kernel<<<rows_grid, 256, 0, s>>>(t, t.eta, codes, p, w, dl);
         g_launches += 2;
         double mean = 0;
-        if (it == 0 && ok(cudaGetLastError())) {
-            rc = aq_mean_loss(dl, n, h, &mean, s);
-            if (rc == B200_OK) loss->push_back(mean);
+        if (it == 0) {
+            B200_CUDA_OK(cudaGetLastError());
+            B200_TRY(aq_mean_loss(dl, n, h, &mean, s));
+            loss->push_back(mean);
         }
-        for (int j = 0; j < t.m && rc == B200_OK; j++) {
+        for (int j = 0; j < t.m; j++) {
             float *cbj = t.pq + (size_t)j * t.ncw * t.dsub;
-            if (!ok(cudaMemcpyAsync(old_cb, cbj, (size_t)t.ncw * t.dsub * 4, cudaMemcpyDeviceToDevice, s)) ||
-                !ok(cudaMemsetAsync(cnt, 0, (size_t)t.ncw * 4, s)))
-                break;
+            B200_CUDA_OK(cudaMemcpyAsync(old_cb, cbj, (size_t)t.ncw * t.dsub * 4, cudaMemcpyDeviceToDevice, s));
+            B200_CUDA_OK(cudaMemsetAsync(cnt, 0, (size_t)t.ncw * 4, s));
             aq_column_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(codes, n, t.m, j, key, row, cnt);
-            if (!ok(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, key, key_s, row, member, (int)n, 0, bits, s))) break;
+            B200_CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, key, key_s, row, member, (int)n, 0, bits, s));
             aq_update_kernel<<<t.ncw, 256, 0, s>>>(t, j, member, cnt, p, w, old_cb);
             aq_refresh_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, s>>>(t, j, codes, old_cb, p);
             g_launches += 4;
-            ok(cudaGetLastError());
+            B200_CUDA_OK(cudaGetLastError());
         }
-        if (rc != B200_OK) break;
         aq_state_kernel<<<rows_grid, 256, 0, s>>>(t, t.eta, codes, p, w, dl);
         g_launches++;
-        if (ok(cudaGetLastError())) rc = aq_mean_loss(dl, n, h, &mean, s);
-        if (rc == B200_OK) loss->push_back(mean);
+        B200_CUDA_OK(cudaGetLastError());
+        B200_TRY(aq_mean_loss(dl, n, h, &mean, s));
+        loss->push_back(mean);
     }
-    cudaStreamSynchronize(s);
-    for (void *q : {(void *)codes, (void *)key, (void *)key_s, (void *)row, (void *)member, (void *)cnt, (void *)p, (void *)w, (void *)dl,
-                    (void *)old_cb, tmp})
-        if (q) cudaFree(q);
-    return rc;
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    return B200_OK;
 }
 
 }  // namespace b200

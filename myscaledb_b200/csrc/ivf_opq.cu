@@ -387,44 +387,38 @@ __global__ void f64_to_f32_kernel(const double *a, int64_t n, float *out) {
 
 int opq_procrustes(const float *res, const float *xhat, int64_t n, int d, float *R, cudaStream_t s) {
     const size_t dd = (size_t)d * d;
-    double *A = nullptr, *V = nullptr, *P = nullptr, *scratch = nullptr;
-    int *flag = nullptr;
-    int rc = B200_OK;
-    auto cuda_ok = [&](cudaError_t e, const char *what) {
-        if (e != cudaSuccess && rc == B200_OK) rc = fail(B200_ERR_CUDA, std::string("OPQ Procrustes step: ") + what + ": " + cudaGetErrorString(e));
-        return rc == B200_OK;
-    };
-    if (cuda_ok(cudaMalloc(&A, dd * 8), "cudaMalloc") && cuda_ok(cudaMalloc(&V, dd * 8), "cudaMalloc") && cuda_ok(cudaMalloc(&P, dd * 8), "cudaMalloc") &&
-        cuda_ok(cudaMalloc(&scratch, (size_t)3 * d * 8), "cudaMalloc") && cuda_ok(cudaMalloc(&flag, 4), "cudaMalloc")) {
-        const dim3 tiles((unsigned)ceil_div(d, 64), (unsigned)ceil_div(d, 64));
-        // A column-major = M^T row-major: A[j][i] = M[i][j] = sum_r res[r][i] xhat[r][j]
-        atb_f64_kernel<float><<<tiles, 256, 0, s>>>(xhat, d, res, d, n, d, d, A);
-        identity_f64_kernel<<<grid_of((int64_t)dd), 256, 0, s>>>(V, d);
-        g_launches += 2;
-        const int np = d + (d & 1);
-        for (int sweep = 0; sweep < kJacobiMaxSweeps && rc == B200_OK; sweep++) {
-            int any = 0;
-            cuda_ok(cudaMemsetAsync(flag, 0, 4, s), "memset");
-            for (int r = 0; r < np - 1; r++) jacobi_round_kernel<<<(unsigned)(np / 2), 256, 0, s>>>(A, V, d, np, r, flag);
-            g_launches += np - 1;
-            cuda_ok(cudaGetLastError(), "Jacobi round");
-            cuda_ok(cudaMemcpyAsync(&any, flag, 4, cudaMemcpyDeviceToHost, s), "flag read-back");
-            cuda_ok(cudaStreamSynchronize(s), "Jacobi sweep");
-            if (!any) break;
-        }
-        if (rc == B200_OK) {
-            polar_complete_kernel<<<1, 1024, 0, s>>>(A, d, scratch, scratch + d, scratch + 2 * d);
-            // R[i][j] = sum_k U[i][k] V[j][k]: U and V are column-major, so this is A^T B over k
-            atb_f64_kernel<double><<<tiles, 256, 0, s>>>(A, d, V, d, d, d, d, P);
-            f64_to_f32_kernel<<<grid_of((int64_t)dd), 256, 0, s>>>(P, (int64_t)dd, R);
-            g_launches += 3;
-            cuda_ok(cudaGetLastError(), "polar factor");
-            cuda_ok(cudaStreamSynchronize(s), "polar factor");
-        }
+    DevMem A_b, V_b, P_b, scratch_b, flag_b;
+    B200_TRY(A_b.alloc(dd * 8));
+    B200_TRY(V_b.alloc(dd * 8));
+    B200_TRY(P_b.alloc(dd * 8));
+    B200_TRY(scratch_b.alloc((size_t)3 * d * 8));
+    B200_TRY(flag_b.alloc(4));
+    double *A = A_b.as<double>(), *V = V_b.as<double>(), *P = P_b.as<double>(), *scratch = scratch_b.as<double>();
+    int *flag = flag_b.as<int>();
+    const dim3 tiles((unsigned)ceil_div(d, 64), (unsigned)ceil_div(d, 64));
+    // A column-major = M^T row-major: A[j][i] = M[i][j] = sum_r res[r][i] xhat[r][j]
+    atb_f64_kernel<float><<<tiles, 256, 0, s>>>(xhat, d, res, d, n, d, d, A);
+    identity_f64_kernel<<<grid_of((int64_t)dd), 256, 0, s>>>(V, d);
+    g_launches += 2;
+    const int np = d + (d & 1);
+    for (int sweep = 0; sweep < kJacobiMaxSweeps; sweep++) {
+        int any = 0;
+        B200_CUDA_OK(cudaMemsetAsync(flag, 0, 4, s));
+        for (int r = 0; r < np - 1; r++) jacobi_round_kernel<<<(unsigned)(np / 2), 256, 0, s>>>(A, V, d, np, r, flag);
+        g_launches += np - 1;
+        B200_CUDA_OK(cudaGetLastError());
+        B200_CUDA_OK(cudaMemcpyAsync(&any, flag, 4, cudaMemcpyDeviceToHost, s));
+        B200_CUDA_OK(cudaStreamSynchronize(s));
+        if (!any) break;
     }
-    for (void *p : {(void *)A, (void *)V, (void *)P, (void *)scratch, (void *)flag})
-        if (p) cudaFree(p);
-    return rc;
+    polar_complete_kernel<<<1, 1024, 0, s>>>(A, d, scratch, scratch + d, scratch + 2 * d);
+    // R[i][j] = sum_k U[i][k] V[j][k]: U and V are column-major, so this is A^T B over k
+    atb_f64_kernel<double><<<tiles, 256, 0, s>>>(A, d, V, d, d, d, d, P);
+    f64_to_f32_kernel<<<grid_of((int64_t)dd), 256, 0, s>>>(P, (int64_t)dd, R);
+    g_launches += 3;
+    B200_CUDA_OK(cudaGetLastError());
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    return B200_OK;
 }
 
 // out[i] = max_j |P[i][j] - (i == j)|, one thread per row
@@ -437,18 +431,15 @@ __global__ void eye_row_err_kernel(const double *P, int d, double *out) {
 }
 
 int opq_orthonormal_error(const float *R, int d, double *max_err, cudaStream_t s) {
-    double *P = nullptr;
-    if (cudaMalloc(&P, ((size_t)d * d + d) * 8) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(B200_ERR_NOMEM, "cudaMalloc failed (OPQ rotation check)");
-    }
+    DevMem P_b;
+    B200_TRY(P_b.alloc(((size_t)d * d + d) * 8));
+    double *P = P_b.as<double>();
     atb_f64_kernel<float><<<dim3((unsigned)ceil_div(d, 64), (unsigned)ceil_div(d, 64)), 256, 0, s>>>(R, d, R, d, d, d, d, P);
     eye_row_err_kernel<<<(unsigned)ceil_div(d, 128), 128, 0, s>>>(P, d, P + (size_t)d * d);
     g_launches += 2;
     std::vector<double> h(d);
     const cudaError_t e = cudaMemcpyAsync(h.data(), P + (size_t)d * d, (size_t)d * 8, cudaMemcpyDeviceToHost, s);
     const cudaError_t e2 = cudaStreamSynchronize(s);
-    cudaFree(P);
     if (e != cudaSuccess || e2 != cudaSuccess) return fail(B200_ERR_CUDA, std::string("OPQ rotation check: ") + cudaGetErrorString(e != cudaSuccess ? e : e2));
     double m = 0;
     for (double v : h) m = std::max(m, v);   // NaN rows (none: R is checked finite first) would not raise it

@@ -96,10 +96,6 @@ extern "C" int b200_bitmap_and_device(const uint8_t *d_a, const uint8_t *d_b, in
 }
 
 namespace {
-struct Scratch {
-    char *d = nullptr;
-    ~Scratch() { if (d) cudaFree(d); }
-};
 int device_ok() {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
@@ -117,16 +113,17 @@ extern "C" int b200_bitmap_and(const uint8_t *a, const uint8_t *b, int64_t nbits
     B200_TRY(device_ok());
     if (nbits == 0) return B200_OK;
     const int64_t nbytes = ceil_div(nbits, 8), nwords = ceil_div(nbytes, 4);
-    Scratch s;
-    B200_CUDA_OK(cudaMalloc(&s.d, (size_t)nwords * 4 * 3));
-    B200_CUDA_OK(cudaMemset(s.d, 0, (size_t)nwords * 4 * 3));
-    B200_CUDA_OK(cudaMemcpy(s.d, a, nbytes, cudaMemcpyHostToDevice));
-    B200_CUDA_OK(cudaMemcpy(s.d + nwords * 4, b, nbytes, cudaMemcpyHostToDevice));
-    bitmap_and_kernel<<<blocks_for(nwords), 256>>>((const uint32_t *)s.d, (const uint32_t *)(s.d + nwords * 4), nwords,
-                                                   (uint32_t *)(s.d + nwords * 8));
+    DevMem s;
+    B200_TRY(s.alloc((size_t)nwords * 4 * 3));
+    char *d = s.as<char>();
+    B200_CUDA_OK(cudaMemset(d, 0, (size_t)nwords * 4 * 3));
+    B200_CUDA_OK(cudaMemcpy(d, a, nbytes, cudaMemcpyHostToDevice));
+    B200_CUDA_OK(cudaMemcpy(d + nwords * 4, b, nbytes, cudaMemcpyHostToDevice));
+    bitmap_and_kernel<<<blocks_for(nwords), 256>>>((const uint32_t *)d, (const uint32_t *)(d + nwords * 4), nwords,
+                                                   (uint32_t *)(d + nwords * 8));
     g_launches++;
     B200_CUDA_OK(cudaGetLastError());
-    B200_CUDA_OK(cudaMemcpy(out, s.d + nwords * 8, nbytes, cudaMemcpyDeviceToHost));
+    B200_CUDA_OK(cudaMemcpy(out, d + nwords * 8, nbytes, cudaMemcpyDeviceToHost));
     return B200_OK;
 }
 
@@ -138,20 +135,21 @@ extern "C" int b200_real_bitmap(const uint8_t *filter_bits, int64_t n_new_rows, 
     B200_TRY(device_ok());
     const int64_t fbytes = ceil_div(n_new_rows, 8), owords = ceil_div(ceil_div(total_vec, 8), 4);
     if (total_vec == 0) return B200_OK;
-    Scratch s;
+    DevMem s;
     const size_t o_f = 0, o_ids = round_up(fbytes, 256), o_src = o_ids + (size_t)n_new_rows * 8, o_out = round_up(o_src + n_new_rows, 256);
-    B200_CUDA_OK(cudaMalloc(&s.d, o_out + (size_t)owords * 4 + 256));
-    B200_CUDA_OK(cudaMemset(s.d + o_out, 0, (size_t)owords * 4));
+    B200_TRY(s.alloc(o_out + (size_t)owords * 4 + 256));
+    char *d = s.as<char>();
+    B200_CUDA_OK(cudaMemset(d + o_out, 0, (size_t)owords * 4));
     if (n_new_rows) {
-        B200_CUDA_OK(cudaMemcpy(s.d + o_f, filter_bits, fbytes, cudaMemcpyHostToDevice));
-        B200_CUDA_OK(cudaMemcpy(s.d + o_ids, inverted_row_ids_map, (size_t)n_new_rows * 8, cudaMemcpyHostToDevice));
-        B200_CUDA_OK(cudaMemcpy(s.d + o_src, inverted_row_sources_map, n_new_rows, cudaMemcpyHostToDevice));
-        real_bitmap_kernel<<<blocks_for(n_new_rows), 256>>>((const uint8_t *)(s.d + o_f), n_new_rows, (const uint64_t *)(s.d + o_ids),
-                                                            (const uint8_t *)(s.d + o_src), own_id, total_vec, (uint32_t *)(s.d + o_out));
+        B200_CUDA_OK(cudaMemcpy(d + o_f, filter_bits, fbytes, cudaMemcpyHostToDevice));
+        B200_CUDA_OK(cudaMemcpy(d + o_ids, inverted_row_ids_map, (size_t)n_new_rows * 8, cudaMemcpyHostToDevice));
+        B200_CUDA_OK(cudaMemcpy(d + o_src, inverted_row_sources_map, n_new_rows, cudaMemcpyHostToDevice));
+        real_bitmap_kernel<<<blocks_for(n_new_rows), 256>>>((const uint8_t *)(d + o_f), n_new_rows, (const uint64_t *)(d + o_ids),
+                                                            (const uint8_t *)(d + o_src), own_id, total_vec, (uint32_t *)(d + o_out));
         g_launches++;
         B200_CUDA_OK(cudaGetLastError());
     }
-    B200_CUDA_OK(cudaMemcpy(out_bits, s.d + o_out, ceil_div(total_vec, 8), cudaMemcpyDeviceToHost));
+    B200_CUDA_OK(cudaMemcpy(out_bits, d + o_out, ceil_div(total_vec, 8), cudaMemcpyDeviceToHost));
     return B200_OK;
 }
 
@@ -160,15 +158,16 @@ extern "C" int b200_remap_labels(const uint64_t *row_ids_map, int64_t map_len, i
     if (!row_ids_map || !labels || map_len < 0 || n < 0) return fail(B200_ERR_INVALID, "bad arguments");
     B200_TRY(device_ok());
     if (n == 0 || map_len == 0) return B200_OK;
-    Scratch s;
+    DevMem s;
     const size_t o_l = round_up(map_len * 8, 256);
-    B200_CUDA_OK(cudaMalloc(&s.d, o_l + (size_t)n * 8 + 256));
-    B200_CUDA_OK(cudaMemcpy(s.d, row_ids_map, (size_t)map_len * 8, cudaMemcpyHostToDevice));
-    B200_CUDA_OK(cudaMemcpy(s.d + o_l, labels, (size_t)n * 8, cudaMemcpyHostToDevice));
-    remap_labels_kernel<<<blocks_for(n), 256>>>((const uint64_t *)s.d, map_len, (int64_t *)(s.d + o_l), n);
+    B200_TRY(s.alloc(o_l + (size_t)n * 8 + 256));
+    char *d = s.as<char>();
+    B200_CUDA_OK(cudaMemcpy(d, row_ids_map, (size_t)map_len * 8, cudaMemcpyHostToDevice));
+    B200_CUDA_OK(cudaMemcpy(d + o_l, labels, (size_t)n * 8, cudaMemcpyHostToDevice));
+    remap_labels_kernel<<<blocks_for(n), 256>>>((const uint64_t *)d, map_len, (int64_t *)(d + o_l), n);
     g_launches++;
     B200_CUDA_OK(cudaGetLastError());
-    B200_CUDA_OK(cudaMemcpy(labels, s.d + o_l, (size_t)n * 8, cudaMemcpyDeviceToHost));
+    B200_CUDA_OK(cudaMemcpy(labels, d + o_l, (size_t)n * 8, cudaMemcpyDeviceToHost));
     return B200_OK;
 }
 

@@ -222,6 +222,13 @@ def launch_count(reset=False) -> int:
     return int(lib().b200_launch_count(C.c_int(1 if reset else 0)))
 
 
+def device_bytes() -> int:
+    """Bytes of device memory the library holds (every index, corpus, workspace and per-thread scratch)."""
+    f = lib().b200_device_bytes
+    f.restype = C.c_int64
+    return int(f())
+
+
 class BM25Index:
     """Per-part BM25 index resident in HBM (mirror of the TantivyIndexStore calls,
     src/Storages/MergeTree/TantivyIndexStore.cpp:742-998)."""

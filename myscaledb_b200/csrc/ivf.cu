@@ -1369,6 +1369,35 @@ static int parse_float_param(const char *json, const char *key, double defv, dou
     return 0;
 }
 
+// The search keys of a params string (include/b200_search.h), read once per search by search_opts, their only reader; params
+// null: the index's defaults.  Only search_width is read signed: a negative value of another key reads as absent.  Reading
+// validates nothing: each key is checked where the path that uses it runs, so a key of a path not taken is accepted as given.
+struct SearchOpts {
+    int exact_batch, prefilter, filter_probe;
+    int nprobe;          // clamped to [1, nlist]
+    int max_nprobe;      // clamped to [nprobe, nlist]
+    int refine_factor;   // at least 1
+    int graph, ef_s, search_width;
+    int coarse_path, pages_per_chunk, shared_bound;   // A/B switches
+};
+
+static SearchOpts search_opts(const b200_index *ix, const char *params) {
+    SearchOpts o;
+    o.exact_batch = parse_int_param(params, "exact_batch", 0);
+    o.prefilter = parse_int_param(params, "prefilter", 0);
+    o.filter_probe = parse_int_param(params, "filter_probe", 0);
+    o.nprobe = std::max(1, std::min(parse_int_param(params, "nprobe", ix->default_nprobe), ix->nlist));
+    o.max_nprobe = std::max(o.nprobe, std::min(ix->nlist, parse_int_param(params, "max_nprobe", ix->nlist)));
+    o.refine_factor = std::max(1, parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", ix->refine_factor)));
+    o.graph = parse_int_param(params, "graph", 1);
+    o.ef_s = parse_int_param(params, "ef_s", 64);
+    o.search_width = parse_int_param(params, "search_width", 1, true);
+    o.coarse_path = parse_int_param(params, "coarse_path", 0);
+    o.pages_per_chunk = parse_int_param(params, "pages_per_chunk", 0);
+    o.shared_bound = parse_int_param(params, "shared_bound", 1);
+    return o;
+}
+
 extern "C" int b200_index_create(const char *type, int metric, int d, const char *params, b200_index **out) {
     if (!type || !out || d <= 0) return fail(B200_ERR_INVALID, "bad arguments");
     *out = nullptr;
@@ -1508,6 +1537,7 @@ static int pq_code_bytes(int m, int bits) { return (int)round_up(bits == 4 ? (m 
 
 // the per-query tables of the look-up scan take at most this much scratch; larger batches run in query sub-batches
 constexpr int64_t kPqLutScratchBytes = (int64_t)256 << 20;
+static int64_t pq_lut_max_queries(const b200_index *ix) { return std::max<int64_t>(1, kPqLutScratchBytes / ((int64_t)ix->m * pq_codewords(ix->pq_bits) * 4)); }
 
 static size_t payload_row_bytes(const b200_index *ix) {
     if (ix->payload == IVF_PRODUCER_B1) return (size_t)ix->row_pad;
@@ -2230,7 +2260,7 @@ extern "C" int b200_index_add(b200_index *ix, const float *rows, int64_t n) {
     return B200_OK;
 }
 
-static int search_device_locked(b200_index *ix, const float *d_queries, int64_t nq, int k, const char *params, int first_stage_only,
+static int search_device_locked(b200_index *ix, const float *d_queries, int64_t nq, int k, const SearchOpts &o, int first_stage_only,
                                 const uint8_t *d_alive, const uint8_t *h_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids,
                                 int64_t *out_num_candidates, cudaStream_t s);
 
@@ -2251,12 +2281,12 @@ static int build_row_slot(b200_index *ix) {
     return fill_row_slot(ix, ix->d_row_slot.as<uint32_t>());
 }
 
-// graph_degree=D: every row searches the index's own lists with its defaults for k = 2D + 1.  HNSWFLAT: nprobe and the exact
-// re-rank with refine_factor, exactly ix.search(rows, 2D + 1, "graph=0").  MSTG: the first stage only, exactly
-// ix.search(rows, 2D + 1, "graph=0", first_stage_only=True): the graph is built in the metric its walk scores, the same way for
+// graph_degree=D: every row searches the index's own lists (graph=0) with its defaults for k = 2D + 1.  HNSWFLAT: nprobe and the
+// exact re-rank with refine_factor, exactly ix.search(rows, 2D + 1) with graph=0.  MSTG: the first stage only, exactly
+// ix.search(rows, 2D + 1, first_stage_only=True) with graph=0: the graph is built in the metric its walk scores, the same way for
 // either placement of the fp32 rows, and never reads a row over PCIe.  The queries are the fp32 rows (HBM or host memory), or,
 // in an index without them (MSTG keep_raw=0), the bf16 list rows.  BINARYMSTG: its lists are exact, so the search is exactly
-// ix.search(rows, 2D + 1, "graph=0"), its queries the row bytes read back from the binary pages (it keeps no other copy).  Its
+// ix.search(rows, 2D + 1) with graph=0, its queries the row bytes read back from the binary pages (it keeps no other copy).  Its
 // own id dropped, a row's 2D candidates are pruned by rank (CAGRA) and merged with the reverse edges (graph_sm90.cu).  phase_ms
 // then holds candidates | prune | merge in milliseconds.
 static int build_graph_locked(b200_index *ix) {
@@ -2295,7 +2325,7 @@ static int build_graph_locked(b200_index *ix) {
                                            ix->raw ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
         else
             B200_TRY(graph_page_rows(ix->d_pool.p, ix->d_row_slot.as<uint32_t>(), off, m, d, ix->d_pad64, static_cast<float *>(q.p), s));
-        B200_TRY(search_device_locked(ix, static_cast<float *>(q.p), m, K + 1, nullptr, mstg ? 1 : 0, nullptr, nullptr, 0, static_cast<float *>(dis.p),
+        B200_TRY(search_device_locked(ix, static_cast<float *>(q.p), m, K + 1, search_opts(ix, nullptr), mstg ? 1 : 0, nullptr, nullptr, 0, static_cast<float *>(dis.p),
                                       static_cast<int64_t *>(ids.p), nullptr, s));
         B200_TRY(graph_candidates(static_cast<int64_t *>(ids.p), row_slot, m, off, K, static_cast<uint32_t *>(cand.p) + off * K, s));
     }
@@ -2627,6 +2657,21 @@ __global__ void cosine_finish_kernel(const float *q, int64_t nq, int d, int d_pa
     dis[i] = ids[i] >= 0 ? 1.f - dis[i] : FLT_MAX;
 }
 
+// cosine: the IP keys of a search over the raw (unit) rows become distances; the other metrics' keys are already
+static void cosine_finish(const b200_index *ix, const float *d_q, int64_t nq, int k, float *d_out_dis, const int64_t *d_out_ids, cudaStream_t s) {
+    if (ix->metric != B200_METRIC_COSINE) return;
+    cosine_finish_kernel<<<(unsigned)ceil_div(nq * k, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, k, d_out_dis, d_out_ids);
+    g_launches++;
+}
+
+// the prepared queries [nq][d_pad] back to [nq][d] rows in ix->w_qraw, the row form of a corpus search
+static int unpad_queries(b200_index *ix, const float *d_q, int64_t nq, cudaStream_t s) {
+    B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
+    if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
+    else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
+    return B200_OK;
+}
+
 // Pages of a list one work item streams for a scan of n_valid (query, list) pairs (see scan_probes); forced: the
 // "pages_per_chunk" A/B key, 0 = none.
 static uint32_t pages_per_chunk(const b200_index *ix, int64_t n_valid, int forced) {
@@ -2650,7 +2695,7 @@ static uint32_t pages_per_chunk(const b200_index *ix, int64_t n_valid, int force
 // scan, per-query merge, exact second stage.  d_q: the first stage's queries [nq][d_pad] (opq=1: rotated), d_qx: the
 // prepared queries of the exact second stage.  probe: [nq][nprobe] list ids (negative = an invalid slot, skipped by every
 // step).  n_valid: the count of valid slots, sizing the gathered query rows, the work items and the partial lists.  list_len / list_pages: the index's own, or the filtered ones of filter_probe=1.
-static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, const float *d_queries, int64_t nq, int k, int k1, bool two_stage, const char *params,
+static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, const float *d_queries, int64_t nq, int k, int k1, bool two_stage, const SearchOpts &o,
                        const int64_t *probe, int nprobe, int64_t n_valid, const uint32_t *list_len, const uint32_t *list_pages,
                        const uint8_t *d_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
     const int nl = ix->nlist;
@@ -2684,7 +2729,7 @@ static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, cons
     // pays one cold start of its top-k lists.  The page counts (8 to 16, 48 below) were chosen on an earlier GPU and are
     // not re-measured on the H100.  The estimate uses host-side knowledge only (no device -> host round trip on the query path): probed
     // lists <= min(pairs, nlist), their length size-biased.
-    const uint32_t ppc = pages_per_chunk(ix, n_valid, parse_int_param(params, "pages_per_chunk", 0));
+    const uint32_t ppc = pages_per_chunk(ix, n_valid, o.pages_per_chunk);
     const uint32_t max_chunks = (ix->max_list_pages + ppc - 1) / ppc;
     const int64_t max_items = std::min<int64_t>(n_valid * max_chunks, (int64_t)(ceil_div(n_valid, 128) + nl) * max_chunks);
     const int64_t max_parts = n_valid * max_chunks;
@@ -2783,7 +2828,7 @@ static int scan_probes(b200_index *ix, const float *d_q, const float *d_qx, cons
     gp.part_ids = ix->w_pi.as<uint32_t>();
     gp.part_worst = ix->w_pw.as<float>();
     {   // shared per-query bound across the items of this launch (ivf_gemm.h); nothing to share with one list per query
-        if (nprobe > 1 && parse_int_param(params, "shared_bound", 1) != 0) {   // shared_bound=0: A/B switch
+        if (nprobe > 1 && o.shared_bound != 0) {
             B200_TRY(ix->w_qb.reserve((size_t)nq * 4));
             B200_CUDA_OK(cudaMemsetAsync(ix->w_qb.p, 0xff, (size_t)nq * 4, s));
             gp.query_bound = ix->w_qb.as<uint32_t>();
@@ -2892,11 +2937,10 @@ constexpr double kFilterProbeExactFactor = 16.0;
 // the live lists) and a stream synchronise; then the probe rows [nq][P] of the live lists, P = max live lists, and the rest of
 // the search with nprobe := P, its buffers sized by the live lists.  Leaving out a list without a kept row changes no answer:
 // it holds no candidate and the merge does not depend on the order of its inputs.
-static int filter_probe_search(b200_index *ix, const float *d_q, const float *d_qx, int64_t nq, int k, int k1, bool two_stage, const char *params, int nprobe,
+static int filter_probe_search(b200_index *ix, const float *d_q, const float *d_qx, int64_t nq, int k, int k1, bool two_stage, const SearchOpts &o,
                                const uint32_t *list_len, const uint32_t *list_pages, const uint8_t *d_alive, int64_t id_offset, float *d_out_dis,
                                int64_t *d_out_ids, cudaStream_t s) {
     const int nl = ix->nlist;
-    const int max_nprobe = std::max(nprobe, std::min(nl, parse_int_param(params, "max_nprobe", nl)));
     const int64_t chunk = coarse_chunk(nq, nl);
     const bool one_chunk = nq <= chunk;
     B200_TRY(ix->w_cs.reserve((size_t)chunk * nl * 4));
@@ -2914,8 +2958,8 @@ static int filter_probe_search(b200_index *ix, const float *d_q, const float *d_
     for (int64_t q0 = 0; q0 < nq; q0 += chunk) {
         const int64_t nqc = std::min(chunk, nq - q0);
         coarse_keys(q0, nqc);
-        probe_select_kernel<<<(unsigned)nqc, kProbeThreads, 0, s>>>(ix->w_cs.as<float>(), nl, ix->w_flist.as<uint32_t>(), (uint32_t)k1, nprobe,
-                                                                   max_nprobe, d_p + q0, d_live + q0, d_key + q0, d_ties + q0, d_tot);
+        probe_select_kernel<<<(unsigned)nqc, kProbeThreads, 0, s>>>(ix->w_cs.as<float>(), nl, ix->w_flist.as<uint32_t>(), (uint32_t)k1, o.nprobe,
+                                                                   o.max_nprobe, d_p + q0, d_live + q0, d_key + q0, d_ties + q0, d_tot);
         g_launches++;
     }
     B200_CUDA_OK(cudaGetLastError());
@@ -2940,14 +2984,13 @@ static int filter_probe_search(b200_index *ix, const float *d_q, const float *d_
     // Query ranges for the steps after the selection: the whole batch when its scratch, sized as scan_probes sizes it from
     // its live lists, fits the budget; else consecutive ranges that each fit it (at least one query), each sized by its own.  On
     // the look-up-scan indexes a range also keeps its per-query tables within kPqLutScratchBytes.
-    const int forced_ppc = parse_int_param(params, "pages_per_chunk", 0);
     const int64_t qrow_bytes = pq_uses_lut(ix) ? 0 : (int64_t)ix->d_pad64 * 2;
     auto scratch = [&](int64_t nqr, int64_t n_valid) {
-        const int64_t ppc = pages_per_chunk(ix, n_valid, forced_ppc);
+        const int64_t ppc = pages_per_chunk(ix, n_valid, o.pages_per_chunk);
         const int64_t chunks = (ix->max_list_pages + ppc - 1) / ppc;
         return nqr * P * kFilterProbeSlotBytes + n_valid * (qrow_bytes + chunks * ((int64_t)k1 * 8 + 4 + (int64_t)sizeof(IvfGemmItem)));
     };
-    const int64_t qmax = pq_uses_lut(ix) ? std::max<int64_t>(1, kPqLutScratchBytes / ((int64_t)ix->m * pq_codewords(ix->pq_bits) * 4)) : nq;
+    const int64_t qmax = pq_uses_lut(ix) ? pq_lut_max_queries(ix) : nq;
     std::vector<std::pair<int64_t, int64_t>> ranges;   // (end query, live lists of the range)
     if (nq <= qmax && scratch(nq, sum_live) <= kFilterProbeScratchBytes) {
         ranges.emplace_back(nq, sum_live);
@@ -2975,7 +3018,7 @@ static int filter_probe_search(b200_index *ix, const float *d_q, const float *d_
             g_launches++;
             q0 = q1;
         }
-        B200_TRY(scan_probes(ix, d_q + a * ix->d_pad, d_qx + a * ix->d_pad, nullptr, b - a, k, k1, two_stage, params, ix->w_probe.as<int64_t>(), P, ranges[r].second,
+        B200_TRY(scan_probes(ix, d_q + a * ix->d_pad, d_qx + a * ix->d_pad, nullptr, b - a, k, k1, two_stage, o, ix->w_probe.as<int64_t>(), P, ranges[r].second,
                              list_len, list_pages, d_alive, id_offset, d_out_dis + a * k, d_out_ids + a * k, s));
         items += ix->last_items;
         if (split) {   // b200_index_last_scan reports the rows of the whole batch
@@ -2998,13 +3041,6 @@ static int64_t graph_rows_at_cap(const b200_index *ix, int nseeds, int width) {
     return nseeds + (int64_t)graph_iteration_cap(ix->graph_degree, width) * width * ix->graph_degree;
 }
 
-static int graph_ef(const char *params, int k) {
-    return std::max(k, parse_int_param(params, "ef_s", 64));
-}
-
-// search_width=W: parents expanded per iteration, one CTA of a cluster each (1, 2, 4 or 8; default 1, one CTA per query)
-static int graph_width(const char *params) { return parse_int_param(params, "search_width", 1, true); }
-
 // The graph search, asynchronous on s (d_q: the prepared queries [nq][d_pad]): seeds from the list path's first stage at
 // nprobe 1 (the best min(ef_s, 32) ids per query), then one CTA per query (search_width=W > 1: one cluster of W CTAs, W
 // parents per iteration) walks the graph: graph_search_kernel over the fp32 rows in HBM (HNSWFLAT, kc = k),
@@ -3012,15 +3048,17 @@ static int graph_width(const char *params) { return parse_int_param(params, "sea
 // k: its keys are the exact distances; d_queries are its query bytes).  With a second stage
 // (two_stage, MSTG only; kc may equal k, at k = 1024) the walk's best kc rows are re-ranked exactly by refine_device, from HBM
 // or from host memory.
-static int graph_search_locked(b200_index *ix, const float *d_queries, const float *d_q, int64_t nq, int k, int kc, bool two_stage, const char *params,
+static int graph_search_locked(b200_index *ix, const float *d_queries, const float *d_q, int64_t nq, int k, int kc, bool two_stage, const SearchOpts &o,
                                const uint8_t *d_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, cudaStream_t s) {
-    const int ef = graph_ef(params, kc);
-    const int width = graph_width(params);   // validated by search_device_locked
+    const int ef = std::max(kc, o.ef_s);
+    const int width = o.search_width;   // validated by search_device_locked
     const int S = std::min(ef, kGraphMaxSeeds);
     B200_TRY(ix->w_seeds.reserve((size_t)nq * S * 8));
     B200_TRY(ix->w_seedd.reserve((size_t)nq * S * 4));
-    B200_TRY(search_device_locked(ix, d_queries, nq, S, "graph=0 nprobe=1", 1, nullptr, nullptr, 0, ix->w_seedd.as<float>(), ix->w_seeds.as<int64_t>(),
-                                  nullptr, s));
+    SearchOpts seed = search_opts(ix, nullptr);   // the index's defaults at nprobe 1, whatever keys the caller passed
+    seed.graph = 0;
+    seed.nprobe = 1;
+    B200_TRY(search_device_locked(ix, d_queries, nq, S, seed, 1, nullptr, nullptr, 0, ix->w_seedd.as<float>(), ix->w_seeds.as<int64_t>(), nullptr, s));
     ix->last_seed_nq = nq;
     ix->last_seed_s = S;
     unsigned long long *scored = reinterpret_cast<unsigned long long *>(ix->d_flag.as<int>() + 4);
@@ -3065,12 +3103,8 @@ static int graph_search_locked(b200_index *ix, const float *d_queries, const flo
     } else {
         B200_TRY(graph_search(gp, nq, width, s));
     }
-    if (two_stage) {
-        B200_TRY(refine_device(ix, d_q, nq, ix->w_oi.as<int64_t>(), kc, k, id_offset, d_out_dis, d_out_ids, s));
-    } else if (ix->metric == B200_METRIC_COSINE) {
-        cosine_finish_kernel<<<(unsigned)ceil_div(nq * k, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, k, d_out_dis, d_out_ids);
-        g_launches++;
-    }
+    if (two_stage) B200_TRY(refine_device(ix, d_q, nq, ix->w_oi.as<int64_t>(), kc, k, id_offset, d_out_dis, d_out_ids, s));
+    else cosine_finish(ix, d_q, nq, k, d_out_dis, d_out_ids, s);
     ix->last_items = nq * width;   // CTAs launched
     ix->last_graph = true;
     return B200_OK;
@@ -3078,77 +3112,69 @@ static int graph_search_locked(b200_index *ix, const float *d_queries, const flo
 
 // The whole search on the device, asynchronous on s.  d_queries: fp32 [nq][d]; outputs [nq][k].  h_alive: the host copy of
 // d_alive when the caller has one (the exact paths may then score only the rows it keeps), else null.
-static int search_device_locked(b200_index *ix, const float *d_queries, int64_t nq, int k, const char *params, int first_stage_only,
+static int search_device_locked(b200_index *ix, const float *d_queries, int64_t nq, int k, const SearchOpts &o, int first_stage_only,
                                 const uint8_t *d_alive, const uint8_t *h_alive, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids,
                                 int64_t *out_num_candidates, cudaStream_t s) {
     if (out_num_candidates) *out_num_candidates = k;
     if (nq == 0) return B200_OK;
-    const int force_exact = parse_int_param(params, "exact_batch", 0);
-    const int prefilter = parse_int_param(params, "prefilter", 0);   // A/B: 1 never, 2 whenever it fits (exact paths only)
-    if (prefilter < 0 || prefilter > 2) return fail(B200_ERR_INVALID, "prefilter must be 0 (auto), 1 (never) or 2 (always)");
-    const int filter_probe = parse_int_param(params, "filter_probe", 0);
+    if (o.prefilter < 0 || o.prefilter > 2) return fail(B200_ERR_INVALID, "prefilter must be 0 (auto), 1 (never) or 2 (always)");
     // filter_probe=1 below nlist keeps its look-up tables within the budget itself, under its one synchronise
-    const bool fselect_bounds_lut = filter_probe && d_alive && ix->use_ivf &&
-                                    std::max(1, parse_int_param(params, "nprobe", ix->default_nprobe)) < ix->nlist;
-    if (pq_uses_lut(ix) && force_exact != 1 && k <= 1024 && !fselect_bounds_lut) {
+    const bool fselect_bounds_lut = o.filter_probe && d_alive && ix->use_ivf && o.nprobe < ix->nlist;
+    if (pq_uses_lut(ix) && o.exact_batch != 1 && k <= 1024 && !fselect_bounds_lut) {
         // the look-up scan's tables are nq x M KB (4-bit codes: nq x M x 64 B): a larger batch runs as consecutive query
         // sub-batches through the whole search (every query's answer depends on that query alone, so the results are those of
         // one batch)
-        const int64_t qmax = std::max<int64_t>(1, kPqLutScratchBytes / ((int64_t)ix->m * pq_codewords(ix->pq_bits) * 4));
+        const int64_t qmax = pq_lut_max_queries(ix);
         if (nq > qmax) {
             for (int64_t q0 = 0; q0 < nq; q0 += qmax)
-                B200_TRY(search_device_locked(ix, d_queries + q0 * ix->d, std::min(qmax, nq - q0), k, params, first_stage_only, d_alive, h_alive, id_offset,
+                B200_TRY(search_device_locked(ix, d_queries + q0 * ix->d, std::min(qmax, nq - q0), k, o, first_stage_only, d_alive, h_alive, id_offset,
                                               d_out_dis + q0 * k, d_out_ids + q0 * k, out_num_candidates, s));
             return B200_OK;
         }
     }
     if (ix->binary) {
         // binary queries are bytes [nq][d / 8]; list rows are exact, so refine_factor / keep_raw / first_stage_only change nothing
-        if (force_exact == 1) return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available on binary indexes (their lists are exact)");
-        if (filter_probe) return fail(B200_ERR_UNSUPPORTED, "filter_probe is not available on binary indexes (their coarse probe ranks at most 1024 lists)");
+        if (o.exact_batch == 1) return fail(B200_ERR_UNSUPPORTED, "exact_batch=1 is not available on binary indexes (their lists are exact)");
+        if (o.filter_probe) return fail(B200_ERR_UNSUPPORTED, "filter_probe is not available on binary indexes (their coarse probe ranks at most 1024 lists)");
         if (!ix->use_ivf) {
             ix->last_probe.insert(ix->last_probe.end(), nq, 0);
-            return corpus_search_exact(ix->raw.get(), d_queries, nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s);
+            return corpus_search_exact(ix->raw.get(), d_queries, nq, k, d_alive, h_alive, o.prefilter, id_offset, d_out_dis, d_out_ids, s);
         }
     } else {
         B200_TRY(prepare_queries_device(ix, d_queries, nq, s));
     }
     const float *d_q = ix->w_q.as<float>();
-    bool exact = !ix->use_ivf || force_exact == 1;
+    bool exact = !ix->use_ivf || o.exact_batch == 1;
     // graph_degree indexes walk their graph unless asked for the lists (graph=0) or the exact pass (exact_batch=1)
-    const bool graph = ix->d_graph && !exact && parse_int_param(params, "graph", 1) != 0;
+    const bool graph = ix->d_graph && !exact && o.graph != 0;
     // the walk returns kc rows per query: HNSWFLAT's are exact (kc = k); MSTG's are re-ranked from the fp32 rows when it has a
     // second stage (graph_two_stage, the list path's two_stage; kc = min(1024, k x refine_factor), its k1)
     int kc = k;
     bool graph_two_stage = false;
     if (graph) {
         if (k > kGraphMaxEf) return fail(B200_ERR_UNSUPPORTED, "k > 1024 on the graph search");
-        const int ef_s = parse_int_param(params, "ef_s", 64);
-        if (ef_s > kGraphMaxEf) return fail(B200_ERR_INVALID, "ef_s must be at most 1024, got " + std::to_string(ef_s));
-        const int width = graph_width(params);
-        if (!graph_width_ok(width)) return fail(B200_ERR_INVALID, "search_width must be 1, 2, 4 or 8, got " + std::to_string(width));
+        if (o.ef_s > kGraphMaxEf) return fail(B200_ERR_INVALID, "ef_s must be at most 1024, got " + std::to_string(o.ef_s));
+        if (!graph_width_ok(o.search_width)) return fail(B200_ERR_INVALID, "search_width must be 1, 2, 4 or 8, got " + std::to_string(o.search_width));
         if (ix->d_row_slot && !ix->binary) {   // BINARYMSTG: the walk's keys are the exact distances
-            const int refine_factor = std::max(1, parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", ix->refine_factor)));
-            graph_two_stage = has_rows(ix) && refine_factor > 1 && !first_stage_only;
-            if (graph_two_stage) kc = std::min(kGraphMaxEf, k * refine_factor);
+            graph_two_stage = has_rows(ix) && o.refine_factor > 1 && !first_stage_only;
+            if (graph_two_stage) kc = std::min(kGraphMaxEf, k * o.refine_factor);
         }
         if (out_num_candidates) *out_num_candidates = kc;
         // the exact rule scans the fp32 rows in HBM: without them (MSTG keep_raw=0 | 2) the walk always answers, and so does
         // BINARYMSTG's (its lists are the only copy of its rows; a load refuses a v4 binary file with rows)
         if (d_alive && h_alive && ix->raw && !ix->binary) {
-            const int64_t rows_cap = graph_rows_at_cap(ix, std::min(graph_ef(params, kc), kGraphMaxSeeds), width);
+            const int64_t rows_cap = graph_rows_at_cap(ix, std::min(std::max(kc, o.ef_s), kGraphMaxSeeds), o.search_width);
             const int64_t limit = std::min<int64_t>((int64_t)std::ceil(kGraphExactFactor * kc * (double)ix->n / (double)rows_cap) - 1,
-                                                    corpus_prefilter_limit(ix->raw.get(), prefilter, nq, k));
+                                                    corpus_prefilter_limit(ix->raw.get(), o.prefilter, nq, k));
             exact = limit >= 0 && host_count_alive(h_alive, ix->n, limit) <= limit;
             ix->last_probe_exact = exact;
         }
-    } else if (!exact && filter_probe && d_alive && h_alive && ix->raw && !first_stage_only) {
+    } else if (!exact && o.filter_probe && d_alive && h_alive && ix->raw && !first_stage_only) {
         // filter_probe exact rule: a filter that keeps at most kFilterProbeExactFactor x the rows one query's plain probe scans
         // on average is answered by the exact pass over the kept rows (complete and exact) -- only when that pass takes its
         // gathered path for this batch (prefilter mode, nq, k): past the gathered path's limit it would scan every row
-        const int np = std::max(1, std::min(parse_int_param(params, "nprobe", ix->default_nprobe), ix->nlist));
-        const int64_t limit = std::min<int64_t>((int64_t)(kFilterProbeExactFactor * np * (double)ix->n / (double)ix->nlist),
-                                                corpus_prefilter_limit(ix->raw.get(), prefilter, nq, k));
+        const int64_t limit = std::min<int64_t>((int64_t)(kFilterProbeExactFactor * o.nprobe * (double)ix->n / (double)ix->nlist),
+                                                corpus_prefilter_limit(ix->raw.get(), o.prefilter, nq, k));
         exact = limit >= 0 && host_count_alive(h_alive, ix->n, limit) <= limit;
         ix->last_probe_exact = exact;
     }
@@ -3160,30 +3186,23 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
                                               "the exact pass would stream every row over PCIe");
         if (!ix->raw) return fail(B200_ERR_INVALID, "exact search needs the fp32 rows (keep_raw=0 index)");
         // FLAT / fallback-to-flat: exact scan of the raw rows.  The raw corpus wants [nq][d] rows: strip the padding again.
-        B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
-        if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
-        else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
-        B200_TRY(corpus_search_exact(ix->raw.get(), ix->w_qraw.as<float>(), nq, k, d_alive, h_alive, prefilter, id_offset, d_out_dis, d_out_ids, s));
-        if (ix->metric == B200_METRIC_COSINE) {
-            cosine_finish_kernel<<<(unsigned)ceil_div(nq * k, 256), 256, 0, s>>>(d_q, nq, ix->d, ix->d_pad, k, d_out_dis, d_out_ids);
-            g_launches++;
-        }
+        B200_TRY(unpad_queries(ix, d_q, nq, s));
+        B200_TRY(corpus_search_exact(ix->raw.get(), ix->w_qraw.as<float>(), nq, k, d_alive, h_alive, o.prefilter, id_offset, d_out_dis, d_out_ids, s));
+        cosine_finish(ix, d_q, nq, k, d_out_dis, d_out_ids, s);
         return B200_OK;
     }
-    if (graph) return graph_search_locked(ix, d_queries, d_q, nq, k, kc, graph_two_stage, params, d_alive, id_offset, d_out_dis, d_out_ids, s);
+    if (graph) return graph_search_locked(ix, d_queries, d_q, nq, k, kc, graph_two_stage, o, d_alive, id_offset, d_out_dis, d_out_ids, s);
     if (k > 1024) return fail(B200_ERR_UNSUPPORTED, "k > 1024 on IVF indexes");
     const int nl = ix->nlist;
-    int nprobe = parse_int_param(params, "nprobe", ix->default_nprobe);
-    nprobe = std::max(1, std::min(nprobe, nl));
+    const int nprobe = o.nprobe;
     if (ix->binary && nprobe < nl && nprobe > 1024)
         return fail(B200_ERR_UNSUPPORTED, "binary indexes probe at most 1024 lists (the binary corpus k limit), or all of them (nprobe >= nlist)");
-    const int refine_factor = std::max(1, parse_int_param(params, "refine_factor", parse_int_param(params, "reorder_k_factor", ix->refine_factor)));
-    const bool two_stage = has_rows(ix) && refine_factor > 1 && !first_stage_only && !ix->binary;
-    const int k1 = two_stage ? std::min(1024, k * refine_factor) : k;
+    const bool two_stage = has_rows(ix) && o.refine_factor > 1 && !first_stage_only && !ix->binary;
+    const int k1 = two_stage ? std::min(1024, k * o.refine_factor) : k;
     if (out_num_candidates) *out_num_candidates = k1;
     // filter_probe=1 under a filter: the scan sees only the pages with kept rows, and below nlist every query probes as deep
     // as its first k1 kept rows need
-    const bool fprobe = filter_probe && d_alive;
+    const bool fprobe = o.filter_probe && d_alive;
     const bool fselect = fprobe && nprobe < nl;
     const int64_t n_pairs = nq * nprobe;
     if (!fselect && n_pairs >= (int64_t)1 << 31) return fail(B200_ERR_UNSUPPORTED, "nq * nprobe must stay below 2^31");
@@ -3207,7 +3226,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         list_len = ix->w_flist.as<uint32_t>() + nl;
         list_pages = ix->w_fpages.as<uint32_t>();
         if (fselect)
-            return filter_probe_search(ix, d_q, d_qx, nq, k, k1, two_stage, params, nprobe, list_len, list_pages, d_alive, id_offset, d_out_dis, d_out_ids, s);
+            return filter_probe_search(ix, d_q, d_qx, nq, k, k1, two_stage, o, list_len, list_pages, d_alive, id_offset, d_out_dis, d_out_ids, s);
     }
     // ---- coarse probe: nprobe nearest centroids per query (exact FLAT search of the centroid table)
     B200_TRY(ix->w_probe.reserve((size_t)n_pairs * 8));
@@ -3221,9 +3240,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
             B200_TRY(b200_corpus_search_device(ix->coarse.get(), ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s));
         }
     } else {
-        B200_TRY(ix->w_qraw.reserve((size_t)nq * ix->d * 4));
-        if (ix->d == ix->d_pad) B200_CUDA_OK(cudaMemcpyAsync(ix->w_qraw.p, d_q, (size_t)nq * ix->d * 4, cudaMemcpyDeviceToDevice, s));
-        else B200_CUDA_OK(cudaMemcpy2DAsync(ix->w_qraw.p, (size_t)ix->d * 4, d_q, (size_t)ix->d_pad * 4, (size_t)ix->d * 4, nq, cudaMemcpyDeviceToDevice, s));
+        B200_TRY(unpad_queries(ix, d_q, nq, s));
         // The centroid table is small and nprobe is a large k for it: the tensor-core path keeps one k-list per query lane
         // and never gets a selective threshold when k / nlist is a few percent.  The scan kernel's warp lists cost O(k / 32) per
         // insert: use it when its estimated time (FMA-bound, ~1.4 TB/s of table bytes per 8-query pass) undercuts ~1 us per
@@ -3234,8 +3251,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
         bool use_scan = nprobe > 8 && t_scan < t_gemm;
         // nprobe > 8: full ranking keys + warp select (coarse_scores_kernel / coarse_select_kernel above)
         int coarse_path = nprobe > 8 && nprobe <= 1024 ? 3 : use_scan ? 1 : 2;
-        const int forced = parse_int_param(params, "coarse_path", 0);   // A/B: 1 scan kernel, 2 tensor-core path, 3 select
-        if (forced) coarse_path = forced;
+        if (o.coarse_path) coarse_path = o.coarse_path;
         if (coarse_path == 3) {
             const int64_t chunk = coarse_chunk(nq, nl);
             B200_TRY(ix->w_cs.reserve((size_t)chunk * nl * 4));
@@ -3253,7 +3269,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
             ix->last_coarse = 3;
         } else {
             // chosen 2: the corpus' own choice by batch size; forced 2: the tensor-core path whatever the batch
-            b200_corpus_set_path(ix->coarse.get(), coarse_path == 1 ? 1 : forced == 2 ? 2 : 0);
+            b200_corpus_set_path(ix->coarse.get(), coarse_path == 1 ? 1 : o.coarse_path == 2 ? 2 : 0);
             const int rc = b200_corpus_search_device(ix->coarse.get(), ix->w_qraw.as<float>(), nq, nprobe, nullptr, 0, ix->w_pd.as<float>(), ix->w_probe.as<int64_t>(), s);
             b200_corpus_set_path(ix->coarse.get(), 0);
             B200_TRY(rc);
@@ -3264,7 +3280,7 @@ static int search_device_locked(b200_index *ix, const float *d_queries, int64_t 
     }
 
     if (ix->timing) cudaEventRecord(ix->ev_ph[1], s);
-    return scan_probes(ix, d_q, d_qx, d_queries, nq, k, k1, two_stage, params, ix->w_probe.as<int64_t>(), nprobe, n_pairs, list_len, list_pages, d_alive,
+    return scan_probes(ix, d_q, d_qx, d_queries, nq, k, k1, two_stage, o, ix->w_probe.as<int64_t>(), nprobe, n_pairs, list_len, list_pages, d_alive,
                        id_offset, d_out_dis, d_out_ids, s);
 }
 
@@ -3283,20 +3299,26 @@ static void timing_collect(b200_index *ix) {
     ix->timed_pending = false;
 }
 
+// the start of a search under ix->mu: the index's device, the previous search's timing collected, the last_* diagnostics cleared
+static int begin_search_locked(b200_index *ix) {
+    B200_CUDA_OK(cudaSetDevice(ix->device));
+    timing_collect(ix);
+    ix->last_probe.clear();
+    ix->last_probe_exact = false;
+    ix->last_coarse = 0;
+    ix->last_graph = false;
+    return B200_OK;
+}
+
 // Search::VectorIndex::search with device buffers, asynchronous on `stream` (NULL: the index's stream, synchronised)
 extern "C" int b200_index_search_device(b200_index *ix, const float *d_queries, int64_t nq, int k, const char *params, int first_stage_only,
                                         const uint8_t *d_alive_bits, int64_t id_offset, float *d_out_dis, int64_t *d_out_ids, void *stream) {
     if (!ix || (!d_queries && nq > 0) || !d_out_dis || !d_out_ids || nq < 0 || k <= 0) return fail(B200_ERR_INVALID, "bad arguments");
     if (!ix->built) return fail(B200_ERR_INVALID, "index not built");
     std::lock_guard<std::mutex> lk(ix->mu);
-    B200_CUDA_OK(cudaSetDevice(ix->device));
-    timing_collect(ix);
+    B200_TRY(begin_search_locked(ix));
     cudaStream_t s = stream ? reinterpret_cast<cudaStream_t>(stream) : ix->stream;
-    ix->last_probe.clear();
-    ix->last_probe_exact = false;
-    ix->last_coarse = 0;
-    ix->last_graph = false;
-    B200_TRY(search_device_locked(ix, d_queries, nq, k, params, first_stage_only, d_alive_bits, nullptr, id_offset, d_out_dis, d_out_ids, nullptr, s));
+    B200_TRY(search_device_locked(ix, d_queries, nq, k, search_opts(ix, params), first_stage_only, d_alive_bits, nullptr, id_offset, d_out_dis, d_out_ids, nullptr, s));
     if (!stream) B200_CUDA_OK(cudaStreamSynchronize(s));
     return B200_OK;
 }
@@ -3309,13 +3331,8 @@ extern "C" int b200_index_search(b200_index *ix, const float *queries, int64_t n
     if (out_num_candidates) *out_num_candidates = k;
     if (nq == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ix->mu);
-    B200_CUDA_OK(cudaSetDevice(ix->device));
-    timing_collect(ix);
+    B200_TRY(begin_search_locked(ix));
     cudaStream_t s = ix->stream;
-    ix->last_probe.clear();
-    ix->last_probe_exact = false;
-    ix->last_coarse = 0;
-    ix->last_graph = false;
     B200_TRY(ix->w_host_q.reserve((size_t)nq * in_row_bytes(ix)));
     B200_TRY(ix->w_cand.reserve((size_t)nq * k * 12 + 16));
     B200_CUDA_OK(cudaMemcpyAsync(ix->w_host_q.p, queries, (size_t)nq * in_row_bytes(ix), cudaMemcpyHostToDevice, s));
@@ -3328,7 +3345,7 @@ extern "C" int b200_index_search(b200_index *ix, const float *queries, int64_t n
     }
     float *r_d = ix->w_cand.as<float>();
     int64_t *r_i = reinterpret_cast<int64_t *>(reinterpret_cast<char *>(ix->w_cand.p) + (size_t)round_up(nq * k * 4, 8));
-    B200_TRY(search_device_locked(ix, ix->w_host_q.as<float>(), nq, k, params, first_stage_only, d_alive, alive_bits, 0, r_d, r_i, out_num_candidates, s));
+    B200_TRY(search_device_locked(ix, ix->w_host_q.as<float>(), nq, k, search_opts(ix, params), first_stage_only, d_alive, alive_bits, 0, r_d, r_i, out_num_candidates, s));
     B200_CUDA_OK(cudaMemcpyAsync(out_dis, r_d, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaMemcpyAsync(out_ids, r_i, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
